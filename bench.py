@@ -1,7 +1,8 @@
-"""Headline benchmark: Qwen3-4B W4A16 decode / prefill tokens/s on B200 (BASELINE.json).
+"""Headline benchmark: Qwen3-4B W4A16 decode / prefill tokens/s on H100 (BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                     [--workload decode|prefill|serve|serve8k] [--no-extra] [--no-cpu-baseline]
+                    [--dump-outputs DIR]
 
 Workloads (BASELINE.json `configs`; SURVEY.md section 8d):
 
@@ -11,14 +12,20 @@ Workloads (BASELINE.json `configs`; SURVEY.md section 8d):
            The line also carries, under `extra`, the config-2 sweeps (context S in {128,1K,4K,8K} at B=1,
            batch B in {1..64} at S=128) and a short config-3 prefill measurement with its two rooflines.
   prefill  (config 3) a 4096-token prompt through Qwen3ModelWeek3.__call__ in one chunk (and in 512 /
-           128-token chunks under `extra`); a "step" is one whole prefill.  roofline = the tcgen05 W4A16
-           GEMM (tensor bound) + the tcgen05 paged FlashAttention under `extra.attention_roofline`.
+           128-token chunks under `extra`); a "step" is one whole prefill.  roofline = the wgmma W4A16
+           GEMM (tensor bound) + the wgmma paged FlashAttention under `extra.attention_roofline`.
   serve    (config 4) continuous batching, 64 decode slots, 128 requests per GPU, prompts U[128,1024],
            outputs U[32,128], prefill_step 128, page 128, seed 0 (protocol of the reference's
            benches/bench.py:351-572); a "step" is one scheduler iteration, the run is the whole queue.
-  serve8k  (config 5) 8K-context requests sharded i mod N over the ranks, 64 decode slots per GPU;
+  serve8k  (config 5) 8K-context requests sharded i mod N over the ranks, 32 decode slots per GPU;
            --requests defaults to 64 * N (every GPU carries config 5's per-GPU load: at N = 8 this is
            exactly the 512-request configuration), prefill_step 1024.
+
+--steps K sets the number of timed steps of decode (default 128) and prefill (default 8).  It does not apply to
+serve / serve8k, whose timed run is the whole request queue: their `steps` field reports the scheduler iterations
+that run took.  With --impl reference it sets the number of timed CPU decode steps, clamped to 9..16 to bound
+the CPU time (a reference prefill takes 2 samples); the count used is what `steps` reports.  --dump-outputs DIR is available for --impl ours with
+decode and prefill: the serving runs have no single last step whose outputs a caller receives.
 
 At N > 1 every rank serves its own requests (request i -> rank i mod N); weights are drawn on rank 0
 and broadcast once over NCCL; there is no data-path collective.
@@ -30,8 +37,8 @@ Numbers on the JSON line (decode):
             model(...), device -> host read of the sampled token
   roofline  the W4A16 weight-streaming kernel: the 145 projection launches of one token exactly as the
             decode graph issues them (2.137 GB of packed weights, > L2), replayed from a CUDA graph,
-            CUDA-event timed; achieved = algorithmic bytes / time, traffic = ncu DRAM bytes of the same
-            launches (read from the committed capture named in `traffic_source`, null if there is none)
+            CUDA-event timed; achieved = algorithmic bytes / time; traffic and traffic_source stay null
+            (DRAM bytes need a hardware-counter profiler, which this benchmark does not run)
   cpu_baseline  the reference's CPU path (oracle.model: dense bf16 weights, readable operators) on the
             host cores, bounded sample
 """
@@ -74,19 +81,8 @@ def measured_peaks() -> dict:
         return {"hbm_gbs": float(data["hbm_gbs"]), "bf16_tflops": float(data.get("bf16_tflops", 1682.0)),
                 "bf16_tflops_sustained": float(data.get("bf16_tflops_sustained", data.get("bf16_tflops", 1442.5))),
                 "source": "MEASURED_PEAKS.json"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1680.0, "bf16_tflops_sustained": 1440.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def committed_traffic(kernel: str):
-    """(bytes per launch, file) from the committed ncu capture of this round, or (None, None)."""
-    path = ROOT / "profiles" / "traffic.json"
-    if not path.exists():
-        return None, None
-    try:
-        entry = json.loads(path.read_text()).get(kernel)
-        return (int(entry["dram_bytes_per_launch"]), f"profiles/{entry['source']}") if entry else (None, None)
-    except (ValueError, KeyError, TypeError):
-        return None, None
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 - a bound, never a reached rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 def synthetic_prompt(seed: int, length: int, vocab: int) -> list[int]:
@@ -148,6 +144,19 @@ def cuda_time_ms(fn, stream=None) -> float:
     end.record(stream)
     end.synchronize()
     return start.elapsed_time(end)
+
+
+def dump_outputs(directory: str, arrays: dict) -> None:
+    """--dump-outputs: what the timed path returned in its last step, one DIR/<name>.npy per array (floating point as
+    float32, token ids as float64).  Weights and prompts are seeded, so two builds run with the same arguments can be
+    compared output for output."""
+    import numpy as np
+
+    out = Path(directory)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        np.save(out / f"{name}.npy", (t.to(torch.float32) if t.is_floating_point() else t.to(torch.float64)).numpy())
 
 
 def base_line(args, world: int, workload: str) -> dict:
@@ -223,6 +232,8 @@ def run_decode(args) -> None:
     barrier(device)
     ms = max_over_ranks(start.elapsed_time(end), device)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:  # logits of the last timed step [1, V] and the greedy tokens of the last call [take, 1]
+        dump_outputs(args.dump_outputs, {"logits": engine.logits, "tokens": out_tokens})
     # graph replays do not pass through the C ABI; the launches recorded when the step was captured
     # are what each replay executes (plus whatever went through the ABI directly in the region)
     gpu_launches = engine.kernels_per_step * (engine.graph_replays - replays0) + (ext.launch_count() - launches0)
@@ -280,7 +291,7 @@ def run_decode(args) -> None:
             "config": {
                 "workload": "Qwen3-4B W4A16 single-request decode, batch=1 per GPU, paged-KV GQA + dequant matvec",
                 "prompt_len": PROMPT_LEN, "page_size": PAGE_SIZE, "requests_per_gpu": 1, "parallelism": f"dp{world}",
-                "l2_policy": "inputs larger than L2: each step streams 2.14 GB of packed weights (L2 = 126 MB)",
+                "l2_policy": "inputs larger than L2: each step streams 2.14 GB of packed weights (L2 = 50 MB)",
                 "decode_graph": "cuda-graph replay, fused=%s, pdl=%s" % (engine.fused, info["pdl"]),
             },
             "e2e": {"value": round(e2e_value, 2), "unit": UNIT, "h2d_bytes_per_step": 4 + meta_bytes, "d2h_bytes_per_step": 4, "steps": e2e_steps},
@@ -300,7 +311,7 @@ def matvec_roofline(model, engine, ext, device) -> dict:
     """The projection launches of one decode token exactly as the engine issues them (per layer:
     rms_norm+q|k|v, o+residual, rms_norm+gate|up+swiglu, down+residual; then rms_norm+head), M = 1,
     from one captured graph: 2.137 GB of distinct packed weights per replay, so every launch
-    streams from HBM (L2 = 126 MB)."""
+    streams from HBM (L2 = 50 MB)."""
     from tiny_llm_b200.synthetic import weight_stream_bytes
 
     H = model.hidden_size
@@ -342,7 +353,7 @@ def matvec_roofline(model, engine, ext, device) -> dict:
     algorithmic = weight_stream_bytes(margs) + io + 2 * (H + margs.vocab_size)
     peak = measured_peaks()
     achieved = algorithmic / (ms / 1e3) / 1e9
-    traffic, traffic_source = committed_traffic("w4a16_stream5_kernel")
+    traffic, traffic_source = None, None  # no hardware-counter capture (see the module docstring)
     return {
         "kernel": "w4a16_stream5_kernel<bf16, M=1> (W4A16 dequant matvec with fused rms_norm / residual / SwiGLU epilogue)",
         "bound": "hbm", "achieved": round(achieved, 1), "peak": peak["hbm_gbs"], "peak_source": peak["source"], "unit": "GB/s",
@@ -481,7 +492,7 @@ def gemm_roofline(model, ext, device, margs, tokens: int) -> dict:
     flops = prefill_flops(margs, tokens)["projections"]
     launches = 7 * len(model.layers_inner)
     achieved = flops / (ms / 1e3) / 1e12
-    return {"kernel": "w4a16_gemm_kernel / w4a16_gemm2_kernel (tcgen05.mma kind::f16, the pair form cta_group::2 for q|k|v and gate|up; TMEM accumulators, TMA activations, in-kernel W4 dequant)",
+    return {"kernel": "w4a16_skinny_kernel<bf16, 128> on 128-token tiles (swap-AB wgmma m64n128k16, register accumulators, TMA activations and packed weights, in-kernel W4 dequant)",
             "bound": "tensor", "achieved": round(achieved, 1), "peak": peaks["bf16_tflops_sustained"], "peak_source": peaks["source"] + " (sustained)",
             "unit": "TFLOP/s", "frac": round(achieved / peaks["bf16_tflops_sustained"], 4), "traffic": None, "launches": launches,
             "avg_launch_us": round(ms * 1e3 / launches, 2), "algorithmic_flops_per_launch": round(flops / launches),
@@ -531,7 +542,7 @@ def run_prefill(args) -> None:
         tok = greedy_tokens(logits[:, -1, :])
         for c in cache:
             c.release()
-        return tok
+        return tok, logits
 
     for _ in range(warmup):
         one(prompts[0])
@@ -544,13 +555,15 @@ def run_prefill(args) -> None:
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     start.record()
     for i in range(steps):
-        one(prompts[i % 2])
+        tok, logits = one(prompts[i % 2])
     end.record()
     torch.cuda.synchronize()
     barrier(device)
     ms = max_over_ranks(start.elapsed_time(end), device)
     clocks = sampler.stop() if rank == 0 else None
     gpu_launches = ext.launch_count() - launches0
+    if args.dump_outputs and rank == 0:  # the last timed prefill: logits of its last position [1, 1, V], greedy token [1]
+        dump_outputs(args.dump_outputs, {"logits": logits, "tokens": tok})
     value = world * steps * tokens / (ms / 1e3)
     # e2e: prompt ids from pinned host memory, first token read back
     pinned_out = torch.empty(1, dtype=torch.int32, pin_memory=True)
@@ -558,7 +571,7 @@ def run_prefill(args) -> None:
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for _ in range(steps):
-        pinned_out.copy_(one(host_prompt.to(device, non_blocking=True)), non_blocking=True)
+        pinned_out.copy_(one(host_prompt.to(device, non_blocking=True))[0], non_blocking=True)
         torch.cuda.synchronize()
     e2e_s = max_over_ranks(time.perf_counter() - t0, device)
     extra = {}
@@ -601,7 +614,7 @@ def run_serve(args, long_context: bool) -> None:
 
     ext, model, model_ns, rank, world, device, info = setup(args)
     margs = model_ns.args
-    slots = args.slots
+    slots = args.slots or (32 if long_context else 64)  # 32 slots of 8K context: 39 GB of K/V pages on an 80 GB card
     if long_context:
         total = args.requests or 64 * world
         out_len = 128
@@ -632,7 +645,7 @@ def run_serve(args, long_context: bool) -> None:
     # warm-up: a short queue through the same scheduler (captures the B-slot decode graph, sizes the pools)
     warm = [(p[: min(len(p), 2 * prefill_step)], 4) for p, _ in mine[: min(len(mine), slots + 2)]]
     # ... plus one prompt with a ONE-token tail chunk: that tail is a B = 1 decode step, whose engine (private packed
-    # weight copies + graph capture, 30-900 ms depending on the host) otherwise gets built inside the timed region by the
+    # weight copies + graph capture) otherwise gets built inside the timed region by the
     # first such prompt of the queue
     long_enough = [p for p, _ in mine if len(p) > prefill_step + 1]
     if long_enough:
@@ -743,8 +756,8 @@ def run_cpu_baseline(sample_steps: int, warmup_steps: int = 1, mode: str = "deco
     cores = os.cpu_count() or 1
     threads = min(32, cores)
     # Pin the process to `threads` cores BEFORE the first parallel CPU op creates torch's worker pool (the workers
-    # inherit the mask): on a 128-thread host the unpinned run swung 3x between two launches on the same box (22 vs
-    # 69 ms per step: workers migrating across NUMA nodes away from the first-touched weights).
+    # inherit the mask): unpinned, the workers migrate across NUMA nodes away from the first-touched weights and the
+    # step time varies from run to run.
     allowed = None
     try:
         allowed = sorted(os.sched_getaffinity(0))
@@ -790,9 +803,8 @@ def _cpu_baseline_pinned(sample_steps, warmup_steps, mode, synthetic, cores, thr
     greedy_decode(model, prompt, 1 + warmup_steps + sample_steps, timings=timings)
     per_step = sorted(timings["decode_s"][warmup_steps:])
     scale = (full["num_hidden_layers"] * layer_w + head_w) / (CPU_SAMPLE_LAYERS * layer_w + head_w)
-    # Best of N: the GPU boxes' hosts are shared and a CPU decode step (a 2.4 GB GEMV sweep) swings 2-3x from step to
-    # step inside one run (median 20-25 ms, interquartile range > 2x the median on two consecutive runs); the fastest
-    # step is the reproducible one, and it is the most favourable figure for the CPU path.
+    # Best of N: a host may be shared, and a CPU decode step (a 2.4 GB GEMV sweep) varies from step to step inside one
+    # run; the fastest step is the reproducible one, and it is the most favourable figure for the CPU path.
     median_s = statistics.median(per_step)
     sample_s = per_step[0]
     q1, q3 = per_step[len(per_step) // 4], per_step[(3 * len(per_step)) // 4]
@@ -812,7 +824,7 @@ def run_reference(args) -> None:
     steps = args.steps
     workload = args.workload
     mode = "prefill" if workload == "prefill" else "decode"
-    sample = min(max(steps, 9), 16) if mode == "decode" else 2  # a CPU decode step is 20-70 ms: 9-16 samples stay well under a second
+    sample = min(max(steps, 9), 16) if mode == "decode" else 2  # 9-16 CPU decode steps keep the sample short
     base = run_cpu_baseline(sample_steps=sample, warmup_steps=3, mode=mode)
     line = {
         "impl": "reference",
@@ -839,17 +851,23 @@ def run_reference(args) -> None:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=None)
+    ap.add_argument("--steps", type=int, default=None,
+                    help="timed steps of decode (default 128) / prefill (default 8); serve / serve8k time the whole queue; "
+                         "--impl reference clamps it to 9..16 CPU decode steps (2 prefill samples)")
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--workload", choices=sorted(METRICS), default="decode")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the sweeps / secondary measurements under `extra`")
     ap.add_argument("--requests", type=int, default=0, help="serve/serve8k: total requests over all ranks")
-    ap.add_argument("--slots", type=int, default=64, help="serve/serve8k: decode slots per GPU")
+    ap.add_argument("--slots", type=int, default=0, help="serve/serve8k: decode slots per GPU (default 64 / 32)")
     ap.add_argument("--prefill-step", type=int, default=0)
     ap.add_argument("--prompt-len", type=int, default=0, help="prefill: prompt tokens (default 4096)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="decode / prefill: write what the timed path returned in its last step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload not in ("decode", "prefill")):
+        ap.error("--dump-outputs is available for --impl ours with the decode and prefill workloads")
     if args.steps is None:
         args.steps = {"decode": 128, "prefill": 8}.get(args.workload, 0)
     if args.impl == "reference":

@@ -7,7 +7,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and the ``cpu_baseline`` /
 (``tiny-llm_b200/``) never imports ``oracle`` and has no CPU fallback: its
 operators raise when the CUDA extension is missing or when handed CPU tensors.
 
-What it restates (all paths relative to ``/root/reference``):
+What it restates (all paths relative to the tiny-llm repository):
 
 * ``oracle.ops``      - the arithmetic of every native primitive in
   ``src/extensions_ref/src/*.metal`` with the same rounding points (fp32

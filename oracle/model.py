@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE (see ``oracle/__init__.py``).  This is
 ``Qwen3ModelWeek2(mlx_model, checkpoint="kv-cache")``
-(``/root/reference/src/tiny_llm_ref/qwen3_week2.py:251-392``): packed weights
+(``src/tiny_llm_ref/qwen3_week2.py:251-392``): packed weights
 dequantised to dense bf16 at load (``:286``), readable RMSNorm / RoPE / SiLU,
 attention promoted to fp32 (``:138-144``), concat-growth KV cache
 (``kv_cache.py:246-276``), driven by the greedy loop of

@@ -2,9 +2,9 @@
 
 TEST INFRASTRUCTURE (see ``oracle/__init__.py``).  Every function takes and
 returns CPU ``torch`` tensors and follows the arithmetic of one Metal kernel of
-``/root/reference/src/extensions_ref/src`` - fp32 math, storage dtype rounded
+``src/extensions_ref/src`` - fp32 math, storage dtype rounded
 once at the store - together with the builder-time checks of the matching
-``.cpp`` file.  Citations are ``file:line`` relative to ``/root/reference``.
+``.cpp`` file.  Citations are ``file:line`` relative to the tiny-llm repository.
 """
 
 from __future__ import annotations

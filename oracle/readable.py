@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE (see ``oracle/__init__.py``).  These are the only
 operators of the reference that its own code can run on a CPU
-(``/root/reference/main.py:50-61``), so they double as the second, independent
+(``main.py:50-61``), so they double as the second, independent
 restatement that ``oracle.ops`` is cross-checked against - the same
 equalities the reference asserts in ``tests_refsol/test_week_2_day_{4,5}.py``.
 """

@@ -3,7 +3,7 @@
 * ``-m "not gpu"`` (run on a CPU-only box): oracle pinning, host logic driven
   through the CPU stand-in of the extension (``oracle.ext_cpu``), C-ABI export
   checks, gloo data-parallel tests.
-* ``-m gpu`` (run on a B200): the parity tests proper - the product's CUDA
+* ``-m gpu`` (run on an H100): the parity tests proper - the product's CUDA
   path against the oracle on the same seeded inputs, through the C ABI.
 """
 
@@ -22,7 +22,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 @pytest.fixture

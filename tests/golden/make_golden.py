@@ -27,7 +27,7 @@ from oracle.model import ReferenceCpuModel, greedy_decode  # noqa: E402
 
 
 def decode_attention_checksums():
-    """Fixture sweep of /root/reference/tests_refsol/test_week_2_day_5.py:119-163."""
+    """Fixture sweep of tests_refsol/test_week_2_day_5.py:119-163."""
     D, Hq = 128, 4
 
     def fixture(shape, phase):

@@ -1,4 +1,4 @@
-"""B200 decode runtime: fused decode kernels and the CUDA-graph engine must
+"""CUDA decode runtime: fused decode kernels and the CUDA-graph engine must
 reproduce the operator-by-operator path (same rounding points), and the
 device-resident greedy loop must emit the tokens of the host-driven loop."""
 

@@ -1,4 +1,4 @@
-"""Model-level parity on a B200: the Week-2/Week-3 model code and the scheduler
+"""Model-level parity on an H100: the Week-2/Week-3 model code and the scheduler
 running on the CUDA kernels, against the reference's CPU path (oracle.model) on
 identical synthetic weights.  Stated tolerance: teacher-forced log-probabilities
 of the reference's top-4 candidates within 0.25 nat (bf16 activations through

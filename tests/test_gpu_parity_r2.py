@@ -112,7 +112,7 @@ def test_paged_decode_attention_at_serving_sizes_matches_oracle(dev, B, S):
 
 @pytest.mark.parametrize("B,L,ctx,Hq,Hkv,page", [(1, 128, 640, 32, 8, 128), (2, 100, 300, 16, 8, 64), (1, 40, 40, 8, 8, 128), (1, 4, 200, 32, 8, 128)])
 def test_token_major_prefill_attention_is_the_transposed_head_major_result(dev, B, L, ctx, Hq, Hkv, page):
-    """The chunked-prefill engine asks the tcgen05 kernel for [B * L, Hq * D] directly (the o-projection's layout):
+    """The chunked-prefill engine asks the wgmma kernel for [B * L, Hq * D] directly (the o-projection's layout):
     bit-identical to paged_attention + transpose; shapes the kernel does not take (here L = 4) fall back to exactly that."""
     g, D = gen(B * 1000 + L + ctx), 128
     pages = -(-ctx // page)
@@ -169,27 +169,22 @@ def test_qkv_projection_feeding_rope_append_equals_the_two_calls(dev, rows, chun
 
 
 # ------------------------------------------------------------------ GEMM at the config-3 shapes --
-@pytest.mark.parametrize("pairs", [0, 2], ids=["one-cta", "cta-pairs"])
+# One CTA per output tile: the only form on Hopper (the CTA-pair form used Blackwell's cta_group::2).
+@pytest.mark.parametrize("tiling", ["one-cta"])
 @pytest.mark.parametrize("shape", [(4096, 9728, 2560), (4096, 2560, 19456 // 2), (4096, 4096, 2560), (1000, 256, 392)],
                          ids=lambda s: "x".join(map(str, s)))
-def test_prefill_gemm_full_size_matches_oracle_on_sampled_rows(dev, shape, pairs):
-    """M = 4096 at the Qwen3-4B down / gate / o shapes (and a ragged one: 1000 rows, 392 features) on BOTH prefill
-    kernels - two / four 128-token tiles per CTA (w4a16_gemm.cu) and the cta_group::2 pair kernel (w4a16_gemm2.cu):
-    sampled token rows against the tiled kernel's arithmetic restated on the CPU (weights rounded to bf16 before the
-    MMA, quantized_matmul.metal:183-194; fp32 accumulation), and the two kernels against each other bit for bit on the
-    whole matrix (same rounding points, same accumulation order along the reduction)."""
+def test_prefill_gemm_full_size_matches_oracle_on_sampled_rows(dev, shape, tiling):
+    """M = 4096 at the Qwen3-4B down / gate / o shapes (and a ragged one: 1000 rows, 392 features) on the prefill
+    kernel (128-token tiles, w4a16_skinny.cu): sampled token rows against the tiled kernel's arithmetic restated on the
+    CPU (weights rounded to bf16 before the MMA, quantized_matmul.metal:183-194; fp32 accumulation), and two launches
+    against each other bit for bit on the whole matrix (fixed accumulation order along the reduction)."""
     M, N, K = shape
     g = gen(M + N + K)
     words, scales, biases = rand_packed(K, N, g)
     a = torch.randn(M, N, generator=g).to(BF16)
     args = (scales.to(dev), biases.to(dev), 128, 4, a.to(dev), words.to(dev), True)
-    try:
-        ext.set_gemm_pairs(pairs)
-        got_dev = ext.quantized_matmul(*args)
-        ext.set_gemm_pairs(0)
-        other = ext.quantized_matmul(*args)
-    finally:
-        ext.set_gemm_pairs(1)
+    got_dev = ext.quantized_matmul(*args)
+    other = ext.quantized_matmul(*args)
     got = got_dev.cpu()
     rows = sorted({0, 1, 127, 128, 255, 256, M // 2 - 1, M // 2, M - 1})
     w = oracle.dequantize_weights(words, scales, biases, 128, 4).float()
@@ -262,7 +257,7 @@ def test_engine_batch_with_idle_slots_matches_cpu_oracle(dev, B):
 
 def test_serving_path_engine_matches_cpu_oracle(dev):
     """The step as the serving configurations run it - 32 slots behind 1024-token block tables (64-slot pages): more than
-    16 K slot-tokens, so q|k|v projection + RoPE + append as one fused launch pair, attention on the tcgen05 streaming
+    16 K slot-tokens, so q|k|v projection + RoPE + append as one fused launch pair, attention on the wgmma streaming
     kernel with its split count from the table width, swap-AB projections with the RMSNorm folded into the reduction,
     and a 16-row step graph (occupied slots 0..12) - against the reference CPU path request by request: teacher-forced
     log-probabilities of the oracle's top-4 candidates within 0.25 nat over three steps."""

@@ -257,7 +257,7 @@ def test_array_masks_are_not_supported():
 
 
 def test_decode_batch_append_matches_per_request_writes(cpu_ext):
-    """The single-launch decode append (B200 extension) must leave pools and
+    """The single-launch decode append (CUDA extension) must leave pools and
     metadata exactly as the reference's per-request loop does."""
     def run(batched: bool):
         pool = TinyKvPagedPool(page_size=4)
@@ -296,7 +296,7 @@ def test_decode_batch_append_matches_per_request_writes(cpu_ext):
 
 
 # ---------------------------------------------------------------------------------------------
-# B200 runtime additions to the cache objects (engine.py): deferred one-token appends and bulk slot appends must be
+# CUDA runtime additions to the cache objects (engine.py): deferred one-token appends and bulk slot appends must be
 # indistinguishable from the reference's per-token bookkeeping (paged_kv_cache.py:279-306).
 def _pool_with_capacity(pages, page_size=4):
     pool = TinyKvPagedPool(page_size=page_size)

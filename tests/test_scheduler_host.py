@@ -1,6 +1,6 @@
 """Continuous-batching scheduler against fake models: exact call traces,
 EOS/max_seq_len handling and release-exactly-once, pinned by the literals of
-/root/reference/tests_refsol/test_week_3_day_2.py (tests/golden/reference_literals.json).
+tests_refsol/test_week_3_day_2.py (tests/golden/reference_literals.json).
 CPU-only."""
 
 import json

@@ -1,7 +1,7 @@
 // Decode-side attention kernels (HBM-bound K/V streaming, fp32 online softmax).
 //
 //  * decode_attention_kernel       - dense K/V, reference week2_decode_attention
-//    (/root/reference/src/extensions_ref/src/week2_kernels.metal:119-235).
+//    (src/extensions_ref/src/week2_kernels.metal:119-235).
 //  * paged_rowwise_kernel          - generic paged attention, one CTA per query
 //    row; any dtype/head-dim/page-size (reference paged_attention_decode and the
 //    f32 scalar path, paged_attention.metal:108-248, :508-674).
@@ -9,7 +9,7 @@
 //    (request, KV head, row group, KV split).  All query heads that share a KV
 //    head are processed together so K/V bytes are read ONCE per KV head (the
 //    Metal kernel re-reads them per query head), the context is split across
-//    CTAs (flash-decoding) so a single request still fills 148 SMs, and every
+//    CTAs (flash-decoding) so a single request still fills every SM, and every
 //    K/V access is a 128-bit load of a fully used 32-byte sector.
 //
 // Causality is bottom-right aligned everywhere: query row l of an L-row chunk
@@ -443,7 +443,7 @@ __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_merge_kernel(const floa
     const size_t qi = blockIdx.x;
     const int d = threadIdx.x, lane = d & 31;
     const float *pm = ws_m + qi * splits, *pl = ws_l + qi * splits;
-    // Latency matters here (the whole long-context decode attention of one request is ~17 us): every warp reduces the
+    // Latency matters here (the whole long-context decode attention of one request is a few microseconds): every warp reduces the
     // split scalars on its own with ONE load round per lane (splits <= 32) and a shuffle tree, then the output column is
     // gathered eight independent loads at a time.  (The first version walked the splits in two dependent loops: 2 x
     // splits L2 round trips per thread.)  Fixed order everywhere: same bits on every run.
@@ -497,7 +497,7 @@ int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_
     if (allow_split) {
         const long long target = 4LL * sm_count();
         long long want = ceil_div_ll(target, base_ctas);
-        const long long most = bound / 128 > 0 ? bound / 128 : 1;  // at least 128 tokens per split (512 measured 3.6x slower at S = 1024: the per-step chain dominates)
+        const long long most = bound / 128 > 0 ? bound / 128 : 1;  // at least 128 tokens per split (larger minimums lengthen the per-step chain at short contexts)
         if (want > most) want = most;
         if (want > GQA_MAX_SPLITS) want = GQA_MAX_SPLITS;
         if (want < 1) want = 1;
@@ -556,7 +556,7 @@ int launch_paged_decode(const void *q, const void *kp, const void *vp, const int
                         int is_causal, int num_kv_heads, int num_heads, int dtype, void *ws, size_t ws_bytes,
                         cudaStream_t st) {
     const bool fast = dtype == TL_BF16 && D == GQA_D && aligned16(q) && aligned16(kp) && aligned16(vp);
-    // Long contexts stream K/V through the TMA + tcgen05 kernel (attention_prefill_tc.cu; the G x L query rows ride
+    // Long contexts stream K/V through the TMA + wgmma kernel (attention_prefill_tc.cu; the G x L query rows ride
     // in a 128-row MMA tile - the tensor-core time is far below the HBM time of the tile even at 4 live rows); short
     // ones stay on the cp.async kernel, whose fixed cost per CTA is lower.  TL_DECODE_TC: 0 never, 1 always (when supported).
     static const int tc_mode = [] { const char *e = getenv("TL_DECODE_TC"); return e == nullptr ? -1 : atoi(e); }();
@@ -574,7 +574,7 @@ int launch_paged_decode(const void *q, const void *kp, const void *vp, const int
                                 num_kv_heads, num_heads, dtype, st);
 }
 
-// Prefill path (L > 8): bf16 / D = 128 runs the tcgen05 + TMA flash kernel (attention_prefill_tc.cu)
+// Prefill path (L > 8): bf16 / D = 128 runs the wgmma + TMA flash kernel (attention_prefill_tc.cu)
 // when the page size is a multiple of 64 and Hq/Hkv divides 128 (TL_PREFILL_TC=0 turns it off), else
 // the mma.sync flash kernel (attention_prefill.cu); TL_PREFILL_FA=0 selects the older CUDA-core
 // GQA-grouped kernel as a control; everything else is row-wise.

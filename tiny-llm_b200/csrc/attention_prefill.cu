@@ -1,10 +1,8 @@
 // Paged causal prefill attention on the tensor cores (bf16, head_dim 128).
 //
 // Replaces paged_attention_prefill / the tiled FlashAttention of the reference
-// (/root/reference/src/extensions_ref/src/paged_attention.metal:250-506,
-// flash_attention.metal) for L > 8.  Measured before this kernel existed: the CUDA-core
-// GQA kernel ran a 4096-token layer in 20.7 ms (6.6 TF/s, 0.4 % of the bf16 peak) and was 88 %
-// of a Qwen3-4B prefill.
+// (src/extensions_ref/src/paged_attention.metal:250-506,
+// flash_attention.metal) for L > 8, where the CUDA-core GQA kernel would dominate a Qwen3-4B prefill.
 //
 // Shape of the computation (FlashAttention-2 style, one pass, online softmax):
 //   grid  = (ceil(L / 64) query tiles, B * Hq heads), longest (last) query tiles first
@@ -16,8 +14,8 @@
 //   mask  = bottom-right aligned causal limit clamp(ctx - L + l + 1, 0, ctx) per query row
 //           (attention.py:40-58 semantics), rows/pages outside the context contribute nothing
 //
-// This is the mma.sync version: correct, ~30x the kernel it replaces, but not the tcgen05/TMEM
-// pipeline a Blackwell-native prefill deserves - that is round-2 work (DESIGN.md section 4).
+// This is the mma.sync version; page sizes that are a multiple of 64 take the wgmma + TMA kernel
+// (attention_prefill_tc.cu, DESIGN.md section 4).
 #include <math_constants.h>
 
 #include "common.cuh"

@@ -1,7 +1,6 @@
-// Paged causal FlashAttention prefill on the 5th-generation tensor cores (tcgen05 + TMEM + TMA),
-// bf16, head_dim 128, L > 8.
+// Paged causal FlashAttention prefill on the Hopper tensor cores (wgmma + TMA), bf16, head_dim 128, L > 8.
 //
-// Replaces paged_attention_mma_bf16_d128 (/root/reference/src/extensions_ref/src/
+// Replaces paged_attention_mma_bf16_d128 (src/extensions_ref/src/
 // paged_attention.metal:250-506): same arithmetic - fp32 scores in base 2 (:414 scale_log2),
 // bottom-right causal limit key <= row + (context - L) (:411), fp32 running max / sum, the
 // probabilities rounded to bf16 before P V (:439-444), output = O / sum (0 when nothing is visible).
@@ -11,24 +10,19 @@
 // fetches is shared by all the query heads that need it, and the causal frontier is almost the same
 // for every row (RH <= 128 positions apart).  Per 64-key tile:
 //
-//   warp 4 (one lane)  TMA producer: Q once (3-D map [D, L, B*Hq], box 64 x RH x G, 128-byte
-//                      swizzle = the K-major UMMA layout), then K and V tiles - a (page, kv head)
-//                      slab is one contiguous [page x 128] bf16 block, fetched as 4-D boxes
-//                      [64 d x 64 keys] keyed by block_table (invalid page ids land outside the
-//                      tensor and are zero-filled by the TMA unit) - through a 2-stage ring;
-//   warp 5 (one lane)  MMA issuer: S = Q K^T  (tcgen05.mma kind::f16, M128 N64 K16 x 8, K tile =
-//                      K-major B operand), then O += P V (M128 N128 K16 x 4, V tile = MN-major B
-//                      operand straight from the page layout), accumulators S and O in TMEM;
-//   warps 0-3          softmax: thread = MMA row = TMEM lane.  tcgen05.ld the 64 scores of its row,
-//                      scale, mask, running max (no shuffles: a thread owns the row), exp2, row sum,
-//                      bf16 probabilities -> shared memory in the swizzled K-major layout (A operand
-//                      of P V).  O is rescaled IN TMEM (tcgen05.ld / st) only when a row's maximum
-//                      grows by more than 2^8 since the last rescale: P and the row sum always use
-//                      the same (possibly stale) maximum, so the result is exact.
-//                      Epilogue: O / sum -> bf16 -> global.
-//
-// 256 TMEM columns and 112 KB of shared memory per CTA: two CTAs per SM, so one CTA's softmax
-// overlaps the other's MMAs without an intra-CTA ping-pong.
+//   warp 0 (one lane)    TMA producer: Q once (3-D map [D, L, B*Hq], box 64 x RH x G, 128-byte
+//                        swizzle = the K-major wgmma layout), then K and V tiles - a (page, kv head)
+//                        slab is one contiguous [page x 128] bf16 block, fetched as 4-D boxes
+//                        [64 d x 64 keys] keyed by block_table (invalid page ids land outside the
+//                        tensor and are zero-filled by the TMA unit) - through a TC_STAGES ring;
+//   warpgroups 1, 2      64 MMA rows each: S = Q K^T (wgmma m64n64k16 x 8, both operands K-major in
+//                        shared memory, fp32 scores in registers), softmax in registers (a row lives
+//                        in the four lanes of a quad: two shuffles for its maximum), the bf16
+//                        probabilities stay in registers as the A operand of O += P V (wgmma
+//                        m64n128k16 x 4, V tile = MN-major B operand straight from the page layout).
+//                        O is rescaled only when a row's maximum grows by more than 2^8 since the last
+//                        rescale: P and the row sum always use the same (possibly stale) maximum, so
+//                        the result is exact.  Epilogue: O / sum -> bf16 -> global.
 #include <stdlib.h>
 #include <math_constants.h>
 
@@ -37,7 +31,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
-#include "tc05.cuh"
+#include "wgmma.cuh"
 
 namespace tl {
 
@@ -46,37 +40,21 @@ typedef __nv_bfloat16 bf16;
 constexpr int TC_D = 128;         // head dim
 constexpr int TC_BM = 128;        // MMA rows per CTA (G heads x RH query positions)
 constexpr int TC_BN = 64;         // keys per tile
-constexpr int TC_STAGES = 2;
-constexpr int TC_THREADS = 6 * 32;
-constexpr int TC_SOFTMAX_THREADS = 128;
+constexpr int TC_STAGES = 3;
+constexpr int TC_CONSUMERS = 2;   // consumer warpgroups, 64 rows each
+constexpr int TC_THREADS = 128 * (1 + TC_CONSUMERS);
 constexpr int TC_Q_BYTES = TC_BM * TC_D * 2;        // 32 KiB: two 64-column halves of [128 rows x 128 B]
 constexpr int TC_KV_TILE = TC_BN * TC_D * 2;        // 16 KiB: two 64-column halves of [64 rows x 128 B]
-constexpr int TC_P_BYTES = TC_BM * TC_BN * 2;       // 16 KiB: [128 rows x 128 B]
 constexpr int TC_Q_OFF = 0;
-constexpr int TC_P_OFF = TC_Q_OFF + TC_Q_BYTES;
-constexpr int TC_K_OFF = TC_P_OFF + TC_P_BYTES;
+constexpr int TC_K_OFF = TC_Q_OFF + TC_Q_BYTES;
 constexpr int TC_V_OFF = TC_K_OFF + TC_STAGES * TC_KV_TILE;
 constexpr int TC_BAR_OFF = TC_V_OFF + TC_STAGES * TC_KV_TILE;
 constexpr int TC_SMEM_BYTES = TC_BAR_OFF + 256;
-constexpr int TC_TMEM_COLS = 256;  // S (two buffers): columns [0, 64) and [64, 128), O: columns [128, 256)
-constexpr int TC_TMEM_O = 128;
 constexpr float TC_LOG2E = 1.44269504089f;
 constexpr float TC_RESCALE_THRESHOLD = 8.0f;  // log2: rescale O when a row maximum grew by more than 2^8
 
-// kind::f16 instruction descriptor: bf16 x bf16 -> f32, A K-major; b_mn: B operand MN-major.
-__host__ __device__ constexpr uint32_t tc_instr_desc(int n, bool b_mn) {
-    return (1u << 4)                                // c_format = f32
-           | (1u << 7)                              // a_format = bf16
-           | (1u << 10)                             // b_format = bf16
-           | (0u << 15)                             // a_major = K
-           | ((b_mn ? 1u : 0u) << 16)               // b_major
-           | (static_cast<uint32_t>(n >> 3) << 17)  // n_dim
-           | (static_cast<uint32_t>(TC_BM >> 4) << 24);
-}
-
-// ex2.approx.ftz: one MUFU instruction (exp2f() adds denormal-range scaling, ~3 more instructions per element; ncu of the
-// first version: 10.7 instructions per score element, issue slots 54 % busy with the tensor pipe at 40 %).  Relative error
-// 2^-22; the reference kernel uses fast::exp2 (paged_attention.metal:428-436).
+// ex2.approx.ftz: one MUFU instruction (exp2f() adds denormal-range scaling).  Relative error 2^-22; the reference
+// kernel uses fast::exp2 (paged_attention.metal:428-436).
 __device__ __forceinline__ float tc_ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -98,18 +76,13 @@ struct TcArgs {
     float *ws_o, *ws_m, *ws_l;
 };
 
-// PT: the probabilities of a tile stay in TENSOR memory - P_j (bf16 pairs, 32 columns) overwrites the first half of the
-// score buffer S_j it was computed from, and P V reads its A operand from there (the TS form of tcgen05.mma).  The
-// shared-memory form kept ONE P tile, so the exponentials of tile j could not start before P V of tile j-1 had finished
-// reading it; now the exponentials overlap it (the wait sits just before the barrier arrival, and in the rare rescale
-// of O), and the eight 16-byte stores + proxy fence per row become one tcgen05.st.  Buffer reuse needs no barrier: S_{j+2} is issued behind P V_j in the same MMA queue.
-template <bool PT>
-__global__ void __launch_bounds__(TC_THREADS, 2)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const TcArgs a) {
     extern __shared__ __align__(1024) unsigned char tsm[];
     griddep_launch();  // programmatic dependent launch (common.cuh): the successor may set itself up under this grid
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x) >> 7, 0);  // warpgroup, provably warp-uniform
     const int split = static_cast<int>(blockIdx.x) % a.splits;
     const int qb = static_cast<int>(gridDim.x) / a.splits - 1 - static_cast<int>(blockIdx.x) / a.splits;  // long (late) query blocks first
     const int kvh = blockIdx.y, b = blockIdx.z;
@@ -126,47 +99,35 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int t0 = min(split * tps, all_tiles);
     const int n_tiles = min(tps, all_tiles - t0);  // this CTA: global tiles t0 .. t0 + n_tiles - 1
 
-    const uint32_t q_base = g_smem_u32(tsm + TC_Q_OFF), p_base = g_smem_u32(tsm + TC_P_OFF);
+    const uint32_t q_base = g_smem_u32(tsm + TC_Q_OFF);
     const uint32_t k_base = g_smem_u32(tsm + TC_K_OFF), v_base = g_smem_u32(tsm + TC_V_OFF);
     const uint32_t bar = g_smem_u32(tsm + TC_BAR_OFF);
-    const uint32_t q_full = bar, s_full = bar + 8 /* two: one per S buffer */, p_full = bar + 24, pv_done = bar + 32;
-    const uint32_t k_full = bar + 40, k_empty = k_full + 8 * TC_STAGES, v_full = k_full + 16 * TC_STAGES, v_empty = k_full + 24 * TC_STAGES;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tsm + TC_BAR_OFF + 40 + 32 * TC_STAGES);
+    const uint32_t q_full = bar;
+    const uint32_t k_full = bar + 8, k_empty = k_full + 8 * TC_STAGES, v_full = k_full + 16 * TC_STAGES, v_empty = k_full + 24 * TC_STAGES;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_q) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_k) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_v) : "memory");
     }
-    if (warp == 5 && lane == 0) {
+    if (warp == 1 && lane == 0) {
         g_mbar_init(q_full, 1);
-        g_mbar_init(s_full, 1);
-        g_mbar_init(s_full + 8, 1);
-        g_mbar_init(p_full, TC_SOFTMAX_THREADS / 32);  // one arrival per softmax warp
-        g_mbar_init(pv_done, 1);
         for (int i = 0; i < TC_STAGES; ++i) {
             g_mbar_init(k_full + 8 * i, 1);
-            g_mbar_init(k_empty + 8 * i, 1);
+            g_mbar_init(k_empty + 8 * i, TC_CONSUMERS);  // one arrival per consumer warpgroup
             g_mbar_init(v_full + 8 * i, 1);
-            g_mbar_init(v_empty + 8 * i, 1);
+            g_mbar_init(v_empty + 8 * i, TC_CONSUMERS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(g_smem_u32(tmem_slot)), "n"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    g_tc_fence_before();
     __syncthreads();
-    g_tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     // q and the newest K/V rows are the predecessor's output, and this grid overwrites buffers (output, split partials)
     // the predecessor may still read; block tables and context lengths are step inputs uploaded before the chain.
     griddep_wait();
 
-    if (warp == 4) {
+    if (wg_idx == 0) {
         // ------------------------------------------------------------ TMA producer
-        if (n_tiles > 0) {  // whole warp, one elected lane issues (see the MMA warp)
+        if (warp == 0 && n_tiles > 0) {  // whole warp, one elected lane issues
             const int head0 = b * a.Hq + kvh * a.G;
             if (g_elect_one()) {
                 g_mbar_expect_tx(q_full, TC_Q_BYTES);
@@ -199,221 +160,144 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
                 if (++s == TC_STAGES) s = 0, ph ^= 1u;
             }
         }
-    } else if (warp == 5) {
-        // ------------------------------------------------------------ MMA issuer
-        // Order: S_0, then per tile j: S_{j+1} (second score buffer) | wait P_j | O += P_j V_j.  The tensor core works
-        // on the next tile's scores while the softmax warps are busy with this tile's.
-        // The whole warp walks the loop (uniform control flow, running stage / phase counters, descriptors derived by
-        // adding to three base descriptors), one elected lane issues (tc05.cuh: g_elect_one - behind `if (lane == 0)`
-        // every tcgen05 instruction sat in an ELECT loop with its operands moved through R2UR, and the issue latency
-        // of a tile was of the order of its 512 cycles of tensor work).
-        if (n_tiles > 0) {
-            constexpr uint32_t idesc_s = tc_instr_desc(TC_BN, false);
-            constexpr uint32_t idesc_o = tc_instr_desc(TC_D, true);
-            const uint64_t qdesc0 = g_smem_desc_sw128(q_base, 0, 1024), pdesc0 = g_smem_desc_sw128(p_base, 0, 1024);
-            const uint64_t kdesc0 = g_smem_desc_sw128(k_base, 0, 1024);
-            // V: 16 keys = 2 groups of 8 rows (SBO 1024 B); the two 64-wide d blocks are TC_KV_TILE/2 apart (LBO)
-            const uint64_t vdesc0 = g_smem_desc_sw128(v_base, TC_KV_TILE / 2, 1024);
-            g_mbar_wait(q_full, 0);
-            int ks = 0, vs = 0;
-            uint32_t kph = 0, vph = 0;
-            auto issue_scores = [&](int j) {  // S_j = Q K_j^T: both operands K-major, two 64-wide halves of the head dimension
-                g_mbar_wait(k_full + 8 * ks, kph);
-                g_tc_fence_after();
-                if (g_elect_one()) {
-                    const uint64_t kd = kdesc0 + static_cast<uint64_t>(ks * (TC_KV_TILE >> 4));
-#pragma unroll
-                    for (int k = 0; k < TC_D / 16; ++k) {
-                        const uint32_t half = (k >> 2), kk = (k & 3);
-                        g_tc_mma(tmem + (j & 1) * TC_BN, qdesc0 + half * (TC_Q_BYTES / 2 >> 4) + 2 * kk, kd + half * (TC_KV_TILE / 2 >> 4) + 2 * kk,
-                                 idesc_s, k > 0 ? 1u : 0u);
-                    }
-                    g_tc_commit(k_empty + 8 * ks);       // K stage reusable once these MMAs have read it
-                    g_tc_commit(s_full + 8 * (j & 1));   // ... and the scores of tile j are complete
-                }
-                __syncwarp();
-                if (++ks == TC_STAGES) ks = 0, kph ^= 1u;
-            };
-            issue_scores(0);
-            for (int j = 0; j < n_tiles; ++j) {
-                // score buffer (j+1)&1 was last read for tile j-1, whose P has been waited for below
-                if (j + 1 < n_tiles) issue_scores(j + 1);
-                // ---- O += P V: P K-major [128 x 64 keys], V MN-major [64 keys x 128 d] as loaded from the page
-                g_mbar_wait(p_full, j & 1);
-                g_mbar_wait(v_full + 8 * vs, vph);
-                g_tc_fence_after();
-                if (g_elect_one()) {
-                    const uint64_t vd = vdesc0 + static_cast<uint64_t>(vs * (TC_KV_TILE >> 4));
-#pragma unroll
-                    for (int k = 0; k < TC_BN / 16; ++k) {
-                        if constexpr (PT)  // 16 keys = 8 columns of bf16 pairs per K step
-                            g_tc_mma_ts(tmem + TC_TMEM_O, tmem + (j & 1) * TC_BN + 8 * k, vd + k * (2048 >> 4), idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-                        else
-                            g_tc_mma(tmem + TC_TMEM_O, pdesc0 + 2 * k, vd + k * (2048 >> 4), idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-                    }
-                    g_tc_commit(v_empty + 8 * vs);
-                    g_tc_commit(pv_done);  // O holds tiles 0..j and the P buffer is free again
-                }
-                __syncwarp();
-                if (++vs == TC_STAGES) vs = 0, vph ^= 1u;
-            }
-        }
     } else {
-        // ------------------------------------------------------------ softmax warps (thread = row = TMEM lane)
-        const int r = threadIdx.x;                 // 0..127
-        const int g = r / a.RH, lq = r - g * a.RH;  // query head of the KV group, position inside the block
-        const int l = q0 + lq;
-        const bool row_valid = l < a.L && ctx > 0;
-        // last key this row may see (bottom-right causal alignment, paged_attention.metal:411)
-        const int limit = !row_valid ? -1 : (a.is_causal ? min(ctx - 1, l + (ctx - a.L)) : ctx - 1);
-        const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-        float m_used = -CUDART_INF_F, l_sum = 0.f;
+        // ------------------------------------------------------------ consumers: 64 MMA rows per warpgroup
+        // Thread t of the warpgroup holds rows r0 = 16 (t / 32) + (t % 32) / 4 and r0 + 8 of the warpgroup's 64, and the
+        // columns 8 j + 2 (t % 4) + {0, 1} of each (wgmma accumulator layout, wgmma.cuh).
+        const int wg = wg_idx - 1;
+        const int t = threadIdx.x & 127;
+        int lq[2], g[2], l[2], limit[2];
+        bool row_valid[2];
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+            const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * rr;  // MMA row 0..127
+            g[rr] = r / a.RH, lq[rr] = r - g[rr] * a.RH;                   // query head of the KV group, position inside the block
+            l[rr] = q0 + lq[rr];
+            row_valid[rr] = l[rr] < a.L && ctx > 0;
+            // last key this row may see (bottom-right causal alignment, paged_attention.metal:411)
+            limit[rr] = !row_valid[rr] ? -1 : (a.is_causal ? min(ctx - 1, l[rr] + (ctx - a.L)) : ctx - 1);
+        }
+        float o[TC_D / 2];
+#pragma unroll
+        for (int i = 0; i < TC_D / 2; ++i) o[i] = 0.f;
+        float m_used[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_sum[2] = {0.f, 0.f};  // l_sum: this thread's columns only
         const int32_t *table = a.block_table + static_cast<size_t>(b) * a.max_pages;
+        const uint32_t q_wg = q_base + wg * (64 * 128);  // this warpgroup's 64 rows of each 64-column half of Q
+        if (n_tiles > 0) g_mbar_wait(q_full, 0);
+        int s = 0;
+        uint32_t ph = 0;
         for (int j = 0; j < n_tiles; ++j) {
             const int lp = (t0 + j) / a.tiles_per_page;
             const int pid = table[lp];
             const bool page_ok = pid >= 0 && pid < a.num_pages;
-            g_mbar_wait(s_full + 8 * (j & 1), (j >> 1) & 1);
-            g_tc_fence_after();
-            uint32_t sv[2][32];
-            g_tmem_ld32_nowait(tmem + lane_base + (j & 1) * TC_BN, sv[0]);
-            g_tmem_ld32_nowait(tmem + lane_base + (j & 1) * TC_BN + 32, sv[1]);
-            g_tmem_ld_wait();
+            // ---- S = Q K_j^T: both operands K-major, two 64-wide halves of the head dimension
+            float sc[TC_BN / 2];
+#pragma unroll
+            for (int i = 0; i < TC_BN / 2; ++i) sc[i] = 0.f;
+            g_mbar_wait(k_full + 8 * s, ph);
+            wgmma_reg_fence(sc);
+            wgmma_fence();
+            {
+                const uint32_t kb = k_base + s * TC_KV_TILE;
+#pragma unroll
+                for (int k = 0; k < TC_D / 16; ++k) {
+                    const uint32_t half = k >> 2, kk = k & 3;
+                    Wgmma<bf16, TC_BN>::ss(sc, g_wgmma_desc(q_wg + half * (TC_Q_BYTES / 2) + 32 * kk, 16, 1024),
+                                           g_wgmma_desc(kb + half * (TC_KV_TILE / 2) + 32 * kk, 16, 1024), k > 0 ? 1u : 0u);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_reg_fence(sc);
+            if (t == 0) g_mbar_arrive(k_empty + 8 * s);  // K stage reusable: this warpgroup's MMAs have read it
+            // ---- softmax of the tile: sc[4 c8 + 2 rr + e] = S[row rr, key 8 c8 + 2 (t % 4) + e]
             const int key0 = (t0 + j) * TC_BN;
-            const int visible = page_ok ? min(limit - key0 + 1, TC_BN) : 0;  // keys [0, visible) of the tile
-            // raw maximum (the scale is positive, so it commutes with max); masking only on boundary tiles
-            float raw_max = -CUDART_INF_F;
-            if (visible >= TC_BN) {
+            uint32_t pa[TC_BN / 16][4];  // bf16 probabilities as the A operand of the four P V K steps
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
+            for (int rr = 0; rr < 2; ++rr) {
+                const int visible = page_ok ? min(limit[rr] - key0 + 1, TC_BN) : 0;  // keys [0, visible) of the tile
+                // raw maximum (the scale is positive, so it commutes with max); masking only on boundary tiles
+                float raw_max = -CUDART_INF_F;
 #pragma unroll
-                    for (int c = 0; c < 32; ++c) raw_max = fmaxf(raw_max, __uint_as_float(sv[h][c]));
-            } else {
+                for (int c8 = 0; c8 < TC_BN / 8; ++c8)
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) {
-                        if ((h * 32 + c) >= visible) sv[h][c] = 0xff800000u;  // -inf: exp2 gives exactly 0
-                        raw_max = fmaxf(raw_max, __uint_as_float(sv[h][c]));
+                    for (int e = 0; e < 2; ++e) {
+                        float &v = sc[4 * c8 + 2 * rr + e];
+                        if (visible < TC_BN && 8 * c8 + 2 * (lane & 3) + e >= visible) v = -CUDART_INF_F;  // exp2 gives exactly 0
+                        raw_max = fmaxf(raw_max, v);
                     }
-            }
-            const float tile_max = raw_max * a.scale_log2;  // -inf stays -inf
-            if constexpr (!PT)
-                if (j > 0) g_mbar_wait(pv_done, (j - 1) & 1);  // P V of tile j-1 complete: O is stable, the P buffer is free
-            // lazy rescale: keep the stale maximum unless this tile exceeds it by more than 2^8
-            const bool grow = tile_max > m_used + TC_RESCALE_THRESHOLD || (m_used == -CUDART_INF_F && tile_max != -CUDART_INF_F);
-            if (__any_sync(0xffffffffu, grow) && j > 0) {
-                if constexpr (PT) g_mbar_wait(pv_done, (j - 1) & 1);  // O must be stable while it is rescaled
-                g_tc_fence_after();
-                const float m_new = grow ? tile_max : m_used;
-                const float alpha = (grow && m_used != -CUDART_INF_F) ? exp2f(m_used - m_new) : (grow ? 0.f : 1.f);
-                l_sum *= alpha;
+                raw_max = fmaxf(raw_max, __shfl_xor_sync(0xffffffffu, raw_max, 1));
+                raw_max = fmaxf(raw_max, __shfl_xor_sync(0xffffffffu, raw_max, 2));
+                const float tile_max = raw_max * a.scale_log2;  // -inf stays -inf
+                // lazy rescale: keep the stale maximum unless this tile exceeds it by more than 2^8
+                const bool grow = tile_max > m_used[rr] + TC_RESCALE_THRESHOLD || (m_used[rr] == -CUDART_INF_F && tile_max != -CUDART_INF_F);
+                if (grow) {
+                    if (j > 0) {
+                        const float alpha = m_used[rr] != -CUDART_INF_F ? exp2f(m_used[rr] - tile_max) : 0.f;
+                        l_sum[rr] *= alpha;
 #pragma unroll
-                for (int cb = 0; cb < TC_D / 32; ++cb) {
-                    uint32_t ov[32];
-                    g_tmem_ld32(tmem + lane_base + TC_TMEM_O + cb * 32, ov);
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) ov[c] = __float_as_uint(__uint_as_float(ov[c]) * alpha);
-                    g_tmem_st32(tmem + lane_base + TC_TMEM_O + cb * 32, ov);
+                        for (int c8 = 0; c8 < TC_D / 8; ++c8) {
+                            o[4 * c8 + 2 * rr] *= alpha;
+                            o[4 * c8 + 2 * rr + 1] *= alpha;
+                        }
+                    }
+                    m_used[rr] = tile_max;
                 }
-                g_tmem_st_wait();
-                m_used = m_new;
-            } else if (grow) {
-                m_used = tile_max;  // first tile: nothing accumulated yet
-            }
-            const float m_eff = m_used == -CUDART_INF_F ? 0.f : m_used;
-            float tile_sum = 0.f;
-            uint32_t pk[32];  // 64 bf16 probabilities
+                const float m_eff = m_used[rr] == -CUDART_INF_F ? 0.f : m_used[rr];
+                float tile_sum = 0.f;
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int c = 0; c < 32; c += 2) {
-                    const float p0 = tc_ex2(fmaf(__uint_as_float(sv[h][c]), a.scale_log2, -m_eff));
-                    const float p1 = tc_ex2(fmaf(__uint_as_float(sv[h][c + 1]), a.scale_log2, -m_eff));
+                for (int c8 = 0; c8 < TC_BN / 8; ++c8) {
+                    const float p0 = tc_ex2(fmaf(sc[4 * c8 + 2 * rr], a.scale_log2, -m_eff));
+                    const float p1 = tc_ex2(fmaf(sc[4 * c8 + 2 * rr + 1], a.scale_log2, -m_eff));
                     tile_sum += p0 + p1;
-                    pk[h * 16 + c / 2] = pack2<bf16>(p0, p1);
+                    // K step c8 / 2: registers {row r0, keys +0..7}, {r0 + 8, +0..7}, {r0, +8..15}, {r0 + 8, +8..15}
+                    pa[c8 >> 1][2 * (c8 & 1) + rr] = pack2<bf16>(p0, p1);
                 }
-            l_sum += tile_sum;
-            if constexpr (PT) {
-                // lane = row, column c = keys (2c, 2c + 1) of the tile: over the first 32 columns of the score buffer just read
-                g_tmem_st32(tmem + lane_base + (j & 1) * TC_BN, pk);
-                g_tmem_st_wait();
-                // Do not ARRIVE for tile j before P V of tile j-1 has completed (its exponentials above did overlap it): p_full
-                // counts four arrivals per phase, and a warp that ran a whole tile ahead would arrive twice in one phase and
-                // complete it without the slowest warp - P V_j then read rows that were not written yet (1907 of 16.7 M
-                // outputs off by up to 3 % in the constant-V test of the first version).
-                if (j > 0) g_mbar_wait(pv_done, (j - 1) & 1);
-            } else {
-                // P row r: 128 bytes = 8 chunks of 16 B, chunk c at (c ^ (r & 7)) - the 128-byte swizzle of a K-major tile
-                unsigned char *prow = tsm + TC_P_OFF + r * 128;
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    *reinterpret_cast<uint4 *>(prow + ((c ^ (r & 7)) << 4)) = make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-                g_fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's async proxy
+                l_sum[rr] += tile_sum;
             }
-            g_tc_fence_before();    // orders this thread's tcgen05.ld / st before the MMAs released by the arrive
-            __syncwarp();           // one arrival per warp: 128 arrivals on one mbarrier are 128 serialised shared-memory atomics
-            if (lane == 0) g_mbar_arrive(p_full);
+            // ---- O += P V: P from registers, V MN-major [64 keys x 128 d] as loaded from the page
+            g_mbar_wait(v_full + 8 * s, ph);
+            wgmma_reg_fence(o);
+            wgmma_fence();
+            {
+                const uint32_t vb = v_base + s * TC_KV_TILE;
+#pragma unroll
+                for (int k = 0; k < TC_BN / 16; ++k)  // 16 keys = two 8-row groups of 128 B
+                    Wgmma<bf16, TC_D, 1>::rs(o, pa[k], g_wgmma_desc(vb + k * 2048, TC_KV_TILE / 2, 1024), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_reg_fence(o);
+            if (t == 0) g_mbar_arrive(v_empty + 8 * s);
+            if (++s == TC_STAGES) s = 0, ph ^= 1u;
         }
         // ---- epilogue: O / sum -> bf16 -> out[(b*Hq + head) * L + l, :]
-        if (n_tiles > 0) {
-            g_mbar_wait(pv_done, (n_tiles - 1) & 1);
-            g_tc_fence_after();
-        }
-        const size_t out_row = static_cast<size_t>(b * a.Hq + kvh * a.G + g) * a.L + l;
-        if (a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
-            const size_t slot = out_row * a.splits + split;
-            float *po = a.ws_o + slot * TC_D;
 #pragma unroll
-            for (int cb = 0; cb < TC_D / 32; ++cb) {
-                uint32_t ov[32];
-                if (n_tiles > 0) {  // warp-uniform: tcgen05.ld is warp-collective, rows beyond L take part too
-                    g_tmem_ld32(tmem + lane_base + TC_TMEM_O + cb * 32, ov);
-                } else {
+        for (int rr = 0; rr < 2; ++rr) {
+            float lt = l_sum[rr];
+            lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+            lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+            if (l[rr] >= a.L) continue;
+            const size_t out_row = static_cast<size_t>(b * a.Hq + kvh * a.G + g[rr]) * a.L + l[rr];
+            const int col = 2 * (lane & 3);
+            if (a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
+                const size_t slot = out_row * a.splits + split;
+                float *po = a.ws_o + slot * TC_D;
 #pragma unroll
-                    for (int c = 0; c < 32; ++c) ov[c] = 0u;
+                for (int c8 = 0; c8 < TC_D / 8; ++c8)
+                    *reinterpret_cast<float2 *>(po + 8 * c8 + col) = make_float2(o[4 * c8 + 2 * rr], o[4 * c8 + 2 * rr + 1]);
+                if ((lane & 3) == 0) {
+                    a.ws_m[slot] = (m_used[rr] == -CUDART_INF_F || !row_valid[rr]) ? -1e30f : m_used[rr];
+                    a.ws_l[slot] = row_valid[rr] ? lt : 0.f;
                 }
-                if (l < a.L) {
-#pragma unroll
-                    for (int c = 0; c < 32; c += 4)
-                        *reinterpret_cast<uint4 *>(po + cb * 32 + c) = make_uint4(ov[c], ov[c + 1], ov[c + 2], ov[c + 3]);
-                }
-            }
-            if (l < a.L) {
-                a.ws_m[slot] = (m_used == -CUDART_INF_F || !row_valid) ? -1e30f : m_used;
-                a.ws_l[slot] = row_valid ? l_sum : 0.f;
-            }
-        } else {
-        const float inv = (l_sum == 0.f || !row_valid) ? 0.f : 1.0f / l_sum;
-        bf16 *dst = a.out + (a.out_token_major ? (static_cast<size_t>(b) * a.L + l) * a.Hq + (kvh * a.G + g) : out_row) * TC_D;
-#pragma unroll
-        for (int cb = 0; cb < TC_D / 32; ++cb) {
-            uint32_t ov[32];
-            if (n_tiles > 0) {
-                g_tmem_ld32(tmem + lane_base + TC_TMEM_O + cb * 32, ov);
             } else {
+                const float inv = (lt == 0.f || !row_valid[rr]) ? 0.f : 1.0f / lt;
+                bf16 *dst = a.out + (a.out_token_major ? (static_cast<size_t>(b) * a.L + l[rr]) * a.Hq + (kvh * a.G + g[rr]) : out_row) * TC_D;
 #pragma unroll
-                for (int c = 0; c < 32; ++c) ov[c] = 0u;
-            }
-            if (l < a.L) {
-#pragma unroll
-                for (int c = 0; c < 32; c += 8) {
-                    uint4 o;
-                    o.x = pack2<bf16>(__uint_as_float(ov[c]) * inv, __uint_as_float(ov[c + 1]) * inv);
-                    o.y = pack2<bf16>(__uint_as_float(ov[c + 2]) * inv, __uint_as_float(ov[c + 3]) * inv);
-                    o.z = pack2<bf16>(__uint_as_float(ov[c + 4]) * inv, __uint_as_float(ov[c + 5]) * inv);
-                    o.w = pack2<bf16>(__uint_as_float(ov[c + 6]) * inv, __uint_as_float(ov[c + 7]) * inv);
-                    *reinterpret_cast<uint4 *>(dst + cb * 32 + c) = o;
-                }
+                for (int c8 = 0; c8 < TC_D / 8; ++c8)
+                    *reinterpret_cast<uint32_t *>(dst + 8 * c8 + col) = pack2<bf16>(o[4 * c8 + 2 * rr] * inv, o[4 * c8 + 2 * rr + 1] * inv);
             }
         }
-        }
-    }
-    g_tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        g_tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TC_TMEM_COLS) : "memory");
     }
 }
 
@@ -501,10 +385,8 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     }
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
-            cudaFuncSetAttribute(paged_prefill_tc_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess ||
-            cudaFuncSetAttribute(paged_prefill_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
-            cudaFuncSetAttribute(paged_prefill_tc_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+        if (cudaFuncSetAttribute(paged_prefill_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
+            cudaFuncSetAttribute(paged_prefill_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
             return fail(TL_ECUDA, "paged_attention: cannot raise shared memory limit");
         configured = true;
     }
@@ -515,11 +397,10 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     a.tiles_per_split = static_cast<int>(max_tiles < 1 ? 1 : max_tiles);
     if (allow_split && ws != nullptr && !out_token_major) {
         // Split count: the one that minimises waves x (tiles per CTA + fixed cost) + merge launch, in units of one 64-key
-        // tile (~1.45 us of HBM time at a 1/296 share), with 296 CTA slots, ~3 tiles of fixed cost per CTA (set-up, Q load,
-        // epilogue) and 2 + splits / 4 for the merge launch (it reads one partial per split and row).  (The first policy aimed at 4 x #SMs CTAs: at 64 requests x 1024 tokens
-        // that is 1024 CTAs in 3.5 -> 4 waves plus a merge, 60 us, where 512 unsplit CTAs need 2 waves.)
+        // tile, with one CTA slot per SM, ~3 tiles of fixed cost per CTA (set-up, Q load, epilogue) and 2 + splits / 4
+        // for the merge launch (it reads one partial per split and row).
         const long long base = static_cast<long long>(q_blocks) * num_kv_heads * B;
-        const long long slots = 2LL * sm_count();
+        const long long slots = sm_count();
         const size_t rows_total = static_cast<size_t>(rows) * L;
         long long best = 1, best_cost = -1;
         for (long long sp = 1; sp <= 32 && sp <= (max_tiles > 1 ? max_tiles : 1); ++sp) {
@@ -540,9 +421,7 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     }
     dim3 grid(q_blocks * a.splits, num_kv_heads, B);
     if (grid.y > 65535 || grid.z > 65535) return fail(TL_EINVAL, "paged_attention: too many heads / requests for one launch");
-    static const bool p_tmem = [] { const char *e = getenv("TL_FA_P_TMEM"); return e == nullptr || e[0] != '0'; }();  // 0: P through shared memory (control)
-    cudaError_t le = p_tmem ? launch_chained(paged_prefill_tc_kernel<true>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a)
-                            : launch_chained(paged_prefill_tc_kernel<false>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
+    cudaError_t le = launch_chained(paged_prefill_tc_kernel, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
     if (le != cudaSuccess) return fail(TL_ECUDA, "paged_attention: launch failed: %s", cudaGetErrorString(le));
     TL_LAUNCH_CHECK("paged_prefill_tc");
     if (a.splits > 1) return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, rows * L, a.splits, st);

@@ -1,7 +1,7 @@
-"""Build libtiny_llm_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libtiny_llm_b200.so (sm_90a only) in-tree with nvcc.
 
 The reference drives CMake through mlx.extension.CMakeBuild
-(/root/reference/src/extensions_ref/build.py:11-24, CMakeLists.txt:32-84) to
+(src/extensions_ref/build.py:11-24, CMakeLists.txt:32-84) to
 produce a metallib plus a nanobind module; here one nvcc invocation per
 translation unit produces objects that are linked into a C-ABI shared library
 loaded with ctypes.  nvcc cross-compiles without a GPU.
@@ -30,7 +30,6 @@ SOURCES = [
     "elementwise.cu",
     "w4a16_matvec.cu",
     "w4a16_gemm.cu",
-    "w4a16_gemm2.cu",
     "w4a16_skinny.cu",
     "attention_decode.cu",
     "attention_prefill.cu",
@@ -40,7 +39,7 @@ SOURCES = [
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -84,7 +83,7 @@ def build(verbose: bool = False) -> Path:
         objs = list(pool.map(lambda s: _compile(s, verbose), SOURCES))
     newest = max(o.stat().st_mtime for o in objs)
     if not LIB.exists() or LIB.stat().st_mtime < newest:
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static",
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static",
                "-o", str(LIB), *map(str, objs), "-lcuda"]
         proc = subprocess.run(cmd, capture_output=True, text=True)
         if proc.returncode != 0:

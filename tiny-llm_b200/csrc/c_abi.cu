@@ -41,7 +41,7 @@ int sm_count() {
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
             cached = n;
         else
-            cached = 148;
+            cached = 132;  // H100 SXM
     }
     return cached;
 }
@@ -75,8 +75,8 @@ int tl_device_info(int *sms, int *major, int *minor) {
 
 // ------------------------------------------------------------ W4A16 ------
 // Dispatch by activation rows (use_simdgroup): M <= 8 weight-streaming matvec (the reference's matvec limit,
-// quantize.py:162-163); 9..128 swap-AB tcgen05 GEMM with split reduction (w4a16_skinny.cu); above that the
-// 128 x 128-tile tcgen05 GEMM.  The streaming kernel also takes what the tensor-core kernels cannot.
+// quantize.py:162-163); 9..128 swap-AB wgmma GEMM with split reduction (w4a16_skinny.cu); above that the same
+// kernel on 128-token tiles.  The streaming kernel also takes what the tensor-core kernels cannot.
 static bool use_skinny_kernel(int M, int N, int K, int dtype, int use_simdgroup) {
     return use_simdgroup && M > TL_MATVEC_REF_ROWS && w4a16_skinny_supported(M, N, K, dtype);
 }
@@ -255,7 +255,7 @@ int tl_paged_attention_token_major(const void *q, const void *key_pages, const v
     if (!q || !key_pages || !value_pages || !block_table || !context_lens || !out) return fail(TL_EINVAL, "paged_attention: null pointer");
     if (!paged_prefill_tc_supported(L, num_pages, page_size, num_kv_heads, num_heads) || !aligned16(q) || !aligned16(out) || !aligned16(key_pages) ||
         !aligned16(value_pages))
-        return fail(TL_EINVAL, "paged_attention_token_major: needs the tcgen05 kernel (bf16, D = 128, pages a multiple of 64 slots)");
+        return fail(TL_EINVAL, "paged_attention_token_major: needs the wgmma kernel (bf16, D = 128, pages a multiple of 64 slots)");
     return launch_paged_prefill_tc(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages, scale,
                                    is_causal, num_kv_heads, num_heads, false, nullptr, 0, as_stream(stream), true);
 }
@@ -405,16 +405,9 @@ extern "C" int tl_debug_trace(unsigned long long *device_events, unsigned int *d
     trace_bind_matvec(device_events, device_count, capacity);
     trace_bind_attention(device_events, device_count, capacity);
     trace_bind_skinny(device_events, device_count, capacity);
-    trace_bind_gemm(device_events, device_count, capacity);
-    trace_bind_gemm2(device_events, device_count, capacity);
     return TL_OK;
 }
 #endif
-
-int tl_set_gemm_pairs(int mode) {
-    set_gemm_pairs(mode);
-    return TL_OK;
-}
 
 int tl_set_pdl(int enabled) {
     set_use_pdl(enabled != 0);

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels of tiny-llm_b200.
+// Shared device/host helpers for the sm_90a kernels of tiny-llm_b200.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -129,7 +129,7 @@ __device__ __forceinline__ __half ld_cg(const __half *p) {
 // running (the predecessor lets it in with griddep_launch(), or implicitly by exiting).  It must execute
 // griddep_wait() before it reads anything the predecessor wrote and before it writes anything the predecessor may
 // still read; the wait returns once the predecessor grid has COMPLETED and its writes are visible.  Everything a
-// kernel does before the wait (barrier init, TMEM allocation, tensor-map prefetch, weight prefetch) overlaps the
+// kernel does before the wait (barrier init, tensor-map prefetch, weight prefetch) overlaps the
 // predecessor's tail.  Data written by an earlier kernel of such a chain is read through L2 (ld_cg / TMA), never
 // through a possibly stale L1 line.
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -1,12 +1,11 @@
 // Fused decode attention for the Week-3 Qwen3 model (bf16, paged KV, L == 1): one launch does
 // q/k RMSNorm -> RoPE -> K/V append -> paged GQA attention for every (request, KV head), i.e. the
 // operator sequence rms_norm x2 -> rope x2 -> paged_cache_update x2 -> paged_attention of
-// /root/reference/src/tiny_llm_ref/qwen3_week3.py:62-105 with the kernel arithmetic of
-// /root/reference/src/extensions_ref/src/paged_attention.metal:108-248, every rounding point kept.
+// src/tiny_llm_ref/qwen3_week3.py:62-105 with the kernel arithmetic of
+// src/extensions_ref/src/paged_attention.metal:108-248, every rounding point kept.
 //
-// (Round 1 also carried a whole-step persistent kernel in this file; it lost to the CUDA-graph +
-// programmatic-dependent-launch path by 1.8x - 0.63 ms of grid barriers and 0.47 ms of staging per
-// token, profiles/r01_mega_timeline.json - and was retired in round 2.)
+// (An earlier whole-step persistent kernel in this file lost to the CUDA-graph + programmatic-dependent-launch
+// path - its time went to grid barriers and staging - and was retired.)
 #include <algorithm>
 #include <stdlib.h>
 #include <math_constants.h>

@@ -3,7 +3,7 @@
 // 128-bit coalesced accesses when alignment allows, fp32 math, one rounding.
 //
 // Arithmetic follows the reference Metal kernels (paths relative to
-// /root/reference/src/extensions_ref/src): week2_kernels.metal:6-117,
+// src/extensions_ref/src): week2_kernels.metal:6-117,
 // quantized_matmul.metal:58-89, paged_attention.metal:82-106.
 #include <float.h>
 #include <limits.h>
@@ -194,8 +194,8 @@ __global__ void rope_kernel(const T *__restrict__ x, const int32_t *__restrict__
 }
 
 // Prefill-sized inputs, full rotation (dims == D): one thread per (b, l, pair) forms the frequency
-// (double exp2/log2) and sincosf ONCE and walks the H heads - the per-element kernel above spent
-// 77 us per call at L = 4096 recomputing them 32 times over.
+// (double exp2/log2) and sincosf ONCE and walks the H heads - the per-element kernel above recomputes
+// them once per head.
 template <typename T>
 __global__ void rope_heads_kernel(const T *__restrict__ x, const int32_t *__restrict__ offsets, T *__restrict__ out, int B, int L,
                                   int H, int D, float base, int traditional) {
@@ -702,9 +702,8 @@ __global__ void decode_qk_norm_rope_append_kernel(const T *qkv, const T *__restr
 // w + 16, ...; lane l owns the RoPE pairs (l, l + 64) and (l + 32, l + 96), so the angle arithmetic (a double-precision
 // exp2 and a sincosf per pair) is done once per lane instead of once per head, and the sum of squares is two warp
 // reductions.  All of a warp's loads are issued before the first is used (one L2
-// round trip; a first version that walked its heads one after the other was SLOWER than the one-CTA-per-head form:
-// 9.8 vs 5.8 us at 64 rows).  Measured (ncu, per layer): 8.7 -> 6.3 us for a 128-token chunk, 5.8 -> 6.4 us at 64
-// rows - a dependent-latency chain either way (load -> trig -> norm -> store), the gain is the chunk's 6144 tiny CTAs.  Bit-identical to the per-head kernel: the squares are added in the same tree (pairs
+// round trip; a first version that walked its heads one after the other was slower than the one-CTA-per-head form).
+// A dependent-latency chain either way (load -> trig -> norm -> store); the gain is the chunk's 6144 tiny CTAs.  Bit-identical to the per-head kernel: the squares are added in the same tree (pairs
 // 0..31 and 32..63 reduced separately, then summed).
 constexpr int QKN_WARPS = 16, QKN_MAXH = 4;  // up to 64 heads (q + k + v) per row
 // PLANES: qkv does not exist in memory - its rows are still the fp32 partial planes of the q|k|v projection's split

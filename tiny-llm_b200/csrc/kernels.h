@@ -54,13 +54,7 @@ int launch_w4a16_vanilla(const void *scales, const void *biases, const void *a, 
                          int N, int K, int dtype, cudaStream_t st);
 
 
-// w4a16_gemm2.cu (CTA pairs, tcgen05 cta_group::2: M > 256)
-bool w4a16_gemm2_supported(int M, int N, int K, int dtype);
-void set_gemm_pairs(int mode);  // 0 never, 1 where the pair grid fills the SMs (default), 2 every M > 256
-int launch_w4a16_gemm2(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
-                       cudaStream_t st);
-
-// w4a16_skinny.cu (swap-AB tcgen05 GEMM with split reduction, 9 <= M <= 128)
+// w4a16_skinny.cu (swap-AB wgmma GEMM: split reduction for 9 <= M <= 128, 128-token tiles for prefill)
 bool w4a16_skinny_supported(int M, int N, int K, int dtype);
 int w4a16_skinny_splits(int M, int N, int K);
 size_t w4a16_skinny_workspace(int M, int N, int K);
@@ -71,12 +65,14 @@ int launch_w4a16_skinny(const void *scales, const void *biases, const void *a, c
                         float norm_eps = 0.f, void *normed = nullptr, bool *norm_done = nullptr, int *planes_out = nullptr);
 // planes_out (optional): with a split reduction the launch stops after the GEMM (partial planes [splits][M][K] fp32 in the
 // workspace, *planes_out = splits) and the caller's fused kernel adds them; *planes_out = 1 means `out` is complete
+int launch_w4a16_tiles(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
+                       cudaStream_t st);
 bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype);
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,
                                   int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages, cudaStream_t st, bool chunk);
 
-// w4a16_gemm.cu (tcgen05 prefill GEMM)
+// w4a16_gemm.cu (prefill GEMM: dispatch onto launch_w4a16_tiles)
 bool w4a16_gemm_supported(int M, int N, int K, int dtype);
 int w4a16_gemm_split(int M, int N, int K, int use_split_k);
 size_t w4a16_gemm_workspace(int M, int N, int K, int dtype, int use_split_k);
@@ -88,8 +84,6 @@ int launch_w4a16_gemm(const void *scales, const void *biases, const void *a, con
 void trace_bind_matvec(unsigned long long *buf, unsigned int *n, unsigned int cap);
 void trace_bind_attention(unsigned long long *buf, unsigned int *n, unsigned int cap);
 void trace_bind_skinny(unsigned long long *buf, unsigned int *n, unsigned int cap);
-void trace_bind_gemm(unsigned long long *buf, unsigned int *n, unsigned int cap);
-void trace_bind_gemm2(unsigned long long *buf, unsigned int *n, unsigned int cap);
 #endif
 size_t decode_attention_fused_workspace(int batch, int num_heads, int num_kv_heads);
 int launch_decode_attention_fused(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
@@ -108,14 +102,14 @@ int launch_paged_decode(const void *q, const void *kp, const void *vp, const int
                         int is_causal, int num_kv_heads, int num_heads, int dtype, void *ws, size_t ws_bytes,
                         cudaStream_t st);
 
-// attention_prefill_tc.cu (tcgen05 + TMA flash prefill; page_size % 64 == 0, Hq/Hkv divides 128)
+// attention_prefill_tc.cu (wgmma + TMA flash prefill; page_size % 64 == 0, Hq/Hkv divides 128)
 bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_heads, int num_heads);
 int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, bool allow_split, void *ws, size_t ws_bytes, cudaStream_t st, bool out_token_major = false);
 int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws_l, void *out, int rows_total, int splits, cudaStream_t st);
 
-// attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the tcgen05 kernel does not take)
+// attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the wgmma kernel does not take)
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, cudaStream_t st);

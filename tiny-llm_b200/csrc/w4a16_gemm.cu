@@ -1,310 +1,21 @@
-// W4A16 prefill GEMM on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// W4A16 prefill GEMM on the Hopper tensor cores: dispatch onto the swap-AB wgmma kernel of w4a16_skinny.cu with
+// 128-token tiles (launch_w4a16_tiles), plus the tensor-map encoder shared by the TMA kernels.
 //
 //   out[m, n] = sum_k a[m, k] * T(code[n, k] * scale[n, k/128] + bias[n, k/128])
 //
-// (reference naming: a [M, N_red], b [K_out, N_red/8]; in this file m = token,
-// n = output feature, k = reduction index).  Replaces
-// quantized_matmul_simdgroup_w4a16_g128 (/root/reference/src/extensions_ref/src/
-// quantized_matmul.metal:96-249): like that kernel the weight is rounded to the
-// activation dtype when it is dequantised into shared memory (:183-194) and the
-// accumulation is fp32.
-//
-// One CTA computes a 128 (tokens) x 128 (features) tile; the reduction runs in
-// 64-element blocks through a 4-stage shared-memory ring:
-//   warp 0        : TMA producer - the activation tile [128 x 64] bf16 arrives by
-//                   cp.async.bulk.tensor with the 128-byte swizzle (tokens beyond M
-//                   are zero-filled by the TMA unit);
-//   warps 4..11   : dequantisers - thread (row, half) reads 16 packed bytes of weight
-//                   row `row`, turns 32 codes into bf16 (LOP3 magic -> exact q ->
-//                   one HFMA2 for q*scale+bias, a single rounding) and stores them in
-//                   the same K-major 128B-swizzled layout the MMA expects, then
-//                   fence.proxy.async + mbarrier arrive;
-//   warp 1        : one elected thread issues tcgen05.mma (M128 N128 K16, bf16 x bf16
-//                   -> fp32 in TMEM) four times per stage and tcgen05.commit's the
-//                   stage back to the producers;
-//   warps 4..11   : epilogue - tcgen05.ld the fp32 accumulators (one TMEM lane = one
-//                   token row per thread), round to the output dtype, 16-byte stores.
-// Packed weights are read once per 128-token tile (L2 absorbs the re-reads across
-// token tiles); activations are read once per 128-feature tile.
+// (reference naming: a [M, N_red], b [K_out, N_red/8]; here m = token, n = output feature, k = reduction index).
+// Replaces quantized_matmul_simdgroup_w4a16_g128 (src/extensions_ref/src/quantized_matmul.metal:96-249):
+// like that kernel the weight is rounded to the activation dtype when it is dequantised into shared memory (:183-194)
+// and the accumulation is fp32.
 #include <cuda.h>
 #include <stdlib.h>
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
 #include "kernels.h"
-#include "tc05.cuh"
-#include "trace.cuh"
+#include "wgmma.cuh"
 
 namespace tl {
-
-constexpr int GM = 128;       // tokens per tile   (UMMA M)
-constexpr int GN = 128;       // features per tile (UMMA N)
-constexpr int GK = 64;        // reduction elements per stage (128 bytes: one swizzle atom)
-constexpr int GSTAGES_MAX = 4;  // stages of the shared-memory ring (MT <= 2); 3 for MT = 4: 80 KiB per stage
-constexpr int G_DEQ_WARPS = 8;
-constexpr int G_THREADS = (4 + G_DEQ_WARPS) * 32;
-constexpr int G_TILE_BYTES = GM * GK * 2;  // 16 KiB, same for A and B tiles
-constexpr int G_TMEM_COLS = 128;
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows are 128 B
-// apart, 8-row groups 1024 B apart (stride byte offset), descriptor version 1 (sm_100).
-__device__ __forceinline__ uint64_t g_smem_desc(uint32_t addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((addr & 0x3FFFFu) >> 4);          // [0,14)  start address / 16
-    d |= static_cast<uint64_t>(0) << 16;                          // [16,30) leading byte offset (unused for swizzled K-major)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // [32,46) stride byte offset / 16
-    d |= static_cast<uint64_t>(1) << 46;                          // [46,48) descriptor version
-    d |= static_cast<uint64_t>(2) << 61;                          // [61,64) layout: SWIZZLE_128B
-    return d;
-}
-
-// kind::f16 instruction descriptor: fp32 accumulate, A/B both K-major.
-template <typename T>
-__host__ __device__ constexpr uint32_t g_instr_desc() {
-    const uint32_t fmt = sizeof(T) == 2 && std::is_same<T, __nv_bfloat16>::value ? 1u : 0u;  // 0 = f16, 1 = bf16
-    return (1u << 4)            // c_format = f32
-           | (fmt << 7)         // a_format
-           | (fmt << 10)        // b_format
-           | (0u << 15)         // a_major = K
-           | (0u << 16)         // b_major = K
-           | ((GN >> 3) << 17)  // n_dim
-           | ((GM >> 4) << 24); // m_dim
-}
-
-template <typename T>
-struct Deq;
-template <>
-struct Deq<__nv_bfloat16> {
-    using V2 = __nv_bfloat162;
-    static constexpr uint32_t MAGIC = 0x43004300u;  // (128, 128)
-};
-template <>
-struct Deq<__half> {
-    using V2 = __half2;
-    static constexpr uint32_t MAGIC = 0x64006400u;  // (1024, 1024)
-};
-
-// MT token tiles (128 rows each) share one dequantised weight tile per stage: the dequantisers are
-// the busiest warps of this kernel, and with MT = 2 their work per flop halves (measured at
-// M = 4096 with MT = 1: 470-550 TF/s, 28-33 % of the bf16 peak).
-template <int MT>
-struct GemmSmem {
-    static constexpr int STAGES = MT <= 2 ? GSTAGES_MAX : 2;
-    static constexpr int A_STAGE = MT * G_TILE_BYTES;
-    static constexpr int A_OFF = 0;
-    static constexpr int B_OFF = STAGES * A_STAGE;
-    static constexpr int BAR_OFF = B_OFF + STAGES * G_TILE_BYTES;
-    static constexpr int BYTES = BAR_OFF + 256;
-};
-
-template <typename T, int MT>
-__global__ void __launch_bounds__(G_THREADS, 1) w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const T *__restrict__ scales,
-                                                                  const T *__restrict__ biases, const uint32_t *__restrict__ b,
-                                                                  T *__restrict__ out, int M, int N, int K, int vec_store) {
-    extern __shared__ __align__(1024) unsigned char gsm[];
-#if TL_TRACE
-    // per-block cycle stamps of CTA (0,0) (tools/gemm_blocks.py): role 0 = MMA warp (k: activation tile ready, weight tile
-    // ready, MMAs issued), role 1 = first dequantiser thread (k: loop top, math done, stage free, handed over)
-    __shared__ unsigned long long trc[2][40][4];
-#define G_TRC(role, i, k)                                                                                                    \
-    do {                                                                                                                     \
-        if (blockIdx.x == 0 && blockIdx.y == 0 && (threadIdx.x & 31) == 0 && (i) < 40) trc[role][i][k] = clock64();         \
-    } while (0)
-#else
-#define G_TRC(role, i, k) do { } while (0)
-#endif
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n_tile = blockIdx.x, m_tile = blockIdx.y;
-    const int num_kb = N / GK;
-    const int G = N / 128;
-
-    using Smem = GemmSmem<MT>;
-    constexpr int GSTAGES = Smem::STAGES;
-    constexpr int TMEM_COLS = G_TMEM_COLS * MT;
-    const uint32_t a_base = g_smem_u32(gsm + Smem::A_OFF);
-    const uint32_t b_base = g_smem_u32(gsm + Smem::B_OFF);
-    const uint32_t bar_base = g_smem_u32(gsm + Smem::BAR_OFF);
-    // ONE "full" barrier per stage: the TMA's expect_tx arrival + byte count and the eight dequantiser warps arrive on
-    // it, so the MMA warp pays one try_wait (~90 cycles) per block, not two: whatever it executes between the last MMA
-    // of a block and the first of the next is time the tensor core idles (its queue holds one or two MMAs).
-    const uint32_t full = bar_base, empty = bar_base + 8 * GSTAGES;
-    const uint32_t tmem_full = bar_base + 16 * GSTAGES;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(gsm + Smem::BAR_OFF + 16 * GSTAGES + 8);
-
-    if (warp == 0 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < GSTAGES; ++i) {
-            g_mbar_init(full + 8 * i, 1 + G_DEQ_WARPS);  // the producer's expect_tx arrival + one per dequantiser warp
-            g_mbar_init(empty + 8 * i, 1);
-        }
-        g_mbar_init(tmem_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(g_smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    g_tc_fence_before();
-    __syncthreads();
-    g_tc_fence_after();
-    const uint32_t tmem_d = *tmem_slot;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer (activations): whole warp, one elected lane issues
-        int s = 0;
-        uint32_t ph = 1;  // producer side: the first pass through the ring does not wait
-        for (int kb = 0; kb < num_kb; ++kb) {
-            g_mbar_wait(empty + 8 * s, ph);
-            if (g_elect_one()) {
-                g_mbar_expect_tx(full + 8 * s, Smem::A_STAGE);
-#pragma unroll
-                for (int i = 0; i < MT; ++i)  // token rows beyond M are zero-filled by the TMA unit
-                    g_tma_load_2d(a_base + s * Smem::A_STAGE + i * G_TILE_BYTES, &tmap_a, kb * GK, (m_tile * MT + i) * GM, full + 8 * s);
-            }
-            __syncwarp();
-            if (++s == GSTAGES) s = 0, ph ^= 1u;
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer
-        // The whole warp walks the loop (uniform control flow, running stage / phase counters instead of a division per
-        // block), one elected lane issues: behind `if (lane == 0)` the compiler wrapped every tcgen05 instruction in an
-        // ELECT loop and moved its operands through R2UR - ~1000 cycles of issue latency per reduction block, more than
-        // the 512 cycles of tensor work of a two-tile stage (tc05.cuh: g_elect_one).
-        constexpr uint32_t idesc = g_instr_desc<T>();
-        const uint64_t adesc0 = g_smem_desc(a_base), bdesc0 = g_smem_desc(b_base);
-        int s = 0;
-        uint32_t ph = 0;
-        for (int kb = 0; kb < num_kb; ++kb) {
-            g_mbar_wait(full + 8 * s, ph);
-            G_TRC(0, kb, 0);
-            G_TRC(0, kb, 1);
-            g_tc_fence_after();
-            if (g_elect_one()) {
-                const uint64_t bdesc = bdesc0 + static_cast<uint64_t>(s * (G_TILE_BYTES >> 4));
-#pragma unroll
-                for (int i = 0; i < MT; ++i) {
-                    const uint64_t adesc = adesc0 + static_cast<uint64_t>((s * Smem::A_STAGE + i * G_TILE_BYTES) >> 4);
-#pragma unroll
-                    for (int k = 0; k < GK / 16; ++k)  // +32 bytes along K per step: +2 in the (addr >> 4) field
-                        g_tc_mma(tmem_d + i * G_TMEM_COLS, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                g_tc_commit(empty + 8 * s);  // stage reusable once these MMAs have read it
-            }
-            __syncwarp();
-            G_TRC(0, kb, 2);
-            if (++s == GSTAGES) s = 0, ph ^= 1u;
-        }
-        if (g_elect_one()) g_tc_commit(tmem_full);
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ------------------------------------------------ dequantisers, then epilogue
-        const int dt = threadIdx.x - 128;      // 0 .. 255
-        // adjacent lanes = the two 16-byte halves of ONE weight row: a warp's load touches 16 full 32-byte sectors (the
-        // first version mapped lane <-> row, 32 half-used sectors per load, each fetched again by the warp holding the other half)
-        const int row = dt >> 1;               // feature row of the tile
-        const int half = dt & 1;               // which 32 of the stage's 64 reduction elements
-        const int n = min(n_tile * GN + row, K - 1);
-        const uint32_t *wrow = b + static_cast<size_t>(n) * (N / 8);
-        const T *srow = scales + static_cast<size_t>(n) * G;
-        const T *crow = biases + static_cast<size_t>(n) * G;
-        using V2 = typename Deq<T>::V2;
-        const uint32_t magic = Deq<T>::MAGIC;
-        const V2 offset2 = *reinterpret_cast<const V2 *>(&magic);
-        uint4 packed = *reinterpret_cast<const uint4 *>(wrow + half * 4);
-        T sc_next = srow[0], bi_next = crow[0];
-        for (int kb = 0; kb < num_kb; ++kb) {
-            const int s = kb % GSTAGES;
-            const uint32_t ph = (kb / GSTAGES) & 1;
-            if (warp == 4) G_TRC(1, kb, 0);
-            const uint4 cur = packed;
-            const T sc = sc_next, bi = bi_next;
-            if (kb + 1 < num_kb) {  // next block's words and scale pair: one round trip ahead of their use
-                packed = *reinterpret_cast<const uint4 *>(wrow + (kb + 1) * 8 + half * 4);
-                sc_next = srow[(kb + 1) >> 1], bi_next = crow[(kb + 1) >> 1];
-            }
-            V2 s2, b2;
-            s2.x = sc, s2.y = sc, b2.x = bi, b2.y = bi;
-            uint32_t outw[16];
-            const uint32_t wv[4] = {cur.x, cur.y, cur.z, cur.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                uint32_t p[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    uint32_t bits = ((wv[j] >> (4 * i)) & 0x000F000Fu) | magic;  // (128 + q_i, 128 + q_{i+4})
-                    V2 q = __hsub2(*reinterpret_cast<V2 *>(&bits), offset2);     // exact codes
-                    V2 v = __hfma2(q, s2, b2);                                    // q*scale+bias, one rounding
-                    p[i] = *reinterpret_cast<uint32_t *>(&v);
-                }
-                outw[4 * j + 0] = __byte_perm(p[0], p[1], 0x5410);  // (e0, e1)
-                outw[4 * j + 1] = __byte_perm(p[2], p[3], 0x5410);  // (e2, e3)
-                outw[4 * j + 2] = __byte_perm(p[0], p[1], 0x7632);  // (e4, e5)
-                outw[4 * j + 3] = __byte_perm(p[2], p[3], 0x7632);  // (e6, e7)
-            }
-            if (warp == 4) G_TRC(1, kb, 1);
-            g_mbar_wait(empty + 8 * s, ph ^ 1);
-            if (warp == 4) G_TRC(1, kb, 2);
-            unsigned char *tile = gsm + Smem::B_OFF + s * G_TILE_BYTES + row * 128;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int chunk = half * 4 + j;  // 16-byte chunk (8 elements) along K
-                *reinterpret_cast<uint4 *>(tile + ((chunk ^ (row & 7)) << 4)) =
-                    make_uint4(outw[4 * j], outw[4 * j + 1], outw[4 * j + 2], outw[4 * j + 3]);
-            }
-            g_fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's async proxy
-            __syncwarp();           // one arrival per warp instead of 256 serialised shared-memory atomics per stage
-            if (lane == 0) g_mbar_arrive(full + 8 * s);
-            if (warp == 4) G_TRC(1, kb, 3);
-        }
-        // ---- epilogue: TMEM lane = token row; warps 4-7 take columns 0..63, warps 8-11 columns 64..127
-        g_mbar_wait(tmem_full, 0);
-        g_tc_fence_after();
-        const int q = warp & 3;                 // TMEM lane quarter this warp may access
-        const int col_half = (warp - 4) >> 2;   // 0 or 1
-#pragma unroll
-        for (int cbi = 0; cbi < 2 * MT; ++cbi) {
-            const int i = cbi >> 1, cb = cbi & 1;
-            const int m = (m_tile * MT + i) * GM + q * 32 + lane;
-            const int col0 = col_half * 64 + cb * 32;
-            uint32_t v[32];
-            g_tmem_ld32(tmem_d + (static_cast<uint32_t>(q * 32) << 16) + i * G_TMEM_COLS + col0, v);
-            if (m < M) {
-                T *dst = out + static_cast<size_t>(m) * K + n_tile * GN + col0;
-                const int valid = min(32, K - (n_tile * GN + col0));
-                if (vec_store && valid == 32) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        uint4 o;
-                        o.x = pack2<T>(__uint_as_float(v[8 * j + 0]), __uint_as_float(v[8 * j + 1]));
-                        o.y = pack2<T>(__uint_as_float(v[8 * j + 2]), __uint_as_float(v[8 * j + 3]));
-                        o.z = pack2<T>(__uint_as_float(v[8 * j + 4]), __uint_as_float(v[8 * j + 5]));
-                        o.w = pack2<T>(__uint_as_float(v[8 * j + 6]), __uint_as_float(v[8 * j + 7]));
-                        *reinterpret_cast<uint4 *>(dst + 8 * j) = o;
-                    }
-                } else {
-                    for (int j = 0; j < valid; ++j) dst[j] = from_f<T>(__uint_as_float(v[j]));
-                }
-            }
-        }
-    }
-    g_tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        g_tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(TMEM_COLS) : "memory");
-    }
-#if TL_TRACE
-    if (blockIdx.x == 0 && blockIdx.y == 0 && g_trace_buf != nullptr) {  // tag = 20000 + role * 1000 + block * 4 + k
-        for (int e = threadIdx.x; e < 2 * 40 * 4; e += G_THREADS) {
-            const int role = e / 160, rest = e - role * 160;
-            if (rest / 4 < num_kb && !(role == 0 && (rest & 3) == 3)) {
-                const unsigned at = atomicAdd(g_trace_n, 1u);
-                if (at < g_trace_cap) g_trace_buf[2 * at] = 20000 + role * 1000 + rest, g_trace_buf[2 * at + 1] = trc[role][rest / 4][rest & 3];
-            }
-        }
-    }
-#endif
-}
 
 // ---------------------------------------------------------------- host side --
 PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
@@ -320,80 +31,27 @@ PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
     return fn;
 }
 
-static bool gemm_disabled() {
-    static int cached = -1;
-    if (cached < 0) {
-        const char *e = getenv("TL_NO_TCGEN05");
-        cached = (e != nullptr && e[0] == '1') ? 1 : 0;
-    }
-    return cached == 1;
+// TL_NO_TC_GEMM=1: M > 128 projections on the streaming kernel instead (A/B control).
+static bool tc_gemm_disabled() {
+    static const bool off = [] { const char *e = getenv("TL_NO_TC_GEMM"); return e != nullptr && e[0] == '1'; }();
+    return off;
 }
 
 bool w4a16_gemm_supported(int M, int N, int K, int dtype) {
-    if (gemm_disabled()) return false;
+    if (tc_gemm_disabled()) return false;
     return (dtype == TL_BF16 || dtype == TL_F16) && M > 0 && K > 0 && N % 128 == 0;
 }
 
-// The B200 schedule never splits the reduction: a 128x128 tile already runs N/64
-// MMA stages back to back, and small-M problems go to the streaming kernel.  A
-// split-K request therefore runs the very same kernel (bit-identical results,
-// tests_refsol/test_week_2_day_7.py:80-109).
+// The schedule never splits the reduction: a 128 x 128 tile already runs N/128 group blocks back to back, and
+// small-M problems go to the streaming or split-reduction kernels.  A split-K request therefore runs the very same
+// kernel (bit-identical results, tests_refsol/test_week_2_day_7.py:80-109).
 int w4a16_gemm_split(int, int, int, int) { return 1; }
 size_t w4a16_gemm_workspace(int, int, int, int, int) { return 0; }
 
-template <typename T, int MT>
-static int gemm_launch(const CUtensorMap &map, const void *scales, const void *biases, const void *b, void *out, int M, int N, int K,
-                       int vec_store, cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(w4a16_gemm_kernel<T, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<MT>::BYTES);
-        if (e != cudaSuccess) return fail(TL_ECUDA, "quantized_matmul: cannot raise shared memory limit: %s", cudaGetErrorString(e));
-        configured = true;
-    }
-    dim3 grid(ceil_div(K, GN), ceil_div(M, GM * MT));
-    w4a16_gemm_kernel<T, MT><<<grid, G_THREADS, GemmSmem<MT>::BYTES, st>>>(map, static_cast<const T *>(scales), static_cast<const T *>(biases),
-                                                                           static_cast<const uint32_t *>(b), static_cast<T *>(out), M, N, K,
-                                                                           vec_store);
-    TL_LAUNCH_CHECK("w4a16_gemm");
-    return TL_OK;
-}
-
-template <typename T>
-static int gemm_t(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K,
-                  cudaStream_t st) {
-    PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-    if (encode == nullptr) return fail(TL_ECUDA, "quantized_matmul: cuTensorMapEncodeTiled is unavailable");
-    if (!aligned16(a) || !aligned16(b)) return fail(TL_EINVAL, "quantized_matmul: a and b must be 16-byte aligned");
-    CUtensorMap map;
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(N), static_cast<cuuint64_t>(M)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(N) * 2};
-    const cuuint32_t box[2] = {GK, GM};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    CUresult r = encode(&map, dt, 2, const_cast<void *>(a), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(TL_ECUDA, "quantized_matmul: cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-    const int vec_store = (K % 8 == 0 && aligned16(out)) ? 1 : 0;
-    // Four token tiles per CTA leave room for a 2-stage ring only: measured at M = 4096, that wins for the
-    // short reductions (N = 2560: q|k|v 641 -> 769 TF/s, gate|up 782 -> 882) and loses for the long ones
-    // (N = 9728: 706 -> 655), so it is used up to N = 3072.  TL_GEMM_MT caps the tile count (A/B runs).
-    static const int mt_max = [] { const char *e = getenv("TL_GEMM_MT"); return e ? atoi(e) : 4; }();
-    if (M > 2 * GM && mt_max >= 4 && N <= 3072) return gemm_launch<T, 4>(map, scales, biases, b, out, M, N, K, vec_store, st);
-    return M > GM && mt_max >= 2 ? gemm_launch<T, 2>(map, scales, biases, b, out, M, N, K, vec_store, st)
-                                 : gemm_launch<T, 1>(map, scales, biases, b, out, M, N, K, vec_store, st);
-}
-
 int launch_w4a16_gemm(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K,
                       int dtype, int /*use_split_k*/, void * /*ws*/, size_t /*ws_bytes*/, cudaStream_t st) {
-    if (M == 0 || K == 0) return TL_OK;
-    if (w4a16_gemm2_supported(M, N, K, dtype)) return launch_w4a16_gemm2(scales, biases, a, b, out, M, N, K, dtype, st);  // CTA pairs
-    if (dtype == TL_BF16) return gemm_t<__nv_bfloat16>(scales, biases, a, b, out, M, N, K, st);
-    if (dtype == TL_F16) return gemm_t<__half>(scales, biases, a, b, out, M, N, K, st);
-    return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    if (dtype != TL_BF16 && dtype != TL_F16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    return launch_w4a16_tiles(scales, biases, a, b, out, M, N, K, dtype, st);
 }
-
-#if TL_TRACE
-void trace_bind_gemm(unsigned long long *buf, unsigned int *n, unsigned int cap) { trace_bind(buf, n, cap); }
-#endif
 
 }  // namespace tl

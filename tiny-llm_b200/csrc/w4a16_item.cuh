@@ -1,10 +1,8 @@
 // Building blocks of the W4A16 weight-streaming kernel (w4a16_matvec.cu): activation staging,
 // the register-pipelined weight unit and the tensor-core consumer.
 //
-// Why this shape (measured on B200, profiles/r01_kbench_*): the first three streaming kernels
-// all stalled at ~2 TB/s no matter how the bytes were fetched.  SASS of the cp.async-ring
-// version showed 334 instructions per 1-KiB weight group per warp - the kernel was
-// instruction-issue bound, not memory bound.  The budget below is ~100 per KiB:
+// Why this shape: the earlier streaming kernels were instruction-issue bound, not memory bound
+// (SASS of the cp.async-ring version: 334 instructions per 1-KiB weight group per warp).  The budget below is ~100 per KiB:
 //
 //   * weights go global -> registers (ld.global.nc, 128-bit, immediate offsets from one running
 //     pointer per row); no shared-memory ring, so no LDGSTS, no wait_group/syncwarp, no slot math;
@@ -28,7 +26,7 @@ namespace tl {
 // a single LOP3 with the mask read from the constant bank.
 static __constant__ uint32_t k_w4_mask = 0x000F000Fu;
 // Experiment switch: x >> s as the high word of x * 2^(32-s) (IMAD.HI, FMA pipe) instead of SHF
-// (ALU pipe).  Measured slower on B200 (lm_head 56 -> 69 us): kept only for the record.
+// (ALU pipe).  Off by default; kept as an A/B switch.
 #ifndef W4_SHR_IMADHI
 #define W4_SHR_IMADHI 0
 #endif

@@ -3,10 +3,10 @@
 //   out[m, k] = sum_n a[m, n] * (code[k, n] * scale[k, n/128] + bias[k, n/128])
 //
 // a [M, N] (bf16|f16), b [K, N/8] packed u32 (code i of a word = (w >> 4i) & 15,
-// /root/reference/src/tiny_llm_ref/quantize.py:113-115), scales/biases [K, N/128].
+// src/tiny_llm_ref/quantize.py:113-115), scales/biases [K, N/128].
 //
 // w4a16_stream5_kernel is the decode kernel (reference: quantized_matvec_x4_fast,
-// /root/reference/src/extensions_ref/src/quantized_matmul.metal:441-538): every packed
+// src/extensions_ref/src/quantized_matmul.metal:441-538): every packed
 // weight byte is read exactly once with 128-bit loads that bypass L1; activations (tiny,
 // shared by every CTA) are staged once per CTA in shared memory.  The per-weight ALU work
 // would exceed the HBM time on CUDA cores (~3 ops/weight), so the 16 x 128 code tile of
@@ -36,13 +36,8 @@ int launch_w4a16_stream(const void *scales, const void *biases, const void *a, c
 // v5: register-pipelined streaming, contiguous rows per CTA (see w4a16_item.cuh for the
 // instruction budget of the inner loop).
 //
-// History, all measured on B200 (profiles/r01_kbench_*, tools/s4_timeline.py):
-//   v1 (register prefetch, 2 KB in flight per warp), v2 (producer warp + 256-byte cp.async.bulk
-//   ring) and v3 (per-warp cp.async rings) stalled near 2 TB/s: ~330 instructions per KiB of
-//   weights - issue bound.  v4 (register pipeline, ~120 instructions per KiB) reached 3.9 TB/s on
-//   the tied head but dealt 16-row tiles to fixed-size warp teams: 1216 tiles over 1184 teams
-//   made 32 teams work twice as long as the rest (gate|up: 11 us instead of 6), and every tile
-//   ended with two named barriers and a dependent residual load.
+// Earlier forms - register prefetch, a producer warp with a cp.async.bulk ring, per-warp cp.async rings - were
+// instruction-issue bound; fixed-size 16-row tiles dealt to warp teams left a tail of teams working twice as long.
 // v5 gives CTA c the contiguous rows of chunks [C*c/grid, C*(c+1)/grid) (C = K/16 chunks, all
 // CTAs within one chunk of each other) and deals the CTA's (chunk, unit) pairs to its warps as
 // equal contiguous ranges.  A warp accumulates a chunk in registers and parks the partial sums in
@@ -61,22 +56,19 @@ int launch_w4a16_stream(const void *scales, const void *biases, const void *a, c
 //   epilogue RESIDUAL: out = T(float(res) + float(T(acc)))   (qwen3_week3.py:204-206)
 //   epilogue SWIGLU_PAIRS: rows 16c+r / 16c+8+r hold gate / up feature 8c+r;
 //                     out[m, 8c+r] = T(silu(T(acc_gate)) * T(acc_up))  (week2_kernels.metal:115-116)
-// Round-2 experiments that did NOT pay and were removed again (numbers: DESIGN.md section 4, profiles/r02_decode_ab.jsonl):
+// Experiments that did not pay and were removed again:
 //   * 8-warp CTAs, two per SM, one from each of two consecutive launches (so that launch n+1 prefetches while launch n
-//     consumes): the consume phase is issue-bound, half the warps per launch doubled it (gate|up 5.4 -> 11.9 us) and the
-//     token went 1.44 -> 1.75 ms;
-//   * a device-flag hand-off between dependent launches instead of griddepcontrol.wait: 1.44 -> 1.55 ms (the CTAs of the
-//     consumer cannot start before the producer's CTAs exit anyway, the flag traffic only adds);
+//     consumes): the consume phase is issue-bound, and half the warps per launch made it slower;
+//   * a device-flag hand-off between dependent launches instead of griddepcontrol.wait (the CTAs of the consumer
+//     cannot start before the producer's CTAs exit anyway, the flag traffic only adds);
 //   * forcing the largest shared-memory carveout: the register pipeline keeps up to 128 KiB of weight loads in flight per
-//     SM and those loads are staged in L1 lines even with L1::no_allocate - with ~1 KiB of L1 left every projection was
-//     1.75x slower (lm_head 49 -> 86 us, token 1.42 -> 1.95 ms).  No carveout preference is set here;
-//   * a sixth generation that moved the weight stream from registers to per-warp TMA rings in shared memory (512-thread
-//     CTAs at 64 registers, two per SM so that two consecutive launches overlap on every SM): parity-green, but the
-//     consume phase pays a shared-memory read per weight word and 296 CTAs hand over more slowly than 140 -
-//     1.43 -> 1.99 ms (profiles/r02_stream6_timeline.txt);
-//   * asking the CTA's whole weight slice into L2 (cp.async.bulk.prefetch.L2) before griddepcontrol.wait, so that the
-//     consume phase would stream from L2: gate|up consume 4.64 -> 4.48 us, but the prefetch traffic competes with the
-//     activation round trip of the staging step (2.75 -> 3.2 us): 1.426 -> 1.461 ms.
+//     SM and those loads are staged in L1 lines even with L1::no_allocate - with ~1 KiB of L1 left every projection
+//     slowed down.  No carveout preference is set here;
+//   * moving the weight stream from registers to per-warp TMA rings in shared memory (512-thread CTAs at 64 registers,
+//     two per SM): correct, but the consume phase pays a shared-memory read per weight word and twice the CTAs hand
+//     over more slowly;
+//   * asking the CTA's whole weight slice into L2 (cp.async.bulk.prefetch.L2) before griddepcontrol.wait: the prefetch
+//     traffic competes with the activation round trip of the staging step.
 constexpr int S5_WARPS = 16;
 #ifndef S5_DEPTH_SMALL
 #define S5_DEPTH_SMALL 4
@@ -277,7 +269,7 @@ void trace_bind_matvec(unsigned long long *buf, unsigned int *n, unsigned int ca
 
 // Programmatic dependent launch is on by default (tl_set_pdl(0) or TL_PDL=0 turns it off): every
 // kernel that carries the attribute reads its predecessor's output only after griddepcontrol.wait,
-// so stream order semantics are unchanged; measured 1.83 -> 1.55 ms per Qwen3-4B token.
+// so stream order semantics are unchanged.
 static bool pdl_default() {
     const char *e = getenv("TL_PDL");
     return !(e != nullptr && e[0] == '0');
@@ -303,7 +295,7 @@ static size_t stream5_smem_bytes(int N, int K, int MP, int grid) {
 // ---- launch geometry
 // One CTA per SM minus TL_S5_RESERVE (default 8): the few CTAs of the kernel behind it (the 8-CTA attention launch, the
 // first CTAs of the next projection) then start early under programmatic dependent launch and issue their independent
-// loads while this one is still running (round 1: 1.499 -> 1.399 ms/token; 16 reserved: no further gain).
+// loads while this one is still running.
 static int stream5_grid(int K) {
     static const int reserve = [] { const char *e = getenv("TL_S5_RESERVE"); const int v = e ? atoi(e) : 8; return v < 0 ? 0 : v; }();
     const int all = (K + 15) / 16;

@@ -1,1 +1,1 @@
-"""Native extension packages of the B200 backend (mirrors ``src/extensions_ref``)."""
+"""Native extension packages of the CUDA backend (mirrors ``src/extensions_ref``)."""

@@ -1,6 +1,6 @@
 """tiny_llm_b200 - tiny-llm's Qwen3 inference operators, models and scheduler
-re-hosted on torch tensors over the sm_100a extension.  The public names are
-those of ``tiny_llm_ref`` (``/root/reference/src/tiny_llm_ref/__init__.py``)."""
+re-hosted on torch tensors over the sm_90a extension.  The public names are
+those of ``tiny_llm_ref`` (``src/tiny_llm_ref/__init__.py``)."""
 
 from .attention import *  # noqa: F401,F403
 from .attention import paged_attention, scaled_dot_product_attention_grouped, scaled_dot_product_attention_simple, causal_mask

@@ -1,4 +1,4 @@
-"""Attention operators (``/root/reference/src/tiny_llm_ref/attention.py``).
+"""Attention operators (``src/tiny_llm_ref/attention.py``).
 
 ``paged_attention`` keeps the reference's model-facing contract - query
 ``[B, H_q, L, D]``, page storage ``[P, H_kv, page_size, D]``, int32
@@ -119,7 +119,7 @@ def paged_attention(
     block_table_host: np.ndarray | None = None,
     context_lens_host: np.ndarray | None = None,
 ) -> torch.Tensor:
-    """Paged attention backed by the sm_100a extension (attention.py:69-178)."""
+    """Paged attention backed by the sm_90a extension (attention.py:69-178)."""
     if isinstance(mask, torch.Tensor):
         raise NotImplementedError("Paged attention only supports mask=None or causal")
     if mask is not None and mask != "causal":

@@ -1,6 +1,6 @@
 """Readable Week-1 operators on torch tensors.
 
-Signatures of ``/root/reference/src/tiny_llm_ref/basics.py:5-26``.  These are
+Signatures of ``src/tiny_llm_ref/basics.py:5-26``.  These are
 the un-fused building blocks the early Week-2 checkpoints still use; they run
 as ordinary torch ops on whatever device the tensors live on.
 """

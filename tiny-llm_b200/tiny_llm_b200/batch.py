@@ -1,5 +1,5 @@
 """Continuous batching with chunked prefill
-(``/root/reference/src/tiny_llm_ref/batch.py``).
+(``src/tiny_llm_ref/batch.py``).
 
 Scheduling policy, verbatim from the reference loop (batch.py:164-270): at most
 one request is being prefilled, ``prefill_step`` tokens per iteration and always

@@ -1,10 +1,10 @@
 """Checkpoint front door: MLX 4-bit safetensors -> the ``mlx_model`` duck type.
 
 The reference loads ``Qwen/Qwen3-*-MLX-4bit`` with ``mlx_lm.load``
-(``/root/reference/main.py:96-98``, ``batch-main.py:62-64``) and hands the
+(``main.py:96-98``, ``batch-main.py:62-64``) and hands the
 resulting object to ``dispatch_model``; the models only look at ``.args`` and at
 ``weight / scales / biases / group_size / bits`` of every quantised layer
-(``/root/reference/src/tiny_llm_ref/qwen3_week3.py:225-313``).  An MLX 4-bit
+(``src/tiny_llm_ref/qwen3_week3.py:225-313``).  An MLX 4-bit
 checkpoint directory is ``config.json`` + ``model*.safetensors`` whose tensors
 are named ``model.layers.{i}.self_attn.q_proj.{weight,scales,biases}`` ... with
 ``weight`` packed uint32 ``[out, in/8]`` in exactly the nibble order

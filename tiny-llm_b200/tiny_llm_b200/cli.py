@@ -1,6 +1,6 @@
 """Command-line front doors: the equivalents of the reference's ``main.py`` (one prompt,
-``/root/reference/main.py:1-190``) and ``batch-main.py`` (continuous batching,
-``/root/reference/batch-main.py:1-102``) over a checkpoint DIRECTORY (MLX 4-bit safetensors layout,
+``main.py:1-190``) and ``batch-main.py`` (continuous batching,
+``batch-main.py:1-102``) over a checkpoint DIRECTORY (MLX 4-bit safetensors layout,
 see checkpoint.py; there is no hub download here).
 
     python -m tiny_llm_b200.cli generate --model /path/to/Qwen3-4B-MLX-4bit --prompt "..." [--loader week3]

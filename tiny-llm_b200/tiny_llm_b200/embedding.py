@@ -1,4 +1,4 @@
-"""Embedding tables (``/root/reference/src/tiny_llm_ref/embedding.py``)."""
+"""Embedding tables (``src/tiny_llm_ref/embedding.py``)."""
 
 from __future__ import annotations
 

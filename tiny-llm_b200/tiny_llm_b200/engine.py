@@ -1,7 +1,7 @@
-"""CUDA-graph decode engine for the Week-3 paged model (B200 host runtime).
+"""CUDA-graph decode engine for the Week-3 paged model (CUDA host runtime).
 
 The reference issues ~500 operator calls per generated token from a Python loop
-(SURVEY.md section 3.1); at B200 speeds one W4A16 projection lasts about a
+(SURVEY.md section 3.1); at these speeds one W4A16 projection lasts about a
 microsecond, so per-call dispatch would leave the GPU idle >90 % of the time.
 The engine keeps the operator semantics and removes the dispatch:
 
@@ -158,7 +158,7 @@ class DecodeEngine:
         # The one-launch attention is a latency design (few CTAs, K/V rows staged per lane): it wins while the
         # step is launch-bound.  With many slots or long contexts the K/V stream dominates and the step uses
         # q/k norm + rope + append as one small launch followed by tl_paged_attention, whose long-context path
-        # is the TMA + tcgen05 streaming kernel (attention_prefill_tc.cu).  TL_ATTENTION_FUSED=0/1 forces either.
+        # is the TMA + wgmma streaming kernel (attention_prefill_tc.cu).  TL_ATTENTION_FUSED=0/1 forces either.
         fused_env = os.environ.get("TL_ATTENTION_FUSED")
         fused_pays = self.B * self.max_seq_len <= int(os.environ.get("TL_ATTENTION_FUSED_MAX_TOKENS", "16384"))
         self._attention_fused = (self.fused and self.D == 128 and self.Hq // self.Hkv <= 4
@@ -173,7 +173,7 @@ class DecodeEngine:
         # full one and step() replays the smallest that covers the highest occupied slot: every kernel of the wide
         # path costs by rows (swap-AB column count, attention CTAs, reduction planes).  All variants stay on the
         # >= 9-row kernels and the split counts do not depend on the row count, so a row's result is bit-identical
-        # whichever variant computed it.  (Config 4 runs 64 slots with ~20 live: decode step p50 3.31 -> 3.02 ms.)
+        # whichever variant computed it.  (Config 4 runs 64 slots with ~20 live.)
         rows_env = os.environ.get("TL_ROW_VARIANTS", "1")
         self._variants = sorted({r for r in (16, 32, 64) if r < self.B} | {self.B}) if (self.fused and self.B > 16 and rows_env != "0") else [self.B]
         self._graphs: dict = {}
@@ -245,7 +245,7 @@ class DecodeEngine:
         m = self.model
         B, Hq, Hkv, D = (self.B if R is None else R), self.Hq, self.Hkv, self.D
         offsets, context_lens = self.offsets[:B], self.context_lens[:B]
-        # More than 8 rows: the projections run on the swap-AB tcgen05 kernel (w4a16_skinny.cu: weights streamed once
+        # More than 8 rows: the projections run on the swap-AB wgmma kernel (w4a16_skinny.cu: weights streamed once
         # for all rows), which has no prologue, so RMSNorm is its own (tiny) launch; the rounding points are the same.
         wide = self.B > 8
 
@@ -408,8 +408,7 @@ class DecodeEngine:
         Cost per step at B = 64: one identity check per slot; the 36 per-layer cache objects of a
         request are touched only when its tail page overflows (once per ``page_size`` tokens) - the
         one-token appends in between are deferred (``TinyKvPagedCache._lazy``) and settled when
-        somebody reads ``page_lens`` / ``offset``.  Round 1 walked 36 x B objects every step
-        (0.4-1 ms of Python at B = 64, VERDICT weak #10)."""
+        somebody reads ``page_lens`` / ``offset``, instead of walking 36 x B objects every step."""
         first_ctx = [0] * self.B
         slots0 = self._slot_caches(caches, 0)
         page = self.page_size
@@ -554,10 +553,10 @@ class DecodeEngine:
 
 class PrefillEngine:
     """CUDA-graph replay of ONE chunked-prefill step (``Request.try_prefill``: B = 1, up to ``chunk`` prompt tokens,
-    ``/root/reference/src/tiny_llm_ref/batch.py:48-76``) for the Week-3 paged model.
+    ``src/tiny_llm_ref/batch.py:48-76``) for the Week-3 paged model.
 
     The reference (and the operator path of this backend) issues ~20 operator calls per layer per chunk from
-    Python: ~700 launches, 10-25 ms of host time for a 128-token chunk whose GPU work is ~1.5 ms.  Here the
+    Python: ~700 launches, whose host time exceeds the GPU work of a 128-token chunk.  Here the
     chunk's whole forward pass is captured once over static buffers; what changes between chunks is DATA in one
     pinned block: the token ids, per-token RoPE positions and post-append lengths, the request's block-table
     row per layer and the final context length.  A short (tail) chunk is RIGHT-aligned in the ``chunk`` rows:
@@ -565,7 +564,7 @@ class PrefillEngine:
     rule of paged attention (``key <= row + ctx - L``) then gives every real row exactly its own prefix.
 
     Per layer: rms_norm -> q|k|v projection (one launch) -> q/k norm + RoPE + K/V append for all rows (one
-    launch, ``tl_chunk_qk_norm_rope_append``) -> paged FlashAttention (tcgen05) -> o projection + residual ->
+    launch, ``tl_chunk_qk_norm_rope_append``) -> paged FlashAttention (wgmma) -> o projection + residual ->
     rms_norm -> gate|up (+ SwiGLU) -> down + residual.  Rounding points are those of the operator sequence.
     Integer page bookkeeping stays in the request's ``TinyKvPagedCache`` objects (``append_slots``)."""
 
@@ -646,7 +645,7 @@ class PrefillEngine:
                 q = ext.chunk_qk_norm_rope_append(proj(h, pk.qkv), at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                   self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
                                                   Hq, Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
-            # [L, Hq * D]: the tcgen05 kernel writes the o-projection's layout itself (else: attention + one transpose copy)
+            # [L, Hq * D]: the wgmma kernel writes the o-projection's layout itself (else: attention + one transpose copy)
             y = ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
                                                 True, Hkv, Hq)
             if skinny:  # the residual projections return the next RMSNorm's output too (DecodeEngine._forward_fused_layers)

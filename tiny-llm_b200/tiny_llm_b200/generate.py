@@ -1,5 +1,5 @@
 """Single-request greedy generation with a KV cache
-(``/root/reference/src/tiny_llm_ref/generate.py:49-81``)."""
+(``src/tiny_llm_ref/generate.py:49-81``)."""
 
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     """The loop of ``simple_generate_with_kv_cache`` on token ids: the whole
     prompt is prefilled at offset 0 (its last-row logits give the first token),
     then one token per step at a growing offset.  Returns the generated ids.
-    ``sampler`` (``make_sampler``; B200 extension - the reference's cached loop is greedy only) draws
+    ``sampler`` (``make_sampler``; CUDA extension - the reference's cached loop is greedy only) draws
     from ``logits - logsumexp`` instead of taking the arg-max."""
     kv_cache = model.create_kv_cache()
     produced: list[int] = []

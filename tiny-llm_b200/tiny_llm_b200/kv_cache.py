@@ -1,12 +1,12 @@
 """KV-cache interfaces and the dense caches
-(``/root/reference/src/tiny_llm_ref/kv_cache.py``).
+(``src/tiny_llm_ref/kv_cache.py``).
 
 ``BatchingKvCache`` is the decode-slot table of the continuous-batching
 scheduler: a fixed number of slots, each holding one request's cache (or
 nothing).  ``update_and_fetch`` is the Week-3-day-1 dense path (right-aligned
 padding + additive mask); ``update_and_fetch_paged`` appends one chunk per
-active slot into the shared page pool and returns block-table metadata.  On
-B200 the per-slot appends of a decode step (one token per request) are
+active slot into the shared page pool and returns block-table metadata.  Here
+the per-slot appends of a decode step (one token per request) are
 collapsed into a single device-driven launch; all integer bookkeeping stays on
 the host and is identical to the reference's.
 """

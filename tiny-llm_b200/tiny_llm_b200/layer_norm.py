@@ -1,4 +1,4 @@
-"""Readable RMSNorm (``/root/reference/src/tiny_llm_ref/layer_norm.py:4-15``)."""
+"""Readable RMSNorm (``src/tiny_llm_ref/layer_norm.py:4-15``)."""
 
 from __future__ import annotations
 

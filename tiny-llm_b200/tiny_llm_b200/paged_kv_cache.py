@@ -1,4 +1,4 @@
-"""Paged KV storage (``/root/reference/src/tiny_llm_ref/paged_kv_cache.py``).
+"""Paged KV storage (``src/tiny_llm_ref/paged_kv_cache.py``).
 
 One ``TinyKvPagedPool`` per transformer layer owns the physical page slab
 ``[capacity, H_kv, page_size, D]`` for keys and for values; every request holds
@@ -199,7 +199,7 @@ class TinyKvPagedPool:
         self.slab_version = next(_SLAB_VERSIONS)
 
     def reserve(self, num_pages: int, heads: int, head_dim: int, dtype=torch.bfloat16, device="cuda") -> None:
-        """B200 extension: size the slab once (one counted growth) so that page
+        """CUDA extension: size the slab once (one counted growth) so that page
         base addresses stay fixed, which CUDA-graph replay of the decode step
         needs.  Logical page accounting is unchanged."""
         if self.capacity >= num_pages:
@@ -300,7 +300,7 @@ class TinyKvPagedCache(TinyKvCache):
         self.page_ids: list[int] = []
         self._page_lens: list[int] = []
         self._offset = 0
-        # B200 runtime (engine.py): while a request decodes inside the CUDA-graph engine, one-token
+        # CUDA runtime (engine.py): while a request decodes inside the CUDA-graph engine, one-token
         # appends that fit in the tail page are DEFERRED - counted once per request instead of once
         # per layer object - and folded into page_lens / offset the moment anybody looks at them.
         self._lazy = None
@@ -357,7 +357,7 @@ class TinyKvPagedCache(TinyKvCache):
         total = key.shape[2]
         mine = self._snapshot_state()
         theirs = self.pool._snapshot_state()
-        # B200: when nothing overrides the per-page writer, the host bookkeeping below runs with the
+        # CUDA: when nothing overrides the per-page writer, the host bookkeeping below runs with the
         # launch-free reserve_page_slice and ALL page slices are written by one device launch at the
         # end (same bytes, same page/offset evolution, same all-or-nothing behaviour: the launch
         # happens only after every check and allocation has succeeded)

@@ -1,4 +1,4 @@
-"""Readable table-driven RoPE (``/root/reference/src/tiny_llm_ref/positional_encoding.py:4-66``)."""
+"""Readable table-driven RoPE (``src/tiny_llm_ref/positional_encoding.py:4-66``)."""
 
 from __future__ import annotations
 

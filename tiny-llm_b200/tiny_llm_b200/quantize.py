@@ -1,6 +1,6 @@
 """W4A16 operator layer: same callables as
-``/root/reference/src/tiny_llm_ref/quantize.py`` over torch tensors and the
-B200 extension.
+``src/tiny_llm_ref/quantize.py`` over torch tensors and the
+CUDA extension.
 
 Packed weights are ``[K, N/8]`` 32-bit words (``torch.uint32`` or ``int32``
 with the same bit pattern - torch has no uint32 arithmetic); code ``i`` of a

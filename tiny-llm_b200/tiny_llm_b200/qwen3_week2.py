@@ -1,9 +1,9 @@
 """Week-2 Qwen3 model with its cumulative optimisation checkpoints
-(``/root/reference/src/tiny_llm_ref/qwen3_week2.py``).
+(``src/tiny_llm_ref/qwen3_week2.py``).
 
 ``checkpoint`` selects how far along the course the model is: ``"kv-cache"``
 runs dense bf16 weights through the readable operators, each later name turns
-on one more B200 kernel family (``WEEK2_CHECKPOINTS``, qwen3_week2.py:19-28).
+on one more CUDA kernel family (``WEEK2_CHECKPOINTS``, qwen3_week2.py:19-28).
 The KV cache is the dense concat cache; the fused decode-attention kernel is
 used only for ``L <= 2`` and ``S <= 256`` (qwen3_week2.py:30-31,124-136),
 everything else takes the fp32 readable attention (:138-144).

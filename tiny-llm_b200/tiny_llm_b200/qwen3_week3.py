@@ -1,5 +1,5 @@
 """Week-3 Qwen3 model: W4A16 projections, fused norm/RoPE/SwiGLU kernels and
-paged-KV attention (``/root/reference/src/tiny_llm_ref/qwen3_week3.py``).
+paged-KV attention (``src/tiny_llm_ref/qwen3_week3.py``).
 
 Constructor, ``create_kv_cache`` and ``__call__(inputs, offset, cache,
 logits_to_keep)`` keep the reference's contract; the only contact with weights
@@ -195,7 +195,7 @@ class Qwen3ModelWeek3:
         for index, layer in enumerate(mlx_model.model.layers[: self.num_hidden_layers]):
             if is_qwen3_moe_sparse_layer(args, index):
                 raise NotImplementedError(
-                    "Qwen3-MoE layers are outside the B200 hot-path scope (SURVEY.md section 2, row 12)"
+                    "Qwen3-MoE layers are outside the CUDA hot-path scope (SURVEY.md section 2, row 12)"
                 )
             attn = layer.self_attn
             mlp = Qwen3MLP(
@@ -229,14 +229,14 @@ class Qwen3ModelWeek3:
         self.norm = FastRMSNorm(args.hidden_size, weight=mlx_model.model.norm.weight, eps=args.rms_norm_eps)
         self.w_lm_head = None if args.tie_word_embeddings else packed(mlx_model.lm_head)
         self.mlx_model = mlx_model
-        # B200 runtime: decode steps (L == 1) of CUDA-resident paged requests are replayed
+        # CUDA runtime: decode steps (L == 1) of CUDA-resident paged requests are replayed
         # from a captured CUDA graph instead of ~500 per-operator dispatches (engine.py).
         # None = automatic (on for CUDA inputs), False = always operator by operator.
         self.use_decode_graph: bool | None = None
         self.decode_graph_max_seq_len = 8192
         self._decode_engines: dict = {}
         self._applies_memo = None
-        # B200 runtime: chunked-prefill steps (B == 1, 1 < L <= prefill_graph_len) of CUDA-resident paged requests
+        # CUDA runtime: chunked-prefill steps (B == 1, 1 < L <= prefill_graph_len) of CUDA-resident paged requests
         # replay a captured chunk graph too (engine.PrefillEngine).  0 disables; None = automatic (128, the scheduler's
         # default prefill_step) once a decode engine exists, i.e. once the page slabs have been reserved.
         self.prefill_graph_len: int | None = None
@@ -368,8 +368,7 @@ class Qwen3ModelWeek3:
             chunk = 128
         L = inputs.shape[1]
         # 2 <= L: tail chunks of a few tokens replay the graph too (right-aligned in its rows).  On the operator path they
-        # are ~700 host-bound launches - 20-30 ms each, 6 % of config 4's requests have such a tail, and their cost
-        # swung the serving number by +-10 % with the load of the (shared) host.
+        # are ~700 host-bound launches each, and their cost follows the load of the host.
         if not (1 < L <= chunk) or not PrefillEngine.supported(self, inputs.device):
             return None
         if isinstance(offset, torch.Tensor):

@@ -1,4 +1,4 @@
-"""``make_sampler(temp, top_p, top_k)`` (``/root/reference/src/tiny_llm_ref/sampler.py:5-25``) on
+"""``make_sampler(temp, top_p, top_k)`` (``src/tiny_llm_ref/sampler.py:5-25``) on
 torch tensors: greedy at ``temp == 0``; otherwise mask everything outside the ``top_k`` most likely
 tokens, then everything outside the smallest prefix of the sorted distribution whose mass reaches
 ``top_p`` (a token is kept while the mass BEFORE it is < top_p, ``:19``), divide by ``temp`` and draw

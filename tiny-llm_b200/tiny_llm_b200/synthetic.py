@@ -3,8 +3,8 @@
 There is no network here, so benchmarks and tests run on random weights of the
 right architecture (SURVEY.md section 8d).  The object mirrors what
 ``mlx_lm.load`` returns as far as the models look at it
-(``/root/reference/src/tiny_llm_ref/qwen3_week3.py:225-313``; minimal fake at
-``/root/reference/tests/utils.py:12-69``): ``.args`` plus
+(``src/tiny_llm_ref/qwen3_week3.py:225-313``; minimal fake at
+``tests/utils.py:12-69``): ``.args`` plus
 ``.model.{embed_tokens, layers[i].{self_attn, mlp, *_layernorm}, norm}`` where
 every quantised layer carries ``weight`` (packed u32), ``scales``, ``biases``,
 ``group_size`` and ``bits``.
@@ -178,7 +178,7 @@ def named_tensors(node, prefix=""):
 def weight_stream_bytes(args) -> int:
     """Packed bytes one decode token must stream (projections of every layer +
     tied head): 0.53125 B per weight = N/2 codes + 4 B of scale/bias per 128
-    (/root/reference/book/src/week2-03-quantize-model.md:179-181)."""
+    (book/src/week2-03-quantize-model.md:179-181)."""
     q_width = args.num_attention_heads * args.head_dim
     kv_width = args.num_key_value_heads * args.head_dim
     per_layer = args.hidden_size * (q_width + 2 * kv_width) + q_width * args.hidden_size + 3 * args.hidden_size * args.intermediate_size

@@ -1,5 +1,5 @@
 """Fused model operators: signatures of
-``/root/reference/src/tiny_llm_ref/week2_kernels.py`` over the B200 extension."""
+``src/tiny_llm_ref/week2_kernels.py`` over the CUDA extension."""
 
 from __future__ import annotations
 

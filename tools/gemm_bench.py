@@ -1,5 +1,5 @@
 """Per-shape timing of the prefill GEMM (Qwen3-4B projections at M rows, default 4096):
-  [TL_GEMM2=0] python tools/gemm_bench.py [M]
+  python tools/gemm_bench.py [M]
 CUDA events around 20 back-to-back launches after 5 warm-up calls; weights of the next launch differ (4 copies > L2)."""
 import json
 import os

@@ -1,7 +1,6 @@
 """In-kernel timeline of the swap-AB GEMM (debug build with -DTL_TRACE=1, CTA 0):
   TL_LIB=.../libtiny_llm_b200_trace.so python tools/skinny_timeline.py
-Tags: 30 entry, 31 set-up done (barriers, TMEM, scales), 32 first packed box landed, 33 last weight tile handed over,
-34 accumulators complete, 35 epilogue stored, 36 exit."""
+Tags: 30 entry, 31 set-up done (barriers), 34 accumulators complete, 36 exit."""
 import ctypes
 import sys
 from pathlib import Path
