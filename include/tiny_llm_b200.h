@@ -58,16 +58,15 @@ long long tl_launch_count(void);
  * Replaces quantized_matmul (tiny_llm_ext.h:12-21, quantized_matmul.cpp:14-80,
  * eval_gpu :111-240).  scales/biases [K, N/128] (f16|bf16), a [M, N],
  * b [K, N/8] u32, out [M, K].  Kernel selection:
- *   use_simdgroup && M <= TL_MATVEC_REF_ROWS : weight-streaming tensor-core
- *       matvec, weights kept fp32-exact (reference: M <= 8 matvec, quantize.py:162-163);
- *   use_simdgroup && M <= 128                : swap-AB wgmma GEMM with the reduction split over
+ *   !use_simdgroup                  : scalar control kernel;
+ *   M <= TL_MATVEC_REF_ROWS         : weight-streaming tensor-core matvec, weights kept fp32-exact (reference:
+ *       M <= 8 matvec, quantize.py:162-163), up to TL_MATVEC_MAX_ROWS rows per pass;
+ *   TL_MATVEC_REF_ROWS < M <= 128   : swap-AB wgmma GEMM with the reduction split over
  *       CTAs (reference: quantized_matmul_splitk, quantized_matmul.metal:251-293), weights rounded to
  *       the activation dtype before the MMA, fp32 partial planes added in split order;
- *   use_simdgroup                            : the same wgmma kernel on 128-token tiles, weights rounded to
- *       the activation dtype before the MMA (reference: simdgroup tile);
- *   !use_simdgroup                           : scalar control kernel.
- * (Shapes a tensor-core kernel cannot take - odd alignments - fall back to the streaming kernel, which
- * handles up to TL_MATVEC_MAX_ROWS rows per pass.)
+ *   M > 128                         : the same wgmma kernel on 128-token tiles, weights rounded to
+ *       the activation dtype before the MMA (reference: simdgroup tile).
+ * The wgmma kernels need a and b 16-byte aligned; otherwise the call returns TL_EINVAL.
  * The split of the reduction is a scheduling decision of this backend (SURVEY 8a' item 12): it depends only on
  * (N, K), never on use_split_k, so a split request and a plain request run the very same kernel with
  * bit-identical results (tests_refsol/test_week_2_day_7.py:80-109).

@@ -292,17 +292,16 @@ def test_serving_path_engine_matches_cpu_oracle(dev):
             table.remove_request(b)
 
 
-def test_row_variant_graphs_give_the_bits_of_the_full_step(dev, monkeypatch):
+def test_row_variant_graphs_give_the_bits_of_the_full_step(dev):
     """A 64-slot engine whose occupied slots are a short prefix replays the 16- or 32-row step graph: the logits of
     the occupied rows must be bit-identical to what the full 64-row graph produces (same kernels, same split counts),
     and a later step with a high slot occupied must pick the wide graph again."""
     ns = to_device(synthetic_qwen3("tiny-d128", seed=5, realistic=True, max_position_embeddings=512), dev)
     B, g = 64, gen(64)
 
-    def run(variants: str, slots):
-        monkeypatch.setenv("TL_ROW_VARIANTS", variants)
+    def run(variants: bool, slots):
         model = Qwen3ModelWeek3(ns, page_size=16)
-        engine = DecodeEngine(model, B, 128, dev)
+        engine = DecodeEngine(model, B, 128, dev, _row_variants=variants)
         engine.reserve_pools()
         tables = [BatchingKvCache(max_active_requests=B, max_seq_len=128) for _ in range(model.num_hidden_layers)]
         prompts = {b: [3 + (11 * b + j) % 400 for j in range(4 + b % 7)] for b in slots}
@@ -323,8 +322,8 @@ def test_row_variant_graphs_give_the_bits_of_the_full_step(dev, monkeypatch):
         return outs, engine
 
     for slots, want_rows in (([0, 1, 2, 5, 9], 16), ([0, 3, 17, 30], 32), ([2, 40, 63], 64)):
-        narrow, eng = run("1", slots)
-        full, _ = run("0", slots)
+        narrow, eng = run(True, slots)
+        full, _ = run(False, slots)
         assert eng.variant_replays[want_rows] == 2 and sum(eng.variant_replays.values()) == 2
         for a, b in zip(narrow, full):
             assert torch.equal(a[slots], b[slots])

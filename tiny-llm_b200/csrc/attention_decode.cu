@@ -16,8 +16,6 @@
 // sees keys < clamp(ctx - L + l + 1, 0, ctx)   (paged_attention.metal:158-160).
 #include <math_constants.h>
 
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "kernels.h"
 
@@ -226,7 +224,6 @@ constexpr int GQA_D = 128;
 constexpr int GQA_WARPS = 4;
 constexpr int GQA_THREADS = GQA_WARPS * 32;
 constexpr int GQA_STEP = GQA_WARPS * 4;  // tokens per CTA iteration (4 per warp, 8 lanes each)
-constexpr int GQA_MAX_SPLITS = 32;
 constexpr int GQA_RING = 6;          // cp.async steps in flight per lane (64 B each)
 constexpr int GQA_PAGE_CACHE = 264;  // page ids of one split kept in shared memory
 
@@ -477,11 +474,6 @@ int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws
     return TL_OK;
 }
 
-size_t paged_decode_workspace(int rows, int L, int D, int num_kv_heads, int num_heads, int dtype) {
-    if (dtype != TL_BF16 || D != GQA_D) return 0;
-    return static_cast<size_t>(rows) * L * GQA_MAX_SPLITS * (GQA_D + 2) * sizeof(float);
-}
-
 int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out,
                      int rows, int L, int num_pages, int page_size, int max_pages, float scale, int is_causal,
                      int num_kv_heads, int num_heads, bool allow_split, void *ws, size_t ws_bytes, cudaStream_t st) {
@@ -499,7 +491,7 @@ int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_
         long long want = ceil_div_ll(target, base_ctas);
         const long long most = bound / 128 > 0 ? bound / 128 : 1;  // at least 128 tokens per split (larger minimums lengthen the per-step chain at short contexts)
         if (want > most) want = most;
-        if (want > GQA_MAX_SPLITS) want = GQA_MAX_SPLITS;
+        if (want > PAGED_MAX_SPLITS) want = PAGED_MAX_SPLITS;
         if (want < 1) want = 1;
         splits = static_cast<int>(want);
     }
@@ -549,51 +541,6 @@ int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_
         TL_LAUNCH_CHECK("paged_gqa_merge");
     }
     return TL_OK;
-}
-
-int launch_paged_decode(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out,
-                        int rows, int L, int D, int num_pages, int page_size, int max_pages, float scale,
-                        int is_causal, int num_kv_heads, int num_heads, int dtype, void *ws, size_t ws_bytes,
-                        cudaStream_t st) {
-    const bool fast = dtype == TL_BF16 && D == GQA_D && aligned16(q) && aligned16(kp) && aligned16(vp);
-    // Long contexts stream K/V through the TMA + wgmma kernel (attention_prefill_tc.cu; the G x L query rows ride
-    // in a 128-row MMA tile - the tensor-core time is far below the HBM time of the tile even at 4 live rows); short
-    // ones stay on the cp.async kernel, whose fixed cost per CTA is lower.  TL_DECODE_TC: 0 never, 1 always (when supported).
-    static const int tc_mode = [] { const char *e = getenv("TL_DECODE_TC"); return e == nullptr ? -1 : atoi(e); }();
-    static const long long tc_min_keys = [] { const char *e = getenv("TL_DECODE_TC_MIN"); return e == nullptr ? 1024LL : atoll(e); }();
-    const int group = num_kv_heads > 0 ? num_heads / num_kv_heads : 0;
-    if (fast && tc_mode != 0 && aligned16(out) && rows % num_heads == 0 && group > 0 && L <= 128 / group &&
-        paged_prefill_tc_supported(L, num_pages, page_size, num_kv_heads, num_heads) &&
-        (tc_mode == 1 || static_cast<long long>(max_pages) * page_size >= tc_min_keys))
-        return launch_paged_prefill_tc(q, kp, vp, bt, cl, out, rows, L, num_pages, page_size, max_pages, scale, is_causal, num_kv_heads,
-                                       num_heads, true, ws, ws_bytes, st);
-    if (fast)
-        return launch_paged_gqa(q, kp, vp, bt, cl, out, rows, L, num_pages, page_size, max_pages, scale, is_causal,
-                                num_kv_heads, num_heads, true, ws, ws_bytes, st);
-    return launch_paged_rowwise(q, kp, vp, bt, cl, out, rows, L, D, num_pages, page_size, max_pages, scale, is_causal,
-                                num_kv_heads, num_heads, dtype, st);
-}
-
-// Prefill path (L > 8): bf16 / D = 128 runs the wgmma + TMA flash kernel (attention_prefill_tc.cu)
-// when the page size is a multiple of 64 and Hq/Hkv divides 128 (TL_PREFILL_TC=0 turns it off), else
-// the mma.sync flash kernel (attention_prefill.cu); TL_PREFILL_FA=0 selects the older CUDA-core
-// GQA-grouped kernel as a control; everything else is row-wise.
-int launch_paged_prefill(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out,
-                         int rows, int L, int D, int num_pages, int page_size, int max_pages, float scale,
-                         int is_causal, int num_kv_heads, int num_heads, int dtype, cudaStream_t st) {
-    const bool fast = dtype == TL_BF16 && D == GQA_D && aligned16(q) && aligned16(kp) && aligned16(vp);
-    static const bool fa_off = [] { const char *e = getenv("TL_PREFILL_FA"); return e != nullptr && e[0] == '0'; }();
-    if (fast && !fa_off && aligned16(out) && rows % num_heads == 0 && paged_prefill_tc_supported(L, num_pages, page_size, num_kv_heads, num_heads))
-        return launch_paged_prefill_tc(q, kp, vp, bt, cl, out, rows, L, num_pages, page_size, max_pages, scale, is_causal, num_kv_heads,
-                                       num_heads, false, nullptr, 0, st);
-    if (fast && !fa_off && rows <= 65535)  // tensor-core flash kernel (attention_prefill.cu); TL_PREFILL_FA=0: CUDA-core control
-        return launch_paged_prefill_fa(q, kp, vp, bt, cl, out, rows, L, num_pages, page_size, max_pages, scale, is_causal, num_kv_heads,
-                                       num_heads, st);
-    if (fast)
-        return launch_paged_gqa(q, kp, vp, bt, cl, out, rows, L, num_pages, page_size, max_pages, scale, is_causal,
-                                num_kv_heads, num_heads, false, nullptr, 0, st);
-    return launch_paged_rowwise(q, kp, vp, bt, cl, out, rows, L, D, num_pages, page_size, max_pages, scale, is_causal,
-                                num_kv_heads, num_heads, dtype, st);
 }
 
 }  // namespace tl

@@ -23,11 +23,7 @@
 //                        O is rescaled only when a row's maximum grows by more than 2^8 since the last
 //                        rescale: P and the row sum always use the same (possibly stale) maximum, so
 //                        the result is exact.  Epilogue: O / sum -> bf16 -> global.
-#include <stdlib.h>
 #include <math_constants.h>
-
-#include <mutex>
-#include <unordered_map>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -302,63 +298,21 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 }
 
 // ---------------------------------------------------------------- host side --
-// Tensor maps are cached per (base pointer, shape): a prefill of 36 layers x N chunks re-uses a
-// handful of distinct operands, and cuTensorMapEncodeTiled costs microseconds per call.
-struct MapKey {
-    const void *ptr;
-    unsigned long long d0, d1, d2, d3;
-    unsigned b1, b2;
-    bool operator==(const MapKey &o) const { return ptr == o.ptr && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && d3 == o.d3 && b1 == o.b1 && b2 == o.b2; }
-};
-struct MapKeyHash {
-    size_t operator()(const MapKey &k) const {
-        size_t h = reinterpret_cast<size_t>(k.ptr);
-        for (unsigned long long v : {k.d0, k.d1, k.d2, k.d3, static_cast<unsigned long long>(k.b1), static_cast<unsigned long long>(k.b2)})
-            h = h * 1000003u ^ static_cast<size_t>(v);
-        return h;
-    }
-};
-static int cached_map(CUtensorMap *out, const void *ptr, int rank, const cuuint64_t *dims, const cuuint32_t *box) {
-    static std::mutex mu;
-    static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-    MapKey key{ptr, dims[0], dims[1], dims[2], rank > 3 ? dims[3] : 0, box[1], box[2]};
-    std::lock_guard<std::mutex> lock(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) {
-        *out = it->second;
-        return TL_OK;
-    }
-    PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-    if (encode == nullptr) return fail(TL_ECUDA, "paged_attention: cuTensorMapEncodeTiled is unavailable");
-    cuuint64_t strides[3];
-    cuuint64_t acc = 2;
-    for (int i = 0; i + 1 < rank; ++i) {
-        acc *= dims[i];
-        strides[i] = acc;
-    }
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUtensorMap map;
-    CUresult r = encode(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void *>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(TL_ECUDA, "paged_attention: cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-    if (cache.size() > 4096) cache.clear();
-    cache.emplace(key, map);
-    *out = map;
-    return TL_OK;
+// bf16 Q / K / V with the 128-byte swizzle (the K-major wgmma layout), 256-byte L2 promotion.
+static int tc_map(CUtensorMap *out, const void *ptr, int rank, const cuuint64_t *dims, const cuuint32_t *box) {
+    return cached_tensor_map(out, ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, dims, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "paged_attention");
 }
 
 bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_heads, int num_heads) {
-    static const bool off = [] { const char *e = getenv("TL_PREFILL_TC"); return e != nullptr && e[0] == '0'; }();
-    if (off || num_kv_heads < 1 || num_heads % num_kv_heads != 0) return false;
+    if (num_kv_heads < 1 || num_heads % num_kv_heads != 0) return false;
     const int G = num_heads / num_kv_heads;
     if (G < 1 || G > TC_BM || (TC_BM % G) != 0) return false;
     return L > 0 && num_pages > 0 && page_size >= TC_BN && page_size % TC_BN == 0;
 }
 
-// allow_split (decode, L <= 8): the key range of every (request, KV head) is cut into up to GQA_MAX_SPLITS (32, the
-// size paged_decode_workspace() budgets for) pieces of >= 4 tiles so that a small batch still fills the GPU; the
-// partials are combined by paged_gqa_merge_kernel.
+// allow_split (decode, L <= 8): the key range of every (request, KV head) is cut into up to PAGED_MAX_SPLITS pieces of
+// >= 4 tiles so that a small batch still fills the GPU; the partials are combined by paged_gqa_merge_kernel.
 int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, bool allow_split, void *ws, size_t ws_bytes, cudaStream_t st, bool out_token_major) {
@@ -375,13 +329,13 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     {
         const cuuint64_t dims[3] = {TC_D, static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(rows)};
         const cuuint32_t box[3] = {64, static_cast<cuuint32_t>(a.RH), static_cast<cuuint32_t>(G)};
-        if (int e = cached_map(&mq, q, 3, dims, box)) return e;
+        if (int e = tc_map(&mq, q, 3, dims, box)) return e;
     }
     {
         const cuuint64_t dims[4] = {TC_D, static_cast<cuuint64_t>(page_size), static_cast<cuuint64_t>(num_kv_heads), static_cast<cuuint64_t>(num_pages)};
         const cuuint32_t box[4] = {64, TC_BN, 1, 1};
-        if (int e = cached_map(&mk, kp, 4, dims, box)) return e;
-        if (int e = cached_map(&mv, vp, 4, dims, box)) return e;
+        if (int e = tc_map(&mk, kp, 4, dims, box)) return e;
+        if (int e = tc_map(&mv, vp, 4, dims, box)) return e;
     }
     static bool configured = false;
     if (!configured) {
@@ -403,7 +357,7 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
         const long long slots = sm_count();
         const size_t rows_total = static_cast<size_t>(rows) * L;
         long long best = 1, best_cost = -1;
-        for (long long sp = 1; sp <= 32 && sp <= (max_tiles > 1 ? max_tiles : 1); ++sp) {
+        for (long long sp = 1; sp <= PAGED_MAX_SPLITS && sp <= (max_tiles > 1 ? max_tiles : 1); ++sp) {
             const long long tps = (max_tiles + sp - 1) / sp;
             const long long real = (max_tiles + tps - 1) / tps;
             if (real != sp) continue;

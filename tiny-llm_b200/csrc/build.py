@@ -19,7 +19,7 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent
 ROOT = CSRC.parent.parent
 OUT_DIR = CSRC.parent / "extensions_b200" / "tiny_llm_ext_b200"
-# Experiment builds: TL_DEFINES="-DS4_DEPTH_SMALL=3 ..." TL_LIB_SUFFIX=_d3 python build.py
+# Experiment builds: TL_DEFINES="-DS5_DEPTH_SMALL=3 ..." TL_LIB_SUFFIX=_d3 python build.py
 # -> libtiny_llm_b200_d3.so next to the product library (tools/kbench.py --lib selects it).
 SUFFIX = os.environ.get("TL_LIB_SUFFIX", "")
 LIB = OUT_DIR / f"libtiny_llm_b200{SUFFIX}.so"
@@ -29,12 +29,12 @@ SOURCES = [
     "c_abi.cu",
     "elementwise.cu",
     "w4a16_matvec.cu",
-    "w4a16_gemm.cu",
     "w4a16_skinny.cu",
     "attention_decode.cu",
     "attention_prefill.cu",
     "attention_prefill_tc.cu",
     "decode_attention_fused.cu",
+    "tma.cu",
 ]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

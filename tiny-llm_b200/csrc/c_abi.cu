@@ -48,6 +48,51 @@ int sm_count() {
 
 static bool float_dtype(int dtype) { return dtype == TL_F32 || dtype == TL_F16 || dtype == TL_BF16; }
 
+// ------------------------------------------------------- kernel selection --
+// W4A16 projections, by activation rows M: up to 8 the weight-streaming kernel (w4a16_matvec.cu, the reference's matvec
+// limit, quantize.py:162-163); 9..128 the swap-AB wgmma kernel with the reduction split over CTAs (w4a16_skinny.cu),
+// one token tile; above that the same kernel on 128-token tiles.  !use_simdgroup is the scalar control kernel.
+// Row counts 9..128 share that kernel and its split count (a function of N and K), so the decode engine's 16-, 32- and
+// 64-row graphs give a row the same bits.
+constexpr int SKINNY_MIN_ROWS = TL_MATVEC_REF_ROWS + 1;
+enum class W4Path { VANILLA, STREAM, SKINNY, TILES };
+
+// `fused`: the call is one of the fused forms.  Only the split-reduction launch carries their epilogues, so they keep
+// M > 128 on the streaming kernel.  The wgmma kernels read a plain [M, N] activation through TMA: a prologue or a row
+// stride other than N needs the streaming kernel.
+static W4Path w4a16_path(int M, int N, int K, int dtype, bool use_simdgroup, bool fused, int prologue, int lda) {
+    if (!use_simdgroup) return W4Path::VANILLA;
+    const bool wgmma = (dtype == TL_BF16 || dtype == TL_F16) && K > 0 && N % 128 == 0 && prologue == TL_PRO_NONE && lda == N;
+    if (wgmma && M >= SKINNY_MIN_ROWS && M <= 128) return W4Path::SKINNY;
+    if (wgmma && !fused && M > 128) return W4Path::TILES;
+    return W4Path::STREAM;
+}
+
+// Paged attention.  bf16 with D = 128 has the tensor-core and GQA-grouped kernels, which read q and K/V in 16-byte
+// vectors; everything else runs the row-wise kernel.  Decode steps (L <= PAGED_DECODE_ROWS) split each request's key
+// range over CTAs so that a small batch still fills the GPU.  Their workspace follows from dtype and D alone
+// (tl_paged_attention_workspace); pointer alignment only chooses between kernels that fit it.
+enum class PagedPath { ROWWISE, GQA, FLASH, WGMMA };
+constexpr int PAGED_D = 128;
+constexpr int PAGED_DECODE_ROWS = 8;  // query positions of a decode step (the reference's decode branch, paged_attention.cpp:168)
+// From this key range (max_pages x page_size) decode streams K/V through TMA into the wgmma kernel; below it the
+// cp.async GQA kernel, whose fixed cost per CTA is lower, is faster.
+constexpr long long PAGED_WGMMA_MIN_KEYS = 1024;
+
+// `decode`: L <= PAGED_DECODE_ROWS on tl_paged_attention; the token-major form has only the unsplit wgmma kernel and
+// passes false.
+static PagedPath paged_attention_path(const void *q, const void *kp, const void *vp, const void *out, int rows, int L, int D, int num_pages,
+                                      int page_size, int max_pages, int num_kv_heads, int num_heads, int dtype, bool decode) {
+    if (dtype != TL_BF16 || D != PAGED_D || !aligned16(q) || !aligned16(kp) || !aligned16(vp)) return PagedPath::ROWWISE;
+    const bool wgmma = aligned16(out) && paged_prefill_tc_supported(L, num_pages, page_size, num_kv_heads, num_heads);
+    if (decode) {
+        const bool one_tile = L <= 128 / (num_heads / num_kv_heads);  // the G x L query rows of a KV head fill one 128-row MMA tile
+        return wgmma && one_tile && static_cast<long long>(max_pages) * page_size >= PAGED_WGMMA_MIN_KEYS ? PagedPath::WGMMA : PagedPath::GQA;
+    }
+    if (wgmma) return PagedPath::WGMMA;
+    return rows <= 65535 ? PagedPath::FLASH : PagedPath::GQA;  // the mma.sync kernel puts the query rows on grid.y
+}
+
 }  // namespace tl
 
 using namespace tl;
@@ -74,26 +119,13 @@ int tl_device_info(int *sms, int *major, int *minor) {
 }
 
 // ------------------------------------------------------------ W4A16 ------
-// Dispatch by activation rows (use_simdgroup): M <= 8 weight-streaming matvec (the reference's matvec limit,
-// quantize.py:162-163); 9..128 swap-AB wgmma GEMM with split reduction (w4a16_skinny.cu); above that the same
-// kernel on 128-token tiles.  The streaming kernel also takes what the tensor-core kernels cannot.
-static bool use_skinny_kernel(int M, int N, int K, int dtype, int use_simdgroup) {
-    return use_simdgroup && M > TL_MATVEC_REF_ROWS && w4a16_skinny_supported(M, N, K, dtype);
-}
-static bool use_stream_kernel(int M, int N, int K, int dtype, int use_simdgroup) {
-    return use_simdgroup && !use_skinny_kernel(M, N, K, dtype, use_simdgroup) &&
-           (M <= TL_MATVEC_MAX_ROWS || !w4a16_gemm_supported(M, N, K, dtype));
-}
-
-size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_simdgroup, int use_split_k) {
-    if (!use_simdgroup) return 0;
-    if (use_skinny_kernel(M, N, K, dtype, use_simdgroup)) return w4a16_skinny_workspace(M, N, K);
-    if (use_stream_kernel(M, N, K, dtype, use_simdgroup)) return 0;
-    return w4a16_gemm_workspace(M, N, K, dtype, use_split_k);
+size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_simdgroup, int /*use_split_k*/) {
+    if (w4a16_path(M, N, K, dtype, use_simdgroup, false, TL_PRO_NONE, N) == W4Path::SKINNY) return w4a16_skinny_workspace(M, N, K);
+    return 0;
 }
 
 int tl_quantized_matmul(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N,
-                        int K, int dtype, int use_simdgroup, int use_split_k, void *workspace, size_t workspace_bytes,
+                        int K, int dtype, int use_simdgroup, int /*use_split_k*/, void *workspace, size_t workspace_bytes,
                         void *stream) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
     if (M < 0 || N <= 0 || K < 0) return fail(TL_EINVAL, "quantized_matmul: negative dimension");
@@ -103,12 +135,14 @@ int tl_quantized_matmul(const void *scales, const void *biases, const void *a, c
         return fail(TL_EINVAL, "quantized_matmul: null pointer");
     }
     cudaStream_t st = as_stream(stream);
-    if (!use_simdgroup) return launch_w4a16_vanilla(scales, biases, a, b, out, M, N, K, dtype, st);
-    if (M > 0 && K > 0 && use_skinny_kernel(M, N, K, dtype, use_simdgroup))
-        return launch_w4a16_skinny(scales, biases, a, b, out, nullptr, M, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st);
-    if (use_stream_kernel(M, N, K, dtype, use_simdgroup))
-        return launch_w4a16_stream(scales, biases, a, b, out, M, N, K, dtype, st);
-    return launch_w4a16_gemm(scales, biases, a, b, out, M, N, K, dtype, use_split_k, workspace, workspace_bytes, st);
+    switch (w4a16_path(M, N, K, dtype, use_simdgroup, false, TL_PRO_NONE, N)) {
+        case W4Path::VANILLA: return launch_w4a16_vanilla(scales, biases, a, b, out, M, N, K, dtype, st);
+        case W4Path::SKINNY:
+            return launch_w4a16_skinny(scales, biases, a, b, out, nullptr, M, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st);
+        case W4Path::TILES: return launch_w4a16_tiles(scales, biases, a, b, out, M, N, K, dtype, st);
+        case W4Path::STREAM: break;
+    }
+    return launch_w4a16_fused(scales, biases, b, out, a, nullptr, nullptr, M, N, K, N, TL_PRO_NONE, TL_EPI_NONE, 0.f, dtype, st);
 }
 
 int tl_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight, void *out,
@@ -215,9 +249,10 @@ int tl_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *
                                            src_token_stride, dtype, as_stream(stream));
 }
 
-size_t tl_paged_attention_workspace(int rows, int L, int D, int num_kv_heads, int num_heads, int dtype) {
-    if (L > 8) return 0;
-    return paged_decode_workspace(rows, L, D, num_kv_heads, num_heads, dtype);
+size_t tl_paged_attention_workspace(int rows, int L, int D, int /*num_kv_heads*/, int /*num_heads*/, int dtype) {
+    // partial O, running max and sum of every query row and split of the split-KV decode kernels
+    if (L > PAGED_DECODE_ROWS || dtype != TL_BF16 || D != PAGED_D) return 0;
+    return static_cast<size_t>(rows) * L * PAGED_MAX_SPLITS * (PAGED_D + 2) * sizeof(float);
 }
 
 int tl_paged_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
@@ -237,12 +272,22 @@ int tl_paged_attention(const void *q, const void *key_pages, const void *value_p
     if (!q || !key_pages || !value_pages || !block_table || !context_lens || !out)
         return fail(TL_EINVAL, "paged_attention: null pointer");
     cudaStream_t st = as_stream(stream);
-    if (L <= 8)
-        return launch_paged_decode(q, key_pages, value_pages, block_table, context_lens, out, rows, L, D, num_pages,
-                                   page_size, max_pages, scale, is_causal, num_kv_heads, num_heads, dtype, workspace,
-                                   workspace_bytes, st);
-    return launch_paged_prefill(q, key_pages, value_pages, block_table, context_lens, out, rows, L, D, num_pages,
-                                page_size, max_pages, scale, is_causal, num_kv_heads, num_heads, dtype, st);
+    const bool decode = L <= PAGED_DECODE_ROWS;
+    switch (paged_attention_path(q, key_pages, value_pages, out, rows, L, D, num_pages, page_size, max_pages, num_kv_heads, num_heads, dtype,
+                                 decode)) {
+        case PagedPath::WGMMA:
+            return launch_paged_prefill_tc(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages,
+                                           scale, is_causal, num_kv_heads, num_heads, decode, workspace, workspace_bytes, st);
+        case PagedPath::FLASH:
+            return launch_paged_prefill_fa(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages,
+                                           scale, is_causal, num_kv_heads, num_heads, st);
+        case PagedPath::GQA:
+            return launch_paged_gqa(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages, scale,
+                                    is_causal, num_kv_heads, num_heads, decode, workspace, workspace_bytes, st);
+        case PagedPath::ROWWISE: break;
+    }
+    return launch_paged_rowwise(q, key_pages, value_pages, block_table, context_lens, out, rows, L, D, num_pages, page_size, max_pages, scale,
+                                is_causal, num_kv_heads, num_heads, dtype, st);
 }
 
 int tl_paged_attention_token_major(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
@@ -253,8 +298,8 @@ int tl_paged_attention_token_major(const void *q, const void *key_pages, const v
         return fail(TL_EINVAL, "paged_attention_token_major: bad shape");
     if (static_cast<long long>(rows) * L == 0) return TL_OK;
     if (!q || !key_pages || !value_pages || !block_table || !context_lens || !out) return fail(TL_EINVAL, "paged_attention: null pointer");
-    if (!paged_prefill_tc_supported(L, num_pages, page_size, num_kv_heads, num_heads) || !aligned16(q) || !aligned16(out) || !aligned16(key_pages) ||
-        !aligned16(value_pages))
+    if (paged_attention_path(q, key_pages, value_pages, out, rows, L, PAGED_D, num_pages, page_size, max_pages, num_kv_heads, num_heads, TL_BF16,
+                             false) != PagedPath::WGMMA)
         return fail(TL_EINVAL, "paged_attention_token_major: needs the wgmma kernel (bf16, D = 128, pages a multiple of 64 slots)");
     return launch_paged_prefill_tc(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages, scale,
                                    is_causal, num_kv_heads, num_heads, false, nullptr, 0, as_stream(stream), true);
@@ -273,7 +318,7 @@ int tl_argmax(const void *logits, int32_t *out_tokens, int rows, int vocab, int 
 }
 
 size_t tl_quantized_matmul_fused_workspace(int M, int N, int K, int lda, int prologue, int dtype) {
-    if (prologue == TL_PRO_NONE && lda == N && use_skinny_kernel(M, N, K, dtype, 1)) return w4a16_skinny_workspace(M, N, K);
+    if (w4a16_path(M, N, K, dtype, true, true, prologue, lda) == W4Path::SKINNY) return w4a16_skinny_workspace(M, N, K);
     return 0;
 }
 
@@ -290,7 +335,7 @@ int tl_quantized_matmul_fused(const void *scales, const void *biases, const void
     if (M == 0 || K == 0) return TL_OK;
     if (!scales || !biases || !b || !out || !p0 || (prologue != TL_PRO_NONE && !p1) || (epilogue == TL_EPI_RESIDUAL && !residual))
         return fail(TL_EINVAL, "quantized_matmul_fused: null pointer");
-    if (prologue == TL_PRO_NONE && lda == N && use_skinny_kernel(M, N, K, dtype, 1))
+    if (w4a16_path(M, N, K, dtype, true, true, prologue, lda) == W4Path::SKINNY)
         return launch_w4a16_skinny(scales, biases, p0, b, out, residual, M, N, K, epilogue, dtype, workspace, workspace_bytes, as_stream(stream));
     return launch_w4a16_fused(scales, biases, b, out, p0, p1, residual, M, N, K, lda, prologue, epilogue, eps, dtype,
                               as_stream(stream));
@@ -306,7 +351,7 @@ int tl_quantized_matmul_residual_norm(const void *scales, const void *biases, co
     if (!scales || !biases || !b || !out || !p0 || !residual) return fail(TL_EINVAL, "quantized_matmul_residual_norm: null pointer");
     bool norm_done = false;
     int rc;
-    if (use_skinny_kernel(M, N, K, dtype, 1))
+    if (w4a16_path(M, N, K, dtype, true, true, TL_PRO_NONE, N) == W4Path::SKINNY)
         rc = launch_w4a16_skinny(scales, biases, p0, b, out, residual, M, N, K, TL_EPI_RESIDUAL, dtype, workspace, workspace_bytes, as_stream(stream),
                                  norm_weight, norm_eps, normed_out, &norm_done);
     else
@@ -331,7 +376,7 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
     cudaStream_t st = as_stream(stream);
     int planes = 1;
     int rc;
-    if (use_skinny_kernel(rows, N, K, dtype, 1) && qkv_planes_rope_supported(num_heads, num_kv_heads, head_dim, dtype))
+    if (w4a16_path(rows, N, K, dtype, true, true, TL_PRO_NONE, N) == W4Path::SKINNY && qkv_planes_rope_supported(num_heads, num_kv_heads, head_dim, dtype))
         rc = launch_w4a16_skinny(scales, biases, p0, b, qkv_scratch, nullptr, rows, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st, nullptr, 0.f,
                                  nullptr, nullptr, &planes);
     else

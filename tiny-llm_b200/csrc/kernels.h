@@ -39,12 +39,9 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
                                       int num_pages, int page_size, int max_pages, int dtype, cudaStream_t st, bool chunk = false);
 
 // w4a16_matvec.cu
-// Weight-streaming tensor-core kernel for M <= 32 rows per pass (larger M is
-// processed in 32-row passes), and the scalar control kernel.
-int launch_w4a16_stream(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N,
-                        int K, int dtype, cudaStream_t st);
-// TMA-bulk streaming kernel with optional fused prologue (0 none: p0 = a; 1 rms_norm: p0 = x, p1 = norm weight;
-// 2 swiglu: p0 = gate, p1 = up; lda = row stride of p0/p1 in elements) and epilogue (0 none; 1 out = residual + result).
+// Weight-streaming tensor-core kernel, up to 32 rows per pass (larger M is processed in passes), with optional fused
+// prologue (0 none: p0 = a; 1 rms_norm: p0 = x, p1 = norm weight; 2 swiglu: p0 = gate, p1 = up; lda = row stride of
+// p0/p1 in elements) and epilogue (0 none; 1 out = residual + result); and the scalar control kernel.
 int launch_w4a16_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
                        const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype,
                        cudaStream_t st);
@@ -53,9 +50,7 @@ bool use_pdl();
 int launch_w4a16_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
                          int N, int K, int dtype, cudaStream_t st);
 
-
 // w4a16_skinny.cu (swap-AB wgmma GEMM: split reduction for 9 <= M <= 128, 128-token tiles for prefill)
-bool w4a16_skinny_supported(int M, int N, int K, int dtype);
 int w4a16_skinny_splits(int M, int N, int K);
 size_t w4a16_skinny_workspace(int M, int N, int K);
 // norm_w / normed (optional, residual epilogue): also write normed = rms_norm(out, norm_w, norm_eps); *norm_done tells
@@ -71,13 +66,6 @@ bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype);
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,
                                   int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages, cudaStream_t st, bool chunk);
-
-// w4a16_gemm.cu (prefill GEMM: dispatch onto launch_w4a16_tiles)
-bool w4a16_gemm_supported(int M, int N, int K, int dtype);
-int w4a16_gemm_split(int M, int N, int K, int use_split_k);
-size_t w4a16_gemm_workspace(int M, int N, int K, int dtype, int use_split_k);
-int launch_w4a16_gemm(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N,
-                      int K, int dtype, int use_split_k, void *ws, size_t ws_bytes, cudaStream_t st);
 
 // decode_attention_fused.cu
 #if defined(TL_TRACE) && TL_TRACE
@@ -96,11 +84,18 @@ int launch_decode_attention_fused(const void *qkv, const void *q_norm_weight, co
 int launch_decode_attention(const void *q, const void *k, const void *v, const float *mask, void *out, int q_rows,
                             int L, int S, int D, int num_heads, int num_kv_heads, float scale, int is_causal,
                             int has_mask, int dtype, cudaStream_t st);
-size_t paged_decode_workspace(int rows, int L, int D, int num_kv_heads, int num_heads, int dtype);
-int launch_paged_decode(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out,
-                        int rows, int L, int D, int num_pages, int page_size, int max_pages, float scale,
-                        int is_causal, int num_kv_heads, int num_heads, int dtype, void *ws, size_t ws_bytes,
-                        cudaStream_t st);
+// Any dtype / head size / page size: one CTA per query row.
+int launch_paged_rowwise(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows, int L,
+                         int D, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads, int num_heads,
+                         int dtype, cudaStream_t st);
+// bf16, D = 128, 16-byte aligned q / K / V: the CUDA-core GQA-grouped kernel; allow_split cuts the key range into up to
+// PAGED_MAX_SPLITS pieces (partials in ws) so that a small batch still fills the GPU.
+int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows, int L,
+                     int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads, int num_heads, bool allow_split,
+                     void *ws, size_t ws_bytes, cudaStream_t st);
+// Split-KV decode cuts a request's key range into at most this many pieces: the merge kernel then reads the scalars
+// of all splits in one load per lane of a warp.  The workspace of tl_paged_attention is sized for it.
+constexpr int PAGED_MAX_SPLITS = 32;
 
 // attention_prefill_tc.cu (wgmma + TMA flash prefill; page_size % 64 == 0, Hq/Hkv divides 128)
 bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_heads, int num_heads);
@@ -113,8 +108,5 @@ int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, cudaStream_t st);
-int launch_paged_prefill(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out,
-                         int rows, int L, int D, int num_pages, int page_size, int max_pages, float scale,
-                         int is_causal, int num_kv_heads, int num_heads, int dtype, cudaStream_t st);
 
 }  // namespace tl

@@ -22,16 +22,6 @@
 
 namespace tl {
 
-int launch_w4a16_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
-                       const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype,
-                       cudaStream_t st);
-
-int launch_w4a16_stream(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N,
-                        int K, int dtype, cudaStream_t st) {
-    if (M == 0 || K == 0) return TL_OK;
-    return launch_w4a16_fused(scales, biases, b, out, a, nullptr, nullptr, M, N, K, N, 0, 0, 0.f, dtype, st);
-}
-
 // ---------------------------------------------------------------------------
 // v5: register-pipelined streaming, contiguous rows per CTA (see w4a16_item.cuh for the
 // instruction budget of the inner loop).
@@ -293,13 +283,13 @@ static size_t stream5_smem_bytes(int N, int K, int MP, int grid) {
 }
 
 // ---- launch geometry
-// One CTA per SM minus TL_S5_RESERVE (default 8): the few CTAs of the kernel behind it (the 8-CTA attention launch, the
-// first CTAs of the next projection) then start early under programmatic dependent launch and issue their independent
-// loads while this one is still running.
+// One CTA per SM minus S5_RESERVED_SMS: the few CTAs of the kernel behind it (the 8-CTA attention launch, the first CTAs
+// of the next projection) then start early under programmatic dependent launch and issue their independent loads while
+// this one is still running.
+constexpr int S5_RESERVED_SMS = 8;
 static int stream5_grid(int K) {
-    static const int reserve = [] { const char *e = getenv("TL_S5_RESERVE"); const int v = e ? atoi(e) : 8; return v < 0 ? 0 : v; }();
     const int all = (K + 15) / 16;
-    int sms = sm_count() - reserve;
+    int sms = sm_count() - S5_RESERVED_SMS;
     if (sms < 1) sms = 1;
     return all < sms ? all : sms;
 }

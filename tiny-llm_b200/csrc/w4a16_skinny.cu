@@ -21,10 +21,7 @@
 //                      quantized_matmul.metal:183-194) and stores them in the K-major 128-byte-swizzled layout
 //                      wgmma reads; then the warpgroup issues eight wgmma m64nNTk16 (fp32 accumulators in
 //                      registers) and dequantises the next block while they run (two A stages per warpgroup).
-#include <stdlib.h>
-
-#include <mutex>
-#include <unordered_map>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -394,13 +391,6 @@ __global__ void __launch_bounds__(256) w4a16_skinny_reduce_norm_kernel(const flo
 }
 
 // ---------------------------------------------------------------- host side --
-bool w4a16_skinny_supported(int M, int N, int K, int dtype) {
-    static const bool off = [] { const char *e = getenv("TL_SKINNY"); return e != nullptr && e[0] == '0'; }();
-    static const int min_rows = [] { const char *e = getenv("TL_SKINNY_MIN_ROWS"); return e ? atoi(e) : 9; }();
-    if (off) return false;
-    return (dtype == TL_BF16 || dtype == TL_F16) && M >= min_rows && M <= 128 && K > 0 && N % 128 == 0;
-}
-
 // Split policy (ours; the reference's constants are M4-Pro tuning, quantized_matmul.cpp:138-150): the split count that
 // minimises waves x (group blocks per CTA + fixed cost) + reduce launch, with `slots` CTAs resident at once (one per
 // SM), a fixed cost per CTA worth ~10 group blocks (barrier set-up, first TMA round trips, epilogue) and ~8 for the
@@ -427,49 +417,19 @@ size_t w4a16_skinny_workspace(int M, int N, int K) {
     return splits > 1 ? static_cast<size_t>(splits) * M * K * sizeof(float) : 0;
 }
 
-struct SkMapKey {
-    const void *ptr;
-    unsigned long long d0, d1;
-    unsigned b0, b1;
-    int kind;
-    bool operator==(const SkMapKey &o) const { return ptr == o.ptr && d0 == o.d0 && d1 == o.d1 && b0 == o.b0 && b1 == o.b1 && kind == o.kind; }
-};
-struct SkMapKeyHash {
-    size_t operator()(const SkMapKey &k) const {
-        size_t h = reinterpret_cast<size_t>(k.ptr);
-        for (unsigned long long v : {k.d0, k.d1, static_cast<unsigned long long>(k.b0), static_cast<unsigned long long>(k.b1), static_cast<unsigned long long>(k.kind)})
-            h = h * 1000003u ^ static_cast<size_t>(v);
-        return h;
-    }
-};
-// 2-D tensor maps cached per (pointer, shape): kind 0 = 16-bit activations [rows, cols] with the 128-byte swizzle,
-// kind 1 = packed weights as bytes [rows, cols/2], 128-byte boxes with the 128-byte swizzle.
-static int sk_cached_map(CUtensorMap *out, const void *ptr, int kind, cuuint64_t cols, cuuint64_t rows, cuuint32_t box_cols, cuuint32_t box_rows,
-                         CUtensorMapDataType dt, size_t elem) {
-    static std::mutex mu;
-    static std::unordered_map<SkMapKey, CUtensorMap, SkMapKeyHash> cache;
-    SkMapKey key{ptr, cols, rows, box_cols, box_rows, kind * 4 + static_cast<int>(dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT16)};
-    std::lock_guard<std::mutex> lock(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) {
-        *out = it->second;
-        return TL_OK;
-    }
-    PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-    if (encode == nullptr) return fail(TL_ECUDA, "quantized_matmul: cuTensorMapEncodeTiled is unavailable");
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {cols * elem};
-    const cuuint32_t box[2] = {box_cols, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUtensorMap map;
-    CUresult r = encode(&map, dt, 2, const_cast<void *>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(TL_ECUDA, "quantized_matmul: cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-    if (cache.size() > 8192) cache.clear();
-    cache.emplace(key, map);
-    *out = map;
-    return TL_OK;
+// Tensor maps of the activations a [M, N] (16-bit, [nt tokens x 64] boxes) and of the packed weights b [K, N/2] (bytes,
+// 128 rows x 128-byte boxes), both with the 128-byte swizzle wgmma reads.
+template <typename T>
+static int sk_maps(CUtensorMap *ma, CUtensorMap *mw, const void *a, const void *b, int M, int N, int K, int nt) {
+    const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const cuuint64_t a_dims[2] = {static_cast<cuuint64_t>(N), static_cast<cuuint64_t>(M)};
+    const cuuint32_t a_box[2] = {SK_KB, static_cast<cuuint32_t>(nt)};
+    const cuuint64_t w_dims[2] = {static_cast<cuuint64_t>(N) / 2, static_cast<cuuint64_t>(K)};
+    const cuuint32_t w_box[2] = {SK_PG * SK_GB / 2, SK_FEAT};
+    if (int e = cached_tensor_map(ma, a, dt, 2, a_dims, a_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "quantized_matmul"))
+        return e;
+    return cached_tensor_map(mw, b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, w_dims, w_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                             "quantized_matmul");
 }
 
 template <typename T, int NT>
@@ -505,9 +465,7 @@ static int skinny_t(const void *scales, const void *biases, const void *a, const
         return fail(TL_EWORKSPACE, "quantized_matmul: workspace too small (%zu < %zu)", ws_bytes, w4a16_skinny_workspace(M, N, K));
     args.partials = static_cast<float *>(ws);
     CUtensorMap ma, mw;
-    const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    if (int e = sk_cached_map(&ma, a, 0, N, M, SK_KB, NT, dt, 2)) return e;
-    if (int e = sk_cached_map(&mw, b, 1, static_cast<cuuint64_t>(N) / 2, K, SK_PG * SK_GB / 2, SK_FEAT, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1)) return e;
+    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, NT)) return e;
     const dim3 grid(tiles * args.splits);
     int rc;
     switch (NT) {
@@ -564,9 +522,7 @@ static int tiles_t(const void *scales, const void *biases, const void *a, const 
     args.M = M, args.N = N, args.K = K, args.epilogue = SK_EPI_NONE;
     args.splits = 1, args.gb_per_split = N / SK_GB;
     CUtensorMap ma, mw;
-    const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    if (int e = sk_cached_map(&ma, a, 0, N, M, SK_KB, 128, dt, 2)) return e;
-    if (int e = sk_cached_map(&mw, b, 1, static_cast<cuuint64_t>(N) / 2, K, SK_PG * SK_GB / 2, SK_FEAT, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1)) return e;
+    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, 128)) return e;
     const dim3 grid((K + SK_FEAT - 1) / SK_FEAT, (M + 127) / 128);
     if (grid.y > 65535) return fail(TL_EINVAL, "quantized_matmul: too many rows for one launch");
     return skinny_launch<T, 128>(ma, mw, args, grid, st);

@@ -250,7 +250,9 @@ struct Wgmma<__half, 128, 0> {
     }
 };
 
-// cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda).
-PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder();
+// tma.cu: *out = the tensor map of the dense row-major tensor at ptr (dims innermost first, box in elements; dtype bytes,
+// bf16 or f16), encoded once per distinct argument set and cached.  `what` prefixes the error message.
+int cached_tensor_map(CUtensorMap *out, const void *ptr, CUtensorMapDataType dtype, int rank, const cuuint64_t *dims, const cuuint32_t *box,
+                      CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char *what);
 
 }  // namespace tl

@@ -25,8 +25,6 @@ front and the engine re-captures if a slab pointer changes.
 
 from __future__ import annotations
 
-import os
-
 from types import SimpleNamespace
 
 import numpy as np
@@ -36,6 +34,10 @@ from extensions_b200 import tiny_llm_ext_b200 as ext
 
 from .kv_cache import BatchingKvCache
 from .paged_kv_cache import TinyKvPagedCache
+
+# Decode attention runs as one fused launch while slots x max_seq_len stays within this: beyond it the K/V stream, not
+# the launch count, bounds the step.
+FUSED_ATTENTION_MAX_SLOT_TOKENS = 16384
 
 
 def _concat_weights(parts):
@@ -97,7 +99,8 @@ class _SlotRecord:
 
 
 class DecodeEngine:
-    def __init__(self, model, batch_size: int, max_seq_len: int, device, log_capacity: int = 4096, fused: bool = True):
+    def __init__(self, model, batch_size: int, max_seq_len: int, device, log_capacity: int = 4096, fused: bool = True, *,
+                 _row_variants: bool = True):
         self.model = model
         self.B = batch_size
         self.device = torch.device(device)
@@ -158,13 +161,11 @@ class DecodeEngine:
         # The one-launch attention is a latency design (few CTAs, K/V rows staged per lane): it wins while the
         # step is launch-bound.  With many slots or long contexts the K/V stream dominates and the step uses
         # q/k norm + rope + append as one small launch followed by tl_paged_attention, whose long-context path
-        # is the TMA + wgmma streaming kernel (attention_prefill_tc.cu).  TL_ATTENTION_FUSED=0/1 forces either.
-        fused_env = os.environ.get("TL_ATTENTION_FUSED")
-        fused_pays = self.B * self.max_seq_len <= int(os.environ.get("TL_ATTENTION_FUSED_MAX_TOKENS", "16384"))
+        # is the TMA + wgmma streaming kernel (attention_prefill_tc.cu).
         self._attention_fused = (self.fused and self.D == 128 and self.Hq // self.Hkv <= 4
                                  and model.embedding.weight.scales.dtype == torch.bfloat16
                                  and not getattr(attn0.rope, "traditional", False)
-                                 and (fused_env == "1" or (fused_env != "0" and fused_pays)))
+                                 and self.B * self.max_seq_len <= FUSED_ATTENTION_MAX_SLOT_TOKENS)
         if self._attention_fused:
             self._rope_inv_freq = ext.rope_inv_freq_table(self.D, attn0.rope.base, self.device)
             self._attn_ws = torch.empty(ext.decode_attention_fused_workspace(self.B, self.Hq, self.Hkv), dtype=torch.float32, device=self.device)
@@ -173,9 +174,9 @@ class DecodeEngine:
         # full one and step() replays the smallest that covers the highest occupied slot: every kernel of the wide
         # path costs by rows (swap-AB column count, attention CTAs, reduction planes).  All variants stay on the
         # >= 9-row kernels and the split counts do not depend on the row count, so a row's result is bit-identical
-        # whichever variant computed it.  (Config 4 runs 64 slots with ~20 live.)
-        rows_env = os.environ.get("TL_ROW_VARIANTS", "1")
-        self._variants = sorted({r for r in (16, 32, 64) if r < self.B} | {self.B}) if (self.fused and self.B > 16 and rows_env != "0") else [self.B]
+        # whichever variant computed it.  (Config 4 runs 64 slots with ~20 live.)  _row_variants=False keeps only the
+        # full-width graph: the reference those bits are tested against.
+        self._variants = sorted({r for r in (16, 32, 64) if r < self.B} | {self.B}) if (self.fused and self.B > 16 and _row_variants) else [self.B]
         self._graphs: dict = {}
         self.variant_replays = {r: 0 for r in self._variants}
 
