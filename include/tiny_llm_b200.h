@@ -107,13 +107,31 @@ int tl_paged_cache_update(void *pages, const void *values, int num_pages, int he
                           int length, int page_id, int start, int dtype, void *stream);
 /* q,out [B*Hq, L, D]; pages [P, Hkv, page, D]; block_table int32 [B, max_pages]
  * (-1 padded); context_lens int32 [B] (post-append).  D <= 128; the tensor-core
- * prefill branch (L > 8, bf16) requires D == 128.  Rows that see no key are
- * written as zeros.  Workspace holds split-KV partials for the decode branch. */
+ * prefill branch (L > 8, bf16) requires D == 128.  Query row l of request b
+ * sees the keys < min(clamp(ctx - L + l + 1, 0, ctx), max_pages * page_size)
+ * when causal (< min(ctx, max_pages * page_size) otherwise), ctx =
+ * context_lens[b]: a context longer than the block table keeps its causal
+ * alignment and loses the keys past the table.  Keys in pages whose id is < 0
+ * or >= num_pages are skipped.  Rows that see no key are written as zeros.
+ * Workspace holds split-KV partials for the decode branch. */
 size_t tl_paged_attention_workspace(int rows, int L, int D, int num_kv_heads, int num_heads, int dtype);
 int tl_paged_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
                        const int32_t *context_lens, void *out, int rows, int L, int D, int num_pages,
                        int page_size, int max_pages, float scale, int is_causal, int num_kv_heads, int num_heads,
                        int dtype, void *workspace, size_t workspace_bytes, void *stream);
+/* The kernel tl_paged_attention would run for these arguments (nothing is launched or read; the pointers only count
+ * for their 16-byte alignment): one of TL_PAGED_*, or a negative TL_E* code for arguments tl_paged_attention rejects.
+ *   TL_PAGED_ROWWISE : one CTA per query row; every dtype, head size and page size;
+ *   TL_PAGED_GQA     : bf16, D == 128, 16-byte aligned q / K / V; CUDA cores, the query heads of a KV head together;
+ *                      decode steps (L <= 8) split the key range over CTAs (plus a merge launch);
+ *   TL_PAGED_FLASH   : bf16, D == 128 prefill (L > 8) on mma.sync, for page sizes or head ratios the wgmma kernel
+ *                      does not take;
+ *   TL_PAGED_WGMMA   : bf16, D == 128, pages a multiple of 64 slots, Hq / Hkv divides 128, out 16-byte aligned; every
+ *                      prefill, and decode steps whose G x L query rows fill one 128-row tile and whose block table
+ *                      spans at least 1024 keys (split like the GQA kernel). */
+enum { TL_PAGED_ROWWISE = 0, TL_PAGED_GQA = 1, TL_PAGED_FLASH = 2, TL_PAGED_WGMMA = 3 };
+int tl_paged_attention_route(const void *q, const void *key_pages, const void *value_pages, const void *out, int rows, int L, int D,
+                             int num_pages, int page_size, int max_pages, int num_kv_heads, int num_heads, int dtype);
 /* The prefill form with the output written token-major: out [B, L, Hq * D] (the layout the o-projection takes; saves
  * the transpose copy of a chunked-prefill step).  bf16, D == 128, pages a multiple of 64 slots (the wgmma kernel);
  * TL_EINVAL otherwise - callers then use tl_paged_attention and transpose. */

@@ -122,3 +122,79 @@ def test_gate_up_interleave_layout_and_span_record():
         raise AssertionError("rows not divisible by 8 must be rejected")
     assert ctypes.sizeof(ext.PageSpanList) == 4 * 64 * 4 + 4
     assert ext.EPI_SWIGLU_PAIRS == 2 and ext.PAGE_SPANS == 64
+
+
+# ------------------------------------------------------- paged attention routing --
+# tl_paged_attention_route answers from sizes and pointer alignment alone, so the selection rules of
+# paged_attention_path() (c_abi.cu) are checked here with made-up addresses: nothing is read or launched.
+A16, A2 = 0x7F0000010000, 0x7F0000010002  # 16-byte aligned, and 2 bytes past that (a bf16 element offset)
+BF, F32 = torch.bfloat16, torch.float32
+
+
+def route(L=1, D=128, page=64, max_pages=16, Hq=32, Hkv=8, B=1, dtype=BF, q=A16, k=A16, v=A16, out=A16, num_pages=64):
+    return ext.paged_attention_route(q, k, v, out, B * Hq, L, D, num_pages, page, max_pages, Hkv, Hq, dtype)
+
+
+def test_route_rowwise_for_f32_other_head_sizes_and_unaligned_operands():
+    assert route(dtype=F32) == ext.PAGED_ROWWISE
+    assert route(dtype=F32, L=300) == ext.PAGED_ROWWISE
+    for D in (64, 80, 127):
+        assert route(D=D) == ext.PAGED_ROWWISE
+    for where in ("q", "k", "v"):
+        assert route(**{where: A2}) == ext.PAGED_ROWWISE, where
+        assert route(L=100, **{where: A2}) == ext.PAGED_ROWWISE, where
+    assert route(q=A16 + 8) == ext.PAGED_ROWWISE  # 8-byte alignment is not enough for the 16-byte vector loads
+
+
+def test_route_decode_key_range_boundary():
+    # PAGED_WGMMA_MIN_KEYS = 1024: the block table's capacity, not the context, decides
+    assert route(page=64, max_pages=15) == ext.PAGED_GQA
+    assert route(page=64, max_pages=16) == ext.PAGED_WGMMA
+    assert route(page=128, max_pages=7) == ext.PAGED_GQA
+    assert route(page=128, max_pages=8) == ext.PAGED_WGMMA
+    assert route(page=1024, max_pages=1) == ext.PAGED_WGMMA
+    # pages that are not a multiple of 64 slots never reach the wgmma kernel
+    assert route(page=16, max_pages=4096) == ext.PAGED_GQA
+    assert route(page=96, max_pages=100) == ext.PAGED_GQA
+    assert route(page=192, max_pages=100) == ext.PAGED_WGMMA
+    # the wgmma kernel writes out with 16-byte stores
+    assert route(page=64, max_pages=16, out=A2) == ext.PAGED_GQA
+
+
+def test_route_decode_rows_and_one_tile_rule():
+    # PAGED_DECODE_ROWS = 8: L <= 8 is a decode step, L = 9 a prefill whatever the key range
+    assert route(L=8, page=64, max_pages=1, Hq=8, Hkv=8) == ext.PAGED_GQA
+    assert route(L=9, page=64, max_pages=1, Hq=8, Hkv=8) == ext.PAGED_WGMMA
+    assert route(L=9, page=16, max_pages=1, Hq=8, Hkv=8) == ext.PAGED_FLASH
+    # decode reaches the wgmma kernel only while the G x L query rows of a KV head fit one 128-row tile
+    assert route(L=8, Hq=32, Hkv=2) == ext.PAGED_WGMMA  # G = 16: 128 rows
+    assert route(L=8, Hq=32, Hkv=1) == ext.PAGED_GQA    # G = 32: 256 rows
+    assert route(L=4, Hq=32, Hkv=1) == ext.PAGED_WGMMA  # 128 rows
+    assert route(L=5, Hq=32, Hkv=1) == ext.PAGED_GQA    # 160 rows
+    assert route(L=1, Hq=128, Hkv=1) == ext.PAGED_WGMMA
+    assert route(L=2, Hq=128, Hkv=1) == ext.PAGED_GQA
+
+
+def test_route_prefill_head_ratio_page_size_and_grid_limit():
+    assert route(L=100) == ext.PAGED_WGMMA
+    assert route(L=100, page=16) == ext.PAGED_FLASH
+    assert route(L=100, page=32) == ext.PAGED_FLASH
+    assert route(L=100, Hq=6, Hkv=2) == ext.PAGED_FLASH     # G = 3 does not divide 128
+    assert route(L=100, Hq=256, Hkv=1) == ext.PAGED_FLASH   # G = 256 > 128
+    assert route(L=100, Hq=128, Hkv=1) == ext.PAGED_WGMMA
+    assert route(L=100, out=A2) == ext.PAGED_FLASH
+    # the mma.sync kernel puts the B * Hq query rows on grid.y (at most 65535)
+    assert route(L=100, page=16, Hq=1, Hkv=1, B=65535) == ext.PAGED_FLASH
+    assert route(L=100, page=16, Hq=1, Hkv=1, B=65536) == ext.PAGED_GQA
+    assert route(L=100, page=64, Hq=1, Hkv=1, B=65536) == ext.PAGED_WGMMA
+
+
+def test_route_rejects_what_paged_attention_rejects():
+    with pytest.raises(RuntimeError, match="num_heads must be divisible"):
+        route(Hq=6, Hkv=4)
+    with pytest.raises(RuntimeError, match="float32 or bfloat16"):
+        route(dtype=torch.float16)
+    with pytest.raises(RuntimeError, match="bfloat16 prefill requires head dimension 128"):
+        route(L=9, D=64)
+    with pytest.raises(RuntimeError, match=r"range \[1, 128\]"):
+        route(D=256, dtype=F32)

@@ -13,7 +13,10 @@
 //    K/V access is a 128-bit load of a fully used 32-byte sector.
 //
 // Causality is bottom-right aligned everywhere: query row l of an L-row chunk
-// sees keys < clamp(ctx - L + l + 1, 0, ctx)   (paged_attention.metal:158-160).
+// sees keys < clamp(ctx - L + l + 1, 0, ctx)   (paged_attention.metal:158-160),
+// then at most the max_pages * page_size keys of the block table.  The shift uses
+// the unclamped context, so every kernel keeps the same rows aligned when a
+// context is longer than its table.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -244,7 +247,8 @@ __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_kernel(
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int j = lane >> 3;  // token slot of this lane group
     const int c = lane & 7;   // 16-dim chunk owned by this lane
-    const int ctx = min(cl[batch], max_pages * page_size);
+    const int ctx = cl[batch];
+    const int cap = max_pages * page_size;  // keys the block table can hold
     const float scale2 = scale * LOG2E;
 
     float qv[RG][16], acc[RG][16], m[RG], l[RG];
@@ -261,7 +265,7 @@ __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_kernel(
         if (row < R) {
             const int hl = row / L, pos = row - hl * L;
             const int qi = (batch * num_heads + kv_head * G + hl) * L + pos;
-            vis[r] = is_causal ? min(max(ctx - L + pos + 1, 0), ctx) : ctx;
+            vis[r] = min(is_causal ? min(max(ctx - L + pos + 1, 0), ctx) : ctx, cap);  // causal shift first, as paged_rowwise_kernel
             vis_max = max(vis_max, vis[r]);
             const uint4 *src = reinterpret_cast<const uint4 *>(q + static_cast<size_t>(qi) * GQA_D + c * 16);
             const uint4 a = src[0], b = src[1];

@@ -12,7 +12,8 @@
 //           ldmatrix), S = Q K^T and O += P V with mma.sync.m16n8k16 (fp32 accumulate),
 //           probabilities rounded to bf16 for the second product (as every flash kernel does)
 //   mask  = bottom-right aligned causal limit clamp(ctx - L + l + 1, 0, ctx) per query row
-//           (attention.py:40-58 semantics), rows/pages outside the context contribute nothing
+//           (attention.py:40-58 semantics), then at most the block table's keys; rows/pages
+//           outside the context contribute nothing
 //
 // This is the mma.sync version; page sizes that are a multiple of 64 take the wgmma + TMA kernel
 // (attention_prefill_tc.cu, DESIGN.md section 4).
@@ -69,9 +70,11 @@ __global__ void __launch_bounds__(FA_THREADS) paged_prefill_fa_kernel(const bf16
     const int head_row = blockIdx.y;
     const int b = head_row / Hq, h = head_row - b * Hq;
     const int kvh = h / (Hq / Hkv);
-    const int ctx = min(cl[b], max_pages * page_size);
+    const int ctx_all = cl[b];
+    const int ctx = min(ctx_all, max_pages * page_size);  // keys the block table holds
     const int q0 = qt * FA_BM;
-    auto limit = [&](int l) { return causal ? max(0, min(ctx, ctx - L + l + 1)) : ctx; };
+    // the causal shift uses the whole context, the block table clamps afterwards (attention_decode.cu)
+    auto limit = [&](int l) { return min(causal ? max(0, min(ctx_all, ctx_all - L + l + 1)) : ctx_all, ctx); };
     const int kmax = limit(min(q0 + FA_BM - 1, L - 1));  // keys any row of this tile may see
     const int nkt = (kmax + FA_BN - 1) / FA_BN;
     if (threadIdx.x < 2) bad[threadIdx.x] = 0;

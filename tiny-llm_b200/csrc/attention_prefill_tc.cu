@@ -83,10 +83,12 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int qb = static_cast<int>(gridDim.x) / a.splits - 1 - static_cast<int>(blockIdx.x) / a.splits;  // long (late) query blocks first
     const int kvh = blockIdx.y, b = blockIdx.z;
     const int q0 = qb * a.RH;
-    const int ctx = min(a.context_lens[b], a.max_pages * a.page_size);
+    // The causal shift uses the whole context, the block table clamps afterwards (attention_decode.cu).
+    const int ctx = a.context_lens[b];
+    const int cap = a.max_pages * a.page_size;
     // keys any row of this CTA may see: [0, key_end)
     const int last_row = min(q0 + a.RH, a.L) - 1;
-    const int key_end = ctx <= 0 ? 0 : (a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx);
+    const int key_end = ctx <= 0 ? 0 : min(a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx, cap);
     const int all_tiles = (key_end + TC_BN - 1) / TC_BN;
     // Split-KV: the launch fixes the NUMBER of splits from the block table's width (the grid of a captured graph cannot
     // follow the context), the tiles are dealt out here from the request's real length, so a request far below the
@@ -171,7 +173,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             l[rr] = q0 + lq[rr];
             row_valid[rr] = l[rr] < a.L && ctx > 0;
             // last key this row may see (bottom-right causal alignment, paged_attention.metal:411)
-            limit[rr] = !row_valid[rr] ? -1 : (a.is_causal ? min(ctx - 1, l[rr] + (ctx - a.L)) : ctx - 1);
+            limit[rr] = !row_valid[rr] ? -1 : min(a.is_causal ? min(ctx - 1, l[rr] + (ctx - a.L)) : ctx - 1, cap - 1);
         }
         float o[TC_D / 2];
 #pragma unroll

@@ -72,7 +72,7 @@ static W4Path w4a16_path(int M, int N, int K, int dtype, bool use_simdgroup, boo
 // vectors; everything else runs the row-wise kernel.  Decode steps (L <= PAGED_DECODE_ROWS) split each request's key
 // range over CTAs so that a small batch still fills the GPU.  Their workspace follows from dtype and D alone
 // (tl_paged_attention_workspace); pointer alignment only chooses between kernels that fit it.
-enum class PagedPath { ROWWISE, GQA, FLASH, WGMMA };
+enum class PagedPath { ROWWISE = TL_PAGED_ROWWISE, GQA = TL_PAGED_GQA, FLASH = TL_PAGED_FLASH, WGMMA = TL_PAGED_WGMMA };
 constexpr int PAGED_D = 128;
 constexpr int PAGED_DECODE_ROWS = 8;  // query positions of a decode step (the reference's decode branch, paged_attention.cpp:168)
 // From this key range (max_pages x page_size) decode streams K/V through TMA into the wgmma kernel; below it the
@@ -255,10 +255,7 @@ size_t tl_paged_attention_workspace(int rows, int L, int D, int /*num_kv_heads*/
     return static_cast<size_t>(rows) * L * PAGED_MAX_SPLITS * (PAGED_D + 2) * sizeof(float);
 }
 
-int tl_paged_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
-                       const int32_t *context_lens, void *out, int rows, int L, int D, int num_pages, int page_size,
-                       int max_pages, float scale, int is_causal, int num_kv_heads, int num_heads, int dtype,
-                       void *workspace, size_t workspace_bytes, void *stream) {
+static int check_paged_attention(int rows, int L, int D, int num_pages, int page_size, int max_pages, int num_kv_heads, int num_heads, int dtype) {
     if (dtype != TL_F32 && dtype != TL_BF16)
         return fail(TL_EDTYPE, "paged_attention: q, key_pages, and value_pages must have the same float32 or bfloat16 dtype");
     if (num_heads <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0)
@@ -268,6 +265,21 @@ int tl_paged_attention(const void *q, const void *key_pages, const void *value_p
     if (L < 0 || num_pages <= 0 || page_size <= 0 || max_pages <= 0) return fail(TL_EINVAL, "paged_attention: bad shape");
     if (L > 8 && dtype == TL_BF16 && D != 128)
         return fail(TL_EINVAL, "paged_attention: bfloat16 prefill requires head dimension 128");
+    return TL_OK;
+}
+
+int tl_paged_attention_route(const void *q, const void *key_pages, const void *value_pages, const void *out, int rows, int L, int D,
+                             int num_pages, int page_size, int max_pages, int num_kv_heads, int num_heads, int dtype) {
+    if (int e = check_paged_attention(rows, L, D, num_pages, page_size, max_pages, num_kv_heads, num_heads, dtype)) return e;
+    return static_cast<int>(paged_attention_path(q, key_pages, value_pages, out, rows, L, D, num_pages, page_size, max_pages, num_kv_heads,
+                                                 num_heads, dtype, L <= PAGED_DECODE_ROWS));
+}
+
+int tl_paged_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                       const int32_t *context_lens, void *out, int rows, int L, int D, int num_pages, int page_size,
+                       int max_pages, float scale, int is_causal, int num_kv_heads, int num_heads, int dtype,
+                       void *workspace, size_t workspace_bytes, void *stream) {
+    if (int e = check_paged_attention(rows, L, D, num_pages, page_size, max_pages, num_kv_heads, num_heads, dtype)) return e;
     if (static_cast<long long>(rows) * L == 0) return TL_OK;
     if (!q || !key_pages || !value_pages || !block_table || !context_lens || !out)
         return fail(TL_EINVAL, "paged_attention: null pointer");

@@ -35,6 +35,7 @@ __all__ = [
     "paged_cache_update",
     "paged_attention",
     # CUDA extension
+    "paged_attention_route",
     "paged_cache_append_decode",
     "add",
     "argmax",
@@ -79,6 +80,7 @@ _SIGNATURES = {
     "tl_paged_cache_append_decode": (_I, [_VP] * 6 + [_I] * 7 + [_VP]),
     "tl_paged_attention_workspace": (_SZ, [_I] * 6),
     "tl_paged_attention": (_I, [_VP] * 6 + [_I] * 6 + [_F] + [_I] * 4 + [_VP, _SZ, _VP]),
+    "tl_paged_attention_route": (_I, [_VP] * 4 + [_I] * 9),
     "tl_argmax_workspace": (_SZ, [_I, _I]),
     "tl_argmax": (_I, [_VP, _VP, _I, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
@@ -462,6 +464,23 @@ def paged_attention(
         )
     )
     return out
+
+
+PAGED_ROWWISE, PAGED_GQA, PAGED_FLASH, PAGED_WGMMA = 0, 1, 2, 3
+
+
+def paged_attention_route(q, key_pages, value_pages, out, rows, L, D, num_pages, page_size, max_pages, num_kv_heads, num_heads, dtype):
+    """The kernel ``paged_attention`` runs for these arguments (``PAGED_ROWWISE`` / ``PAGED_GQA`` / ``PAGED_FLASH`` /
+    ``PAGED_WGMMA``), decided without launching or reading anything.  ``q``, ``key_pages``, ``value_pages`` and
+    ``out`` are tensors or plain addresses: only their 16-byte alignment counts.  ``dtype`` is a torch dtype."""
+
+    def addr(x):
+        return x.data_ptr() if isinstance(x, torch.Tensor) else int(x)
+
+    code = _lib.tl_paged_attention_route(addr(q), addr(key_pages), addr(value_pages), addr(out), int(rows), int(L), int(D), int(num_pages),
+                                         int(page_size), int(max_pages), int(num_kv_heads), int(num_heads), _DTYPE_CODE[dtype])
+    _check(min(code, 0))
+    return code
 
 
 # ---- CUDA extension (not in the reference module) -------------------------
