@@ -7,7 +7,7 @@ import torch
 
 from extensions_b200 import tiny_llm_ext_b200 as ext
 from tiny_llm_b200 import BatchingKvCache, ContinuousBatcher, Qwen3ModelWeek3
-from tiny_llm_b200.engine import DecodeEngine
+from tiny_llm_b200.engine import DecodeEngine, PrefillEngine
 from tiny_llm_b200.synthetic import synthetic_qwen3
 
 pytestmark = pytest.mark.gpu
@@ -278,6 +278,20 @@ def test_graph_step_with_split_kv_attention_matches_operator_path(dev, tiny_gpu)
         torch.testing.assert_close(pool._value_pages[pid, :, slot].float(), ref_pool._value_pages[rid, :, slot].float(), rtol=2**-6, atol=5e-2)
         tok = int(torch.argmax(want[0, -1].float()))
         offset += 1
+
+
+def test_engines_of_one_model_share_one_packed_weight_copy(dev, tiny_gpu):
+    """Decode engines on both sides of the 8-row split and a prefill engine use the model's one packed copy of the
+    fused q|k|v and gate|up weights; an engine without the fused path builds none."""
+    model = Qwen3ModelWeek3(tiny_gpu, page_size=64)
+    DecodeEngine(model, 1, 256, dev, fused=False)
+    assert model._packed_layers is None
+    engines = [DecodeEngine(model, 1, 256, dev), DecodeEngine(model, 16, 256, dev), PrefillEngine(model, 32, 256, dev)]
+    for layer in range(model.num_hidden_layers):
+        for name in ("qkv", "gate_up"):
+            for field in ("weight", "scales", "biases"):
+                ptrs = {getattr(getattr(e._packed[layer], name), field).data_ptr() for e in engines}
+                assert len(ptrs) == 1, f"layer {layer} {name}.{field}: one copy per engine"
 
 
 def test_device_resident_greedy_loop_equals_host_driven_loop(dev, tiny_gpu):

@@ -86,6 +86,22 @@ def test_week3_defaults_and_pool_sharing(tiny, cpu_ext):
         assert a[layer].page_ids == a[0].page_ids and a[layer].page_lens == a[0].page_lens
 
 
+def test_packed_layers_are_built_once_per_model(cpu_ext):
+    """The graph engines' fused q|k|v and gate|up weights: one copy per model, asked for by every engine."""
+    model = Qwen3ModelWeek3(synthetic_qwen3("tiny-d128", seed=0, realistic=True, max_position_embeddings=512), page_size=64)
+    packed = model.packed_layers()
+    assert model.packed_layers() is packed and len(packed) == model.num_hidden_layers
+    as_i32 = lambda w: w.view(torch.int32) if w.dtype == torch.uint32 else w
+    for block, pk in zip(model.layers_inner, packed, strict=True):
+        at, mlp = block.self_attn, block.mlp
+        assert torch.equal(pk.qkv.weight, torch.cat([as_i32(at.wq.weight), as_i32(at.wk.weight), as_i32(at.wv.weight)]))
+        for field in ("scales", "biases"):
+            assert torch.equal(getattr(pk.qkv, field), torch.cat([getattr(w, field) for w in (at.wq, at.wk, at.wv)]))
+        assert torch.equal(pk.gate_up.weight, cpu_ext.interleave_gate_up(as_i32(mlp.w_gate.weight), as_i32(mlp.w_up.weight)))
+        for field in ("scales", "biases"):
+            assert torch.equal(getattr(pk.gate_up, field), cpu_ext.interleave_gate_up(getattr(mlp.w_gate, field), getattr(mlp.w_up, field)))
+
+
 def test_week2_offset_mismatch_and_logits_to_keep(tiny, cpu_ext):
     model = Qwen3ModelWeek2(tiny)
     cache = model.create_kv_cache()

@@ -67,6 +67,127 @@ def _interleave_gate_up(gate, up):
     )
 
 
+def pack_layers(model) -> list:
+    """Per layer, the weights of the fused launches: q|k|v and gate|up share their input, so they stream as one launch
+    each.  ``Qwen3ModelWeek3.packed_layers`` keeps one such copy per model for all of its engines."""
+    return [SimpleNamespace(qkv=_concat_weights([b.self_attn.wq, b.self_attn.wk, b.self_attn.wv]),
+                            gate_up=_interleave_gate_up(b.mlp.w_gate, b.mlp.w_up))
+            for b in model.layers_inner]
+
+
+def _normed(h, norm):
+    return ext.rms_norm(h, norm._weight_as(h.dtype, h.device), norm.eps)
+
+
+def _proj(h, w):
+    return ext.quantized_matmul(w.scales, w.biases, w.group_size, w.bits, h, w.weight, True)
+
+
+def _swap_ab_layers(model, x, attention):
+    """The layer stack for 9 to 128 rows ``x`` (decode slots or prefill tokens); returns the final hidden rows, already
+    normalised.  The projections run on the swap-AB wgmma kernel (w4a16_skinny.cu: weights streamed once for all rows),
+    which has no prologue, so the first RMSNorm is its own (tiny) launch; after that the residual projections (o, down)
+    hand the NEXT RMSNorm's output back together with the residual stream (one launch: the kernel that adds the
+    split-reduction planes has the whole row in registers).  The rounding points are those of the operator sequence.
+    ``attention(i, block, h)`` runs layer ``i``'s q|k|v projection and attention on the normalised rows ``h`` and
+    returns ``[rows, Hq * D]``."""
+    layers = list(model.layers_inner)
+    packed = model.packed_layers()
+    h = _normed(x, layers[0].input_layernorm)
+    for i, block in enumerate(layers):
+        wo, wd, gate_up = block.self_attn.wo, block.mlp.w_down, packed[i].gate_up
+        ln2 = block.post_attention_layernorm
+        y = attention(i, block, h)
+        x, h = ext.quantized_matmul_residual_norm(wo.scales, wo.biases, wo.weight, y, x, ln2._weight_as(x.dtype, x.device), ln2.eps)
+        act = ext.quantized_matmul_fused(gate_up.scales, gate_up.biases, gate_up.weight, h, epilogue=ext.EPI_SWIGLU_PAIRS)
+        nxt = layers[i + 1].input_layernorm if i + 1 < len(layers) else model.norm
+        x, h = ext.quantized_matmul_residual_norm(wd.scales, wd.biases, wd.weight, act, x, nxt._weight_as(x.dtype, x.device), nxt.eps)
+    return h
+
+
+class _GraphEngine:
+    """What the decode and prefill engines share: the geometry, one pinned int32 metadata block with its device mirror
+    (each engine lays it out as ``header | block tables`` and initialises the tables to -1), the event that keeps the
+    pinned block from being rewritten while its upload is still in flight, and graph capture on a side stream.
+
+    Page slabs must not move while a graph is alive, so the graphs are re-captured when a pool's slab version changes.
+    The warm-up passes of every capture really run: with the previous step's metadata still on the device they would
+    append a stale token's K/V through a stale block table - possibly into a page that has been released and handed to
+    another request since (slabs move when a second engine reserves more pages).  So ``_capture`` first sets the device
+    metadata to all-idle (``_set_idle``: nothing is appended, attention sees no keys); every replay uploads the real
+    block first."""
+
+    def __init__(self, model, max_seq_len: int, device, header_len: int, table_rows: int):
+        self.model = model
+        self.device = torch.device(device)
+        self.page_size = model.page_size
+        self.max_pages = (max_seq_len + self.page_size - 1) // self.page_size
+        self.max_seq_len = self.max_pages * self.page_size
+        self.n_layers = model.num_hidden_layers
+        attn = model.layers_inner[0].self_attn
+        self.Hq, self.Hkv, self.D = attn.num_heads, attn.num_kv_heads, attn.head_dim
+        # tables: [layers, table_rows, max_pages]
+        self._meta_len = header_len + self.n_layers * table_rows * self.max_pages
+        self.meta_host = torch.empty(self._meta_len, dtype=torch.int32, pin_memory=True)
+        self.meta_np = self.meta_host.numpy()
+        self.meta_np[:header_len] = 0
+        self.meta_np[header_len:] = -1
+        self.meta_dev = self.meta_host.to(self.device, copy=True)
+        self._upload_event = torch.cuda.Event()
+        self._upload_pending = False
+        self._stream = torch.cuda.Stream(device=self.device)
+        self._graph = None
+        self._slab_ptrs = None
+        self.captures = 0  # graph (re-)captures: 1 + one per move of the page slabs
+        self.logits = None
+
+    def reserve_pools(self, pages_per_layer: int) -> None:
+        for pool in self.model.page_pools:
+            pool.reserve(pages_per_layer, self.Hkv, self.D, dtype=torch.bfloat16, device=self.device)
+
+    def _slabs(self):
+        return tuple(p.slab_version for p in self.model.page_pools)  # changes whenever a pool's slabs are (re)allocated
+
+    def _ensure_graph(self) -> None:
+        if self._graph is None or self._slab_ptrs != self._slabs():
+            self._capture()
+
+    def _capture(self) -> None:
+        self.captures += 1
+        self._slab_ptrs = self._slabs()
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self._capture_graphs()
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _graph_of(self, body, pool=None, warmups: int = 2) -> torch.cuda.CUDAGraph:
+        """Run ``body`` ``warmups`` times (lazy kernel attribute setup must not happen under capture), then capture it
+        on the side stream, into ``pool`` if given.  ``self._launches`` is the number of library launches captured."""
+        for _ in range(warmups):
+            body()
+        self._stream.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        launched = ext.launch_count()
+        with torch.cuda.graph(graph, stream=self._stream, pool=pool):
+            body()
+        self._launches = ext.launch_count() - launched
+        return graph
+
+    def _host_write_begin(self) -> None:
+        """The pinned block is about to be rewritten: the previous upload must have been consumed
+        (a caller that keeps sampling on the device never synchronises between steps)."""
+        if self._upload_pending:
+            self._upload_event.synchronize()
+            self._upload_pending = False
+
+    def _upload_meta(self, dev, host) -> None:
+        """Copy the pinned block (or a prefix of it) to its device mirror on the current stream."""
+        dev.copy_(host, non_blocking=True)
+        self._upload_event.record()
+        self._upload_pending = True
+
+
 class _LockstepGroup:
     """The per-layer cache objects of ONE request plus the number of one-token appends the engine
     has accounted for but not yet written into them (see ``TinyKvPagedCache._lazy``)."""
@@ -98,66 +219,38 @@ class _SlotRecord:
         self.pages = len(c0.page_ids)
 
 
-class DecodeEngine:
+class DecodeEngine(_GraphEngine):
+    """One decode step of ``B`` slots as a CUDA graph (module docstring).  Metadata block:
+    ``tokens [B] | offsets [B] | context_lens [B] | block tables [Ly, B, MP]``.  The fused path uses the model's one
+    packed weight copy (``Qwen3ModelWeek3.packed_layers``); B > 8 runs the layer stack shared with the prefill engine
+    (``_swap_ab_layers``)."""
+
     def __init__(self, model, batch_size: int, max_seq_len: int, device, log_capacity: int = 4096, fused: bool = True, *,
                  _row_variants: bool = True):
-        self.model = model
-        self.B = batch_size
-        self.device = torch.device(device)
-        self.page_size = model.page_size
-        self.max_pages = (max_seq_len + self.page_size - 1) // self.page_size
-        self.max_seq_len = self.max_pages * self.page_size
-        self.n_layers = model.num_hidden_layers
-        attn = model.layers_inner[0].self_attn
-        self.Hq, self.Hkv, self.D = attn.num_heads, attn.num_kv_heads, attn.head_dim
+        B = self.B = batch_size
+        super().__init__(model, max_seq_len, device, 3 * B, B)
         self.V = model.vocab_size
         self.log_capacity = log_capacity
-
-        B, Ly, MP = self.B, self.n_layers, self.max_pages
-        # one int32 block: tokens | offsets | context_lens | block tables [Ly, B, MP]
-        self._meta_len = 3 * B + Ly * B * MP
-        self.meta_host = torch.empty(self._meta_len, dtype=torch.int32, pin_memory=True)
-        self.meta_np = self.meta_host.numpy()
-        self.meta_np[: 3 * B] = 0
-        self.meta_np[3 * B :] = -1
-        self.meta_dev = torch.zeros(self._meta_len, dtype=torch.int32, device=self.device)
         self._meta_dev_head, self._meta_host_head = self.meta_dev[: 3 * B], self.meta_host[: 3 * B]  # the per-step upload
         self.tokens = self.meta_dev[0:B]
         self.offsets = self.meta_dev[B : 2 * B]
         self.context_lens = self.meta_dev[2 * B : 3 * B]
-        self.tables = self.meta_dev[3 * B :].view(Ly, B, MP)
-        self.tables_np = self.meta_np[3 * B :].reshape(Ly, B, MP)
+        self.tables = self.meta_dev[3 * B :].view(self.n_layers, B, self.max_pages)
+        self.tables_np = self.meta_np[3 * B :].reshape(self.n_layers, B, self.max_pages)
         self.next_tokens = torch.zeros(B, dtype=torch.int32, device=self.device)
         self.out_log = torch.full((log_capacity * B,), -1, dtype=torch.int32, device=self.device)
         self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self.logits = None
         # per slot: the request group (its per-layer cache objects) the table rows reflect
         self._recs: list[_SlotRecord | None] = [None] * B
         self._tables_dirty = True
-        self._upload_event = torch.cuda.Event()
-        self._upload_pending = False
         self.h2d_bytes = 0  # bytes copied host -> device by step() / decode_on_device() so far
-        self._graph = None
         self._graph_loop = None
-        self._slab_ptrs = None
-        self._stream = torch.cuda.Stream(device=self.device)
         self.graph_replays = 0
-        self.captures = 0  # graph (re-)captures: 1 + one per move of the page slabs
         self.kernels_per_step = 0
-        rope = attn.rope
-        self.fused = bool(fused) and not rope.traditional and rope.dims == self.D and self.D % 2 == 0
-        self._packed = None
-        if self.fused:
-            # q|k|v and gate|up share their input, so they stream as one launch each.
-            self._packed = [
-                SimpleNamespace(
-                    qkv=_concat_weights([b.self_attn.wq, b.self_attn.wk, b.self_attn.wv]),
-                    gate_up=_interleave_gate_up(b.mlp.w_gate, b.mlp.w_up),
-                )
-                for b in model.layers_inner
-            ]
-        # one-launch attention (q/k norm + rope + append + paged GQA) when the head layout allows it
         attn0 = model.layers_inner[0].self_attn
+        self.fused = bool(fused) and not attn0.rope.traditional and attn0.rope.dims == self.D and self.D % 2 == 0
+        self._packed = model.packed_layers() if self.fused else None
+        # one-launch attention (q/k norm + rope + append + paged GQA) when the head layout allows it
         # The one-launch attention is a latency design (few CTAs, K/V rows staged per lane): it wins while the
         # step is launch-bound.  With many slots or long contexts the K/V stream dominates and the step uses
         # q/k norm + rope + append as one small launch followed by tl_paged_attention, whose long-context path
@@ -180,14 +273,8 @@ class DecodeEngine:
         self._graphs: dict = {}
         self.variant_replays = {r: 0 for r in self._variants}
 
-    # ------------------------------------------------------------------ pools --
     def reserve_pools(self, pages_per_layer: int | None = None) -> None:
-        pages = pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1
-        for pool in self.model.page_pools:
-            pool.reserve(pages, self.Hkv, self.D, dtype=torch.bfloat16, device=self.device)
-
-    def _slabs(self):
-        return tuple(p.slab_version for p in self.model.page_pools)  # changes whenever a pool's slabs are (re)allocated
+        super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
 
     # ------------------------------------------------------------ graph body --
     def _forward_unfused(self) -> None:
@@ -198,16 +285,13 @@ class DecodeEngine:
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens, emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits)  # [B, H]
 
-        def proj(h, w):
-            return ext.quantized_matmul(w.scales, w.biases, w.group_size, w.bits, h, w.weight, True)
-
         for i, block in enumerate(m.layers_inner):
             at = block.self_attn
             pool = m.page_pools[i]
-            h = ext.rms_norm(x, block.input_layernorm._weight_as(x.dtype, x.device), block.input_layernorm.eps)
-            q = proj(h, at.wq).view(B, 1, Hq, D)
-            k = proj(h, at.wk).view(B, 1, Hkv, D)
-            v = proj(h, at.wv).view(B, Hkv, 1, D)
+            h = _normed(x, block.input_layernorm)
+            q = _proj(h, at.wq).view(B, 1, Hq, D)
+            k = _proj(h, at.wk).view(B, 1, Hkv, D)
+            v = _proj(h, at.wv).view(B, Hkv, 1, D)
             q = ext.rms_norm(q, at.q_norm._weight_as(x.dtype, x.device), at.q_norm.eps)
             k = ext.rms_norm(k, at.k_norm._weight_as(x.dtype, x.device), at.k_norm.eps)
             q = ext.rope(q, self.offsets, at.rope.dims, at.rope.base, at.rope.traditional)
@@ -215,13 +299,13 @@ class DecodeEngine:
             ext.paged_cache_append_decode(pool._key_pages, pool._value_pages, k.view(B, Hkv, 1, D), v, self.tables[i], self.context_lens)
             y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
-            x = ext.add(x, proj(y.view(B, Hq * D), at.wo))
-            h = ext.rms_norm(x, block.post_attention_layernorm._weight_as(x.dtype, x.device), block.post_attention_layernorm.eps)
+            x = ext.add(x, _proj(y.view(B, Hq * D), at.wo))
+            h = _normed(x, block.post_attention_layernorm)
             mlp = block.mlp
-            x = ext.add(x, proj(ext.swiglu(proj(h, mlp.w_gate), proj(h, mlp.w_up)), mlp.w_down))
-        x = ext.rms_norm(x, m.norm._weight_as(x.dtype, x.device), m.norm.eps)
+            x = ext.add(x, _proj(ext.swiglu(_proj(h, mlp.w_gate), _proj(h, mlp.w_up)), mlp.w_down))
+        x = _normed(x, m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
-        logits = proj(x, head)
+        logits = _proj(x, head)
         self.next_tokens.copy_(ext.argmax(logits))
         if self.logits is None:
             self.logits = torch.empty_like(logits)
@@ -236,113 +320,90 @@ class DecodeEngine:
         R = self.B if rows is None else rows
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens[:R], emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits)
-        logits = self._forward_fused_layers(x, R)
+        head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
+        if self.B > 8:
+            h = _swap_ab_layers(m, x, self._swap_ab_attention(R))
+            logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, h)
+        else:
+            x = self._matvec_layers(x)
+            logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
+                                                prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
         self.next_tokens[:R].copy_(ext.argmax(logits))
         if self.logits is None:
             self.logits = torch.zeros((self.B, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
 
-    def _forward_fused_layers(self, x, R: int | None = None):
+    def _swap_ab_attention(self, R: int):
+        """The attention of ``_swap_ab_layers`` for the first ``R`` slots."""
+        m, Hq, Hkv, D = self.model, self.Hq, self.Hkv, self.D
+        offsets, context_lens = self.offsets[:R], self.context_lens[:R]
+
+        def attention(i, block, h):
+            at, pk, pool = block.self_attn, self._packed[i], m.page_pools[i]
+            if self._attention_fused:
+                qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h)
+                return ext.decode_attention_fused(qkv, at.q_norm._weight_as(h.dtype, h.device), at.k_norm._weight_as(h.dtype, h.device),
+                                                  offsets, self.tables[i][:R], context_lens, self._rope_inv_freq,
+                                                  pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
+                                                  self.max_seq_len, workspace=self._attn_ws)
+            # projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel, q|k|v is never written
+            q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
+                                            at.k_norm._weight_as(h.dtype, h.device), offsets, self.tables[i][:R], context_lens,
+                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps)
+            y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
+                                    at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
+            return y.view(R, Hq * D)
+
+        return attention
+
+    def _matvec_layers(self, x):
+        """The layer stack for at most 8 slots on the streaming matvec kernel, with RMSNorm as its prologue and the
+        residual add as its epilogue; returns the residual stream before the final norm."""
         m = self.model
-        B, Hq, Hkv, D = (self.B if R is None else R), self.Hq, self.Hkv, self.D
-        offsets, context_lens = self.offsets[:B], self.context_lens[:B]
-        # More than 8 rows: the projections run on the swap-AB wgmma kernel (w4a16_skinny.cu: weights streamed once
-        # for all rows), which has no prologue, so RMSNorm is its own (tiny) launch; the rounding points are the same.
-        wide = self.B > 8
-
-        def normed(h, norm):
-            return ext.rms_norm(h, norm._weight_as(h.dtype, h.device), norm.eps)
-
-        layers = list(m.layers_inner)
-        # wide path: the residual projections (o, down) hand the NEXT RMSNorm's output back together with the residual
-        # stream (one launch: the kernel that adds the split-reduction planes has the whole row in registers)
-        h = normed(x, layers[0].input_layernorm) if wide else None
-        for i, block in enumerate(layers):
+        B, Hq, Hkv, D = self.B, self.Hq, self.Hkv, self.D
+        for i, block in enumerate(m.layers_inner):
             at, pk, pool = block.self_attn, self._packed[i], m.page_pools[i]
             ln1, ln2 = block.input_layernorm, block.post_attention_layernorm
-            qkv = None
-            if wide and self._attention_fused:
-                qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h)
-            elif not wide:
-                qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, x, ln1._weight_as(x.dtype, x.device),
-                                                 prologue=ext.PRO_RMSNORM, eps=ln1.eps)
+            qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, x, ln1._weight_as(x.dtype, x.device),
+                                             prologue=ext.PRO_RMSNORM, eps=ln1.eps)
             if self._attention_fused:
                 y = ext.decode_attention_fused(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
-                                               offsets, self.tables[i][:B], context_lens, self._rope_inv_freq,
+                                               self.offsets, self.tables[i], self.context_lens, self._rope_inv_freq,
                                                pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
                                                self.max_seq_len, workspace=self._attn_ws)
             else:
-                if wide:  # projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel, q|k|v is never written
-                    q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(x.dtype, x.device),
-                                                    at.k_norm._weight_as(x.dtype, x.device), offsets, self.tables[i][:B], context_lens,
-                                                    pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps)
-                else:
-                    q = ext.decode_qk_norm_rope_append(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
-                                                       offsets, self.tables[i][:B], context_lens, pool._key_pages, pool._value_pages,
-                                                       Hq, Hkv, at.rope.base, at.q_norm.eps)
-                y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:B], context_lens,
+                q = ext.decode_qk_norm_rope_append(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
+                                                   self.offsets, self.tables[i], self.context_lens, pool._key_pages, pool._value_pages,
+                                                   Hq, Hkv, at.rope.base, at.q_norm.eps)
+                y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
                                         at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             wd = block.mlp.w_down
-            if wide:
-                x, h = ext.quantized_matmul_residual_norm(at.wo.scales, at.wo.biases, at.wo.weight, y.view(B, Hq * D), x,
-                                                          ln2._weight_as(x.dtype, x.device), ln2.eps)
-                act = ext.quantized_matmul_fused(pk.gate_up.scales, pk.gate_up.biases, pk.gate_up.weight, h, epilogue=ext.EPI_SWIGLU_PAIRS)
-                nxt = layers[i + 1].input_layernorm if i + 1 < len(layers) else m.norm
-                x, h = ext.quantized_matmul_residual_norm(wd.scales, wd.biases, wd.weight, act, x, nxt._weight_as(x.dtype, x.device), nxt.eps)
-                continue
             x = ext.quantized_matmul_fused(at.wo.scales, at.wo.biases, at.wo.weight, y.view(B, Hq * D), residual=x, epilogue=ext.EPI_RESIDUAL)
             act = ext.quantized_matmul_fused(pk.gate_up.scales, pk.gate_up.biases, pk.gate_up.weight, x, ln2._weight_as(x.dtype, x.device),
                                              prologue=ext.PRO_RMSNORM, eps=ln2.eps, epilogue=ext.EPI_SWIGLU_PAIRS)  # [B, inter]
             x = ext.quantized_matmul_fused(wd.scales, wd.biases, wd.weight, act, residual=x, epilogue=ext.EPI_RESIDUAL)
-        head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
-        if wide:
-            return ext.quantized_matmul_fused(head.scales, head.biases, head.weight, h)
-        return ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
-                                          prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
+        return x
 
-    def _capture(self) -> None:
-        self.captures += 1
-        self._slab_ptrs = self._slabs()
+    def _set_idle(self) -> None:
+        self.meta_dev[2 * self.B : 3 * self.B].zero_()  # context_lens
+        self.meta_dev[3 * self.B :].fill_(-1)
+        self._tables_dirty = True
+
+    def _capture_graphs(self) -> None:
         forward = self._forward_fused if self.fused else self._forward_unfused
-        with torch.cuda.stream(self._stream):
-            self._stream.wait_stream(torch.cuda.current_stream(self.device))
-            # The warm-up passes really run: with the previous step's metadata still on the device they
-            # would append a stale token's K/V through a stale block table - possibly into a page that
-            # has been released and handed to another request since (slabs move when a second engine
-            # reserves more pages).  All slots idle: appends are skipped and attention returns zeros;
-            # step() / decode_on_device() upload the real block before they replay.
-            self.meta_dev[2 * self.B : 3 * self.B].zero_()
-            self.meta_dev[3 * self.B :].fill_(-1)
-            self._tables_dirty = True
-            for _ in range(2):  # warm-up: lazy kernel attribute setup must not happen under capture
-                forward()
-            self._stream.synchronize()
-            self._graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self._graph, stream=self._stream):
-                forward()
-            self._graph_loop = torch.cuda.CUDAGraph()
-            launched = ext.launch_count()
-            with torch.cuda.graph(self._graph_loop, stream=self._stream, pool=self._graph.pool()):
-                forward()
-                ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
-            # kernels of libtiny_llm_b200.so recorded into one self-advancing step
-            self.kernels_per_step = ext.launch_count() - launched
-            self._graphs = {self.B: self._graph}
-            for rows in self._variants:
-                if rows == self.B:
-                    continue
-                for _ in range(2):  # warm-up (metadata still all-idle): the narrower kernels set their attributes lazily
-                    forward(rows)
-                self._stream.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self._stream, pool=self._graph.pool()):
-                    forward(rows)
-                self._graphs[rows] = g
-        torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
-    def _ensure_graph(self) -> None:
-        if self._graph is None or self._slab_ptrs != self._slabs():
-            self._capture()
+        def self_advancing_step():
+            forward()
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        self._graph = self._graph_of(forward)
+        # the same step (already warmed up) with token feedback and position advance, for decode_on_device
+        self._graph_loop = self._graph_of(self_advancing_step, pool=self._graph.pool(), warmups=0)
+        self.kernels_per_step = self._launches  # kernels of libtiny_llm_b200.so recorded into one self-advancing step
+        self._graphs = {self.B: self._graph}
+        for rows in self._variants:
+            if rows != self.B:  # the warm-ups run with the metadata still all-idle: the narrower kernels set their attributes lazily
+                self._graphs[rows] = self._graph_of(lambda: forward(rows), pool=self._graph.pool())
 
     # ------------------------------------------------------- host bookkeeping --
     def _slot_caches(self, caches, layer: int):
@@ -472,24 +533,14 @@ class DecodeEngine:
         rec.pages = len(group_caches[0].page_ids)
         self._tables_dirty = True
 
-    def _host_write_begin(self) -> None:
-        """The pinned block is about to be rewritten: the previous upload must have been consumed
-        (a caller that keeps sampling on the device never synchronises between steps)."""
-        if self._upload_pending:
-            self._upload_event.synchronize()
-            self._upload_pending = False
-
     def _upload(self) -> None:
-        B = self.B
         if self._tables_dirty:
-            self.meta_dev.copy_(self.meta_host, non_blocking=True)
+            self._upload_meta(self.meta_dev, self.meta_host)
             self.h2d_bytes += self._meta_len * 4
             self._tables_dirty = False
         else:  # tokens | offsets | context_lens only: the block tables on the device are current
-            self._meta_dev_head.copy_(self._meta_host_head, non_blocking=True)
-            self.h2d_bytes += 3 * B * 4
-        self._upload_event.record()
-        self._upload_pending = True
+            self._upload_meta(self._meta_dev_head, self._meta_host_head)
+            self.h2d_bytes += 3 * self.B * 4
 
     def upload_bytes_per_step(self) -> int:
         """Host -> device bytes of a steady-state step (block tables travel only when a page was added)."""
@@ -552,7 +603,7 @@ class DecodeEngine:
         return self.out_log[: steps * B].view(steps, B)
 
 
-class PrefillEngine:
+class PrefillEngine(_GraphEngine):
     """CUDA-graph replay of ONE chunked-prefill step (``Request.try_prefill``: B = 1, up to ``chunk`` prompt tokens,
     ``src/tiny_llm_ref/batch.py:48-76``) for the Week-3 paged model.
 
@@ -567,46 +618,24 @@ class PrefillEngine:
     Per layer: rms_norm -> q|k|v projection (one launch) -> q/k norm + RoPE + K/V append for all rows (one
     launch, ``tl_chunk_qk_norm_rope_append``) -> paged FlashAttention (wgmma) -> o projection + residual ->
     rms_norm -> gate|up (+ SwiGLU) -> down + residual.  Rounding points are those of the operator sequence.
+    Chunks of up to 128 tokens run the layer stack the wide decode step uses (``_swap_ab_layers``), with the
+    model's one packed weight copy (``Qwen3ModelWeek3.packed_layers``).
     Integer page bookkeeping stays in the request's ``TinyKvPagedCache`` objects (``append_slots``)."""
 
     def __init__(self, model, chunk: int, max_seq_len: int, device):
-        self.model, self.L, self.device = model, int(chunk), torch.device(device)
-        self.page_size = model.page_size
-        self.max_pages = (max_seq_len + self.page_size - 1) // self.page_size
-        self.max_seq_len = self.max_pages * self.page_size
-        attn = model.layers_inner[0].self_attn
-        self.Hq, self.Hkv, self.D = attn.num_heads, attn.num_kv_heads, attn.head_dim
-        self.n_layers = model.num_hidden_layers
-        L, Ly, MP = self.L, self.n_layers, self.max_pages
+        L = self.L = int(chunk)
         # one int32 block: tokens [L] | offsets [L] | context_lens [L] | ctx_after [1] | tables [Ly, MP]
-        self._meta_len = 3 * L + 1 + Ly * MP
-        self.meta_host = torch.empty(self._meta_len, dtype=torch.int32, pin_memory=True)
-        self.meta_np = self.meta_host.numpy()
-        self.meta_np[:] = 0
-        self.meta_np[3 * L + 1:] = -1
-        self.meta_dev = torch.zeros(self._meta_len, dtype=torch.int32, device=self.device)
-        self.meta_dev[3 * L + 1:] = -1
+        super().__init__(model, max_seq_len, device, 3 * L + 1, 1)
         self.tokens = self.meta_dev[0:L].view(1, L)
         self.offsets = self.meta_dev[L:2 * L]
         self.ctxs = self.meta_dev[2 * L:3 * L]
         self.ctx_after = self.meta_dev[3 * L:3 * L + 1]
-        self.tables = self.meta_dev[3 * L + 1:].view(Ly, MP)
-        self.tables_np = self.meta_np[3 * L + 1:].reshape(Ly, MP)
-        self.logits = None
+        self.tables = self.meta_dev[3 * L + 1:].view(self.n_layers, self.max_pages)
+        self.tables_np = self.meta_np[3 * L + 1:].reshape(self.n_layers, self.max_pages)
         self.next_token = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self._graph = None
-        self._slab_ptrs = None
-        self._stream = torch.cuda.Stream(device=self.device)
-        self._upload_event = torch.cuda.Event()
-        self._upload_pending = False
         self.replays = 0
-        self.captures = 0
         self.kernels_per_chunk = 0
-        self._packed = [
-            SimpleNamespace(qkv=_concat_weights([b.self_attn.wq, b.self_attn.wk, b.self_attn.wv]),
-                            gate_up=_interleave_gate_up(b.mlp.w_gate, b.mlp.w_up))
-            for b in model.layers_inner
-        ]
+        self._packed = model.packed_layers()
 
     @staticmethod
     def supported(model, device) -> bool:
@@ -616,80 +645,51 @@ class PrefillEngine:
                 and model.embedding.weight.scales.dtype == torch.bfloat16 and model.page_size % 64 == 0
                 and 128 % (attn.num_heads // attn.num_kv_heads) == 0)
 
-    def _slabs(self):
-        return tuple(p.slab_version for p in self.model.page_pools)  # changes whenever a pool's slabs are (re)allocated
+    def _attention(self, i, block, h):
+        """Layer ``i``'s q|k|v projection, q/k norm + RoPE + K/V append and paged FlashAttention for the chunk's rows
+        -> ``[L, Hq * D]`` (the wgmma kernel writes the o-projection's layout itself; else attention + one transpose copy)."""
+        at, pk, pool = block.self_attn, self._packed[i], self.model.page_pools[i]
+        Hq, Hkv = self.Hq, self.Hkv
+        if self.L <= 128:  # projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel
+            q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
+                                            at.k_norm._weight_as(h.dtype, h.device), self.offsets, self.tables[i], self.ctxs,
+                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, chunk=True)  # [Hq, L, D]
+        else:
+            q = ext.chunk_qk_norm_rope_append(_proj(h, pk.qkv), at.q_norm._weight_as(h.dtype, h.device), at.k_norm._weight_as(h.dtype, h.device),
+                                              self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
+                                              Hq, Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
+        return ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
+                                               True, Hkv, Hq)
 
     def _forward(self) -> None:
         m, L = self.model, self.L
-        Hq, Hkv, D = self.Hq, self.Hkv, self.D
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens, emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits).view(L, -1)
-        skinny = L <= 128  # the fused epilogues live in the <= 128-row tensor-core kernel; longer chunks use the 128 x 128-tile GEMM
-
-        def normed(h, norm):
-            return ext.rms_norm(h, norm._weight_as(h.dtype, h.device), norm.eps)
-
-        def proj(h, w):
-            return ext.quantized_matmul(w.scales, w.biases, w.group_size, w.bits, h, w.weight, True)
-
-        layers = list(m.layers_inner)
-        h = normed(x, layers[0].input_layernorm) if skinny else None
-        for i, block in enumerate(layers):
-            at, pk, pool = block.self_attn, self._packed[i], m.page_pools[i]
-            if not skinny:
-                h = normed(x, block.input_layernorm)
-            if skinny:  # q|k|v projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel
-                q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(x.dtype, x.device),
-                                                at.k_norm._weight_as(x.dtype, x.device), self.offsets, self.tables[i], self.ctxs,
-                                                pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, chunk=True)  # [Hq, L, D]
-            else:
-                q = ext.chunk_qk_norm_rope_append(proj(h, pk.qkv), at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
-                                                  self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
-                                                  Hq, Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
-            # [L, Hq * D]: the wgmma kernel writes the o-projection's layout itself (else: attention + one transpose copy)
-            y = ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
-                                                True, Hkv, Hq)
-            if skinny:  # the residual projections return the next RMSNorm's output too (DecodeEngine._forward_fused_layers)
-                ln2, wd = block.post_attention_layernorm, block.mlp.w_down
-                x, h = ext.quantized_matmul_residual_norm(at.wo.scales, at.wo.biases, at.wo.weight, y, x, ln2._weight_as(x.dtype, x.device), ln2.eps)
-                act = ext.quantized_matmul_fused(pk.gate_up.scales, pk.gate_up.biases, pk.gate_up.weight, h, epilogue=ext.EPI_SWIGLU_PAIRS)
-                nxt = layers[i + 1].input_layernorm if i + 1 < len(layers) else m.norm
-                x, h = ext.quantized_matmul_residual_norm(wd.scales, wd.biases, wd.weight, act, x, nxt._weight_as(x.dtype, x.device), nxt.eps)
-            else:
-                x = ext.add(x, proj(y, at.wo))
-                h = normed(x, block.post_attention_layernorm)
-                x = ext.add(x, proj(ext.swiglu(proj(h, block.mlp.w_gate), proj(h, block.mlp.w_up)), block.mlp.w_down))
         # logits_to_keep = 1: the hidden state is sliced before the final norm (qwen3_week3.py:330-338); RMSNorm is row-wise,
         # so the last row of the already normalised chunk is the same thing
-        last = h[L - 1:L] if skinny else normed(x[L - 1:L], m.norm)
+        if L <= 128:  # the fused epilogues live in the <= 128-row tensor-core kernel; longer chunks use the 128 x 128-tile GEMM
+            last = _swap_ab_layers(m, x, self._attention)[L - 1:L]
+        else:
+            for i, block in enumerate(m.layers_inner):
+                h = _normed(x, block.input_layernorm)
+                x = ext.add(x, _proj(self._attention(i, block, h), block.self_attn.wo))
+                h = _normed(x, block.post_attention_layernorm)
+                x = ext.add(x, _proj(ext.swiglu(_proj(h, block.mlp.w_gate), _proj(h, block.mlp.w_up)), block.mlp.w_down))
+            last = _normed(x[L - 1:L], m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
-        logits = proj(last, head)
+        logits = _proj(last, head)
         self.next_token.copy_(ext.argmax(logits))
         if self.logits is None:
             self.logits = torch.empty_like(logits)
         self.logits.copy_(logits)
 
-    def _capture(self) -> None:
-        self.captures += 1
-        self._slab_ptrs = self._slabs()
-        with torch.cuda.stream(self._stream):
-            self._stream.wait_stream(torch.cuda.current_stream(self.device))
-            # warm-up passes run for real: all rows padding (context 0 -> no append), no visible keys
-            self.meta_dev[2 * self.L:3 * self.L + 1].zero_()
-            self.meta_dev[3 * self.L + 1:].fill_(-1)
-            for _ in range(2):
-                self._forward()
-            self._stream.synchronize()
-            self._graph = torch.cuda.CUDAGraph()
-            launched = ext.launch_count()
-            with torch.cuda.graph(self._graph, stream=self._stream):
-                self._forward()
-            self.kernels_per_chunk = ext.launch_count() - launched
-        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+    def _set_idle(self) -> None:
+        self.meta_dev[2 * self.L:3 * self.L + 1].zero_()  # all rows padding (context 0 -> no append), no visible keys
+        self.meta_dev[3 * self.L + 1:].fill_(-1)
 
-    def reserve_pools(self, pages_per_layer: int) -> None:
-        for pool in self.model.page_pools:
-            pool.reserve(pages_per_layer, self.Hkv, self.D, dtype=torch.bfloat16, device=self.device)
+    def _capture_graphs(self) -> None:
+        self._graph = self._graph_of(self._forward)
+        self.kernels_per_chunk = self._launches
 
     def applies(self, tokens: int, offset: int, cache) -> bool:
         if not (0 < tokens <= self.L) or offset + tokens > self.max_seq_len:
@@ -709,16 +709,13 @@ class PrefillEngine:
         caches and return (logits [1, 1, V] of the last token - a static buffer -, greedy next token [1])."""
         on_device = isinstance(token_ids, torch.Tensor)
         r, L = (int(token_ids.numel()) if on_device else len(token_ids)), self.L
-        if self._upload_pending:
-            self._upload_event.synchronize()
-            self._upload_pending = False
+        self._host_write_begin()
         for layer, layer_cache in enumerate(cache):
             layer_cache.append_slots(r)
             n = len(layer_cache.page_ids)
             self.tables_np[layer, :n] = layer_cache.page_ids
             self.tables_np[layer, n:] = -1
-        if self._graph is None or self._slab_ptrs != self._slabs():
-            self._capture()
+        self._ensure_graph()
         pad = L - r
         meta = self.meta_np
         meta[0:L] = 0
@@ -731,9 +728,7 @@ class PrefillEngine:
         cur = torch.cuda.current_stream(self.device)
         self._stream.wait_stream(cur)
         with torch.cuda.stream(self._stream):
-            self.meta_dev.copy_(self.meta_host, non_blocking=True)
-            self._upload_event.record()
-            self._upload_pending = True
+            self._upload_meta(self.meta_dev, self.meta_host)
             if on_device:  # ids stay on the device: no host round trip for the prompt
                 self.meta_dev[pad:L].copy_(token_ids.reshape(-1).to(torch.int32), non_blocking=True)
             self._graph.replay()
