@@ -74,6 +74,20 @@ long long tl_launch_count(void);
  * no initialisation needed). */
 #define TL_MATVEC_REF_ROWS 8
 #define TL_MATVEC_MAX_ROWS 32
+/* The kernel a W4A16 projection runs (nothing is launched or read; the pointers only count for their alignment):
+ * TL_W4_VANILLA / TL_W4_STREAM / TL_W4_SKINNY / TL_W4_TILES as selected above, or a negative TL_E* code for arguments
+ * the launch rejects (a or b not 16-byte aligned on the wgmma paths, misaligned operands or too wide a row on the
+ * streaming kernel).  `fused` selects the rule of tl_quantized_matmul_fused / tl_quantized_matmul_residual_norm (which
+ * keep M > 128 on the streaming kernel and take a prologue and a row stride lda >= N); the plain call needs
+ * prologue TL_PRO_NONE and lda == N.  The facts of the chosen kernel are written, 0 where they do not apply:
+ *   *splits, *gb_per_split : SKINNY / TILES, the reduction split and the 128-wide groups per split (TILES: 1 and N/128);
+ *   *rows_per_pass, *units : STREAM, activation rows per pass (a power of two <= TL_MATVEC_MAX_ROWS: larger M runs in
+ *                            several passes) and 128-column groups per weight unit (2 when N % 256 == 0, scales and
+ *                            biases are 4-byte aligned and M <= 16; otherwise 1).
+ * The split count depends on the SM count of the current device. */
+enum { TL_W4_VANILLA = 0, TL_W4_STREAM = 1, TL_W4_SKINNY = 2, TL_W4_TILES = 3 };
+int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, const void *a, const void *b,
+                              const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass, int *units);
 size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_simdgroup, int use_split_k);
 int tl_quantized_matmul(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
                         int N, int K, int dtype, int use_simdgroup, int use_split_k, void *workspace,

@@ -198,3 +198,87 @@ def test_route_rejects_what_paged_attention_rejects():
         route(L=9, D=64)
     with pytest.raises(RuntimeError, match=r"range \[1, 128\]"):
         route(D=256, dtype=F32)
+
+
+# ---------------------------------------------------------------- W4A16 routing --
+# tl_quantized_matmul_route runs the selection of the W4A16 launches (w4a16_path(), w4a16_skinny_splits() and the
+# streaming kernel's plan) without a device.  Without a GPU the split count assumes 132 SMs (an H100 SXM).
+F16 = torch.float16
+
+
+def w4_route(M, N, K, lda=None, prologue=0, fused=False, simd=True, dtype=BF, a=A16, b=A16, scales=A16, biases=A16):
+    return ext.quantized_matmul_route(M, N, K, N if lda is None else lda, prologue, fused, simd, dtype, a, b, scales, biases)
+
+
+def test_w4_route_row_boundaries():
+    for dtype in (BF, F16):
+        assert w4_route(8, 2560, 1024, dtype=dtype)[0] == ext.W4_STREAM
+        assert w4_route(9, 2560, 1024, dtype=dtype)[0] == ext.W4_SKINNY
+        assert w4_route(128, 2560, 1024, dtype=dtype)[0] == ext.W4_SKINNY
+        assert w4_route(129, 2560, 1024, dtype=dtype) == (ext.W4_TILES, 1, 20, 0, 0)
+        assert w4_route(1, 2560, 1024, dtype=dtype, simd=False) == (ext.W4_VANILLA, 0, 0, 0, 0)
+        assert w4_route(300, 2560, 1024, dtype=dtype, simd=False)[0] == ext.W4_VANILLA
+    # the fused forms carry their epilogues only on the split-reduction launch: M > 128 stays on the streaming kernel
+    assert w4_route(128, 2560, 1024, fused=True)[0] == ext.W4_SKINNY
+    assert w4_route(129, 2560, 1024, fused=True) == (ext.W4_STREAM, 0, 0, 32, 1)
+    assert w4_route(1000, 2560, 1024, fused=True)[0] == ext.W4_STREAM
+
+
+def test_w4_route_prologue_or_row_stride_forces_the_streaming_kernel():
+    for prologue in (1, 2):
+        for M in (9, 64, 128):
+            assert w4_route(M, 2560, 1024, prologue=prologue, fused=True)[0] == ext.W4_STREAM
+    assert w4_route(64, 2560, 1024, lda=2568, fused=True)[0] == ext.W4_STREAM
+    assert w4_route(64, 2560, 1024, lda=2560, fused=True)[0] == ext.W4_SKINNY
+    with pytest.raises(RuntimeError, match="needs a fused form"):
+        w4_route(1, 2560, 1024, prologue=1)
+    with pytest.raises(RuntimeError, match="needs a fused form"):
+        w4_route(1, 2560, 1024, lda=2568)
+
+
+def test_w4_route_rejects_misaligned_operands_of_the_wgmma_kernels():
+    for M in (9, 129):
+        for where in ("a", "b"):
+            with pytest.raises(RuntimeError, match="16-byte aligned"):
+                w4_route(M, 2560, 1024, **{where: A2})
+    # the streaming kernel reads a and b with 16-byte loads too; scales and biases only need 2 bytes
+    with pytest.raises(RuntimeError, match="16-byte aligned"):
+        w4_route(1, 2560, 1024, a=A2)
+    with pytest.raises(RuntimeError, match="16-byte aligned"):
+        w4_route(4, 2560, 1024, lda=2564, fused=True)
+    assert w4_route(9, 2560, 1024, scales=A2)[0] == ext.W4_SKINNY
+    with pytest.raises(RuntimeError, match="float16 or bfloat16"):
+        w4_route(1, 2560, 1024, dtype=torch.float32)
+
+
+def test_w4_route_streaming_units():
+    # two 128-column groups per unit need an even group count, 4-byte aligned scale/bias rows and at most 16 rows
+    assert w4_route(1, 2560, 1024)[4] == 2
+    assert w4_route(16, 2560, 1024, lda=2568, fused=True)[4] == 2
+    assert w4_route(17, 2560, 1024, lda=2568, fused=True)[4] == 1
+    for N in (128, 384, 1152):
+        assert w4_route(1, N, 100)[4] == 1, N
+    assert w4_route(1, 2560, 1024, scales=A2)[4] == 1
+    assert w4_route(1, 2560, 1024, biases=A2)[4] == 1
+
+
+def test_w4_route_streaming_rows_per_pass():
+    for M, rpp in ((1, 1), (2, 2), (3, 4), (5, 8), (8, 8)):
+        assert w4_route(M, 2560, 1024)[3] == rpp, M
+    for M in (32, 33, 200):
+        assert w4_route(M, 2560, 2560, lda=2568, fused=True)[3] == 32, M
+    # a 9728-wide reduction leaves shared memory for 8 activation rows per pass: 16 rows run in two passes, 17 in three
+    for M in (8, 16, 17):
+        assert w4_route(M, 9728, 2560, prologue=2, fused=True)[3] == 8, M
+    assert w4_route(4, 9728, 2560)[3] == 4
+
+
+def test_w4_route_skinny_splits():
+    # 76 group blocks over 20 feature tiles: 6 splits of 13 on 132 SMs (an odd split length starts every second split
+    # in the second half of a two-group TMA box)
+    if not torch.cuda.is_available():
+        assert w4_route(16, 9728, 2560)[:3] == (ext.W4_SKINNY, 6, 13)
+    route, splits, gbps, rpp, units = w4_route(33, 2560, 1000)
+    assert route == ext.W4_SKINNY and splits > 1 and (splits - 1) * gbps < 20 <= splits * gbps and (rpp, units) == (0, 0)
+    # the split count is a function of (N, K) alone: every row count of one token tile gets the same split
+    assert len({w4_route(M, 2560, 9728)[1:3] for M in (9, 16, 17, 64, 65, 128)}) == 1

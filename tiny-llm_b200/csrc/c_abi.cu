@@ -329,6 +329,36 @@ int tl_argmax(const void *logits, int32_t *out_tokens, int rows, int vocab, int 
     return launch_argmax(logits, out_tokens, rows, vocab, dtype, workspace, workspace_bytes, as_stream(stream));
 }
 
+int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, const void *a, const void *b,
+                              const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass, int *units) {
+    if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    if (M < 0 || N <= 0 || K < 0 || lda < N || N % 128 != 0) return fail(TL_EINVAL, "quantized_matmul_route: bad shape");
+    if (prologue < TL_PRO_NONE || prologue > TL_PRO_SWIGLU || (!fused && (prologue != TL_PRO_NONE || lda != N)))
+        return fail(TL_EINVAL, "quantized_matmul_route: a prologue or a row stride needs a fused form");
+    int s = 0, gbps = 0, rpp = 0, u = 0;
+    const W4Path path = w4a16_path(M, N, K, dtype, use_simdgroup != 0, fused != 0, prologue, lda);
+    if (path == W4Path::SKINNY || path == W4Path::TILES) {
+        if (!aligned16(a) || !aligned16(b)) return fail(TL_EINVAL, "quantized_matmul: a and b must be 16-byte aligned");
+        if (path == W4Path::SKINNY)
+            s = w4a16_skinny_splits(M, N, K, &gbps);
+        else
+            s = 1, gbps = N / 128;
+    } else if (path == W4Path::STREAM) {
+        if (int e = w4a16_stream_plan(M, N, K, lda, a, nullptr, b, scales, biases, &rpp, &u)) return e;
+    }
+    if (splits) *splits = s;
+    if (gb_per_split) *gb_per_split = gbps;
+    if (rows_per_pass) *rows_per_pass = rpp;
+    if (units) *units = u;
+    switch (path) {
+        case W4Path::VANILLA: return TL_W4_VANILLA;
+        case W4Path::STREAM: return TL_W4_STREAM;
+        case W4Path::SKINNY: return TL_W4_SKINNY;
+        case W4Path::TILES: break;
+    }
+    return TL_W4_TILES;
+}
+
 size_t tl_quantized_matmul_fused_workspace(int M, int N, int K, int lda, int prologue, int dtype) {
     if (w4a16_path(M, N, K, dtype, true, true, prologue, lda) == W4Path::SKINNY) return w4a16_skinny_workspace(M, N, K);
     return 0;

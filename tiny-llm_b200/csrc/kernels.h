@@ -49,9 +49,13 @@ void set_use_pdl(bool on);
 bool use_pdl();
 int launch_w4a16_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
                          int N, int K, int dtype, cudaStream_t st);
+// Rows per pass and 128-column groups per unit of the streaming kernel, or TL_EINVAL for operands it cannot take.
+int w4a16_stream_plan(int M, int N, int K, int lda, const void *p0, const void *p1, const void *b, const void *scales, const void *biases,
+                      int *rows_per_pass, int *units);
 
 // w4a16_skinny.cu (swap-AB wgmma GEMM: split reduction for 9 <= M <= 128, 128-token tiles for prefill)
-int w4a16_skinny_splits(int M, int N, int K);
+// Split count of the reduction; *gb_per_split (optional) receives the 128-wide group blocks of each split.
+int w4a16_skinny_splits(int M, int N, int K, int *gb_per_split = nullptr);
 size_t w4a16_skinny_workspace(int M, int N, int K);
 // norm_w / normed (optional, residual epilogue): also write normed = rms_norm(out, norm_w, norm_eps); *norm_done tells
 // whether the launch did it (split reduction, K <= 4096) or the caller still has to run rms_norm

@@ -294,13 +294,30 @@ static int stream5_grid(int K) {
     return all < sms ? all : sms;
 }
 
+// Launch plan of the streaming kernel: rows of `a` per pass (a power of two <= TL_MATVEC_MAX_ROWS, as many as fit in
+// shared memory) and 128-column groups per unit (2 when N % 256 == 0, the scale/bias rows are 4-byte aligned and at
+// most 16 rows are streamed: 32 rows x pairs would spill).  The launch and tl_quantized_matmul_route both use it.
+int w4a16_stream_plan(int M, int N, int K, int lda, const void *p0, const void *p1, const void *b, const void *scales, const void *biases,
+                      int *rows_per_pass, int *units) {
+    if (!aligned16(p0) || !aligned16(b) || (p1 && !aligned16(p1)) || (lda % 8) != 0)
+        return fail(TL_EINVAL, "quantized_matmul: operands must be 16-byte aligned");
+    if (K >= (1 << 24)) return fail(TL_EINVAL, "quantized_matmul: more than 2^24 output features");
+    const bool pairs = (N % 256) == 0 && (reinterpret_cast<uintptr_t>(scales) & 3u) == 0 && (reinterpret_cast<uintptr_t>(biases) & 3u) == 0;
+    int rpp = w4_pad_cols(M < TL_MATVEC_MAX_ROWS ? M : TL_MATVEC_MAX_ROWS);
+    const int grid_x = stream5_grid(K);
+    while (rpp > 1 && stream5_smem_bytes(N, K, rpp, grid_x) > S5_SMEM_MAX) rpp /= 2;
+    if (stream5_smem_bytes(N, K, rpp, grid_x) > S5_SMEM_MAX)
+        return fail(TL_EINVAL, "quantized_matmul: activations do not fit in shared memory (N=%d, K=%d, rows=%d)", N, K, rpp);
+    *rows_per_pass = rpp;
+    *units = pairs && M <= 16 ? 2 : 1;
+    return TL_OK;
+}
+
 template <typename T, int MP, int U>
 static int stream5_launch(StreamArgs args, cudaStream_t st) {
     const int grid_x = stream5_grid(args.K);
     const size_t smem = stream5_smem_bytes(args.N, args.K, MP, grid_x);
     const size_t limit = S5_SMEM_MAX;
-    if (smem > limit)
-        return fail(TL_EINVAL, "quantized_matmul: activations do not fit in shared memory (N=%d, K=%d, rows=%d)", args.N, args.K, MP);
     static bool configured = false;  // per process: one device per process (DESIGN.md section 5)
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(w4a16_stream5_kernel<T, MP, U>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -326,12 +343,7 @@ static int stream5_launch(StreamArgs args, cudaStream_t st) {
 
 template <typename T, int U>
 static int stream5_u(StreamArgs args, cudaStream_t st) {
-    // rows of `a` handled per pass: as many (power of two, <= 32) as fit in shared memory
-    int rpp = w4_pad_cols(args.M < 32 ? args.M : 32);
-    const int grid_x = stream5_grid(args.K);
-    while (rpp > 1 && stream5_smem_bytes(args.N, args.K, rpp, grid_x) > S5_SMEM_MAX) rpp /= 2;
-    args.rows_per_pass = rpp;
-    switch (rpp) {
+    switch (args.rows_per_pass) {
         case 1: return stream5_launch<T, 1, U>(args, st);
         case 2: return stream5_launch<T, 2, U>(args, st);
         case 4: return stream5_launch<T, 4, U>(args, st);
@@ -343,12 +355,11 @@ static int stream5_u(StreamArgs args, cudaStream_t st) {
 
 template <typename T>
 static int stream5_t(StreamArgs args, cudaStream_t st) {
-    if (!aligned16(args.p0) || !aligned16(args.b) || (args.p1 && !aligned16(args.p1)) || (args.lda % 8) != 0)
-        return fail(TL_EINVAL, "quantized_matmul: operands must be 16-byte aligned");
-    if (args.K >= (1 << 24)) return fail(TL_EINVAL, "quantized_matmul: more than 2^24 output features");
-    const bool pairs = (args.N % 256) == 0 && (reinterpret_cast<uintptr_t>(args.scales) & 3u) == 0 &&
-                       (reinterpret_cast<uintptr_t>(args.biases) & 3u) == 0;
-    return (pairs && args.M <= 16) ? stream5_u<T, 2>(args, st) : stream5_u<T, 1>(args, st);  // 32 rows x pairs would spill
+    int units = 1;
+    if (int e = w4a16_stream_plan(args.M, args.N, args.K, args.lda, args.p0, args.p1, args.b, args.scales, args.biases, &args.rows_per_pass,
+                                  &units))
+        return e;
+    return units == 2 ? stream5_u<T, 2>(args, st) : stream5_u<T, 1>(args, st);
 }
 
 int launch_w4a16_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,

@@ -396,7 +396,7 @@ __global__ void __launch_bounds__(256) w4a16_skinny_reduce_norm_kernel(const flo
 // SM), a fixed cost per CTA worth ~10 group blocks (barrier set-up, first TMA round trips, epilogue) and ~8 for the
 // extra reduce launch.
 static int skinny_slots(int) { return sm_count(); }
-int w4a16_skinny_splits(int M, int N, int K) {
+int w4a16_skinny_splits(int M, int N, int K, int *gb_per_split) {
     const int tiles = (K + SK_FEAT - 1) / SK_FEAT;
     const int num_gb = N / SK_GB;
     const int slots = skinny_slots(M);
@@ -409,6 +409,7 @@ int w4a16_skinny_splits(int M, int N, int K) {
         const long long cost = waves * (gbps + 10) + (real > 1 ? 8 : 0);  // in units of one group block
         if (best_cost < 0 || cost < best_cost) best_cost = cost, best = real;
     }
+    if (gb_per_split != nullptr) *gb_per_split = (num_gb + best - 1) / best;
     return best;
 }
 
@@ -455,12 +456,10 @@ static int skinny_t(const void *scales, const void *biases, const void *a, const
     if (!aligned16(a) || !aligned16(b)) return fail(TL_EINVAL, "quantized_matmul: a and b must be 16-byte aligned");
     const int NT = M <= 16 ? 16 : (M <= 32 ? 32 : (M <= 64 ? 64 : 128));
     const int tiles = (K + SK_FEAT - 1) / SK_FEAT;
-    const int num_gb = N / SK_GB;
     SkArgs args{};
     args.scales = scales, args.biases = biases, args.residual = residual, args.out = out;
     args.M = M, args.N = N, args.K = K, args.epilogue = epilogue;
-    args.splits = w4a16_skinny_splits(M, N, K);
-    args.gb_per_split = (num_gb + args.splits - 1) / args.splits;
+    args.splits = w4a16_skinny_splits(M, N, K, &args.gb_per_split);
     if (args.splits > 1 && (ws == nullptr || ws_bytes < w4a16_skinny_workspace(M, N, K)))
         return fail(TL_EWORKSPACE, "quantized_matmul: workspace too small (%zu < %zu)", ws_bytes, w4a16_skinny_workspace(M, N, K));
     args.partials = static_cast<float *>(ws);

@@ -41,6 +41,7 @@ __all__ = [
     "argmax",
     "decode_advance",
     "quantized_matmul_fused",
+    "quantized_matmul_route",
     "decode_qk_norm_rope_append",
     "chunk_qk_norm_rope_append",
     "set_pdl",
@@ -87,6 +88,7 @@ _SIGNATURES = {
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
     "tl_quantized_matmul_fused_workspace": (_SZ, [_I] * 6),
+    "tl_quantized_matmul_route": (_I, [_I] * 8 + [_VP] * 4 + [ctypes.POINTER(_I)] * 4),
     "tl_quantized_matmul_fused": (_I, [_VP] * 7 + [_I] * 6 + [_F, _I, _VP, _SZ, _VP]),
     "tl_quantized_matmul_residual_norm": (_I, [_VP] * 8 + [_I] * 3 + [_F, _I, _VP, _SZ, _VP]),
     "tl_decode_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
@@ -564,6 +566,7 @@ def quantized_matmul_fused(scales, biases, b, p0, p1=None, residual=None, prolog
     if scales.dtype not in _HALF or p0.dtype != scales.dtype or biases.dtype != scales.dtype:
         raise RuntimeError("quantized_matmul: a must be the same dtype as scales")
     _gpu("quantized_matmul_fused", scales, biases, b, p0)
+    _contig("quantized_matmul_fused", b=b, scales=scales, biases=biases)
     lda = p0.stride(0)
     if prologue == PRO_SWIGLU and (p1 is None or p1.shape != p0.shape or p1.stride(0) != lda or p1.stride(1) != 1):
         raise RuntimeError("quantized_matmul_fused: gate and up must share shape and strides")
@@ -587,6 +590,26 @@ def quantized_matmul_fused(scales, biases, b, p0, p1=None, residual=None, prolog
         )
     )
     return out
+
+
+W4_VANILLA, W4_STREAM, W4_SKINNY, W4_TILES = 0, 1, 2, 3
+
+
+def quantized_matmul_route(M, N, K, lda, prologue, fused, use_simdgroup, dtype, a, b, scales, biases):
+    """The kernel a W4A16 projection runs, decided without launching or reading anything: ``(route, splits,
+    gb_per_split, rows_per_pass, units)`` with ``route`` one of ``W4_VANILLA`` / ``W4_STREAM`` / ``W4_SKINNY`` /
+    ``W4_TILES`` (``include/tiny_llm_b200.h`` documents the other fields).  ``fused`` selects the rule of
+    ``quantized_matmul_fused`` / ``quantized_matmul_residual_norm``.  ``a``, ``b``, ``scales`` and ``biases`` are tensors
+    or plain addresses: only their alignment counts.  ``dtype`` is a torch dtype."""
+
+    def addr(x):
+        return x.data_ptr() if isinstance(x, torch.Tensor) else int(x)
+
+    facts = [_I() for _ in range(4)]
+    code = _lib.tl_quantized_matmul_route(int(M), int(N), int(K), int(lda), int(prologue), int(bool(fused)), int(bool(use_simdgroup)),
+                                          _DTYPE_CODE[dtype], addr(a), addr(b), addr(scales), addr(biases), *map(ctypes.byref, facts))
+    _check(min(code, 0))
+    return (code, *(f.value for f in facts))
 
 
 def paged_attention_token_major(query, key_pages, value_pages, block_table, context_lens, scale, is_causal, num_kv_heads, num_heads, stream=None):
@@ -629,6 +652,7 @@ def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight,
     if tuple(norm_weight.shape) != (K,) or not norm_weight.is_contiguous():
         raise RuntimeError("quantized_matmul_residual_norm: norm weight must be [K]")
     _gpu("quantized_matmul_residual_norm", scales, biases, b, p0, residual, norm_weight)
+    _contig("quantized_matmul_residual_norm", b=b, scales=scales, biases=biases)
     out = torch.empty((M, K), dtype=p0.dtype, device=p0.device)
     normed = torch.empty_like(out)
     code = _DTYPE_CODE[p0.dtype]
