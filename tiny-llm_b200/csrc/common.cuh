@@ -88,7 +88,9 @@ __device__ __forceinline__ float warp_max(float v) {
 // Streaming (read-once) 128-bit global load that does not allocate in L1.
 __device__ __forceinline__ uint4 ldg_stream(const void *p) {
     uint4 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+    // .L2::128B: a miss on one 64-byte half of a weight row's 128-byte line fetches the whole line; the same warp's
+    // next load reads the other half (decode +1-2 % on H100, DESIGN.md section 4)
+    asm volatile("ld.global.nc.L1::no_allocate.L2::128B.v4.u32 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                  : "l"(p));
     return r;

@@ -58,10 +58,17 @@ namespace tl {
 //     two per SM): correct, but the consume phase pays a shared-memory read per weight word and twice the CTAs hand
 //     over more slowly;
 //   * asking the CTA's whole weight slice into L2 (cp.async.bulk.prefetch.L2) before griddepcontrol.wait: the prefetch
-//     traffic competes with the activation round trip of the staging step.
+//     traffic competes with the activation round trip of the staging step;
+//   * a lookahead: each CTA, once its own units were requested, asking L2 (cp.async.bulk.prefetch.L2 for the weight
+//     rows, prefetch.global.L2 for scales and biases) for the slice the same CTA index of the NEXT projection streams.
+//     Decode lost 5-9 % at every placement and cap tried (DESIGN.md section 4): q|k|v, o and down already have
+//     (almost) all of their units in flight before the dependency wait, so the extra requests only lengthen the
+//     consume phase, and the next launch's griddepcontrol.wait waits for this grid to complete.
 constexpr int S5_WARPS = 16;
+// Units per warp in flight for up to 8 rows.  3 (96 KiB per SM) keeps the kernel free of register spills; 4 spilled
+// 24-48 bytes per thread and 4, 5, 6 were each slower on H100 (DESIGN.md section 4).
 #ifndef S5_DEPTH_SMALL
-#define S5_DEPTH_SMALL 4
+#define S5_DEPTH_SMALL 3
 #endif
 enum { PRO_NONE = W4_PRO_NONE, PRO_RMSNORM = W4_PRO_RMSNORM, PRO_SWIGLU = W4_PRO_SWIGLU };
 enum { EPI_NONE = 0, EPI_RESIDUAL = 1, EPI_SWIGLU_PAIRS = 2 };
