@@ -106,6 +106,15 @@ int tl_rms_norm(const void *x, const void *weight, void *out, int rows, int dim,
 /* x,out [B, L, H, D]; offsets int32 [B]; rotates the first `dims` of D. */
 int tl_rope(const void *x, const int32_t *offsets, void *out, int B, int L, int H, int D, int dims, float base,
             int traditional, int dtype, void *stream);
+/* The kernels tl_rms_norm and tl_rope run (nothing is launched or read; pointers only count for their 16-byte
+ * alignment), or a negative TL_E* code for arguments the launch rejects.
+ *   tl_rms_norm_route : threads per row, 32 (one warp; dim <= 512) or 256 (one CTA); *vec = 1 when every access is a
+ *                       16-byte vector (dim a multiple of 16 bytes, x, weight and out 16-byte aligned), else 0;
+ *   tl_rope_route     : TL_ROPE_HEADS, one thread per (token, pair) walking the H heads (dims == D, H > 1, B * L >= 64),
+ *                       else TL_ROPE_ELEMENT, one thread per (token, head, pair or copied tail element). */
+enum { TL_ROPE_ELEMENT = 0, TL_ROPE_HEADS = 1 };
+int tl_rms_norm_route(int dim, int dtype, const void *x, const void *weight, const void *out, int *vec);
+int tl_rope_route(int B, int L, int H, int D, int dims, int dtype);
 /* out = gate / (1 + exp(-gate)) * up, `size` elements. */
 int tl_swiglu(const void *gate, const void *up, void *out, long long size, int dtype, void *stream);
 /* Dense-KV GQA attention: q,out [q_rows, L, D] with q_rows = B*Hq; k,v [B*Hkv, S, D];
@@ -222,6 +231,12 @@ int tl_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, co
                                   void *q_out, void *key_pages, void *value_pages, int batch, int num_heads,
                                   int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size,
                                   int max_pages, int dtype, void *stream);
+/* The kernel tl_decode_qk_norm_rope_append, tl_chunk_qk_norm_rope_append and the second half of
+ * tl_qkv_project_rope_append run (nothing is launched), or a negative TL_E* code for arguments they reject:
+ * TL_QKN_ROW, one CTA per row with 16 warps sharing the row's angles (bf16, D == 128, Hq + 2 Hkv <= 64; the only
+ * kernel that reads split-reduction planes), else TL_QKN_HEAD, one CTA per (head, row). */
+enum { TL_QKN_HEAD = 0, TL_QKN_ROW = 1 };
+int tl_qk_norm_rope_route(int num_heads, int num_kv_heads, int head_dim, int dtype);
 /* Prefill-chunk form of the same kernel: the rows of qkv [tokens, (Hq + 2*Hkv) * D] are consecutive tokens of ONE
  * request (one shared block-table row, int32 [max_pages]); offsets[t] is the RoPE position and context_lens[t]
  * the post-append length of token t (0 = padding row: nothing is appended), all DEVICE data, so a captured
@@ -253,7 +268,9 @@ int tl_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *
  * row-concatenated projection output; context_lens are post-append; rope_inv_freq holds the 64
  * float64 frequencies base^(-i/64); out [B, Hq * 128]; max_context bounds every context_lens[b]
  * (it fixes the split count, so a captured launch stays valid as the contexts grow);
- * workspace: tl_decode_attention_fused_workspace() floats. */
+ * workspace: tl_decode_attention_fused_workspace() floats.  A context longer than the block table
+ * (max_pages * page_size) is clamped to it for the attention and for the append alike: the row's
+ * K/V land in the table's last slot.  tl_decode_qk_norm_rope_append skips such a row instead. */
 size_t tl_decode_attention_fused_workspace(int batch, int num_heads, int num_kv_heads);
 int tl_decode_attention_fused(const void *qkv, const void *q_norm_weight, const void *k_norm_weight,
                               const int32_t *offsets, const int32_t *block_table, const int32_t *context_lens,

@@ -282,3 +282,164 @@ def test_w4_route_skinny_splits():
     assert route == ext.W4_SKINNY and splits > 1 and (splits - 1) * gbps < 20 <= splits * gbps and (rpp, units) == (0, 0)
     # the split count is a function of (N, K) alone: every row count of one token tile gets the same split
     assert len({w4_route(M, 2560, 9728)[1:3] for M in (9, 16, 17, 64, 65, 128)}) == 1
+
+
+# ------------------------------------------------------------ element-wise routing --
+# tl_rms_norm_route, tl_rope_route and tl_qk_norm_rope_route call the selection functions the launches use
+# (rms_norm_path, rope_heads_path, qkv_planes_rope_supported in elementwise.cu).
+def test_rms_norm_route_threads_per_row_and_vector_accesses():
+    for dtype, epv in ((BF, 8), (F16, 8), (F32, 4)):
+        assert ext.rms_norm_route(512, dtype, A16, A16, A16) == (32, True)
+        assert ext.rms_norm_route(513, dtype, A16, A16, A16) == (256, False)
+        assert ext.rms_norm_route(4096, dtype, A16, A16, A16) == (256, True)
+        assert ext.rms_norm_route(16, dtype, A16, A16, A16) == (32, True)
+        assert ext.rms_norm_route(4096 + epv, dtype, A16, A16, A16) == (256, True)
+        assert ext.rms_norm_route(4096 + epv // 2, dtype, A16, A16, A16) == (256, False)
+        for where in range(3):  # a 2-byte offset of x, weight or out takes the scalar path
+            ptrs = [A16, A16, A16]
+            ptrs[where] = A2
+            assert ext.rms_norm_route(2560, dtype, *ptrs) == (256, False)
+    assert ext._lib.tl_rms_norm_route(128, 7, A16, A16, A16, None) == -2  # TL_EDTYPE
+    assert ext._lib.tl_rms_norm_route(0, 2, A16, A16, A16, None) == -1    # TL_EINVAL
+
+
+def test_rope_route_per_pair_kernel_needs_heads_tokens_and_full_rotation():
+    for dtype in (BF, F16, F32):
+        assert ext.rope_route(1, 64, 2, 128, 128, dtype) == ext.ROPE_HEADS
+        assert ext.rope_route(8, 8, 32, 128, 128, dtype) == ext.ROPE_HEADS
+        assert ext.rope_route(7, 9, 32, 128, 128, dtype) == ext.ROPE_ELEMENT   # B * L = 63
+        assert ext.rope_route(8, 8, 1, 128, 128, dtype) == ext.ROPE_ELEMENT    # H = 1
+        assert ext.rope_route(8, 8, 4, 128, 64, dtype) == ext.ROPE_ELEMENT     # dims < D: the tail is copied
+    with pytest.raises(RuntimeError, match="dims must be positive, even"):
+        ext.rope_route(1, 1, 1, 64, 66, BF)
+
+
+def test_qk_norm_rope_route_row_kernel_up_to_64_bf16_heads_of_128():
+    assert ext.qk_norm_rope_route(32, 8, 128, BF) == ext.QKN_ROW
+    assert ext.qk_norm_rope_route(48, 8, 128, BF) == ext.QKN_ROW   # 64 heads: every warp holds QKN_MAXH = 4
+    assert ext.qk_norm_rope_route(50, 7, 128, BF) == ext.QKN_ROW
+    assert ext.qk_norm_rope_route(64, 8, 128, BF) == ext.QKN_HEAD  # 80 heads (Qwen3-32B)
+    assert ext.qk_norm_rope_route(49, 8, 128, BF) == ext.QKN_HEAD  # 65 heads
+    assert ext.qk_norm_rope_route(32, 8, 128, F32) == ext.QKN_HEAD
+    assert ext.qk_norm_rope_route(8, 2, 64, BF) == ext.QKN_HEAD
+    assert ext.qk_norm_rope_route(8, 2, 256, BF) == ext.QKN_HEAD
+    with pytest.raises(RuntimeError, match="bfloat16 or float32 required"):
+        ext.qk_norm_rope_route(8, 2, 128, F16)
+    with pytest.raises(RuntimeError, match="bad shape"):
+        ext.qk_norm_rope_route(8, 2, 514, BF)
+
+
+# ------------------------------------------------------------- fused-form input checks --
+def _qk_args(B=2, Hq=4, Hkv=2, D=8, dtype=BF, **over):
+    """CPU arguments of decode_qk_norm_rope_append / decode_attention_fused that pass every builder check."""
+    a = dict(qkv=torch.zeros(B, (Hq + 2 * Hkv) * D, dtype=dtype), q_norm_weight=torch.ones(D, dtype=dtype),
+             k_norm_weight=torch.ones(D, dtype=dtype), offsets=torch.zeros(B, dtype=torch.int32),
+             block_table=torch.zeros(B, 3, dtype=torch.int32), context_lens=torch.ones(B, dtype=torch.int32),
+             key_pages=torch.zeros(4, Hkv, 16, D, dtype=dtype), value_pages=torch.zeros(4, Hkv, 16, D, dtype=dtype))
+    a.update(over)
+    return a
+
+
+QK_OPS = ("decode_qk_norm_rope_append", "chunk_qk_norm_rope_append", "decode_attention_fused")
+QK_BAD = {  # name: (argument, bad value for head size D and 2 rows, message)
+    "k_norm-dtype": ("k_norm_weight", lambda D: torch.ones(D, dtype=F32), r"k_norm_weight must have the dtype of qkv"),
+    "q_norm-length": ("q_norm_weight", lambda D: torch.ones(D - 1, dtype=BF), r"q_norm_weight must be contiguous \[head_dim = {D}\]"),
+    "k_norm-strided": ("k_norm_weight", lambda D: torch.ones(2 * D, dtype=BF)[::2], r"k_norm_weight must be contiguous \[head_dim = {D}\]"),
+    "offsets-dtype": ("offsets", lambda D: torch.zeros(2, dtype=torch.int64), "offsets must be int32"),
+    "offsets-short": ("offsets", lambda D: torch.zeros(1, dtype=torch.int32), r"offsets must hold one entry per row \(\[2\]\)"),
+    "context_lens-dtype": ("context_lens", lambda D: torch.ones(2, dtype=torch.int64), "context_lens must be int32"),
+    "context_lens-rank": ("context_lens", lambda D: torch.ones(2, 1, dtype=torch.int32), r"context_lens must hold one entry per row \(\[2\]\)"),
+}
+# inputs an older check of the same operator refuses first, with its own message
+QK_EARLIER = {
+    ("chunk_qk_norm_rope_append", "offsets-short"): "one block-table row, one offset and one context length per token",
+    ("decode_attention_fused", "k_norm-dtype"): "dtype mismatch",
+    ("decode_attention_fused", "context_lens-dtype"): r"block_table must be int32 \[B, max_pages\] and context_lens int32 \[B\]",
+}
+
+
+def _call_qk(op, **over):
+    """One call of op on CPU tensors: D = 8 for the standalone forms, 128 for decode_attention_fused."""
+    D = 128 if op == "decode_attention_fused" else 8
+    a = _qk_args(D=D, **over)
+    if op == "chunk_qk_norm_rope_append" and "block_table" not in over:
+        a["block_table"] = a["block_table"][0]
+    if op == "decode_attention_fused":
+        return ext.decode_attention_fused(a["qkv"], a["q_norm_weight"], a["k_norm_weight"], a["offsets"], a["block_table"], a["context_lens"],
+                                          torch.zeros(D // 2, dtype=torch.float64), a["key_pages"], a["value_pages"], 4, 2, 1e-6, 1.0, 16)
+    return getattr(ext, op)(*a.values(), 4, 2, 1e6, 1e-6)
+
+
+@pytest.mark.parametrize("op", QK_OPS)
+def test_fused_q_k_norm_forms_accept_good_inputs_up_to_the_device_check(op):
+    with pytest.raises(RuntimeError, match=f"^{op}: the course extension is GPU-only$"):
+        _call_qk(op)
+
+
+@pytest.mark.parametrize("op", QK_OPS)
+@pytest.mark.parametrize("case", sorted(QK_BAD))
+def test_fused_q_k_norm_forms_check_their_inputs_before_the_device(op, case):
+    arg, bad, msg = QK_BAD[case]
+    D = 128 if op == "decode_attention_fused" else 8
+    msg = QK_EARLIER.get((op, case), msg.replace("{D}", str(D)))
+    with pytest.raises(RuntimeError, match=f"^{op}: {msg}"):
+        _call_qk(op, **{arg: bad(D)})
+
+
+def test_decode_q_k_norm_checks_the_block_table():
+    for bt, msg in ((torch.zeros(2, 3, dtype=torch.int64), "block_table must be int32"),
+                    (torch.zeros(3, 3, dtype=torch.int32), r"block_table must be int32 \[2, max_pages\]"),
+                    (torch.zeros(6, dtype=torch.int32), r"block_table must be int32 \[2, max_pages\]")):
+        with pytest.raises(RuntimeError, match=f"decode_qk_norm_rope_append: {msg}"):
+            ext.decode_qk_norm_rope_append(*_qk_args(block_table=bt).values(), 4, 2, 1e6, 1e-6)
+    a = _qk_args()
+    a["block_table"] = torch.zeros(3, dtype=torch.int64)
+    with pytest.raises(RuntimeError, match="chunk_qk_norm_rope_append: block_table_row must be int32"):
+        ext.chunk_qk_norm_rope_append(*a.values(), 4, 2, 1e6, 1e-6)
+
+
+def test_qkv_project_rope_append_checks_its_inputs_before_the_device():
+    D, Hq, Hkv, N, rows = 128, 2, 1, 256, 3
+    K = (Hq + 2 * Hkv) * D
+
+    def call(chunk=False, **over):
+        a = dict(scales=torch.zeros(K, N // 128, dtype=BF), biases=torch.zeros(K, N // 128, dtype=BF), b=torch.zeros(K, N // 8, dtype=torch.int32),
+                 p0=torch.zeros(rows, N, dtype=BF), q_norm_weight=torch.ones(D, dtype=BF), k_norm_weight=torch.ones(D, dtype=BF),
+                 offsets=torch.zeros(rows, dtype=torch.int32), block_table=torch.zeros(3, dtype=torch.int32) if chunk else torch.zeros(rows, 3, dtype=torch.int32),
+                 context_lens=torch.ones(rows, dtype=torch.int32), key_pages=torch.zeros(4, Hkv, 16, D, dtype=BF),
+                 value_pages=torch.zeros(4, Hkv, 16, D, dtype=BF))
+        a.update(over)
+        return ext.qkv_project_rope_append(*a.values(), Hq, Hkv, 1e6, 1e-6, chunk=chunk)
+
+    with pytest.raises(RuntimeError, match="GPU-only"):
+        call()
+    with pytest.raises(RuntimeError, match="GPU-only"):
+        call(chunk=True)
+    bad = [
+        (dict(q_norm_weight=torch.ones(D, dtype=torch.float32)), "q_norm_weight must have the dtype of qkv"),
+        (dict(k_norm_weight=torch.ones(64, dtype=BF)), r"k_norm_weight must be contiguous \[head_dim = 128\]"),
+        (dict(offsets=torch.zeros(rows, dtype=torch.int64)), "offsets must be int32"),
+        (dict(offsets=torch.zeros(rows - 1, dtype=torch.int32)), "offsets must hold one entry per row"),
+        (dict(context_lens=torch.ones(rows + 1, dtype=torch.int32)), "context_lens must hold one entry per row"),
+        (dict(block_table=torch.zeros(rows, 3, dtype=torch.int64)), "block_table must be int32"),
+        (dict(block_table=torch.zeros(rows + 1, 3, dtype=torch.int32)), r"block_table must be int32 \[3, max_pages\]"),
+        (dict(biases=torch.zeros(K, N // 128, dtype=F16)), "contiguous bfloat16 inputs required"),
+        (dict(value_pages=torch.zeros(4, Hkv, 16, D, dtype=F32)), "contiguous bfloat16 inputs required"),
+    ]
+    for over, msg in bad:
+        with pytest.raises(RuntimeError, match=f"qkv_project_rope_append: {msg}"):
+            call(**over)
+    with pytest.raises(RuntimeError, match=r"qkv_project_rope_append: block_table must be int32 \[max_pages\]"):
+        call(chunk=True, block_table=torch.zeros(rows, 3, dtype=torch.int32))
+
+
+def test_qkv_project_rope_append_bounds_the_head_size_like_the_other_q_k_forms():
+    """The per-head kernel holds at most 8 warp partials (head_dim <= 512), as tl_decode_qk_norm_rope_append checks."""
+    lib = ext._lib
+
+    def call(D):
+        return lib.tl_qkv_project_rope_append(*([None] * 13), 1, 128, 1, 1, D, 1e6, 1e-6, 1, 16, 1, 0, 2, None, 0, None)
+
+    assert call(514) == -1 and b"qkv_project_rope_append: bad shape" in lib.tl_last_error()
+    assert call(512) == -1 and b"qkv_project_rope_append: null pointer" in lib.tl_last_error()  # the shape is accepted
+    assert ext.qk_norm_rope_route(1, 1, 512, BF) == ext.QKN_HEAD

@@ -25,16 +25,17 @@ from dataclasses import dataclass
 import torch
 
 F64 = torch.float64
-BF16, F16 = torch.bfloat16, torch.float16
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 U = 2.0**-24  # fp32 unit roundoff
-_P = {BF16: 8, F16: 11}  # significand bits
-_EMIN = {BF16: -126, F16: -14}
+_P = {BF16: 8, F16: 11, F32: 24}  # significand bits
+_EMIN = {BF16: -126, F16: -14, F32: -126}
 # The streaming kernel feeds code q to the tensor cores as the exact number SHIFT + q and subtracts SHIFT * sum(a)
 # through the accumulator input (w4a16_item.cuh).
 SHIFT = {BF16: 128.0, F16: 1024.0}
 PRO_NONE, PRO_RMSNORM, PRO_SWIGLU = 0, 1, 2
 EPI_NONE, EPI_RESIDUAL, EPI_SWIGLU_PAIRS = 0, 1, 2
 SILU_SLOPE = 1.1  # max |silu'(x)| = 1.0998 (at x ~ 2.4)
+SWIGLU_REL = 8 * U  # fp32 g / (1 + expf(-g)) * u: expf (2 ulp = 4u), 1 + e (u), the division and the product (2u)
 
 
 # ------------------------------------------------------------------ rounding --
@@ -143,7 +144,7 @@ def prologue64(p0, p1, prologue, eps, dtype):
     else:
         up = p1.to(F64)
         p = x / (1.0 + torch.exp(-x)) * up
-        rel = 8 * U
+        rel = SWIGLU_REL
     return round_to(p, dtype), spread(p, rel * p.abs(), dtype)
 
 
@@ -255,7 +256,7 @@ def error_bound(r, W, path, splits=1, gb_per_split=None, norm_chain=None):
         g, u = round_to(r.acc[:, gi], dtype), round_to(r.acc[:, ui], dtype)
         dg, du = spread(r.acc[:, gi], E[:, gi], dtype), spread(r.acc[:, ui], E[:, ui], dtype)
         pre = silu64(g) * u
-        Ep = SILU_SLOPE * dg * (u.abs() + du) + silu64(g).abs() * du + 8 * U * pre.abs()
+        Ep = SILU_SLOPE * dg * (u.abs() + du) + silu64(g).abs() * du + SWIGLU_REL * pre.abs()
         # below gate = -87 silu(gate) = gate e^gate leaves fp32's normal range (expf(-gate) overflows near 88.7): the
         # kernel's quotient may be 0
         Ep = torch.where(g - dg < -87.0, Ep + pre.abs(), Ep)

@@ -174,6 +174,23 @@ int tl_rope(const void *x, const int32_t *offsets, void *out, int B, int L, int 
     return launch_rope(x, offsets, out, B, L, H, D, dims, base, traditional, dtype, as_stream(stream));
 }
 
+int tl_rms_norm_route(int dim, int dtype, const void *x, const void *weight, const void *out, int *vec) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "rms_norm: expected float32, float16, or bfloat16");
+    if (dim <= 0) return fail(TL_EINVAL, "rms_norm: bad shape");
+    bool v;
+    const int tpr = rms_norm_path(dim, dtype, x, weight, out, &v);
+    if (vec) *vec = v;
+    return tpr;
+}
+
+int tl_rope_route(int B, int L, int H, int D, int dims, int dtype) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "rope: expected float32, float16, or bfloat16");
+    if (B < 0 || L < 0 || H < 0 || D <= 0) return fail(TL_EINVAL, "rope: expected x=[B,L,H,D] and one int32 offset per batch row");
+    if (dims <= 0 || dims > D || dims % 2 != 0)
+        return fail(TL_EINVAL, "rope: dims must be positive, even, and no larger than the head dimension");
+    return rope_heads_path(B, L, H, D, dims) ? TL_ROPE_HEADS : TL_ROPE_ELEMENT;
+}
+
 int tl_swiglu(const void *gate, const void *up, void *out, long long size, int dtype, void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "swiglu: expected float32, float16, or bfloat16");
     if (size < 0) return fail(TL_EINVAL, "swiglu: negative size");
@@ -407,7 +424,7 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
                                void *key_pages, void *value_pages, int rows, int N, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
                                int num_pages, int page_size, int max_pages, int chunk, int dtype, void *workspace, size_t workspace_bytes, void *stream) {
     if (dtype != TL_BF16) return fail(TL_EDTYPE, "qkv_project_rope_append: bfloat16 required");
-    if (rows < 0 || N <= 0 || N % 128 != 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || num_pages <= 0 ||
+    if (rows < 0 || N <= 0 || N % 128 != 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512 || num_pages <= 0 ||
         page_size <= 0 || max_pages <= 0)
         return fail(TL_EINVAL, "qkv_project_rope_append: bad shape");
     if (rows == 0) return TL_OK;
@@ -432,6 +449,13 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
     return launch_decode_qk_norm_rope_append(qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out, key_pages,
                                              value_pages, rows, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size, max_pages, dtype,
                                              st, chunk != 0);
+}
+
+int tl_qk_norm_rope_route(int num_heads, int num_kv_heads, int head_dim, int dtype) {
+    if (dtype != TL_F32 && dtype != TL_BF16) return fail(TL_EDTYPE, "decode_qk_norm_rope_append: bfloat16 or float32 required");
+    if (num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512)
+        return fail(TL_EINVAL, "decode_qk_norm_rope_append: bad shape");
+    return qkv_planes_rope_supported(num_heads, num_kv_heads, head_dim, dtype) ? TL_QKN_ROW : TL_QKN_HEAD;
 }
 
 int tl_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, const void *k_norm_weight,

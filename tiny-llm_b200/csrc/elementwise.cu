@@ -121,14 +121,21 @@ __global__ void __launch_bounds__(256) rms_norm_kernel(const T *x, const T *__re
     }
 }
 
+// Threads per row (32 up to 512 elements, else 256) and whether every access can be a 16-byte vector.
+int rms_norm_path(int dim, int dtype, const void *x, const void *w, const void *out, bool *vec) {
+    const int epv = 16 / (dtype == TL_F32 ? 4 : 2);
+    *vec = dim % epv == 0 && aligned16(x) && aligned16(w) && aligned16(out);
+    return dim <= 512 ? 32 : 256;
+}
+
 template <typename T>
-static int rms_norm_t(const void *x, const void *w, void *out, int rows, int dim, float eps, cudaStream_t st) {
-    constexpr int EPV = Vec<T>::N;
-    const bool vec = dim % EPV == 0 && aligned16(x) && aligned16(w) && aligned16(out);
+static int rms_norm_t(const void *x, const void *w, void *out, int rows, int dim, float eps, int dtype, cudaStream_t st) {
+    bool vec;
+    const int tpr = rms_norm_path(dim, dtype, x, w, out, &vec);
     const T *xp = static_cast<const T *>(x);
     const T *wp = static_cast<const T *>(w);
     T *op = static_cast<T *>(out);
-    if (dim <= 512) {
+    if (tpr == 32) {
         dim3 grid(ceil_div(rows, 8));
         if (vec)
             launch_chained(rms_norm_kernel<T, 32, true>, grid, dim3(256), 0, st, xp, wp, op, rows, dim, eps);
@@ -149,9 +156,9 @@ int launch_rms_norm(const void *x, const void *w, void *out, int rows, int dim, 
                     cudaStream_t st) {
     if (rows == 0) return TL_OK;
     switch (dtype) {
-        case TL_F32: return rms_norm_t<float>(x, w, out, rows, dim, eps, st);
-        case TL_F16: return rms_norm_t<__half>(x, w, out, rows, dim, eps, st);
-        case TL_BF16: return rms_norm_t<__nv_bfloat16>(x, w, out, rows, dim, eps, st);
+        case TL_F32: return rms_norm_t<float>(x, w, out, rows, dim, eps, dtype, st);
+        case TL_F16: return rms_norm_t<__half>(x, w, out, rows, dim, eps, dtype, st);
+        case TL_BF16: return rms_norm_t<__nv_bfloat16>(x, w, out, rows, dim, eps, dtype, st);
     }
     return fail(TL_EDTYPE, "rms_norm: expected float32, float16, or bfloat16");
 }
@@ -219,12 +226,15 @@ __global__ void rope_heads_kernel(const T *__restrict__ x, const int32_t *__rest
     }
 }
 
+// The per-(token, pair) kernel pays off once there are several heads to walk and enough tokens to fill the GPU.
+bool rope_heads_path(int B, int L, int H, int D, int dims) { return dims == D && H > 1 && static_cast<long long>(B) * L >= 64; }
+
 template <typename T>
 static int rope_t(const void *x, const int32_t *off, void *out, int B, int L, int H, int D, int dims, float base,
                   int traditional, cudaStream_t st) {
     const long long total = static_cast<long long>(B) * L * H * (dims / 2 + D - dims);
     if (total == 0) return TL_OK;
-    if (dims == D && H > 1 && static_cast<long long>(B) * L >= 64) {
+    if (rope_heads_path(B, L, H, D, dims)) {
         const long long work = static_cast<long long>(B) * L * (D / 2);
         const long long nb = ceil_div_ll(work, 128);
         if (nb > INT_MAX) return fail(TL_EINVAL, "rope: tensor too large");
@@ -836,7 +846,7 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
     const long long q_head_stride = chunk ? static_cast<long long>(batch) * D : D;
     const int threads = ((D / 2 + 31) / 32) * 32;
     dim3 grid(Hq + 2 * Hkv, batch);
-    if (D == 128 && dtype == TL_BF16 && Hq + 2 * Hkv <= QKN_WARPS * QKN_MAXH) {  // one CTA per row (see the kernel's comment)
+    if (qkv_planes_rope_supported(Hq, Hkv, D, dtype)) {  // one CTA per row (see the kernel's comment)
         using T = __nv_bfloat16;
         launch_chained(decode_qk_norm_rope_append_d128_kernel<T, false>, dim3(batch), dim3(QKN_WARPS * 32), 0, st, static_cast<const T *>(qkv),
                        static_cast<const float *>(nullptr), 0, 0LL, static_cast<const T *>(q_norm_w), static_cast<const T *>(k_norm_w), offsets, block_table, context_lens, static_cast<T *>(q_out),
@@ -861,7 +871,8 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
     return TL_OK;
 }
 
-// q/k norm + RoPE + append straight from the split-reduction planes of the q|k|v projection (bf16, D == 128, <= 64 heads)
+// The row kernel's shapes (bf16, D == 128, <= 64 heads): it runs the standalone forms there, and only it can take the
+// split-reduction planes of the q|k|v projection; everything else runs the per-head kernel
 bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype) { return D == 128 && dtype == TL_BF16 && Hq + 2 * Hkv <= QKN_WARPS * QKN_MAXH; }
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,

@@ -10,6 +10,10 @@
 namespace tl {
 
 // elementwise.cu
+// Kernel selection, shared by the launches and the tl_*_route exports: rms_norm's threads per row (32 | 256, *vec: 16-byte
+// accesses) and whether rope runs the per-(token, pair) kernel.  q/k norm: qkv_planes_rope_supported (the row kernel).
+int rms_norm_path(int dim, int dtype, const void *x, const void *w, const void *out, bool *vec);
+bool rope_heads_path(int B, int L, int H, int D, int dims);
 int launch_rms_norm(const void *x, const void *w, void *out, int rows, int dim, float eps, int dtype, cudaStream_t st);
 int launch_rope(const void *x, const int32_t *off, void *out, int B, int L, int H, int D, int dims, float base,
                 int traditional, int dtype, cudaStream_t st);

@@ -30,6 +30,9 @@ __all__ = [
     "quantized_embedding",
     "rms_norm",
     "rope",
+    "rms_norm_route",
+    "rope_route",
+    "qk_norm_rope_route",
     "swiglu",
     "decode_attention",
     "paged_cache_update",
@@ -74,6 +77,9 @@ _SIGNATURES = {
     "tl_quantized_embedding": (_I, [_VP] * 5 + [_I] * 4 + [_VP]),
     "tl_rms_norm": (_I, [_VP] * 3 + [_I, _I, _F, _I, _VP]),
     "tl_rope": (_I, [_VP] * 3 + [_I] * 5 + [_F, _I, _I, _VP]),
+    "tl_rms_norm_route": (_I, [_I, _I] + [_VP] * 3 + [ctypes.POINTER(_I)]),
+    "tl_rope_route": (_I, [_I] * 6),
+    "tl_qk_norm_rope_route": (_I, [_I] * 4),
     "tl_swiglu": (_I, [_VP] * 3 + [_LL, _I, _VP]),
     "tl_add": (_I, [_VP] * 3 + [_LL, _I, _VP]),
     "tl_decode_attention": (_I, [_VP] * 5 + [_I] * 6 + [_F, _I, _I, _I, _VP]),
@@ -143,6 +149,31 @@ def _contig(op: str, **named: torch.Tensor) -> None:
     for name, t in named.items():
         if not t.is_contiguous():
             raise RuntimeError(f"{op}: {name} must be contiguous")
+
+
+def _norm_weights(op: str, dtype: torch.dtype, head_dim: int, **named: torch.Tensor) -> None:
+    """Per-head RMSNorm weights: the kernels read head_dim contiguous elements of the activation dtype."""
+    for name, w in named.items():
+        if w.dtype != dtype:
+            raise RuntimeError(f"{op}: {name} must have the dtype of qkv ({dtype})")
+        if tuple(w.shape) != (head_dim,) or not w.is_contiguous():
+            raise RuntimeError(f"{op}: {name} must be contiguous [head_dim = {head_dim}]")
+
+
+def _int32(op: str, rows: int | None = None, **named: torch.Tensor) -> None:
+    """int32 index tensors; with ``rows``, one entry per row ([rows])."""
+    for name, t in named.items():
+        if t.dtype != torch.int32:
+            raise RuntimeError(f"{op}: {name} must be int32")
+        if rows is not None and (t.dim() != 1 or t.shape[0] != rows):
+            raise RuntimeError(f"{op}: {name} must hold one entry per row ([{rows}])")
+
+
+def _block_table(op: str, block_table: torch.Tensor, rows: int | None) -> None:
+    """int32 [rows, max_pages], or (rows None: a prefill chunk) the request's int32 [max_pages] row."""
+    _int32(op, block_table=block_table)
+    if block_table.dim() != (1 if rows is None else 2) or (rows is not None and block_table.shape[0] != rows):
+        raise RuntimeError(f"{op}: block_table must be int32 " + ("[max_pages]" if rows is None else f"[{rows}, max_pages]"))
 
 
 def _stream_ptr(stream, ref: torch.Tensor) -> int:
@@ -296,6 +327,39 @@ def rope(x, offsets, dims, base, traditional=False, stream=None):
                      _DTYPE_CODE[x.dtype], _stream_ptr(stream, x))
     )
     return out
+
+
+ROPE_ELEMENT, ROPE_HEADS = 0, 1
+QKN_HEAD, QKN_ROW = 0, 1
+
+
+def rms_norm_route(dim, dtype, x, weight, out):
+    """The kernel ``rms_norm`` runs, decided without launching or reading anything: ``(threads_per_row, vec)`` with
+    32 or 256 threads per row and ``vec`` True for 16-byte accesses.  ``x``, ``weight`` and ``out`` are tensors or plain
+    addresses: only their 16-byte alignment counts.  ``dtype`` is a torch dtype."""
+
+    def addr(t):
+        return t.data_ptr() if isinstance(t, torch.Tensor) else int(t)
+
+    vec = _I()
+    code = _lib.tl_rms_norm_route(int(dim), _DTYPE_CODE[dtype], addr(x), addr(weight), addr(out), ctypes.byref(vec))
+    _check(min(code, 0))
+    return code, bool(vec.value)
+
+
+def rope_route(B, L, H, D, dims, dtype):
+    """``ROPE_HEADS`` (one thread per (token, pair) walking the heads) or ``ROPE_ELEMENT``: the kernel ``rope`` runs."""
+    code = _lib.tl_rope_route(int(B), int(L), int(H), int(D), int(dims), _DTYPE_CODE[dtype])
+    _check(min(code, 0))
+    return code
+
+
+def qk_norm_rope_route(num_heads, num_kv_heads, head_dim, dtype):
+    """``QKN_ROW`` (one CTA per row) or ``QKN_HEAD`` (one CTA per head and row): the kernel the fused q/k norm + RoPE +
+    K/V append runs in ``decode_qk_norm_rope_append``, ``chunk_qk_norm_rope_append`` and ``qkv_project_rope_append``."""
+    code = _lib.tl_qk_norm_rope_route(int(num_heads), int(num_kv_heads), int(head_dim), _DTYPE_CODE[dtype])
+    _check(min(code, 0))
+    return code
 
 
 def swiglu(gate, up, stream=None):
@@ -679,6 +743,9 @@ def chunk_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_
         raise RuntimeError("chunk_qk_norm_rope_append: dtype mismatch")
     if block_table_row.dim() != 1 or offsets.numel() != T or context_lens.numel() != T:
         raise RuntimeError("chunk_qk_norm_rope_append: one block-table row, one offset and one context length per token")
+    _int32("chunk_qk_norm_rope_append", T, offsets=offsets, context_lens=context_lens)
+    _int32("chunk_qk_norm_rope_append", block_table_row=block_table_row)
+    _norm_weights("chunk_qk_norm_rope_append", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
     _gpu("chunk_qk_norm_rope_append", qkv, q_norm_weight, k_norm_weight, offsets, block_table_row, context_lens, key_pages, value_pages)
     _contig("chunk_qk_norm_rope_append", qkv=qkv, offsets=offsets, block_table_row=block_table_row, context_lens=context_lens,
             key_pages=key_pages, value_pages=value_pages)
@@ -713,6 +780,9 @@ def decode_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block
         raise RuntimeError("decode_qk_norm_rope_append: qkv must be [B, (Hq + 2*Hkv) * D]")
     if qkv.dtype != key_pages.dtype or value_pages.dtype != key_pages.dtype or q_norm_weight.dtype != qkv.dtype:
         raise RuntimeError("decode_qk_norm_rope_append: dtype mismatch")
+    _norm_weights("decode_qk_norm_rope_append", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
+    _int32("decode_qk_norm_rope_append", B, offsets=offsets, context_lens=context_lens)
+    _block_table("decode_qk_norm_rope_append", block_table, B)
     _gpu("decode_qk_norm_rope_append", qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages)
     _contig("decode_qk_norm_rope_append", qkv=qkv, offsets=offsets, block_table=block_table, context_lens=context_lens,
             key_pages=key_pages, value_pages=value_pages)
@@ -739,9 +809,16 @@ def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight,
     K = b.shape[0]
     if K != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads or b.shape[1] * 8 != N:
         raise RuntimeError("qkv_project_rope_append: weight rows must be (Hq + 2*Hkv) * D")
-    if p0.dtype != torch.bfloat16 or key_pages.dtype != p0.dtype or scales.dtype != p0.dtype or not p0.is_contiguous():
+    if (p0.dtype != torch.bfloat16 or key_pages.dtype != p0.dtype or value_pages.dtype != p0.dtype or scales.dtype != p0.dtype
+            or biases.dtype != p0.dtype or not p0.is_contiguous()):
         raise RuntimeError("qkv_project_rope_append: contiguous bfloat16 inputs required")
-    _gpu("qkv_project_rope_append", scales, biases, b, p0, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages)
+    op = "qkv_project_rope_append"
+    _norm_weights(op, p0.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
+    _int32(op, rows, offsets=offsets, context_lens=context_lens)
+    _block_table(op, block_table, None if chunk else rows)
+    _gpu(op, scales, biases, b, p0, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages)
+    _contig(op, b=b, scales=scales, biases=biases, offsets=offsets, block_table=block_table, context_lens=context_lens, key_pages=key_pages,
+            value_pages=value_pages)
     scratch = torch.empty((rows, K), dtype=p0.dtype, device=p0.device)
     q_out = torch.empty((num_heads, rows, D) if chunk else (rows, num_heads, D), dtype=p0.dtype, device=p0.device)
     code = _DTYPE_CODE[p0.dtype]
@@ -784,6 +861,8 @@ def decode_attention_fused(qkv, q_norm_weight, k_norm_weight, offsets, block_tab
         raise RuntimeError("decode_attention_fused: rope_inv_freq must be float64 [head_dim / 2]")
     if block_table.dim() != 2 or block_table.shape[0] != B or block_table.dtype != torch.int32 or context_lens.dtype != torch.int32:
         raise RuntimeError("decode_attention_fused: block_table must be int32 [B, max_pages] and context_lens int32 [B]")
+    _norm_weights("decode_attention_fused", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
+    _int32("decode_attention_fused", B, offsets=offsets, context_lens=context_lens)
     _gpu("decode_attention_fused", qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, rope_inv_freq, key_pages, value_pages)
     _contig("decode_attention_fused", qkv=qkv, offsets=offsets, block_table=block_table, context_lens=context_lens,
             key_pages=key_pages, value_pages=value_pages, rope_inv_freq=rope_inv_freq)
