@@ -278,6 +278,19 @@ int tl_decode_attention_fused(const void *qkv, const void *q_norm_weight, const 
                               float *workspace, int batch, int num_heads, int num_kv_heads, int head_dim, float eps,
                               float scale, int num_pages, int page_size, int max_pages, int max_context, int dtype,
                               void *stream);
+/* The same with rows_per_request (1..8) consecutive query rows per request, e.g. the verify pass of
+ * speculative decoding: qkv [B R, (Hq + 2 Hkv) * 128], offsets / context_lens [B R], out [B R, Hq * 128],
+ * block_table [B, max_pages] shared by the rows of a request.  Row j of a request must have context
+ * context_lens[row 0] + j (or all rows 0: an idle request).  Each row's output, and the K/V it appends, equal
+ * bit for bit tl_decode_attention_fused run on that row alone with the rows before it already appended (the
+ * split count follows B and max_context, not B R).  rows_per_request == 1 is tl_decode_attention_fused. */
+size_t tl_decode_attention_fused_rows_workspace(int batch, int rows_per_request, int num_heads, int num_kv_heads);
+int tl_decode_attention_fused_rows(const void *qkv, const void *q_norm_weight, const void *k_norm_weight,
+                                   const int32_t *offsets, const int32_t *block_table, const int32_t *context_lens,
+                                   const double *rope_inv_freq, void *key_pages, void *value_pages, void *out,
+                                   float *workspace, int batch, int rows_per_request, int num_heads, int num_kv_heads,
+                                   int head_dim, float eps, float scale, int num_pages, int page_size, int max_pages,
+                                   int max_context, int dtype, void *stream);
 /* Programmatic dependent launch for the streaming kernels (on by default; 0 turns it off,
  * TL_PDL=0 in the environment does the same). */
 int tl_set_pdl(int enabled);

@@ -493,7 +493,7 @@ int tl_chunk_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, con
 
 size_t tl_decode_attention_fused_workspace(int batch, int num_heads, int num_kv_heads) {
     if (batch < 1 || num_heads < 1 || num_kv_heads < 1) return 0;
-    return decode_attention_fused_workspace(batch, num_heads, num_kv_heads);
+    return decode_attention_fused_workspace(batch, 1, num_heads, num_kv_heads);
 }
 
 int tl_decode_attention_fused(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
@@ -501,14 +501,29 @@ int tl_decode_attention_fused(const void *qkv, const void *q_norm_weight, const 
                               void *key_pages, void *value_pages, void *out, float *workspace, int batch, int num_heads,
                               int num_kv_heads, int head_dim, float eps, float scale, int num_pages, int page_size,
                               int max_pages, int max_context, int dtype, void *stream) {
+    return tl_decode_attention_fused_rows(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, rope_inv_freq,
+                                          key_pages, value_pages, out, workspace, batch, 1, num_heads, num_kv_heads, head_dim, eps,
+                                          scale, num_pages, page_size, max_pages, max_context, dtype, stream);
+}
+
+size_t tl_decode_attention_fused_rows_workspace(int batch, int rows_per_request, int num_heads, int num_kv_heads) {
+    if (batch < 1 || rows_per_request < 1 || rows_per_request > 8 || num_heads < 1 || num_kv_heads < 1) return 0;
+    return decode_attention_fused_workspace(batch, rows_per_request, num_heads, num_kv_heads);
+}
+
+int tl_decode_attention_fused_rows(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
+                                   const int32_t *block_table, const int32_t *context_lens, const double *rope_inv_freq,
+                                   void *key_pages, void *value_pages, void *out, float *workspace, int batch,
+                                   int rows_per_request, int num_heads, int num_kv_heads, int head_dim, float eps, float scale,
+                                   int num_pages, int page_size, int max_pages, int max_context, int dtype, void *stream) {
     if (batch == 0) return TL_OK;
     if (!qkv || !q_norm_weight || !k_norm_weight || !offsets || !block_table || !context_lens || !rope_inv_freq || !key_pages ||
         !value_pages || !out || !workspace)
         return fail(TL_EINVAL, "decode_attention_fused: null pointer");
     if (batch < 0 || page_size < 1 || max_pages < 1 || num_pages < 0) return fail(TL_EINVAL, "decode_attention_fused: bad sizes");
     return launch_decode_attention_fused(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, rope_inv_freq,
-                                         key_pages, value_pages, out, workspace, batch, num_heads, num_kv_heads, head_dim, eps,
-                                         scale, num_pages, page_size, max_pages, max_context, dtype, as_stream(stream));
+                                         key_pages, value_pages, out, workspace, batch, rows_per_request, num_heads, num_kv_heads,
+                                         head_dim, eps, scale, num_pages, page_size, max_pages, max_context, dtype, as_stream(stream));
 }
 
 #if TL_TRACE

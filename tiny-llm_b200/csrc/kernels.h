@@ -81,12 +81,14 @@ void trace_bind_matvec(unsigned long long *buf, unsigned int *n, unsigned int ca
 void trace_bind_attention(unsigned long long *buf, unsigned int *n, unsigned int cap);
 void trace_bind_skinny(unsigned long long *buf, unsigned int *n, unsigned int cap);
 #endif
-size_t decode_attention_fused_workspace(int batch, int num_heads, int num_kv_heads);
+// batch = requests; each carries rows_per_request (1..8) consecutive query rows (qkv / out / offsets / context_lens
+// have batch * rows_per_request rows, the block table has batch rows)
+size_t decode_attention_fused_workspace(int batch, int rows_per_request, int num_heads, int num_kv_heads);
 int launch_decode_attention_fused(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, const double *rope_inv_freq,
-                                  void *key_pages, void *value_pages, void *out, float *workspace, int batch, int num_heads,
-                                  int num_kv_heads, int head_dim, float eps, float scale, int num_pages, int page_size,
-                                  int max_pages, int max_context, int dtype, cudaStream_t st);
+                                  void *key_pages, void *value_pages, void *out, float *workspace, int batch, int rows_per_request,
+                                  int num_heads, int num_kv_heads, int head_dim, float eps, float scale, int num_pages,
+                                  int page_size, int max_pages, int max_context, int dtype, cudaStream_t st);
 
 // attention_decode.cu
 int launch_decode_attention(const void *q, const void *k, const void *v, const float *mask, void *out, int q_rows,

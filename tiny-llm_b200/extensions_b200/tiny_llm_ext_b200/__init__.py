@@ -101,6 +101,8 @@ _SIGNATURES = {
     "tl_chunk_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
     "tl_decode_attention_fused_workspace": (_SZ, [_I, _I, _I]),
     "tl_decode_attention_fused": (_I, [_VP] * 11 + [_I] * 4 + [_F, _F] + [_I] * 5 + [_VP]),
+    "tl_decode_attention_fused_rows_workspace": (_SZ, [_I, _I, _I, _I]),
+    "tl_decode_attention_fused_rows": (_I, [_VP] * 11 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP]),
     "tl_paged_cache_append_chunk": (_I, [_VP] * 5 + [_I] * 4 + [ctypes.c_longlong, ctypes.c_longlong, _I, _VP]),
     "tl_set_pdl": (_I, [_I]),
 }
@@ -842,25 +844,47 @@ def rope_inv_freq_table(head_dim: int, base: float, device) -> torch.Tensor:
     return torch.pow(torch.tensor(float(base), dtype=torch.float64), -torch.arange(half, dtype=torch.float64) / half).to(device)
 
 
-def decode_attention_fused_workspace(batch: int, num_heads: int, num_kv_heads: int) -> int:
-    return int(_lib.tl_decode_attention_fused_workspace(int(batch), int(num_heads), int(num_kv_heads)))
+def decode_attention_fused_workspace(batch: int, num_heads: int, num_kv_heads: int, rows_per_request: int = 1) -> int:
+    """float32 values of the split workspace for ``batch`` requests of ``rows_per_request`` query rows each."""
+    R = _rows_per_request("decode_attention_fused_workspace", rows_per_request)
+    if R == 1:
+        return int(_lib.tl_decode_attention_fused_workspace(int(batch), int(num_heads), int(num_kv_heads)))
+    return int(_lib.tl_decode_attention_fused_rows_workspace(int(batch), R, int(num_heads), int(num_kv_heads)))
+
+
+def _rows_per_request(op: str, rows_per_request) -> int:
+    if isinstance(rows_per_request, bool) or not isinstance(rows_per_request, int) or not 1 <= rows_per_request <= 8:
+        raise RuntimeError(f"{op}: rows_per_request must be an int in [1, 8]")
+    return rows_per_request
 
 
 def decode_attention_fused(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, rope_inv_freq, key_pages,
-                           value_pages, num_heads, num_kv_heads, eps, scale, max_context, out=None, workspace=None, stream=None):
+                           value_pages, num_heads, num_kv_heads, eps, scale, max_context, out=None, workspace=None, stream=None,
+                           rows_per_request=1):
     """One decode step of attention for ``qkv [B, (Hq + 2 Hkv) * 128]`` (bf16): per-head q/k RMSNorm +
     RoPE, append of the newest K/V row, paged GQA attention (context_lens are post-append) ->
-    ``[B, Hq * 128]``.  ``max_context`` bounds every context length (it fixes the split count)."""
+    ``[B, Hq * 128]``.  ``max_context`` bounds every context length (it fixes the split count).
+
+    ``rows_per_request = R`` (1..8): the ``B`` rows are ``B / R`` requests of R consecutive query rows each (row j of
+    a request at context ``context_lens[row 0] + j``), sharing one block-table row (``[B / R, max_pages]``).  Every
+    row equals, bit for bit, the single-row call on it alone with the rows before it already appended."""
+    R = _rows_per_request("decode_attention_fused", rows_per_request)
     B = qkv.shape[0]
     P, Hkv, page_size, D = key_pages.shape
     if qkv.dim() != 2 or qkv.shape[1] != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads:
         raise RuntimeError("decode_attention_fused: qkv must be [B, (Hq + 2*Hkv) * D]")
+    if R > 1 and B % R != 0:
+        raise RuntimeError(f"decode_attention_fused: qkv rows must be a multiple of rows_per_request ({R})")
+    requests = B // R
     if qkv.dtype != key_pages.dtype or value_pages.dtype != key_pages.dtype or q_norm_weight.dtype != qkv.dtype or k_norm_weight.dtype != qkv.dtype:
         raise RuntimeError("decode_attention_fused: dtype mismatch")
     if rope_inv_freq.dtype != torch.float64 or rope_inv_freq.numel() != D // 2:
         raise RuntimeError("decode_attention_fused: rope_inv_freq must be float64 [head_dim / 2]")
-    if block_table.dim() != 2 or block_table.shape[0] != B or block_table.dtype != torch.int32 or context_lens.dtype != torch.int32:
-        raise RuntimeError("decode_attention_fused: block_table must be int32 [B, max_pages] and context_lens int32 [B]")
+    if R == 1:
+        if block_table.dim() != 2 or block_table.shape[0] != B or block_table.dtype != torch.int32 or context_lens.dtype != torch.int32:
+            raise RuntimeError("decode_attention_fused: block_table must be int32 [B, max_pages] and context_lens int32 [B]")
+    elif block_table.dim() != 2 or block_table.shape[0] != requests or block_table.dtype != torch.int32 or context_lens.dtype != torch.int32:
+        raise RuntimeError("decode_attention_fused: block_table must be int32 [B / rows_per_request, max_pages] and context_lens int32 [B]")
     _norm_weights("decode_attention_fused", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
     _int32("decode_attention_fused", B, offsets=offsets, context_lens=context_lens)
     _gpu("decode_attention_fused", qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, rope_inv_freq, key_pages, value_pages)
@@ -868,19 +892,20 @@ def decode_attention_fused(qkv, q_norm_weight, k_norm_weight, offsets, block_tab
             key_pages=key_pages, value_pages=value_pages, rope_inv_freq=rope_inv_freq)
     if out is None:
         out = torch.empty((B, num_heads * D), dtype=qkv.dtype, device=qkv.device)
-    need = decode_attention_fused_workspace(B, num_heads, num_kv_heads)
+    need = decode_attention_fused_workspace(requests, num_heads, num_kv_heads, rows_per_request=R)
     if workspace is None:
         workspace = torch.empty(need, dtype=torch.float32, device=qkv.device)
     elif workspace.dtype != torch.float32 or workspace.numel() < need or not workspace.is_cuda:
         raise RuntimeError("decode_attention_fused: workspace must hold decode_attention_fused_workspace() float32 values")
-    _check(
-        _lib.tl_decode_attention_fused(
-            qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table.data_ptr(),
+    args = (qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table.data_ptr(),
             context_lens.data_ptr(), rope_inv_freq.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), out.data_ptr(),
-            workspace.data_ptr(), B, int(num_heads), int(num_kv_heads), D, float(eps), float(scale), P, page_size,
-            block_table.shape[1], int(max_context), _DTYPE_CODE[qkv.dtype], _stream_ptr(stream, qkv),
-        )
-    )
+            workspace.data_ptr())
+    tail = (int(num_heads), int(num_kv_heads), D, float(eps), float(scale), P, page_size, block_table.shape[1], int(max_context),
+            _DTYPE_CODE[qkv.dtype], _stream_ptr(stream, qkv))
+    if R == 1:
+        _check(_lib.tl_decode_attention_fused(*args, B, *tail))
+    else:
+        _check(_lib.tl_decode_attention_fused_rows(*args, requests, R, *tail))
     return out
 
 

@@ -8,7 +8,7 @@ from .basics import linear, silu, softmax
 from .batch import ContinuousBatcher, Request, batch_generate
 from .checkpoint import load_checkpoint, load_tokenizer, save_checkpoint
 from .embedding import Embedding, QuantizedEmbedding
-from .generate import greedy_generate_ids, simple_generate_with_kv_cache
+from .generate import greedy_generate_ids, simple_generate_with_kv_cache, speculative_generate, speculative_generate_ids
 from .kv_cache import BatchingKvCache, TinyKvCache, TinyKvFullCache
 from .layer_norm import RMSNorm
 from .models import dispatch_model, shortcut_name_to_full_name

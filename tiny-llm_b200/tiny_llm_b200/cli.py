@@ -6,6 +6,8 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli generate --model /path/to/Qwen3-4B-MLX-4bit --prompt "..." [--loader week3]
     python -m tiny_llm_b200.cli batch    --model /path/to/ckpt --prompts-file prompts.txt --batch-size 5
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --max-new-tokens 8   (no files needed)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
+        (speculative decoding: same ids as greedy; acceptance stats on stderr)
 """
 
 from __future__ import annotations
@@ -68,7 +70,27 @@ def cmd_generate(args) -> int:
             tokenizer.detokenizer.add_token(token)
             print(tokenizer.detokenizer.last_segment, end="", flush=True)
 
-    produced = greedy_generate_ids(model, ids, args.max_new_tokens, eos_token_id=getattr(tokenizer, "eos_token_id", None), device=device,
+    eos = getattr(tokenizer, "eos_token_id", None)
+    if args.draft_model or args.draft_synthetic:
+        from .generate import speculative_generate_ids
+
+        if sampler is not None:
+            raise SystemExit("speculative decoding is greedy: drop --sampler-temp")
+        if args.draft_model and args.draft_synthetic:
+            raise SystemExit("give one draft: --draft-model or --draft-synthetic, not both")
+        draft_args = argparse.Namespace(**{**vars(args), "model": args.draft_model, "synthetic": args.draft_synthetic})
+        draft_ns, draft_tokenizer, draft_name = _load(draft_args, device)
+        if tokenizer is not None and draft_tokenizer is not None and tokenizer.get_vocab() != draft_tokenizer.get_vocab():
+            raise SystemExit("draft and target tokenizers use different token ids")
+        draft = _model(args, draft_ns, draft_name)
+        produced, stats = speculative_generate_ids(draft, model, ids, args.max_new_tokens, proposal_length=args.proposal_length,
+                                                   eos_token_ids=() if eos is None else (eos,), device=device, on_token=emit)
+        proposed, accepted = sum(p for p, _ in stats), sum(a for _, a in stats)
+        print(f"\nspeculative: {len(stats)} rounds, {accepted}/{proposed} proposals accepted"
+              + (f" ({accepted / proposed:.2f})" if proposed else ""), file=sys.stderr)
+        print()
+        return 0
+    produced = greedy_generate_ids(model, ids, args.max_new_tokens, eos_token_id=eos, device=device,
                                    on_token=emit, sampler=sampler)
     print()
     return 0 if produced is not None else 1
@@ -114,6 +136,9 @@ def main(argv=None) -> int:
     sub.choices["generate"].add_argument("--sampler-temp", type=float, default=0.0)
     sub.choices["generate"].add_argument("--sampler-top-p", type=float, default=None)
     sub.choices["generate"].add_argument("--sampler-top-k", type=int, default=None)
+    sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
+    sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")
+    sub.choices["generate"].add_argument("--proposal-length", type=int, default=4, help="draft tokens proposed per round")
     sub.choices["batch"].add_argument("--prompts-file", default=None)
     sub.choices["batch"].add_argument("--batch-size", type=int, default=5)
     sub.choices["batch"].add_argument("--prefill-step", type=int, default=128)

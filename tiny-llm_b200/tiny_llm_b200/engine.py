@@ -25,6 +25,7 @@ front and the engine re-captures if a slab pointer changes.
 
 from __future__ import annotations
 
+import gc
 from types import SimpleNamespace
 
 import numpy as np
@@ -169,8 +170,16 @@ class _GraphEngine:
         self._stream.synchronize()
         graph = torch.cuda.CUDAGraph()
         launched = ext.launch_count()
-        with torch.cuda.graph(graph, stream=self._stream, pool=pool):
-            body()
+        # No garbage collection inside the capture: a collected engine frees its pinned metadata block, and the host
+        # allocator's event calls on another stream invalidate a global-mode capture.
+        gc_was_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(graph, stream=self._stream, pool=pool):
+                body()
+        finally:
+            if gc_was_enabled:
+                gc.enable()
         self._launches = ext.launch_count() - launched
         return graph
 
@@ -221,23 +230,26 @@ class _SlotRecord:
 
 class DecodeEngine(_GraphEngine):
     """One decode step of ``B`` slots as a CUDA graph (module docstring).  Metadata block:
-    ``tokens [B] | offsets [B] | context_lens [B] | block tables [Ly, B, MP]``.  The fused path uses the model's one
-    packed weight copy (``Qwen3ModelWeek3.packed_layers``); B > 8 runs the layer stack shared with the prefill engine
-    (``_swap_ab_layers``)."""
+    ``tokens [N] | offsets [N] | context_lens [N] | block tables [Ly, B, MP]`` with ``N = B * rows_per_request`` query
+    rows (``rows_per_request > 1``: ``VerifyEngine``, consecutive tokens of one request per slot).  The fused path uses
+    the model's one packed weight copy (``Qwen3ModelWeek3.packed_layers``); B > 8 runs the layer stack shared with the
+    prefill engine (``_swap_ab_layers``)."""
 
     def __init__(self, model, batch_size: int, max_seq_len: int, device, log_capacity: int = 4096, fused: bool = True, *,
-                 _row_variants: bool = True):
+                 _row_variants: bool = True, rows_per_request: int = 1):
         B = self.B = batch_size
-        super().__init__(model, max_seq_len, device, 3 * B, B)
+        self._rows_per_request = rows_per_request
+        N = self.rows = B * rows_per_request
+        super().__init__(model, max_seq_len, device, 3 * N, B)
         self.V = model.vocab_size
         self.log_capacity = log_capacity
-        self._meta_dev_head, self._meta_host_head = self.meta_dev[: 3 * B], self.meta_host[: 3 * B]  # the per-step upload
-        self.tokens = self.meta_dev[0:B]
-        self.offsets = self.meta_dev[B : 2 * B]
-        self.context_lens = self.meta_dev[2 * B : 3 * B]
-        self.tables = self.meta_dev[3 * B :].view(self.n_layers, B, self.max_pages)
-        self.tables_np = self.meta_np[3 * B :].reshape(self.n_layers, B, self.max_pages)
-        self.next_tokens = torch.zeros(B, dtype=torch.int32, device=self.device)
+        self._meta_dev_head, self._meta_host_head = self.meta_dev[: 3 * N], self.meta_host[: 3 * N]  # the per-step upload
+        self.tokens = self.meta_dev[0:N]
+        self.offsets = self.meta_dev[N : 2 * N]
+        self.context_lens = self.meta_dev[2 * N : 3 * N]
+        self.tables = self.meta_dev[3 * N :].view(self.n_layers, B, self.max_pages)
+        self.tables_np = self.meta_np[3 * N :].reshape(self.n_layers, B, self.max_pages)
+        self.next_tokens = torch.zeros(N, dtype=torch.int32, device=self.device)
         self.out_log = torch.full((log_capacity * B,), -1, dtype=torch.int32, device=self.device)
         self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         # per slot: the request group (its per-layer cache objects) the table rows reflect
@@ -255,13 +267,11 @@ class DecodeEngine(_GraphEngine):
         # step is launch-bound.  With many slots or long contexts the K/V stream dominates and the step uses
         # q/k norm + rope + append as one small launch followed by tl_paged_attention, whose long-context path
         # is the TMA + wgmma streaming kernel (attention_prefill_tc.cu).
-        self._attention_fused = (self.fused and self.D == 128 and self.Hq // self.Hkv <= 4
-                                 and model.embedding.weight.scales.dtype == torch.bfloat16
-                                 and not getattr(attn0.rope, "traditional", False)
-                                 and self.B * self.max_seq_len <= FUSED_ATTENTION_MAX_SLOT_TOKENS)
+        self._attention_fused = self.fused and DecodeEngine.fused_attention_applies(model, self.B * self.max_seq_len)
         if self._attention_fused:
             self._rope_inv_freq = ext.rope_inv_freq_table(self.D, attn0.rope.base, self.device)
-            self._attn_ws = torch.empty(ext.decode_attention_fused_workspace(self.B, self.Hq, self.Hkv), dtype=torch.float32, device=self.device)
+            self._attn_ws = torch.empty(ext.decode_attention_fused_workspace(self.B, self.Hq, self.Hkv, rows_per_request=rows_per_request),
+                                        dtype=torch.float32, device=self.device)
         # Row variants: the scheduler fills slots from index 0 (batch.py:220-226), so while few requests are live the
         # occupied slots are a prefix of the table.  A step graph over the first 16 / 32 rows is captured beside the
         # full one and step() replays the smallest that covers the highest occupied slot: every kernel of the wide
@@ -272,6 +282,15 @@ class DecodeEngine(_GraphEngine):
         self._variants = sorted({r for r in (16, 32, 64) if r < self.B} | {self.B}) if (self.fused and self.B > 16 and _row_variants) else [self.B]
         self._graphs: dict = {}
         self.variant_replays = {r: 0 for r in self._variants}
+
+    @staticmethod
+    def fused_attention_applies(model, slot_tokens: int) -> bool:
+        """The one-launch attention's conditions on the model, for ``slots x max_seq_len`` = ``slot_tokens``."""
+        attn0 = model.layers_inner[0].self_attn
+        rope = attn0.rope
+        return (not rope.traditional and rope.dims == attn0.head_dim and attn0.head_dim == 128
+                and attn0.num_heads // attn0.num_kv_heads <= 4 and model.embedding.weight.scales.dtype == torch.bfloat16
+                and slot_tokens <= FUSED_ATTENTION_MAX_SLOT_TOKENS)
 
     def reserve_pools(self, pages_per_layer: int | None = None) -> None:
         super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
@@ -317,7 +336,7 @@ class DecodeEngine(_GraphEngine):
         Every rounding point of the operator-by-operator sequence is kept.
         ``rows``: only the first ``rows`` slots (a row variant, see __init__)."""
         m = self.model
-        R = self.B if rows is None else rows
+        R = self.rows if rows is None else rows
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens[:R], emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
@@ -330,7 +349,7 @@ class DecodeEngine(_GraphEngine):
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
         self.next_tokens[:R].copy_(ext.argmax(logits))
         if self.logits is None:
-            self.logits = torch.zeros((self.B, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
+            self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
 
     def _swap_ab_attention(self, R: int):
@@ -360,7 +379,7 @@ class DecodeEngine(_GraphEngine):
         """The layer stack for at most 8 slots on the streaming matvec kernel, with RMSNorm as its prologue and the
         residual add as its epilogue; returns the residual stream before the final norm."""
         m = self.model
-        B, Hq, Hkv, D = self.B, self.Hq, self.Hkv, self.D
+        B, Hq, Hkv, D = x.shape[0], self.Hq, self.Hkv, self.D
         for i, block in enumerate(m.layers_inner):
             at, pk, pool = block.self_attn, self._packed[i], m.page_pools[i]
             ln1, ln2 = block.input_layernorm, block.post_attention_layernorm
@@ -370,7 +389,7 @@ class DecodeEngine(_GraphEngine):
                 y = ext.decode_attention_fused(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                self.offsets, self.tables[i], self.context_lens, self._rope_inv_freq,
                                                pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
-                                               self.max_seq_len, workspace=self._attn_ws)
+                                               self.max_seq_len, workspace=self._attn_ws, rows_per_request=self._rows_per_request)
             else:
                 q = ext.decode_qk_norm_rope_append(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                    self.offsets, self.tables[i], self.context_lens, pool._key_pages, pool._value_pages,
@@ -385,8 +404,8 @@ class DecodeEngine(_GraphEngine):
         return x
 
     def _set_idle(self) -> None:
-        self.meta_dev[2 * self.B : 3 * self.B].zero_()  # context_lens
-        self.meta_dev[3 * self.B :].fill_(-1)
+        self.meta_dev[2 * self.rows : 3 * self.rows].zero_()  # context_lens
+        self.meta_dev[3 * self.rows :].fill_(-1)
         self._tables_dirty = True
 
     def _capture_graphs(self) -> None:
@@ -397,6 +416,10 @@ class DecodeEngine(_GraphEngine):
             ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
 
         self._graph = self._graph_of(forward)
+        self._graphs = {self.B: self._graph}
+        if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
+            self.kernels_per_step = self._launches
+            return
         # the same step (already warmed up) with token feedback and position advance, for decode_on_device
         self._graph_loop = self._graph_of(self_advancing_step, pool=self._graph.pool(), warmups=0)
         self.kernels_per_step = self._launches  # kernels of libtiny_llm_b200.so recorded into one self-advancing step
@@ -540,11 +563,11 @@ class DecodeEngine(_GraphEngine):
             self._tables_dirty = False
         else:  # tokens | offsets | context_lens only: the block tables on the device are current
             self._upload_meta(self._meta_dev_head, self._meta_host_head)
-            self.h2d_bytes += 3 * self.B * 4
+            self.h2d_bytes += 3 * self.rows * 4
 
     def upload_bytes_per_step(self) -> int:
         """Host -> device bytes of a steady-state step (block tables travel only when a page was added)."""
-        return 3 * self.B * 4
+        return 3 * self.rows * 4
 
     # ------------------------------------------------------------------ steps --
     def step(self, tokens, offsets, caches):
@@ -601,6 +624,63 @@ class DecodeEngine(_GraphEngine):
         cur.wait_stream(self._stream)
         self.graph_replays += steps
         return self.out_log[: steps * B].view(steps, B)
+
+
+class VerifyEngine(DecodeEngine):
+    """The verify pass of speculative decoding as one CUDA graph: ``T`` (2..8) consecutive tokens of ONE request, i.e.
+    ``T`` decode steps in a single pass over the weights.  Metadata block: ``tokens [T] | offsets [T] | context_lens [T]
+    | block tables [Ly, 1, MP]``, row j at position ``ctx0 + j`` with context ``ctx0 + j + 1``.
+
+    It runs the B = 1 decode step's launches at M = T: embedding, the matvec layer stack with the T-row fused attention
+    (``decode_attention_fused(rows_per_request=T)``), the RMSNorm-prologue head and argmax.  The streaming projections
+    compute every row as they do alone and the attention row j as the decode step with rows < j appended, so logits,
+    argmax and the appended K/V equal, bit for bit, T successive B = 1 decode steps at the same ``max_seq_len``.  The
+    host bookkeeping is ``DecodeEngine``'s (one slot, ``_advance_host(caches, T)``)."""
+
+    def __init__(self, model, rows: int, max_seq_len: int, device):
+        if not 2 <= rows <= 8:
+            raise ValueError("the verify step takes 2 to 8 rows")
+        if not VerifyEngine.supported(model, device, max_seq_len):
+            raise ValueError("the verify step needs the B = 1 decode step's fused matvec + fused attention path")
+        super().__init__(model, 1, max_seq_len, device, rows_per_request=rows)
+        self.T = rows
+        assert self.fused and self._attention_fused and self._variants == [1]
+
+    @staticmethod
+    def supported(model, device, max_seq_len: int) -> bool:
+        """Where the B = 1 decode engine itself runs fused matvec + fused attention."""
+        return torch.device(device).type == "cuda" and DecodeEngine.fused_attention_applies(model, max_seq_len)
+
+    def reserve_pools(self, pages_per_layer: int | None = None) -> None:
+        raise RuntimeError("the verify step shares the B = 1 decode engine's pool reservation")
+
+    def step(self, tokens, offsets, caches):
+        raise TypeError("a verify engine runs verify(), not decode steps")
+
+    def decode_on_device(self, tokens, offsets, caches, steps: int):
+        raise TypeError("a verify engine runs verify(), not decode steps")
+
+    def verify(self, token: int, proposals, offset: int, caches):
+        """Append ``[token, *proposals]`` (T ids at positions ``offset``..; ``proposals`` a list, or an int32 device tensor
+        that never visits the host) to the request's caches and return (logits [T, V] static buffer, greedy next token
+        per row [T])."""
+        T = self.T
+        self._host_write_begin()
+        self._advance_host(caches, T)
+        self._ensure_graph()
+        on_device = isinstance(proposals, torch.Tensor)
+        self.meta_np[0] = token
+        if not on_device:
+            self.meta_np[1:T] = proposals
+        pos = np.arange(T, dtype=np.int32) + offset
+        self.meta_np[T : 2 * T] = pos
+        self.meta_np[2 * T : 3 * T] = pos + 1
+        self._upload()
+        if on_device:
+            self.tokens[1:].copy_(proposals.reshape(-1).to(torch.int32), non_blocking=True)
+        self._graph.replay()
+        self.graph_replays += 1
+        return self.logits, self.next_tokens
 
 
 class PrefillEngine(_GraphEngine):

@@ -241,6 +241,7 @@ class Qwen3ModelWeek3:
         # default prefill_step) once a decode engine exists, i.e. once the page slabs have been reserved.
         self.prefill_graph_len: int | None = None
         self._prefill_engines: dict = {}
+        self._verify_engines: dict = {}
         self._packed_layers: list | None = None
         self._paged = enable_paged_attention
 
@@ -270,6 +271,28 @@ class Qwen3ModelWeek3:
             engine.reserve_pools((batch_size + 1) * engine.max_pages + 1)
             self._decode_engines[key] = engine
         return self._decode_engines[key]
+
+    def verify_applies(self, device=None) -> bool:
+        """Whether ``verify_engine`` runs on this model: CUDA paged caches and the shapes of the fused decode path."""
+        from .engine import VerifyEngine
+
+        dev = device if device is not None else self.embedding.weight.scales.device
+        return (self._paged and self.use_decode_graph is not False and torch.device(dev).type == "cuda"
+                and VerifyEngine.supported(self, dev, self.decode_graph_max_seq_len))
+
+    def verify_engine(self, rows: int, device=None):
+        """The (cached) graph of one speculative verify pass over ``rows`` tokens of one request (``engine.VerifyEngine``).
+        It uses the ``max_seq_len`` of the B = 1 decode engine that ``model(...)`` runs a single request with (so the
+        attention splits match) and that engine's page reservation (the slabs do not move when the two alternate)."""
+        from .engine import VerifyEngine
+
+        limit = self.decode_graph_max_seq_len
+        key = (rows, limit)
+        if key not in self._verify_engines:
+            dev = device if device is not None else self.embedding.weight.scales.device
+            self.decode_engine(1, limit, dev)
+            self._verify_engines[key] = VerifyEngine(self, rows, limit, dev)
+        return self._verify_engines[key]
 
     def _graph_decode_applies(self, inputs, cache) -> bool:
         if self.use_decode_graph is False or not self._paged or inputs.dim() != 2 or inputs.shape[1] != 1 or not inputs.is_cuda:
