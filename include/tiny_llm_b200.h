@@ -180,6 +180,15 @@ int tl_add(const void *a, const void *b, void *out, long long size, int dtype, v
 int tl_argmax(const void *logits, int32_t *out_tokens, int rows, int vocab, int dtype, void *workspace,
               size_t workspace_bytes, void *stream);
 size_t tl_argmax_workspace(int rows, int vocab);
+/* Seeded sampling of one token per row of logits [rows, vocab] (rows <= 65535, vocab <= 409,600), parameters per row
+ * as device arrays: temperature f32, top_k i32 (on when 0 < k < vocab), top_p f32 (on when 0 < p < 1), seed i64 and
+ * positions i32 (the index of the token being drawn).  temperature == 0, or a row whose maximum is not finite, returns
+ * tl_argmax's token.  Otherwise the token is argmax over the keep set {x >= max(x_(k), v*)} of
+ * x / temperature - log(-log u), u from Philox4x32-10 at counter (i >> 2, position, 0, 0) and key (seed low word,
+ * seed high word), word i % 4 (DESIGN.md section 8): a pure function of (row, parameters, seed, position).
+ * No workspace; deterministic. */
+int tl_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+              const int32_t *positions, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
 /* Fused W4A16 projection for the decode hot loop: the weight-streaming kernel of
  * tl_quantized_matmul with the neighbouring element-wise operator folded in.
  * Rounding points are those of the unfused call sequence, so results are

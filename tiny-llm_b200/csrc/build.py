@@ -34,6 +34,7 @@ SOURCES = [
     "attention_prefill.cu",
     "attention_prefill_tc.cu",
     "decode_attention_fused.cu",
+    "sampling.cu",
     "tma.cu",
 ]
 

@@ -346,6 +346,16 @@ int tl_argmax(const void *logits, int32_t *out_tokens, int rows, int vocab, int 
     return launch_argmax(logits, out_tokens, rows, vocab, dtype, workspace, workspace_bytes, as_stream(stream));
 }
 
+int tl_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+              const int32_t *positions, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample: bad shape");
+    if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
+    if (rows == 0) return TL_OK;
+    if (!logits || !temperature || !top_k || !top_p || !seed || !positions || !out_tokens) return fail(TL_EINVAL, "sample: null pointer");
+    return launch_sample(logits, temperature, top_k, top_p, seed, positions, out_tokens, rows, vocab, dtype, as_stream(stream));
+}
+
 int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, const void *a, const void *b,
                               const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass, int *units) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");

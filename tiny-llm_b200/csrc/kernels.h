@@ -34,6 +34,11 @@ size_t argmax_workspace(int rows, int vocab);
 int launch_argmax(const void *logits, int32_t *out, int rows, int vocab, int dtype, void *ws, size_t ws_bytes,
                   cudaStream_t st);
 
+// sampling.cu: cluster size and fp32 entries per CTA for a row of `vocab` (TL_EINVAL beyond the staging limit)
+int sample_plan(int vocab, int *cluster, int *slice);
+int launch_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                  const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+
 int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                           int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, cudaStream_t st);
 

@@ -42,6 +42,7 @@ __all__ = [
     "paged_cache_append_decode",
     "add",
     "argmax",
+    "sample",
     "decode_advance",
     "quantized_matmul_fused",
     "quantized_matmul_route",
@@ -91,6 +92,7 @@ _SIGNATURES = {
     "tl_argmax_workspace": (_SZ, [_I, _I]),
     "tl_argmax": (_I, [_VP, _VP, _I, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
+    "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
     "tl_quantized_matmul_fused_workspace": (_SZ, [_I] * 6),
@@ -598,6 +600,25 @@ def argmax(logits, stream=None):
     ws = _workspace(ws_bytes, logits.device)
     _check(_lib.tl_argmax(logits.data_ptr(), out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype],
                           None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, logits)))
+    return out
+
+
+def sample(logits, temperature, top_k, top_p, seed, positions, stream=None):
+    """Seeded token per row of ``logits [rows, vocab]`` -> int32 ``[rows]`` (``tl_sample``).  Per-row device arrays:
+    ``temperature`` float32 (0: greedy, ``argmax``'s token), ``top_k`` int32 (on for 0 < k < vocab), ``top_p`` float32
+    (on for 0 < p < 1), ``seed`` int64 and ``positions`` int32, the index of the token being drawn."""
+    if logits.dtype not in _FLOATS or logits.dim() != 2:
+        raise RuntimeError("sample: expected 2D float logits")
+    rows = logits.shape[0]
+    for name, t, dtype in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+                           ("seed", seed, torch.int64), ("positions", positions, torch.int32)):
+        if t.dtype != dtype or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"sample: {name} must be {str(dtype).replace('torch.', '')} [{rows}]")
+    _contig("sample", logits=logits, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, positions=positions)
+    _gpu("sample", logits, temperature, top_k, top_p, seed, positions)
+    out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
+    _check(_lib.tl_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(), positions.data_ptr(),
+                          out.data_ptr(), rows, logits.shape[1], _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
 
 

@@ -14,7 +14,7 @@ from .layer_norm import RMSNorm
 from .models import dispatch_model, shortcut_name_to_full_name
 from .paged_kv_cache import PagedKvMetadata, TinyKvPagedCache, TinyKvPagedPool
 from .positional_encoding import RoPE
-from .sampler import make_sampler
+from .sampler import SamplingParams, make_sampler
 from .quantize import (
     QuantizedWeights,
     dequantize_linear,

@@ -23,6 +23,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200
 
 from .kv_cache import BatchingKvCache
+from .sampler import sample_tokens, sampling_per_request
 
 
 def greedy_tokens(logits: torch.Tensor) -> torch.Tensor:
@@ -60,7 +61,9 @@ class Request:
 
     ``prompt`` is a string (encoded with ``tokenizer``) or, for synthetic
     serving runs, a sequence of token ids (``tokenizer`` may then be ``None``;
-    pass ``eos_token_id`` explicitly if one is wanted)."""
+    pass ``eos_token_id`` explicitly if one is wanted).  ``sampling`` (a
+    ``SamplingParams``) draws the request's tokens with the seeded ``tl_sample``
+    kernel; None keeps them greedy."""
 
     def __init__(
         self,
@@ -72,8 +75,10 @@ class Request:
         max_seq_len: int | None = None,
         eos_token_id: int | None = None,
         device=None,
+        sampling=None,
     ):
         self.prompt = prompt
+        self.sampling = sampling
         self.model = model
         if isinstance(prompt, str):
             ids = tokenizer.encode(prompt, add_special_tokens=False)
@@ -104,7 +109,12 @@ class Request:
             raise ValueError("prefill called after done")
         total = self.prefill_tokens.numel()
         chunk = min(self.prefill_max_step, total - self.offset)
-        token = _step(self.model, self.prefill_tokens[self.offset : self.offset + chunk][None], [self.offset], self.kv_cache)
+        ids = self.prefill_tokens[self.offset : self.offset + chunk][None]
+        if self.sampling is None:
+            token = _step(self.model, ids, [self.offset], self.kv_cache)
+        else:  # only the last chunk's token is used: the prompt's first token is drawn at position `total`
+            logits = self.model(ids, [self.offset], self.kv_cache, logits_to_keep=1)[:, -1, :]
+            token = sample_tokens(logits, [self.sampling], [total]) if self.offset + chunk == total else None
         self.offset += chunk
         for layer_cache in self.kv_cache:
             layer_cache.materialize()
@@ -161,10 +171,13 @@ def _print_progress(slots, pending, queued: int, tick: int, started: datetime):
 
 
 class ContinuousBatcher:
-    """The reference scheduling loop as a steppable object."""
+    """The reference scheduling loop as a steppable object.  ``sampling``: None (greedy, the reference's loop), one
+    ``SamplingParams`` for every prompt or a list with one per prompt; a request's tokens are then drawn by the seeded
+    ``tl_sample`` kernel from its last prefill chunk's and every decode step's logits, and do not depend on its slot or
+    on the other requests."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
-                 eos_token_id=None, device=None, max_new_tokens=None):
+                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None):
         if max_seq_len <= 0:
             raise ValueError("max_seq_len must be positive")
         if batch_size <= 0:
@@ -174,6 +187,7 @@ class ContinuousBatcher:
         self.model = model
         self.tokenizer = tokenizer
         self.queue = list(prompts)
+        self.sampling = sampling_per_request(sampling, len(self.queue))
         self.max_seq_len = max_seq_len
         self.batch_size = batch_size
         self.prefill_step = prefill_step
@@ -250,6 +264,7 @@ class ContinuousBatcher:
             self.pending = Request(
                 self.model, self.tokenizer, prompt, self.prefill_step, self.next_request_idx,
                 max_seq_len=self.max_seq_len, eos_token_id=self.eos_token_id, device=self.device,
+                sampling=None if self.sampling is None else self.sampling[self.next_request_idx],
             )
             self.next_request_idx += 1
 
@@ -297,7 +312,11 @@ class ContinuousBatcher:
             t0 = time.perf_counter() if self.record_timing else 0.0
             span = self._gpu_span("decode")
             batch = torch.tensor(tokens, dtype=torch.int32, device=self.device).reshape(-1, 1)
-            sampled = _step(self.model, batch, offsets, self.kv_cache)
+            if self.sampling is None:
+                sampled = _step(self.model, batch, offsets, self.kv_cache)
+            else:  # slot i draws the token at position offset + 1; idle and greedy slots get argmax's token
+                logits = self.model(batch, offsets, self.kv_cache, logits_to_keep=1)[:, -1, :]
+                sampled = sample_tokens(logits, [None if s is None else s.sampling for s in self.slots], [o + 1 for o in offsets])
             if span is not None:
                 span.record()
             host = sampled.reshape(-1).tolist()  # one device->host read per step

@@ -6,6 +6,8 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli generate --model /path/to/Qwen3-4B-MLX-4bit --prompt "..." [--loader week3]
     python -m tiny_llm_b200.cli batch    --model /path/to/ckpt --prompts-file prompts.txt --batch-size 5
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --max-new-tokens 8   (no files needed)
+    python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3;9,2,4" --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
+        (seeded sampling with the tl_sample kernel: the same seed gives the same tokens)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
 """
@@ -53,13 +55,18 @@ def _prompt_ids(args, tokenizer, prompt: str | None):
 
 def cmd_generate(args) -> int:
     from .generate import greedy_generate_ids
-    from .sampler import make_sampler
+    from .sampler import SamplingParams, make_sampler
 
     device = torch.device(args.device)
     ns, tokenizer, name = _load(args, device)
     model = _model(args, ns, name)
     ids = _prompt_ids(args, tokenizer, args.prompt)
-    sampler = None if args.sampler_temp == 0 else make_sampler(args.sampler_temp, top_p=args.sampler_top_p, top_k=args.sampler_top_k)
+    sampler = sampling = None
+    if args.sampler_temp != 0:
+        if device.type == "cuda":  # the seeded kernel
+            sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed)
+        else:
+            sampler = make_sampler(args.sampler_temp, top_p=args.sampler_top_p, top_k=args.sampler_top_k)
     if tokenizer is not None:
         tokenizer.detokenizer.reset()
 
@@ -74,7 +81,7 @@ def cmd_generate(args) -> int:
     if args.draft_model or args.draft_synthetic:
         from .generate import speculative_generate_ids
 
-        if sampler is not None:
+        if sampler is not None or sampling is not None:
             raise SystemExit("speculative decoding is greedy: drop --sampler-temp")
         if args.draft_model and args.draft_synthetic:
             raise SystemExit("give one draft: --draft-model or --draft-synthetic, not both")
@@ -91,13 +98,14 @@ def cmd_generate(args) -> int:
         print()
         return 0
     produced = greedy_generate_ids(model, ids, args.max_new_tokens, eos_token_id=eos, device=device,
-                                   on_token=emit, sampler=sampler)
+                                   on_token=emit, sampler=sampler, sampling=sampling)
     print()
     return 0 if produced is not None else 1
 
 
 def cmd_batch(args) -> int:
     from .batch import batch_generate
+    from .sampler import SamplingParams
 
     device = torch.device(args.device)
     ns, tokenizer, name = _load(args, device)
@@ -111,8 +119,13 @@ def cmd_batch(args) -> int:
     else:
         queue = [tokenizer.apply_chat_template([{"role": "user", "content": p}], tokenize=False, add_generation_prompt=True,
                                                enable_thinking=args.enable_thinking) for p in prompts]
+    sampling = None
+    if args.sampler_temp != 0:  # request i draws with seed `--seed + i`
+        sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i)
+                    for i in range(len(queue))]
     results = batch_generate(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
-                             verbose=not args.quiet, device=device, max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None)
+                             verbose=not args.quiet, device=device, max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None,
+                             sampling=sampling)
     for idx, text in sorted(results):
         print(f"--- request {idx}\n{text}")
     return 0
@@ -133,9 +146,11 @@ def main(argv=None) -> int:
         p.add_argument("--disable-paged-attention", action="store_true")
         p.add_argument("--enable-thinking", action="store_true")
         p.add_argument("--max-new-tokens", type=int, default=128)
-    sub.choices["generate"].add_argument("--sampler-temp", type=float, default=0.0)
-    sub.choices["generate"].add_argument("--sampler-top-p", type=float, default=None)
-    sub.choices["generate"].add_argument("--sampler-top-k", type=int, default=None)
+    for name in ("generate", "batch"):
+        sub.choices[name].add_argument("--sampler-temp", type=float, default=0.0)
+        sub.choices[name].add_argument("--sampler-top-p", type=float, default=None)
+        sub.choices[name].add_argument("--sampler-top-k", type=int, default=None)
+        sub.choices[name].add_argument("--seed", type=int, default=0, help="seed of the sampled draw on CUDA (`batch`: request i uses seed + i)")
     sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
     sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")
     sub.choices["generate"].add_argument("--proposal-length", type=int, default=4, help="draft tokens proposed per round")

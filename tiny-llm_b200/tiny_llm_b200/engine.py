@@ -17,7 +17,9 @@ The engine keeps the operator semantics and removes the dispatch:
   (``append_token_slot``), so block tables, page ids and counters are identical;
 * ``decode_on_device`` runs N greedy steps with no host involvement at all
   (token feedback + position advance by ``tl_decode_advance``, pages allocated
-  ahead) - the device-resident number of bench.py.
+  ahead) - the device-resident number of bench.py.  With ``sampling`` it replays
+  a second self-advancing graph that draws each slot's token with the seeded
+  ``tl_sample`` kernel instead of ``tl_argmax``.
 
 Page slabs must not move while a graph is alive: pools are ``reserve()``d up
 front and the engine re-captures if a slab pointer changes.
@@ -282,6 +284,17 @@ class DecodeEngine(_GraphEngine):
         self._variants = sorted({r for r in (16, 32, 64) if r < self.B} | {self.B}) if (self.fused and self.B > 16 and _row_variants) else [self.B]
         self._graphs: dict = {}
         self.variant_replays = {r: 0 for r in self._variants}
+        # decode_on_device(sampling=...): per-slot parameters in their own pinned block (seed i64 | temperature f32 |
+        # top_k i32 | top_p f32, B each), uploaded only when they change; the sampled graph is captured on first use
+        self._graph_sample = None
+        self.kernels_per_sampled_step = 0
+        self._samp_host = torch.zeros(20 * B, dtype=torch.uint8, pin_memory=True)
+        self._samp_dev = self._samp_host.to(self.device, copy=True)
+        self._samp_key = None
+        self._samp_seed = self._samp_dev[: 8 * B].view(torch.int64)
+        self._samp_temperature = self._samp_dev[8 * B : 12 * B].view(torch.float32)
+        self._samp_top_k = self._samp_dev[12 * B : 16 * B].view(torch.int32)
+        self._samp_top_p = self._samp_dev[16 * B : 20 * B].view(torch.float32)
 
     @staticmethod
     def fused_attention_applies(model, slot_tokens: int) -> bool:
@@ -296,7 +309,17 @@ class DecodeEngine(_GraphEngine):
         super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
 
     # ------------------------------------------------------------ graph body --
-    def _forward_unfused(self) -> None:
+    def _next_tokens(self, logits, R: int, sampled: bool) -> None:
+        """The step's token per row: ``tl_argmax``, or (the sampled graph) ``tl_sample`` with the per-slot parameters at
+        position ``context_lens``, the index of the token being drawn."""
+        if sampled:
+            tokens = ext.sample(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
+                                self.context_lens[:R])
+        else:
+            tokens = ext.argmax(logits)
+        self.next_tokens[:R].copy_(tokens)
+
+    def _forward_unfused(self, sampled: bool = False) -> None:
         """One decode step over the static buffers, operator by operator (the
         call sequence of qwen3_week3.py:55-121,139-146,196-207,320-338 at L == 1)."""
         m = self.model
@@ -325,12 +348,12 @@ class DecodeEngine(_GraphEngine):
         x = _normed(x, m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
         logits = _proj(x, head)
-        self.next_tokens.copy_(ext.argmax(logits))
+        self._next_tokens(logits, B, sampled)
         if self.logits is None:
             self.logits = torch.empty_like(logits)
         self.logits.copy_(logits)
 
-    def _forward_fused(self, rows: int | None = None) -> None:
+    def _forward_fused(self, rows: int | None = None, sampled: bool = False) -> None:
         """Same step in ~7 launches per layer: norm / SwiGLU / residual folded into
         the streaming projections, q/k norm + RoPE + K/V append in one kernel.
         Every rounding point of the operator-by-operator sequence is kept.
@@ -347,7 +370,7 @@ class DecodeEngine(_GraphEngine):
             x = self._matvec_layers(x)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
-        self.next_tokens[:R].copy_(ext.argmax(logits))
+        self._next_tokens(logits, R, sampled)
         if self.logits is None:
             self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
@@ -417,6 +440,7 @@ class DecodeEngine(_GraphEngine):
 
         self._graph = self._graph_of(forward)
         self._graphs = {self.B: self._graph}
+        self._graph_sample = None  # captured again on first use, over the current slabs
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -427,6 +451,47 @@ class DecodeEngine(_GraphEngine):
         for rows in self._variants:
             if rows != self.B:  # the warm-ups run with the metadata still all-idle: the narrower kernels set their attributes lazily
                 self._graphs[rows] = self._graph_of(lambda: forward(rows), pool=self._graph.pool())
+
+    def _ensure_sample_graph(self) -> None:
+        """Capture the sampled self-advancing step (after ``_ensure_graph``, before the metadata upload: the warm-up
+        runs over all-idle metadata, as every capture does)."""
+        if self._graph_sample is not None:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def sampled_step():
+            forward(sampled=True)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self._graph_sample = self._graph_of(sampled_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_sampled_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_sampling(self, sampling) -> None:
+        """Write the per-slot parameters into their pinned block (one ``SamplingParams`` for all slots or one per
+        slot, None: greedy) and upload it if they changed."""
+        from .sampler import SamplingParams, sampling_tensors
+
+        B = self.B
+        per = [sampling] * B if isinstance(sampling, SamplingParams) else list(sampling)
+        if len(per) != B or not all(p is None or isinstance(p, SamplingParams) for p in per):
+            raise ValueError(f"sampling must be one SamplingParams or a list of {B} (one per slot)")
+        key = tuple(per)
+        if key == self._samp_key:
+            return
+        self._host_write_begin()
+        temperature, top_k, top_p, seed = (t.numpy() for t in sampling_tensors(per, "cpu"))
+        host = self._samp_host.numpy()
+        host[: 8 * B] = seed.view(np.uint8)
+        host[8 * B : 12 * B] = temperature.view(np.uint8)
+        host[12 * B : 16 * B] = top_k.view(np.uint8)
+        host[16 * B : 20 * B] = top_p.view(np.uint8)
+        self._upload_meta(self._samp_dev, self._samp_host)
+        self.h2d_bytes += 20 * B
+        self._samp_key = key
 
     # ------------------------------------------------------- host bookkeeping --
     def _slot_caches(self, caches, layer: int):
@@ -601,26 +666,32 @@ class DecodeEngine(_GraphEngine):
         self.graph_replays += 1
         return self.logits.view(B, 1, self.V), self.next_tokens
 
-    def decode_on_device(self, tokens, offsets, caches, steps: int) -> torch.Tensor:
+    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None) -> torch.Tensor:
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
-        back to back.  Returns the sampled tokens ``[steps, B]`` (device)."""
+        back to back.  Returns the sampled tokens ``[steps, B]`` (device).
+        ``sampling`` (one ``SamplingParams`` or one per slot, None entries greedy) replays the sampled graph instead:
+        slot b's token at position p is ``tl_sample``'s draw with its parameters, p = its offset + 1."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         B = self.B
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
+        if sampling is not None:
+            self._ensure_sample_graph()
+            self._set_sampling(sampling)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
+        graph = self._graph_loop if sampling is None else self._graph_sample
         cur = torch.cuda.current_stream(self.device)
         self._stream.wait_stream(cur)
         with torch.cuda.stream(self._stream):
             self._upload()
             self.step_counter.zero_()
             for i in range(steps):
-                self._graph_loop.replay()
+                graph.replay()
         cur.wait_stream(self._stream)
         self.graph_replays += steps
         return self.out_log[: steps * B].view(steps, B)

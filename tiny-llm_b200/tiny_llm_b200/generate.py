@@ -6,6 +6,7 @@ from __future__ import annotations
 import torch
 
 from .batch import greedy_tokens
+from .sampler import sample_tokens
 
 
 def _release_kv_cache(kv_cache) -> None:
@@ -14,12 +15,17 @@ def _release_kv_cache(kv_cache) -> None:
             layer_cache.release()
 
 
-def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: int | None = None, device=None, on_token=None, sampler=None):
+def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: int | None = None, device=None, on_token=None, sampler=None,
+                        sampling=None):
     """The loop of ``simple_generate_with_kv_cache`` on token ids: the whole
     prompt is prefilled at offset 0 (its last-row logits give the first token),
     then one token per step at a growing offset.  Returns the generated ids.
     ``sampler`` (``make_sampler``; CUDA extension - the reference's cached loop is greedy only) draws
-    from ``logits - logsumexp`` instead of taking the arg-max."""
+    from ``logits - logsumexp`` instead of taking the arg-max.  ``sampling`` (a ``SamplingParams``) draws each token
+    with the seeded ``tl_sample`` kernel instead, at its position in the sequence: the ids equal a prefill plus
+    ``DecodeEngine.decode_on_device(sampling=...)``."""
+    if sampler is not None and sampling is not None:
+        raise ValueError("give sampler or sampling, not both")
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
     try:
@@ -27,7 +33,9 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
         offset = 0
         while len(produced) < max_new_tokens:
             logits = model(tokens[None], offset, kv_cache, logits_to_keep=1)
-            if sampler is None:
+            if sampling is not None:
+                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()])
+            elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])
             else:
                 row = logits[:, -1, :].to(torch.float32)

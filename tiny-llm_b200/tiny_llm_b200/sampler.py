@@ -8,6 +8,10 @@ reproducible."""
 
 from __future__ import annotations
 
+import math
+import numbers
+from dataclasses import dataclass
+
 import torch
 
 
@@ -29,3 +33,68 @@ def make_sampler(temp: float, top_p: float | None = None, top_k: int | None = No
         return torch.multinomial(probs, 1, generator=generator).squeeze(-1)
 
     return sample
+
+
+@dataclass(frozen=True)
+class SamplingParams:
+    """One request's seeded sampling on the CUDA path (``tl_sample``, DESIGN.md section 8).  ``temperature == 0`` is
+    greedy, the ``argmax`` token.  Otherwise the token is drawn from ``softmax(logits / temperature)`` restricted to the
+    keep set of ``top_k`` (on for ``0 < top_k < vocab``; ties at the k-th value are kept) and ``top_p`` (on for
+    ``0 < top_p < 1``; a token is kept while the probability mass strictly above it is ``< top_p``).  The draw is a pure
+    function of (logits row, parameters, ``seed``, position of the drawn token): the same request gives the same tokens
+    in any batch, slot or engine."""
+
+    temperature: float
+    top_k: int | None = None
+    top_p: float | None = None
+    seed: int = 0
+
+    def __post_init__(self):
+        t = self.temperature
+        if isinstance(t, bool) or not isinstance(t, numbers.Real) or not math.isfinite(t) or t < 0:
+            raise ValueError(f"temperature must be a finite number >= 0, got {t!r}")
+        k = self.top_k
+        if k is not None and (isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 0):
+            raise ValueError(f"top_k must be None or an int >= 0, got {k!r}")
+        p = self.top_p
+        if p is not None and (isinstance(p, bool) or not isinstance(p, numbers.Real) or not math.isfinite(p)):
+            raise ValueError(f"top_p must be None or a finite number, got {p!r}")
+        s = self.seed
+        if isinstance(s, bool) or not isinstance(s, numbers.Integral) or not 0 <= s < 1 << 64:
+            raise ValueError(f"seed must be an int in [0, 2**64), got {s!r}")
+
+
+GREEDY = SamplingParams(0.0)
+
+
+def sampling_per_request(sampling, n: int) -> list | None:
+    """``sampling`` as given to the batcher (None, one ``SamplingParams`` or one per request) -> None or a list of
+    ``n`` entries."""
+    if sampling is None:
+        return None
+    if isinstance(sampling, SamplingParams):
+        return [sampling] * n
+    per = list(sampling)
+    if len(per) != n or not all(isinstance(p, SamplingParams) for p in per):
+        raise ValueError(f"sampling must be one SamplingParams or a list of {n} (one per prompt)")
+    return per
+
+
+def sampling_tensors(params, device) -> tuple[torch.Tensor, ...]:
+    """The per-row device arrays of ``ext.sample`` (temperature, top_k, top_p, seed) for a list of ``SamplingParams``
+    (None: greedy)."""
+    params = [GREEDY if p is None else p for p in params]
+    return (torch.tensor([float(p.temperature) for p in params], dtype=torch.float32, device=device),
+            torch.tensor([min(p.top_k or 0, (1 << 31) - 1) for p in params], dtype=torch.int32, device=device),
+            torch.tensor([0.0 if p.top_p is None else float(p.top_p) for p in params], dtype=torch.float32, device=device),
+            torch.tensor([p.seed - (1 << 64) if p.seed >= 1 << 63 else p.seed for p in params], dtype=torch.int64, device=device))
+
+
+def sample_tokens(logits: torch.Tensor, params, positions) -> torch.Tensor:
+    """One seeded token per row of ``logits [rows, vocab]`` with the ``tl_sample`` kernel; ``params`` one
+    ``SamplingParams`` (or None: greedy) per row, ``positions`` the index of each drawn token -> int32 ``[rows]``."""
+    from extensions_b200 import tiny_llm_ext_b200 as ext
+
+    temperature, top_k, top_p, seed = sampling_tensors(params, logits.device)
+    pos = torch.as_tensor(positions, dtype=torch.int32).to(logits.device)
+    return ext.sample(logits.contiguous(), temperature, top_k, top_p, seed, pos)
