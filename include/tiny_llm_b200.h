@@ -300,6 +300,48 @@ int tl_decode_attention_fused_rows(const void *qkv, const void *q_norm_weight, c
                                    float *workspace, int batch, int rows_per_request, int num_heads, int num_kv_heads,
                                    int head_dim, float eps, float scale, int num_pages, int page_size, int max_pages,
                                    int max_context, int dtype, void *stream);
+/* ---- Qwen3-MoE sparse block (moe.py:36-89 of the reference) ----------------
+ * One layer runs: router projection (tl_quantized_matmul*), tl_moe_topk, tl_moe_group, tl_moe_gather,
+ * tl_moe_grouped_matmul (gate|up, EPI_SWIGLU_PAIRS, sorted output), tl_moe_grouped_matmul (down, scattered back to
+ * the original row order with out_index = perm), tl_moe_combine.  All are capture-safe: outputs are sized by
+ * R = T * k rows and E experts, nothing synchronises and no count is read by the host.  Rounding (DESIGN.md):
+ *   probs = T(softmax_fp32(logits)); ids = the k largest probs, descending, ties to the lower id; scores = probs[ids],
+ *   with norm: T(score / T(sum_fp32 scores in slot order)); expert outputs rounded to T; SwiGLU rounded once;
+ *   r = T(sum_fp32 over slots of T(y_j * score_j)); x' = T(x + r).
+ * A row's result depends only on that row. */
+#define TL_MOE_MAX_EXPERTS 256
+#define TL_MOE_MAX_TOPK 8
+/* logits [T, E] -> probs [T, E] (dtype of logits), ids int32 [T, k], scores [T, k].  E <= 256, 1 <= k <= min(8, E). */
+int tl_moe_topk(const void *logits, void *probs, int32_t *ids, void *scores, int T, int E, int k, int norm_topk_prob, int dtype, void *stream);
+/* ids int32 [R] (each in [0, E); others are clamped) -> offsets int32 [E + 1] (segment of expert e in sorted order),
+ * perm int32 [R] (sorted position -> row, stable within an expert) and, with nt > 0, the tile table of the grouped
+ * GEMM: tiles int32 [tl_moe_tile_table_size(R, E, nt)] = {count, (expert, first sorted row) x count}, one entry per
+ * nt-row piece of each expert's segment, experts in order. */
+int tl_moe_group(const int32_t *ids, int R, int E, int nt, int32_t *offsets, int32_t *perm, int32_t *tiles, void *stream);
+int tl_moe_tile_table_size(int R, int E, int nt);
+/* xs[j] = x[perm[j] / rows_per_source] for j < R; x [R / rows_per_source, H].  With norm_weight: the row's RMSNorm
+ * T(x * rsqrt(mean(x^2) + eps) * w). */
+int tl_moe_gather(const void *x, const int32_t *perm, const void *norm_weight, float eps, void *xs, int R, int rows_per_source, int H, int dtype,
+                  void *stream);
+/* Grouped W4A16 projection of R = T * k expert-sorted rows a [R, N] by the experts b [E K, N / 8], scales / biases
+ * [E K, N / 128]: row j uses expert e with offsets[e] <= j < offsets[e + 1].  out [R, K] (EPI_NONE) or [R, K / 2]
+ * (EPI_SWIGLU_PAIRS over each expert's interleaved gate|up rows), row j stored at out_index[j] when out_index is given,
+ * else at j.  tiles: tl_moe_group's table for the nt tl_moe_grouped_matmul_route reports (unused on the control route). */
+int tl_moe_grouped_matmul(const void *scales, const void *biases, const void *b, const void *a, void *out, const int32_t *offsets,
+                          const int32_t *tiles, const int32_t *out_index, int T, int k, int E, int N, int K, int epilogue, int dtype, void *stream);
+/* The kernel tl_moe_grouped_matmul runs (nothing is launched or read; a and b only count for their alignment):
+ *   TL_MOE_WGMMA   : the swap-AB wgmma kernel, one CTA = 128 features of one expert x nt sorted rows, no split;
+ *                    16-bit dtype, K % 128 == 0, a and b 16-byte aligned.  nt = the smallest of 16 / 32 / 64 / 128 at
+ *                    least ceil(T k / E); *max_tiles = the CTA rows launched;
+ *   TL_MOE_CONTROL : the scalar control kernel (one thread per output); *nt = *max_tiles = 0.
+ * or a negative TL_E* code for arguments the launch rejects. */
+enum { TL_MOE_CONTROL = 0, TL_MOE_WGMMA = 1 };
+int tl_moe_grouped_matmul_route(int T, int k, int E, int N, int K, int epilogue, int dtype, const void *a, const void *b, int *nt, int *max_tiles);
+/* out [T, H] = T(residual + T(sum_fp32 over j < k of T(y[t k + j] * scores[t, j]))) (no residual: the sum alone);
+ * y [T k, H] in original row order.  With norm_weight, normed_out = the RMSNorm of out (H <= 4096). */
+int tl_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_weight, float eps, void *out, void *normed_out,
+                   int T, int k, int H, int dtype, void *stream);
+
 /* Programmatic dependent launch for the streaming kernels (on by default; 0 turns it off,
  * TL_PDL=0 in the environment does the same). */
 int tl_set_pdl(int enabled);

@@ -559,4 +559,89 @@ int tl_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offs
                                  as_stream(stream));
 }
 
+// ------------------------------------------------------------- Qwen3-MoE --
+static int moe_shape(const char *op, int T, int k, int E) {
+    if (T < 0 || E <= 0 || k <= 0) return fail(TL_EINVAL, "%s: bad shape (T = %d, k = %d, E = %d)", op, T, k, E);
+    if (E > TL_MOE_MAX_EXPERTS) return fail(TL_EINVAL, "%s: at most %d experts (got %d)", op, TL_MOE_MAX_EXPERTS, E);
+    if (k > TL_MOE_MAX_TOPK || k > E) return fail(TL_EINVAL, "%s: top-k must be in [1, min(%d, experts)] (got k = %d, E = %d)", op, TL_MOE_MAX_TOPK, k, E);
+    if (static_cast<long long>(T) * k > (1 << 30)) return fail(TL_EINVAL, "%s: too many rows", op);
+    return TL_OK;
+}
+
+// Upper bound of the tiles of R rows over at most min(E, R) non-empty experts: sum ceil(c_e / nt) <= (R + (nt - 1) min(E, R)) / nt.
+static int moe_max_tiles(int R, int E, int nt) { return static_cast<int>((static_cast<long long>(R) + static_cast<long long>(nt - 1) * (E < R ? E : R)) / nt); }
+
+int tl_moe_topk(const void *logits, void *probs, int32_t *ids, void *scores, int T, int E, int k, int norm_topk_prob, int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "moe_topk: expected float32, float16, or bfloat16");
+    if (int e = moe_shape("moe_topk", T, k, E)) return e;
+    if (T == 0) return TL_OK;
+    if (!logits || !probs || !ids || !scores) return fail(TL_EINVAL, "moe_topk: null pointer");
+    return launch_moe_topk(logits, probs, ids, scores, T, E, k, norm_topk_prob != 0, dtype, as_stream(stream));
+}
+
+int tl_moe_tile_table_size(int R, int E, int nt) {
+    if (R < 0 || E <= 0 || E > TL_MOE_MAX_EXPERTS || nt < 0) return fail(TL_EINVAL, "moe_group: bad shape");
+    return nt > 0 ? 1 + 2 * moe_max_tiles(R, E, nt) : 0;
+}
+
+int tl_moe_group(const int32_t *ids, int R, int E, int nt, int32_t *offsets, int32_t *perm, int32_t *tiles, void *stream) {
+    if (R < 0 || E <= 0 || nt < 0) return fail(TL_EINVAL, "moe_group: bad shape (R = %d, E = %d, nt = %d)", R, E, nt);
+    if (E > TL_MOE_MAX_EXPERTS) return fail(TL_EINVAL, "moe_group: at most %d experts (got %d)", TL_MOE_MAX_EXPERTS, E);
+    if (!offsets || (R > 0 && (!ids || !perm)) || (nt > 0 && !tiles)) return fail(TL_EINVAL, "moe_group: null pointer");
+    return launch_moe_group(ids, R, E, nt, offsets, perm, tiles, as_stream(stream));
+}
+
+int tl_moe_gather(const void *x, const int32_t *perm, const void *norm_weight, float eps, void *xs, int R, int rows_per_source, int H, int dtype,
+                  void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "moe_gather: expected float32, float16, or bfloat16");
+    if (R < 0 || rows_per_source <= 0 || H <= 0) return fail(TL_EINVAL, "moe_gather: bad shape");
+    if (R == 0) return TL_OK;
+    if (!x || !perm || !xs) return fail(TL_EINVAL, "moe_gather: null pointer");
+    return launch_moe_gather(x, perm, norm_weight, eps, xs, R, rows_per_source, H, dtype, as_stream(stream));
+}
+
+int tl_moe_grouped_matmul_route(int T, int k, int E, int N, int K, int epilogue, int dtype, const void *a, const void *b, int *nt, int *max_tiles) {
+    if (nt) *nt = 0;
+    if (max_tiles) *max_tiles = 0;
+    if (int e = moe_shape("moe_grouped_matmul", T, k, E)) return e;
+    if (N <= 0 || N % 128 != 0 || K <= 0) return fail(TL_EINVAL, "moe_grouped_matmul: N must be a positive multiple of 128 and K positive");
+    if (epilogue != TL_EPI_NONE && epilogue != TL_EPI_SWIGLU_PAIRS) return fail(TL_EINVAL, "moe_grouped_matmul: epilogue must be none or swiglu pairs");
+    if (epilogue == TL_EPI_SWIGLU_PAIRS && K % 16 != 0) return fail(TL_EINVAL, "moe_grouped_matmul: interleaved gate|up rows need K %% 16 == 0");
+    if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "moe_grouped_matmul: scales must be float16 or bfloat16");
+    const int R = T * k;
+    if (K % 128 != 0 || !aligned16(a) || !aligned16(b)) return TL_MOE_CONTROL;
+    const int per = (R + E - 1) / E;
+    const int n = per <= 16 ? 16 : (per <= 32 ? 32 : (per <= 64 ? 64 : 128));
+    const int tiles = moe_max_tiles(R, E, n);
+    if (tiles > 65535) return TL_MOE_CONTROL;
+    if (nt) *nt = n;
+    if (max_tiles) *max_tiles = tiles;
+    return TL_MOE_WGMMA;
+}
+
+int tl_moe_grouped_matmul(const void *scales, const void *biases, const void *b, const void *a, void *out, const int32_t *offsets,
+                          const int32_t *tiles, const int32_t *out_index, int T, int k, int E, int N, int K, int epilogue, int dtype, void *stream) {
+    int nt = 0, max_tiles = 0;
+    const int route = tl_moe_grouped_matmul_route(T, k, E, N, K, epilogue, dtype, a, b, &nt, &max_tiles);
+    if (route < 0) return route;
+    const int R = T * k;
+    if (R == 0) return TL_OK;
+    if (!scales || !biases || !b || !a || !out || !offsets) return fail(TL_EINVAL, "moe_grouped_matmul: null pointer");
+    if (route == TL_MOE_CONTROL)
+        return launch_moe_grouped_vanilla(scales, biases, a, b, out, offsets, out_index, R, E, N, K, epilogue, dtype, as_stream(stream));
+    if (!tiles) return fail(TL_EINVAL, "moe_grouped_matmul: the wgmma route needs the tile table");
+    return launch_w4a16_grouped(scales, biases, a, b, out, offsets, tiles, out_index, R, E, N, K, epilogue, nt, max_tiles, dtype, as_stream(stream));
+}
+
+int tl_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_weight, float eps, void *out, void *normed_out,
+                   int T, int k, int H, int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "moe_combine: expected float32, float16, or bfloat16");
+    if (T < 0 || k <= 0 || k > TL_MOE_MAX_TOPK || H <= 0) return fail(TL_EINVAL, "moe_combine: bad shape (T = %d, k = %d, H = %d)", T, k, H);
+    if ((norm_weight == nullptr) != (normed_out == nullptr)) return fail(TL_EINVAL, "moe_combine: norm weight and normed output go together");
+    if (norm_weight != nullptr && H > 4096) return fail(TL_EINVAL, "moe_combine: the fused norm takes H <= 4096");
+    if (T == 0) return TL_OK;
+    if (!y || !scores || !out) return fail(TL_EINVAL, "moe_combine: null pointer");
+    return launch_moe_combine(y, scores, residual, norm_weight, eps, out, normed_out, T, k, H, dtype, as_stream(stream));
+}
+
 }  // extern "C"

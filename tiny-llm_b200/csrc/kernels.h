@@ -75,10 +75,23 @@ int launch_w4a16_skinny(const void *scales, const void *biases, const void *a, c
 // workspace, *planes_out = splits) and the caller's fused kernel adds them; *planes_out = 1 means `out` is complete
 int launch_w4a16_tiles(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
                        cudaStream_t st);
+// Grouped expert GEMM over expert-sorted rows (MoE; tl_moe_grouped_matmul): K % 128 == 0, splits == 1
+int launch_w4a16_grouped(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets, const int32_t *tiles,
+                         const int32_t *out_index, int R, int E, int N, int K, int epilogue, int nt, int max_tiles, int dtype, cudaStream_t st);
 bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype);
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,
                                   int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages, cudaStream_t st, bool chunk);
+
+// moe.cu (Qwen3-MoE routing, grouping, gather, combine and the grouped control kernel)
+int launch_moe_topk(const void *logits, void *probs, int32_t *ids, void *scores, int rows, int E, int k, int norm, int dtype, cudaStream_t st);
+int launch_moe_group(const int32_t *ids, int R, int E, int nt, int32_t *offsets, int32_t *perm, int32_t *tiles, cudaStream_t st);
+int launch_moe_gather(const void *x, const int32_t *perm, const void *norm_w, float eps, void *xs, int R, int rows_per_source, int H, int dtype,
+                      cudaStream_t st);
+int launch_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_w, float eps, void *out, void *normed, int T,
+                       int k, int H, int dtype, cudaStream_t st);
+int launch_moe_grouped_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets,
+                               const int32_t *out_index, int R, int E, int N, int K, int epilogue, int dtype, cudaStream_t st);
 
 // decode_attention_fused.cu
 #if defined(TL_TRACE) && TL_TRACE

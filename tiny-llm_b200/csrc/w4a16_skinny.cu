@@ -63,6 +63,9 @@ struct SkArgs {
     int M, N, K;       // tokens, reduction, features
     int splits, gb_per_split;  // reduction split in units of 128-wide group blocks
     int epilogue;
+    // grouped (MoE) form: tile table [count, (expert, first sorted row) x count], expert segments offsets [E + 1], and
+    // optionally the destination row of each sorted row
+    const int32_t *tiles, *offsets, *out_index;
 };
 
 template <typename T>
@@ -78,7 +81,10 @@ struct SkNum<__half> {
     static constexpr uint32_t MAGIC = 0x64006400u;
 };
 
-template <typename T, int NT>
+// GROUPED (MoE experts): the activation rows are sorted by expert; CTA row blockIdx.y is entry blockIdx.y of the tile
+// table (expert e, first sorted row), its weights are rows e K + tile * 128 of the stacked [E K, N / 8] experts, rows
+// past the expert's segment are computed and not stored, and CTAs past the table's count exit.  splits == 1.
+template <typename T, int NT, bool GROUPED = false>
 __global__ void __launch_bounds__(SK_THREADS, 1)
 w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const SkArgs args) {
     using Smem = SkSmem<NT>;
@@ -88,7 +94,7 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x) >> 7, 0);  // warpgroup, provably warp-uniform
     const int tile = blockIdx.x / args.splits, split = blockIdx.x - tile * args.splits;
-    const int m0 = blockIdx.y * NT;  // first token of this CTA
+    int m0 = blockIdx.y * NT;  // first token of this CTA
     const int G = args.N / SK_GB;  // group blocks of the whole reduction = quantisation groups per row
     const int gb0 = min(split * args.gb_per_split, G), gb1 = min(gb0 + args.gb_per_split, G);
     const int n_gb = gb1 - gb0;
@@ -98,6 +104,15 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     // predecessor: barrier init, the packed-weight TMA ring and the dequantisers run ahead of griddep_wait(), i.e. under
     // the predecessor's tail.
     griddep_launch();
+    int m_end = args.M, wrow0 = tile * SK_FEAT;  // rows stored below m_end; first packed-weight row of the tile
+    if constexpr (GROUPED) {
+        griddep_wait();  // the tile table is the predecessor's output, and it names the weights
+        if (static_cast<int>(blockIdx.y) >= ld_cg(args.tiles)) return;
+        const int e = ld_cg(args.tiles + 1 + 2 * blockIdx.y);
+        m0 = ld_cg(args.tiles + 2 + 2 * blockIdx.y);
+        m_end = ld_cg(args.offsets + e + 1);
+        wrow0 = e * args.K + tile * SK_FEAT;
+    }
 
     const uint32_t a_base = g_smem_u32(ssm + Smem::A_OFF), b_base = g_smem_u32(ssm + Smem::B_OFF), p_base = g_smem_u32(ssm + Smem::P_OFF);
     const uint32_t bar = g_smem_u32(ssm + Smem::BAR_OFF);
@@ -130,7 +145,7 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             g_mbar_wait(p_empty + 8 * ps, ph);
             if (g_elect_one()) {
                 g_mbar_expect_tx(p_full + 8 * ps, SK_PACKED_BYTES);  // columns past the row end are zero-filled and still counted
-                g_tma_load_2d(p_base + ps * SK_PACKED_BYTES, &tmap_w, (gb0 + i * SK_PG) * (SK_GB / 2), tile * SK_FEAT, p_full + 8 * ps);
+                g_tma_load_2d(p_base + ps * SK_PACKED_BYTES, &tmap_w, (gb0 + i * SK_PG) * (SK_GB / 2), wrow0, p_full + 8 * ps);
             }
             __syncwarp();
             if (++ps == PSTAGES) ps = 0, ph ^= 1u;
@@ -159,7 +174,7 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         using V2 = typename SkNum<T>::V2;
         const uint32_t magic = SkNum<T>::MAGIC;
         const V2 offset2 = *reinterpret_cast<const V2 *>(&magic);
-        const size_t srow = static_cast<size_t>(min(tile * SK_FEAT + frow, args.K - 1)) * G;
+        const size_t srow = static_cast<size_t>(GROUPED ? wrow0 + frow : min(tile * SK_FEAT + frow, args.K - 1)) * G;
         const unsigned short *sc = reinterpret_cast<const unsigned short *>(args.scales) + srow + gb0;
         const unsigned short *bi = reinterpret_cast<const unsigned short *>(args.biases) + srow + gb0;
         const uint32_t swz = static_cast<uint32_t>(row & 7);  // == frow & 7
@@ -267,7 +282,10 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                 for (int c = 0; c < 2; ++c) {
                     const int m = mq + 8 * (i >> 2) + c;
                     const float gate = to_f(from_f<T>(acc[i + c])), up = to_f(from_f<T>(acc[i + 2 + c]));
-                    if (m < args.M && n0 < args.K) out[static_cast<size_t>(m) * (args.K / 2) + feat] = from_f<T>((gate / (1.0f + expf(-gate))) * up);
+                    if (m < m_end && n0 < args.K) {
+                        const int orow = GROUPED && args.out_index != nullptr ? ld_cg(args.out_index + m) : m;
+                        out[static_cast<size_t>(orow) * (args.K / 2) + feat] = from_f<T>((gate / (1.0f + expf(-gate))) * up);
+                    }
                 }
         } else {
             T *out = static_cast<T *>(args.out);
@@ -275,10 +293,11 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #pragma unroll
             for (int i = 0; i < NT / 2; ++i) {
                 const int m = mq + 8 * (i >> 2) + (i & 1), n = n0 + 8 * ((i >> 1) & 1);
-                if (m < args.M && n < args.K) {
+                if (m < m_end && n < args.K) {
                     T vb = from_f<T>(acc[i]);
                     if (args.epilogue == SK_EPI_RESIDUAL) vb = from_f<T>(to_f(ld_cg(res + static_cast<size_t>(m) * args.K + n)) + to_f(vb));
-                    out[static_cast<size_t>(m) * args.K + n] = vb;
+                    const int orow = GROUPED && args.out_index != nullptr ? ld_cg(args.out_index + m) : m;
+                    out[static_cast<size_t>(orow) * args.K + n] = vb;
                 }
             }
         }
@@ -433,17 +452,18 @@ static int sk_maps(CUtensorMap *ma, CUtensorMap *mw, const void *a, const void *
                              "quantized_matmul");
 }
 
-template <typename T, int NT>
+template <typename T, int NT, bool GROUPED = false>
 static int skinny_launch(const CUtensorMap &ma, const CUtensorMap &mw, const SkArgs &args, dim3 grid, cudaStream_t st) {
     constexpr size_t smem = SkSmem<NT>::BYTES;
+    auto *kernel = w4a16_skinny_kernel<T, NT, GROUPED>;
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(w4a16_skinny_kernel<T, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess ||
-            cudaFuncSetAttribute(w4a16_skinny_kernel<T, NT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+        if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess ||
+            cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
             return fail(TL_ECUDA, "quantized_matmul: cannot raise shared memory limit");
         configured = true;
     }
-    cudaError_t e = launch_chained(w4a16_skinny_kernel<T, NT>, grid, dim3(SK_THREADS), smem, st, ma, mw, args);
+    cudaError_t e = launch_chained(kernel, grid, dim3(SK_THREADS), smem, st, ma, mw, args);
     if (e != cudaSuccess) return fail(TL_ECUDA, "w4a16_skinny: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("w4a16_skinny");
     return TL_OK;
@@ -533,6 +553,36 @@ int launch_w4a16_tiles(const void *scales, const void *biases, const void *a, co
     if (dtype == TL_BF16) return tiles_t<__nv_bfloat16>(scales, biases, a, b, out, M, N, K, st);
     if (dtype == TL_F16) return tiles_t<__half>(scales, biases, a, b, out, M, N, K, st);
     return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+}
+
+// Grouped expert GEMM (MoE): R expert-sorted rows of a [R, N], E experts of K output features stacked in b [E K, N / 8],
+// NT-row tiles listed by tl_moe_group, max_tiles CTA rows of which the table's count run.
+template <typename T>
+static int grouped_t(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets, const int32_t *tiles,
+                     const int32_t *out_index, int R, int E, int N, int K, int epilogue, int nt, int max_tiles, cudaStream_t st) {
+    SkArgs args{};
+    args.scales = scales, args.biases = biases, args.out = out;
+    args.M = R, args.N = N, args.K = K, args.epilogue = epilogue;
+    args.splits = 1, args.gb_per_split = N / SK_GB;
+    args.tiles = tiles, args.offsets = offsets, args.out_index = out_index;
+    CUtensorMap ma, mw;
+    if (int e = sk_maps<T>(&ma, &mw, a, b, R, N, E * K, nt)) return e;
+    const dim3 grid(K / SK_FEAT, max_tiles);
+    switch (nt) {
+        case 16: return skinny_launch<T, 16, true>(ma, mw, args, grid, st);
+        case 32: return skinny_launch<T, 32, true>(ma, mw, args, grid, st);
+        case 64: return skinny_launch<T, 64, true>(ma, mw, args, grid, st);
+        default: return skinny_launch<T, 128, true>(ma, mw, args, grid, st);
+    }
+}
+
+int launch_w4a16_grouped(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets, const int32_t *tiles,
+                         const int32_t *out_index, int R, int E, int N, int K, int epilogue, int nt, int max_tiles, int dtype, cudaStream_t st) {
+    if (R == 0 || K == 0) return TL_OK;
+    if (dtype == TL_BF16)
+        return grouped_t<__nv_bfloat16>(scales, biases, a, b, out, offsets, tiles, out_index, R, E, N, K, epilogue, nt, max_tiles, st);
+    if (dtype == TL_F16) return grouped_t<__half>(scales, biases, a, b, out, offsets, tiles, out_index, R, E, N, K, epilogue, nt, max_tiles, st);
+    return fail(TL_EDTYPE, "moe_grouped_matmul: scales must be float16 or bfloat16");
 }
 
 }  // namespace tl

@@ -55,6 +55,12 @@ __all__ = [
     "quantized_matmul_residual_norm",
     "paged_attention_token_major",
     "qkv_project_rope_append",
+    "moe_topk",
+    "moe_group",
+    "moe_gather",
+    "moe_grouped_matmul",
+    "moe_grouped_matmul_route",
+    "moe_combine",
 ]
 
 _HERE = Path(__file__).resolve().parent
@@ -107,6 +113,13 @@ _SIGNATURES = {
     "tl_decode_attention_fused_rows": (_I, [_VP] * 11 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP]),
     "tl_paged_cache_append_chunk": (_I, [_VP] * 5 + [_I] * 4 + [ctypes.c_longlong, ctypes.c_longlong, _I, _VP]),
     "tl_set_pdl": (_I, [_I]),
+    "tl_moe_topk": (_I, [_VP] * 4 + [_I] * 5 + [_VP]),
+    "tl_moe_tile_table_size": (_I, [_I] * 3),
+    "tl_moe_group": (_I, [_VP, _I, _I, _I] + [_VP] * 4),
+    "tl_moe_gather": (_I, [_VP] * 3 + [_F, _VP] + [_I] * 4 + [_VP]),
+    "tl_moe_grouped_matmul_route": (_I, [_I] * 7 + [_VP] * 2 + [ctypes.POINTER(_I)] * 2),
+    "tl_moe_grouped_matmul": (_I, [_VP] * 8 + [_I] * 7 + [_VP]),
+    "tl_moe_combine": (_I, [_VP] * 4 + [_F, _VP, _VP] + [_I] * 4 + [_VP]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -928,6 +941,154 @@ def decode_attention_fused(qkv, q_norm_weight, k_norm_weight, offsets, block_tab
     else:
         _check(_lib.tl_decode_attention_fused_rows(*args, requests, R, *tail))
     return out
+
+
+# ---- Qwen3-MoE sparse block (include/tiny_llm_b200.h, "Qwen3-MoE") -------------
+MOE_CONTROL, MOE_WGMMA = 0, 1
+MOE_MAX_EXPERTS, MOE_MAX_TOPK = 256, 8
+
+
+def _moe_shape(op: str, E: int, k: int) -> None:
+    if E <= 0 or E > MOE_MAX_EXPERTS:
+        raise RuntimeError(f"{op}: at most {MOE_MAX_EXPERTS} experts (got {E})")
+    if k <= 0 or k > MOE_MAX_TOPK or k > E:
+        raise RuntimeError(f"{op}: top-k must be in [1, min({MOE_MAX_TOPK}, experts)] (got k = {k}, E = {E})")
+
+
+def moe_topk(logits, top_k, norm_topk_prob=False, stream=None):
+    """Router top-k of ``logits [T, E]``: ``(probs [T, E], ids int32 [T, k], scores [T, k])`` with probs the rounded
+    fp32 softmax, ids the k largest probs in descending order (ties to the lower expert id) and scores optionally
+    renormalised over the k (``include/tiny_llm_b200.h`` gives the rounding points)."""
+    if logits.dtype not in _FLOATS or logits.dim() != 2:
+        raise RuntimeError("moe_topk: expected 2D float logits [T, E]")
+    T, E = logits.shape
+    _moe_shape("moe_topk", E, int(top_k))
+    _gpu("moe_topk", logits)
+    _contig("moe_topk", logits=logits)
+    probs = torch.empty_like(logits)
+    ids = torch.empty((T, top_k), dtype=torch.int32, device=logits.device)
+    scores = torch.empty((T, top_k), dtype=logits.dtype, device=logits.device)
+    _check(_lib.tl_moe_topk(logits.data_ptr(), probs.data_ptr(), ids.data_ptr(), scores.data_ptr(), T, E, int(top_k), int(bool(norm_topk_prob)),
+                            _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+    return probs, ids, scores
+
+
+def moe_group(ids, num_experts, nt=0, stream=None):
+    """Expert grouping of ``ids`` (int32, R entries): ``(offsets int32 [E + 1], perm int32 [R], tiles)`` with perm the
+    stable sort of the rows by expert and, for ``nt > 0``, the grouped GEMM's tile table (else None)."""
+    if ids.dtype != torch.int32:
+        raise RuntimeError("moe_group: ids must be int32")
+    E = int(num_experts)
+    if E <= 0 or E > MOE_MAX_EXPERTS:
+        raise RuntimeError(f"moe_group: at most {MOE_MAX_EXPERTS} experts (got {E})")
+    if nt < 0:
+        raise RuntimeError("moe_group: nt must be >= 0")
+    _gpu("moe_group", ids)
+    _contig("moe_group", ids=ids)
+    R = ids.numel()
+    offsets = torch.empty((E + 1,), dtype=torch.int32, device=ids.device)
+    perm = torch.empty((R,), dtype=torch.int32, device=ids.device)
+    size = int(_lib.tl_moe_tile_table_size(R, E, int(nt)))
+    _check(min(size, 0))
+    tiles = torch.empty((size,), dtype=torch.int32, device=ids.device) if size > 0 else None
+    _check(_lib.tl_moe_group(ids.data_ptr(), R, E, int(nt), offsets.data_ptr(), perm.data_ptr(), None if tiles is None else tiles.data_ptr(),
+                             _stream_ptr(stream, ids)))
+    return offsets, perm, tiles
+
+
+def moe_gather(x, perm, rows_per_source, norm_weight=None, eps=0.0, stream=None):
+    """``xs[j] = x[perm[j] // rows_per_source]`` (optionally RMSNorm-ed with ``norm_weight``) -> ``[R, H]``."""
+    if x.dtype not in _FLOATS or x.dim() != 2:
+        raise RuntimeError("moe_gather: expected 2D float x [rows, H]")
+    if perm.dtype != torch.int32 or perm.dim() != 1:
+        raise RuntimeError("moe_gather: perm must be int32 [R]")
+    if int(rows_per_source) <= 0:
+        raise RuntimeError("moe_gather: rows_per_source must be positive")
+    H = x.shape[1]
+    if norm_weight is not None and (norm_weight.dtype != x.dtype or tuple(norm_weight.shape) != (H,)):
+        raise RuntimeError("moe_gather: norm weight must be [H] in the dtype of x")
+    _gpu("moe_gather", x, perm, *([] if norm_weight is None else [norm_weight]))
+    _contig("moe_gather", x=x, perm=perm, **({} if norm_weight is None else {"norm_weight": norm_weight}))
+    R = perm.numel()
+    xs = torch.empty((R, H), dtype=x.dtype, device=x.device)
+    _check(_lib.tl_moe_gather(x.data_ptr(), perm.data_ptr(), None if norm_weight is None else norm_weight.data_ptr(), float(eps), xs.data_ptr(), R,
+                              int(rows_per_source), H, _DTYPE_CODE[x.dtype], _stream_ptr(stream, x)))
+    return xs
+
+
+def moe_grouped_matmul_route(T, k, E, N, K, epilogue, dtype, a, b):
+    """The kernel ``moe_grouped_matmul`` runs: ``(route, nt, max_tiles)`` with route ``MOE_WGMMA`` or ``MOE_CONTROL``.
+    ``a`` and ``b`` are tensors or plain addresses (only their alignment counts); ``dtype`` is a torch dtype."""
+
+    def addr(t):
+        return t.data_ptr() if isinstance(t, torch.Tensor) else int(t)
+
+    nt, tiles = _I(), _I()
+    code = _lib.tl_moe_grouped_matmul_route(int(T), int(k), int(E), int(N), int(K), int(epilogue), _DTYPE_CODE[dtype], addr(a), addr(b),
+                                            ctypes.byref(nt), ctypes.byref(tiles))
+    _check(min(code, 0))
+    return code, nt.value, tiles.value
+
+
+def moe_grouped_matmul(scales, biases, b, a, offsets, tiles, top_k, out_index=None, epilogue=EPI_NONE, stream=None):
+    """Grouped W4A16 projection of the expert-sorted rows ``a [R, N]`` (R = T * top_k) by the experts ``b [E, K, N/8]``
+    (scales / biases ``[E, K, N/128]``), segments ``offsets [E + 1]`` and tile table ``tiles`` from ``moe_group`` (with
+    the ``nt`` of ``moe_grouped_matmul_route``).  Returns ``[R, K]`` (``EPI_SWIGLU_PAIRS``: ``[R, K/2]`` over each
+    expert's interleaved gate|up rows); row j lands at ``out_index[j]`` when given."""
+    if b.dim() != 3 or scales.dim() != 3 or a.dim() != 2:
+        raise RuntimeError("moe_grouped_matmul: expected b [E, K, N/8], scales [E, K, N/128] and a [R, N]")
+    E, K, words = b.shape
+    R, N = a.shape
+    if words * 8 != N or N % 128 or tuple(scales.shape) != (E, K, N // 128) or scales.shape != biases.shape:
+        raise RuntimeError("moe_grouped_matmul: incompatible parameter shapes")
+    if scales.dtype not in _HALF or a.dtype != scales.dtype or biases.dtype != scales.dtype or b.dtype not in _PACKED:
+        raise RuntimeError("moe_grouped_matmul: a, scales and biases must share a 16-bit dtype and b must be 32-bit words")
+    _moe_shape("moe_grouped_matmul", E, int(top_k))
+    if R % top_k:
+        raise RuntimeError("moe_grouped_matmul: rows must be a multiple of top_k")
+    if epilogue not in (EPI_NONE, EPI_SWIGLU_PAIRS) or (epilogue == EPI_SWIGLU_PAIRS and K % 16):
+        raise RuntimeError("moe_grouped_matmul: epilogue must be EPI_NONE or EPI_SWIGLU_PAIRS (K % 16 == 0)")
+    _int32("moe_grouped_matmul", offsets=offsets)
+    if offsets.numel() != E + 1:
+        raise RuntimeError("moe_grouped_matmul: offsets must be int32 [E + 1]")
+    if out_index is not None:
+        _int32("moe_grouped_matmul", R, out_index=out_index)
+    extra = [t for t in (tiles, out_index) if t is not None]
+    _gpu("moe_grouped_matmul", scales, biases, b, a, offsets, *extra)
+    _contig("moe_grouped_matmul", scales=scales, biases=biases, b=b, a=a, offsets=offsets)
+    T = R // top_k
+    route, nt, _ = moe_grouped_matmul_route(T, top_k, E, N, K, epilogue, a.dtype, a, b)
+    if route == MOE_WGMMA and (tiles is None or tiles.numel() != int(_lib.tl_moe_tile_table_size(R, E, nt))):
+        raise RuntimeError(f"moe_grouped_matmul: the wgmma route needs moe_group's tile table for nt = {nt}")
+    out = torch.empty((R, K // 2 if epilogue == EPI_SWIGLU_PAIRS else K), dtype=a.dtype, device=a.device)
+    _check(_lib.tl_moe_grouped_matmul(scales.data_ptr(), biases.data_ptr(), b.data_ptr(), a.data_ptr(), out.data_ptr(), offsets.data_ptr(),
+                                      None if tiles is None else tiles.data_ptr(), None if out_index is None else out_index.data_ptr(), T,
+                                      int(top_k), E, N, K, int(epilogue), _DTYPE_CODE[a.dtype], _stream_ptr(stream, a)))
+    return out
+
+
+def moe_combine(y, scores, residual=None, norm_weight=None, eps=0.0, stream=None):
+    """``out[t] = T(residual[t] + T(sum_j T(y[t k + j] * scores[t, j])))`` (without residual: the rounded sum) for
+    ``y [T k, H]`` and ``scores [T, k]``; with ``norm_weight`` returns ``(out, rms_norm(out))``."""
+    if y.dtype not in _FLOATS or y.dim() != 2 or scores.dim() != 2 or scores.dtype != y.dtype:
+        raise RuntimeError("moe_combine: expected y [T k, H] and scores [T, k] of one float dtype")
+    T, k = scores.shape
+    H = y.shape[1]
+    if k <= 0 or k > MOE_MAX_TOPK or y.shape[0] != T * k:
+        raise RuntimeError(f"moe_combine: y must be [T * k, H] with 1 <= k <= {MOE_MAX_TOPK}")
+    if residual is not None and (residual.dtype != y.dtype or tuple(residual.shape) != (T, H)):
+        raise RuntimeError("moe_combine: residual must be [T, H] in the dtype of y")
+    if norm_weight is not None and (norm_weight.dtype != y.dtype or tuple(norm_weight.shape) != (H,) or H > 4096):
+        raise RuntimeError("moe_combine: norm weight must be [H] (H <= 4096) in the dtype of y")
+    extra = {n: t for n, t in (("residual", residual), ("norm_weight", norm_weight)) if t is not None}
+    _gpu("moe_combine", y, scores, *extra.values())
+    _contig("moe_combine", y=y, scores=scores, **extra)
+    out = torch.empty((T, H), dtype=y.dtype, device=y.device)
+    normed = None if norm_weight is None else torch.empty_like(out)
+    _check(_lib.tl_moe_combine(y.data_ptr(), scores.data_ptr(), None if residual is None else residual.data_ptr(),
+                               None if norm_weight is None else norm_weight.data_ptr(), float(eps), out.data_ptr(),
+                               None if normed is None else normed.data_ptr(), T, k, H, _DTYPE_CODE[y.dtype], _stream_ptr(stream, y)))
+    return out if normed is None else (out, normed)
 
 
 def set_pdl(enabled: bool) -> None:

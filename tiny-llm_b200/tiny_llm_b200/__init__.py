@@ -11,6 +11,7 @@ from .embedding import Embedding, QuantizedEmbedding
 from .generate import greedy_generate_ids, simple_generate_with_kv_cache, speculative_generate, speculative_generate_ids
 from .kv_cache import BatchingKvCache, TinyKvCache, TinyKvFullCache
 from .layer_norm import RMSNorm
+from .moe import Moe, grouped_expert_linear, route_topk
 from .models import dispatch_model, shortcut_name_to_full_name
 from .paged_kv_cache import PagedKvMetadata, TinyKvPagedCache, TinyKvPagedPool
 from .positional_encoding import RoPE

@@ -36,6 +36,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200 as ext
 
 from .kv_cache import BatchingKvCache
+from .moe import Moe
 from .paged_kv_cache import TinyKvPagedCache
 
 # Decode attention runs as one fused launch while slots x max_seq_len stays within this: beyond it the K/V stream, not
@@ -74,7 +75,7 @@ def pack_layers(model) -> list:
     """Per layer, the weights of the fused launches: q|k|v and gate|up share their input, so they stream as one launch
     each.  ``Qwen3ModelWeek3.packed_layers`` keeps one such copy per model for all of its engines."""
     return [SimpleNamespace(qkv=_concat_weights([b.self_attn.wq, b.self_attn.wk, b.self_attn.wv]),
-                            gate_up=_interleave_gate_up(b.mlp.w_gate, b.mlp.w_up))
+                            gate_up=b.mlp.w_gate_up if isinstance(b.mlp, Moe) else _interleave_gate_up(b.mlp.w_gate, b.mlp.w_up))
             for b in model.layers_inner]
 
 
@@ -84,6 +85,23 @@ def _normed(h, norm):
 
 def _proj(h, w):
     return ext.quantized_matmul(w.scales, w.biases, w.group_size, w.bits, h, w.weight, True)
+
+
+def _moe_mlp(moe, x, h=None, ln2=None, nxt=None):
+    """The sparse MLP of one layer (``moe.Moe``) in place of the dense gate|up and down launches: returns the residual
+    stream ``x`` plus the expert mixture.  ``h``: the rows already normalised by the post-attention RMSNorm; without it
+    (the matvec stack) the router projection takes ``ln2`` as its prologue and the gather applies it to each row.  With
+    ``nxt`` (the next RMSNorm) the combine also returns its output, as ``(x, h)``.  Every row is routed, idle slots and
+    padding rows included: a row's result depends only on that row."""
+    w = moe.w_router
+    if h is None:
+        norm = (ln2._weight_as(x.dtype, x.device), ln2.eps)
+        logits = ext.quantized_matmul_fused(w.scales, w.biases, w.weight, x, norm[0], prologue=ext.PRO_RMSNORM, eps=norm[1])
+    else:
+        norm, logits = None, _proj(h, w)
+    _, ids, scores = ext.moe_topk(logits, moe.num_experts_per_tok, moe.norm_topk_prob)
+    return moe.experts(x if h is None else h, ids, scores, residual=x, gather_norm=norm,
+                       next_norm=None if nxt is None else (nxt._weight_as(x.dtype, x.device), nxt.eps))
 
 
 def _swap_ab_layers(model, x, attention):
@@ -98,12 +116,16 @@ def _swap_ab_layers(model, x, attention):
     packed = model.packed_layers()
     h = _normed(x, layers[0].input_layernorm)
     for i, block in enumerate(layers):
-        wo, wd, gate_up = block.self_attn.wo, block.mlp.w_down, packed[i].gate_up
+        wo, gate_up = block.self_attn.wo, packed[i].gate_up
         ln2 = block.post_attention_layernorm
         y = attention(i, block, h)
         x, h = ext.quantized_matmul_residual_norm(wo.scales, wo.biases, wo.weight, y, x, ln2._weight_as(x.dtype, x.device), ln2.eps)
-        act = ext.quantized_matmul_fused(gate_up.scales, gate_up.biases, gate_up.weight, h, epilogue=ext.EPI_SWIGLU_PAIRS)
         nxt = layers[i + 1].input_layernorm if i + 1 < len(layers) else model.norm
+        if isinstance(block.mlp, Moe):
+            x, h = _moe_mlp(block.mlp, x, h, nxt=nxt)
+            continue
+        wd = block.mlp.w_down
+        act = ext.quantized_matmul_fused(gate_up.scales, gate_up.biases, gate_up.weight, h, epilogue=ext.EPI_SWIGLU_PAIRS)
         x, h = ext.quantized_matmul_residual_norm(wd.scales, wd.biases, wd.weight, act, x, nxt._weight_as(x.dtype, x.device), nxt.eps)
     return h
 
@@ -344,6 +366,9 @@ class DecodeEngine(_GraphEngine):
             x = ext.add(x, _proj(y.view(B, Hq * D), at.wo))
             h = _normed(x, block.post_attention_layernorm)
             mlp = block.mlp
+            if isinstance(mlp, Moe):
+                x = _moe_mlp(mlp, x, h)
+                continue
             x = ext.add(x, _proj(ext.swiglu(_proj(h, mlp.w_gate), _proj(h, mlp.w_up)), mlp.w_down))
         x = _normed(x, m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
@@ -419,8 +444,11 @@ class DecodeEngine(_GraphEngine):
                                                    Hq, Hkv, at.rope.base, at.q_norm.eps)
                 y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
                                         at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
-            wd = block.mlp.w_down
             x = ext.quantized_matmul_fused(at.wo.scales, at.wo.biases, at.wo.weight, y.view(B, Hq * D), residual=x, epilogue=ext.EPI_RESIDUAL)
+            if isinstance(block.mlp, Moe):
+                x = _moe_mlp(block.mlp, x, ln2=ln2)
+                continue
+            wd = block.mlp.w_down
             act = ext.quantized_matmul_fused(pk.gate_up.scales, pk.gate_up.biases, pk.gate_up.weight, x, ln2._weight_as(x.dtype, x.device),
                                              prologue=ext.PRO_RMSNORM, eps=ln2.eps, epilogue=ext.EPI_SWIGLU_PAIRS)  # [B, inter]
             x = ext.quantized_matmul_fused(wd.scales, wd.biases, wd.weight, act, residual=x, epilogue=ext.EPI_RESIDUAL)
@@ -719,8 +747,10 @@ class VerifyEngine(DecodeEngine):
 
     @staticmethod
     def supported(model, device, max_seq_len: int) -> bool:
-        """Where the B = 1 decode engine itself runs fused matvec + fused attention."""
-        return torch.device(device).type == "cuda" and DecodeEngine.fused_attention_applies(model, max_seq_len)
+        """Where the B = 1 decode engine itself runs fused matvec + fused attention, on dense models only (the verify pass
+        does not take the MoE block)."""
+        return (torch.device(device).type == "cuda" and DecodeEngine.fused_attention_applies(model, max_seq_len)
+                and not any(isinstance(b.mlp, Moe) for b in model.layers_inner))
 
     def reserve_pools(self, pages_per_layer: int | None = None) -> None:
         raise RuntimeError("the verify step shares the B = 1 decode engine's pool reservation")
@@ -825,6 +855,9 @@ class PrefillEngine(_GraphEngine):
                 h = _normed(x, block.input_layernorm)
                 x = ext.add(x, _proj(self._attention(i, block, h), block.self_attn.wo))
                 h = _normed(x, block.post_attention_layernorm)
+                if isinstance(block.mlp, Moe):
+                    x = _moe_mlp(block.mlp, x, h)
+                    continue
                 x = ext.add(x, _proj(ext.swiglu(_proj(h, block.mlp.w_gate), _proj(h, block.mlp.w_up)), block.mlp.w_down))
             last = _normed(x[L - 1:L], m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight

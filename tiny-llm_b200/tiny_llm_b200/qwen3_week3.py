@@ -18,6 +18,7 @@ import torch
 from .attention import paged_attention
 from .embedding import QuantizedEmbedding
 from .kv_cache import TinyKvCache
+from .moe import Moe
 from .paged_kv_cache import TinyKvPagedCache, TinyKvPagedPool
 from .quantize import QuantizedWeights, quantized_linear
 from .week2_kernels import (
@@ -128,7 +129,7 @@ class Qwen3TransformerBlock:
         k_norm: torch.Tensor,
         w_input_layernorm: torch.Tensor,
         w_post_attention_layernorm: torch.Tensor,
-        mlp: Qwen3MLP,
+        mlp: Qwen3MLP | Moe,
         max_seq_len: int = 32768,
         theta: int = 1000000,
         use_paged_attention: bool = True,
@@ -193,18 +194,25 @@ class Qwen3ModelWeek3:
         )
         self.layers_inner = []
         for index, layer in enumerate(mlx_model.model.layers[: self.num_hidden_layers]):
-            if is_qwen3_moe_sparse_layer(args, index):
-                raise NotImplementedError(
-                    "Qwen3-MoE layers are outside the CUDA hot-path scope (SURVEY.md section 2, row 12)"
-                )
             attn = layer.self_attn
-            mlp = Qwen3MLP(
-                args.hidden_size,
-                args.intermediate_size,
-                packed(layer.mlp.gate_proj),
-                packed(layer.mlp.up_proj),
-                packed(layer.mlp.down_proj),
-            )
+            if is_qwen3_moe_sparse_layer(args, index):
+                switch = layer.mlp.switch_mlp
+                mlp = Moe(
+                    w_router=packed(layer.mlp.gate),
+                    w_gate=packed(switch.gate_proj),
+                    w_up=packed(switch.up_proj),
+                    w_down=packed(switch.down_proj),
+                    num_experts_per_tok=args.num_experts_per_tok,
+                    norm_topk_prob=args.norm_topk_prob,
+                )
+            else:
+                mlp = Qwen3MLP(
+                    args.hidden_size,
+                    args.intermediate_size,
+                    packed(layer.mlp.gate_proj),
+                    packed(layer.mlp.up_proj),
+                    packed(layer.mlp.down_proj),
+                )
             self.layers_inner.append(
                 Qwen3TransformerBlock(
                     num_attention_heads=args.num_attention_heads,

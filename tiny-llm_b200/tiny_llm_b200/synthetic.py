@@ -30,6 +30,14 @@ CONFIGS = {
     # small shapes for tests (same structure, every kernel family exercised)
     "tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=32, intermediate_size=256, vocab_size=128),
     "tiny-d128": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=128, intermediate_size=384, vocab_size=512),
+    # Qwen3-MoE (published Qwen3-30B-A3B config: every layer sparse, untied head)
+    "qwen3-30b-a3b": dict(hidden_size=2048, num_hidden_layers=48, num_attention_heads=32, num_key_value_heads=4, head_dim=128, intermediate_size=6144,
+                          vocab_size=151936, num_experts=128, num_experts_per_tok=8, moe_intermediate_size=768, norm_topk_prob=True,
+                          decoder_sparse_step=1, mlp_only_layers=[], tie_word_embeddings=False),
+    # a dense layer and a sparse layer in one small model
+    "tiny-moe-d128": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=128, intermediate_size=384,
+                          vocab_size=512, num_experts=8, num_experts_per_tok=2, moe_intermediate_size=128, norm_topk_prob=True,
+                          decoder_sparse_step=1, mlp_only_layers=[0]),
 }
 
 
@@ -40,6 +48,12 @@ def make_args(name_or_dims, **overrides) -> SimpleNamespace:
     dims.setdefault("rope_theta", 1000000)
     dims.setdefault("tie_word_embeddings", True)
     dims.update(overrides)
+    if dims.get("num_experts", 0) > 0:  # Qwen3-MoE keys (mlx_lm qwen3_moe.ModelArgs)
+        dims.setdefault("num_experts_per_tok", 8)
+        dims.setdefault("moe_intermediate_size", dims["intermediate_size"])
+        dims.setdefault("norm_topk_prob", True)
+        dims.setdefault("decoder_sparse_step", 1)
+        dims.setdefault("mlp_only_layers", [])
     return SimpleNamespace(**dims)
 
 
@@ -117,10 +131,34 @@ def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realis
     def norm(dim: int) -> SimpleNamespace:
         return _empty_norm(dim, device) if empty else _norm_weight(dim, gen)
 
+    def experts(out_dim: int, in_dim: int) -> SimpleNamespace:
+        """SwitchLinear layout: [E, out, in/8] codes, [E, out, in/128] scales and biases."""
+        parts = [layer(out_dim, in_dim) for _ in range(args.num_experts)]
+        stacked = {key: torch.stack([getattr(p, key).view(torch.int32) if key == "weight" else getattr(p, key) for p in parts])
+                   for key in ("weight", "scales", "biases")}
+        stacked["weight"] = stacked["weight"].view(torch.uint32)
+        return SimpleNamespace(**stacked, group_size=GROUP_SIZE, bits=BITS)
+
+    def mlp(index: int) -> SimpleNamespace:
+        sparse = (getattr(args, "num_experts", 0) > 0 and index not in args.mlp_only_layers
+                  and (index + 1) % args.decoder_sparse_step == 0)  # qwen3_week3.is_qwen3_moe_sparse_layer
+        if sparse:
+            inter = args.moe_intermediate_size
+            return SimpleNamespace(
+                gate=layer(args.num_experts, args.hidden_size),
+                switch_mlp=SimpleNamespace(gate_proj=experts(inter, args.hidden_size), up_proj=experts(inter, args.hidden_size),
+                                           down_proj=experts(args.hidden_size, inter)),
+            )
+        return SimpleNamespace(
+            gate_proj=layer(args.intermediate_size, args.hidden_size),
+            up_proj=layer(args.intermediate_size, args.hidden_size),
+            down_proj=layer(args.hidden_size, args.intermediate_size),
+        )
+
     q_width = args.num_attention_heads * args.head_dim
     kv_width = args.num_key_value_heads * args.head_dim
     layers = []
-    for _ in range(args.num_hidden_layers):
+    for index in range(args.num_hidden_layers):
         layers.append(
             SimpleNamespace(
                 self_attn=SimpleNamespace(
@@ -131,11 +169,7 @@ def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realis
                     q_norm=norm(args.head_dim),
                     k_norm=norm(args.head_dim),
                 ),
-                mlp=SimpleNamespace(
-                    gate_proj=layer(args.intermediate_size, args.hidden_size),
-                    up_proj=layer(args.intermediate_size, args.hidden_size),
-                    down_proj=layer(args.hidden_size, args.intermediate_size),
-                ),
+                mlp=mlp(index),
                 input_layernorm=norm(args.hidden_size),
                 post_attention_layernorm=norm(args.hidden_size),
             )
