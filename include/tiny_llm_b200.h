@@ -189,6 +189,35 @@ size_t tl_argmax_workspace(int rows, int vocab);
  * No workspace; deterministic. */
 int tl_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
               const int32_t *positions, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
+ * launch, one cluster of CTAs per row (DESIGN.md section 8a).
+ *
+ * The distribution reported is the raw model distribution, lp_i = x_i - m - log S with m the row maximum and
+ * S = sum_i exp(x_i - m): the reference's logits - logsumexp(logits).  Temperature, top-k and top-p do not enter it;
+ * a sampled token reports its raw log-probability.  Rounding points, in order:
+ *   d_i = fl32(x_i - m);  e_i = expf(d_i);  E_i = round-to-nearest(e_i * 2^40) as a 64-bit integer;
+ *   S_fx = sum_i E_i over the non-NaN entries (exact, so the same bits in any order, row count, row index or graph);
+ *   log_s = logf(fl32(S_fx) * 2^-40)  (the conversion rounds, the scaling is exact: S >= 1);
+ *   lp(x) = fl32(fl32(x - m) - log_s),  lse = fl32(m + log_s).
+ * Per row r, written at row o = r + (out_index ? *out_index * rows : 0); with out_index (device), the outputs are logs
+ * of out_capacity such blocks and a launch whose *out_index is outside [0, out_capacity) writes nothing (as
+ * tl_decode_advance treats its token log; out_capacity is ignored without out_index):
+ *   lse[o];
+ *   targets (device, may be NULL: every target -1): for t = targets[r] in [0, vocab), target_lp[o] = lp(x_t) and
+ *     target_rank[o] = 1 + #{i : x_i > x_t}; t outside [0, vocab) or x_t NaN gives NaN and rank 0;
+ *   top_n (device, may be NULL: max_n for every row), 0 <= max_n <= TL_LOGPROBS_MAX_N: the min(top_n[r], max_n)
+ *     largest entries in top_ids[o * max_n + j] (int32) and top_lp[...] (lp(x), the target's expression: bit-identical
+ *     when the target is listed), in descending order with ties to the lower id (tl_argmax's first-maximum rule);
+ *     slots past the listed entries hold id -1 and -inf.  top_ids / top_lp may be NULL when max_n == 0.
+ * NaN entries are never listed, never counted in S and never counted in a rank; -inf entries are ordinary entries
+ * with lp -inf.  A row whose maximum is not finite (+inf, every non-NaN entry -inf, or every entry NaN) reports
+ * lse = that maximum (NaN when every entry is NaN) and NaN for every lp, with ranks and top-N ids by the rules above.
+ * targets and top_n are read after the programmatic-dependent-launch wait, so the previous launch may write them.
+ * No workspace; deterministic. */
+#define TL_LOGPROBS_MAX_N 20
+int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
+                int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
+                void *stream);
 /* Fused W4A16 projection for the decode hot loop: the weight-streaming kernel of
  * tl_quantized_matmul with the neighbouring element-wise operator folded in.
  * Rounding points are those of the unfused call sequence, so results are

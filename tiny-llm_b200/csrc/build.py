@@ -35,6 +35,7 @@ SOURCES = [
     "attention_prefill_tc.cu",
     "decode_attention_fused.cu",
     "sampling.cu",
+    "logprobs.cu",
     "moe.cu",
     "tma.cu",
 ]

@@ -356,6 +356,20 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
     return launch_sample(logits, temperature, top_k, top_p, seed, positions, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
+int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
+                int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
+                void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "logprobs: expected float32, float16, or bfloat16");
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "logprobs: bad shape");
+    if (max_n < 0 || max_n > TL_LOGPROBS_MAX_N) return fail(TL_EINVAL, "logprobs: max_n must be in [0, %d]", TL_LOGPROBS_MAX_N);
+    if (out_index && out_capacity < 0) return fail(TL_EINVAL, "logprobs: bad out_capacity");
+    if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
+    if (rows == 0) return TL_OK;
+    if (!logits || !lse || !target_lp || !target_rank || (max_n > 0 && (!top_ids || !top_lp))) return fail(TL_EINVAL, "logprobs: null pointer");
+    return launch_logprobs(logits, targets, top_n, out_index, lse, target_lp, target_rank, top_ids, top_lp, rows, vocab, max_n,
+                           out_index ? out_capacity : 1, dtype, as_stream(stream));
+}
+
 int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, const void *a, const void *b,
                               const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass, int *units) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");

@@ -38,6 +38,11 @@ int launch_argmax(const void *logits, int32_t *out, int rows, int vocab, int dty
 int sample_plan(int vocab, int *cluster, int *slice);
 int launch_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+// logprobs.cu: same cluster plan as sampling.cu
+constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
+int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,
+                    int32_t *rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
+                    cudaStream_t st);
 
 int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                           int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, cudaStream_t st);

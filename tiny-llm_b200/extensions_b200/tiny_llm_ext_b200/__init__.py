@@ -43,6 +43,8 @@ __all__ = [
     "add",
     "argmax",
     "sample",
+    "logprobs",
+    "LOGPROBS_MAX_N",
     "decode_advance",
     "quantized_matmul_fused",
     "quantized_matmul_route",
@@ -99,6 +101,7 @@ _SIGNATURES = {
     "tl_argmax": (_I, [_VP, _VP, _I, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
+    "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
     "tl_quantized_matmul_fused_workspace": (_SZ, [_I] * 6),
@@ -633,6 +636,55 @@ def sample(logits, temperature, top_k, top_p, seed, positions, stream=None):
     _check(_lib.tl_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(), positions.data_ptr(),
                           out.data_ptr(), rows, logits.shape[1], _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
+
+
+LOGPROBS_MAX_N = 20
+
+
+def logprobs(logits, targets=None, top_n=None, max_n=0, out=None, out_index=None, stream=None):
+    """Log-probabilities of the raw distribution of each row of ``logits [rows, vocab]`` (``tl_logprobs``).
+    ``targets`` int32 ``[rows]`` (device; -1: none), ``top_n`` int32 ``[rows]`` (device; None: ``max_n`` for every row),
+    ``0 <= max_n <= 20``.  Returns ``(lse, target_lp, target_rank, top_ids, top_lp)``: float32 / float32 / int32
+    ``[rows]`` and int32 / float32 ``[rows, max_n]`` (ids -1 and -inf past each row's list).  ``out`` (those five
+    tensors with a leading ``[capacity, ...]`` dimension) and ``out_index`` (int32 ``[1]``, device) write row r at
+    ``out[...][out_index, r]`` instead: a captured graph logs step after step into one buffer.  An ``out_index`` outside
+    ``[0, capacity)`` writes nothing."""
+    if logits.dtype not in _FLOATS or logits.dim() != 2:
+        raise RuntimeError("logprobs: expected 2D float logits")
+    if not isinstance(max_n, int) or isinstance(max_n, bool) or not 0 <= max_n <= LOGPROBS_MAX_N:
+        raise RuntimeError(f"logprobs: max_n must be an integer in [0, {LOGPROBS_MAX_N}]")
+    rows, vocab = logits.shape
+    named = {"logits": logits}
+    for name, t in (("targets", targets), ("top_n", top_n)):
+        if t is not None:
+            if t.dtype != torch.int32 or t.dim() != 1 or t.shape[0] != rows:
+                raise RuntimeError(f"logprobs: {name} must be int32 [{rows}]")
+            named[name] = t
+    if out is None:
+        if out_index is not None:
+            raise RuntimeError("logprobs: out_index needs out")
+        dev = logits.device
+        out = (torch.empty(rows, dtype=torch.float32, device=dev), torch.empty(rows, dtype=torch.float32, device=dev),
+               torch.empty(rows, dtype=torch.int32, device=dev), torch.empty((rows, max_n), dtype=torch.int32, device=dev),
+               torch.empty((rows, max_n), dtype=torch.float32, device=dev))
+        lead = ()
+    else:
+        if out_index is None or out_index.dtype != torch.int32 or out_index.numel() != 1:
+            raise RuntimeError("logprobs: out needs out_index, int32 [1]")
+        named["out_index"] = out_index
+        lead = (out[0].shape[0],)
+    shapes = (lead + (rows,),) * 3 + (lead + (rows, max_n),) * 2
+    for t, shape, dtype in zip(out, shapes, (torch.float32, torch.float32, torch.int32, torch.int32, torch.float32)):
+        if t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError("logprobs: out must be float32 lse, float32 lp, int32 rank [..., rows], int32 ids and float32 lp [..., rows, max_n]")
+    _contig("logprobs", **named)
+    _gpu("logprobs", *named.values(), *out)
+    lse, lp, rank, ids, top = out
+    _check(_lib.tl_logprobs(logits.data_ptr(), None if targets is None else targets.data_ptr(), None if top_n is None else top_n.data_ptr(),
+                            None if out_index is None else out_index.data_ptr(), lse.data_ptr(), lp.data_ptr(), rank.data_ptr(),
+                            ids.data_ptr() if max_n else None, top.data_ptr() if max_n else None, rows, vocab, max_n,
+                            lead[0] if lead else 1, _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+    return lse, lp, rank, ids, top
 
 
 def decode_advance(tokens, next_tokens, offsets, context_lens, out_log, step_counter, stream=None):

@@ -16,6 +16,7 @@ from .models import dispatch_model, shortcut_name_to_full_name
 from .paged_kv_cache import PagedKvMetadata, TinyKvPagedCache, TinyKvPagedPool
 from .positional_encoding import RoPE
 from .sampler import SamplingParams, make_sampler
+from .logprobs import PromptScore, TokenLogprobs, score_ids, token_logprobs
 from .quantize import (
     QuantizedWeights,
     dequantize_linear,

@@ -23,6 +23,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200
 
 from .kv_cache import BatchingKvCache
+from .logprobs import _check_n, token_logprobs
 from .sampler import sample_tokens, sampling_per_request
 
 
@@ -63,7 +64,8 @@ class Request:
     serving runs, a sequence of token ids (``tokenizer`` may then be ``None``;
     pass ``eos_token_id`` explicitly if one is wanted).  ``sampling`` (a
     ``SamplingParams``) draws the request's tokens with the seeded ``tl_sample``
-    kernel; None keeps them greedy."""
+    kernel; None keeps them greedy.  ``logprobs`` (an int N) records one
+    ``TokenLogprobs`` per generated token in ``logprob_entries``."""
 
     def __init__(
         self,
@@ -76,9 +78,12 @@ class Request:
         eos_token_id: int | None = None,
         device=None,
         sampling=None,
+        logprobs=None,
     ):
         self.prompt = prompt
         self.sampling = sampling
+        self.logprobs = logprobs
+        self.logprob_entries: list = []
         self.model = model
         if isinstance(prompt, str):
             ids = tokenizer.encode(prompt, add_special_tokens=False)
@@ -110,11 +115,16 @@ class Request:
         total = self.prefill_tokens.numel()
         chunk = min(self.prefill_max_step, total - self.offset)
         ids = self.prefill_tokens[self.offset : self.offset + chunk][None]
-        if self.sampling is None:
+        entry = None
+        if self.sampling is None and self.logprobs is None:
             token = _step(self.model, ids, [self.offset], self.kv_cache)
         else:  # only the last chunk's token is used: the prompt's first token is drawn at position `total`
             logits = self.model(ids, [self.offset], self.kv_cache, logits_to_keep=1)[:, -1, :]
-            token = sample_tokens(logits, [self.sampling], [total]) if self.offset + chunk == total else None
+            token = None
+            if self.offset + chunk == total:
+                token = greedy_tokens(logits) if self.sampling is None else sample_tokens(logits, [self.sampling], [total])
+                if self.logprobs is not None:
+                    entry = token_logprobs(logits, token, self.logprobs)[0]
         self.offset += chunk
         for layer_cache in self.kv_cache:
             layer_cache.materialize()
@@ -124,15 +134,17 @@ class Request:
                 self.is_done = True
                 self.finish_reason = "max seq len"
             else:
-                self.decode_done(int(token.reshape(-1)[0]), False)
+                self.decode_done(int(token.reshape(-1)[0]), False, entry)
 
-    def decode_done(self, token, update_offset=True):
+    def decode_done(self, token, update_offset=True, entry=None):
         if self.is_done:
             raise ValueError("decode called after done")
         if token == self.eos_token_id:
             self.is_done = True
             self.finish_reason = "EOS"
             return
+        if entry is not None:
+            self.logprob_entries.append(entry)
         self.detokenizer.add_token(token)
         self.next_token = token
         if update_offset:
@@ -174,10 +186,12 @@ class ContinuousBatcher:
     """The reference scheduling loop as a steppable object.  ``sampling``: None (greedy, the reference's loop), one
     ``SamplingParams`` for every prompt or a list with one per prompt; a request's tokens are then drawn by the seeded
     ``tl_sample`` kernel from its last prefill chunk's and every decode step's logits, and do not depend on its slot or
-    on the other requests."""
+    on the other requests.  ``logprobs`` (an int N in [0, 20]) fills ``self.logprobs[prompt_idx]`` with one
+    ``TokenLogprobs`` per generated token: the first from the prompt's last prefill chunk, the others from the decode
+    step that produced them (one ``ext.logprobs`` launch over all slots per step, idle slots with target -1)."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
-                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None):
+                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None):
         if max_seq_len <= 0:
             raise ValueError("max_seq_len must be positive")
         if batch_size <= 0:
@@ -188,6 +202,8 @@ class ContinuousBatcher:
         self.tokenizer = tokenizer
         self.queue = list(prompts)
         self.sampling = sampling_per_request(sampling, len(self.queue))
+        self.logprobs_n = None if logprobs is None else _check_n(logprobs)
+        self.logprobs: dict[int, list] = {}
         self.max_seq_len = max_seq_len
         self.batch_size = batch_size
         self.prefill_step = prefill_step
@@ -265,7 +281,10 @@ class ContinuousBatcher:
                 self.model, self.tokenizer, prompt, self.prefill_step, self.next_request_idx,
                 max_seq_len=self.max_seq_len, eos_token_id=self.eos_token_id, device=self.device,
                 sampling=None if self.sampling is None else self.sampling[self.next_request_idx],
+                logprobs=self.logprobs_n,
             )
+            if self.logprobs_n is not None:
+                self.logprobs[self.next_request_idx] = self.pending.logprob_entries
             self.next_request_idx += 1
 
         if self.pending is not None:
@@ -312,21 +331,30 @@ class ContinuousBatcher:
             t0 = time.perf_counter() if self.record_timing else 0.0
             span = self._gpu_span("decode")
             batch = torch.tensor(tokens, dtype=torch.int32, device=self.device).reshape(-1, 1)
-            if self.sampling is None:
+            entries = None
+            if self.sampling is None and self.logprobs_n is None:
                 sampled = _step(self.model, batch, offsets, self.kv_cache)
             else:  # slot i draws the token at position offset + 1; idle and greedy slots get argmax's token
                 logits = self.model(batch, offsets, self.kv_cache, logits_to_keep=1)[:, -1, :]
-                sampled = sample_tokens(logits, [None if s is None else s.sampling for s in self.slots], [o + 1 for o in offsets])
+                if self.sampling is None:
+                    sampled = greedy_tokens(logits)
+                else:
+                    sampled = sample_tokens(logits, [None if s is None else s.sampling for s in self.slots], [o + 1 for o in offsets])
+                if self.logprobs_n is not None:
+                    live = torch.tensor([s is not None for s in self.slots], device=sampled.device)
+                    targets = torch.where(live, sampled.reshape(-1).to(torch.int32), -1)
+                    entries = token_logprobs(logits, targets, self.logprobs_n)
             if span is not None:
                 span.record()
-            host = sampled.reshape(-1).tolist()  # one device->host read per step
+            # one device->host read per step (with logprobs, the entries carry the tokens: idle slots hold -1 and are skipped)
+            host = sampled.reshape(-1).tolist() if entries is None else [e.token for e in entries]
             if self.record_timing:
                 self.decode_step_ms.append((time.perf_counter() - t0) * 1e3)
             self.decode_steps += 1
             for i, request in enumerate(self.slots):
                 if request is None:
                     continue
-                request.decode_done(int(host[i]))
+                request.decode_done(int(host[i]), entry=None if entries is None else entries[i])
                 self.decode_tokens += 1
                 self.generated[request.prompt_idx] = self.generated.get(request.prompt_idx, 0) + (0 if request.is_done else 1)
                 reason = None
@@ -370,8 +398,11 @@ class ContinuousBatcher:
 
 
 def batch_generate(model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True, **kwargs):
-    """batch.py:136-285 - returns ``[(prompt_idx, text), ...]`` in completion order."""
-    return ContinuousBatcher(
+    """batch.py:136-285 - returns ``[(prompt_idx, text), ...]`` in completion order.  With ``logprobs=N`` it returns
+    ``(results, logprobs)`` instead, ``logprobs[prompt_idx]`` the request's ``TokenLogprobs`` (``ContinuousBatcher``)."""
+    batcher = ContinuousBatcher(
         model, tokenizer, prompts, max_seq_len=max_seq_len, batch_size=batch_size, prefill_step=prefill_step,
         verbose=verbose, **kwargs
-    ).run()
+    )
+    results = batcher.run()
+    return results if kwargs.get("logprobs") is None else (results, batcher.logprobs)

@@ -10,6 +10,10 @@ see checkpoint.py; there is no hub download here).
         (seeded sampling with the tl_sample kernel: the same seed gives the same tokens)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
+        (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
+    python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
+        (teacher-forced log-probability of every prompt token and the prompt's perplexity)
 """
 
 from __future__ import annotations
@@ -53,6 +57,19 @@ def _prompt_ids(args, tokenizer, prompt: str | None):
     return tokenizer.encode(text, add_special_tokens=False)
 
 
+def _token_text(tokenizer, token: int) -> str:
+    if tokenizer is None:
+        return str(token)
+    return repr(tokenizer.decode([token]))
+
+
+def _print_logprobs(entries, tokenizer, file=None) -> None:
+    """One line per entry: the token, its log-probability and rank, then its alternatives."""
+    for e in entries:
+        alts = ", ".join(f"{_token_text(tokenizer, i)} {v:.4f}" for i, v in e.top)
+        print(f"  {_token_text(tokenizer, e.token)}\tlogprob {e.logprob:.4f}\trank {e.rank}" + (f"\t| {alts}" if alts else ""), file=file)
+
+
 def cmd_generate(args) -> int:
     from .generate import greedy_generate_ids
     from .sampler import SamplingParams, make_sampler
@@ -83,6 +100,8 @@ def cmd_generate(args) -> int:
 
         if sampler is not None or sampling is not None:
             raise SystemExit("speculative decoding is greedy: drop --sampler-temp")
+        if args.logprobs is not None:
+            raise SystemExit("speculative decoding does not report log-probabilities: drop --logprobs")
         if args.draft_model and args.draft_synthetic:
             raise SystemExit("give one draft: --draft-model or --draft-synthetic, not both")
         draft_args = argparse.Namespace(**{**vars(args), "model": args.draft_model, "synthetic": args.draft_synthetic})
@@ -98,13 +117,17 @@ def cmd_generate(args) -> int:
         print()
         return 0
     produced = greedy_generate_ids(model, ids, args.max_new_tokens, eos_token_id=eos, device=device,
-                                   on_token=emit, sampler=sampler, sampling=sampling)
+                                   on_token=emit, sampler=sampler, sampling=sampling, logprobs=args.logprobs)
     print()
+    if args.logprobs is not None:
+        produced, entries = produced
+        print("logprobs (raw model distribution):")
+        _print_logprobs(entries, tokenizer)
     return 0 if produced is not None else 1
 
 
 def cmd_batch(args) -> int:
-    from .batch import batch_generate
+    from .batch import ContinuousBatcher
     from .sampler import SamplingParams
 
     device = torch.device(args.device)
@@ -123,18 +146,45 @@ def cmd_batch(args) -> int:
     if args.sampler_temp != 0:  # request i draws with seed `--seed + i`
         sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i)
                     for i in range(len(queue))]
-    results = batch_generate(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
-                             verbose=not args.quiet, device=device, max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None,
-                             sampling=sampling)
+    batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
+                                verbose=not args.quiet, device=device,
+                                max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None, sampling=sampling,
+                                logprobs=args.logprobs)
+    results = batcher.run()
     for idx, text in sorted(results):
         print(f"--- request {idx}\n{text}")
+        if args.logprobs is not None:
+            _print_logprobs(batcher.logprobs.get(idx, []), tokenizer)
+    return 0
+
+
+def cmd_score(args) -> int:
+    from .logprobs import score_ids
+
+    device = torch.device(args.device)
+    ns, tokenizer, name = _load(args, device)
+    model = _model(args, ns, name)
+    if args.prompt_ids:
+        ids = [int(t) for t in args.prompt_ids.split(",")]
+    elif tokenizer is None:
+        raise SystemExit("a text prompt needs the checkpoint's tokenizer files; use --prompt-ids")
+    else:
+        ids = tokenizer.encode(args.prompt, add_special_tokens=False)
+    if len(ids) < 2:
+        raise SystemExit("scoring needs a prompt of at least two tokens")
+    result = score_ids(model, ids, chunk=args.chunk, top_n=args.logprobs or 0, device=device)
+    print(f"prompt: {len(ids)} tokens; first token {_token_text(tokenizer, ids[0])} is not scored")
+    _print_logprobs(result.entries, tokenizer)
+    print(f"total nll {result.nll:.4f} nats over {len(result.entries)} tokens, perplexity {result.perplexity:.4f}")
+    if result.next_top:
+        print("next token: " + ", ".join(f"{_token_text(tokenizer, i)} {v:.4f}" for i, v in result.next_top))
     return 0
 
 
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="tiny_llm_b200.cli")
     sub = ap.add_subparsers(dest="command", required=True)
-    for name, fn in (("generate", cmd_generate), ("batch", cmd_batch)):
+    for name, fn in (("generate", cmd_generate), ("batch", cmd_batch), ("score", cmd_score)):
         p = sub.add_parser(name)
         p.set_defaults(fn=fn)
         p.add_argument("--model", default=None, help="checkpoint directory (config.json + *.safetensors [+ tokenizer files])")
@@ -151,6 +201,10 @@ def main(argv=None) -> int:
         sub.choices[name].add_argument("--sampler-top-p", type=float, default=None)
         sub.choices[name].add_argument("--sampler-top-k", type=int, default=None)
         sub.choices[name].add_argument("--seed", type=int, default=0, help="seed of the sampled draw on CUDA (`batch`: request i uses seed + i)")
+    for name in ("generate", "batch", "score"):
+        sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
+                                       help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")
+    sub.choices["score"].add_argument("--chunk", type=int, default=512, help="prompt tokens per forward pass (bounds the live logits)")
     sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
     sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")
     sub.choices["generate"].add_argument("--proposal-length", type=int, default=4, help="draft tokens proposed per round")
@@ -162,6 +216,8 @@ def main(argv=None) -> int:
     args = ap.parse_args(argv)
     if not args.model and not args.synthetic:
         ap.error("--model or --synthetic is required")
+    if args.logprobs is not None and not 0 <= args.logprobs <= 20:
+        ap.error("--logprobs must be in [0, 20]")
     return args.fn(args)
 
 

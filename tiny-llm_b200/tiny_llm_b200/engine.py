@@ -317,6 +317,16 @@ class DecodeEngine(_GraphEngine):
         self._samp_temperature = self._samp_dev[8 * B : 12 * B].view(torch.float32)
         self._samp_top_k = self._samp_dev[12 * B : 16 * B].view(torch.int32)
         self._samp_top_p = self._samp_dev[16 * B : 20 * B].view(torch.float32)
+        # decode_on_device(logprobs=...): one more graph per (greedy | sampled) step, the same body plus one tl_logprobs
+        # launch on the step's tokens, logging into [log_capacity, B(, max_n)] buffers at the step counter; per-slot
+        # top-N counts in their own pinned block.  All of it is allocated / captured on first use.
+        self._graph_lp: dict = {}
+        self._lp_max_n = None
+        self._lp_log = None
+        self._lp_host = None
+        self._lp_dev = None
+        self._lp_key = None
+        self.kernels_per_logprobs_step = 0
 
     @staticmethod
     def fused_attention_applies(model, slot_tokens: int) -> bool:
@@ -469,6 +479,7 @@ class DecodeEngine(_GraphEngine):
         self._graph = self._graph_of(forward)
         self._graphs = {self.B: self._graph}
         self._graph_sample = None  # captured again on first use, over the current slabs
+        self._graph_lp = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -497,6 +508,48 @@ class DecodeEngine(_GraphEngine):
             self._graph_sample = self._graph_of(sampled_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_sampled_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _ensure_logprobs_graph(self, sampled: bool, max_n: int) -> None:
+        """Capture the self-advancing step with one ``tl_logprobs`` launch after the token choice (targets: the tokens it
+        just wrote), logging at ``step_counter`` (same conditions as ``_ensure_sample_graph``)."""
+        if self._lp_max_n != max_n:
+            B, cap, dev = self.B, self.log_capacity, self.device
+            self._graph_lp = {}
+            self._lp_max_n = max_n
+            self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
+                            torch.zeros((cap, B), dtype=torch.int32, device=dev), torch.zeros((cap, B, max_n), dtype=torch.int32, device=dev),
+                            torch.zeros((cap, B, max_n), dtype=torch.float32, device=dev))
+            if self._lp_host is None:
+                self._lp_host = torch.zeros(B, dtype=torch.int32, pin_memory=True)
+                self._lp_dev = self._lp_host.to(self.device, copy=True)
+            self._lp_key = None
+        if sampled in self._graph_lp:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def logprobs_step():
+            forward(sampled=sampled)
+            ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()  # the warm-up logs at the counter: a previous run may have left it at log_capacity
+            self._graph_lp[sampled] = self._graph_of(logprobs_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_logprobs_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_top_n(self, per: list[int]) -> None:
+        """Write the per-slot top-N counts into their pinned block and upload it if they changed."""
+        key = tuple(per)
+        if key == self._lp_key:
+            return
+        self._host_write_begin()
+        self._lp_host.numpy()[:] = per
+        self._upload_meta(self._lp_dev, self._lp_host)
+        self.h2d_bytes += 4 * self.B
+        self._lp_key = key
 
     def _set_sampling(self, sampling) -> None:
         """Write the per-slot parameters into their pinned block (one ``SamplingParams`` for all slots or one per
@@ -694,25 +747,42 @@ class DecodeEngine(_GraphEngine):
         self.graph_replays += 1
         return self.logits.view(B, 1, self.V), self.next_tokens
 
-    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None) -> torch.Tensor:
+    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
         ``sampling`` (one ``SamplingParams`` or one per slot, None entries greedy) replays the sampled graph instead:
-        slot b's token at position p is ``tl_sample``'s draw with its parameters, p = its offset + 1."""
+        slot b's token at position p is ``tl_sample``'s draw with its parameters, p = its offset + 1.
+        ``logprobs`` (an int N in [0, 20] for every slot, or one per slot) replays the same step with one ``tl_logprobs``
+        launch on the tokens it chose and returns ``(tokens, (logprob [steps, B], rank [steps, B], top_ids [steps, B, N],
+        top_logprobs [steps, B, N]))``, device views of the engine's logs (overwritten by the next call)."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         B = self.B
+        top_n = None
+        if logprobs is not None:
+            from .logprobs import _check_n
+
+            top_n = [_check_n(logprobs)] * B if isinstance(logprobs, int) else [_check_n(0 if n is None else n) for n in logprobs]
+            if len(top_n) != B:
+                raise ValueError(f"logprobs must be one int or a list of {B} (one per slot)")
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
-        if sampling is not None:
+        if top_n is not None:
+            self._ensure_logprobs_graph(sampling is not None, max(top_n))
+            self._set_top_n(top_n)
+        elif sampling is not None:
             self._ensure_sample_graph()
+        if sampling is not None:
             self._set_sampling(sampling)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
-        graph = self._graph_loop if sampling is None else self._graph_sample
+        if top_n is not None:
+            graph = self._graph_lp[sampling is not None]
+        else:
+            graph = self._graph_loop if sampling is None else self._graph_sample
         cur = torch.cuda.current_stream(self.device)
         self._stream.wait_stream(cur)
         with torch.cuda.stream(self._stream):
@@ -722,7 +792,11 @@ class DecodeEngine(_GraphEngine):
                 graph.replay()
         cur.wait_stream(self._stream)
         self.graph_replays += steps
-        return self.out_log[: steps * B].view(steps, B)
+        out = self.out_log[: steps * B].view(steps, B)
+        if top_n is None:
+            return out
+        _, lp, rank, ids, top = self._lp_log
+        return out, (lp[:steps], rank[:steps], ids[:steps], top[:steps])
 
 
 class VerifyEngine(DecodeEngine):

@@ -6,6 +6,7 @@ from __future__ import annotations
 import torch
 
 from .batch import greedy_tokens
+from .logprobs import _check_n, token_logprobs
 from .sampler import sample_tokens
 
 
@@ -16,18 +17,23 @@ def _release_kv_cache(kv_cache) -> None:
 
 
 def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: int | None = None, device=None, on_token=None, sampler=None,
-                        sampling=None):
+                        sampling=None, logprobs: int | None = None):
     """The loop of ``simple_generate_with_kv_cache`` on token ids: the whole
     prompt is prefilled at offset 0 (its last-row logits give the first token),
     then one token per step at a growing offset.  Returns the generated ids.
     ``sampler`` (``make_sampler``; CUDA extension - the reference's cached loop is greedy only) draws
     from ``logits - logsumexp`` instead of taking the arg-max.  ``sampling`` (a ``SamplingParams``) draws each token
     with the seeded ``tl_sample`` kernel instead, at its position in the sequence: the ids equal a prefill plus
-    ``DecodeEngine.decode_on_device(sampling=...)``."""
+    ``DecodeEngine.decode_on_device(sampling=...)``.
+    ``logprobs`` (an int N in [0, 20]) returns ``(ids, entries)`` instead: one ``TokenLogprobs`` per generated id, from
+    the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives)."""
     if sampler is not None and sampling is not None:
         raise ValueError("give sampler or sampling, not both")
+    if logprobs is not None:
+        _check_n(logprobs)
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
+    entries: list = []
     try:
         tokens = torch.as_tensor(list(prompt_ids), dtype=torch.int32, device=device)
         offset = 0
@@ -44,13 +50,15 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
             if eos_token_id is not None and value == eos_token_id:
                 break
             produced.append(value)
+            if logprobs is not None:
+                entries.extend(token_logprobs(logits[:, -1, :], [value], logprobs))
             if on_token is not None:
                 on_token(value)
             offset += tokens.numel()
             tokens = token.reshape(1).to(torch.int32)
     finally:
         _release_kv_cache(kv_cache)
-    return produced
+    return produced if logprobs is None else (produced, entries)
 
 
 def simple_generate_with_kv_cache(model, tokenizer, prompt: str, max_new_tokens: int = 1 << 30) -> str:
