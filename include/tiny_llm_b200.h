@@ -189,6 +189,28 @@ size_t tl_argmax_workspace(int rows, int vocab);
  * No workspace; deterministic. */
 int tl_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
               const int32_t *positions, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* tl_sample with token-history penalties and min-p (DESIGN.md section 8b).  Extra per-row device arrays: repetition,
+ * presence, frequency and min_p (f32), and state (int32 [rows, vocab], read and written) with, for token i of row r,
+ * bit 30 set when i occurs in the request's prompt and bits 0-29 the number of times i has been drawn for the request
+ * so far (the first token, drawn from the last prefill chunk, included).  Repetition applies to prompt and generated
+ * tokens, presence and frequency to generated tokens only (vLLM's semantics).
+ * With s = state[r, i], c = s & (2^30 - 1), seen = (s & 2^30) || c > 0, each staged fp32 logit x becomes, one IEEE
+ * round-to-nearest operation per step and in this order:
+ *   x1 = seen && rep != 1 ? (x > 0 ? x / rep : x * rep) : x;
+ *   x2 = c > 0 ? x1 - fl(freq * (float)c) : x1;
+ *   x3 = c > 0 ? x2 - presence : x2;
+ * (NaN stays NaN).  Everything tl_sample does then runs on the penalised row x3: the first-maximum argmax (so
+ * temperature 0 is greedy on the penalised row), the non-finite-maximum rule, top-k, top-p and the Gumbel draw.
+ * min_p (on for min_p > 0; values above 1 act as 1) adds the bound x >= thr, thr = fl(m + fl(T * L)), m the penalised
+ * maximum and L = log(min_p) in double rounded once to f32: the keep set is {x >= max(x_(k), v*, thr)}, all three
+ * bounds taken over the whole penalised row.  A row with rep == 1, presence == 0 and frequency == 0 does not read its
+ * state, and its draw is tl_sample's.
+ * After the draw, state[r, token] += 1 for every row with positions[r] > 0 (idle decode slots and capture warm-ups
+ * run at position 0 and change nothing).  A draw is a pure function of (logits row, state row, parameters, seed,
+ * position). */
+int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                        const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                        const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
 /* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
  * launch, one cluster of CTAs per row (DESIGN.md section 8a).
  *

@@ -356,6 +356,20 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
     return launch_sample(logits, temperature, top_k, top_p, seed, positions, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
+int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                        const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                        const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_penalized: expected float32, float16, or bfloat16");
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_penalized: bad shape");
+    if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
+    if (rows == 0) return TL_OK;
+    if (!logits || !temperature || !top_k || !top_p || !seed || !positions || !repetition || !presence || !frequency || !min_p || !state ||
+        !out_tokens)
+        return fail(TL_EINVAL, "sample_penalized: null pointer");
+    return launch_sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
+                                   out_tokens, rows, vocab, dtype, as_stream(stream));
+}
+
 int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
                 int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
                 void *stream) {

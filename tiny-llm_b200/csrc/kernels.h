@@ -38,6 +38,9 @@ int launch_argmax(const void *logits, int32_t *out, int rows, int vocab, int dty
 int sample_plan(int vocab, int *cluster, int *slice);
 int launch_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                            const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                            const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
 // logprobs.cu: same cluster plan as sampling.cu
 constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
 int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,

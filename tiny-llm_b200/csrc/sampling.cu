@@ -16,6 +16,12 @@
 //   3. one Gumbel pass: argmax over the kept i of x_i / T + g_i, g_i = -log(-log u_i), u_i from Philox4x32-10 at
 //      counter (i >> 2, pos, 0, 0) and key (seed lo, seed hi); then the cluster argmax.
 // Integer sums and first-maximum-wins merges make every launch give the same bits, whatever the row count.
+//
+// The penalised form (PEN, tl_sample_penalized, DESIGN.md section 8b) reads the row's int32 token state (bit 30: in
+// the prompt, bits 0-29: times drawn) right after staging and rewrites the staged values in place with the repetition,
+// frequency and presence penalties; every later step runs on that penalised row.  min-p adds a third lower bound on
+// the keep threshold after the radix levels, and rank 0 adds 1 to the drawn token's count once every CTA has read
+// its state slice.
 #include <cooperative_groups.h>
 
 #include <climits>
@@ -48,11 +54,32 @@ __device__ __forceinline__ float gumbel(uint32_t w) {
     return -logf(-logf(u));
 }
 
-template <typename T, int LEVELS>
+// Per-row arrays of the penalised form; state is [rows, vocab].  Unused (all null) by the plain form.
+struct Penalties {
+    const float *repetition, *presence, *frequency, *min_p;
+    int32_t *state;
+    int svec;  // the state rows are 16-byte aligned (vocab % 4 == 0 and an aligned base)
+};
+
+constexpr int32_t STATE_PROMPT = 1 << 30;
+constexpr int32_t STATE_COUNT = STATE_PROMPT - 1;
+
+// x1 = seen && r != 1 ? (x > 0 ? x / r : x * r) : x;  x2 = c > 0 ? x1 - f c : x1;  x3 = c > 0 ? x2 - pres : x2, each
+// operation rounded on its own (no contraction into an fma).
+__device__ __forceinline__ float penalize(float x, int32_t s, float r, float pres, float f) {
+    const int32_t c = s & STATE_COUNT;
+    if ((s & STATE_PROMPT) || c > 0) {
+        if (r != 1.f) x = x > 0.f ? __fdiv_rn(x, r) : __fmul_rn(x, r);
+    }
+    if (c > 0) x = __fsub_rn(__fsub_rn(x, __fmul_rn(f, __int2float_rn(c))), pres);
+    return x;
+}
+
+template <typename T, int LEVELS, bool PEN>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restrict__ logits, const float *__restrict__ temperature,
                                                                 const int32_t *__restrict__ top_k, const float *__restrict__ top_p,
                                                                 const int64_t *__restrict__ seed, const int32_t *__restrict__ positions,
-                                                                int32_t *__restrict__ out, int vocab, int slice, int vec) {
+                                                                int32_t *__restrict__ out, int vocab, int slice, int vec, Penalties pen) {
     extern __shared__ float4 smem_dyn[];
     float *xs = reinterpret_cast<float *>(smem_dyn);
     __shared__ unsigned int h_count[2][BINS];  // double-buffered: level l + 2 reuses l's buffer after all remote reads of it
@@ -85,8 +112,28 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     const float temp = temperature[row];
     stage_slice(logits + static_cast<size_t>(row) * vocab + begin, xs, n, vec != 0);
     __syncthreads();
+    if constexpr (PEN) {
+        const float r = pen.repetition[row], pres = pen.presence[row], f = pen.frequency[row];
+        if (r != 1.f || pres != 0.f || f != 0.f) {  // with every penalty off the values stay as staged: no state read
+            const int32_t *st = pen.state + static_cast<size_t>(row) * vocab + begin;
+            if (pen.svec) {  // n is a multiple of 4 here: the slice start is, and so is vocab
+                for (int i = threadIdx.x * 4; i < n; i += SAMPLE_THREADS * 4) {
+                    const int4 s = *reinterpret_cast<const int4 *>(st + i);
+                    float4 x = *reinterpret_cast<const float4 *>(xs + i);
+                    x.x = penalize(x.x, s.x, r, pres, f);
+                    x.y = penalize(x.y, s.y, r, pres, f);
+                    x.z = penalize(x.z, s.z, r, pres, f);
+                    x.w = penalize(x.w, s.w, r, pres, f);
+                    *reinterpret_cast<float4 *>(xs + i) = x;
+                }
+            } else {
+                for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) xs[i] = penalize(xs[i], st[i], r, pres, f);
+            }
+            __syncthreads();
+        }
+    }
 
-    // ---- 1. first-maximum-wins argmax of the raw row
+    // ---- 1. first-maximum-wins argmax of the (penalised) row
     Best mine{-INFINITY, INT_MAX};
     for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) mine = better(mine, Best{xs[i], begin + i});
     mine = warp_best(mine);
@@ -105,7 +152,13 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     __syncthreads();
     const Best best = row_max;
     if (!(temp > 0.f) || !isfinite(best.v)) {
-        if (rank == 0 && threadIdx.x == 0) out[row] = best.i == INT_MAX ? 0 : best.i;
+        if (rank == 0 && threadIdx.x == 0) {
+            const int token = best.i == INT_MAX ? 0 : best.i;
+            out[row] = token;
+            if constexpr (PEN) {  // every CTA read its state slice before the cluster barrier above
+                if (positions[row] > 0) pen.state[static_cast<size_t>(row) * vocab + token] += 1;
+            }
+        }
         cluster.sync();  // no CTA leaves while another may still read its pub_max
         return;
     }
@@ -215,7 +268,14 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
         }
         __syncthreads();
     }
-    const uint32_t tau = s_prefix;
+    uint32_t tau = s_prefix;
+    if constexpr (PEN) {  // min-p: x >= m + T log(min_p), a bound on the whole row like the two above
+        const float mp = pen.min_p[row];
+        if (mp > 0.f) {
+            const float log_p = static_cast<float>(log(static_cast<double>(fminf(mp, 1.f))));
+            tau = max(tau, order_key(__fadd_rn(m, __fmul_rn(temp, log_p))));
+        }
+    }
 
     // ---- 3. Gumbel-max over the kept entries, 4 consecutive entries per Philox call
     const uint32_t pos = static_cast<uint32_t>(positions[row]);
@@ -248,17 +308,22 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     if (rank == 0 && threadIdx.x == 0) {
         Best d{-INFINITY, INT_MAX};
         for (int r = 0; r < C; ++r) d = better(d, *cluster.map_shared_rank(&pub_draw, r));
-        out[row] = d.i == INT_MAX ? best.i : d.i;  // the row maximum is always kept: INT_MAX cannot happen
+        const int token = d.i == INT_MAX ? best.i : d.i;  // the row maximum is always kept: INT_MAX cannot happen
+        out[row] = token;
+        if constexpr (PEN) {
+            if (positions[row] > 0) pen.state[static_cast<size_t>(row) * vocab + token] += 1;
+        }
     }
     cluster.sync();
 }
 
-template <typename T, int LEVELS>
+template <typename T, int LEVELS, bool PEN>
 int launch_sample_t(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
-                    const int32_t *positions, int32_t *out, int rows, int vocab, int cluster, int slice, int vec, cudaStream_t st) {
+                    const int32_t *positions, int32_t *out, int rows, int vocab, int cluster, int slice, int vec, const Penalties &pen,
+                    cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
+        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
             return fail(TL_ECUDA, "sample: cannot raise shared memory limit");
         configured = true;
     }
@@ -277,10 +342,33 @@ int launch_sample_t(const void *logits, const float *temperature, const int32_t 
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl() ? 2 : 1;
     const T *x = static_cast<const T *>(logits);
-    cudaError_t e = cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec);
+    cudaError_t e =
+        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen);
     if (e != cudaSuccess) return fail(TL_ECUDA, "sample: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("sample");
     return TL_OK;
+}
+
+template <bool PEN>
+int launch_sample_any(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                      const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, const Penalties &pen, cudaStream_t st) {
+    if (rows == 0) return TL_OK;
+    int cluster = 0, slice = 0;
+    if (int e = sample_plan(vocab, &cluster, &slice)) return e;
+    const int per16 = dtype == TL_F32 ? 4 : 8;
+    const int vec = (vocab % per16 == 0 && aligned16(logits)) ? 1 : 0;
+    switch (dtype) {
+        case TL_F32:
+            return launch_sample_t<float, 4, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec, pen,
+                                                  st);
+        case TL_F16:
+            return launch_sample_t<__half, 4, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec,
+                                                   pen, st);
+        case TL_BF16:  // a bf16 value's key has 16 significant bits: two levels
+            return launch_sample_t<__nv_bfloat16, 2, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
+                                                           vec, pen, st);
+        default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
+    }
 }
 
 }  // namespace
@@ -298,21 +386,14 @@ int sample_plan(int vocab, int *cluster, int *slice) {
 
 int launch_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
-    if (rows == 0) return TL_OK;
-    int cluster = 0, slice = 0;
-    if (int e = sample_plan(vocab, &cluster, &slice)) return e;
-    const int per16 = dtype == TL_F32 ? 4 : 8;
-    const int vec = (vocab % per16 == 0 && aligned16(logits)) ? 1 : 0;
-    switch (dtype) {
-        case TL_F32:
-            return launch_sample_t<float, 4>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec, st);
-        case TL_F16:
-            return launch_sample_t<__half, 4>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec, st);
-        case TL_BF16:  // a bf16 value's key has 16 significant bits: two levels
-            return launch_sample_t<__nv_bfloat16, 2>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
-                                                      vec, st);
-        default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
-    }
+    return launch_sample_any<false>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{}, st);
+}
+
+int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                            const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                            const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
+    const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    return launch_sample_any<true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, st);
 }
 
 }  // namespace tl

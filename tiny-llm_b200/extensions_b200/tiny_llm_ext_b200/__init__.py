@@ -43,6 +43,7 @@ __all__ = [
     "add",
     "argmax",
     "sample",
+    "sample_penalized",
     "logprobs",
     "LOGPROBS_MAX_N",
     "decode_advance",
@@ -101,6 +102,7 @@ _SIGNATURES = {
     "tl_argmax": (_I, [_VP, _VP, _I, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
+    "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
@@ -635,6 +637,32 @@ def sample(logits, temperature, top_k, top_p, seed, positions, stream=None):
     out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
     _check(_lib.tl_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(), positions.data_ptr(),
                           out.data_ptr(), rows, logits.shape[1], _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+    return out
+
+
+def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None):
+    """``sample`` with token-history penalties and min-p (``tl_sample_penalized``) -> int32 ``[rows]``.  Further
+    per-row device arrays: ``repetition``, ``presence``, ``frequency`` and ``min_p`` float32 ``[rows]``, and ``state``
+    int32 ``[rows, vocab]`` (bit 30: token in the prompt, bits 0-29: times drawn), read, and for rows with
+    ``positions > 0`` incremented at the drawn token."""
+    if logits.dtype not in _FLOATS or logits.dim() != 2:
+        raise RuntimeError("sample_penalized: expected 2D float logits")
+    rows, vocab = logits.shape
+    for name, t, dtype in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+                           ("seed", seed, torch.int64), ("positions", positions, torch.int32), ("repetition", repetition, torch.float32),
+                           ("presence", presence, torch.float32), ("frequency", frequency, torch.float32), ("min_p", min_p, torch.float32)):
+        if t.dtype != dtype or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"sample_penalized: {name} must be {str(dtype).replace('torch.', '')} [{rows}]")
+    if state.dtype != torch.int32 or tuple(state.shape) != (rows, vocab):
+        raise RuntimeError(f"sample_penalized: state must be int32 [{rows}, {vocab}]")
+    named = dict(logits=logits, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, positions=positions, repetition=repetition,
+                 presence=presence, frequency=frequency, min_p=min_p, state=state)
+    _contig("sample_penalized", **named)
+    _gpu("sample_penalized", *named.values())
+    out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
+    _check(_lib.tl_sample_penalized(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                    positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(), min_p.data_ptr(),
+                                    state.data_ptr(), out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
 
 

@@ -24,7 +24,7 @@ from extensions_b200 import tiny_llm_ext_b200
 
 from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, token_logprobs
-from .sampler import sample_tokens, sampling_per_request
+from .sampler import any_penalized, sample_tokens, sampling_per_request, token_state_row
 
 
 def greedy_tokens(logits: torch.Tensor) -> torch.Tensor:
@@ -64,8 +64,10 @@ class Request:
     serving runs, a sequence of token ids (``tokenizer`` may then be ``None``;
     pass ``eos_token_id`` explicitly if one is wanted).  ``sampling`` (a
     ``SamplingParams``) draws the request's tokens with the seeded ``tl_sample``
-    kernel; None keeps them greedy.  ``logprobs`` (an int N) records one
-    ``TokenLogprobs`` per generated token in ``logprob_entries``."""
+    kernel; None keeps them greedy.  A penalised ``sampling`` draws the first
+    token against the prompt-only token state (``token_state_row``).  ``logprobs``
+    (an int N) records one ``TokenLogprobs`` per generated token in
+    ``logprob_entries``."""
 
     def __init__(
         self,
@@ -122,7 +124,13 @@ class Request:
             logits = self.model(ids, [self.offset], self.kv_cache, logits_to_keep=1)[:, -1, :]
             token = None
             if self.offset + chunk == total:
-                token = greedy_tokens(logits) if self.sampling is None else sample_tokens(logits, [self.sampling], [total])
+                if self.sampling is None:
+                    token = greedy_tokens(logits)
+                else:
+                    state = None
+                    if self.sampling.penalized:
+                        state = token_state_row(self.prefill_tokens, [], logits.shape[-1], device=logits.device)[None]
+                    token = sample_tokens(logits, [self.sampling], [total], state)
                 if self.logprobs is not None:
                     entry = token_logprobs(logits, token, self.logprobs)[0]
         self.offset += chunk
@@ -188,7 +196,12 @@ class ContinuousBatcher:
     ``tl_sample`` kernel from its last prefill chunk's and every decode step's logits, and do not depend on its slot or
     on the other requests.  ``logprobs`` (an int N in [0, 20]) fills ``self.logprobs[prompt_idx]`` with one
     ``TokenLogprobs`` per generated token: the first from the prompt's last prefill chunk, the others from the decode
-    step that produced them (one ``ext.logprobs`` launch over all slots per step, idle slots with target -1)."""
+    step that produced them (one ``ext.logprobs`` launch over all slots per step, idle slots with target -1).
+
+    Penalised requests (``SamplingParams.penalized``) keep their token state in one int32 ``[batch_size, vocab]`` slab,
+    allocated when the first of them enters a slot.  From then on every admission rebuilds the slot's row from the
+    prompt and the first token, and every decode step with a penalised slot is one ``tl_sample_penalized`` launch over
+    all slots (idle slots at position 0, so their rows do not change); the kernel counts each drawn token."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
                  eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None):
@@ -231,6 +244,7 @@ class ContinuousBatcher:
         self._gpu_events: list[tuple[str, object, object]] = []  # (kind, start, end) CUDA events on the current stream
         self.peak_active_requests = 0
         self.peak_live_pages = 0
+        self.token_state: torch.Tensor | None = None  # [batch_size, vocab] int32, on first penalised admission
 
     # -- bookkeeping ---------------------------------------------------------
     def idle(self) -> bool:
@@ -267,6 +281,16 @@ class ContinuousBatcher:
         self.peak_active_requests = max(self.peak_active_requests, len(live))
         pages = sum(len(getattr(r.kv_cache[0], "page_ids", ())) for r in live) * len(self.kv_cache)  # layers move in lockstep
         self.peak_live_pages = max(self.peak_live_pages, pages)
+
+    def _admit_state(self, request: Request, slot: int) -> None:
+        """Rebuild the slot's token-state row from the request's prompt and first token (allocating the slab when the
+        first penalised request arrives)."""
+        if self.token_state is None:
+            if request.sampling is None or not request.sampling.penalized:
+                return
+            vocab = self.model.vocab_size
+            self.token_state = torch.zeros((self.batch_size, vocab), dtype=torch.int32, device=request.prefill_tokens.device)
+        token_state_row(request.prefill_tokens, [request.next_token], self.token_state.shape[1], out=self.token_state[slot])
 
     def _budget_spent(self, request: Request) -> bool:
         if self.max_new_tokens is None:
@@ -316,6 +340,7 @@ class ContinuousBatcher:
                         if self.slots[i] is None:
                             for layer_cache, table in zip(request.kv_cache, self.kv_cache):
                                 table.add_request(layer_cache, i)
+                            self._admit_state(request, i)
                             self.slots[i] = request
                             self.pending = None
                             moved = True
@@ -338,8 +363,10 @@ class ContinuousBatcher:
                 logits = self.model(batch, offsets, self.kv_cache, logits_to_keep=1)[:, -1, :]
                 if self.sampling is None:
                     sampled = greedy_tokens(logits)
-                else:
-                    sampled = sample_tokens(logits, [None if s is None else s.sampling for s in self.slots], [o + 1 for o in offsets])
+                else:  # idle slots draw greedily at position 0: a penalised launch leaves their state rows alone
+                    params = [None if s is None else s.sampling for s in self.slots]
+                    positions = [0 if s is None else o + 1 for s, o in zip(self.slots, offsets)]
+                    sampled = sample_tokens(logits, params, positions, self.token_state if any_penalized(params) else None)
                 if self.logprobs_n is not None:
                     live = torch.tensor([s is not None for s in self.slots], device=sampled.device)
                     targets = torch.where(live, sampled.reshape(-1).to(torch.int32), -1)

@@ -8,6 +8,8 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --max-new-tokens 8   (no files needed)
     python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3;9,2,4" --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
         (seeded sampling with the tl_sample kernel: the same seed gives the same tokens)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --sampler-temp 0.7 --presence-penalty 1.5 --min-p 0.05
+        (token-history penalties and min-p; with --sampler-temp 0 the greedy token of the penalised logits)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
@@ -70,6 +72,14 @@ def _print_logprobs(entries, tokenizer, file=None) -> None:
         print(f"  {_token_text(tokenizer, e.token)}\tlogprob {e.logprob:.4f}\trank {e.rank}" + (f"\t| {alts}" if alts else ""), file=file)
 
 
+def _penalties(args) -> dict:
+    """The ``SamplingParams`` penalty fields the flags turn on (an empty dict when every one is off)."""
+    given = dict(repetition_penalty=args.repetition_penalty, presence_penalty=args.presence_penalty,
+                 frequency_penalty=args.frequency_penalty, min_p=args.min_p)
+    off = dict(repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_p=0.0)
+    return {k: v for k, v in given.items() if v != off[k]}
+
+
 def cmd_generate(args) -> int:
     from .generate import greedy_generate_ids
     from .sampler import SamplingParams, make_sampler
@@ -79,9 +89,10 @@ def cmd_generate(args) -> int:
     model = _model(args, ns, name)
     ids = _prompt_ids(args, tokenizer, args.prompt)
     sampler = sampling = None
-    if args.sampler_temp != 0:
-        if device.type == "cuda":  # the seeded kernel
-            sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed)
+    penalties = _penalties(args)
+    if args.sampler_temp != 0 or penalties:
+        if device.type == "cuda" or penalties:  # the seeded kernel
+            sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed, **penalties)
         else:
             sampler = make_sampler(args.sampler_temp, top_p=args.sampler_top_p, top_k=args.sampler_top_k)
     if tokenizer is not None:
@@ -143,8 +154,9 @@ def cmd_batch(args) -> int:
         queue = [tokenizer.apply_chat_template([{"role": "user", "content": p}], tokenize=False, add_generation_prompt=True,
                                                enable_thinking=args.enable_thinking) for p in prompts]
     sampling = None
-    if args.sampler_temp != 0:  # request i draws with seed `--seed + i`
-        sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i)
+    penalties = _penalties(args)
+    if args.sampler_temp != 0 or penalties:  # request i draws with seed `--seed + i`
+        sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i, **penalties)
                     for i in range(len(queue))]
     batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
                                 verbose=not args.quiet, device=device,
@@ -201,6 +213,13 @@ def main(argv=None) -> int:
         sub.choices[name].add_argument("--sampler-top-p", type=float, default=None)
         sub.choices[name].add_argument("--sampler-top-k", type=int, default=None)
         sub.choices[name].add_argument("--seed", type=int, default=0, help="seed of the sampled draw on CUDA (`batch`: request i uses seed + i)")
+        sub.choices[name].add_argument("--repetition-penalty", type=float, default=1.0,
+                                       help="divide positive (multiply negative) logits of prompt and generated tokens (> 0; 1: off)")
+        sub.choices[name].add_argument("--presence-penalty", type=float, default=0.0, help="subtract from the logits of generated tokens")
+        sub.choices[name].add_argument("--frequency-penalty", type=float, default=0.0,
+                                       help="subtract this times the count of each generated token")
+        sub.choices[name].add_argument("--min-p", type=float, default=0.0,
+                                       help="keep tokens at least this fraction as likely as the top one (0: off)")
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")

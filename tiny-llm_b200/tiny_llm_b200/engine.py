@@ -19,7 +19,9 @@ The engine keeps the operator semantics and removes the dispatch:
   (token feedback + position advance by ``tl_decode_advance``, pages allocated
   ahead) - the device-resident number of bench.py.  With ``sampling`` it replays
   a second self-advancing graph that draws each slot's token with the seeded
-  ``tl_sample`` kernel instead of ``tl_argmax``.
+  ``tl_sample`` kernel instead of ``tl_argmax``, and with a penalised slot a
+  third one with ``tl_sample_penalized`` over per-slot token counts kept on the
+  device.
 
 Page slabs must not move while a graph is alive: pools are ``reserve()``d up
 front and the engine re-captures if a slab pointer changes.
@@ -327,6 +329,15 @@ class DecodeEngine(_GraphEngine):
         self._lp_dev = None
         self._lp_key = None
         self.kernels_per_logprobs_step = 0
+        # decode_on_device(sampling=<penalised>): the penalised sampled graph, the per-slot token state [B, V] it reads and
+        # counts into, and the penalty parameters in their own pinned block (repetition | presence | frequency | min_p
+        # f32, B each), all on first use
+        self._graph_pen = None
+        self.kernels_per_penalized_step = 0
+        self.token_counts = None
+        self._pen_host = None
+        self._pen_dev = None
+        self._pen_key = None
 
     @staticmethod
     def fused_attention_applies(model, slot_tokens: int) -> bool:
@@ -341,17 +352,22 @@ class DecodeEngine(_GraphEngine):
         super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
 
     # ------------------------------------------------------------ graph body --
-    def _next_tokens(self, logits, R: int, sampled: bool) -> None:
+    def _next_tokens(self, logits, R: int, sampled: bool, penalized: bool = False) -> None:
         """The step's token per row: ``tl_argmax``, or (the sampled graph) ``tl_sample`` with the per-slot parameters at
-        position ``context_lens``, the index of the token being drawn."""
-        if sampled:
+        position ``context_lens``, the index of the token being drawn, or (the penalised graph) ``tl_sample_penalized``
+        over ``token_counts``."""
+        if penalized:
+            pen = self._pen_dev.view(torch.float32).view(4, self.B)
+            tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
+                                          self.context_lens[:R], pen[0, :R], pen[1, :R], pen[2, :R], pen[3, :R], self.token_counts[:R])
+        elif sampled:
             tokens = ext.sample(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
                                 self.context_lens[:R])
         else:
             tokens = ext.argmax(logits)
         self.next_tokens[:R].copy_(tokens)
 
-    def _forward_unfused(self, sampled: bool = False) -> None:
+    def _forward_unfused(self, sampled: bool = False, penalized: bool = False) -> None:
         """One decode step over the static buffers, operator by operator (the
         call sequence of qwen3_week3.py:55-121,139-146,196-207,320-338 at L == 1)."""
         m = self.model
@@ -383,12 +399,12 @@ class DecodeEngine(_GraphEngine):
         x = _normed(x, m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
         logits = _proj(x, head)
-        self._next_tokens(logits, B, sampled)
+        self._next_tokens(logits, B, sampled, penalized)
         if self.logits is None:
             self.logits = torch.empty_like(logits)
         self.logits.copy_(logits)
 
-    def _forward_fused(self, rows: int | None = None, sampled: bool = False) -> None:
+    def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False) -> None:
         """Same step in ~7 launches per layer: norm / SwiGLU / residual folded into
         the streaming projections, q/k norm + RoPE + K/V append in one kernel.
         Every rounding point of the operator-by-operator sequence is kept.
@@ -405,7 +421,7 @@ class DecodeEngine(_GraphEngine):
             x = self._matvec_layers(x)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
-        self._next_tokens(logits, R, sampled)
+        self._next_tokens(logits, R, sampled, penalized)
         if self.logits is None:
             self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
@@ -479,6 +495,7 @@ class DecodeEngine(_GraphEngine):
         self._graph = self._graph_of(forward)
         self._graphs = {self.B: self._graph}
         self._graph_sample = None  # captured again on first use, over the current slabs
+        self._graph_pen = None
         self._graph_lp = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
@@ -509,9 +526,28 @@ class DecodeEngine(_GraphEngine):
             self.kernels_per_sampled_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
-    def _ensure_logprobs_graph(self, sampled: bool, max_n: int) -> None:
+    def _ensure_penalized_graph(self) -> None:
+        """Capture the penalised sampled self-advancing step (same conditions as ``_ensure_sample_graph``; the warm-up
+        runs at context 0, so it counts nothing)."""
+        if self._graph_pen is not None:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def penalized_step():
+            forward(sampled=True, penalized=True)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self._graph_pen = self._graph_of(penalized_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_penalized_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _ensure_logprobs_graph(self, sampled: bool, max_n: int, penalized: bool = False) -> None:
         """Capture the self-advancing step with one ``tl_logprobs`` launch after the token choice (targets: the tokens it
-        just wrote), logging at ``step_counter`` (same conditions as ``_ensure_sample_graph``)."""
+        just wrote), logging at ``step_counter`` (same conditions as ``_ensure_sample_graph``).  One graph per
+        (sampled, penalized)."""
         if self._lp_max_n != max_n:
             B, cap, dev = self.B, self.log_capacity, self.device
             self._graph_lp = {}
@@ -523,12 +559,12 @@ class DecodeEngine(_GraphEngine):
                 self._lp_host = torch.zeros(B, dtype=torch.int32, pin_memory=True)
                 self._lp_dev = self._lp_host.to(self.device, copy=True)
             self._lp_key = None
-        if sampled in self._graph_lp:
+        if (sampled, penalized) in self._graph_lp:
             return
         forward = self._forward_fused if self.fused else self._forward_unfused
 
         def logprobs_step():
-            forward(sampled=sampled)
+            forward(sampled=sampled, penalized=penalized)
             ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
             ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
 
@@ -536,7 +572,7 @@ class DecodeEngine(_GraphEngine):
             self._stream.wait_stream(torch.cuda.current_stream(self.device))
             self._set_idle()
             self.step_counter.zero_()  # the warm-up logs at the counter: a previous run may have left it at log_capacity
-            self._graph_lp[sampled] = self._graph_of(logprobs_step, pool=self._graph.pool(), warmups=1)
+            self._graph_lp[(sampled, penalized)] = self._graph_of(logprobs_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_logprobs_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
@@ -551,15 +587,54 @@ class DecodeEngine(_GraphEngine):
         self.h2d_bytes += 4 * self.B
         self._lp_key = key
 
-    def _set_sampling(self, sampling) -> None:
-        """Write the per-slot parameters into their pinned block (one ``SamplingParams`` for all slots or one per
-        slot, None: greedy) and upload it if they changed."""
-        from .sampler import SamplingParams, sampling_tensors
+    def _per_slot_sampling(self, sampling) -> list:
+        from .sampler import SamplingParams
 
         B = self.B
         per = [sampling] * B if isinstance(sampling, SamplingParams) else list(sampling)
         if len(per) != B or not all(p is None or isinstance(p, SamplingParams) for p in per):
             raise ValueError(f"sampling must be one SamplingParams or a list of {B} (one per slot)")
+        return per
+
+    def _alloc_penalties(self) -> None:
+        """The token counts and the penalty block, on first use (before the penalised graphs are captured over them)."""
+        if self.token_counts is None:
+            self.token_counts = torch.zeros((self.B, self.V), dtype=torch.int32, device=self.device)
+            self._pen_host = torch.zeros(16 * self.B, dtype=torch.uint8, pin_memory=True)
+            self._pen_dev = self._pen_host.to(self.device, copy=True)
+
+    def _set_penalties(self, per: list, history) -> None:
+        """Rebuild the token-count rows ``history`` gives (per slot ``(prompt_ids, generated_ids)`` or None: keep the
+        row) and upload the penalty parameters if they changed."""
+        from .sampler import penalty_tensors, token_state_row
+
+        B = self.B
+        if history is not None:
+            history = list(history)
+            if len(history) != B:
+                raise ValueError(f"history must hold one (prompt_ids, generated_ids) or None per slot ({B})")
+            for b, h in enumerate(history):
+                if h is not None:
+                    prompt_ids, generated_ids = h
+                    token_state_row(prompt_ids, generated_ids, self.V, out=self.token_counts[b])
+        key = tuple(per)
+        if key == self._pen_key:
+            return
+        self._host_write_begin()
+        host = self._pen_host.numpy()
+        for j, t in enumerate(penalty_tensors(per, "cpu")):
+            host[4 * B * j : 4 * B * (j + 1)] = t.numpy().view(np.uint8)
+        self._upload_meta(self._pen_dev, self._pen_host)
+        self.h2d_bytes += 16 * B
+        self._pen_key = key
+
+    def _set_sampling(self, sampling) -> None:
+        """Write the per-slot parameters into their pinned block (one ``SamplingParams`` for all slots or one per
+        slot, None: greedy) and upload it if they changed."""
+        from .sampler import sampling_tensors
+
+        B = self.B
+        per = self._per_slot_sampling(sampling)
         key = tuple(per)
         if key == self._samp_key:
             return
@@ -747,7 +822,7 @@ class DecodeEngine(_GraphEngine):
         self.graph_replays += 1
         return self.logits.view(B, 1, self.V), self.next_tokens
 
-    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None):
+    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
@@ -755,7 +830,11 @@ class DecodeEngine(_GraphEngine):
         slot b's token at position p is ``tl_sample``'s draw with its parameters, p = its offset + 1.
         ``logprobs`` (an int N in [0, 20] for every slot, or one per slot) replays the same step with one ``tl_logprobs``
         launch on the tokens it chose and returns ``(tokens, (logprob [steps, B], rank [steps, B], top_ids [steps, B, N],
-        top_logprobs [steps, B, N]))``, device views of the engine's logs (overwritten by the next call)."""
+        top_logprobs [steps, B, N]))``, device views of the engine's logs (overwritten by the next call).
+        With a penalised slot in ``sampling`` the step is ``tl_sample_penalized`` over ``token_counts [B, V]``, which
+        it updates at every drawn token.  ``history`` (per slot ``(prompt_ids, generated_ids)``, or None) rebuilds those
+        slots' rows first; None continues from the rows as the engine holds them.  A call without a penalised slot
+        replays the graphs it would without penalties and does not read ``history``."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         B = self.B
@@ -766,21 +845,34 @@ class DecodeEngine(_GraphEngine):
             top_n = [_check_n(logprobs)] * B if isinstance(logprobs, int) else [_check_n(0 if n is None else n) for n in logprobs]
             if len(top_n) != B:
                 raise ValueError(f"logprobs must be one int or a list of {B} (one per slot)")
+        penalized = False
+        if sampling is not None:
+            from .sampler import any_penalized
+
+            penalized = any_penalized(self._per_slot_sampling(sampling))
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
+        if penalized:
+            self._alloc_penalties()
         if top_n is not None:
-            self._ensure_logprobs_graph(sampling is not None, max(top_n))
+            self._ensure_logprobs_graph(sampling is not None, max(top_n), penalized)
             self._set_top_n(top_n)
+        elif penalized:
+            self._ensure_penalized_graph()
         elif sampling is not None:
             self._ensure_sample_graph()
         if sampling is not None:
             self._set_sampling(sampling)
+        if penalized:
+            self._set_penalties(self._per_slot_sampling(sampling), history)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
         if top_n is not None:
-            graph = self._graph_lp[sampling is not None]
+            graph = self._graph_lp[(sampling is not None, penalized)]
+        elif penalized:
+            graph = self._graph_pen
         else:
             graph = self._graph_loop if sampling is None else self._graph_sample
         cur = torch.cuda.current_stream(self.device)

@@ -7,7 +7,7 @@ import torch
 
 from .batch import greedy_tokens
 from .logprobs import _check_n, token_logprobs
-from .sampler import sample_tokens
+from .sampler import sample_tokens, token_state_row
 
 
 def _release_kv_cache(kv_cache) -> None:
@@ -24,7 +24,8 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     ``sampler`` (``make_sampler``; CUDA extension - the reference's cached loop is greedy only) draws
     from ``logits - logsumexp`` instead of taking the arg-max.  ``sampling`` (a ``SamplingParams``) draws each token
     with the seeded ``tl_sample`` kernel instead, at its position in the sequence: the ids equal a prefill plus
-    ``DecodeEngine.decode_on_device(sampling=...)``.
+    ``DecodeEngine.decode_on_device(sampling=...)``.  A penalised ``sampling`` keeps the request's ``[1, vocab]`` token
+    state, built from the prompt; each launch counts the token it draws.
     ``logprobs`` (an int N in [0, 20]) returns ``(ids, entries)`` instead: one ``TokenLogprobs`` per generated id, from
     the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives)."""
     if sampler is not None and sampling is not None:
@@ -34,13 +35,16 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
     entries: list = []
+    state = None
     try:
         tokens = torch.as_tensor(list(prompt_ids), dtype=torch.int32, device=device)
         offset = 0
         while len(produced) < max_new_tokens:
             logits = model(tokens[None], offset, kv_cache, logits_to_keep=1)
             if sampling is not None:
-                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()])
+                if sampling.penalized and state is None:
+                    state = token_state_row(tokens, [], logits.shape[-1], device=logits.device)[None]
+                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state)
             elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])
             else:

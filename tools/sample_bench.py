@@ -2,8 +2,10 @@
 
 * ``tl_argmax`` against ``tl_sample`` with temperature only, top-k 50, top-p 0.9 and both, and ``make_sampler`` (torch
   ops: sort + cumsum + multinomial) on the same rows, at 1, 8 and 64 rows (CUDA events over 200 launches);
-* ``decode_on_device`` tok/s, greedy against sampled (temperature 0.7, top-p 0.9, top-k 50), at B = 1 and B = 64 on
-  Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
+* ``tl_sample_penalized`` (repetition 1.1, presence 0.5, frequency 0.3, with and without min-p 0.05; temperature 0.7,
+  top-p 0.9, top-k 50) against ``tl_sample`` with the same top-k / top-p, same rows, random token states;
+* ``decode_on_device`` tok/s, greedy against sampled (temperature 0.7, top-p 0.9, top-k 50) and sampled with those
+  penalties, at B = 1 and B = 64 on Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
 
   python tools/sample_bench.py [--out tools_out/sample_bench.json]
 """
@@ -23,12 +25,13 @@ sys.path[:0] = [str(ROOT), str(ROOT / "tiny-llm_b200")]
 from extensions_b200 import tiny_llm_ext_b200 as ext  # noqa: E402
 from tiny_llm_b200 import BatchingKvCache, Qwen3ModelWeek3, SamplingParams, make_sampler  # noqa: E402
 from tiny_llm_b200.engine import DecodeEngine  # noqa: E402
-from tiny_llm_b200.sampler import sampling_tensors  # noqa: E402
+from tiny_llm_b200.sampler import penalty_tensors, sampling_tensors  # noqa: E402
 from tiny_llm_b200.synthetic import synthetic_qwen3  # noqa: E402
 
 DEV = torch.device("cuda:0")
 V = 151936
 CONFIGS = {"temperature": dict(), "top_k 50": dict(top_k=50), "top_p 0.9": dict(top_p=0.9), "both": dict(top_k=50, top_p=0.9)}
+PENALTIES = dict(repetition_penalty=1.1, presence_penalty=0.5, frequency_penalty=0.3)
 
 
 def card() -> str:
@@ -64,13 +67,21 @@ def kernel_table() -> dict:
             sampler = make_sampler(0.7, top_p=kw.get("top_p"), top_k=kw.get("top_k"), generator=torch.Generator(device=DEV).manual_seed(0))
             lp = torch.log_softmax(logits.float(), dim=-1)
             res[f"make_sampler {name}"] = timed(lambda: sampler(lp), reps=50)
+        # the penalised kernel on the same rows; positions 0 keep the states as they are across the repetitions
+        state = torch.randint(0, 3, (rows, V), generator=g, device=DEV, dtype=torch.int32)
+        zero = torch.zeros(rows, dtype=torch.int32, device=DEV)
+        for name, kw in (("penalties", PENALTIES), ("penalties + min_p 0.05", dict(PENALTIES, min_p=0.05))):
+            params = [SamplingParams(0.7, top_k=50, top_p=0.9, seed=i, **kw) for i in range(rows)]
+            t, k, p, s = sampling_tensors(params, DEV)
+            pen = penalty_tensors(params, DEV)
+            res[f"sample_penalized {name}"] = timed(lambda: ext.sample_penalized(logits, t, k, p, s, zero, *pen, state))
         out[rows] = res
         print(f"rows {rows}: " + ", ".join(f"{k} {v:.1f} us" for k, v in res.items()), flush=True)
     return out
 
 
 def decode_rates(model, B, ctx=128, steps=64, rounds=3) -> dict:
-    msl = ctx + 2 * (rounds + 1) * steps + 64
+    msl = ctx + 3 * (rounds + 1) * steps + 64
     engine = DecodeEngine(model, B, msl, DEV)
     engine.reserve_pools()
     tables = [BatchingKvCache(max_active_requests=B, max_seq_len=msl) for _ in range(model.num_hidden_layers)]
@@ -79,14 +90,15 @@ def decode_rates(model, B, ctx=128, steps=64, rounds=3) -> dict:
         for c, t in zip(cache, tables):
             c.append_slots(ctx)
             t.add_request(c, b)
-    sampling = SamplingParams(0.7, top_k=50, top_p=0.9, seed=1)
+    modes = {"greedy": None, "sampled": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1),
+             "penalized": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, **PENALTIES)}
     offsets, tokens = [ctx] * B, [1] * B
-    times = {"greedy": [], "sampled": []}
+    times = {m: [] for m in modes}
     for r in range(rounds + 1):
-        for mode in ("greedy", "sampled"):
+        for mode, sampling in modes.items():
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            log = engine.decode_on_device(tokens, offsets, tables, steps, sampling=None if mode == "greedy" else sampling)
+            log = engine.decode_on_device(tokens, offsets, tables, steps, sampling=sampling)
             b.record()
             b.synchronize()
             tokens = log[-1].tolist()
@@ -95,9 +107,11 @@ def decode_rates(model, B, ctx=128, steps=64, rounds=3) -> dict:
                 times[mode].append(a.elapsed_time(b))
     res = {m: B * steps * len(v) / (sum(v) / 1e3) for m, v in times.items()}
     res["step_ms"] = {m: sum(v) / len(v) / steps for m, v in times.items()}
-    res["kernels_per_step"] = {"greedy": engine.kernels_per_step, "sampled": engine.kernels_per_sampled_step}
+    res["kernels_per_step"] = {"greedy": engine.kernels_per_step, "sampled": engine.kernels_per_sampled_step,
+                               "penalized": engine.kernels_per_penalized_step}
     print(f"B {B}: greedy {res['greedy']:.1f} tok/s, sampled {res['sampled']:.1f} tok/s "
-          f"({(res['sampled'] / res['greedy'] - 1) * 100:+.2f} %)", flush=True)
+          f"({(res['sampled'] / res['greedy'] - 1) * 100:+.2f} %), penalized {res['penalized']:.1f} tok/s "
+          f"({(res['penalized'] / res['sampled'] - 1) * 100:+.2f} % against sampled)", flush=True)
     return res
 
 
