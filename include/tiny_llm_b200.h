@@ -320,6 +320,28 @@ typedef struct tl_page_span_list {
 int tl_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *keys, const void *values,
                                 const tl_page_span_list *spans, int num_pages, int heads, int page_size, int head_dim,
                                 long long src_head_stride, long long src_token_stride, int dtype, void *stream);
+/* Prefix copy-on-write (prefix caching): for every record i of `copies`, in ONE launch,
+ *   key_slab[layer][dst, :, 0:slots, :] = key_slab[layer][src, :, 0:slots, :]   (and the same for values)
+ * over slabs [num_pages[layer], heads, page_size, head_dim] that share heads, page_size, head_dim and dtype.
+ * Rows at or beyond `slots` of the destination are not written; the source is never written.  Both records are
+ * HOST pointers passed by value to the kernel: together 3.3 KiB, under the 4 KiB kernel-parameter limit, so a
+ * longer list goes out as several launches.  Checked before any device call: dtype, layer < slabs->n, both pages
+ * inside that layer's slab, 1 <= slots <= page_size, src != dst, no destination named twice in one layer and no
+ * page that is a destination and a source in one layer (the records of a launch run concurrently). */
+#define TL_PREFIX_COPY_LAYERS 64
+#define TL_PREFIX_COPIES 128
+typedef struct tl_kv_slab_table {
+    void *key[TL_PREFIX_COPY_LAYERS];
+    void *value[TL_PREFIX_COPY_LAYERS];
+    int32_t num_pages[TL_PREFIX_COPY_LAYERS];
+    int32_t n;
+} tl_kv_slab_table;
+typedef struct tl_prefix_copy_list {
+    int32_t layer[TL_PREFIX_COPIES], src[TL_PREFIX_COPIES], dst[TL_PREFIX_COPIES], slots[TL_PREFIX_COPIES];
+    int32_t n;
+} tl_prefix_copy_list;
+int tl_paged_cache_copy_prefix(const tl_kv_slab_table *slabs, const tl_prefix_copy_list *copies, int heads, int page_size,
+                               int head_dim, int dtype, void *stream);
 /* Fused decode attention, L == 1 (bf16, head_dim 128, <= 4 query heads per KV head): per-head
  * q/k RMSNorm + RoPE, append of the newest K/V row and paged GQA attention in ONE launch (plus a
  * merge launch when the context is split over several CTAs).  Replaces, with the same rounding

@@ -266,6 +266,34 @@ int tl_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *
                                            src_token_stride, dtype, as_stream(stream));
 }
 
+int tl_paged_cache_copy_prefix(const tl_kv_slab_table *slabs, const tl_prefix_copy_list *copies, int heads, int page_size,
+                               int head_dim, int dtype, void *stream) {
+    if (dtype != TL_F32 && dtype != TL_BF16) return fail(TL_EDTYPE, "paged_cache_copy_prefix: float32 or bfloat16 pages required");
+    if (!slabs || slabs->n < 0 || slabs->n > TL_PREFIX_COPY_LAYERS) return fail(TL_EINVAL, "paged_cache_copy_prefix: bad slab table");
+    if (!copies || copies->n < 0 || copies->n > TL_PREFIX_COPIES) return fail(TL_EINVAL, "paged_cache_copy_prefix: bad copy list");
+    if (heads <= 0 || page_size <= 0 || head_dim <= 0) return fail(TL_EINVAL, "paged_cache_copy_prefix: bad shape");
+    for (int i = 0; i < copies->n; ++i) {
+        const int layer = copies->layer[i], src = copies->src[i], dst = copies->dst[i], slots = copies->slots[i];
+        if (layer < 0 || layer >= slabs->n) return fail(TL_EINVAL, "paged_cache_copy_prefix: record %d names layer %d of %d", i, layer, slabs->n);
+        if (!slabs->key[layer] || !slabs->value[layer]) return fail(TL_EINVAL, "paged_cache_copy_prefix: null slab of layer %d", layer);
+        const int pages = slabs->num_pages[layer];
+        if (src < 0 || src >= pages || dst < 0 || dst >= pages)
+            return fail(TL_EINVAL, "paged_cache_copy_prefix: record %d: page outside the %d pages of layer %d", i, pages, layer);
+        if (slots < 1 || slots > page_size)
+            return fail(TL_EINVAL, "paged_cache_copy_prefix: record %d: slots %d outside [1, %d]", i, slots, page_size);
+        if (src == dst) return fail(TL_EINVAL, "paged_cache_copy_prefix: record %d copies page %d onto itself", i, src);
+        for (int j = 0; j < i; ++j) {
+            if (copies->layer[j] != layer) continue;
+            if (copies->dst[j] == dst)
+                return fail(TL_EINVAL, "paged_cache_copy_prefix: destination page %d named twice in layer %d", dst, layer);
+            if (copies->dst[j] == src || copies->src[j] == dst)  // the records would race within the launch
+                return fail(TL_EINVAL, "paged_cache_copy_prefix: page %d is both a source and a destination in layer %d",
+                            copies->dst[j] == src ? src : dst, layer);
+        }
+    }
+    return launch_paged_cache_copy_prefix(*slabs, *copies, heads, page_size, head_dim, dtype, as_stream(stream));
+}
+
 size_t tl_paged_attention_workspace(int rows, int L, int D, int /*num_kv_heads*/, int /*num_heads*/, int dtype) {
     // partial O, running max and sum of every query row and split of the split-KV decode kernels
     if (L > PAGED_DECODE_ROWS || dtype != TL_BF16 || D != PAGED_D) return 0;

@@ -485,6 +485,52 @@ int launch_paged_cache_append_chunk(void *key_pages, void *value_pages, const vo
     return TL_OK;
 }
 
+// Prefix copy-on-write: record blockIdx.y, K (blockIdx.z == 0) or V (1).  A (page, head) is one contiguous run of
+// page_size * dvec vectors, of which the first slots * dvec are copied.  Plain 16-byte loads and stores: every run is
+// contiguous and the copy has no reuse, so staging it through shared memory (cp.async.bulk) would add a barrier per
+// run without saving a byte of HBM traffic.
+template <typename V>
+__global__ void paged_cache_copy_prefix_kernel(const tl_kv_slab_table slabs, const tl_prefix_copy_list copies, int heads,
+                                               int page_size, int dvec) {
+    const int c = blockIdx.y;
+    const int layer = copies.layer[c], slots = copies.slots[c];
+    V *slab = static_cast<V *>(blockIdx.z == 0 ? slabs.key[layer] : slabs.value[layer]);
+    const size_t page_elems = static_cast<size_t>(heads) * page_size * dvec;
+    const V *__restrict__ src = slab + static_cast<size_t>(copies.src[c]) * page_elems;
+    V *__restrict__ dst = slab + static_cast<size_t>(copies.dst[c]) * page_elems;
+    const int run = slots * dvec, head_stride = page_size * dvec;
+    const int total = heads * run;
+    for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
+        const int h = idx / run, e = idx - h * run;
+        const size_t at = static_cast<size_t>(h) * head_stride + e;
+        dst[at] = src[at];
+    }
+}
+
+int launch_paged_cache_copy_prefix(const tl_kv_slab_table &slabs, const tl_prefix_copy_list &copies, int heads, int page_size,
+                                   int head_dim, int dtype, cudaStream_t st) {
+    if (copies.n == 0) return TL_OK;
+    const int esize = dtype == TL_F32 ? 4 : 2;
+    bool vec = (head_dim * esize) % 16 == 0;
+    for (int i = 0; i < copies.n && vec; ++i)
+        vec = aligned16(slabs.key[copies.layer[i]]) && aligned16(slabs.value[copies.layer[i]]);
+    int longest = 0;
+    for (int i = 0; i < copies.n; ++i) longest = copies.slots[i] > longest ? copies.slots[i] : longest;
+    const int threads = 256;
+    const int dvec = vec ? head_dim * esize / 16 : head_dim;
+    // 16 CTAs of 256 threads cover a whole 128-slot page of 8 heads x 128 dims in 4 bf16 vectors per thread
+    const long long work = static_cast<long long>(heads) * longest * dvec;
+    dim3 grid(static_cast<unsigned>(std::min<long long>(ceil_div_ll(work, threads), 16)), copies.n, 2);
+    if (vec)
+        paged_cache_copy_prefix_kernel<uint4><<<grid, threads, 0, st>>>(slabs, copies, heads, page_size, dvec);
+    else if (esize == 4)
+        paged_cache_copy_prefix_kernel<uint32_t><<<grid, threads, 0, st>>>(slabs, copies, heads, page_size, dvec);
+    else
+        paged_cache_copy_prefix_kernel<uint16_t><<<grid, threads, 0, st>>>(slabs, copies, heads, page_size, dvec);
+    TL_LAUNCH_CHECK("paged_cache_copy_prefix");
+    return TL_OK;
+}
+
 // Decode-batch append: row b owns token ctx[b]-1; page id and slot are read
 // from device memory (graph-replayable).  keys/values [B, H, 1, D].
 template <typename V>

@@ -26,6 +26,8 @@ int launch_paged_cache_update(void *pages, const void *values, int heads, int pa
 int launch_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *keys, const void *values,
                                     const tl_page_span_list &spans, int heads, int page_size, int head_dim, long long src_head_stride,
                                     long long src_token_stride, int dtype, cudaStream_t st);
+int launch_paged_cache_copy_prefix(const tl_kv_slab_table &slabs, const tl_prefix_copy_list &copies, int heads, int page_size,
+                                   int head_dim, int dtype, cudaStream_t st);
 int launch_paged_cache_append_decode(void *key_pages, void *value_pages, const void *keys, const void *values,
                                      const int32_t *block_table, const int32_t *context_lens, int batch,
                                      int num_pages, int heads, int page_size, int head_dim, int max_pages, int dtype,

@@ -40,6 +40,7 @@ __all__ = [
     # CUDA extension
     "paged_attention_route",
     "paged_cache_append_decode",
+    "paged_cache_copy_prefix",
     "add",
     "argmax",
     "sample",
@@ -117,6 +118,7 @@ _SIGNATURES = {
     "tl_decode_attention_fused_rows_workspace": (_SZ, [_I, _I, _I, _I]),
     "tl_decode_attention_fused_rows": (_I, [_VP] * 11 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP]),
     "tl_paged_cache_append_chunk": (_I, [_VP] * 5 + [_I] * 4 + [ctypes.c_longlong, ctypes.c_longlong, _I, _VP]),
+    "tl_paged_cache_copy_prefix": (_I, [_VP, _VP] + [_I] * 4 + [_VP]),
     "tl_set_pdl": (_I, [_I]),
     "tl_moe_topk": (_I, [_VP] * 4 + [_I] * 5 + [_VP]),
     "tl_moe_tile_table_size": (_I, [_I] * 3),
@@ -495,6 +497,94 @@ def paged_cache_append_chunk(key_pages, value_pages, keys, values, spans, stream
                                              P, H, page_size, D, keys.stride(1), keys.stride(2), _DTYPE_CODE[key_pages.dtype],
                                              _stream_ptr(stream, key_pages))
         )
+
+
+PREFIX_COPY_LAYERS = 64
+PREFIX_COPIES = 128
+
+
+class KvSlabTable(ctypes.Structure):
+    """``tl_kv_slab_table``: per layer, the K and V slab base pointers and the slab's page count (up to 64 layers)."""
+
+    _fields_ = [("key", ctypes.c_void_p * PREFIX_COPY_LAYERS), ("value", ctypes.c_void_p * PREFIX_COPY_LAYERS),
+                ("num_pages", ctypes.c_int32 * PREFIX_COPY_LAYERS), ("n", ctypes.c_int32)]
+
+
+class PrefixCopyList(ctypes.Structure):
+    """``tl_prefix_copy_list``: (layer, source page, destination page, slots) of up to 128 copies."""
+
+    _fields_ = [("layer", ctypes.c_int32 * PREFIX_COPIES), ("src", ctypes.c_int32 * PREFIX_COPIES), ("dst", ctypes.c_int32 * PREFIX_COPIES),
+                ("slots", ctypes.c_int32 * PREFIX_COPIES), ("n", ctypes.c_int32)]
+
+
+def check_prefix_copies(key_slabs, value_slabs, copies) -> list[tuple[int, int, int, int]]:
+    """Every check of ``paged_cache_copy_prefix`` that needs no device: the slabs (one ``[P, H, page_size, D]`` K and V
+    per layer, one dtype, shared H / page_size / D, P per layer) and the records.  Returns the records as int tuples."""
+    if len(key_slabs) != len(value_slabs) or not key_slabs:
+        raise RuntimeError("paged_cache_copy_prefix: one key and one value slab per layer required")
+    dtype, shape = key_slabs[0].dtype, tuple(key_slabs[0].shape[1:])
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise RuntimeError("paged_cache_copy_prefix: float32 or bfloat16 pages required")
+    for k, v in zip(key_slabs, value_slabs):
+        if k.dtype != dtype or v.dtype != dtype:
+            raise RuntimeError("paged_cache_copy_prefix: every slab must have the same float32 or bfloat16 dtype")
+        if k.dim() != 4 or k.shape != v.shape or tuple(k.shape[1:]) != shape:
+            raise RuntimeError("paged_cache_copy_prefix: expected K/V slabs [P, H, page_size, D] with one H, page_size and D")
+    page_size = shape[1]
+    out, dsts, srcs = [], set(), set()
+    for rec in copies:
+        layer, src, dst, slots = (int(x) for x in rec)
+        if not 0 <= layer < len(key_slabs):
+            raise RuntimeError(f"paged_cache_copy_prefix: layer {layer} outside the {len(key_slabs)} slabs")
+        pages = key_slabs[layer].shape[0]
+        if not (0 <= src < pages and 0 <= dst < pages):
+            raise RuntimeError(f"paged_cache_copy_prefix: page outside the {pages} pages of layer {layer}")
+        if not 1 <= slots <= page_size:
+            raise RuntimeError(f"paged_cache_copy_prefix: slots {slots} outside [1, {page_size}]")
+        if src == dst:
+            raise RuntimeError(f"paged_cache_copy_prefix: page {src} copied onto itself")
+        if (layer, dst) in dsts:
+            raise RuntimeError(f"paged_cache_copy_prefix: destination page {dst} named twice in layer {layer}")
+        if (layer, dst) in srcs or (layer, src) in dsts:
+            raise RuntimeError(f"paged_cache_copy_prefix: a page is both a source and a destination in layer {layer}")
+        dsts.add((layer, dst))
+        srcs.add((layer, src))
+        out.append((layer, src, dst, slots))
+    return out
+
+
+def paged_cache_copy_prefix(key_slabs, value_slabs, copies, stream=None):
+    """Copy on write of shared KV pages: for each ``(layer, src_page, dst_page, slots)`` of ``copies``,
+    ``key_slabs[layer][dst, :, :slots] = key_slabs[layer][src, :, :slots]`` and the same for values.  Rows at or beyond
+    ``slots`` of the destination and the source are not written.  One launch per 64 layers and 128 records."""
+    recs = check_prefix_copies(key_slabs, value_slabs, copies)
+    _gpu("paged_cache_copy_prefix", *key_slabs, *value_slabs)
+    for t in (*key_slabs, *value_slabs):
+        if not t.is_contiguous():
+            raise RuntimeError("paged_cache_copy_prefix: slabs must be contiguous")
+    if not recs:
+        return
+    _, H, page_size, D = key_slabs[0].shape
+    for base in range(0, len(key_slabs), PREFIX_COPY_LAYERS):
+        group = [r for r in recs if base <= r[0] < base + PREFIX_COPY_LAYERS]
+        if not group:
+            continue
+        table = KvSlabTable()
+        layers = range(base, min(base + PREFIX_COPY_LAYERS, len(key_slabs)))
+        table.n = len(layers)
+        for i, layer in enumerate(layers):
+            table.key[i], table.value[i] = key_slabs[layer].data_ptr(), value_slabs[layer].data_ptr()
+            table.num_pages[i] = key_slabs[layer].shape[0]
+        for first in range(0, len(group), PREFIX_COPIES):
+            part = group[first : first + PREFIX_COPIES]
+            rec = PrefixCopyList()
+            rec.n = len(part)
+            for i, (layer, src, dst, slots) in enumerate(part):
+                rec.layer[i], rec.src[i], rec.dst[i], rec.slots[i] = layer - base, src, dst, slots
+            _check(
+                _lib.tl_paged_cache_copy_prefix(ctypes.byref(table), ctypes.byref(rec), H, page_size, D, _DTYPE_CODE[key_slabs[0].dtype],
+                                                _stream_ptr(stream, key_slabs[0]))
+            )
 
 
 def paged_attention(

@@ -64,9 +64,11 @@ def scaled_dot_product_attention_grouped(query, key, value, scale=None, mask=Non
 
 def _raise_first_metadata_error(ctx_rows, table_rows, page_size, max_pages, num_physical_pages, L) -> None:
     """The reference's row-by-row scan (attention.py:133-158); run only after the
-    vectorised pre-check found a violation, to raise the identical first error."""
-    seen: set[int] = set()
+    vectorised pre-check found a violation, to raise the identical first error.
+    A page may be live in several rows (a prompt prefix shared through the prefix
+    cache), never twice in one row."""
     for b, (ctx, row) in enumerate(zip(ctx_rows, table_rows)):
+        seen: set[int] = set()
         if ctx < 0:
             raise ValueError(f"context_lens[{b}] must be nonnegative")
         live = (ctx + page_size - 1) // page_size
@@ -93,11 +95,12 @@ def validate_paged_metadata(ctx: np.ndarray, table: np.ndarray, page_size: int, 
     live_pages = (ctx64 + page_size - 1) // page_size
     live = np.arange(max_pages, dtype=np.int64)[None, :] < live_pages[:, None]
     ids = table[live]
+    in_row = np.nonzero(live)[0].astype(np.int64) * max(num_physical_pages, 1) + ids  # distinct while ids are in range
     clean = (
         not (ctx64 < 0).any()
         and not (live_pages > max_pages).any()
         and not ((ids < 0) | (ids >= num_physical_pages)).any()
-        and np.unique(ids).size == ids.size
+        and np.unique(in_row).size == in_row.size
         and not (table[~live] != -1).any()
         and not ((ctx64 > 0) & (ctx64 < L)).any()
     )

@@ -81,6 +81,7 @@ class Request:
         device=None,
         sampling=None,
         logprobs=None,
+        prefix_cache=None,
     ):
         self.prompt = prompt
         self.sampling = sampling
@@ -109,6 +110,13 @@ class Request:
         self.next_token = None
         self.offset = 0
         self.prompt_idx = prompt_idx
+        # prefix caching: the request starts on the cached pages of the longest indexed prefix of its prompt and
+        # prefills from there; its prompt is indexed once prefilled
+        self.prefix_cache = prefix_cache
+        self.prompt_ids = ids if prefix_cache is not None else None
+        self.reused_tokens = 0
+        if prefix_cache is not None:
+            self.reused_tokens = self.offset = prefix_cache.adopt(prefix_cache.lookup(ids), self.kv_cache)
 
     def try_prefill(self):
         """Advance the prompt by at most ``prefill_max_step`` tokens (batch.py:48-76)."""
@@ -138,6 +146,8 @@ class Request:
             layer_cache.materialize()
         if self.offset == total:
             self.is_prefill_done = True
+            if self.prefix_cache is not None:
+                self.prefix_cache.insert(self.prompt_ids, self.kv_cache)
             if self.max_seq_len is not None and self.offset >= self.max_seq_len:
                 self.is_done = True
                 self.finish_reason = "max seq len"
@@ -198,13 +208,18 @@ class ContinuousBatcher:
     ``TokenLogprobs`` per generated token: the first from the prompt's last prefill chunk, the others from the decode
     step that produced them (one ``ext.logprobs`` launch over all slots per step, idle slots with target -1).
 
+    ``prefix_cache=True`` turns on the model's prefix index (``Qwen3ModelWeek3.enable_prefix_cache``): a request
+    admitted to prefill starts on the cached KV pages of the longest indexed prefix of its prompt and prefills only the
+    rest; its prompt is indexed once prefilled.  ``reused_tokens[prompt_idx]`` and ``self.reused_total`` record the
+    reuse; tokens, sampling, penalties and logprobs are those of a full prefill.
+
     Penalised requests (``SamplingParams.penalized``) keep their token state in one int32 ``[batch_size, vocab]`` slab,
     allocated when the first of them enters a slot.  From then on every admission rebuilds the slot's row from the
     prompt and the first token, and every decode step with a penalised slot is one ``tl_sample_penalized`` launch over
     all slots (idle slots at position 0, so their rows do not change); the kernel counts each drawn token."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
-                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None):
+                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None, prefix_cache=False):
         if max_seq_len <= 0:
             raise ValueError("max_seq_len must be positive")
         if batch_size <= 0:
@@ -245,6 +260,9 @@ class ContinuousBatcher:
         self.peak_active_requests = 0
         self.peak_live_pages = 0
         self.token_state: torch.Tensor | None = None  # [batch_size, vocab] int32, on first penalised admission
+        self.prefix_cache = model.enable_prefix_cache() if prefix_cache else None
+        self.reused_tokens: dict[int, int] = {}
+        self.reused_total = 0
 
     # -- bookkeeping ---------------------------------------------------------
     def idle(self) -> bool:
@@ -279,7 +297,10 @@ class ContinuousBatcher:
         if self.pending is not None:
             live.append(self.pending)
         self.peak_active_requests = max(self.peak_active_requests, len(live))
-        pages = sum(len(getattr(r.kv_cache[0], "page_ids", ())) for r in live) * len(self.kv_cache)  # layers move in lockstep
+        if self.prefix_cache is None:
+            pages = sum(len(getattr(r.kv_cache[0], "page_ids", ())) for r in live) * len(self.kv_cache)  # layers move in lockstep
+        else:  # a page shared through the prefix cache counts once
+            pages = len({p for r in live for p in r.kv_cache[0].page_ids}) * len(self.kv_cache)
         self.peak_live_pages = max(self.peak_live_pages, pages)
 
     def _admit_state(self, request: Request, slot: int) -> None:
@@ -305,8 +326,11 @@ class ContinuousBatcher:
                 self.model, self.tokenizer, prompt, self.prefill_step, self.next_request_idx,
                 max_seq_len=self.max_seq_len, eos_token_id=self.eos_token_id, device=self.device,
                 sampling=None if self.sampling is None else self.sampling[self.next_request_idx],
-                logprobs=self.logprobs_n,
+                logprobs=self.logprobs_n, prefix_cache=self.prefix_cache,
             )
+            if self.prefix_cache is not None:
+                self.reused_tokens[self.next_request_idx] = self.pending.reused_tokens
+                self.reused_total += self.pending.reused_tokens
             if self.logprobs_n is not None:
                 self.logprobs[self.next_request_idx] = self.pending.logprob_entries
             self.next_request_idx += 1

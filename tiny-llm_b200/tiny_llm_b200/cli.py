@@ -16,6 +16,8 @@ see checkpoint.py; there is no hub download here).
         (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
     python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
         (teacher-forced log-probability of every prompt token and the prompt's perplexity)
+    python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3,8;5,17,3,9" --prefix-cache
+        (requests share the KV pages of a common prompt prefix; reused tokens per request and cache stats after the text)
 """
 
 from __future__ import annotations
@@ -158,15 +160,21 @@ def cmd_batch(args) -> int:
     if args.sampler_temp != 0 or penalties:  # request i draws with seed `--seed + i`
         sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i, **penalties)
                     for i in range(len(queue))]
+    if args.prefix_cache and not hasattr(model, "enable_prefix_cache"):
+        raise SystemExit("--prefix-cache needs the paged week3 model")
     batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
                                 verbose=not args.quiet, device=device,
                                 max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None, sampling=sampling,
-                                logprobs=args.logprobs)
+                                logprobs=args.logprobs, prefix_cache=args.prefix_cache)
     results = batcher.run()
     for idx, text in sorted(results):
         print(f"--- request {idx}\n{text}")
+        if args.prefix_cache:
+            print(f"reused tokens: {batcher.reused_tokens.get(idx, 0)}")
         if args.logprobs is not None:
             _print_logprobs(batcher.logprobs.get(idx, []), tokenizer)
+    if args.prefix_cache:
+        print("prefix cache: " + ", ".join(f"{k} {v}" for k, v in batcher.prefix_cache.stats().items()))
     return 0
 
 
@@ -232,6 +240,8 @@ def main(argv=None) -> int:
     sub.choices["batch"].add_argument("--prefill-step", type=int, default=128)
     sub.choices["batch"].add_argument("--max-seq-len", type=int, default=512)
     sub.choices["batch"].add_argument("--quiet", action="store_true")
+    sub.choices["batch"].add_argument("--prefix-cache", action="store_true",
+                                      help="share the KV pages of prompt prefixes computed before (paged week3 model)")
     args = ap.parse_args(argv)
     if not args.model and not args.synthetic:
         ap.error("--model or --synthetic is required")

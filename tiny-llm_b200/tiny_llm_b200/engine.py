@@ -748,7 +748,7 @@ class DecodeEngine(_GraphEngine):
             need = max(0, -(-(tail + steps - self.page_size) // self.page_size))
             if len(c.page_ids) + need > self.max_pages:
                 raise ValueError("request exceeds the engine's max_seq_len")
-            if need > len(c.pool.free_page_ids) + (c.pool.capacity - c.pool.num_pages):
+            if need and need > c.pool.pages_available():
                 raise RuntimeError("page pool slab exhausted: reserve() more pages before decoding")
 
     def _advance_pages(self, b: int, rec: "_SlotRecord", steps: int) -> None:
@@ -1050,7 +1050,7 @@ class PrefillEngine(_GraphEngine):
             if pool._key_pages is None or pool._key_pages.dtype != torch.bfloat16:
                 return False
             fresh = -(-(offset + tokens) // self.page_size) - len(layer_cache.page_ids)
-            if fresh > len(pool.free_page_ids) + (pool.capacity - pool.num_pages):
+            if fresh > 0 and fresh > pool.pages_available():
                 return False
         return True
 

@@ -17,7 +17,7 @@ def _release_kv_cache(kv_cache) -> None:
 
 
 def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: int | None = None, device=None, on_token=None, sampler=None,
-                        sampling=None, logprobs: int | None = None):
+                        sampling=None, logprobs: int | None = None, prefix_cache: bool = False):
     """The loop of ``simple_generate_with_kv_cache`` on token ids: the whole
     prompt is prefilled at offset 0 (its last-row logits give the first token),
     then one token per step at a growing offset.  Returns the generated ids.
@@ -27,7 +27,9 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     ``DecodeEngine.decode_on_device(sampling=...)``.  A penalised ``sampling`` keeps the request's ``[1, vocab]`` token
     state, built from the prompt; each launch counts the token it draws.
     ``logprobs`` (an int N in [0, 20]) returns ``(ids, entries)`` instead: one ``TokenLogprobs`` per generated id, from
-    the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives)."""
+    the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives).
+    ``prefix_cache=True`` starts the request on the model's prefix index (``Qwen3ModelWeek3.enable_prefix_cache``):
+    only the prompt past its longest cached prefix is prefilled, and the prompt is indexed afterwards."""
     if sampler is not None and sampling is not None:
         raise ValueError("give sampler or sampling, not both")
     if logprobs is not None:
@@ -37,13 +39,18 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     entries: list = []
     state = None
     try:
-        tokens = torch.as_tensor(list(prompt_ids), dtype=torch.int32, device=device)
-        offset = 0
+        ids = [int(t) for t in prompt_ids]
+        prompt = torch.as_tensor(ids, dtype=torch.int32, device=device)
+        index = model.enable_prefix_cache() if prefix_cache else None
+        offset = 0 if index is None else index.adopt(index.lookup(ids), kv_cache)
+        tokens = prompt[offset:]
         while len(produced) < max_new_tokens:
             logits = model(tokens[None], offset, kv_cache, logits_to_keep=1)
+            if index is not None and offset + tokens.numel() == len(ids):
+                index.insert(ids, kv_cache)
             if sampling is not None:
                 if sampling.penalized and state is None:
-                    state = token_state_row(tokens, [], logits.shape[-1], device=logits.device)[None]
+                    state = token_state_row(prompt, [], logits.shape[-1], device=logits.device)[None]
                 token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state)
             elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])

@@ -11,6 +11,13 @@ counters included: LIFO free list (:135-142), storage growth to
 ``max(4, num_pages, 2*capacity)`` copying ``num_pages-1`` old pages (:154-182),
 fill-the-tail-then-allocate appends with snapshot/rollback (:271-312),
 ``block_table`` objects cached per (page ids, width) (:364-377).
+
+Prefix caching (``prefix_cache.py``) adds shared pages: a page is referenced once
+by every request cache holding it plus once if the prefix index holds it, and goes
+back to the free list only when the last reference is dropped.  A write may only
+land in a page its writer alone references, and in a page the index holds as a
+partial node only at or beyond the indexed length (``check_write``).  Without an
+index no page is ever shared and every path above is unchanged.
 """
 
 from __future__ import annotations
@@ -65,6 +72,11 @@ class TinyKvPagedPool:
         self.slab_version = 0  # no slab yet
         self.copied_pages_on_growth = 0
         self.copied_bytes_on_growth = 0
+        # prefix caching: references beyond a page's first, the pages the prefix index holds (-> indexed length,
+        # page_size for a full node) and the index itself (it evicts its least recently used unreferenced leaf)
+        self.extra_refs: dict[int, int] = {}
+        self.indexed: dict[int, int] = {}
+        self.prefix_index = None
 
     # ---- views and sizes ---------------------------------------------------
     @property
@@ -86,6 +98,14 @@ class TinyKvPagedPool:
     @property
     def num_free_pages(self) -> int:
         return len(self.free_page_ids)
+
+    def pages_available(self) -> int:
+        """Pages an allocation can still take without growing the slab: free, never used within the slab, and held by
+        the prefix index alone (evicted on demand)."""
+        n = len(self.free_page_ids) + (self.capacity - self.num_pages)
+        if self.prefix_index is not None:
+            n += self.prefix_index.evictable_pages()
+        return n
 
     @property
     def storage_nbytes(self) -> int:
@@ -146,7 +166,10 @@ class TinyKvPagedPool:
 
     # ---- allocator ----------------------------------------------------------
     def allocate_page(self) -> int:
-        """Newest freed page first, else the next never-used id (:132-142)."""
+        """Newest freed page first, else (prefix caching) the least recently used page only the prefix index holds,
+        else the next never-used id (:132-142)."""
+        if not self.free_page_ids and self.prefix_index is not None:
+            self.prefix_index.evict_one()
         if self.free_page_ids:
             page_id = self.free_page_ids.pop()
             self.reused_page_allocations += 1
@@ -157,11 +180,54 @@ class TinyKvPagedPool:
         return page_id
 
     def free_page(self, page_id: int) -> None:
-        """Ids stay stable; stale bytes are masked by page_lens (:236-242)."""
+        """Drop one reference; the last one returns the page.  Ids stay stable; stale bytes are masked by page_lens
+        (:236-242)."""
         if page_id not in self.used_page_ids:
             raise ValueError(f"Page {page_id} is already free")
+        extra = self.extra_refs.get(page_id)
+        if extra:
+            if extra == 1:
+                del self.extra_refs[page_id]
+            else:
+                self.extra_refs[page_id] = extra - 1
+            return
         self.used_page_ids.remove(page_id)
         self.free_page_ids.append(page_id)
+
+    def make_room(self, pages: int) -> None:
+        """Evict prefix-index pages until ``pages`` are on the free list or nothing more is evictable, so that the
+        allocations of a transactional append never evict (an eviction touches every layer's pool)."""
+        while len(self.free_page_ids) < pages and self.prefix_index is not None and self.prefix_index.evict_one():
+            pass
+
+    def share_page(self, page_id: int) -> None:
+        """One more reference to a live page (a request adopting it, or the prefix index)."""
+        if page_id not in self.used_page_ids:
+            raise ValueError(f"Page {page_id} is free and cannot be shared")
+        self.extra_refs[page_id] = self.extra_refs.get(page_id, 0) + 1
+
+    def refcount(self, page_id: int) -> int:
+        return 0 if page_id not in self.used_page_ids else 1 + self.extra_refs.get(page_id, 0)
+
+    def check_write(self, page_id: int, start: int) -> None:
+        """Raise unless a request holding ``page_id`` may write its slots from ``start`` on: no other request holds
+        the page, and a page the prefix index holds is written only at or beyond its indexed length."""
+        if self.extra_refs:
+            holders = 1 + self.extra_refs.get(page_id, 0) - (page_id in self.indexed)
+            if holders > 1:
+                raise RuntimeError(f"write into page {page_id}, which {holders} requests share")
+        if self.indexed:
+            floor = self.indexed.get(page_id)
+            if floor is not None and start < floor:
+                raise RuntimeError(f"write at slot {start} of page {page_id}, below its {floor} slots held by the prefix cache")
+
+    def ensure_capacity(self) -> None:
+        """Grow the slab (same rule as an append) so that every allocated page has storage."""
+        if self._key_pages is None:
+            raise ValueError("Paged K/V storage does not exist yet")
+        if self.capacity < self.num_pages:
+            _, H, _, D = self._key_pages.shape
+            self._grow(max(4, self.num_pages, self.capacity * 2), H, D, self._key_pages.dtype, self._key_pages.device)
 
     def read_page(self, page_id: int) -> tuple[torch.Tensor, torch.Tensor]:
         if self._key_pages is None or self._value_pages is None:
@@ -355,6 +421,11 @@ class TinyKvPagedCache(TinyKvCache):
         """Fill the tail page, then take fresh pages; all-or-nothing (:271-312)."""
         self.pool.validate_page_chunk(key, value)
         total = key.shape[2]
+        tail_room = self.page_size - self.page_lens[-1] if self.page_ids else 0
+        if tail_room and total:
+            self.pool.check_write(self.page_ids[-1], self.page_lens[-1])
+        if self.pool.prefix_index is not None:
+            self.pool.make_room(-(-(total - min(tail_room, total)) // self.page_size))
         mine = self._snapshot_state()
         theirs = self.pool._snapshot_state()
         # CUDA: when nothing overrides the per-page writer, the host bookkeeping below runs with the
@@ -397,9 +468,11 @@ class TinyKvPagedCache(TinyKvCache):
             return
         tail_room = self.page_size - self.page_lens[-1] if self.page_ids else 0
         fresh = max(0, -(-(count - tail_room) // self.page_size))
-        if fresh > len(self.pool.free_page_ids) + (self.pool.capacity - self.pool.num_pages):
+        if fresh > self.pool.pages_available():
             raise RuntimeError("page pool slab exhausted: reserve() more pages before prefilling")
         take = min(tail_room, count)
+        if take:
+            self.pool.check_write(self.page_ids[-1], self.page_lens[-1])
         if take:
             self.page_lens[-1] += take
         left = count - take
@@ -418,10 +491,11 @@ class TinyKvPagedCache(TinyKvCache):
         The pool slab must already cover the page (``pool.reserve``)."""
         if self.page_ids and self.page_lens[-1] < self.page_size:
             slot = self.page_lens[-1]
-            self.page_lens[-1] += 1
             page_id = self.page_ids[-1]
+            self.pool.check_write(page_id, slot)
+            self.page_lens[-1] += 1
         else:
-            if not self.pool.free_page_ids and self.pool.num_pages >= self.pool.capacity:
+            if self.pool.pages_available() < 1:
                 raise RuntimeError("page pool slab exhausted: reserve() more pages before decoding")
             page_id = self.pool.allocate_page()
             self.page_ids.append(page_id)
@@ -429,6 +503,34 @@ class TinyKvPagedCache(TinyKvCache):
             slot = 0
         self.offset += 1
         return page_id, slot
+
+    def adopt_prefix(self, page_ids: list[int], page_lens: list[int], tokens: int) -> int | None:
+        """Start this fresh cache on a cached prefix of ``tokens`` tokens: take a reference on each of ``page_ids``
+        (full pages, ``page_lens`` their fills) and, when ``tokens`` reaches past them, allocate a private page for
+        the remaining slots - the copy-on-write destination - with its storage ensured.  Returns that page's id
+        (None without one); the caller copies the slots into it before anything reads them."""
+        if self.page_ids or self._offset or (self._lazy is not None and self._lazy.pending):
+            raise ValueError("adopt_prefix needs a fresh cache")
+        if len(page_lens) != len(page_ids) or any(n != self.page_size for n in page_lens):
+            raise ValueError("only full pages can be shared")
+        rest = tokens - self.page_size * len(page_ids)
+        if not 0 <= rest < self.page_size:
+            raise ValueError(f"{tokens} tokens do not fit {len(page_ids)} shared pages plus one partial page")
+        for page_id in page_ids:
+            if page_id not in self.pool.used_page_ids:
+                raise ValueError(f"Page {page_id} is free and cannot be shared")
+        for page_id in page_ids:
+            self.pool.share_page(page_id)
+        self.page_ids = list(page_ids)
+        self._page_lens = list(page_lens)
+        dst = None
+        if rest:
+            dst = self.pool.allocate_page()
+            self.page_ids.append(dst)
+            self._page_lens.append(rest)
+            self.pool.ensure_capacity()
+        self._offset = tokens
+        return dst
 
     def validate_append(self, key: torch.Tensor, value: torch.Tensor) -> None:
         self.pool.validate_page_chunk(key, value)
@@ -514,12 +616,15 @@ class TinyKvPagedCache(TinyKvCache):
         if keep == 0:
             self.release()
             return
-        self.epoch += 1
         pages_needed = (keep + self.page_size - 1) // self.page_size
+        tail = keep - self.page_size * (pages_needed - 1)
+        if tail < self.page_size:  # the next append writes this page from slot `tail` on
+            self.pool.check_write(self.page_ids[pages_needed - 1], tail)
+        self.epoch += 1
         while len(self.page_ids) > pages_needed:
             self.page_lens.pop()
             self.pool.free_page(self.page_ids.pop())
-        self.page_lens[-1] = keep - self.page_size * (pages_needed - 1)
+        self.page_lens[-1] = tail
         self.offset = keep
 
     def release(self):

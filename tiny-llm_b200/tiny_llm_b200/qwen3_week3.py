@@ -252,10 +252,20 @@ class Qwen3ModelWeek3:
         self._verify_engines: dict = {}
         self._packed_layers: list | None = None
         self._paged = enable_paged_attention
+        self.prefix_cache = None  # prefix_cache.PrefixCache over page_pools, once enable_prefix_cache() is called
 
     def create_kv_cache(self) -> list[TinyKvCache]:
         """One logical cache per layer, all sharing that layer's pool."""
         return [TinyKvPagedCache(pool=pool) for pool in self.page_pools]
+
+    def enable_prefix_cache(self):
+        """The model's prefix index (``prefix_cache.PrefixCache``), created over ``page_pools`` on first call: requests
+        whose prompts share a prefix with one prefilled before share its KV pages.  Off until called."""
+        if self.prefix_cache is None:
+            from .prefix_cache import PrefixCache
+
+            self.prefix_cache = PrefixCache(self.page_pools)
+        return self.prefix_cache
 
     # ---- CUDA-graph decode path ------------------------------------------------
     def packed_layers(self) -> list:
