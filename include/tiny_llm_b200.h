@@ -211,6 +211,44 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
 int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                         const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                         const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* Regex-constrained sampling (DESIGN.md section 8c).  One descriptor per row, in device memory (40 bytes):
+ *   mask           uint32 [num_states + 1, ceil(vocab / 32)]: bit t of row s set iff token t is allowed in state s;
+ *                  NULL: the row is unconstrained and draws exactly as tl_sample / tl_sample_penalized;
+ *   dfa            int32 [num_states, 256], the byte DFA (-1: dead);
+ *   token_offsets  int32 [vocab + 1] and token_bytes: each token's bytes (EOS and never-emitted ids: none);
+ *   num_states     S, the DFA's state count; state S is the terminal state after EOS;
+ *   state          the row's current state, read and (rank 0, after the draw) written by tl_sample_constrained. */
+typedef struct tl_constraint_row {
+    const uint32_t *mask;
+    const int32_t *dfa;
+    const int32_t *token_offsets;
+    const uint8_t *token_bytes;
+    int32_t num_states;
+    int32_t state;
+} tl_constraint_row;
+/* The token masks of a byte DFA over a vocabulary, in one launch.  dfa int32 [num_states, 256] (-1: dead; every state
+ * live), accept uint8 [num_states], token_offsets int32 [vocab + 1] with token_bytes, eos_ids int32 [num_eos].
+ * masks (uint32 [num_states + 1, ceil(vocab / 32)], written whole) gets, for s < S, bit t iff token t has bytes and
+ * walking them from s never reaches -1, or t is an EOS id and accept[s]; row S (terminal) has exactly the EOS bits.
+ * reach (uint32 [num_states, ceil(num_states / 32)], zeroed by the caller) gets bit e of row s for every allowed token
+ * with bytes that leads from s to e.  The table is staged in shared memory up to 192 states (16-byte aligned dfa),
+ * read from global memory beyond.  Deterministic. */
+int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
+                              const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks, uint32_t *reach,
+                              void *stream);
+/* tl_sample (repetition, presence, frequency, min_p and state all NULL) or tl_sample_penalized (all given) restricted
+ * per row to the tokens constraints[r] allows (read after the programmatic-dependent-launch wait).  For a row with a
+ * mask, after staging and after the penalty rewrite the entries of disallowed tokens (every entry when the state is
+ * outside [0, S]) are dropped as NaN entries are: the first-maximum argmax of greedy and non-finite-maximum rows,
+ * the top-k count, the top-p mass, min-p's maximum and the Gumbel draw (Philox counters unchanged) all run on the
+ * allowed entries.  A row whose mask allows every token therefore draws exactly the unconstrained kernel's token.
+ * The token is always allowed: a row without an allowed non-NaN entry returns the lowest allowed id (0 if none).
+ * After the draw, for rows with a mask and positions[r] > 0, constraints[r].state becomes S when the token has no
+ * bytes (EOS) or the state was S, else the DFA walk of its bytes.  Log-probabilities (tl_logprobs) are unaffected. */
+int tl_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                          const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                          const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab,
+                          int dtype, void *stream);
 /* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
  * launch, one cluster of CTAs per row (DESIGN.md section 8a).
  *

@@ -398,6 +398,32 @@ int tl_sample_penalized(const void *logits, const float *temperature, const int3
                                    out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
+int tl_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                          const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                          const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab,
+                          int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_constrained: expected float32, float16, or bfloat16");
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_constrained: bad shape");
+    if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
+    if (rows == 0) return TL_OK;
+    if (!logits || !temperature || !top_k || !top_p || !seed || !positions || !constraints || !out_tokens)
+        return fail(TL_EINVAL, "sample_constrained: null pointer");
+    const int given = !!repetition + !!presence + !!frequency + !!min_p + !!state;
+    if (given != 0 && given != 5) return fail(TL_EINVAL, "sample_constrained: give every penalty array and the state, or none");
+    return launch_sample_constrained(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
+                                     constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
+}
+
+int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
+                              const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks, uint32_t *reach,
+                              void *stream) {
+    if (num_states <= 0 || vocab <= 0 || num_eos < 0) return fail(TL_EINVAL, "constraint_token_masks: bad shape");
+    if (!dfa || !accept || !token_offsets || !token_bytes || (num_eos > 0 && !eos_ids) || !masks || !reach)
+        return fail(TL_EINVAL, "constraint_token_masks: null pointer");
+    return launch_constraint_token_masks(dfa, accept, num_states, token_offsets, token_bytes, vocab, eos_ids, num_eos, masks, reach,
+                                         as_stream(stream));
+}
+
 int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
                 int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
                 void *stream) {

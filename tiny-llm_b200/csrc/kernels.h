@@ -43,6 +43,14 @@ int launch_sample(const void *logits, const float *temperature, const int32_t *t
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                             const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype,
+                              cudaStream_t st);
+// constrained.cu
+int launch_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
+                                  const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks,
+                                  uint32_t *reach, cudaStream_t st);
 // logprobs.cu: same cluster plan as sampling.cu
 constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
 int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,

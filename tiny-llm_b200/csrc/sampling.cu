@@ -22,6 +22,11 @@
 // frequency and presence penalties; every later step runs on that penalised row.  min-p adds a third lower bound on
 // the keep threshold after the radix levels, and rank 0 adds 1 to the drawn token's count once every CTA has read
 // its state slice.
+//
+// The constrained form (MASK, tl_sample_constrained, DESIGN.md section 8c) reads the row's tl_constraint_row after
+// the wait.  For a row with a mask, the staged entries of disallowed tokens become NaN after the penalty rewrite:
+// NaN entries are never counted, weighed, kept or drawn, so every later step runs on the allowed entries alone.  Rank 0
+// walks the drawn token's bytes through the DFA and writes the row's new state, for rows with position > 0.
 #include <cooperative_groups.h>
 
 #include <climits>
@@ -75,11 +80,33 @@ __device__ __forceinline__ float penalize(float x, int32_t s, float r, float pre
     return x;
 }
 
-template <typename T, int LEVELS, bool PEN>
+// The constrained row's state after `token`: S (terminal) after an allowed token without bytes (EOS) or in S, else the
+// DFA walk of the token's bytes (-1 once dead, which an allowed token never reaches).  A state outside [0, S] stays.
+__device__ __forceinline__ int32_t constraint_advance(const tl_constraint_row &c, int token) {
+    int32_t s = c.state;
+    if (s < 0 || s >= c.num_states) return s;
+    const int b0 = c.token_offsets[token], b1 = c.token_offsets[token + 1];
+    if (b0 == b1) return c.num_states;
+    for (int j = b0; j < b1 && s >= 0; ++j) s = c.dfa[s * 256 + c.token_bytes[j]];
+    return s;
+}
+
+// The lowest id the row's mask allows (0 when it allows none): the token of a row without an allowed non-NaN entry.
+__device__ __forceinline__ int constraint_lowest(const tl_constraint_row &c, int vocab) {
+    if (c.state < 0 || c.state > c.num_states) return 0;
+    const int words = (vocab + 31) >> 5;
+    const uint32_t *m = c.mask + static_cast<size_t>(c.state) * words;
+    for (int w = 0; w < words; ++w)
+        if (m[w]) return min(vocab - 1, 32 * w + __ffs(m[w]) - 1);
+    return 0;
+}
+
+template <typename T, int LEVELS, bool PEN, bool MASK>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restrict__ logits, const float *__restrict__ temperature,
                                                                 const int32_t *__restrict__ top_k, const float *__restrict__ top_p,
                                                                 const int64_t *__restrict__ seed, const int32_t *__restrict__ positions,
-                                                                int32_t *__restrict__ out, int vocab, int slice, int vec, Penalties pen) {
+                                                                int32_t *__restrict__ out, int vocab, int slice, int vec, Penalties pen,
+                                                                tl_constraint_row *con) {
     extern __shared__ float4 smem_dyn[];
     float *xs = reinterpret_cast<float *>(smem_dyn);
     __shared__ unsigned int h_count[2][BINS];  // double-buffered: level l + 2 reuses l's buffer after all remote reads of it
@@ -132,6 +159,19 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
             __syncthreads();
         }
     }
+    if constexpr (MASK) {
+        const uint32_t *mask = con[row].mask;
+        if (mask) {  // disallowed entries (and every entry of a state outside [0, S]) become NaN
+            const int32_t state = con[row].state, S = con[row].num_states;
+            const bool known = state >= 0 && state <= S;
+            const uint32_t *m = mask + static_cast<size_t>(known ? state : 0) * ((vocab + 31) >> 5);
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const int t = begin + i;
+                if (!known || !((__ldg(m + (t >> 5)) >> (t & 31)) & 1u)) xs[i] = NAN;
+            }
+            __syncthreads();
+        }
+    }
 
     // ---- 1. first-maximum-wins argmax of the (penalised) row
     Best mine{-INFINITY, INT_MAX};
@@ -153,10 +193,16 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     const Best best = row_max;
     if (!(temp > 0.f) || !isfinite(best.v)) {
         if (rank == 0 && threadIdx.x == 0) {
-            const int token = best.i == INT_MAX ? 0 : best.i;
+            int token = best.i == INT_MAX ? 0 : best.i;
+            if constexpr (MASK) {
+                if (con[row].mask && best.i == INT_MAX) token = constraint_lowest(con[row], vocab);
+            }
             out[row] = token;
             if constexpr (PEN) {  // every CTA read its state slice before the cluster barrier above
                 if (positions[row] > 0) pen.state[static_cast<size_t>(row) * vocab + token] += 1;
+            }
+            if constexpr (MASK) {  // and its constraint state
+                if (con[row].mask && positions[row] > 0) con[row].state = constraint_advance(con[row], token);
             }
         }
         cluster.sync();  // no CTA leaves while another may still read its pub_max
@@ -313,17 +359,20 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
         if constexpr (PEN) {
             if (positions[row] > 0) pen.state[static_cast<size_t>(row) * vocab + token] += 1;
         }
+        if constexpr (MASK) {
+            if (con[row].mask && positions[row] > 0) con[row].state = constraint_advance(con[row], token);
+        }
     }
     cluster.sync();
 }
 
-template <typename T, int LEVELS, bool PEN>
+template <typename T, int LEVELS, bool PEN, bool MASK>
 int launch_sample_t(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                     const int32_t *positions, int32_t *out, int rows, int vocab, int cluster, int slice, int vec, const Penalties &pen,
-                    cudaStream_t st) {
+                    tl_constraint_row *con, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
+        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
             return fail(TL_ECUDA, "sample: cannot raise shared memory limit");
         configured = true;
     }
@@ -343,15 +392,16 @@ int launch_sample_t(const void *logits, const float *temperature, const int32_t 
     cfg.numAttrs = use_pdl() ? 2 : 1;
     const T *x = static_cast<const T *>(logits);
     cudaError_t e =
-        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen);
+        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN, MASK>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen, con);
     if (e != cudaSuccess) return fail(TL_ECUDA, "sample: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("sample");
     return TL_OK;
 }
 
-template <bool PEN>
+template <bool PEN, bool MASK>
 int launch_sample_any(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
-                      const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, const Penalties &pen, cudaStream_t st) {
+                      const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, const Penalties &pen, tl_constraint_row *con,
+                      cudaStream_t st) {
     if (rows == 0) return TL_OK;
     int cluster = 0, slice = 0;
     if (int e = sample_plan(vocab, &cluster, &slice)) return e;
@@ -359,14 +409,14 @@ int launch_sample_any(const void *logits, const float *temperature, const int32_
     const int vec = (vocab % per16 == 0 && aligned16(logits)) ? 1 : 0;
     switch (dtype) {
         case TL_F32:
-            return launch_sample_t<float, 4, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec, pen,
-                                                  st);
+            return launch_sample_t<float, 4, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec,
+                                                        pen, con, st);
         case TL_F16:
-            return launch_sample_t<__half, 4, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec,
-                                                   pen, st);
+            return launch_sample_t<__half, 4, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
+                                                         vec, pen, con, st);
         case TL_BF16:  // a bf16 value's key has 16 significant bits: two levels
-            return launch_sample_t<__nv_bfloat16, 2, PEN>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
-                                                           vec, pen, st);
+            return launch_sample_t<__nv_bfloat16, 2, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
+                                                                 slice, vec, pen, con, st);
         default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
     }
 }
@@ -386,14 +436,25 @@ int sample_plan(int vocab, int *cluster, int *slice) {
 
 int launch_sample(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
-    return launch_sample_any<false>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{}, st);
+    return launch_sample_any<false, false>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{}, nullptr, st);
 }
 
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                             const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
     const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
-    return launch_sample_any<true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, st);
+    return launch_sample_any<true, false>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, nullptr, st);
+}
+
+int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype,
+                              cudaStream_t st) {
+    if (!state)
+        return launch_sample_any<false, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{},
+                                              constraints, st);
+    const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    return launch_sample_any<true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, constraints, st);
 }
 
 }  // namespace tl

@@ -45,6 +45,8 @@ __all__ = [
     "argmax",
     "sample",
     "sample_penalized",
+    "sample_constrained",
+    "constraint_token_masks",
     "logprobs",
     "LOGPROBS_MAX_N",
     "decode_advance",
@@ -104,6 +106,8 @@ _SIGNATURES = {
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
+    "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
+    "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
@@ -754,6 +758,74 @@ def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetit
                                     positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(), min_p.data_ptr(),
                                     state.data_ptr(), out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
+
+
+CONSTRAINT_ROW_WORDS = 5  # int64 words of one tl_constraint_row (40 bytes)
+
+
+def sample_constrained(logits, temperature, top_k, top_p, seed, positions, constraints, repetition=None, presence=None, frequency=None,
+                       min_p=None, state=None, stream=None):
+    """``sample`` (no penalty arrays) or ``sample_penalized`` (all of them) restricted per row to the tokens of its
+    constraint (``tl_sample_constrained``) -> int32 ``[rows]``.  ``constraints`` int64 ``[rows, 5]``: one
+    ``tl_constraint_row`` per row (all zero: unconstrained), whose state the launch advances for rows with
+    ``positions > 0``."""
+    if logits.dtype not in _FLOATS or logits.dim() != 2:
+        raise RuntimeError("sample_constrained: expected 2D float logits")
+    rows, vocab = logits.shape
+    pen = (repetition, presence, frequency, min_p, state)
+    if any(t is None for t in pen) and any(t is not None for t in pen):
+        raise RuntimeError("sample_constrained: give every penalty array and the state, or none")
+    checks = [("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+              ("seed", seed, torch.int64), ("positions", positions, torch.int32)]
+    if state is not None:
+        checks += [("repetition", repetition, torch.float32), ("presence", presence, torch.float32), ("frequency", frequency, torch.float32),
+                   ("min_p", min_p, torch.float32)]
+        if state.dtype != torch.int32 or tuple(state.shape) != (rows, vocab):
+            raise RuntimeError(f"sample_constrained: state must be int32 [{rows}, {vocab}]")
+    for name, t, dtype in checks:
+        if t.dtype != dtype or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"sample_constrained: {name} must be {str(dtype).replace('torch.', '')} [{rows}]")
+    if constraints.dtype != torch.int64 or tuple(constraints.shape) != (rows, CONSTRAINT_ROW_WORDS):
+        raise RuntimeError(f"sample_constrained: constraints must be int64 [{rows}, {CONSTRAINT_ROW_WORDS}]")
+    named = dict(logits=logits, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, positions=positions, constraints=constraints)
+    if state is not None:
+        named.update(repetition=repetition, presence=presence, frequency=frequency, min_p=min_p, state=state)
+    _contig("sample_constrained", **named)
+    _gpu("sample_constrained", *named.values())
+    out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
+    ptr = [None if t is None else t.data_ptr() for t in pen]
+    _check(_lib.tl_sample_constrained(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                      positions.data_ptr(), *ptr, constraints.data_ptr(), out.data_ptr(), rows, vocab,
+                                      _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+    return out
+
+
+def constraint_token_masks(dfa, accept, token_offsets, token_bytes, eos_ids, stream=None):
+    """Token masks of a byte DFA over a vocabulary (``tl_constraint_token_masks``).  ``dfa`` int32 ``[S, 256]``,
+    ``accept`` uint8 ``[S]``, ``token_offsets`` int32 ``[V + 1]``, ``token_bytes`` uint8, ``eos_ids`` int32 ``[E]``.
+    Returns ``(masks, reach)``: int32 ``[S + 1, ceil(V / 32)]`` (bit t of row s: token t allowed in state s; row S the
+    terminal state) and int32 ``[S, ceil(S / 32)]`` (bit e of row s: an allowed token leads from s to e)."""
+    if dfa.dtype != torch.int32 or dfa.dim() != 2 or dfa.shape[1] != 256 or dfa.shape[0] == 0:
+        raise RuntimeError("constraint_token_masks: dfa must be int32 [S, 256]")
+    S = dfa.shape[0]
+    if accept.dtype != torch.uint8 or tuple(accept.shape) != (S,):
+        raise RuntimeError(f"constraint_token_masks: accept must be uint8 [{S}]")
+    if token_offsets.dtype != torch.int32 or token_offsets.dim() != 1 or token_offsets.shape[0] < 2:
+        raise RuntimeError("constraint_token_masks: token_offsets must be int32 [V + 1]")
+    if token_bytes.dtype != torch.uint8 or token_bytes.dim() != 1:
+        raise RuntimeError("constraint_token_masks: token_bytes must be uint8")
+    if eos_ids.dtype != torch.int32 or eos_ids.dim() != 1:
+        raise RuntimeError("constraint_token_masks: eos_ids must be int32 [E]")
+    named = dict(dfa=dfa, accept=accept, token_offsets=token_offsets, token_bytes=token_bytes, eos_ids=eos_ids)
+    _contig("constraint_token_masks", **named)
+    _gpu("constraint_token_masks", *named.values())
+    V = token_offsets.shape[0] - 1
+    masks = torch.empty((S + 1, (V + 31) // 32), dtype=torch.int32, device=dfa.device)
+    reach = torch.zeros((S, (S + 31) // 32), dtype=torch.int32, device=dfa.device)
+    _check(_lib.tl_constraint_token_masks(dfa.data_ptr(), accept.data_ptr(), S, token_offsets.data_ptr(), token_bytes.data_ptr(), V,
+                                          eos_ids.data_ptr() if eos_ids.numel() else None, eos_ids.numel(), masks.data_ptr(),
+                                          reach.data_ptr(), _stream_ptr(stream, dfa)))
+    return masks, reach
 
 
 LOGPROBS_MAX_N = 20

@@ -24,7 +24,7 @@ from extensions_b200 import tiny_llm_ext_b200
 
 from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, token_logprobs
-from .sampler import any_penalized, sample_tokens, sampling_per_request, token_state_row
+from .sampler import any_constrained, any_penalized, sample_tokens, sampling_per_request, token_state_row
 
 
 def greedy_tokens(logits: torch.Tensor) -> torch.Tensor:
@@ -65,7 +65,8 @@ class Request:
     pass ``eos_token_id`` explicitly if one is wanted).  ``sampling`` (a
     ``SamplingParams``) draws the request's tokens with the seeded ``tl_sample``
     kernel; None keeps them greedy.  A penalised ``sampling`` draws the first
-    token against the prompt-only token state (``token_state_row``).  ``logprobs``
+    token against the prompt-only token state (``token_state_row``).  A constrained ``sampling`` draws the first token
+    under the start state of ``constraint_row``, its one-row descriptor, which that launch advances.  ``logprobs``
     (an int N) records one ``TokenLogprobs`` per generated token in
     ``logprob_entries``."""
 
@@ -87,6 +88,7 @@ class Request:
         self.sampling = sampling
         self.logprobs = logprobs
         self.logprob_entries: list = []
+        self.constraint_row = None  # int64 [1, 5] tl_constraint_row, made with the first token's draw
         self.model = model
         if isinstance(prompt, str):
             ids = tokenizer.encode(prompt, add_special_tokens=False)
@@ -138,7 +140,9 @@ class Request:
                     state = None
                     if self.sampling.penalized:
                         state = token_state_row(self.prefill_tokens, [], logits.shape[-1], device=logits.device)[None]
-                    token = sample_tokens(logits, [self.sampling], [total], state)
+                    if self.sampling.constraint is not None:
+                        self.constraint_row = self.sampling.constraint.descriptor()[None]
+                    token = sample_tokens(logits, [self.sampling], [total], state, self.constraint_row)
                 if self.logprobs is not None:
                     entry = token_logprobs(logits, token, self.logprobs)[0]
         self.offset += chunk
@@ -216,7 +220,12 @@ class ContinuousBatcher:
     Penalised requests (``SamplingParams.penalized``) keep their token state in one int32 ``[batch_size, vocab]`` slab,
     allocated when the first of them enters a slot.  From then on every admission rebuilds the slot's row from the
     prompt and the first token, and every decode step with a penalised slot is one ``tl_sample_penalized`` launch over
-    all slots (idle slots at position 0, so their rows do not change); the kernel counts each drawn token."""
+    all slots (idle slots at position 0, so their rows do not change); the kernel counts each drawn token.
+
+    Constrained requests (``SamplingParams.constraint``) keep their automaton state in one int64 ``[batch_size, 5]``
+    slab of ``tl_constraint_row`` descriptors, allocated when the first of them enters a slot.  Admission copies the
+    request's row (advanced by its prefill draw) into the slot on the device; idle and unconstrained slots hold zero
+    rows.  Every decode step with a constrained slot is one ``tl_sample_constrained`` launch over all slots."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
                  eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None, prefix_cache=False):
@@ -260,6 +269,7 @@ class ContinuousBatcher:
         self.peak_active_requests = 0
         self.peak_live_pages = 0
         self.token_state: torch.Tensor | None = None  # [batch_size, vocab] int32, on first penalised admission
+        self.constraint_rows: torch.Tensor | None = None  # [batch_size, 5] int64, on first constrained admission
         self.prefix_cache = model.enable_prefix_cache() if prefix_cache else None
         self.reused_tokens: dict[int, int] = {}
         self.reused_total = 0
@@ -313,6 +323,18 @@ class ContinuousBatcher:
             self.token_state = torch.zeros((self.batch_size, vocab), dtype=torch.int32, device=request.prefill_tokens.device)
         token_state_row(request.prefill_tokens, [request.next_token], self.token_state.shape[1], out=self.token_state[slot])
 
+    def _admit_constraint(self, request: Request, slot: int) -> None:
+        """Copy the request's constraint descriptor into the slot's row (a device copy), or zero the row."""
+        if self.constraint_rows is None:
+            if request.constraint_row is None:
+                return
+            self.constraint_rows = torch.zeros((self.batch_size, request.constraint_row.shape[1]), dtype=torch.int64,
+                                               device=request.constraint_row.device)
+        if request.constraint_row is None:
+            self.constraint_rows[slot].zero_()
+        else:
+            self.constraint_rows[slot].copy_(request.constraint_row[0])
+
     def _budget_spent(self, request: Request) -> bool:
         if self.max_new_tokens is None:
             return False
@@ -365,6 +387,7 @@ class ContinuousBatcher:
                             for layer_cache, table in zip(request.kv_cache, self.kv_cache):
                                 table.add_request(layer_cache, i)
                             self._admit_state(request, i)
+                            self._admit_constraint(request, i)
                             self.slots[i] = request
                             self.pending = None
                             moved = True
@@ -390,7 +413,8 @@ class ContinuousBatcher:
                 else:  # idle slots draw greedily at position 0: a penalised launch leaves their state rows alone
                     params = [None if s is None else s.sampling for s in self.slots]
                     positions = [0 if s is None else o + 1 for s, o in zip(self.slots, offsets)]
-                    sampled = sample_tokens(logits, params, positions, self.token_state if any_penalized(params) else None)
+                    sampled = sample_tokens(logits, params, positions, self.token_state if any_penalized(params) else None,
+                                            self.constraint_rows if any_constrained(params) else None)
                 if self.logprobs_n is not None:
                     live = torch.tensor([s is not None for s in self.slots], device=sampled.device)
                     targets = torch.where(live, sampled.reshape(-1).to(torch.int32), -1)
@@ -421,6 +445,8 @@ class ContinuousBatcher:
                     text = request.text()
                     for table in self.kv_cache:
                         table.remove_request(i)
+                    if self.constraint_rows is not None:
+                        self.constraint_rows[i].zero_()
                     self.results.append((request.prompt_idx, text))
                     self.slots[i] = None
             self._progress()

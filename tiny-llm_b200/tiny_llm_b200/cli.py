@@ -18,6 +18,8 @@ see checkpoint.py; there is no hub download here).
         (teacher-forced log-probability of every prompt token and the prompt's perplexity)
     python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3,8;5,17,3,9" --prefix-cache
         (requests share the KV pages of a common prompt prefix; reused tokens per request and cache stats after the text)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --regex "[0-9]{4}-[0-9]{2}-[0-9]{2}"
+        (every generated token keeps the text inside the pattern's language; EOS ends it once it is a match)
 """
 
 from __future__ import annotations
@@ -82,6 +84,27 @@ def _penalties(args) -> dict:
     return {k: v for k, v in given.items() if v != off[k]}
 
 
+def _constraint(args, model, tokenizer, device):
+    """The ``TokenConstraint`` of ``--regex`` over the checkpoint tokenizer's vocabulary (the synthetic vocabulary with
+    ``--synthetic``), or None."""
+    if args.regex is None:
+        return None
+    from .constrained import TokenConstraint, TokenVocabulary
+
+    if device.type != "cuda":
+        raise SystemExit("--regex runs on the CUDA sampling kernel: use a cuda --device")
+    if args.synthetic:
+        vocabulary = TokenVocabulary.synthetic(model.vocab_size)
+    elif tokenizer is None:
+        raise SystemExit("--regex needs the checkpoint's tokenizer files (or --synthetic)")
+    else:
+        vocabulary = TokenVocabulary.from_tokenizer(tokenizer, model.vocab_size)
+    try:
+        return TokenConstraint.compile(args.regex, vocabulary, device=device)
+    except ValueError as exc:
+        raise SystemExit(f"--regex: {exc}")
+
+
 def cmd_generate(args) -> int:
     from .generate import greedy_generate_ids
     from .sampler import SamplingParams, make_sampler
@@ -92,6 +115,11 @@ def cmd_generate(args) -> int:
     ids = _prompt_ids(args, tokenizer, args.prompt)
     sampler = sampling = None
     penalties = _penalties(args)
+    if (args.draft_model or args.draft_synthetic) and args.regex is not None:
+        raise SystemExit("speculative decoding is greedy and unconstrained: drop --regex")
+    constraint = _constraint(args, model, tokenizer, device)
+    if constraint is not None:
+        penalties["constraint"] = constraint
     if args.sampler_temp != 0 or penalties:
         if device.type == "cuda" or penalties:  # the seeded kernel
             sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed, **penalties)
@@ -108,6 +136,8 @@ def cmd_generate(args) -> int:
             print(tokenizer.detokenizer.last_segment, end="", flush=True)
 
     eos = getattr(tokenizer, "eos_token_id", None)
+    if constraint is not None and args.synthetic:
+        eos = constraint.vocabulary.eos_ids[0]
     if args.draft_model or args.draft_synthetic:
         from .generate import speculative_generate_ids
 
@@ -157,13 +187,17 @@ def cmd_batch(args) -> int:
                                                enable_thinking=args.enable_thinking) for p in prompts]
     sampling = None
     penalties = _penalties(args)
+    constraint = _constraint(args, model, tokenizer, device)
+    if constraint is not None:
+        penalties["constraint"] = constraint
     if args.sampler_temp != 0 or penalties:  # request i draws with seed `--seed + i`
         sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i, **penalties)
                     for i in range(len(queue))]
     if args.prefix_cache and not hasattr(model, "enable_prefix_cache"):
         raise SystemExit("--prefix-cache needs the paged week3 model")
+    eos = constraint.vocabulary.eos_ids[0] if constraint is not None and args.synthetic else None
     batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
-                                verbose=not args.quiet, device=device,
+                                verbose=not args.quiet, device=device, eos_token_id=eos,
                                 max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None, sampling=sampling,
                                 logprobs=args.logprobs, prefix_cache=args.prefix_cache)
     results = batcher.run()
@@ -228,6 +262,8 @@ def main(argv=None) -> int:
                                        help="subtract this times the count of each generated token")
         sub.choices[name].add_argument("--min-p", type=float, default=0.0,
                                        help="keep tokens at least this fraction as likely as the top one (0: off)")
+        sub.choices[name].add_argument("--regex", default=None, metavar="PATTERN",
+                                       help="constrain the generated text to fullmatch PATTERN (re.ASCII semantics over UTF-8 bytes)")
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")

@@ -338,6 +338,14 @@ class DecodeEngine(_GraphEngine):
         self._pen_host = None
         self._pen_dev = None
         self._pen_key = None
+        # decode_on_device(sampling=<constrained>): one graph per (penalised, logprobs N or None), the step with
+        # tl_sample_constrained as its token choice, over a [B, 5] int64 slab of tl_constraint_row descriptors whose
+        # states the launches advance; all on first use
+        self._graph_con: dict = {}
+        self.kernels_per_constrained_step = 0
+        self._con_host = None
+        self._con_dev = None
+        self._con_key = None
 
     @staticmethod
     def fused_attention_applies(model, slot_tokens: int) -> bool:
@@ -352,11 +360,18 @@ class DecodeEngine(_GraphEngine):
         super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
 
     # ------------------------------------------------------------ graph body --
-    def _next_tokens(self, logits, R: int, sampled: bool, penalized: bool = False) -> None:
+    def _next_tokens(self, logits, R: int, sampled: bool, penalized: bool = False, constrained: bool = False) -> None:
         """The step's token per row: ``tl_argmax``, or (the sampled graph) ``tl_sample`` with the per-slot parameters at
         position ``context_lens``, the index of the token being drawn, or (the penalised graph) ``tl_sample_penalized``
-        over ``token_counts``."""
-        if penalized:
+        over ``token_counts``, or (a constrained graph) ``tl_sample_constrained`` over the slot descriptors."""
+        if constrained:
+            pen = ()
+            if penalized:
+                p = self._pen_dev.view(torch.float32).view(4, self.B)
+                pen = (p[0, :R], p[1, :R], p[2, :R], p[3, :R], self.token_counts[:R])
+            tokens = ext.sample_constrained(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
+                                            self.context_lens[:R], self._con_dev.view(self.B, -1)[:R], *pen)
+        elif penalized:
             pen = self._pen_dev.view(torch.float32).view(4, self.B)
             tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
                                           self.context_lens[:R], pen[0, :R], pen[1, :R], pen[2, :R], pen[3, :R], self.token_counts[:R])
@@ -367,7 +382,7 @@ class DecodeEngine(_GraphEngine):
             tokens = ext.argmax(logits)
         self.next_tokens[:R].copy_(tokens)
 
-    def _forward_unfused(self, sampled: bool = False, penalized: bool = False) -> None:
+    def _forward_unfused(self, sampled: bool = False, penalized: bool = False, constrained: bool = False) -> None:
         """One decode step over the static buffers, operator by operator (the
         call sequence of qwen3_week3.py:55-121,139-146,196-207,320-338 at L == 1)."""
         m = self.model
@@ -399,12 +414,12 @@ class DecodeEngine(_GraphEngine):
         x = _normed(x, m.norm)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
         logits = _proj(x, head)
-        self._next_tokens(logits, B, sampled, penalized)
+        self._next_tokens(logits, B, sampled, penalized, constrained)
         if self.logits is None:
             self.logits = torch.empty_like(logits)
         self.logits.copy_(logits)
 
-    def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False) -> None:
+    def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False, constrained: bool = False) -> None:
         """Same step in ~7 launches per layer: norm / SwiGLU / residual folded into
         the streaming projections, q/k norm + RoPE + K/V append in one kernel.
         Every rounding point of the operator-by-operator sequence is kept.
@@ -421,7 +436,7 @@ class DecodeEngine(_GraphEngine):
             x = self._matvec_layers(x)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
-        self._next_tokens(logits, R, sampled, penalized)
+        self._next_tokens(logits, R, sampled, penalized, constrained)
         if self.logits is None:
             self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
@@ -497,6 +512,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_sample = None  # captured again on first use, over the current slabs
         self._graph_pen = None
         self._graph_lp = {}
+        self._graph_con = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -548,17 +564,7 @@ class DecodeEngine(_GraphEngine):
         """Capture the self-advancing step with one ``tl_logprobs`` launch after the token choice (targets: the tokens it
         just wrote), logging at ``step_counter`` (same conditions as ``_ensure_sample_graph``).  One graph per
         (sampled, penalized)."""
-        if self._lp_max_n != max_n:
-            B, cap, dev = self.B, self.log_capacity, self.device
-            self._graph_lp = {}
-            self._lp_max_n = max_n
-            self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
-                            torch.zeros((cap, B), dtype=torch.int32, device=dev), torch.zeros((cap, B, max_n), dtype=torch.int32, device=dev),
-                            torch.zeros((cap, B, max_n), dtype=torch.float32, device=dev))
-            if self._lp_host is None:
-                self._lp_host = torch.zeros(B, dtype=torch.int32, pin_memory=True)
-                self._lp_dev = self._lp_host.to(self.device, copy=True)
-            self._lp_key = None
+        self._alloc_logprobs(max_n)
         if (sampled, penalized) in self._graph_lp:
             return
         forward = self._forward_fused if self.fused else self._forward_unfused
@@ -575,6 +581,73 @@ class DecodeEngine(_GraphEngine):
             self._graph_lp[(sampled, penalized)] = self._graph_of(logprobs_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_logprobs_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _alloc_logprobs(self, max_n: int) -> None:
+        """The logs and the top-N block for ``max_n`` (the graphs that log into older buffers are dropped)."""
+        if self._lp_max_n != max_n:
+            B, cap, dev = self.B, self.log_capacity, self.device
+            self._graph_lp = {}
+            self._graph_con = {k: g for k, g in self._graph_con.items() if k[1] is None}
+            self._lp_max_n = max_n
+            self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
+                            torch.zeros((cap, B), dtype=torch.int32, device=dev), torch.zeros((cap, B, max_n), dtype=torch.int32, device=dev),
+                            torch.zeros((cap, B, max_n), dtype=torch.float32, device=dev))
+            if self._lp_host is None:
+                self._lp_host = torch.zeros(B, dtype=torch.int32, pin_memory=True)
+                self._lp_dev = self._lp_host.to(self.device, copy=True)
+            self._lp_key = None
+
+    def _ensure_constrained_graph(self, penalized: bool, max_n: int | None) -> None:
+        """Capture the constrained self-advancing step, with one ``tl_logprobs`` launch when ``max_n`` is given (same
+        conditions as ``_ensure_sample_graph``; the warm-up runs at context 0, so it advances no state).  One graph per
+        (penalized, max_n)."""
+        if (penalized, max_n) in self._graph_con:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def constrained_step():
+            forward(sampled=True, penalized=penalized, constrained=True)
+            if max_n is not None:
+                ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()
+            self._graph_con[(penalized, max_n)] = self._graph_of(constrained_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_constrained_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_constraints(self, per: list, history) -> None:
+        """Upload the slot descriptors when the slots' constraints change or ``history`` is given.  A slot whose
+        ``history`` entry is ``(prompt_ids, generated_ids)`` starts from the host walk of its generated ids; a slot with a
+        new constraint and no history from the start state; every other constrained slot keeps its device state."""
+        from .constrained import descriptor_state, descriptor_values
+
+        B = self.B
+        cons = [None if p is None else p.constraint for p in per]
+        if history is not None:
+            history = list(history)
+            if len(history) != B:
+                raise ValueError(f"history must hold one (prompt_ids, generated_ids) or None per slot ({B})")
+        walked = {b: c.walk(c.start_state, history[b][1]) for b, c in enumerate(cons)
+                  if c is not None and history is not None and history[b] is not None}
+        key = tuple(cons)  # holds the constraints, whose device tables the descriptors point into
+        if self._con_key is not None and all(x is y for x, y in zip(key, self._con_key)) and not walked:
+            return
+        kept = {b for b, c in enumerate(cons) if c is not None and b not in walked and self._con_key is not None and self._con_key[b] is c}
+        current = descriptor_state(self._con_dev.view(B, -1)).tolist() if kept else None  # one read, only when states carry over
+        self._host_write_begin()
+        host = self._con_host.numpy().reshape(B, -1)
+        for b, c in enumerate(cons):
+            state = walked.get(b, current[b] if b in kept else 0)
+            if c is not None and state < 0:
+                raise ValueError(f"slot {b}: its generated ids leave the constraint's language")
+            host[b] = descriptor_values(c, state)
+        self._upload_meta(self._con_dev, self._con_host)
+        self.h2d_bytes += self._con_host.numel() * 8
+        self._con_key = key
 
     def _set_top_n(self, per: list[int]) -> None:
         """Write the per-slot top-N counts into their pinned block and upload it if they changed."""
@@ -834,7 +907,11 @@ class DecodeEngine(_GraphEngine):
         With a penalised slot in ``sampling`` the step is ``tl_sample_penalized`` over ``token_counts [B, V]``, which
         it updates at every drawn token.  ``history`` (per slot ``(prompt_ids, generated_ids)``, or None) rebuilds those
         slots' rows first; None continues from the rows as the engine holds them.  A call without a penalised slot
-        replays the graphs it would without penalties and does not read ``history``."""
+        replays the graphs it would without penalties and does not read ``history``.
+        With a constrained slot (``SamplingParams.constraint``) the step is ``tl_sample_constrained`` over the engine's
+        slot descriptors, captured on first use per (penalised, logprobs); each launch advances the slots' automaton
+        states.  ``history`` also sets a constrained slot's state to the walk of its generated ids; without it a slot
+        keeps its state while its constraint stays the same and starts at the start state otherwise."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         B = self.B
@@ -845,17 +922,29 @@ class DecodeEngine(_GraphEngine):
             top_n = [_check_n(logprobs)] * B if isinstance(logprobs, int) else [_check_n(0 if n is None else n) for n in logprobs]
             if len(top_n) != B:
                 raise ValueError(f"logprobs must be one int or a list of {B} (one per slot)")
-        penalized = False
+        penalized = constrained = False
         if sampling is not None:
-            from .sampler import any_penalized
+            from .sampler import any_constrained, any_penalized
 
-            penalized = any_penalized(self._per_slot_sampling(sampling))
+            per = self._per_slot_sampling(sampling)
+            penalized, constrained = any_penalized(per), any_constrained(per)
+            for p in per:
+                if p is not None and p.constraint is not None and p.constraint.vocab_size != self.V:
+                    raise ValueError(f"the constraint's vocabulary has {p.constraint.vocab_size} ids, the model {self.V}")
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
         if penalized:
             self._alloc_penalties()
-        if top_n is not None:
+        if constrained:
+            if self._con_dev is None:
+                self._con_host = torch.zeros(5 * B, dtype=torch.int64, pin_memory=True)
+                self._con_dev = self._con_host.to(self.device, copy=True)
+            if top_n is not None:
+                self._alloc_logprobs(max(top_n))
+                self._set_top_n(top_n)
+            self._ensure_constrained_graph(penalized, None if top_n is None else max(top_n))
+        elif top_n is not None:
             self._ensure_logprobs_graph(sampling is not None, max(top_n), penalized)
             self._set_top_n(top_n)
         elif penalized:
@@ -866,10 +955,14 @@ class DecodeEngine(_GraphEngine):
             self._set_sampling(sampling)
         if penalized:
             self._set_penalties(self._per_slot_sampling(sampling), history)
+        if constrained:
+            self._set_constraints(self._per_slot_sampling(sampling), history)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
-        if top_n is not None:
+        if constrained:
+            graph = self._graph_con[(penalized, None if top_n is None else max(top_n))]
+        elif top_n is not None:
             graph = self._graph_lp[(sampling is not None, penalized)]
         elif penalized:
             graph = self._graph_pen

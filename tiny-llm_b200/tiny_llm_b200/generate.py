@@ -25,7 +25,9 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     from ``logits - logsumexp`` instead of taking the arg-max.  ``sampling`` (a ``SamplingParams``) draws each token
     with the seeded ``tl_sample`` kernel instead, at its position in the sequence: the ids equal a prefill plus
     ``DecodeEngine.decode_on_device(sampling=...)``.  A penalised ``sampling`` keeps the request's ``[1, vocab]`` token
-    state, built from the prompt; each launch counts the token it draws.
+    state, built from the prompt; each launch counts the token it draws.  A constrained ``sampling`` keeps the
+    request's one-row constraint descriptor: the prompt's first token is drawn under the start state and every launch
+    advances it on the device.
     ``logprobs`` (an int N in [0, 20]) returns ``(ids, entries)`` instead: one ``TokenLogprobs`` per generated id, from
     the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives).
     ``prefix_cache=True`` starts the request on the model's prefix index (``Qwen3ModelWeek3.enable_prefix_cache``):
@@ -37,7 +39,7 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
     entries: list = []
-    state = None
+    state = constraints = None
     try:
         ids = [int(t) for t in prompt_ids]
         prompt = torch.as_tensor(ids, dtype=torch.int32, device=device)
@@ -51,7 +53,9 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
             if sampling is not None:
                 if sampling.penalized and state is None:
                     state = token_state_row(prompt, [], logits.shape[-1], device=logits.device)[None]
-                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state)
+                if sampling.constraint is not None and constraints is None:
+                    constraints = sampling.constraint.descriptor()[None]
+                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state, constraints)
             elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])
             else:
@@ -277,12 +281,15 @@ def _check_proposal_length(proposal_length) -> None:
 
 
 def speculative_generate_ids(draft_model, model, prompt_ids, max_new_tokens: int, proposal_length: int = 4, eos_token_ids=(),
-                             device=None, on_token=None):
+                             device=None, on_token=None, constraint=None):
     """Greedy generation of ``model`` with ``draft_model`` proposing ``proposal_length`` tokens per round.  Returns
     ``(ids, stats)``: the generated ids (those of ``greedy_generate_ids(model, ...)``, token for token) and the per-round
     ``(proposed, accepted)`` counts.  CUDA Week-3 models with ``1 <= proposal_length <= 7`` verify in one captured graph
-    per round (``Qwen3ModelWeek3.verify_engine``); everything else runs the same protocol through ``model(...)``."""
+    per round (``Qwen3ModelWeek3.verify_engine``); everything else runs the same protocol through ``model(...)``.
+    Speculative decoding is greedy and unconstrained: a ``constraint`` is refused with ``ValueError``."""
     _check_proposal_length(proposal_length)
+    if constraint is not None:
+        raise ValueError("speculative decoding is greedy and unconstrained: it takes no constraint")
     prompt_ids = [int(t) for t in prompt_ids]
     if not prompt_ids:
         raise ValueError("prompt must encode to at least one token")

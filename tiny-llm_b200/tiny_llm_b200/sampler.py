@@ -49,7 +49,11 @@ class SamplingParams:
     the prompt or drawn so far; ``frequency_penalty`` subtracts ``frequency_penalty * count`` and ``presence_penalty``
     subtracts itself from every token drawn so far (both may be negative); ``min_p`` (in [0, 1], on above 0) keeps a
     token only when its probability after temperature is at least ``min_p`` times the top one.  The draw, greedy
-    included, then runs on the penalised logits."""
+    included, then runs on the penalised logits.
+
+    ``constraint`` (a ``TokenConstraint``, ``tl_sample_constrained``, DESIGN.md section 8c) restricts every draw to the
+    tokens that keep the text a prefix of the pattern's language (EOS once it is a match); greedy under a constraint is
+    ``SamplingParams(0.0, constraint=c)``.  With a mask that allows every token the draw is the unconstrained one."""
 
     temperature: float
     top_k: int | None = None
@@ -59,6 +63,7 @@ class SamplingParams:
     presence_penalty: float = 0.0
     frequency_penalty: float = 0.0
     min_p: float = 0.0
+    constraint: object = None
 
     def __post_init__(self):
         t = self.temperature
@@ -87,6 +92,11 @@ class SamplingParams:
         m = self.min_p
         if not real(m) or not 0 <= m <= 1:
             raise ValueError(f"min_p must be a number in [0, 1], got {m!r}")
+        if self.constraint is not None:
+            from .constrained import TokenConstraint
+
+            if not isinstance(self.constraint, TokenConstraint):
+                raise ValueError(f"constraint must be None or a TokenConstraint, got {type(self.constraint).__name__}")
 
     @property
     def penalized(self) -> bool:
@@ -124,6 +134,10 @@ def any_penalized(params) -> bool:
     return any(p is not None and p.penalized for p in params)
 
 
+def any_constrained(params) -> bool:
+    return any(p is not None and p.constraint is not None for p in params)
+
+
 def penalty_tensors(params, device) -> tuple[torch.Tensor, ...]:
     """The per-row device arrays ``ext.sample_penalized`` adds to ``sampling_tensors``' (repetition, presence,
     frequency, min_p) for a list of ``SamplingParams`` (None: greedy, every penalty off)."""
@@ -156,15 +170,30 @@ def token_state_row(prompt_ids, generated_ids, vocab: int, out: torch.Tensor | N
     return out
 
 
-def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor | None = None) -> torch.Tensor:
+def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor | None = None,
+                  constraints: torch.Tensor | None = None) -> torch.Tensor:
     """One seeded token per row of ``logits [rows, vocab]`` with the ``tl_sample`` kernel; ``params`` one
     ``SamplingParams`` (or None: greedy) per row, ``positions`` the index of each drawn token -> int32 ``[rows]``.
     When a row is penalised the launch is ``tl_sample_penalized`` over ``state`` (int32 ``[rows, vocab]``, required
-    then), which it updates at the drawn tokens of the rows with position > 0."""
+    then), which it updates at the drawn tokens of the rows with position > 0.  When a row carries a constraint the
+    launch is ``tl_sample_constrained`` over ``constraints`` (int64 ``[rows, 5]`` descriptor rows, required then: the
+    constrained rows' ``TokenConstraint.descriptor``, zero rows elsewhere), whose states it advances likewise."""
     from extensions_b200 import tiny_llm_ext_b200 as ext
 
     temperature, top_k, top_p, seed = sampling_tensors(params, logits.device)
     pos = torch.as_tensor(positions, dtype=torch.int32).to(logits.device)
+    if any_constrained(params):
+        if constraints is None:
+            raise ValueError("a constrained SamplingParams needs the request's constraint descriptor")
+        for p in params:
+            if p is not None and p.constraint is not None and p.constraint.vocab_size != logits.shape[-1]:
+                raise ValueError(f"the constraint's vocabulary has {p.constraint.vocab_size} ids, the logits {logits.shape[-1]}")
+        pen = ()
+        if any_penalized(params):
+            if state is None:
+                raise ValueError("a penalised SamplingParams needs the request's token state")
+            pen = (*penalty_tensors(params, logits.device), state)
+        return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
     if not any_penalized(params):
         return ext.sample(logits.contiguous(), temperature, top_k, top_p, seed, pos)
     if state is None:
