@@ -453,6 +453,50 @@ int tl_moe_grouped_matmul_route(int T, int k, int E, int N, int K, int epilogue,
 int tl_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_weight, float eps, void *out, void *normed_out,
                    int T, int k, int H, int dtype, void *stream);
 
+/* ---- Multi-LoRA: per-row bf16 low-rank adapters over a projection's output (DESIGN.md section 12) ----------------
+ * A SITE is one projection input x [M, N] with up to three output SEGMENTS (q|k|v: 3, o: 1, gate|up: 2, down: 1).
+ * Segment s of row m is the K_s elements at y[s] + m * ldy[s] (host arrays of nseg entries): the segments of one packed
+ * projection side by side (y[s] = base + K_0 + .. + K_{s-1}, ldy[s] = their sum) or one tensor per projection; the
+ * optional residual (host array of nseg pointers, or NULL) has the layout of y.  Per adapter a and segment s there is A_s [r_a, N] and
+ * B_s [K_s, r_a] in bf16 and sc_a = alpha / r_a in fp32.  For a row x (T = bf16) with adapter_ids[row] = a >= 0:
+ *   t_j = T(sum_fp32_i A_s[j,i] * x_i)                 j < r_a  (the intermediate is rounded once, as PEFT's is)
+ *   s_o = sum_fp32_j B_s[o,j] * float(t_j)             fp32, fmaf over j ascending from +0
+ *   y_o = T(fmaf(sc_a, s_o, float(base_o)))            one fp32 rounding of base_o + sc_a * s_o, then T; base_o: y as the
+ *                                                      projection left it (already rounded)
+ * and, with a residual: y_o = T(float(residual_o) + float(y_o)), the operator sequence add(x, lora(proj(h))).
+ * A row with adapter_ids[row] < 0 keeps base's bits (with a residual: T(residual + base)), and so does a segment the
+ * adapter's seg_mask does not name; nothing outside rows [0, M) of y is written.
+ * The i-sum runs in an order fixed by N alone: each of 8 CTAs takes ceil(N / 64) whole 8-element chunks, a lane its
+ * chunks 32 apart in ascending order with one fmaf per element, then the xor butterfly over the lanes, then the CTAs in
+ * order.  A row's result is therefore a pure function of that row and its adapter: the same bits alone, at any index of
+ * any launch, on either route and under graph replay.
+ * Storage is padded to the set's r_max with zeros: a [n_adapters, nseg * r_max, N] (segment s at rows s * r_max ..),
+ * b[s] [n_adapters, K_s, r_max]; rows / columns >= ranks[a] are never read, which equals adding their exact zeros.
+ * ranks[a] in {8, 16, 32, 64}; N % 8 == 0, N <= 12288; a, b[s], x 16-byte aligned.  Capture-safe: nothing is
+ * allocated or synchronised, adapter_ids is device data read after griddepcontrol.wait.
+ * Routes (tl_lora_apply_route; nothing is launched or read):
+ *   TL_LORA_ROWS  (M <= 64)  one 8-CTA cluster per row;
+ *   TL_LORA_TILES (M > 64)   one cluster per 8 consecutive rows: when they name one adapter (a prefill chunk) they share
+ *                            every load of A and B, each row still summed as above, so the bits are those of
+ *                            TL_LORA_ROWS; otherwise the cluster runs its rows one after the other.
+ * Both routes run on CUDA cores; there is no tensor-core route yet. */
+#define TL_LORA_MAX_SEGMENTS 3
+#define TL_LORA_MAX_RANK 64
+#define TL_LORA_MAX_ADAPTERS 32
+typedef struct tl_lora_site {
+    const void *a;           /* bf16 [n_adapters, nseg * r_max, N] */
+    const void *b[3];        /* bf16 [n_adapters, K_s, r_max] per segment */
+    const float *scales;     /* [n_adapters] alpha / r */
+    const int32_t *ranks;    /* [n_adapters] */
+    const int32_t *seg_mask; /* [n_adapters] bit s: the adapter targets segment s */
+    int32_t n_adapters, nseg, r_max, N;
+    int32_t K[3];
+} tl_lora_site;
+enum { TL_LORA_ROWS = 0, TL_LORA_TILES = 1 };
+int tl_lora_apply_route(int M, int dtype, const tl_lora_site *site);
+int tl_lora_apply(const void *x, void *const *y, const void *const *residual, const long long *ldy, const int32_t *adapter_ids,
+                  const tl_lora_site *site, int M, int dtype, void *stream);
+
 /* Programmatic dependent launch for the streaming kernels (on by default; 0 turns it off,
  * TL_PDL=0 in the environment does the same). */
 int tl_set_pdl(int enabled);

@@ -38,6 +38,7 @@ SOURCES = [
     "logprobs.cu",
     "constrained.cu",
     "moe.cu",
+    "lora.cu",
     "tma.cu",
 ]
 

@@ -726,4 +726,20 @@ int tl_moe_combine(const void *y, const void *scores, const void *residual, cons
     return launch_moe_combine(y, scores, residual, norm_weight, eps, out, normed_out, T, k, H, dtype, as_stream(stream));
 }
 
+int tl_lora_apply_route(int M, int dtype, const tl_lora_site *site) { return lora_route(M, dtype, site); }
+
+int tl_lora_apply(const void *x, void *const *y, const void *const *residual, const long long *ldy, const int32_t *adapter_ids,
+                  const tl_lora_site *site, int M, int dtype, void *stream) {
+    const int route = lora_route(M, dtype, site);
+    if (route < 0) return route;
+    if (M == 0) return TL_OK;
+    if (!x || !y || !ldy || !adapter_ids || !site->a || !site->scales || !site->ranks || !site->seg_mask) return fail(TL_EINVAL, "lora_apply: null pointer");
+    if (!aligned16(x) || !aligned16(site->a)) return fail(TL_EINVAL, "lora_apply: x and A must be 16-byte aligned");
+    for (int s = 0; s < site->nseg; ++s)
+        if (!site->b[s] || !aligned16(site->b[s])) return fail(TL_EINVAL, "lora_apply: B of segment %d must be a 16-byte aligned pointer", s);
+    for (int s = 0; s < site->nseg; ++s)
+        if (!y[s] || ldy[s] < site->K[s] || (residual && !residual[s])) return fail(TL_EINVAL, "lora_apply: bad output of segment %d", s);
+    return launch_lora_apply(x, y, residual, ldy, adapter_ids, *site, M, route, as_stream(stream));
+}
+
 }  // extern "C"

@@ -111,6 +111,11 @@ int launch_moe_combine(const void *y, const void *scores, const void *residual, 
 int launch_moe_grouped_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets,
                                const int32_t *out_index, int R, int E, int N, int K, int epilogue, int dtype, cudaStream_t st);
 
+// lora.cu: the route (TL_LORA_ROWS | TL_LORA_TILES) or a negative TL_E* code for a site the launch rejects
+int lora_route(int M, int dtype, const tl_lora_site *site);
+int launch_lora_apply(const void *x, void *const *y, const void *const *residual, const long long *ldy, const int32_t *adapter_ids,
+                      const tl_lora_site &site, int M, int route, cudaStream_t st);
+
 // decode_attention_fused.cu
 #if defined(TL_TRACE) && TL_TRACE
 void trace_bind_matvec(unsigned long long *buf, unsigned int *n, unsigned int cap);

@@ -67,6 +67,9 @@ __all__ = [
     "moe_grouped_matmul",
     "moe_grouped_matmul_route",
     "moe_combine",
+    "LoraSite",
+    "lora_apply",
+    "lora_apply_route",
 ]
 
 _HERE = Path(__file__).resolve().parent
@@ -131,6 +134,8 @@ _SIGNATURES = {
     "tl_moe_grouped_matmul_route": (_I, [_I] * 7 + [_VP] * 2 + [ctypes.POINTER(_I)] * 2),
     "tl_moe_grouped_matmul": (_I, [_VP] * 8 + [_I] * 7 + [_VP]),
     "tl_moe_combine": (_I, [_VP] * 4 + [_F, _VP, _VP] + [_I] * 4 + [_VP]),
+    "tl_lora_apply_route": (_I, [_I, _I, _VP]),
+    "tl_lora_apply": (_I, [_VP] * 6 + [_I, _I, _VP]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -1331,6 +1336,112 @@ def moe_combine(y, scores, residual=None, norm_weight=None, eps=0.0, stream=None
                                None if norm_weight is None else norm_weight.data_ptr(), float(eps), out.data_ptr(),
                                None if normed is None else normed.data_ptr(), T, k, H, _DTYPE_CODE[y.dtype], _stream_ptr(stream, y)))
     return out if normed is None else (out, normed)
+
+
+LORA_MAX_SEGMENTS, LORA_MAX_RANK, LORA_MAX_ADAPTERS = 3, 64, 32
+LORA_RANKS = (8, 16, 32, 64)
+LORA_ROWS, LORA_TILES = 0, 1
+
+
+class _LoraSiteC(ctypes.Structure):
+    """``tl_lora_site``."""
+
+    _fields_ = [("a", _VP), ("b", _VP * 3), ("scales", _VP), ("ranks", _VP), ("seg_mask", _VP),
+                ("n_adapters", ctypes.c_int32), ("nseg", ctypes.c_int32), ("r_max", ctypes.c_int32), ("N", ctypes.c_int32),
+                ("K", ctypes.c_int32 * 3)]
+
+
+class LoraSite:
+    """The packed adapters of one site (``tl_lora_site``): ``a`` bf16 ``[n_adapters, nseg * r_max, N]``, ``b`` one bf16
+    ``[n_adapters, K_s, r_max]`` per segment, ``scales`` f32, ``ranks`` and ``seg_mask`` int32 ``[n_adapters]``.  It keeps
+    the tensors alive for the launches (and captured graphs) that read them."""
+
+    def __init__(self, a, b, scales, ranks, seg_mask):
+        b = list(b)
+        if a.dtype != torch.bfloat16 or a.dim() != 3 or any(t.dtype != torch.bfloat16 or t.dim() != 3 for t in b):
+            raise RuntimeError("lora_apply: A and B must be bfloat16 [n_adapters, rows, cols]")
+        n, J, N = a.shape
+        if not 1 <= len(b) <= LORA_MAX_SEGMENTS or J % len(b) != 0:
+            raise RuntimeError(f"lora_apply: a site has 1 to {LORA_MAX_SEGMENTS} segments, A [n_adapters, nseg * r_max, N]")
+        r_max = J // len(b)
+        if not 1 <= n <= LORA_MAX_ADAPTERS:
+            raise RuntimeError(f"lora_apply: a set holds 1 to {LORA_MAX_ADAPTERS} adapters")
+        if r_max not in LORA_RANKS:
+            raise RuntimeError(f"lora_apply: r_max must be one of {LORA_RANKS}")
+        if N % 8 != 0:
+            raise RuntimeError("lora_apply: the input width must be a multiple of 8")
+        if any(t.shape[0] != n or t.shape[2] != r_max for t in b):
+            raise RuntimeError("lora_apply: every B must be [n_adapters, K_s, r_max]")
+        if scales.dtype != torch.float32 or ranks.dtype != torch.int32 or seg_mask.dtype != torch.int32 \
+                or any(tuple(t.shape) != (n,) for t in (scales, ranks, seg_mask)):
+            raise RuntimeError("lora_apply: scales f32, ranks and seg_mask int32, one entry per adapter")
+        _contig("lora_apply", a=a, scales=scales, ranks=ranks, seg_mask=seg_mask, **{f"b{s}": t for s, t in enumerate(b)})
+        self.a, self.b, self.scales, self.ranks, self.seg_mask = a, b, scales, ranks, seg_mask
+        self.n_adapters, self.nseg, self.r_max, self.N = n, len(b), r_max, N
+        self.K = [t.shape[1] for t in b]
+        ptrs = [t.data_ptr() for t in b] + [None] * (3 - len(b))
+        self.c = _LoraSiteC(a.data_ptr(), (_VP * 3)(*ptrs), scales.data_ptr(), ranks.data_ptr(), seg_mask.data_ptr(), n, len(b), r_max, N,
+                            (ctypes.c_int32 * 3)(*(self.K + [0] * (3 - len(b)))))
+
+
+def _lora_segments(y, site, name):
+    """``y`` (one ``[M, sum K_s]`` tensor holding the segments side by side, or one ``[M, K_s]`` tensor per segment) as
+    per-segment views."""
+    if not all(t.is_contiguous() for t in ([y] if isinstance(y, torch.Tensor) else y)):
+        raise RuntimeError(f"lora_apply: {name} must be contiguous (it is updated in place)")
+    if isinstance(y, torch.Tensor):
+        y2 = y.reshape(-1, y.shape[-1])
+        if y2.shape[1] != sum(site.K):
+            raise RuntimeError(f"lora_apply: {name} must be [M, {sum(site.K)}] (the site's segments side by side)")
+        return list(torch.split(y2, site.K, dim=1))
+    segs = [t.reshape(-1, t.shape[-1]) for t in y]
+    if [t.shape[1] for t in segs] != site.K:
+        raise RuntimeError(f"lora_apply: {name} must hold one [M, K_s] tensor per segment, K = {site.K}")
+    return segs
+
+
+def _lora_args(x, y, adapter_ids, site, residual):
+    if not isinstance(site, LoraSite):
+        raise RuntimeError("lora_apply: site must be a LoraSite")
+    M = adapter_ids.numel()
+    ys = _lora_segments(y, site, "y")
+    rs = None if residual is None else _lora_segments(residual, site, "residual")
+    if x.dtype != torch.bfloat16 or any(t.dtype != torch.bfloat16 for t in ys + (rs or [])):
+        raise RuntimeError("lora_apply: activations must be bfloat16")
+    if x.shape[-1] != site.N or x.numel() != M * site.N:
+        raise RuntimeError(f"lora_apply: x must be [{M}, {site.N}] (one row per adapter id)")
+    for s, t in enumerate(ys):
+        if t.shape[0] != M or t.stride(1) != 1:
+            raise RuntimeError(f"lora_apply: segment {s} of y must be [{M}, {site.K[s]}] with unit column stride")
+        if rs is not None and (rs[s].shape != t.shape or rs[s].stride() != t.stride()):
+            raise RuntimeError("lora_apply: residual must have the layout of y")
+    _int32("lora_apply", M, adapter_ids=adapter_ids)
+    return M, ys, rs
+
+
+def lora_apply_route(M: int, site: LoraSite) -> int:
+    """``LORA_ROWS`` (a cluster per row, M <= 64) or ``LORA_TILES`` (a cluster per 8 rows) for ``M`` rows of ``site``."""
+    route = _lib.tl_lora_apply_route(int(M), _DTYPE_CODE[torch.bfloat16], ctypes.byref(site.c))
+    if route < 0:
+        _check(route)
+    return route
+
+
+def lora_apply(x, y, adapter_ids, site: LoraSite, residual=None, stream=None):
+    """Add each row's adapter to the projection output ``y`` in place and return it (``tl_lora_apply``): row m with
+    ``adapter_ids[m] = a >= 0`` becomes ``T(y + sc_a * B_a T(A_a x))`` per targeted segment, then ``T(residual + y)`` with
+    a residual; rows with a negative id keep their bits (or take the residual add alone).  ``y`` (and ``residual``): one
+    tensor with the site's segments side by side, or a list of one tensor per segment."""
+    M, ys, rs = _lora_args(x, y, adapter_ids, site, residual)
+    _gpu("lora_apply", x, adapter_ids, site.a, *ys, *(rs or []))
+    _contig("lora_apply", x=x, adapter_ids=adapter_ids)
+    n = site.nseg
+    y_ptrs = (_VP * n)(*[t.data_ptr() for t in ys])
+    r_ptrs = None if rs is None else (_VP * n)(*[t.data_ptr() for t in rs])
+    ld = (_LL * n)(*[t.stride(0) if t.shape[0] > 1 else t.shape[1] for t in ys])
+    _check(_lib.tl_lora_apply(x.data_ptr(), y_ptrs, r_ptrs, ld, adapter_ids.data_ptr(), ctypes.byref(site.c), M, _DTYPE_CODE[x.dtype],
+                              _stream_ptr(stream, x)))
+    return y
 
 
 def set_pdl(enabled: bool) -> None:

@@ -24,6 +24,7 @@ from extensions_b200 import tiny_llm_ext_b200
 
 from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, token_logprobs
+from .lora import adapter_ids_of
 from .sampler import any_constrained, any_penalized, sample_tokens, sampling_per_request, token_state_row
 
 
@@ -37,9 +38,9 @@ def greedy_tokens(logits: torch.Tensor) -> torch.Tensor:
     return torch.argmax(logits, dim=-1)
 
 
-def _step(model, y, offsets, kv_cache):
-    """One model call -> one greedy token per row (batch.py:8-13)."""
-    logits = model(y, offsets, kv_cache, logits_to_keep=1)
+def _step(model, y, offsets, kv_cache, **lora):
+    """One model call -> one greedy token per row (batch.py:8-13).  ``lora``: the rows' ``adapter_ids``, when any is named."""
+    logits = model(y, offsets, kv_cache, logits_to_keep=1, **lora)
     return greedy_tokens(logits[:, -1, :])
 
 
@@ -83,8 +84,10 @@ class Request:
         sampling=None,
         logprobs=None,
         prefix_cache=None,
+        adapter_id: int = -1,
     ):
         self.prompt = prompt
+        self.adapter_id = adapter_id  # the request's id in the model's AdapterSet, -1: the base model
         self.sampling = sampling
         self.logprobs = logprobs
         self.logprob_entries: list = []
@@ -118,7 +121,12 @@ class Request:
         self.prompt_ids = ids if prefix_cache is not None else None
         self.reused_tokens = 0
         if prefix_cache is not None:
-            self.reused_tokens = self.offset = prefix_cache.adopt(prefix_cache.lookup(ids), self.kv_cache)
+            match = prefix_cache.lookup(ids) if adapter_id < 0 else prefix_cache.lookup(ids, adapter_id)
+            self.reused_tokens = self.offset = prefix_cache.adopt(match, self.kv_cache)
+
+    def _lora(self) -> dict:
+        """The adapter keyword of the request's model calls (nothing for the base model)."""
+        return {} if self.adapter_id < 0 else {"adapter_ids": [self.adapter_id]}
 
     def try_prefill(self):
         """Advance the prompt by at most ``prefill_max_step`` tokens (batch.py:48-76)."""
@@ -129,9 +137,9 @@ class Request:
         ids = self.prefill_tokens[self.offset : self.offset + chunk][None]
         entry = None
         if self.sampling is None and self.logprobs is None:
-            token = _step(self.model, ids, [self.offset], self.kv_cache)
+            token = _step(self.model, ids, [self.offset], self.kv_cache, **self._lora())
         else:  # only the last chunk's token is used: the prompt's first token is drawn at position `total`
-            logits = self.model(ids, [self.offset], self.kv_cache, logits_to_keep=1)[:, -1, :]
+            logits = self.model(ids, [self.offset], self.kv_cache, logits_to_keep=1, **self._lora())[:, -1, :]
             token = None
             if self.offset + chunk == total:
                 if self.sampling is None:
@@ -151,7 +159,10 @@ class Request:
         if self.offset == total:
             self.is_prefill_done = True
             if self.prefix_cache is not None:
-                self.prefix_cache.insert(self.prompt_ids, self.kv_cache)
+                if self.adapter_id < 0:
+                    self.prefix_cache.insert(self.prompt_ids, self.kv_cache)
+                else:
+                    self.prefix_cache.insert(self.prompt_ids, self.kv_cache, self.adapter_id)
             if self.max_seq_len is not None and self.offset >= self.max_seq_len:
                 self.is_done = True
                 self.finish_reason = "max seq len"
@@ -225,10 +236,15 @@ class ContinuousBatcher:
     Constrained requests (``SamplingParams.constraint``) keep their automaton state in one int64 ``[batch_size, 5]``
     slab of ``tl_constraint_row`` descriptors, allocated when the first of them enters a slot.  Admission copies the
     request's row (advanced by its prefill draw) into the slot on the device; idle and unconstrained slots hold zero
-    rows.  Every decode step with a constrained slot is one ``tl_sample_constrained`` launch over all slots."""
+    rows.  Every decode step with a constrained slot is one ``tl_sample_constrained`` launch over all slots.
+
+    ``adapters`` (None, one name for every prompt, or one name or None per prompt) runs each request under that LoRA
+    adapter of the model's ``AdapterSet`` (``Qwen3ModelWeek3.load_adapters``): its prefill chunks carry its id, its slot
+    carries it from admission to release (``slot_adapter_ids``, -1 for idle and base-model slots), and its prefix-cache
+    lookups see only pages computed under the same adapter.  A request's tokens are those it gets alone."""
 
     def __init__(self, model, tokenizer, prompts, max_seq_len=512, batch_size=5, prefill_step=128, verbose=True,
-                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None, prefix_cache=False):
+                 eos_token_id=None, device=None, max_new_tokens=None, sampling=None, logprobs=None, prefix_cache=False, adapters=None):
         if max_seq_len <= 0:
             raise ValueError("max_seq_len must be positive")
         if batch_size <= 0:
@@ -239,6 +255,8 @@ class ContinuousBatcher:
         self.tokenizer = tokenizer
         self.queue = list(prompts)
         self.sampling = sampling_per_request(sampling, len(self.queue))
+        self.adapter_ids = adapter_ids_of(model, adapters, len(self.queue))  # per prompt, None: no request names one
+        self.slot_adapter_ids = [-1] * batch_size
         self.logprobs_n = None if logprobs is None else _check_n(logprobs)
         self.logprobs: dict[int, list] = {}
         self.max_seq_len = max_seq_len
@@ -349,6 +367,7 @@ class ContinuousBatcher:
                 max_seq_len=self.max_seq_len, eos_token_id=self.eos_token_id, device=self.device,
                 sampling=None if self.sampling is None else self.sampling[self.next_request_idx],
                 logprobs=self.logprobs_n, prefix_cache=self.prefix_cache,
+                adapter_id=-1 if self.adapter_ids is None else self.adapter_ids[self.next_request_idx],
             )
             if self.prefix_cache is not None:
                 self.reused_tokens[self.next_request_idx] = self.pending.reused_tokens
@@ -388,6 +407,7 @@ class ContinuousBatcher:
                                 table.add_request(layer_cache, i)
                             self._admit_state(request, i)
                             self._admit_constraint(request, i)
+                            self.slot_adapter_ids[i] = request.adapter_id
                             self.slots[i] = request
                             self.pending = None
                             moved = True
@@ -404,10 +424,11 @@ class ContinuousBatcher:
             span = self._gpu_span("decode")
             batch = torch.tensor(tokens, dtype=torch.int32, device=self.device).reshape(-1, 1)
             entries = None
+            lora = {} if self.adapter_ids is None else {"adapter_ids": list(self.slot_adapter_ids)}
             if self.sampling is None and self.logprobs_n is None:
-                sampled = _step(self.model, batch, offsets, self.kv_cache)
+                sampled = _step(self.model, batch, offsets, self.kv_cache, **lora)
             else:  # slot i draws the token at position offset + 1; idle and greedy slots get argmax's token
-                logits = self.model(batch, offsets, self.kv_cache, logits_to_keep=1)[:, -1, :]
+                logits = self.model(batch, offsets, self.kv_cache, logits_to_keep=1, **lora)[:, -1, :]
                 if self.sampling is None:
                     sampled = greedy_tokens(logits)
                 else:  # idle slots draw greedily at position 0: a penalised launch leaves their state rows alone
@@ -448,6 +469,7 @@ class ContinuousBatcher:
                     if self.constraint_rows is not None:
                         self.constraint_rows[i].zero_()
                     self.results.append((request.prompt_idx, text))
+                    self.slot_adapter_ids[i] = -1
                     self.slots[i] = None
             self._progress()
 

@@ -20,6 +20,9 @@ see checkpoint.py; there is no hub download here).
         (requests share the KV pages of a common prompt prefix; reused tokens per request and cache stats after the text)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --regex "[0-9]{4}-[0-9]{2}-[0-9]{2}"
         (every generated token keeps the text inside the pattern's language; EOS ends it once it is a match)
+    python -m tiny_llm_b200.cli batch --synthetic tiny-d128 --synthetic-lora a=16 --synthetic-lora b=8:1 \
+        --prompt-ids "5,17,3;5,17,3;5,17,3" --adapters "a;;b"
+        (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
 """
 
 from __future__ import annotations
@@ -51,6 +54,42 @@ def _model(args, ns, name):
     if args.loader == "week2":
         return dispatch_model(name, ns, week=2)
     return dispatch_model(name, ns, week=3, enable_paged_attention=not args.disable_paged_attention)
+
+
+def parse_lora_specs(lora, synthetic_lora):
+    """``--lora NAME=DIR`` and ``--synthetic-lora NAME=RANK[:SEED]`` as ``[(name, directory)]`` and ``[(name, rank, seed)]``."""
+    loaded, made = [], []
+    for spec in lora or []:
+        name, sep, path = spec.partition("=")
+        if not sep or not name or not path:
+            raise SystemExit(f"--lora expects NAME=DIR, got {spec!r}")
+        loaded.append((name, path))
+    for spec in synthetic_lora or []:
+        name, sep, rest = spec.partition("=")
+        rank, _, seed = rest.partition(":")
+        if not sep or not name or not rank.isdigit() or (seed and not seed.isdigit()):
+            raise SystemExit(f"--synthetic-lora expects NAME=RANK[:SEED], got {spec!r}")
+        made.append((name, int(rank), int(seed) if seed else 0))
+    return loaded, made
+
+
+def _load_adapters(args, model, ns) -> None:
+    """Give ``model`` the adapters the flags name (nothing without them)."""
+    from .lora import LoraAdapter
+
+    loaded, made = parse_lora_specs(args.lora, args.synthetic_lora)
+    if not loaded and not made:
+        return
+    if not hasattr(model, "load_adapters"):
+        raise SystemExit("--lora / --synthetic-lora need the week3 model")
+    try:
+        adapters = [LoraAdapter.load(path, name) for name, path in loaded]
+        adapters += [LoraAdapter.synthetic(ns.args, rank, seed=seed, name=name) for name, rank, seed in made]
+        loaded_set = model.load_adapters(adapters)
+    except (ValueError, OSError) as exc:
+        raise SystemExit(f"adapters: {exc}")
+    if getattr(args, "adapter", None) is not None and args.adapter not in loaded_set.names:
+        raise SystemExit(f"--adapter {args.adapter!r} is not among the loaded adapters {loaded_set.names}")
 
 
 def _prompt_ids(args, tokenizer, prompt: str | None):
@@ -105,6 +144,11 @@ def _constraint(args, model, tokenizer, device):
         raise SystemExit(f"--regex: {exc}")
 
 
+def _adapter_kw(args, key: str) -> dict:
+    """``{key: name}`` for ``--adapter NAME`` (nothing without it, so models that take no adapters run as before)."""
+    return {} if args.adapter is None else {key: args.adapter}
+
+
 def cmd_generate(args) -> int:
     from .generate import greedy_generate_ids
     from .sampler import SamplingParams, make_sampler
@@ -112,6 +156,7 @@ def cmd_generate(args) -> int:
     device = torch.device(args.device)
     ns, tokenizer, name = _load(args, device)
     model = _model(args, ns, name)
+    _load_adapters(args, model, ns)
     ids = _prompt_ids(args, tokenizer, args.prompt)
     sampler = sampling = None
     penalties = _penalties(args)
@@ -141,6 +186,8 @@ def cmd_generate(args) -> int:
     if args.draft_model or args.draft_synthetic:
         from .generate import speculative_generate_ids
 
+        if args.adapter is not None or getattr(model, "adapters", None) is not None:
+            raise SystemExit("speculative decoding does not take adapters: drop --lora / --synthetic-lora / --adapter")
         if sampler is not None or sampling is not None:
             raise SystemExit("speculative decoding is greedy: drop --sampler-temp")
         if args.logprobs is not None:
@@ -160,7 +207,7 @@ def cmd_generate(args) -> int:
         print()
         return 0
     produced = greedy_generate_ids(model, ids, args.max_new_tokens, eos_token_id=eos, device=device,
-                                   on_token=emit, sampler=sampler, sampling=sampling, logprobs=args.logprobs)
+                                   on_token=emit, sampler=sampler, sampling=sampling, logprobs=args.logprobs, **_adapter_kw(args, "adapter"))
     print()
     if args.logprobs is not None:
         produced, entries = produced
@@ -176,6 +223,7 @@ def cmd_batch(args) -> int:
     device = torch.device(args.device)
     ns, tokenizer, name = _load(args, device)
     model = _model(args, ns, name)
+    _load_adapters(args, model, ns)
     if args.prompts_file:
         prompts = [line.strip() for line in open(args.prompts_file) if line.strip()]
     else:
@@ -196,10 +244,19 @@ def cmd_batch(args) -> int:
     if args.prefix_cache and not hasattr(model, "enable_prefix_cache"):
         raise SystemExit("--prefix-cache needs the paged week3 model")
     eos = constraint.vocabulary.eos_ids[0] if constraint is not None and args.synthetic else None
-    batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
-                                verbose=not args.quiet, device=device, eos_token_id=eos,
-                                max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None, sampling=sampling,
-                                logprobs=args.logprobs, prefix_cache=args.prefix_cache)
+    extra = {}
+    if args.adapters is not None:  # one name per prompt, empty: the base model
+        names = [n.strip() or None for n in args.adapters.split(";")]
+        if len(names) != len(queue):
+            raise SystemExit(f"--adapters names {len(names)} requests, there are {len(queue)} prompts")
+        extra["adapters"] = names
+    try:
+        batcher = ContinuousBatcher(model, tokenizer, queue, max_seq_len=args.max_seq_len, batch_size=args.batch_size, prefill_step=args.prefill_step,
+                                    verbose=not args.quiet, device=device, eos_token_id=eos,
+                                    max_new_tokens=[args.max_new_tokens] * len(queue) if args.max_new_tokens else None, sampling=sampling,
+                                    logprobs=args.logprobs, prefix_cache=args.prefix_cache, **extra)
+    except (KeyError, ValueError) as exc:  # an adapter name that is not loaded
+        raise SystemExit(f"batch: {exc}")
     results = batcher.run()
     for idx, text in sorted(results):
         print(f"--- request {idx}\n{text}")
@@ -218,6 +275,7 @@ def cmd_score(args) -> int:
     device = torch.device(args.device)
     ns, tokenizer, name = _load(args, device)
     model = _model(args, ns, name)
+    _load_adapters(args, model, ns)
     if args.prompt_ids:
         ids = [int(t) for t in args.prompt_ids.split(",")]
     elif tokenizer is None:
@@ -226,7 +284,7 @@ def cmd_score(args) -> int:
         ids = tokenizer.encode(args.prompt, add_special_tokens=False)
     if len(ids) < 2:
         raise SystemExit("scoring needs a prompt of at least two tokens")
-    result = score_ids(model, ids, chunk=args.chunk, top_n=args.logprobs or 0, device=device)
+    result = score_ids(model, ids, chunk=args.chunk, top_n=args.logprobs or 0, device=device, **_adapter_kw(args, "adapter"))
     print(f"prompt: {len(ids)} tokens; first token {_token_text(tokenizer, ids[0])} is not scored")
     _print_logprobs(result.entries, tokenizer)
     print(f"total nll {result.nll:.4f} nats over {len(result.entries)} tokens, perplexity {result.perplexity:.4f}")
@@ -267,6 +325,14 @@ def main(argv=None) -> int:
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")
+        sub.choices[name].add_argument("--lora", action="append", default=None, metavar="NAME=DIR",
+                                       help="load a PEFT LoRA adapter directory under NAME (repeatable, up to 32)")
+        sub.choices[name].add_argument("--synthetic-lora", action="append", default=None, metavar="NAME=RANK[:SEED]",
+                                       help="a seeded random adapter of RANK (8, 16, 32 or 64) on every projection (repeatable)")
+    for name in ("generate", "score"):
+        sub.choices[name].add_argument("--adapter", default=None, metavar="NAME", help="run the request under this loaded adapter")
+    sub.choices["batch"].add_argument("--adapters", default=None, metavar="A;;B",
+                                      help="one loaded adapter name per prompt, ';' between them (empty: the base model)")
     sub.choices["score"].add_argument("--chunk", type=int, default=512, help="prompt tokens per forward pass (bounds the live logits)")
     sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
     sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")

@@ -132,6 +132,50 @@ def _swap_ab_layers(model, x, attention):
     return h
 
 
+def lora_projection_is_fused(rows: int) -> bool:
+    """Whether ``_lora_layers`` projects ``rows`` rows through ``quantized_matmul_fused`` (else ``quantized_matmul``)."""
+    return rows <= 128
+
+
+def _lora_layers(model, x, ids, attention):
+    """The layer stack of a model with an ``AdapterSet`` (``lora.py``), for any number of rows ``x``; ``ids`` holds one
+    adapter id per row (device data: -1 runs the base model) and ``attention(i, block, qkv)`` turns layer ``i``'s q|k|v
+    rows into ``[rows, Hq * D]``.  Returns the residual stream before the final norm.
+
+    Every adapter delta has to land on its projection's output before the next operator reads it, so the fused
+    prologues and epilogues of the base stacks (RMSNorm into the projection, SwiGLU and the residual out of it) are
+    their own launches here: rms_norm, q|k|v, lora, attention, o, lora (+ residual), rms_norm, gate, up, lora, swiglu,
+    down, lora (+ residual).  A site no adapter of the set targets issues no lora launch (its residual is ``add``).
+    Up to 128 rows the projections are the fused entry's (streaming matvec to 8 rows, swap-AB wgmma split reduction to
+    128); beyond, the plain entry's 128-token wgmma tile GEMM, as in the base prefill engine's per-operator branch (the
+    fused entry would keep such chunks on the streaming matvec, one pass over the weights per 32 rows).
+    The rounding points are those of the operator path with the same ids."""
+    packed, sites = model.packed_layers(), model.adapters.sites
+    if lora_projection_is_fused(x.shape[0]):
+        fused = lambda w, h: ext.quantized_matmul_fused(w.scales, w.biases, w.weight, h)
+    else:
+        fused = lambda w, h: _proj(h, w)
+
+    def plus_residual(inp, out, site):
+        return ext.add(x, out) if site is None else ext.lora_apply(inp, out, ids, site, residual=x)
+
+    for i, block in enumerate(model.layers_inner):
+        at, mlp, st = block.self_attn, block.mlp, sites[i]
+        h = _normed(x, block.input_layernorm)
+        qkv = fused(packed[i].qkv, h)
+        if st.qkv is not None:
+            ext.lora_apply(h, qkv, ids, st.qkv)
+        y = attention(i, block, qkv)
+        x = plus_residual(y, fused(at.wo, y), st.o)
+        h = _normed(x, block.post_attention_layernorm)
+        gate, up = fused(mlp.w_gate, h), fused(mlp.w_up, h)
+        if st.gate_up is not None:
+            ext.lora_apply(h, [gate, up], ids, st.gate_up)
+        act = ext.swiglu(gate, up)
+        x = plus_residual(act, fused(mlp.w_down, act), st.down)
+    return x
+
+
 class _GraphEngine:
     """What the decode and prefill engines share: the geometry, one pinned int32 metadata block with its device mirror
     (each engine lays it out as ``header | block tables`` and initialises the tables to -1), the event that keeps the
@@ -151,6 +195,7 @@ class _GraphEngine:
         self.max_pages = (max_seq_len + self.page_size - 1) // self.page_size
         self.max_seq_len = self.max_pages * self.page_size
         self.n_layers = model.num_hidden_layers
+        self.lora = model.adapters  # an AdapterSet: this is a LoRA engine (``_lora_layers``, per-row adapter ids as device data)
         attn = model.layers_inner[0].self_attn
         self.Hq, self.Hkv, self.D = attn.num_heads, attn.num_kv_heads, attn.head_dim
         # tables: [layers, table_rows, max_pages]
@@ -215,6 +260,24 @@ class _GraphEngine:
         if self._upload_pending:
             self._upload_event.synchronize()
             self._upload_pending = False
+
+    def _alloc_adapter_ids(self, rows: int, key) -> None:
+        """A LoRA engine's adapter id per row, in its own pinned block (all -1: the base model), uploaded when it changes;
+        ``key`` is what ``_set_adapter_ids`` compares against for that state."""
+        self._ad_host = torch.full((rows,), -1, dtype=torch.int32).pin_memory()
+        self.adapter_ids = self._ad_host.to(self.device, copy=True)
+        self._ad_key = key
+
+    def _set_adapter_ids(self, key) -> int:
+        """Upload the rows' ids if they changed: ``key`` is a tuple of one id per row, or one int for all rows.  Returns
+        the bytes copied."""
+        if key == self._ad_key:
+            return 0
+        self._host_write_begin()
+        self._ad_host.numpy()[:] = key
+        self._upload_meta(self.adapter_ids, self._ad_host)
+        self._ad_key = key
+        return 4 * self._ad_host.numel()
 
     def _upload_meta(self, dev, host) -> None:
         """Copy the pinned block (or a prefix of it) to its device mirror on the current stream."""
@@ -346,6 +409,10 @@ class DecodeEngine(_GraphEngine):
         self._con_host = None
         self._con_dev = None
         self._con_key = None
+        if self.lora is not None:
+            if rows_per_request != 1 or not self.fused:
+                raise ValueError("a model with adapters runs one row per slot on the fused decode step")
+            self._alloc_adapter_ids(B, (-1,) * B)
 
     @staticmethod
     def fused_attention_applies(model, slot_tokens: int) -> bool:
@@ -429,7 +496,10 @@ class DecodeEngine(_GraphEngine):
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens[:R], emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits)
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
-        if self.B > 8:
+        if self.lora is not None:
+            x = _normed(_lora_layers(m, x, self.adapter_ids[:R], self._qkv_attention(R)), m.norm)
+            logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x)
+        elif self.B > 8:
             h = _swap_ab_layers(m, x, self._swap_ab_attention(R))
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, h)
         else:
@@ -458,6 +528,26 @@ class DecodeEngine(_GraphEngine):
             q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
                                             at.k_norm._weight_as(h.dtype, h.device), offsets, self.tables[i][:R], context_lens,
                                             pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps)
+            y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
+                                    at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
+            return y.view(R, Hq * D)
+
+        return attention
+
+    def _qkv_attention(self, R: int):
+        """The attention of ``_lora_layers`` for the first ``R`` slots, from q|k|v rows the adapters were already added to."""
+        m, Hq, Hkv, D = self.model, self.Hq, self.Hkv, self.D
+        offsets, context_lens = self.offsets[:R], self.context_lens[:R]
+
+        def attention(i, block, qkv):
+            at, pool = block.self_attn, m.page_pools[i]
+            qw, kw = at.q_norm._weight_as(qkv.dtype, qkv.device), at.k_norm._weight_as(qkv.dtype, qkv.device)
+            if self._attention_fused:
+                return ext.decode_attention_fused(qkv, qw, kw, offsets, self.tables[i][:R], context_lens, self._rope_inv_freq,
+                                                  pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
+                                                  self.max_seq_len, workspace=self._attn_ws)
+            q = ext.decode_qk_norm_rope_append(qkv, qw, kw, offsets, self.tables[i][:R], context_lens, pool._key_pages, pool._value_pages,
+                                               Hq, Hkv, at.rope.base, at.q_norm.eps)
             y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             return y.view(R, Hq * D)
@@ -864,13 +954,26 @@ class DecodeEngine(_GraphEngine):
         return 3 * self.rows * 4
 
     # ------------------------------------------------------------------ steps --
-    def step(self, tokens, offsets, caches):
+    def _adapters_of_call(self, adapter_ids) -> None:
+        """Take the slots' adapter ids of a ``step`` / ``decode_on_device`` call (None: every slot on the base model)."""
+        if self.lora is None:
+            if adapter_ids is not None and any(int(i) >= 0 for i in adapter_ids):
+                raise ValueError("adapter_ids given to an engine of a model without adapters")
+            return
+        ids = [-1] * self.B if adapter_ids is None else [int(i) for i in adapter_ids]
+        if len(ids) != self.B or any(i >= len(self.lora.names) for i in ids):
+            raise ValueError(f"adapter_ids must hold one loaded adapter id (or -1) per slot ({self.B})")
+        self.h2d_bytes += self._set_adapter_ids(tuple(ids))
+
+    def step(self, tokens, offsets, caches, adapter_ids=None):
         """One decode step.  ``tokens``: B ids (list or tensor), ``offsets``: B
-        RoPE positions; returns (logits [B, 1, V] static buffer, next_tokens [B])."""
+        RoPE positions; returns (logits [B, 1, V] static buffer, next_tokens [B]).  ``adapter_ids`` (LoRA engines): one
+        ``AdapterSet`` id per slot, -1 or None for the base model; the same graph serves every mix."""
         B = self.B
         self._host_write_begin()
         ctx = self._advance_host(caches, 1)
         self._ensure_graph()
+        self._adapters_of_call(adapter_ids)
         if isinstance(tokens, torch.Tensor):
             tok_host = None
         else:
@@ -895,7 +998,7 @@ class DecodeEngine(_GraphEngine):
         self.graph_replays += 1
         return self.logits.view(B, 1, self.V), self.next_tokens
 
-    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None):
+    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None, adapter_ids=None):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
@@ -911,7 +1014,8 @@ class DecodeEngine(_GraphEngine):
         With a constrained slot (``SamplingParams.constraint``) the step is ``tl_sample_constrained`` over the engine's
         slot descriptors, captured on first use per (penalised, logprobs); each launch advances the slots' automaton
         states.  ``history`` also sets a constrained slot's state to the walk of its generated ids; without it a slot
-        keeps its state while its constraint stays the same and starts at the start state otherwise."""
+        keeps its state while its constraint stays the same and starts at the start state otherwise.
+        ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         B = self.B
@@ -934,6 +1038,7 @@ class DecodeEngine(_GraphEngine):
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
+        self._adapters_of_call(adapter_ids)
         if penalized:
             self._alloc_penalties()
         if constrained:
@@ -1007,9 +1112,9 @@ class VerifyEngine(DecodeEngine):
     @staticmethod
     def supported(model, device, max_seq_len: int) -> bool:
         """Where the B = 1 decode engine itself runs fused matvec + fused attention, on dense models only (the verify pass
-        does not take the MoE block)."""
+        does not take the MoE block) without adapters (speculative decoding does not take them)."""
         return (torch.device(device).type == "cuda" and DecodeEngine.fused_attention_applies(model, max_seq_len)
-                and not any(isinstance(b.mlp, Moe) for b in model.layers_inner))
+                and not any(isinstance(b.mlp, Moe) for b in model.layers_inner) and getattr(model, "adapters", None) is None)
 
     def reserve_pools(self, pages_per_layer: int | None = None) -> None:
         raise RuntimeError("the verify step shares the B = 1 decode engine's pool reservation")
@@ -1076,6 +1181,8 @@ class PrefillEngine(_GraphEngine):
         self.replays = 0
         self.kernels_per_chunk = 0
         self._packed = model.packed_layers()
+        if self.lora is not None:  # one id per chunk, broadcast to its rows (padding rows carry it too: they are never stored)
+            self._alloc_adapter_ids(L, -1)
 
     @staticmethod
     def supported(model, device) -> bool:
@@ -1101,10 +1208,23 @@ class PrefillEngine(_GraphEngine):
         return ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
                                                True, Hkv, Hq)
 
+    def _qkv_attention(self, i, block, qkv):
+        """``_attention`` from q|k|v rows the adapters were already added to (LoRA engines, any chunk length)."""
+        at, pool = block.self_attn, self.model.page_pools[i]
+        q = ext.chunk_qk_norm_rope_append(qkv, at.q_norm._weight_as(qkv.dtype, qkv.device), at.k_norm._weight_as(qkv.dtype, qkv.device),
+                                          self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
+                                          self.Hq, self.Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
+        return ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
+                                               True, self.Hkv, self.Hq)
+
     def _forward(self) -> None:
         m, L = self.model, self.L
         emb = m.embedding.weight
         x = ext.quantized_embedding(self.tokens, emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits).view(L, -1)
+        if self.lora is not None:
+            x = _lora_layers(m, x, self.adapter_ids, self._qkv_attention)
+            self._finish(_normed(x[L - 1:L], m.norm))
+            return
         # logits_to_keep = 1: the hidden state is sliced before the final norm (qwen3_week3.py:330-338); RMSNorm is row-wise,
         # so the last row of the already normalised chunk is the same thing
         if L <= 128:  # the fused epilogues live in the <= 128-row tensor-core kernel; longer chunks use the 128 x 128-tile GEMM
@@ -1119,6 +1239,10 @@ class PrefillEngine(_GraphEngine):
                     continue
                 x = ext.add(x, _proj(ext.swiglu(_proj(h, block.mlp.w_gate), _proj(h, block.mlp.w_up)), block.mlp.w_down))
             last = _normed(x[L - 1:L], m.norm)
+        self._finish(last)
+
+    def _finish(self, last) -> None:
+        m = self.model
         head = m.w_lm_head if m.w_lm_head is not None else m.embedding.weight
         logits = _proj(last, head)
         self.next_token.copy_(ext.argmax(logits))
@@ -1147,10 +1271,13 @@ class PrefillEngine(_GraphEngine):
                 return False
         return True
 
-    def prefill_chunk(self, token_ids, offset: int, cache):
+    def prefill_chunk(self, token_ids, offset: int, cache, adapter_id: int = -1):
         """Append ``token_ids`` (1..chunk ids at positions offset.., a list or an int32 device tensor) to the request's
-        caches and return (logits [1, 1, V] of the last token - a static buffer -, greedy next token [1])."""
+        caches and return (logits [1, 1, V] of the last token - a static buffer -, greedy next token [1]).
+        ``adapter_id`` (LoRA engines): the request's ``AdapterSet`` id, -1 for the base model."""
         on_device = isinstance(token_ids, torch.Tensor)
+        if self.lora is None and adapter_id >= 0:
+            raise ValueError("adapter_id given to an engine of a model without adapters")
         r, L = (int(token_ids.numel()) if on_device else len(token_ids)), self.L
         self._host_write_begin()
         for layer, layer_cache in enumerate(cache):
@@ -1159,6 +1286,10 @@ class PrefillEngine(_GraphEngine):
             self.tables_np[layer, :n] = layer_cache.page_ids
             self.tables_np[layer, n:] = -1
         self._ensure_graph()
+        if self.lora is not None:
+            if adapter_id >= len(self.lora.names):
+                raise ValueError(f"adapter_id {adapter_id} exceeds the {len(self.lora.names)} loaded adapters")
+            self._set_adapter_ids(int(adapter_id))
         pad = L - r
         meta = self.meta_np
         meta[0:L] = 0

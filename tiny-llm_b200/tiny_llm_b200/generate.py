@@ -7,6 +7,7 @@ import torch
 
 from .batch import greedy_tokens
 from .logprobs import _check_n, token_logprobs
+from .lora import adapter_ids_of
 from .sampler import sample_tokens, token_state_row
 
 
@@ -17,7 +18,7 @@ def _release_kv_cache(kv_cache) -> None:
 
 
 def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: int | None = None, device=None, on_token=None, sampler=None,
-                        sampling=None, logprobs: int | None = None, prefix_cache: bool = False):
+                        sampling=None, logprobs: int | None = None, prefix_cache: bool = False, adapter: str | None = None):
     """The loop of ``simple_generate_with_kv_cache`` on token ids: the whole
     prompt is prefilled at offset 0 (its last-row logits give the first token),
     then one token per step at a growing offset.  Returns the generated ids.
@@ -31,11 +32,16 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     ``logprobs`` (an int N in [0, 20]) returns ``(ids, entries)`` instead: one ``TokenLogprobs`` per generated id, from
     the logits row it was chosen from (raw log-probability, rank and the N most likely alternatives).
     ``prefix_cache=True`` starts the request on the model's prefix index (``Qwen3ModelWeek3.enable_prefix_cache``):
-    only the prompt past its longest cached prefix is prefilled, and the prompt is indexed afterwards."""
+    only the prompt past its longest cached prefix is prefilled, and the prompt is indexed afterwards.
+    ``adapter`` names a LoRA adapter of the model's ``AdapterSet`` (``Qwen3ModelWeek3.load_adapters``): every model call
+    of the request runs under it, and its prefix-cache pages are kept apart from other adapters'."""
     if sampler is not None and sampling is not None:
         raise ValueError("give sampler or sampling, not both")
     if logprobs is not None:
         _check_n(logprobs)
+    lora = adapter_ids_of(model, adapter, 1)
+    lora_kw = {} if lora is None else {"adapter_ids": lora}
+    root = () if lora is None else (lora[0],)  # the prefix index's subtree
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
     entries: list = []
@@ -44,12 +50,12 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
         ids = [int(t) for t in prompt_ids]
         prompt = torch.as_tensor(ids, dtype=torch.int32, device=device)
         index = model.enable_prefix_cache() if prefix_cache else None
-        offset = 0 if index is None else index.adopt(index.lookup(ids), kv_cache)
+        offset = 0 if index is None else index.adopt(index.lookup(ids, *root), kv_cache)
         tokens = prompt[offset:]
         while len(produced) < max_new_tokens:
-            logits = model(tokens[None], offset, kv_cache, logits_to_keep=1)
+            logits = model(tokens[None], offset, kv_cache, logits_to_keep=1, **lora_kw)
             if index is not None and offset + tokens.numel() == len(ids):
-                index.insert(ids, kv_cache)
+                index.insert(ids, kv_cache, *root)
             if sampling is not None:
                 if sampling.penalized and state is None:
                     state = token_state_row(prompt, [], logits.shape[-1], device=logits.device)[None]

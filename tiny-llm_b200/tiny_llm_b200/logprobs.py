@@ -74,10 +74,15 @@ class PromptScore:
     next_top: tuple[tuple[int, float], ...]
 
 
-def score_ids(model, ids, chunk: int = 512, top_n: int = 0, device=None) -> PromptScore:
+def score_ids(model, ids, chunk: int = 512, top_n: int = 0, device=None, adapter: str | None = None) -> PromptScore:
     """Teacher-forced log-probabilities of a prompt.  The prompt goes through ``model(..., logits_to_keep=None)``
     ``chunk`` tokens at a time over one KV cache, so at most ``chunk x vocab`` logits are alive; each chunk's rows are
-    scored by ``ext.logprobs`` with the next ids as targets."""
+    scored by ``ext.logprobs`` with the next ids as targets.  ``adapter`` names a LoRA adapter of the model's
+    ``AdapterSet`` to score under."""
+    from .lora import adapter_ids_of
+
+    lora = adapter_ids_of(model, adapter, 1)
+    lora_kw = {} if lora is None else {"adapter_ids": lora}
     ids = [int(t) for t in ids]
     if len(ids) < 1:
         raise ValueError("score_ids needs at least one token")
@@ -93,7 +98,7 @@ def score_ids(model, ids, chunk: int = 512, top_n: int = 0, device=None) -> Prom
     try:
         for start in range(0, len(ids), chunk):
             piece = all_ids[start : start + chunk]
-            logits = model(piece[None], start, cache, logits_to_keep=None)[0]
+            logits = model(piece[None], start, cache, logits_to_keep=None, **lora_kw)[0]
             _, lp, rank, alt_ids, alt_lp = ext.logprobs(logits.contiguous(), targets[start : start + piece.numel()], None, top_n)
             parts.append((lp, rank, alt_ids, alt_lp))
     finally:

@@ -2,7 +2,9 @@
 
 ``PrefixCache`` is one radix tree per model over token ids, at page granularity.  A node holds the tokens of one page
 and that page's id in every layer's pool; a child is either full (``page_size`` tokens) or partial (fewer, always a
-leaf).  Full pages chain from position 0, so a node's K/V is valid only under its exact ancestry.
+leaf).  Full pages chain from position 0, so a node's K/V is valid only under its exact ancestry.  K/V computed under
+one LoRA adapter is wrong under another, so the tree has one root per adapter id (-1: the base model): a lookup under
+one adapter never sees pages indexed under another.
 
 * ``lookup(prompt)`` walks full pages by exact match and, where the prompt leaves the tree, picks the child (full or
   partial) with the longest common token prefix ``r``: its first ``r`` slots are copied on write into a private page.
@@ -70,6 +72,7 @@ class PrefixCache:
         self.pools = list(pools)
         self.page_size = pools[0].page_size
         self._root = _Node(None, (), None, 0)
+        self._roots = {-1: self._root}  # adapter id -> root of its subtree
         self._nodes: set[_Node] = set()
         self._tick = 0
         self.lookups = self.hits = self.reused_tokens = 0
@@ -86,12 +89,18 @@ class PrefixCache:
         return self.pools[0].extra_refs.get(node.pages[0], 0) > 0
 
     # ---- lookup and adoption -------------------------------------------------------
-    def lookup(self, prompt_ids) -> PrefixMatch:
+    def _root_of(self, adapter: int) -> _Node:
+        root = self._roots.get(adapter)
+        if root is None:
+            root = self._roots[adapter] = _Node(None, (), None, 0)
+        return root
+
+    def lookup(self, prompt_ids, adapter: int = -1) -> PrefixMatch:
         ids = [int(t) for t in prompt_ids]
         P, cap = self.page_size, len(ids) - 1
         self.lookups += 1
         match = PrefixMatch()
-        node, pos = self._root, 0
+        node, pos = self._root_of(adapter), 0
         while pos + P <= cap:
             child = node.children.get(tuple(ids[pos : pos + P]))
             if child is None:
@@ -143,14 +152,14 @@ class PrefixCache:
         return match.reused
 
     # ---- insertion -----------------------------------------------------------------
-    def insert(self, prompt_ids, caches) -> int:
-        """Index the prompt's pages from the request's ``caches`` (prefilled through the whole prompt).  Returns the
-        number of nodes added."""
+    def insert(self, prompt_ids, caches, adapter: int = -1) -> int:
+        """Index the prompt's pages from the request's ``caches`` (prefilled through the whole prompt under ``adapter``).
+        Returns the number of nodes added."""
         ids = [int(t) for t in prompt_ids]
         P = self.page_size
         if caches[0].offset < len(ids):
             raise ValueError("insert needs the whole prompt prefilled")
-        node, pos, added = self._root, 0, 0
+        node, pos, added = self._root_of(adapter), 0, 0
         for index in range(-(-len(ids) // P)):
             key = tuple(ids[pos : pos + P])
             pages = [c.page_ids[index] for c in caches]
@@ -197,7 +206,7 @@ class PrefixCache:
 
     def clear(self) -> None:
         """Drop the index's reference on every page: pages no request holds go back to their pools."""
-        stack = list(self._root.children.values())
+        stack = [n for root in self._roots.values() for n in root.children.values()]
         order = []
         while stack:
             n = stack.pop()

@@ -15,6 +15,8 @@ from typing import Any
 
 import torch
 
+from extensions_b200 import tiny_llm_ext_b200 as ext
+
 from .attention import paged_attention
 from .embedding import QuantizedEmbedding
 from .kv_cache import TinyKvCache
@@ -63,13 +65,18 @@ class Qwen3MultiHeadAttention:
         self.k_norm = FastRMSNorm(head_dim, k_norm, eps=rms_norm_eps)
         self.use_paged_attention = use_paged_attention
 
-    def __call__(self, x, offsets, cache: TinyKvCache, mask=None):
+    def __call__(self, x, offsets, cache: TinyKvCache, mask=None, lora=None):
+        """``lora``: ``(sites, row_ids)``, the layer's ``AdapterSet`` sites and one adapter id per row of ``x``: each
+        targeted projection's output takes its row's adapter (``ext.lora_apply``) before anything reads it."""
         B, L, _ = x.shape
-        q = quantized_linear(x, self.wq).reshape(B, L, self.num_heads, self.head_dim)
-        k = quantized_linear(x, self.wk).reshape(B, L, self.num_kv_heads, self.head_dim)
+        q, k, v = quantized_linear(x, self.wq), quantized_linear(x, self.wk), quantized_linear(x, self.wv)
+        if lora is not None and lora[0].qkv is not None:
+            ext.lora_apply(x, [q, k, v], lora[1], lora[0].qkv)
+        q = q.reshape(B, L, self.num_heads, self.head_dim)
+        k = k.reshape(B, L, self.num_kv_heads, self.head_dim)
         q = self.q_norm(q)
         k = self.k_norm(k)
-        v = quantized_linear(x, self.wv).reshape(B, L, self.num_kv_heads, self.head_dim)
+        v = v.reshape(B, L, self.num_kv_heads, self.head_dim)
         q = self.rope(q, offset=offsets)
         k = self.rope(k, offset=offsets)
         q, k, v = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)  # [B, H, L, D]
@@ -96,7 +103,10 @@ class Qwen3MultiHeadAttention:
             else:
                 y = scaled_dot_product_attention(q, keys, values, scale=self.scale, mask=mask)
         y = y.transpose(1, 2).reshape(B, L, self.num_heads * self.head_dim)
-        return quantized_linear(y, self.wo)
+        out = quantized_linear(y, self.wo)
+        if lora is not None and lora[0].o is not None:
+            ext.lora_apply(y, out, lora[1], lora[0].o)
+        return out
 
 
 class Qwen3MLP:
@@ -107,8 +117,18 @@ class Qwen3MLP:
         self.hidden_dim = hidden_dim
         self.w_gate, self.w_up, self.w_down = w_gate, w_up, w_down
 
-    def __call__(self, x: torch.Tensor) -> torch.Tensor:
-        return quantized_linear(swiglu(quantized_linear(x, self.w_gate), quantized_linear(x, self.w_up)), self.w_down)
+    def __call__(self, x: torch.Tensor, lora=None) -> torch.Tensor:
+        if lora is None:
+            return quantized_linear(swiglu(quantized_linear(x, self.w_gate), quantized_linear(x, self.w_up)), self.w_down)
+        sites, row_ids = lora
+        gate, up = quantized_linear(x, self.w_gate), quantized_linear(x, self.w_up)
+        if sites.gate_up is not None:
+            ext.lora_apply(x, [gate, up], row_ids, sites.gate_up)
+        act = swiglu(gate, up)
+        out = quantized_linear(act, self.w_down)
+        if sites.down is not None:
+            ext.lora_apply(act, out, row_ids, sites.down)
+        return out
 
 
 class Qwen3TransformerBlock:
@@ -156,9 +176,12 @@ class Qwen3TransformerBlock:
             use_paged_attention=use_paged_attention,
         )
 
-    def __call__(self, x, offset, cache: TinyKvCache, mask=None):
-        h = residual_add(x, self.self_attn(self.input_layernorm(x), offset, cache, mask))
-        return residual_add(h, self.mlp(self.post_attention_layernorm(h)))
+    def __call__(self, x, offset, cache: TinyKvCache, mask=None, lora=None):
+        if lora is None:
+            h = residual_add(x, self.self_attn(self.input_layernorm(x), offset, cache, mask))
+            return residual_add(h, self.mlp(self.post_attention_layernorm(h)))
+        h = residual_add(x, self.self_attn(self.input_layernorm(x), offset, cache, mask, lora=lora))
+        return residual_add(h, self.mlp(self.post_attention_layernorm(h), lora=lora))
 
 
 def is_qwen3_moe_sparse_layer(args: Any, layer_idx: int) -> bool:
@@ -253,6 +276,7 @@ class Qwen3ModelWeek3:
         self._packed_layers: list | None = None
         self._paged = enable_paged_attention
         self.prefix_cache = None  # prefix_cache.PrefixCache over page_pools, once enable_prefix_cache() is called
+        self.adapters = None  # lora.AdapterSet, once load_adapters() is called
 
     def create_kv_cache(self) -> list[TinyKvCache]:
         """One logical cache per layer, all sharing that layer's pool."""
@@ -266,6 +290,36 @@ class Qwen3ModelWeek3:
 
             self.prefix_cache = PrefixCache(self.page_pools)
         return self.prefix_cache
+
+    def load_adapters(self, adapters):
+        """Pack ``adapters`` (``lora.LoraAdapter``s) for this model and return the ``lora.AdapterSet``.  From then on a
+        call may name one adapter per batch row (``adapter_ids``), and the graph engines this model builds are the LoRA
+        engines (``engine.py``).  Once, and before any engine exists: captured graphs do not change their launches."""
+        from .lora import AdapterSet
+
+        if self.adapters is not None:
+            raise RuntimeError("load_adapters: this model already has its adapter set (adapters cannot be swapped after loading)")
+        if self._decode_engines or self._prefill_engines or self._verify_engines:
+            raise RuntimeError("load_adapters: call it before the first decode or prefill graph engine exists")
+        if any(isinstance(b.mlp, Moe) for b in self.layers_inner):
+            raise ValueError("load_adapters: adapters on Qwen3-MoE models are not supported")
+        self.adapters = AdapterSet(self.mlx_model.args, adapters, self.embedding.weight.scales.device)
+        return self.adapters
+
+    def _adapter_rows(self, adapter_ids, B: int):
+        """``adapter_ids`` of a call as a list of ``B`` ids, or None when every row runs the base model."""
+        if adapter_ids is None:
+            return None
+        ids = [int(i) for i in adapter_ids]
+        if len(ids) != B:
+            raise ValueError(f"adapter_ids must hold one id per batch row ({B})")
+        if all(i < 0 for i in ids):
+            return None
+        if self.adapters is None:
+            raise ValueError("adapter_ids name an adapter but the model has none loaded (load_adapters)")
+        if any(i >= len(self.adapters.names) for i in ids):
+            raise ValueError(f"adapter_ids {ids} exceed the {len(self.adapters.names)} loaded adapters")
+        return ids
 
     # ---- CUDA-graph decode path ------------------------------------------------
     def packed_layers(self) -> list:
@@ -296,7 +350,7 @@ class Qwen3ModelWeek3:
 
         dev = device if device is not None else self.embedding.weight.scales.device
         return (self._paged and self.use_decode_graph is not False and torch.device(dev).type == "cuda"
-                and VerifyEngine.supported(self, dev, self.decode_graph_max_seq_len))
+                and VerifyEngine.supported(self, dev, self.decode_graph_max_seq_len))  # False with adapters loaded
 
     def verify_engine(self, rows: int, device=None):
         """The (cached) graph of one speculative verify pass over ``rows`` tokens of one request (``engine.VerifyEngine``).
@@ -366,7 +420,7 @@ class Qwen3ModelWeek3:
             limit = min(limit, pages * self.page_size)
         return limit
 
-    def _graph_decode(self, inputs, offset, cache, logits_to_keep):
+    def _graph_decode(self, inputs, offset, cache, logits_to_keep, adapter_ids=None):
         from .kv_cache import BatchingKvCache
 
         if logits_to_keep is not None and logits_to_keep <= 0:
@@ -386,7 +440,7 @@ class Qwen3ModelWeek3:
             if first.max_seq_len is not None and any(s is not None and s.logical_offset() + 1 > first.max_seq_len for s in first.kv_caches):
                 raise ValueError("Paged batch append exceeds max_seq_len")
         engine = self.decode_engine(B, self._graph_limit(cache))
-        logits, _ = engine.step(inputs, offsets, cache)
+        logits, _ = engine.step(inputs, offsets, cache) if self.adapters is None else engine.step(inputs, offsets, cache, adapter_ids=adapter_ids)
         attn = self.layers_inner[0].self_attn
         for entry in cache:
             if isinstance(entry, BatchingKvCache):
@@ -404,7 +458,7 @@ class Qwen3ModelWeek3:
             self._prefill_engines[key] = PrefillEngine(self, chunk, limit, dev)
         return self._prefill_engines[key]
 
-    def _graph_prefill(self, inputs, offset, cache, logits_to_keep):
+    def _graph_prefill(self, inputs, offset, cache, logits_to_keep, adapter_id: int = -1):
         """Route a B == 1 prefill chunk through the captured chunk graph when it applies; None otherwise."""
         from .engine import PrefillEngine
 
@@ -431,19 +485,26 @@ class Qwen3ModelWeek3:
         engine = self.prefill_engine(chunk)
         if not engine.applies(L, off, cache):
             return None
-        logits, _ = engine.prefill_chunk(inputs.reshape(-1), off, cache)
+        logits, _ = engine.prefill_chunk(inputs.reshape(-1), off, cache) if self.adapters is None else \
+            engine.prefill_chunk(inputs.reshape(-1), off, cache, adapter_id=adapter_id)
         return logits.clone()
 
-    def __call__(self, inputs, offset, cache: list[TinyKvCache], logits_to_keep: int | None = None):
+    def __call__(self, inputs, offset, cache: list[TinyKvCache], logits_to_keep: int | None = None, adapter_ids=None):
+        """``adapter_ids``: one ``AdapterSet`` id per batch row (-1: the base model), after ``load_adapters``."""
+        ids = self._adapter_rows(adapter_ids, inputs.shape[0])
         if self._graph_decode_applies(inputs, cache):
-            return self._graph_decode(inputs, offset, cache, logits_to_keep)
+            return self._graph_decode(inputs, offset, cache, logits_to_keep, ids)
         if inputs.dim() == 2 and inputs.shape[1] > 1 and inputs.is_cuda:
-            out = self._graph_prefill(inputs, offset, cache, logits_to_keep)
+            out = self._graph_prefill(inputs, offset, cache, logits_to_keep, -1 if ids is None else ids[0])
             if out is not None:
                 return out
         h = self.embedding(inputs)
-        for block, layer_cache in zip(self.layers_inner, cache):
-            h = block(h, offset, layer_cache, mask="causal")
+        row_ids = None if ids is None else self.adapters.row_ids(ids, inputs.shape[1])
+        for index, (block, layer_cache) in enumerate(zip(self.layers_inner, cache)):
+            if row_ids is None:
+                h = block(h, offset, layer_cache, mask="causal")
+            else:
+                h = block(h, offset, layer_cache, mask="causal", lora=(self.adapters.sites[index], row_ids))
         if logits_to_keep is not None:
             if logits_to_keep <= 0:
                 raise ValueError("logits_to_keep must be positive")
