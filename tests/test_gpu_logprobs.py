@@ -167,6 +167,30 @@ def test_every_output_against_the_float64_reference(cuda_device, V, dtype):
     assert torch.equal(lse0, lse)
 
 
+# one per cluster size C = 1..8 of sample_plan (which tl_logprobs shares), the 151,936 vocabulary and the 409,600 limit
+SWEEP = [1, 7, 4096, 4097, 8193, 12289, 16385, 20481, 24577, 28673, 151936, 409600]
+
+
+@pytest.mark.parametrize("V", SWEEP)
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+def test_cluster_size_sweep(cuda_device, V, dtype):
+    g = torch.Generator().manual_seed(V + 1)
+    if V >= 64:
+        logits, targets = rows_for(V, dtype, g)
+    else:  # too short for the planted rows: random, peaked, tied, and special rows with every target
+        rows = [torch.randn(V, generator=g) * s for s in (1.0, 8.0)] + [torch.zeros(V), torch.full((V,), -math.inf)]
+        if V > 1:
+            special = torch.randn(V, generator=g)
+            special[0], special[V - 1] = math.nan, special.max() + 3
+            rows.append(special)
+        logits = torch.stack(rows).to(dtype)
+        targets = [(r * 3) % V for r in range(len(rows))]
+    R = logits.shape[0]
+    top_n = [(MAX_N, 5, 1, 0, 20, 3)[r % 6] for r in range(R)]
+    worst = check(logits.to(cuda_device), targets, top_n)
+    print(f"V {V} {dtype}: {R} rows, largest lse error {worst:.3f} of its bound")
+
+
 @pytest.mark.parametrize("V", [1000, 151936])
 def test_exact_probes_power_of_two_maxima(cuda_device, V):
     rows = []

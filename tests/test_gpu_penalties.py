@@ -72,7 +72,8 @@ def _tol_accept(x3, T, k, p, mp, seed, pos, got):
         loose &= M < p + eps
     g = ref.gumbel(V, seed, pos)
     score = x / T + g
-    d = 2.0**-21 * (1 + np.abs(g) + np.abs(x / T))
+    m = x[ok].max()
+    d = 2.0**-21 * (1 + np.abs(g) + (np.abs(x) + abs(m)) / T)  # the kernel scores (x - m) / T + g
     if not loose[got]:
         return False
     if not strict.any():

@@ -60,8 +60,8 @@ def test_greedy_rows_equal_argmax(cuda_device, V, dtype):
 
 def _tol_accept(x, T, k, p, seed, pos, got):
     """A draw that differs from the float64 reference passes only when the fp32 operation chain of the kernel could
-    have produced it: (a) the perturbed scores x_i / T + g_i are rounded at x / T, at each logf and at the sum, so each is
-    within d_i = 2^-21 (1 + |g_i| + |x_i / T|) of the float64 value; (b) the mass above an entry is a quotient of sums
+    have produced it: (a) the perturbed scores (x_i - m) / T + g_i are rounded at x - m, at the quotient, at each logf and
+    at the sum, so each is within d_i = 2^-21 (1 + |g_i| + (|x_i| + |m|) / T) of the float64 value less m / T; (b) the mass above an entry is a quotient of sums
     of e_j = expf(x_j - m) (error <= 2^-22 + |x_j - m| 2^-24 relative) in 2^-40 fixed point, so M_i is within
     eps = 2 (2^-22 + R 2^-24) + 2 V 2^-40 / S of its float64 value (R: the row's finite range).  The kernel's token must
     be in the loose keep set (top_p + eps) and its score within d_got + d_best of the best score of the strict keep set
@@ -78,7 +78,8 @@ def _tol_accept(x, T, k, p, seed, pos, got):
         loose &= M < p + eps
     g = ref.gumbel(V, seed, pos)
     score = x / T + g
-    d = 2.0**-21 * (1 + np.abs(g) + np.abs(x / T))
+    m = x[ok].max()
+    d = 2.0**-21 * (1 + np.abs(g) + (np.abs(x) + abs(m)) / T)  # the kernel scores (x - m) / T + g
     if not loose[got]:
         return False
     if not strict.any():

@@ -10,7 +10,8 @@
 //   2. S = sum over non-NaN i of round(expf(fl(x_i - m)) * 2^40), 64-bit integers (exact in any order), and the rank
 //      count #{i : x_i > x_t}.  lp(x) = fl(fl(x - m) - logf(fl(S) * 2^-40)), lse = fl(m + logf(...)).
 //   3. (rows with top_n > 0) radix select of the N-th largest order key on count histograms, 2 levels for bf16 and 4
-//      for fp16 / fp32; when the equal keys at the N-th place are more than the list has room for, 3 more levels
+//      for fp16 / fp32 (the raw values are read, never a penalised row, so a bf16 key keeps its 16 significant bits and
+//      two levels are exact; tl_sample's penalised form needs four); when the equal keys at the N-th place are more than the list has room for, 3 more levels
 //      select the lowest ids among them (keys ~id, 24 bits).  The N chosen entries are gathered by CTA 0 and ordered
 //      by (value descending, id ascending).
 #include <cooperative_groups.h>

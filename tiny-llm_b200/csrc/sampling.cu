@@ -8,13 +8,16 @@
 //
 //   1. load the slice, fp32; the first-maximum-wins argmax of the raw values (tl_argmax's rules) gives the row
 //      maximum m.  Greedy rows (temperature == 0) and rows whose maximum is not finite return that argmax.
-//   2. keep set {x >= tau}: the logits map to order-preserving 32-bit keys; each radix level (2 for bf16, 4 for
-//      fp16 / fp32) is one pass that adds a count and a mass e_i = exp(x_i - m) per 256-entry bin, for the elements
+//   2. keep set {x >= tau}: the logits map to order-preserving 32-bit keys; each radix level (2 for raw bf16 rows, 4
+//      once a penalty can move a value off the bf16 grid, 4 for fp16 / fp32) is one pass that adds a count and a mass e_i = exp(x_i - m) per 256-entry bin, for the elements
 //      that share the prefix chosen so far.  Masses are 2^-40 fixed point in 64 bits, so their sums are exact in any
 //      order.  Counts locate x_(k) and masses locate v* (the smallest value whose mass strictly above is < top_p * S)
 //      in the same pass; where the two searches pick different bins the higher one is tau's and the other search ends.
-//   3. one Gumbel pass: argmax over the kept i of x_i / T + g_i, g_i = -log(-log u_i), u_i from Philox4x32-10 at
-//      counter (i >> 2, pos, 0, 0) and key (seed lo, seed hi); then the cluster argmax.
+//      Top-k with k above the non-NaN count is off, and with top-p off too every non-NaN entry is kept.
+//   3. one Gumbel pass: argmax over the kept i of (x_i - m) / T + g_i, g_i = -log(-log u_i), u_i from Philox4x32-10 at
+//      counter (i >> 2, pos, 0, 0) and key (seed lo, seed hi); then the cluster argmax.  The maximum's term is exactly
+//      0, so a temperature near the bottom of fp32 sends the others to -inf instead of every kept term to +-inf: the
+//      draw is x_i / T + g_i's in exact arithmetic.
 // Integer sums and first-maximum-wins merges make every launch give the same bits, whatever the row count.
 //
 // The penalised form (PEN, tl_sample_penalized, DESIGN.md section 8b) reads the row's int32 token state (bit 30: in
@@ -305,9 +308,10 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
             if (lane == 0) {
                 const int kbin = k_on ? s_bk : -1, pbin = p_on ? s_bp : -1;
                 const int bin = max(kbin, pbin);  // tau = max(x_(k), v*): the higher bin holds it
-                s_k_on = kbin == bin;
-                s_p_on = pbin == bin;
-                s_prefix = prefix | (static_cast<uint32_t>(bin) << shift);
+                // bin < 0: level 0 turned top-k off and top-p is off, so tau stays 0 and every non-NaN entry is kept
+                s_k_on = bin >= 0 && kbin == bin;
+                s_p_on = bin >= 0 && pbin == bin;
+                if (bin >= 0) s_prefix = prefix | (static_cast<uint32_t>(bin) << shift);
                 s_count_above = s_k_on ? s_bk_above : 0;
                 s_mass_above = s_p_on ? s_bp_above : 0;
             }
@@ -341,7 +345,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
         const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-            if (x[j] == x[j] && order_key(x[j]) >= tau) mine = better(mine, Best{__fdiv_rn(x[j], temp) + gumbel(ws[j]), begin + g + j});
+            if (x[j] == x[j] && order_key(x[j]) >= tau)
+                mine = better(mine, Best{__fdiv_rn(__fsub_rn(x[j], m), temp) + gumbel(ws[j]), begin + g + j});
     }
     mine = warp_best(mine);
     if (lane == 0) w_v[warp] = mine.v, w_i[warp] = mine.i;
@@ -414,8 +419,10 @@ int launch_sample_any(const void *logits, const float *temperature, const int32_
         case TL_F16:
             return launch_sample_t<__half, 4, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
                                                          vec, pen, con, st);
-        case TL_BF16:  // a bf16 value's key has 16 significant bits: two levels
-            return launch_sample_t<__nv_bfloat16, 2, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
+        case TL_BF16:  // a raw bf16 value's key has 16 significant bits: two levels.  A penalty rewrites the staged values
+                       // (x / r, x * r, x - f c, x - pres) into arbitrary fp32 values: four levels, or tau would stop
+                       // at a 16-bit prefix and keep every entry of its bucket below x_(k) or v*
+            return launch_sample_t<__nv_bfloat16, PEN ? 4 : 2, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
                                                                  slice, vec, pen, con, st);
         default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
     }

@@ -7,7 +7,7 @@
 * ``decode_on_device`` tok/s, greedy against sampled (temperature 0.7, top-p 0.9, top-k 50) and sampled with those
   penalties, at B = 1 and B = 64 on Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
 
-  python tools/sample_bench.py [--out tools_out/sample_bench.json]
+  python tools/sample_bench.py [--out tools_out/sample_bench.json] [--kernels-only]
 """
 from __future__ import annotations
 
@@ -118,12 +118,16 @@ def decode_rates(model, B, ctx=128, steps=64, rounds=3) -> dict:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
+    ap.add_argument("--kernels-only", action="store_true", help="the per-call kernel table alone, no decode run")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("sample_bench needs a CUDA device")
     result = {"card": card()}
     print(f"card: {result['card']}", flush=True)
     result["kernels_us"] = kernel_table()
+    if args.kernels_only:
+        print(json.dumps(result))
+        return
     ns = synthetic_qwen3("qwen3-4b", seed=0, device=DEV)
     model = Qwen3ModelWeek3(ns, page_size=64)
     result["decode"] = {B: decode_rates(model, B) for B in (1, 64)}
