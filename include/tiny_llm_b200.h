@@ -422,7 +422,9 @@ int tl_decode_attention_fused_rows(const void *qkv, const void *q_norm_weight, c
  * A row's result depends only on that row. */
 #define TL_MOE_MAX_EXPERTS 256
 #define TL_MOE_MAX_TOPK 8
-/* logits [T, E] -> probs [T, E] (dtype of logits), ids int32 [T, k], scores [T, k].  E <= 256, 1 <= k <= min(8, E). */
+/* logits [T, E] -> probs [T, E] (dtype of logits), ids int32 [T, k], scores [T, k].  E <= 256, 1 <= k <= min(8, E).
+ * A NaN probability ranks below every number: a row whose softmax is NaN (a NaN or +inf logit, every logit -inf) gives
+ * ids 0..k-1 and NaN scores. */
 int tl_moe_topk(const void *logits, void *probs, int32_t *ids, void *scores, int T, int E, int k, int norm_topk_prob, int dtype, void *stream);
 /* ids int32 [R] (each in [0, E); others are clamped) -> offsets int32 [E + 1] (segment of expert e in sorted order),
  * perm int32 [R] (sorted position -> row, stable within an expert) and, with nt > 0, the tile table of the grouped

@@ -152,6 +152,23 @@ def test_reference_moe_model_runs_a_dense_and_a_sparse_layer():
     assert len(out) == 3 and all(0 <= t < 512 for t in out)
 
 
+@pytest.mark.parametrize("H, I", [(128, 136), (128, 64), (200, 128), (136, 256)])
+def test_moe_refuses_widths_the_grouped_projections_cannot_take(H, I):
+    """Both grouped projections reduce over whole 128-wide quantisation groups: H (gate|up) and I (down)."""
+    g = torch.Generator().manual_seed(0)
+
+    def experts(E, out_dim, in_dim):
+        words = torch.randint(-(2**31), 2**31, (E, out_dim, in_dim // 8), generator=g, dtype=torch.int64).to(torch.int32)
+        groups = max(1, in_dim // 128)
+        return QuantizedWeights(scales=torch.ones(E, out_dim, groups, dtype=torch.bfloat16), biases=torch.zeros(E, out_dim, groups, dtype=torch.bfloat16),
+                                group_size=128, bits=4, weight=words)
+
+    router = experts(1, 4, H)
+    router = QuantizedWeights(scales=router.scales[0], biases=router.biases[0], group_size=128, bits=4, weight=router.weight[0])
+    with pytest.raises(ValueError, match="multiples of 128"):
+        Moe(router, experts(4, I, H), experts(4, I, H), experts(4, H, I), num_experts_per_tok=2)
+
+
 def test_week3_model_builds_moe_layers_on_the_stand_ins(moe_ext):
     from tiny_llm_b200 import Qwen3ModelWeek3
 

@@ -50,7 +50,9 @@ __global__ void __launch_bounds__(256) moe_topk_kernel(const T *__restrict__ log
         if (e < E) {
             const T p = from_f<T>(v[i] / s);
             probs[static_cast<size_t>(row) * E + e] = p;
-            v[i] = to_f(p);
+            // A NaN softmax (a NaN or +inf logit, or every logit -inf) fails every comparison below; as -0.5 it ranks
+            // under every probability and over the picked and padding entries (-1), so the row still names k experts.
+            v[i] = isnan(to_f(p)) ? -0.5f : to_f(p);
         } else {
             v[i] = -1.f;
         }
@@ -76,7 +78,7 @@ __global__ void __launch_bounds__(256) moe_topk_kernel(const T *__restrict__ log
 #pragma unroll
         for (int i = 0; i < MOE_PER_LANE; ++i)
             if (lane + 32 * i == best_e) v[i] = -1.f;
-        picked[j] = best;
+        picked[j] = best >= 0.f ? best : __int_as_float(0x7fffffff);  // a NaN row's scores stay NaN
         picked_id[j] = best_e;
         total += best;  // slot order
     }
@@ -313,7 +315,8 @@ __global__ void __launch_bounds__(256) moe_combine_kernel(const T *__restrict__ 
                 float acc = 0.f;
 #pragma unroll
                 for (int j = 0; j < TL_MOE_MAX_TOPK; ++j)  // slot order; a fixed trip count keeps sc[] in registers
-                    if (j < k) acc += to_f(from_f<T>(to_f(ld_cg(yr + static_cast<size_t>(j) * H + i)) * sc[j]));
+                    // __fmul_rn: the product is rounded before the sum for fp32 too (not contracted into an fma)
+                    if (j < k) acc += to_f(from_f<T>(__fmul_rn(to_f(ld_cg(yr + static_cast<size_t>(j) * H + i)), sc[j])));
                 T v = from_f<T>(acc);
                 if (residual != nullptr) v = from_f<T>(to_f(ld_cg(residual + static_cast<size_t>(t) * H + i)) + to_f(v));
                 orow[i] = v;

@@ -90,8 +90,9 @@ class Moe:
         E, inter, hidden = _experts(w_gate, "Moe")
         if _experts(w_up, "Moe") != (E, inter, hidden) or _experts(w_down, "Moe") != (E, hidden, inter):
             raise ValueError("Moe: gate / up must be [E, I, H] and down [E, H, I] experts")
-        if inter % 8:
-            raise ValueError("Moe: the experts' intermediate size must be a multiple of 8")
+        if inter % 128 or hidden % 128:
+            # each is the reduction width of one grouped projection, which takes whole 128-wide quantisation groups
+            raise ValueError(f"Moe: the hidden size ({hidden}) and the experts' intermediate size ({inter}) must be multiples of 128")
         self.num_experts, self.intermediate_size, self.hidden_size = E, inter, hidden
 
         def pairs(g: torch.Tensor, u: torch.Tensor) -> torch.Tensor:
