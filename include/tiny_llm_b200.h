@@ -211,6 +211,30 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
 int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                         const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                         const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* Speculative sampling (DESIGN.md section 8d): the rejection rule over one verify pass of T = k + 1 rows
+ * (1 <= T <= 65535, vocab <= TL_SPECULATIVE_SAMPLE_MAX_VOCAB).  target [T, vocab] are the target's logits rows,
+ * draft [k, vocab] the draft's rows each proposal proposals[j] (int32, device) was drawn from, the parameters per row
+ * as tl_sample takes them (all T rows normally carry one request's values) and positions[j] = n_j, the index of the
+ * token row j predicts.  Every device input is read after the programmatic-dependent-launch wait.
+ * Row distributions: temperature 0, or a row whose maximum is not finite, is the point mass at the row's tl_argmax
+ * token; otherwise p_i = exp((x_i - m) / T) / sum over K of the same, K = tl_sample's keep set of x (top-k, top-p),
+ * and 0 outside K; q likewise from the draft row.  q is the distribution tl_sample drew d_j from.
+ * Row j < k accepts iff q_d > 0 and u q_d <= p_d, u = (2 (w >> 9) + 1) 2^-24, w word 0 of Philox4x32-10 at counter
+ * (0, n_j, 1, 0) under the seed key; then out[j] = d_j.  Otherwise out[j] = argmax over {i : p_i > q_i} of
+ * log(p_i - q_i) + g_i, g_i = -log(-log u_i) with u_i from word i % 4 at counter (i >> 2, n_j, 2, 0).  If rounding
+ * left that set empty the row returns the tl_argmax token of x (the kernel compares exact integer masses, so a
+ * rejection always leaves it non-empty).  Row k (the bonus row) is tl_sample's draw on target row k at n_k, bit for
+ * bit.  Counter word 2 is the stream: 0 the ordinary draw (the draft's, the bonus row's), 1 the acceptance uniform,
+ * 2 the residual noise.  The emitted token at n_j is distributed as the target's tl_sample draw; with temperature 0
+ * it is greedy verification; a rejected proposal with q_d > 0 is never the residual.  The kernel sums masses as
+ * 2^-40 fixed-point integers and compares p and q exactly on them: deterministic whatever T or the row index. */
+#define TL_SPECULATIVE_SAMPLE_MAX_VOCAB 204800
+int tl_speculative_sample(const void *target, const void *draft, const int32_t *proposals, const float *temperature,
+                          const int32_t *top_k, const float *top_p, const int64_t *seed, const int32_t *positions,
+                          int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* Copy `bytes` from src to dst + out_index[0] * bytes when 0 <= out_index[0] < capacity (device index; nothing
+ * otherwise): a captured decode step logs its logits rows at the step counter, as tl_logprobs logs. */
+int tl_log_rows(const void *src, void *dst, const int32_t *out_index, int capacity, long long bytes, void *stream);
 /* Regex-constrained sampling (DESIGN.md section 8c).  One descriptor per row, in device memory (40 bytes):
  *   mask           uint32 [num_states + 1, ceil(vocab / 32)]: bit t of row s set iff token t is allowed in state s;
  *                  NULL: the row is unconstrained and draws exactly as tl_sample / tl_sample_penalized;

@@ -35,6 +35,7 @@ SOURCES = [
     "attention_prefill_tc.cu",
     "decode_attention_fused.cu",
     "sampling.cu",
+    "spec_sample.cu",
     "logprobs.cu",
     "constrained.cu",
     "moe.cu",

@@ -414,6 +414,26 @@ int tl_sample_constrained(const void *logits, const float *temperature, const in
                                      constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
+int tl_speculative_sample(const void *target, const void *draft, const int32_t *proposals, const float *temperature,
+                          const int32_t *top_k, const float *top_p, const int64_t *seed, const int32_t *positions, int32_t *out_tokens,
+                          int rows, int vocab, int dtype, void *stream) {
+    if (!float_dtype(dtype)) return fail(TL_EDTYPE, "speculative_sample: expected float32, float16, or bfloat16");
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "speculative_sample: bad shape");
+    if (int e = speculative_sample_plan(vocab, nullptr, nullptr)) return e;
+    if (rows == 0) return TL_OK;
+    if (!target || !temperature || !top_k || !top_p || !seed || !positions || !out_tokens || (rows > 1 && (!draft || !proposals)))
+        return fail(TL_EINVAL, "speculative_sample: null pointer");
+    return launch_speculative_sample(target, draft, proposals, temperature, top_k, top_p, seed, positions, out_tokens, rows, vocab, dtype,
+                                     as_stream(stream));
+}
+
+int tl_log_rows(const void *src, void *dst, const int32_t *out_index, int capacity, long long bytes, void *stream) {
+    if (capacity < 0 || bytes < 0) return fail(TL_EINVAL, "log_rows: bad shape");
+    if (bytes == 0 || capacity == 0) return TL_OK;
+    if (!src || !dst || !out_index) return fail(TL_EINVAL, "log_rows: null pointer");
+    return launch_log_rows(src, dst, out_index, capacity, bytes, as_stream(stream));
+}
+
 int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                               const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks, uint32_t *reach,
                               void *stream) {

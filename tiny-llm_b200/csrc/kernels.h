@@ -57,6 +57,13 @@ int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *t
                     int32_t *rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
                     cudaStream_t st);
 
+// spec_sample.cu: tl_sample's cluster plan with both rows staged
+int speculative_sample_plan(int vocab, int *cluster, int *slice);
+int launch_speculative_sample(const void *target, const void *draft, const int32_t *proposals, const float *temperature,
+                              const int32_t *top_k, const float *top_p, const int64_t *seed, const int32_t *positions, int32_t *out,
+                              int rows, int vocab, int dtype, cudaStream_t st);
+int launch_log_rows(const void *src, void *dst, const int32_t *out_index, int capacity, long long bytes, cudaStream_t st);
+
 int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                           int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, cudaStream_t st);
 

@@ -46,6 +46,9 @@ __all__ = [
     "sample",
     "sample_penalized",
     "sample_constrained",
+    "speculative_sample",
+    "SPECULATIVE_SAMPLE_MAX_VOCAB",
+    "log_rows",
     "constraint_token_masks",
     "logprobs",
     "LOGPROBS_MAX_N",
@@ -108,6 +111,8 @@ _SIGNATURES = {
     "tl_argmax": (_I, [_VP, _VP, _I, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_advance": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
+    "tl_speculative_sample": (_I, [_VP] * 9 + [_I] * 3 + [_VP]),
+    "tl_log_rows": (_I, [_VP] * 3 + [_I, _LL, _VP]),
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
@@ -737,6 +742,57 @@ def sample(logits, temperature, top_k, top_p, seed, positions, stream=None):
     _check(_lib.tl_sample(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(), positions.data_ptr(),
                           out.data_ptr(), rows, logits.shape[1], _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
+
+
+SPECULATIVE_SAMPLE_MAX_VOCAB = 204800
+
+
+def speculative_sample(target, draft, proposals, temperature, top_k, top_p, seed, positions, out=None, stream=None):
+    """The speculative rejection rule over one verify pass (``tl_speculative_sample``, DESIGN.md section 8d) -> int32
+    ``[T]``.  ``target [T, vocab]`` and ``draft [T - 1, vocab]`` logits of one float dtype, ``proposals`` int32
+    ``[T - 1]`` (each drawn by ``sample`` from its draft row with the same parameters), per-row device arrays as
+    ``sample`` takes them and ``positions`` the index n_j of the token row j predicts.  Row j < T - 1 is d_j when
+    accepted, else the residual draw; row T - 1 is ``sample``'s draw on the last target row.  ``out`` (int32 ``[T]``)
+    receives the tokens when given.  vocab is at most ``SPECULATIVE_SAMPLE_MAX_VOCAB``."""
+    if target.dtype not in _FLOATS or target.dim() != 2:
+        raise RuntimeError("speculative_sample: expected 2D float target logits")
+    rows, vocab = target.shape
+    if vocab > SPECULATIVE_SAMPLE_MAX_VOCAB:
+        raise RuntimeError(f"speculative_sample: vocab {vocab} exceeds {SPECULATIVE_SAMPLE_MAX_VOCAB}")
+    k = rows - 1
+    if draft.dtype != target.dtype or tuple(draft.shape) != (k, vocab):
+        raise RuntimeError(f"speculative_sample: draft must be {str(target.dtype).replace('torch.', '')} [{k}, {vocab}]")
+    if proposals.dtype != torch.int32 or tuple(proposals.shape) != (k,):
+        raise RuntimeError(f"speculative_sample: proposals must be int32 [{k}]")
+    for name, t, dtype in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+                           ("seed", seed, torch.int64), ("positions", positions, torch.int32)):
+        if t.dtype != dtype or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"speculative_sample: {name} must be {str(dtype).replace('torch.', '')} [{rows}]")
+    if out is None:
+        out = torch.empty((rows,), dtype=torch.int32, device=target.device)
+    elif out.dtype != torch.int32 or tuple(out.shape) != (rows,):
+        raise RuntimeError(f"speculative_sample: out must be int32 [{rows}]")
+    named = dict(target=target, draft=draft, proposals=proposals, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                 positions=positions, out=out)
+    _contig("speculative_sample", **named)
+    _gpu("speculative_sample", *named.values())
+    _check(_lib.tl_speculative_sample(target.data_ptr(), draft.data_ptr(), proposals.data_ptr(), temperature.data_ptr(), top_k.data_ptr(),
+                                      top_p.data_ptr(), seed.data_ptr(), positions.data_ptr(), out.data_ptr(), rows, vocab,
+                                      _DTYPE_CODE[target.dtype], _stream_ptr(stream, target)))
+    return out
+
+
+def log_rows(src, dst, out_index, stream=None):
+    """``dst[out_index[0]] = src`` when ``0 <= out_index[0] < dst.shape[0]`` (``tl_log_rows``; ``out_index`` int32 ``[1]``
+    on the device): a captured step logs its rows at the step counter."""
+    if src.dtype != dst.dtype or dst.dim() < 1 or tuple(dst.shape[1:]) != tuple(src.shape):
+        raise RuntimeError("log_rows: dst must be [capacity, *src.shape] of src's dtype")
+    if out_index.dtype != torch.int32 or out_index.numel() != 1:
+        raise RuntimeError("log_rows: out_index must be int32 [1]")
+    _contig("log_rows", src=src, dst=dst, out_index=out_index)
+    _gpu("log_rows", src, dst, out_index)
+    _check(_lib.tl_log_rows(src.data_ptr(), dst.data_ptr(), out_index.data_ptr(), dst.shape[0], src.numel() * src.element_size(),
+                            _stream_ptr(stream, src)))
 
 
 def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None):

@@ -12,6 +12,8 @@ see checkpoint.py; there is no hub download here).
         (token-history penalties and min-p; with --sampler-temp 0 the greedy token of the penalised logits)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3 --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
+        (speculative sampling: the same ids as the seeded sampled run without the draft)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
         (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
     python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
@@ -166,7 +168,7 @@ def cmd_generate(args) -> int:
     if constraint is not None:
         penalties["constraint"] = constraint
     if args.sampler_temp != 0 or penalties:
-        if device.type == "cuda" or penalties:  # the seeded kernel
+        if device.type == "cuda" or penalties or args.draft_model or args.draft_synthetic:  # the seeded kernel
             sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed, **penalties)
         else:
             sampler = make_sampler(args.sampler_temp, top_p=args.sampler_top_p, top_k=args.sampler_top_k)
@@ -188,8 +190,9 @@ def cmd_generate(args) -> int:
 
         if args.adapter is not None or getattr(model, "adapters", None) is not None:
             raise SystemExit("speculative decoding does not take adapters: drop --lora / --synthetic-lora / --adapter")
-        if sampler is not None or sampling is not None:
-            raise SystemExit("speculative decoding is greedy: drop --sampler-temp")
+        if penalties:
+            raise SystemExit("speculative sampling takes --sampler-temp, --sampler-top-k, --sampler-top-p and --seed only: "
+                             "drop the penalties and --min-p")
         if args.logprobs is not None:
             raise SystemExit("speculative decoding does not report log-probabilities: drop --logprobs")
         if args.draft_model and args.draft_synthetic:
@@ -200,7 +203,8 @@ def cmd_generate(args) -> int:
             raise SystemExit("draft and target tokenizers use different token ids")
         draft = _model(args, draft_ns, draft_name)
         produced, stats = speculative_generate_ids(draft, model, ids, args.max_new_tokens, proposal_length=args.proposal_length,
-                                                   eos_token_ids=() if eos is None else (eos,), device=device, on_token=emit)
+                                                   eos_token_ids=() if eos is None else (eos,), device=device, on_token=emit,
+                                                   sampling=sampling)
         proposed, accepted = sum(p for p, _ in stats), sum(a for _, a in stats)
         print(f"\nspeculative: {len(stats)} rounds, {accepted}/{proposed} proposals accepted"
               + (f" ({accepted / proposed:.2f})" if proposed else ""), file=sys.stderr)

@@ -406,6 +406,13 @@ class DecodeEngine(_GraphEngine):
         # states the launches advance; all on first use
         self._graph_con: dict = {}
         self.kernels_per_constrained_step = 0
+        # decode_on_device(sampling=..., keep_logits=True): the sampled step plus one tl_log_rows launch that keeps the
+        # step's logits rows in a [capacity, B, V] log at the step counter (a speculative draft's q rows); on first use
+        self._graph_keep = None
+        self._logits_log = None
+        # VerifyEngine.verify(sampling=...): the verify pass with tl_speculative_sample as its token choice, one graph
+        # per draft-logits buffer it reads
+        self._graph_spec: dict = {}
         self._con_host = None
         self._con_dev = None
         self._con_key = None
@@ -427,10 +434,14 @@ class DecodeEngine(_GraphEngine):
         super().reserve_pools(pages_per_layer if pages_per_layer is not None else self.B * self.max_pages + 1)
 
     # ------------------------------------------------------------ graph body --
-    def _next_tokens(self, logits, R: int, sampled: bool, penalized: bool = False, constrained: bool = False) -> None:
+    def _next_tokens(self, logits, R: int, sampled: bool, penalized: bool = False, constrained: bool = False, spec_draft=None) -> None:
         """The step's token per row: ``tl_argmax``, or (the sampled graph) ``tl_sample`` with the per-slot parameters at
         position ``context_lens``, the index of the token being drawn, or (the penalised graph) ``tl_sample_penalized``
-        over ``token_counts``, or (a constrained graph) ``tl_sample_constrained`` over the slot descriptors."""
+        over ``token_counts``, or (a constrained graph) ``tl_sample_constrained`` over the slot descriptors, or (the
+        sampled verify graph, ``spec_draft`` the draft's logits rows) ``tl_speculative_sample`` on the proposals."""
+        if spec_draft is not None:
+            ext.speculative_sample(logits, spec_draft, self.tokens[1:R], *self._spec_params, self.context_lens[:R], out=self.next_tokens[:R])
+            return
         if constrained:
             pen = ()
             if penalized:
@@ -486,7 +497,8 @@ class DecodeEngine(_GraphEngine):
             self.logits = torch.empty_like(logits)
         self.logits.copy_(logits)
 
-    def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False, constrained: bool = False) -> None:
+    def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False, constrained: bool = False,
+                       spec_draft=None) -> None:
         """Same step in ~7 launches per layer: norm / SwiGLU / residual folded into
         the streaming projections, q/k norm + RoPE + K/V append in one kernel.
         Every rounding point of the operator-by-operator sequence is kept.
@@ -506,7 +518,7 @@ class DecodeEngine(_GraphEngine):
             x = self._matvec_layers(x)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
-        self._next_tokens(logits, R, sampled, penalized, constrained)
+        self._next_tokens(logits, R, sampled, penalized, constrained, spec_draft)
         if self.logits is None:
             self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
@@ -603,6 +615,8 @@ class DecodeEngine(_GraphEngine):
         self._graph_pen = None
         self._graph_lp = {}
         self._graph_con = {}
+        self._graph_keep = None
+        self._graph_spec = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -630,6 +644,28 @@ class DecodeEngine(_GraphEngine):
             self._set_idle()
             self._graph_sample = self._graph_of(sampled_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_sampled_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _ensure_keep_graph(self, steps: int) -> None:
+        """Capture the sampled self-advancing step that also logs its logits rows at ``step_counter`` (same conditions as
+        ``_ensure_sample_graph``).  The log holds at least 8 steps and grows, with a new capture, for longer calls."""
+        if self._logits_log is None or self._logits_log.shape[0] < steps:
+            self._logits_log = torch.zeros((max(8, steps), self.B, self.V), dtype=self.logits.dtype, device=self.device)
+            self._graph_keep = None
+        if self._graph_keep is not None:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def keep_step():
+            forward(sampled=True)
+            ext.log_rows(self.logits, self._logits_log, self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()
+            self._graph_keep = self._graph_of(keep_step, pool=self._graph.pool(), warmups=1)
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
     def _ensure_penalized_graph(self) -> None:
@@ -998,7 +1034,8 @@ class DecodeEngine(_GraphEngine):
         self.graph_replays += 1
         return self.logits.view(B, 1, self.V), self.next_tokens
 
-    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None, adapter_ids=None):
+    def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None, adapter_ids=None,
+                         keep_logits: bool = False):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
@@ -1015,9 +1052,18 @@ class DecodeEngine(_GraphEngine):
         slot descriptors, captured on first use per (penalised, logprobs); each launch advances the slots' automaton
         states.  ``history`` also sets a constrained slot's state to the walk of its generated ids; without it a slot
         keeps its state while its constraint stays the same and starts at the start state otherwise.
-        ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above."""
+        ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above.
+        ``keep_logits=True`` (plain ``sampling``: no penalty, constraint or logprobs) replays the sampled step with one
+        more launch that keeps each step's logits rows, and returns ``(tokens, logits [steps, B, V])``, a device view of
+        the engine's log (overwritten by the next call): the rows a speculative draft's proposals were drawn from."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
+        if keep_logits:
+            from .sampler import any_constrained, any_penalized
+
+            per = None if sampling is None else self._per_slot_sampling(sampling)
+            if per is None or logprobs is not None or any_penalized(per) or any_constrained(per):
+                raise ValueError("keep_logits takes plain sampling: no penalties, min-p, constraint or logprobs")
         B = self.B
         top_n = None
         if logprobs is not None:
@@ -1054,6 +1100,8 @@ class DecodeEngine(_GraphEngine):
             self._set_top_n(top_n)
         elif penalized:
             self._ensure_penalized_graph()
+        elif keep_logits:
+            self._ensure_keep_graph(steps)
         elif sampling is not None:
             self._ensure_sample_graph()
         if sampling is not None:
@@ -1071,6 +1119,8 @@ class DecodeEngine(_GraphEngine):
             graph = self._graph_lp[(sampling is not None, penalized)]
         elif penalized:
             graph = self._graph_pen
+        elif keep_logits:
+            graph = self._graph_keep
         else:
             graph = self._graph_loop if sampling is None else self._graph_sample
         cur = torch.cuda.current_stream(self.device)
@@ -1083,6 +1133,8 @@ class DecodeEngine(_GraphEngine):
         cur.wait_stream(self._stream)
         self.graph_replays += steps
         out = self.out_log[: steps * B].view(steps, B)
+        if keep_logits:
+            return out, self._logits_log[:steps]
         if top_n is None:
             return out
         _, lp, rank, ids, top = self._lp_log
@@ -1108,6 +1160,15 @@ class VerifyEngine(DecodeEngine):
         super().__init__(model, 1, max_seq_len, device, rows_per_request=rows)
         self.T = rows
         assert self.fused and self._attention_fused and self._variants == [1]
+        # verify(sampling=...): the request's parameters for all T rows (seed i64 | temperature f32 | top_k i32 | top_p
+        # f32, T each) in a pinned block, uploaded when they change
+        self._spec_host = torch.zeros(20 * rows, dtype=torch.uint8, pin_memory=True)
+        self._spec_dev = self._spec_host.to(self.device, copy=True)
+        self._spec_key = None
+        T = rows
+        self._spec_params = (self._spec_dev[8 * T : 12 * T].view(torch.float32), self._spec_dev[12 * T : 16 * T].view(torch.int32),
+                             self._spec_dev[16 * T : 20 * T].view(torch.float32), self._spec_dev[: 8 * T].view(torch.int64))
+        self.kernels_per_sampled_verify = 0
 
     @staticmethod
     def supported(model, device, max_seq_len: int) -> bool:
@@ -1125,14 +1186,57 @@ class VerifyEngine(DecodeEngine):
     def decode_on_device(self, tokens, offsets, caches, steps: int):
         raise TypeError("a verify engine runs verify(), not decode steps")
 
-    def verify(self, token: int, proposals, offset: int, caches):
+    def _ensure_spec_graph(self, draft) -> None:
+        """Capture the sampled verify pass over the draft-logits buffer ``draft`` (after ``_ensure_graph``, before the
+        metadata upload, as every capture)."""
+        key = (draft.data_ptr(), draft.dtype)
+        if key in self._graph_spec:
+            return
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self._graph_spec[key] = self._graph_of(lambda: self._forward_fused(spec_draft=draft), pool=self._graph.pool(), warmups=1)
+            self.kernels_per_sampled_verify = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_spec_params(self, sampling) -> None:
+        from .sampler import sampling_tensors
+
+        if sampling == self._spec_key:
+            return
+        T = self.T
+        self._host_write_begin()
+        temperature, top_k, top_p, seed = (t.numpy() for t in sampling_tensors([sampling] * T, "cpu"))
+        host = self._spec_host.numpy()
+        host[: 8 * T] = seed.view(np.uint8)
+        host[8 * T : 12 * T] = temperature.view(np.uint8)
+        host[12 * T : 16 * T] = top_k.view(np.uint8)
+        host[16 * T : 20 * T] = top_p.view(np.uint8)
+        self._upload_meta(self._spec_dev, self._spec_host)
+        self.h2d_bytes += 20 * T
+        self._spec_key = sampling
+
+    def verify(self, token: int, proposals, offset: int, caches, sampling=None, draft_logits=None):
         """Append ``[token, *proposals]`` (T ids at positions ``offset``..; ``proposals`` a list, or an int32 device tensor
         that never visits the host) to the request's caches and return (logits [T, V] static buffer, greedy next token
-        per row [T])."""
+        per row [T]).
+        ``sampling`` (a plain ``SamplingParams``: no penalty, min-p or constraint) with ``draft_logits`` (``[T - 1, V]``,
+        device, the rows the proposals were drawn from) replays the sampled verify graph instead: the second result is
+        then ``tl_speculative_sample``'s tokens, row j the proposal when accepted, else the residual draw, row T - 1 the
+        bonus draw.  The draft rows are read device to device; one graph is kept per draft buffer."""
         T = self.T
+        spec = sampling is not None
+        if spec:
+            if sampling.penalized or sampling.constraint is not None:
+                raise ValueError("the sampled verify pass takes plain sampling: no penalties, min-p or constraint")
+            if draft_logits is None or tuple(draft_logits.shape) != (T - 1, self.V) or not draft_logits.is_contiguous():
+                raise ValueError(f"the sampled verify pass needs the draft's contiguous logits rows [{T - 1}, {self.V}]")
         self._host_write_begin()
         self._advance_host(caches, T)
         self._ensure_graph()
+        if spec:
+            self._ensure_spec_graph(draft_logits)
+            self._set_spec_params(sampling)
         on_device = isinstance(proposals, torch.Tensor)
         self.meta_np[0] = token
         if not on_device:
@@ -1143,7 +1247,7 @@ class VerifyEngine(DecodeEngine):
         self._upload()
         if on_device:
             self.tokens[1:].copy_(proposals.reshape(-1).to(torch.int32), non_blocking=True)
-        self._graph.replay()
+        (self._graph_spec[(draft_logits.data_ptr(), draft_logits.dtype)] if spec else self._graph).replay()
         self.graph_replays += 1
         return self.logits, self.next_tokens
 

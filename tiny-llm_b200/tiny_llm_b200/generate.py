@@ -111,10 +111,15 @@ def simple_generate_with_kv_cache(model, tokenizer, prompt: str, max_new_tokens:
 
 
 class _GenericRunner:
-    """Every model action as a ``model(...)`` call, exactly as the reference issues them (any model, any device)."""
+    """Every model action as a ``model(...)`` call, exactly as the reference issues them (any model, any device).
+    With ``sampling`` (a plain ``SamplingParams``, temperature > 0) every token is ``tl_sample``'s draw at its position,
+    the draft keeps the logits row each proposal was drawn from, and ``verify`` returns ``tl_speculative_sample``'s
+    tokens on the target's T rows in place of the argmax predictions (DESIGN.md section 8d)."""
 
-    def __init__(self, model, draft_model, device):
+    def __init__(self, model, draft_model, device, sampling=None):
         self.model, self.draft_model, self.device = model, draft_model, device
+        self.sampling = sampling
+        self._draft_rows: list = []
 
     def round_fits(self, offset: int, k: int) -> bool:
         """Whether a round of ``k`` proposals at ``offset`` can run on this runner (``model(...)`` takes any length)."""
@@ -123,7 +128,12 @@ class _GenericRunner:
     def _step(self, model, ids, offset, cache, n_tokens=1):
         y = torch.as_tensor(ids, dtype=torch.int32, device=self.device)
         logits = model(y[None], offset, cache, logits_to_keep=n_tokens)
-        return [int(v) for v in greedy_tokens(logits[0, -n_tokens:, :]).reshape(-1).tolist()]
+        rows = logits[0, -n_tokens:, :]
+        if self.sampling is None:
+            return [int(v) for v in greedy_tokens(rows).reshape(-1).tolist()]
+        self._last_rows = rows
+        first = offset + len(ids) - n_tokens + 1  # the position of the token row 0 predicts
+        return [int(v) for v in sample_tokens(rows, [self.sampling] * n_tokens, range(first, first + n_tokens)).tolist()]
 
     def prefill(self, model, ids, cache) -> int:
         return self._step(model, ids, 0, cache)[0]
@@ -134,8 +144,11 @@ class _GenericRunner:
     def draft(self, token, offset, cache, k, eos) -> list[int]:
         """Up to ``k`` draft tokens after ``token``; stops after a draft EOS (reference ``_draft_generate``)."""
         out = []
+        self._draft_rows = []
         for _ in range(k):
             token = self._step(self.draft_model, [token], offset, cache)[0]
+            if self.sampling is not None:
+                self._draft_rows.append(self._last_rows)
             out.append(token)
             offset += 1
             if token in eos:
@@ -145,7 +158,20 @@ class _GenericRunner:
     def verify(self, token, proposals, offset, cache) -> tuple[list[int], list[int]]:
         """(target predictions for rows [token, *proposals], the proposals as host ids)."""
         ids = [token, *proposals]
-        return self._step(self.model, ids, offset, cache, len(ids)), list(proposals)
+        if self.sampling is None:
+            return self._step(self.model, ids, offset, cache, len(ids)), list(proposals)
+        from extensions_b200 import tiny_llm_ext_b200 as ext
+
+        from .sampler import sampling_tensors
+
+        T = len(ids)
+        y = torch.as_tensor(ids, dtype=torch.int32, device=self.device)
+        target = self.model(y[None], offset, cache, logits_to_keep=T)[0, -T:, :].contiguous()
+        draft = torch.cat(self._draft_rows[: T - 1]).to(target.dtype) if T > 1 else target[:0]
+        params = sampling_tensors([self.sampling] * T, target.device)
+        positions = torch.arange(offset + 1, offset + T + 1, dtype=torch.int32, device=target.device)
+        out = ext.speculative_sample(target, draft.contiguous(), y[1:].contiguous(), *params, positions)
+        return [int(v) for v in out.tolist()], list(proposals)
 
 
 class _GraphRunner(_GenericRunner):
@@ -164,11 +190,16 @@ class _GraphRunner(_GenericRunner):
 
     def draft(self, token, offset, cache, k, eos):
         engine = self.draft_model.decode_engine(1, self.draft_model.decode_graph_max_seq_len)
-        return engine.decode_on_device([token], [offset], cache, k).reshape(-1)
+        if self.sampling is None:
+            return engine.decode_on_device([token], [offset], cache, k).reshape(-1)
+        out, rows = engine.decode_on_device([token], [offset], cache, k, sampling=self.sampling, keep_logits=True)
+        self._draft_rows = rows.view(k, -1)  # the log's first k rows: a buffer whose address the verify graph keys on
+        return out.reshape(-1)
 
     def verify(self, token, proposals, offset, cache):
         k = int(proposals.numel())
-        _, nxt = self.model.verify_engine(k + 1).verify(token, proposals, offset, cache)
+        kw = {} if self.sampling is None else {"sampling": self.sampling, "draft_logits": self._draft_rows}
+        _, nxt = self.model.verify_engine(k + 1).verify(token, proposals, offset, cache, **kw)
         both = torch.cat([nxt, proposals.to(torch.int32)]).tolist()  # one device->host read per round
         return [int(v) for v in both[: k + 1]], [int(v) for v in both[k + 1 :]]
 
@@ -286,22 +317,43 @@ def _check_proposal_length(proposal_length) -> None:
         raise ValueError("proposal_length must be a non-negative integer")
 
 
+def _spec_sampling(sampling, constraint):
+    """The ``SamplingParams`` speculative decoding samples with (None: greedy), refusing what it does not take."""
+    if constraint is not None:
+        raise ValueError("speculative decoding is greedy and unconstrained: it takes no constraint")
+    if sampling is None:
+        return None
+    from .sampler import SamplingParams
+
+    if not isinstance(sampling, SamplingParams):
+        raise ValueError(f"sampling must be None or a SamplingParams, got {type(sampling).__name__}")
+    if sampling.constraint is not None:
+        raise ValueError("speculative decoding is unconstrained: sampling must carry no constraint")
+    if sampling.penalized:
+        raise ValueError("speculative sampling takes temperature, top-k and top-p only: no penalties or min-p")
+    return None if sampling.temperature == 0 else sampling
+
+
 def speculative_generate_ids(draft_model, model, prompt_ids, max_new_tokens: int, proposal_length: int = 4, eos_token_ids=(),
-                             device=None, on_token=None, constraint=None):
+                             device=None, on_token=None, constraint=None, sampling=None):
     """Greedy generation of ``model`` with ``draft_model`` proposing ``proposal_length`` tokens per round.  Returns
     ``(ids, stats)``: the generated ids (those of ``greedy_generate_ids(model, ...)``, token for token) and the per-round
     ``(proposed, accepted)`` counts.  CUDA Week-3 models with ``1 <= proposal_length <= 7`` verify in one captured graph
     per round (``Qwen3ModelWeek3.verify_engine``); everything else runs the same protocol through ``model(...)``.
-    Speculative decoding is greedy and unconstrained: a ``constraint`` is refused with ``ValueError``."""
+    Speculative decoding is unconstrained: a ``constraint`` is refused with ``ValueError``.
+    ``sampling`` (a ``SamplingParams`` with temperature, top-k, top-p and seed; temperature 0 is the greedy path) samples
+    instead (DESIGN.md section 8d): the draft draws each proposal with ``tl_sample`` and every verify round keeps or
+    replaces it by the rejection rule of ``tl_speculative_sample``, so each emitted token is distributed as the target's
+    own ``tl_sample`` draw at its position.  With the target's weights as draft the ids equal
+    ``greedy_generate_ids(model, sampling=...)``.  Penalties, min-p and constraints are refused with ``ValueError``."""
     _check_proposal_length(proposal_length)
-    if constraint is not None:
-        raise ValueError("speculative decoding is greedy and unconstrained: it takes no constraint")
+    sampling = _spec_sampling(sampling, constraint)
     prompt_ids = [int(t) for t in prompt_ids]
     if not prompt_ids:
         raise ValueError("prompt must encode to at least one token")
     eos = {int(t) for t in eos_token_ids}
     fast = _graph_runner_applies(model, draft_model, device, proposal_length)
-    runner = (_GraphRunner if fast else _GenericRunner)(model, draft_model, device)
+    runner = (_GraphRunner if fast else _GenericRunner)(model, draft_model, device, sampling)
     produced: list[int] = []
 
     def emit(ids):
