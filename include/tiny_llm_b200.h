@@ -106,6 +106,16 @@ int tl_rms_norm(const void *x, const void *weight, void *out, int rows, int dim,
 /* x,out [B, L, H, D]; offsets int32 [B]; rotates the first `dims` of D. */
 int tl_rope(const void *x, const int32_t *offsets, void *out, int B, int L, int H, int D, int dims, float base,
             int traditional, int dtype, void *stream);
+/* RoPE frequency tables.  Every RoPE entry point below has a *_table form taking one more, trailing argument
+ * `const double *inv_freq`: a DEVICE float64 [dims / 2] table of frequencies that replaces base^(-i / (dims / 2))
+ * (base is then unused).  Null is the entry point without the suffix.  A scaled RoPE (YaRN, DESIGN.md "Long
+ * context") passes its blended table; every site of one model must read the same table so that keys written at
+ * prefill and queries rotated at decode use identical angles.  tl_rope_inv_freq writes the unscaled table,
+ * out[i] = base^(-i / (head_dim / 2)) for i < head_dim / 2, with the kernels' own double-precision expression:
+ * a site given that table returns the bits of its base path. */
+int tl_rope_inv_freq(double *out, int head_dim, float base, void *stream);
+int tl_rope_table(const void *x, const int32_t *offsets, void *out, int B, int L, int H, int D, int dims, float base,
+                  int traditional, int dtype, void *stream, const double *inv_freq);
 /* The kernels tl_rms_norm and tl_rope run (nothing is launched or read; pointers only count for their 16-byte
  * alignment), or a negative TL_E* code for arguments the launch rejects.
  *   tl_rms_norm_route : threads per row, 32 (one warp; dim <= 512) or 256 (one CTA); *vec = 1 when every access is a
@@ -161,6 +171,16 @@ int tl_paged_attention_route(const void *q, const void *key_pages, const void *v
 int tl_paged_attention_token_major(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
                                    const int32_t *context_lens, void *out, int rows, int L, int num_pages, int page_size, int max_pages,
                                    float scale, int is_causal, int num_kv_heads, int num_heads, void *stream);
+/* The same with a split of the key range for a prefill chunk with a long prefix: when the block table spans more than
+ * 8,192 keys (max_pages * page_size) the key range of every (request, KV head) is cut into up to 32 pieces (the count
+ * from a wave cost model, the tiles dealt out from each request's real context) and a merge launch writes the
+ * token-major output.  workspace: tl_paged_attention_token_major_workspace() bytes (0 at <= 8,192 keys, where the call
+ * is tl_paged_attention_token_major); null never splits. */
+size_t tl_paged_attention_token_major_workspace(int rows, int L, int page_size, int max_pages);
+int tl_paged_attention_token_major_split(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                         const int32_t *context_lens, void *out, int rows, int L, int num_pages, int page_size, int max_pages,
+                                         float scale, int is_causal, int num_kv_heads, int num_heads, void *workspace, size_t workspace_bytes,
+                                         void *stream);
 
 /* ---- CUDA extension behind the same per-op semantics ---------------------
  * Device-driven K/V append for a decode batch (the batched form of
@@ -344,6 +364,11 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
                                const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table, const int32_t *context_lens, void *q_out,
                                void *key_pages, void *value_pages, int rows, int N, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
                                int num_pages, int page_size, int max_pages, int chunk, int dtype, void *workspace, size_t workspace_bytes, void *stream);
+int tl_qkv_project_rope_append_table(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                     const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                     const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                     int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
+                                     int dtype, void *workspace, size_t workspace_bytes, void *stream, const double *inv_freq);
 /* Decode step, L == 1: per-head q/k RMSNorm + RoPE + K/V append in one launch.
  * qkv [B, (Hq + 2*Hkv) * D] (q heads | k heads | v heads); q_out [B, Hq, D];
  * K/V rows land in the page slot of token context_lens[b]-1 (rows with context
@@ -353,6 +378,10 @@ int tl_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, co
                                   void *q_out, void *key_pages, void *value_pages, int batch, int num_heads,
                                   int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size,
                                   int max_pages, int dtype, void *stream);
+int tl_decode_qk_norm_rope_append_table(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
+                                        const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages,
+                                        int batch, int num_heads, int num_kv_heads, int head_dim, float base, float eps, int num_pages,
+                                        int page_size, int max_pages, int dtype, void *stream, const double *inv_freq);
 /* The kernel tl_decode_qk_norm_rope_append, tl_chunk_qk_norm_rope_append and the second half of
  * tl_qkv_project_rope_append run (nothing is launched), or a negative TL_E* code for arguments they reject:
  * TL_QKN_ROW, one CTA per row with 16 warps sharing the row's angles (bf16, D == 128, Hq + 2 Hkv <= 64; the only
@@ -369,6 +398,10 @@ int tl_chunk_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, con
                                  void *q_out, void *key_pages, void *value_pages, int tokens, int num_heads,
                                  int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size,
                                  int max_pages, int dtype, void *stream);
+int tl_chunk_qk_norm_rope_append_table(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
+                                       const int32_t *block_table_row, const int32_t *context_lens, void *q_out, void *key_pages,
+                                       void *value_pages, int tokens, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
+                                       int num_pages, int page_size, int max_pages, int dtype, void *stream, const double *inv_freq);
 /* Chunk append (CUDA extension of paged_cache_update, paged_attention.cpp:14-31): the rows of ONE
  * request's key/value chunk [1, H, L, D] (element strides src_head_stride / src_token_stride, unit
  * inner stride) are written into up to TL_PAGE_SPANS page slices in one launch:
@@ -410,7 +443,7 @@ int tl_paged_cache_copy_prefix(const tl_kv_slab_table *slabs, const tl_prefix_co
  * points, the call sequence rms_norm, rms_norm, rope, rope, paged_cache_update, paged_attention
  * of src/tiny_llm_ref/qwen3_week3.py:62-105.  qkv [B, (Hq + 2 Hkv) * 128] is the
  * row-concatenated projection output; context_lens are post-append; rope_inv_freq holds the 64
- * float64 frequencies base^(-i/64); out [B, Hq * 128]; max_context bounds every context_lens[b]
+ * float64 frequencies (base^(-i/64), or a scaled table as for the *_table entry points); out [B, Hq * 128]; max_context bounds every context_lens[b]
  * (it fixes the split count, so a captured launch stays valid as the contexts grow);
  * workspace: tl_decode_attention_fused_workspace() floats.  A context longer than the block table
  * (max_pages * page_size) is clamped to it for the attention and for the append alike: the row's

@@ -436,7 +436,7 @@ __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_kernel(
 }
 
 __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_merge_kernel(const float *ws_o, const float *ws_m, const float *ws_l,
-                                                                      __nv_bfloat16 *out, int splits) {
+                                                                      __nv_bfloat16 *out, int splits, int L, int Hq, int token_major) {
     // Dependent launch (common.cuh): the partials are the attention kernel's output, in a workspace every layer rewrites
     // - read them through L2.
     griddep_launch();
@@ -468,12 +468,20 @@ __global__ void __launch_bounds__(GQA_THREADS) paged_gqa_merge_kernel(const floa
         for (int j = 0; j < 8; ++j)
             if (s0 + j < splits) o += v[j] * exp2f(f[j] - gm);
     }
-    out[qi * GQA_D + d] = __float2bfloat16_rn(gl == 0.f ? 0.f : o / gl);
+    // partial row qi is (b * Hq + head) * L + l; token-major output (the o projection's layout) is (b * L + l) * Hq + head.
+    // A split whose tiles all lie past a row's last visible key left m = -1e30, l = 0 for that row: weight 0 here.
+    size_t oi = qi;
+    if (token_major) {
+        const size_t l = qi % L, bh = qi / L;
+        oi = (bh / Hq * L + l) * Hq + bh % Hq;
+    }
+    out[oi * GQA_D + d] = __float2bfloat16_rn(gl == 0.f ? 0.f : o / gl);
 }
 
-int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws_l, void *out, int rows_total, int splits, cudaStream_t st) {
+int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws_l, void *out, int rows_total, int splits, cudaStream_t st,
+                           int L, int Hq, bool token_major) {
     launch_chained(paged_gqa_merge_kernel, dim3(static_cast<unsigned>(rows_total)), dim3(GQA_THREADS), 0, st, ws_o, ws_m, ws_l,
-                   static_cast<__nv_bfloat16 *>(out), splits);
+                   static_cast<__nv_bfloat16 *>(out), splits, L, Hq, token_major ? 1 : 0);
     TL_LAUNCH_CHECK("paged_gqa_merge");
     return TL_OK;
 }
@@ -541,7 +549,7 @@ int launch_paged_gqa(const void *q, const void *kp, const void *vp, const int32_
     TL_LAUNCH_CHECK("paged_gqa");
     if (splits > 1) {
         launch_chained(paged_gqa_merge_kernel, dim3(static_cast<unsigned>(rows * L)), dim3(GQA_THREADS), 0, st, static_cast<const float *>(ws_o),
-                       static_cast<const float *>(ws_m), static_cast<const float *>(ws_l), op, splits);
+                       static_cast<const float *>(ws_m), static_cast<const float *>(ws_l), op, splits, L, num_heads, 0);
         TL_LAUNCH_CHECK("paged_gqa_merge");
     }
     return TL_OK;

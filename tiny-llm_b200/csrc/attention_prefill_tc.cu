@@ -68,7 +68,7 @@ struct TcArgs {
     // split-KV (decode, L <= 8): CTA (query block, split) covers key tiles [split * tiles_per_split, ...) and
     // leaves an unnormalised partial (O fp32, running max in log2 units, sum) for paged_gqa_merge_kernel
     int splits, tiles_per_split;
-    int out_token_major;  // unsplit launches only: out[(b, l, head), :] instead of [(b, head, l), :] (the layout the o-projection takes)
+    int out_token_major;  // out[(b, l, head), :] instead of [(b, head, l), :] (the layout the o-projection takes); split: the merge writes it
     float *ws_o, *ws_m, *ws_l;
 };
 
@@ -313,8 +313,18 @@ bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_
     return L > 0 && num_pages > 0 && page_size >= TC_BN && page_size % TC_BN == 0;
 }
 
-// allow_split (decode, L <= 8): the key range of every (request, KV head) is cut into up to PAGED_MAX_SPLITS pieces of
-// >= 4 tiles so that a small batch still fills the GPU; the partials are combined by paged_gqa_merge_kernel.
+// allow_split: the key range of every (request, KV head) is cut into up to PAGED_MAX_SPLITS pieces so that a small batch
+// still fills the GPU; the partials are combined by paged_gqa_merge_kernel.  Decode (L <= 8, head-major output) splits
+// at any width; the token-major form of a prefill chunk only when the block table spans more than PREFILL_SPLIT_MIN_KEYS
+// keys (a long prefix: unsplit, a 128-row chunk at Qwen3-4B shapes is 32 CTAs that each walk the whole prefix).  Causal
+// masking stays per row inside a split; a split past a row's last visible key leaves an empty partial (m = -1e30, l = 0)
+// that the merge weights by zero.  The split count comes from the block table's width and the tiles are dealt out from
+// the real context inside the kernel, so a row's result does not depend on the graph's grid.
+size_t paged_token_major_workspace(int rows, int L, int page_size, int max_pages) {
+    if (static_cast<long long>(max_pages) * page_size <= PREFILL_SPLIT_MIN_KEYS) return 0;
+    return static_cast<size_t>(rows) * L * PAGED_MAX_SPLITS * (TC_D + 2) * sizeof(float);
+}
+
 int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, bool allow_split, void *ws, size_t ws_bytes, cudaStream_t st, bool out_token_major) {
@@ -351,7 +361,7 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     a.out_token_major = out_token_major ? 1 : 0;
     a.splits = 1;
     a.tiles_per_split = static_cast<int>(max_tiles < 1 ? 1 : max_tiles);
-    if (allow_split && ws != nullptr && !out_token_major) {
+    if (allow_split && ws != nullptr && (!out_token_major || static_cast<long long>(max_pages) * page_size > PREFILL_SPLIT_MIN_KEYS)) {
         // Split count: the one that minimises waves x (tiles per CTA + fixed cost) + merge launch, in units of one 64-key
         // tile, with one CTA slot per SM, ~3 tiles of fixed cost per CTA (set-up, Q load, epilogue) and 2 + splits / 4
         // for the merge launch (it reads one partial per split and row).
@@ -380,7 +390,7 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     cudaError_t le = launch_chained(paged_prefill_tc_kernel, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
     if (le != cudaSuccess) return fail(TL_ECUDA, "paged_attention: launch failed: %s", cudaGetErrorString(le));
     TL_LAUNCH_CHECK("paged_prefill_tc");
-    if (a.splits > 1) return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, rows * L, a.splits, st);
+    if (a.splits > 1) return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, rows * L, a.splits, st, L, num_heads, out_token_major);
     return TL_OK;
 }
 

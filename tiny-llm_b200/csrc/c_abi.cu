@@ -165,13 +165,24 @@ int tl_rms_norm(const void *x, const void *weight, void *out, int rows, int dim,
 
 int tl_rope(const void *x, const int32_t *offsets, void *out, int B, int L, int H, int D, int dims, float base,
             int traditional, int dtype, void *stream) {
+    return tl_rope_table(x, offsets, out, B, L, H, D, dims, base, traditional, dtype, stream, nullptr);
+}
+
+int tl_rope_table(const void *x, const int32_t *offsets, void *out, int B, int L, int H, int D, int dims, float base,
+                  int traditional, int dtype, void *stream, const double *inv_freq) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "rope: expected float32, float16, or bfloat16");
     if (B < 0 || L < 0 || H < 0 || D <= 0) return fail(TL_EINVAL, "rope: expected x=[B,L,H,D] and one int32 offset per batch row");
     if (dims <= 0 || dims > D || dims % 2 != 0)
         return fail(TL_EINVAL, "rope: dims must be positive, even, and no larger than the head dimension");
     if (static_cast<long long>(B) * L * H == 0) return TL_OK;
     if (!x || !offsets || !out) return fail(TL_EINVAL, "rope: null pointer");
-    return launch_rope(x, offsets, out, B, L, H, D, dims, base, traditional, dtype, as_stream(stream));
+    return launch_rope(x, offsets, out, B, L, H, D, dims, base, inv_freq, traditional, dtype, as_stream(stream));
+}
+
+int tl_rope_inv_freq(double *out, int head_dim, float base, void *stream) {
+    if (head_dim <= 0 || head_dim % 2 != 0) return fail(TL_EINVAL, "rope_inv_freq: head_dim must be positive and even");
+    if (!out) return fail(TL_EINVAL, "rope_inv_freq: null pointer");
+    return launch_rope_inv_freq(out, head_dim / 2, base, as_stream(stream));
 }
 
 int tl_rms_norm_route(int dim, int dtype, const void *x, const void *weight, const void *out, int *vec) {
@@ -350,6 +361,19 @@ int tl_paged_attention(const void *q, const void *key_pages, const void *value_p
 int tl_paged_attention_token_major(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
                                    const int32_t *context_lens, void *out, int rows, int L, int num_pages, int page_size, int max_pages,
                                    float scale, int is_causal, int num_kv_heads, int num_heads, void *stream) {
+    return tl_paged_attention_token_major_split(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size,
+                                                max_pages, scale, is_causal, num_kv_heads, num_heads, nullptr, 0, stream);
+}
+
+size_t tl_paged_attention_token_major_workspace(int rows, int L, int page_size, int max_pages) {
+    if (rows <= 0 || L <= 0 || page_size <= 0 || max_pages <= 0) return 0;
+    return paged_token_major_workspace(rows, L, page_size, max_pages);
+}
+
+int tl_paged_attention_token_major_split(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                         const int32_t *context_lens, void *out, int rows, int L, int num_pages, int page_size, int max_pages,
+                                         float scale, int is_causal, int num_kv_heads, int num_heads, void *workspace, size_t workspace_bytes,
+                                         void *stream) {
     if (num_heads <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0 || rows < 0 || rows % num_heads != 0 || L < 0 || num_pages <= 0 ||
         page_size <= 0 || max_pages <= 0)
         return fail(TL_EINVAL, "paged_attention_token_major: bad shape");
@@ -359,7 +383,7 @@ int tl_paged_attention_token_major(const void *q, const void *key_pages, const v
                              false) != PagedPath::WGMMA)
         return fail(TL_EINVAL, "paged_attention_token_major: needs the wgmma kernel (bf16, D = 128, pages a multiple of 64 slots)");
     return launch_paged_prefill_tc(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages, scale,
-                                   is_causal, num_kv_heads, num_heads, false, nullptr, 0, as_stream(stream), true);
+                                   is_causal, num_kv_heads, num_heads, workspace != nullptr, workspace, workspace_bytes, as_stream(stream), true);
 }
 
 // ------------------------------------------------------------------ misc --
@@ -535,6 +559,16 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
                                const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table, const int32_t *context_lens, void *q_out,
                                void *key_pages, void *value_pages, int rows, int N, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
                                int num_pages, int page_size, int max_pages, int chunk, int dtype, void *workspace, size_t workspace_bytes, void *stream) {
+    return tl_qkv_project_rope_append_table(scales, biases, b, p0, qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out,
+                                            key_pages, value_pages, rows, N, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size,
+                                            max_pages, chunk, dtype, workspace, workspace_bytes, stream, nullptr);
+}
+
+int tl_qkv_project_rope_append_table(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                     const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                     const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                     int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
+                                     int dtype, void *workspace, size_t workspace_bytes, void *stream, const double *inv_freq) {
     if (dtype != TL_BF16) return fail(TL_EDTYPE, "qkv_project_rope_append: bfloat16 required");
     if (rows < 0 || N <= 0 || N % 128 != 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512 || num_pages <= 0 ||
         page_size <= 0 || max_pages <= 0)
@@ -556,11 +590,11 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
     if (rc != TL_OK) return rc;
     if (planes > 1)  // the split-reduction planes go straight into the norm / RoPE / append kernel: q|k|v is never written
         return launch_qkv_planes_rope_append(static_cast<const float *>(workspace), planes, q_norm_weight, k_norm_weight, offsets, block_table,
-                                             context_lens, q_out, key_pages, value_pages, rows, num_heads, num_kv_heads, base, eps, num_pages,
-                                             page_size, max_pages, st, chunk != 0);
+                                             context_lens, q_out, key_pages, value_pages, rows, num_heads, num_kv_heads, base, inv_freq, eps,
+                                             num_pages, page_size, max_pages, st, chunk != 0);
     return launch_decode_qk_norm_rope_append(qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out, key_pages,
-                                             value_pages, rows, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size, max_pages, dtype,
-                                             st, chunk != 0);
+                                             value_pages, rows, num_heads, num_kv_heads, head_dim, base, inv_freq, eps, num_pages, page_size, max_pages,
+                                             dtype, st, chunk != 0);
 }
 
 int tl_qk_norm_rope_route(int num_heads, int num_kv_heads, int head_dim, int dtype) {
@@ -575,6 +609,15 @@ int tl_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, co
                                   void *q_out, void *key_pages, void *value_pages, int batch, int num_heads,
                                   int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size,
                                   int max_pages, int dtype, void *stream) {
+    return tl_decode_qk_norm_rope_append_table(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out, key_pages, value_pages,
+                                               batch, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size, max_pages, dtype, stream,
+                                               nullptr);
+}
+
+int tl_decode_qk_norm_rope_append_table(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
+                                        const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages,
+                                        int batch, int num_heads, int num_kv_heads, int head_dim, float base, float eps, int num_pages,
+                                        int page_size, int max_pages, int dtype, void *stream, const double *inv_freq) {
     if (dtype != TL_F32 && dtype != TL_BF16) return fail(TL_EDTYPE, "decode_qk_norm_rope_append: bfloat16 or float32 required");
     if (batch < 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512 ||
         num_pages <= 0 || page_size <= 0 || max_pages <= 0)
@@ -583,7 +626,7 @@ int tl_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, co
     if (!qkv || !q_norm_weight || !k_norm_weight || !offsets || !block_table || !context_lens || !q_out || !key_pages || !value_pages)
         return fail(TL_EINVAL, "decode_qk_norm_rope_append: null pointer");
     return launch_decode_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out,
-                                             key_pages, value_pages, batch, num_heads, num_kv_heads, head_dim, base, eps,
+                                             key_pages, value_pages, batch, num_heads, num_kv_heads, head_dim, base, inv_freq, eps,
                                              num_pages, page_size, max_pages, dtype, as_stream(stream));
 }
 
@@ -591,6 +634,15 @@ int tl_chunk_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, con
                                  const int32_t *block_table_row, const int32_t *context_lens, void *q_out, void *key_pages,
                                  void *value_pages, int tokens, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
                                  int num_pages, int page_size, int max_pages, int dtype, void *stream) {
+    return tl_chunk_qk_norm_rope_append_table(qkv, q_norm_weight, k_norm_weight, offsets, block_table_row, context_lens, q_out, key_pages,
+                                              value_pages, tokens, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size, max_pages,
+                                              dtype, stream, nullptr);
+}
+
+int tl_chunk_qk_norm_rope_append_table(const void *qkv, const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets,
+                                       const int32_t *block_table_row, const int32_t *context_lens, void *q_out, void *key_pages,
+                                       void *value_pages, int tokens, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
+                                       int num_pages, int page_size, int max_pages, int dtype, void *stream, const double *inv_freq) {
     if (dtype != TL_F32 && dtype != TL_BF16) return fail(TL_EDTYPE, "chunk_qk_norm_rope_append: bfloat16 or float32 required");
     if (tokens < 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512 || num_pages <= 0 ||
         page_size <= 0 || max_pages <= 0)
@@ -599,8 +651,8 @@ int tl_chunk_qk_norm_rope_append(const void *qkv, const void *q_norm_weight, con
     if (!qkv || !q_norm_weight || !k_norm_weight || !offsets || !block_table_row || !context_lens || !q_out || !key_pages || !value_pages)
         return fail(TL_EINVAL, "chunk_qk_norm_rope_append: null pointer");
     return launch_decode_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_table_row, context_lens, q_out, key_pages,
-                                             value_pages, tokens, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size,
-                                             max_pages, dtype, as_stream(stream), true);
+                                             value_pages, tokens, num_heads, num_kv_heads, head_dim, base, inv_freq, eps, num_pages,
+                                             page_size, max_pages, dtype, as_stream(stream), true);
 }
 
 size_t tl_decode_attention_fused_workspace(int batch, int num_heads, int num_kv_heads) {

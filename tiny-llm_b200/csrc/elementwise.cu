@@ -164,12 +164,30 @@ int launch_rms_norm(const void *x, const void *w, void *out, int rows, int dim, 
 }
 
 // ------------------------------------------------------------------- RoPE --
+// The frequency of pair i of `half`: the table's entry when the caller passes one (a scaled RoPE such as YaRN: every
+// site of a model reads the same float64 [half] table), else base^(-i/half), formed in double.  rope_inv_freq_kernel
+// writes the unscaled table with this very expression, so the table path and the inline path give the same bits.
+__device__ __forceinline__ double rope_inv_freq(const double *table, int i, int half, float base) {
+    return table != nullptr ? table[i] : exp2(-static_cast<double>(i) / static_cast<double>(half) * log2(static_cast<double>(base)));
+}
+
+__global__ void rope_inv_freq_kernel(double *out, int half, float base) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < half) out[i] = rope_inv_freq(nullptr, i, half, base);
+}
+
+int launch_rope_inv_freq(double *out, int half, float base, cudaStream_t st) {
+    rope_inv_freq_kernel<<<(half + 127) / 128, 128, 0, st>>>(out, half, base);
+    TL_LAUNCH_CHECK("rope_inv_freq");
+    return TL_OK;
+}
+
 // One thread per (b, l, h, item): item < dims/2 rotates one pair, the remaining
 // items copy the un-rotated tail [dims, D).  Consecutive threads touch
 // consecutive elements, so each warp access is one contiguous segment.
 template <typename T>
 __global__ void rope_kernel(const T *__restrict__ x, const int32_t *__restrict__ offsets, T *__restrict__ out, int B,
-                            int L, int H, int D, int dims, float base, int traditional) {
+                            int L, int H, int D, int dims, float base, const double *__restrict__ inv_freq_table, int traditional) {
     const int half_dim = dims / 2;
     const int items = half_dim + (D - dims);
     const long long total = static_cast<long long>(B) * L * H * items;
@@ -185,10 +203,10 @@ __global__ void rope_kernel(const T *__restrict__ x, const int32_t *__restrict__
         out[head_base + d] = x[head_base + d];
         return;
     }
-    // angle = position * base^(-pair/half) (week2_kernels.metal:86-92).  The frequency is
+    // angle = position * base^(-pair/half) (week2_kernels.metal:86-92), or the table's frequency.  The frequency is
     // formed in double so that long contexts (position ~32K) do not inherit the ~1e-7
     // relative error of an fp32 exp2/pow; the product and sincosf stay fp32.
-    const double inv_freq = exp2(-static_cast<double>(item) / static_cast<double>(half_dim) * log2(static_cast<double>(base)));
+    const double inv_freq = rope_inv_freq(inv_freq_table, item, half_dim, base);
     const float angle = static_cast<float>(static_cast<double>(offsets[b] + l) * inv_freq);
     float s, c;
     sincosf(angle, &s, &c);
@@ -205,7 +223,7 @@ __global__ void rope_kernel(const T *__restrict__ x, const int32_t *__restrict__
 // them once per head.
 template <typename T>
 __global__ void rope_heads_kernel(const T *__restrict__ x, const int32_t *__restrict__ offsets, T *__restrict__ out, int B, int L,
-                                  int H, int D, float base, int traditional) {
+                                  int H, int D, float base, const double *__restrict__ inv_freq_table, int traditional) {
     const int half_dim = D / 2;
     const long long total = static_cast<long long>(B) * L * half_dim;
     const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -213,7 +231,7 @@ __global__ void rope_heads_kernel(const T *__restrict__ x, const int32_t *__rest
     const int item = static_cast<int>(idx % half_dim);
     const int l = static_cast<int>((idx / half_dim) % L);
     const int b = static_cast<int>(idx / (static_cast<long long>(half_dim) * L));
-    const double inv_freq = exp2(-static_cast<double>(item) / static_cast<double>(half_dim) * log2(static_cast<double>(base)));
+    const double inv_freq = rope_inv_freq(inv_freq_table, item, half_dim, base);
     const float angle = static_cast<float>(static_cast<double>(offsets[b] + l) * inv_freq);
     float s, c;
     sincosf(angle, &s, &c);
@@ -231,7 +249,7 @@ bool rope_heads_path(int B, int L, int H, int D, int dims) { return dims == D &&
 
 template <typename T>
 static int rope_t(const void *x, const int32_t *off, void *out, int B, int L, int H, int D, int dims, float base,
-                  int traditional, cudaStream_t st) {
+                  const double *inv_freq, int traditional, cudaStream_t st) {
     const long long total = static_cast<long long>(B) * L * H * (dims / 2 + D - dims);
     if (total == 0) return TL_OK;
     if (rope_heads_path(B, L, H, D, dims)) {
@@ -239,7 +257,7 @@ static int rope_t(const void *x, const int32_t *off, void *out, int B, int L, in
         const long long nb = ceil_div_ll(work, 128);
         if (nb > INT_MAX) return fail(TL_EINVAL, "rope: tensor too large");
         rope_heads_kernel<T><<<static_cast<unsigned>(nb), 128, 0, st>>>(static_cast<const T *>(x), off, static_cast<T *>(out), B, L, H, D, base,
-                                                                      traditional);
+                                                                      inv_freq, traditional);
         TL_LAUNCH_CHECK("rope");
         return TL_OK;
     }
@@ -248,17 +266,17 @@ static int rope_t(const void *x, const int32_t *off, void *out, int B, int L, in
     if (blocks > INT_MAX) return fail(TL_EINVAL, "rope: tensor too large");
     rope_kernel<T><<<static_cast<unsigned>(blocks), threads, 0, st>>>(static_cast<const T *>(x), off,
                                                                        static_cast<T *>(out), B, L, H, D, dims, base,
-                                                                       traditional);
+                                                                       inv_freq, traditional);
     TL_LAUNCH_CHECK("rope");
     return TL_OK;
 }
 
 int launch_rope(const void *x, const int32_t *off, void *out, int B, int L, int H, int D, int dims, float base,
-                int traditional, int dtype, cudaStream_t st) {
+                const double *inv_freq, int traditional, int dtype, cudaStream_t st) {
     switch (dtype) {
-        case TL_F32: return rope_t<float>(x, off, out, B, L, H, D, dims, base, traditional, st);
-        case TL_F16: return rope_t<__half>(x, off, out, B, L, H, D, dims, base, traditional, st);
-        case TL_BF16: return rope_t<__nv_bfloat16>(x, off, out, B, L, H, D, dims, base, traditional, st);
+        case TL_F32: return rope_t<float>(x, off, out, B, L, H, D, dims, base, inv_freq, traditional, st);
+        case TL_F16: return rope_t<__half>(x, off, out, B, L, H, D, dims, base, inv_freq, traditional, st);
+        case TL_BF16: return rope_t<__nv_bfloat16>(x, off, out, B, L, H, D, dims, base, inv_freq, traditional, st);
     }
     return fail(TL_EDTYPE, "rope: expected float32, float16, or bfloat16");
 }
@@ -694,8 +712,9 @@ __global__ void decode_qk_norm_rope_append_kernel(const T *qkv, const T *__restr
                                                   const T *__restrict__ kw, const int32_t *__restrict__ offsets,
                                                   const int32_t *__restrict__ bt, const int32_t *__restrict__ cl,
                                                   T *__restrict__ q_out, T *__restrict__ kp, T *__restrict__ vp, int Hq,
-                                                  int Hkv, int D, float base, float eps, int num_pages, int page_size,
-                                                  int max_pages, int bt_stride, long long q_row_stride, long long q_head_stride) {
+                                                  int Hkv, int D, float base, const double *__restrict__ inv_freq_table, float eps,
+                                                  int num_pages, int page_size, int max_pages, int bt_stride, long long q_row_stride,
+                                                  long long q_head_stride) {
     // bt_stride: block-table elements between rows (max_pages: one request per row; 0: every row is a token of ONE
     // request - a prefill chunk).  q_out element (row b, head h) starts at b * q_row_stride + h * q_head_stride.
     __shared__ float warp_part[8];
@@ -727,7 +746,7 @@ __global__ void decode_qk_norm_rope_append_kernel(const T *qkv, const T *__restr
             nre = to_f(from_f<T>(re * inv * to_f(w[i])));
             nim = to_f(from_f<T>(im * inv * to_f(w[i + half])));
         }
-        const double inv_freq = exp2(-static_cast<double>(i) / static_cast<double>(half) * log2(static_cast<double>(base)));
+        const double inv_freq = rope_inv_freq(inv_freq_table, i < half ? i : 0, half, base);
         const float angle = static_cast<float>(static_cast<double>(offsets[b]) * inv_freq);
         float s, c;
         sincosf(angle, &s, &c);
@@ -767,8 +786,8 @@ constexpr int QKN_WARPS = 16, QKN_MAXH = 4;  // up to 64 heads (q + k + v) per r
 template <typename T, bool PLANES>
 __global__ void __launch_bounds__(QKN_WARPS * 32) decode_qk_norm_rope_append_d128_kernel(
     const T *qkv, const float *part, int splits, long long plane, const T *__restrict__ qw, const T *__restrict__ kw, const int32_t *__restrict__ offsets, const int32_t *__restrict__ bt,
-    const int32_t *__restrict__ cl, T *q_out, T *kp, T *vp, int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages,
-    int bt_stride, long long q_row_stride, long long q_head_stride) {
+    const int32_t *__restrict__ cl, T *q_out, T *kp, T *vp, int Hq, int Hkv, float base, const double *__restrict__ inv_freq_table, float eps,
+    int num_pages, int page_size, int max_pages, int bt_stride, long long q_row_stride, long long q_head_stride) {
     constexpr int D = 128, half = 64;
     griddep_launch();
     griddep_wait();  // qkv is the previous kernel's output: read through L2 (common.cuh: programmatic dependent launch)
@@ -823,7 +842,7 @@ __global__ void __launch_bounds__(QKN_WARPS * 32) decode_qk_norm_rope_append_d12
     __shared__ float sn_s[half], cs_s[half];
     if (threadIdx.x < half) {
         const int i = threadIdx.x;
-        const double inv_freq = exp2(-static_cast<double>(i) / static_cast<double>(half) * log2(static_cast<double>(base)));
+        const double inv_freq = rope_inv_freq(inv_freq_table, i, half, base);
         const float angle = static_cast<float>(static_cast<double>(offsets[b]) * inv_freq);
         sincosf(angle, &sn_s[i], &cs_s[i]);
     }
@@ -882,7 +901,7 @@ __global__ void __launch_bounds__(QKN_WARPS * 32) decode_qk_norm_rope_append_d12
 
 int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                       const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages,
-                                      void *value_pages, int batch, int Hq, int Hkv, int D, float base, float eps,
+                                      void *value_pages, int batch, int Hq, int Hkv, int D, float base, const double *inv_freq, float eps,
                                       int num_pages, int page_size, int max_pages, int dtype, cudaStream_t st, bool chunk) {
     if (batch == 0) return TL_OK;
     // chunk: the rows are the tokens of one request (shared block-table row); q_out is [Hq, rows, D], the layout
@@ -896,8 +915,8 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
         using T = __nv_bfloat16;
         launch_chained(decode_qk_norm_rope_append_d128_kernel<T, false>, dim3(batch), dim3(QKN_WARPS * 32), 0, st, static_cast<const T *>(qkv),
                        static_cast<const float *>(nullptr), 0, 0LL, static_cast<const T *>(q_norm_w), static_cast<const T *>(k_norm_w), offsets, block_table, context_lens, static_cast<T *>(q_out),
-                       static_cast<T *>(key_pages), static_cast<T *>(value_pages), Hq, Hkv, base, eps, num_pages, page_size, max_pages, bt_stride,
-                       q_row_stride, q_head_stride);
+                       static_cast<T *>(key_pages), static_cast<T *>(value_pages), Hq, Hkv, base, inv_freq, eps, num_pages, page_size, max_pages,
+                       bt_stride, q_row_stride, q_head_stride);
         TL_LAUNCH_CHECK("decode_qk_norm_rope_append");
         return TL_OK;
     }
@@ -905,7 +924,7 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
     launch_chained(decode_qk_norm_rope_append_kernel<T>, grid, dim3(threads), 0, st,                                  \
         static_cast<const T *>(qkv), static_cast<const T *>(q_norm_w), static_cast<const T *>(k_norm_w), offsets,     \
         block_table, context_lens, static_cast<T *>(q_out), static_cast<T *>(key_pages), static_cast<T *>(value_pages), \
-        Hq, Hkv, D, base, eps, num_pages, page_size, max_pages, bt_stride, q_row_stride, q_head_stride)
+        Hq, Hkv, D, base, inv_freq, eps, num_pages, page_size, max_pages, bt_stride, q_row_stride, q_head_stride)
     if (dtype == TL_BF16)
         TL_QKN(__nv_bfloat16);
     else if (dtype == TL_F32)
@@ -922,7 +941,8 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
 bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype) { return D == 128 && dtype == TL_BF16 && Hq + 2 * Hkv <= QKN_WARPS * QKN_MAXH; }
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,
-                                  int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages, cudaStream_t st, bool chunk) {
+                                  int Hq, int Hkv, float base, const double *inv_freq, float eps, int num_pages, int page_size, int max_pages,
+                                  cudaStream_t st, bool chunk) {
     using T = __nv_bfloat16;
     constexpr int D = 128;
     const int bt_stride = chunk ? 0 : max_pages;
@@ -931,8 +951,8 @@ int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_n
     const long long plane = static_cast<long long>(batch) * (Hq + 2 * Hkv) * D;
     launch_chained(decode_qk_norm_rope_append_d128_kernel<T, true>, dim3(batch), dim3(QKN_WARPS * 32), 0, st, static_cast<const T *>(nullptr), part, splits,
                    plane, static_cast<const T *>(q_norm_w), static_cast<const T *>(k_norm_w), offsets, block_table, context_lens, static_cast<T *>(q_out),
-                   static_cast<T *>(key_pages), static_cast<T *>(value_pages), Hq, Hkv, base, eps, num_pages, page_size, max_pages, bt_stride,
-                   q_row_stride, q_head_stride);
+                   static_cast<T *>(key_pages), static_cast<T *>(value_pages), Hq, Hkv, base, inv_freq, eps, num_pages, page_size, max_pages,
+                   bt_stride, q_row_stride, q_head_stride);
     TL_LAUNCH_CHECK("qkv_planes_rope_append");
     return TL_OK;
 }

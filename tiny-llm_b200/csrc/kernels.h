@@ -15,8 +15,10 @@ namespace tl {
 int rms_norm_path(int dim, int dtype, const void *x, const void *w, const void *out, bool *vec);
 bool rope_heads_path(int B, int L, int H, int D, int dims);
 int launch_rms_norm(const void *x, const void *w, void *out, int rows, int dim, float eps, int dtype, cudaStream_t st);
+// inv_freq: null (base^(-i / (dims/2)) inline) or a float64 [dims/2] frequency table (every RoPE site below)
 int launch_rope(const void *x, const int32_t *off, void *out, int B, int L, int H, int D, int dims, float base,
-                int traditional, int dtype, cudaStream_t st);
+                const double *inv_freq, int traditional, int dtype, cudaStream_t st);
+int launch_rope_inv_freq(double *out, int half, float base, cudaStream_t st);
 int launch_swiglu(const void *gate, const void *up, void *out, long long n, int dtype, cudaStream_t st);
 int launch_add(const void *a, const void *b, void *out, long long n, int dtype, cudaStream_t st);
 int launch_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight,
@@ -69,7 +71,7 @@ int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *
 
 int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                       const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages,
-                                      void *value_pages, int batch, int Hq, int Hkv, int D, float base, float eps,
+                                      void *value_pages, int batch, int Hq, int Hkv, int D, float base, const double *inv_freq, float eps,
                                       int num_pages, int page_size, int max_pages, int dtype, cudaStream_t st, bool chunk = false);
 
 // w4a16_matvec.cu
@@ -106,7 +108,8 @@ int launch_w4a16_grouped(const void *scales, const void *biases, const void *a, 
 bool qkv_planes_rope_supported(int Hq, int Hkv, int D, int dtype);
 int launch_qkv_planes_rope_append(const float *part, int splits, const void *q_norm_w, const void *k_norm_w, const int32_t *offsets,
                                   const int32_t *block_table, const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int batch,
-                                  int Hq, int Hkv, float base, float eps, int num_pages, int page_size, int max_pages, cudaStream_t st, bool chunk);
+                                  int Hq, int Hkv, float base, const double *inv_freq, float eps, int num_pages, int page_size, int max_pages,
+                                  cudaStream_t st, bool chunk);
 
 // moe.cu (Qwen3-MoE routing, grouping, gather, combine and the grouped control kernel)
 int launch_moe_topk(const void *logits, void *probs, int32_t *ids, void *scores, int rows, int E, int k, int norm, int dtype, cudaStream_t st);
@@ -160,7 +163,13 @@ bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_
 int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,
                             int L, int num_pages, int page_size, int max_pages, float scale, int is_causal, int num_kv_heads,
                             int num_heads, bool allow_split, void *ws, size_t ws_bytes, cudaStream_t st, bool out_token_major = false);
-int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws_l, void *out, int rows_total, int splits, cudaStream_t st);
+// token_major: partial row (b * Hq + head) * L + l lands in output row (b * L + l) * Hq + head (the o projection's layout)
+int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws_l, void *out, int rows_total, int splits, cudaStream_t st,
+                           int L = 1, int Hq = 1, bool token_major = false);
+// The token-major (prefill-chunk) form of launch_paged_prefill_tc splits the key range only when the block table spans
+// more than this many keys: every shape below it keeps the unsplit launch and its bits.
+constexpr long long PREFILL_SPLIT_MIN_KEYS = 8192;
+size_t paged_token_major_workspace(int rows, int L, int page_size, int max_pages);
 
 // attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the wgmma kernel does not take)
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,

@@ -30,6 +30,8 @@ __all__ = [
     "quantized_embedding",
     "rms_norm",
     "rope",
+    "rope_table",
+    "rope_default_inv_freq",
     "rms_norm_route",
     "rope_route",
     "qk_norm_rope_route",
@@ -96,6 +98,8 @@ _SIGNATURES = {
     "tl_quantized_embedding": (_I, [_VP] * 5 + [_I] * 4 + [_VP]),
     "tl_rms_norm": (_I, [_VP] * 3 + [_I, _I, _F, _I, _VP]),
     "tl_rope": (_I, [_VP] * 3 + [_I] * 5 + [_F, _I, _I, _VP]),
+    "tl_rope_table": (_I, [_VP] * 3 + [_I] * 5 + [_F, _I, _I, _VP, _VP]),
+    "tl_rope_inv_freq": (_I, [_VP, _I, _F, _VP]),
     "tl_rms_norm_route": (_I, [_I, _I] + [_VP] * 3 + [ctypes.POINTER(_I)]),
     "tl_rope_route": (_I, [_I] * 6),
     "tl_qk_norm_rope_route": (_I, [_I] * 4),
@@ -118,13 +122,18 @@ _SIGNATURES = {
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
+    "tl_qkv_project_rope_append_table": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
+    "tl_paged_attention_token_major_workspace": (_SZ, [_I] * 4),
+    "tl_paged_attention_token_major_split": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP, _SZ, _VP]),
     "tl_quantized_matmul_fused_workspace": (_SZ, [_I] * 6),
     "tl_quantized_matmul_route": (_I, [_I] * 8 + [_VP] * 4 + [ctypes.POINTER(_I)] * 4),
     "tl_quantized_matmul_fused": (_I, [_VP] * 7 + [_I] * 6 + [_F, _I, _VP, _SZ, _VP]),
     "tl_quantized_matmul_residual_norm": (_I, [_VP] * 8 + [_I] * 3 + [_F, _I, _VP, _SZ, _VP]),
     "tl_decode_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
+    "tl_decode_qk_norm_rope_append_table": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP, _VP]),
     "tl_chunk_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
+    "tl_chunk_qk_norm_rope_append_table": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP, _VP]),
     "tl_decode_attention_fused_workspace": (_SZ, [_I, _I, _I]),
     "tl_decode_attention_fused": (_I, [_VP] * 11 + [_I] * 4 + [_F, _F] + [_I] * 5 + [_VP]),
     "tl_decode_attention_fused_rows_workspace": (_SZ, [_I, _I, _I, _I]),
@@ -187,6 +196,15 @@ def _contig(op: str, **named: torch.Tensor) -> None:
     for name, t in named.items():
         if not t.is_contiguous():
             raise RuntimeError(f"{op}: {name} must be contiguous")
+
+
+def _inv_freq(op: str, inv_freq, half: int) -> None:
+    """A RoPE frequency table (``rope_table`` and the ``inv_freq=`` forms): float64 [half], contiguous."""
+    if inv_freq is None:
+        return
+    if inv_freq.dtype != torch.float64 or tuple(inv_freq.shape) != (half,) or not inv_freq.is_contiguous():
+        raise RuntimeError(f"{op}: inv_freq must be a contiguous float64 [{half}] table")
+    _gpu(op, inv_freq)
 
 
 def _norm_weights(op: str, dtype: torch.dtype, head_dim: int, **named: torch.Tensor) -> None:
@@ -350,20 +368,43 @@ def rms_norm(x, weight, eps, stream=None):
 
 def rope(x, offsets, dims, base, traditional=False, stream=None):
     """bindings.cpp:37-38; week2_kernels.cpp:44-55."""
+    return _rope("rope", x, offsets, dims, base, None, traditional, stream)
+
+
+def rope_table(x, offsets, dims, inv_freq, traditional=False, stream=None):
+    """``rope`` with the frequencies of a float64 ``[dims / 2]`` device table (a scaled RoPE such as YaRN,
+    ``rope_scaling.py``) instead of ``base^(-i / (dims / 2))``."""
+    if inv_freq is None:
+        raise RuntimeError("rope_table: inv_freq is required")
+    return _rope("rope_table", x, offsets, dims, 0.0, inv_freq, traditional, stream)
+
+
+def _rope(op, x, offsets, dims, base, inv_freq, traditional, stream):
     if x.dtype not in _FLOATS:
-        raise RuntimeError("rope: expected float32, float16, or bfloat16")
+        raise RuntimeError(f"{op}: expected float32, float16, or bfloat16")
     if x.dim() != 4 or offsets.dtype != torch.int32 or offsets.dim() != 1 or offsets.shape[0] != x.shape[0]:
-        raise RuntimeError("rope: expected x=[B,L,H,D] and one int32 offset per batch row")
+        raise RuntimeError(f"{op}: expected x=[B,L,H,D] and one int32 offset per batch row")
     if dims <= 0 or dims > x.shape[3] or dims % 2 != 0:
-        raise RuntimeError("rope: dims must be positive, even, and no larger than the head dimension")
-    _gpu("rope", x, offsets)
-    _contig("rope", x=x, offsets=offsets)
+        raise RuntimeError(f"{op}: dims must be positive, even, and no larger than the head dimension")
+    _inv_freq(op, inv_freq, int(dims) // 2)
+    _gpu(op, x, offsets)
+    _contig(op, x=x, offsets=offsets)
     out = torch.empty_like(x)
     B, L, H, D = x.shape
-    _check(
-        _lib.tl_rope(x.data_ptr(), offsets.data_ptr(), out.data_ptr(), B, L, H, D, int(dims), float(base), int(bool(traditional)),
-                     _DTYPE_CODE[x.dtype], _stream_ptr(stream, x))
-    )
+    args = (x.data_ptr(), offsets.data_ptr(), out.data_ptr(), B, L, H, D, int(dims), float(base), int(bool(traditional)),
+            _DTYPE_CODE[x.dtype], _stream_ptr(stream, x))
+    _check(_lib.tl_rope(*args) if inv_freq is None else _lib.tl_rope_table(*args, inv_freq.data_ptr()))
+    return out
+
+
+def rope_default_inv_freq(head_dim: int, base: float, device, stream=None) -> torch.Tensor:
+    """float64 ``[head_dim / 2]`` unscaled RoPE frequencies formed on the device with the RoPE kernels' own expression
+    (``exp2(-i / half * log2(base))`` in double): a site given this table computes the bits of its ``base`` path."""
+    if head_dim <= 0 or head_dim % 2:
+        raise RuntimeError("rope_inv_freq: head_dim must be positive and even")
+    out = torch.empty(head_dim // 2, dtype=torch.float64, device=device)
+    _gpu("rope_inv_freq", out)
+    _check(_lib.tl_rope_inv_freq(out.data_ptr(), int(head_dim), float(base), _stream_ptr(stream, out)))
     return out
 
 
@@ -1015,10 +1056,19 @@ def quantized_matmul_route(M, N, K, lda, prologue, fused, use_simdgroup, dtype, 
     return (code, *(f.value for f in facts))
 
 
-def paged_attention_token_major(query, key_pages, value_pages, block_table, context_lens, scale, is_causal, num_kv_heads, num_heads, stream=None):
+def paged_attention_token_major_workspace(rows: int, L: int, page_size: int, max_pages: int) -> int:
+    """Bytes of the split workspace ``paged_attention_token_major(..., workspace=)`` takes for ``rows = B * Hq`` query heads of
+    ``L`` rows over a block table of ``max_pages`` pages: 0 when the table spans at most 8,192 keys (no split there)."""
+    return int(_lib.tl_paged_attention_token_major_workspace(int(rows), int(L), int(page_size), int(max_pages)))
+
+
+def paged_attention_token_major(query, key_pages, value_pages, block_table, context_lens, scale, is_causal, num_kv_heads, num_heads, stream=None,
+                                workspace=None):
     """Prefill attention (L > 8) with the output already in the o-projection's layout: ``query`` [B * Hq, L, D] ->
     ``[B * L, Hq * D]``.  Only on the wgmma kernel (bf16, D = 128, page size a multiple of 64); otherwise - and for
-    L <= 8 - ``paged_attention`` + a transpose copy."""
+    L <= 8 - ``paged_attention`` + a transpose copy.  ``workspace`` (uint8, ``paged_attention_token_major_workspace``
+    bytes): a block table spanning more than 8,192 keys splits the key range over more CTAs and merges the partials;
+    None never splits."""
     rows, L, D = query.shape
     B = rows // num_heads
     P, Hkv, page_size, _ = key_pages.shape
@@ -1027,10 +1077,15 @@ def paged_attention_token_major(query, key_pages, value_pages, block_table, cont
     if fast:
         _gpu("paged_attention", query, key_pages, value_pages, block_table, context_lens)
         out = torch.empty((B * L, num_heads * D), dtype=query.dtype, device=query.device)
-        rc = _lib.tl_paged_attention_token_major(
-            query.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), block_table.data_ptr(), context_lens.data_ptr(), out.data_ptr(),
-            rows, L, P, page_size, block_table.shape[1], float(scale), int(bool(is_causal)), int(num_kv_heads), int(num_heads),
-            _stream_ptr(stream, query))
+        args = (query.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), block_table.data_ptr(), context_lens.data_ptr(), out.data_ptr(),
+                rows, L, P, page_size, block_table.shape[1], float(scale), int(bool(is_causal)), int(num_kv_heads), int(num_heads))
+        if workspace is None:
+            rc = _lib.tl_paged_attention_token_major(*args, _stream_ptr(stream, query))
+        else:
+            if not workspace.is_cuda or not workspace.is_contiguous():
+                raise RuntimeError("paged_attention_token_major: workspace must be a contiguous CUDA tensor")
+            rc = _lib.tl_paged_attention_token_major_split(*args, workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+                                                           _stream_ptr(stream, query))
         if rc == 0:
             return out
     y = paged_attention(query, key_pages, value_pages, block_table, context_lens, scale, is_causal=is_causal, num_kv_heads=num_kv_heads,
@@ -1071,9 +1126,10 @@ def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight,
 
 
 def chunk_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_table_row, context_lens, key_pages, value_pages,
-                              num_heads, num_kv_heads, base, eps, stream=None):
+                              num_heads, num_kv_heads, base, eps, stream=None, inv_freq=None):
     """Prefill-chunk form of ``decode_qk_norm_rope_append``: the rows of ``qkv`` are consecutive tokens of one
-    request; returns the rotated queries ``[Hq, tokens, D]`` (the layout ``paged_attention`` takes)."""
+    request; returns the rotated queries ``[Hq, tokens, D]`` (the layout ``paged_attention`` takes).  ``inv_freq``: a
+    float64 ``[D / 2]`` frequency table replacing ``base`` (``rope_table``)."""
     T = qkv.shape[0]
     P, Hkv, page_size, D = key_pages.shape
     if qkv.dim() != 2 or qkv.shape[1] != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads:
@@ -1085,18 +1141,16 @@ def chunk_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_
     _int32("chunk_qk_norm_rope_append", T, offsets=offsets, context_lens=context_lens)
     _int32("chunk_qk_norm_rope_append", block_table_row=block_table_row)
     _norm_weights("chunk_qk_norm_rope_append", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
+    _inv_freq("chunk_qk_norm_rope_append", inv_freq, D // 2)
     _gpu("chunk_qk_norm_rope_append", qkv, q_norm_weight, k_norm_weight, offsets, block_table_row, context_lens, key_pages, value_pages)
     _contig("chunk_qk_norm_rope_append", qkv=qkv, offsets=offsets, block_table_row=block_table_row, context_lens=context_lens,
             key_pages=key_pages, value_pages=value_pages)
     q_out = torch.empty((num_heads, T, D), dtype=qkv.dtype, device=qkv.device)
-    _check(
-        _lib.tl_chunk_qk_norm_rope_append(
-            qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table_row.data_ptr(),
+    args = (qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table_row.data_ptr(),
             context_lens.data_ptr(), q_out.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), T, int(num_heads),
             int(num_kv_heads), D, float(base), float(eps), P, page_size, block_table_row.shape[0], _DTYPE_CODE[qkv.dtype],
-            _stream_ptr(stream, qkv),
-        )
-    )
+            _stream_ptr(stream, qkv))
+    _check(_lib.tl_chunk_qk_norm_rope_append(*args) if inv_freq is None else _lib.tl_chunk_qk_norm_rope_append_table(*args, inv_freq.data_ptr()))
     return q_out
 
 
@@ -1110,9 +1164,9 @@ def interleave_gate_up(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
 
 
 def decode_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages,
-                               num_heads, num_kv_heads, base, eps, stream=None):
+                               num_heads, num_kv_heads, base, eps, stream=None, inv_freq=None):
     """Fused per-head q/k RMSNorm + RoPE + K/V append of one decode step; returns
-    the rotated queries ``[B, Hq, D]``."""
+    the rotated queries ``[B, Hq, D]``.  ``inv_freq``: a float64 ``[D / 2]`` frequency table replacing ``base``."""
     B = qkv.shape[0]
     P, Hkv, page_size, D = key_pages.shape
     if qkv.dim() != 2 or qkv.shape[1] != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads:
@@ -1122,27 +1176,26 @@ def decode_qk_norm_rope_append(qkv, q_norm_weight, k_norm_weight, offsets, block
     _norm_weights("decode_qk_norm_rope_append", qkv.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
     _int32("decode_qk_norm_rope_append", B, offsets=offsets, context_lens=context_lens)
     _block_table("decode_qk_norm_rope_append", block_table, B)
+    _inv_freq("decode_qk_norm_rope_append", inv_freq, D // 2)
     _gpu("decode_qk_norm_rope_append", qkv, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages)
     _contig("decode_qk_norm_rope_append", qkv=qkv, offsets=offsets, block_table=block_table, context_lens=context_lens,
             key_pages=key_pages, value_pages=value_pages)
     q_out = torch.empty((B, num_heads, D), dtype=qkv.dtype, device=qkv.device)
-    _check(
-        _lib.tl_decode_qk_norm_rope_append(
-            qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table.data_ptr(),
+    args = (qkv.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(), offsets.data_ptr(), block_table.data_ptr(),
             context_lens.data_ptr(), q_out.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), B, int(num_heads),
             int(num_kv_heads), D, float(base), float(eps), P, page_size, block_table.shape[1], _DTYPE_CODE[qkv.dtype],
-            _stream_ptr(stream, qkv),
-        )
-    )
+            _stream_ptr(stream, qkv))
+    _check(_lib.tl_decode_qk_norm_rope_append(*args) if inv_freq is None else _lib.tl_decode_qk_norm_rope_append_table(*args, inv_freq.data_ptr()))
     return q_out
 
 
 def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages,
-                            num_heads, num_kv_heads, base, eps, chunk=False, stream=None):
+                            num_heads, num_kv_heads, base, eps, chunk=False, stream=None, inv_freq=None):
     """``qkv = p0 @ W_qkv^T`` then per-head q/k RMSNorm + RoPE + K/V append (``decode_qk_norm_rope_append``; ``chunk``: the
     rows are consecutive tokens of one request and ``block_table`` is its row).  Returns the rotated queries
     (``[rows, Hq, D]``, or ``[Hq, rows, D]`` for a chunk).  With 9..128 rows the projection's split-reduction planes
-    feed the second kernel directly; results are those of the two separate calls."""
+    feed the second kernel directly; results are those of the two separate calls.  ``inv_freq``: a float64 ``[D / 2]``
+    frequency table replacing ``base``."""
     rows, N = p0.shape
     P, Hkv, page_size, D = key_pages.shape
     K = b.shape[0]
@@ -1155,6 +1208,7 @@ def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight,
     _norm_weights(op, p0.dtype, D, q_norm_weight=q_norm_weight, k_norm_weight=k_norm_weight)
     _int32(op, rows, offsets=offsets, context_lens=context_lens)
     _block_table(op, block_table, None if chunk else rows)
+    _inv_freq(op, inv_freq, D // 2)
     _gpu(op, scales, biases, b, p0, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, key_pages, value_pages)
     _contig(op, b=b, scales=scales, biases=biases, offsets=offsets, block_table=block_table, context_lens=context_lens, key_pages=key_pages,
             value_pages=value_pages)
@@ -1164,19 +1218,18 @@ def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight,
     ws_bytes = _lib.tl_quantized_matmul_fused_workspace(rows, N, K, N, int(PRO_NONE), code)
     ws = _zero_workspace(ws_bytes, p0.device)
     max_pages = block_table.shape[-1]
-    _check(
-        _lib.tl_qkv_project_rope_append(
-            scales.data_ptr(), biases.data_ptr(), b.data_ptr(), p0.data_ptr(), scratch.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(),
+    args = (scales.data_ptr(), biases.data_ptr(), b.data_ptr(), p0.data_ptr(), scratch.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(),
             offsets.data_ptr(), block_table.data_ptr(), context_lens.data_ptr(), q_out.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(),
             rows, N, int(num_heads), int(num_kv_heads), D, float(base), float(eps), P, page_size, max_pages, int(bool(chunk)), code,
-            None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, p0),
-        )
-    )
+            None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, p0))
+    _check(_lib.tl_qkv_project_rope_append(*args) if inv_freq is None else _lib.tl_qkv_project_rope_append_table(*args, inv_freq.data_ptr()))
     return q_out
 
 
 def rope_inv_freq_table(head_dim: int, base: float, device) -> torch.Tensor:
-    """float64 [head_dim / 2] frequencies base^(-i / (head_dim / 2)) (rope.py:13-15 forms them the same way)."""
+    """float64 [head_dim / 2] frequencies base^(-i / (head_dim / 2)) (rope.py:13-15 forms them the same way).  The
+    unscaled ``decode_attention_fused`` path keeps reading this table so that its bits do not change; it can differ in
+    the last bits from ``rope_default_inv_freq``, the kernels' inline expression that every other site (and YaRN) uses."""
     half = head_dim // 2
     return torch.pow(torch.tensor(float(base), dtype=torch.float64), -torch.arange(half, dtype=torch.float64) / half).to(device)
 

@@ -24,6 +24,7 @@ from types import SimpleNamespace
 
 import torch
 
+from .rope_scaling import parse_rope_scaling
 from .synthetic import named_tensors
 
 ARG_KEYS = ("num_hidden_layers", "hidden_size", "vocab_size", "num_attention_heads", "num_key_value_heads", "head_dim",
@@ -58,6 +59,11 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
     if missing:
         raise ValueError(f"config.json lacks {missing}")
     args = SimpleNamespace(**{k: config[k] for k in ARG_KEYS})
+    # RoPE scaling: static YaRN is applied (rope_scaling.py); any other type raises ValueError here rather than load and
+    # compute every position wrongly
+    scaling = parse_rope_scaling(config.get("rope_scaling"), args.max_position_embeddings)
+    if scaling is not None:
+        args.rope_scaling = scaling.to_config()
     tensors = _read_tensors(path)
 
     def take(name: str) -> torch.Tensor:
@@ -98,6 +104,9 @@ def save_checkpoint(model_ns: SimpleNamespace, path) -> None:
     path.mkdir(parents=True, exist_ok=True)
     first = model_ns.model.embed_tokens
     config = {k: getattr(model_ns.args, k) for k in ARG_KEYS}
+    scaling = parse_rope_scaling(getattr(model_ns.args, "rope_scaling", None), model_ns.args.max_position_embeddings)
+    if scaling is not None:
+        config["rope_scaling"] = scaling.to_config()
     config["quantization"] = {"group_size": first.group_size, "bits": first.bits}
     config["model_type"] = "qwen3"
     (path / "config.json").write_text(json.dumps(config, indent=1))

@@ -40,7 +40,9 @@ def _load(args, device):
     from .synthetic import synthetic_qwen3
 
     if args.synthetic:
-        return synthetic_qwen3(args.synthetic, seed=0, device=device, realistic=args.synthetic.startswith("tiny")), None, "Qwen/Qwen3-synthetic"
+        extra = {} if args.rope_scaling is None else {"rope_scaling": args.rope_scaling}
+        return (synthetic_qwen3(args.synthetic, seed=0, device=device, realistic=args.synthetic.startswith("tiny"), **extra), None,
+                "Qwen/Qwen3-synthetic")
     ns = load_checkpoint(args.model, device=device)
     tokenizer = None
     try:
@@ -54,8 +56,29 @@ def _model(args, ns, name):
     from .models import dispatch_model
 
     if args.loader == "week2":
+        if args.max_context is not None:
+            raise SystemExit("--max-context needs the paged week3 model")
         return dispatch_model(name, ns, week=2)
-    return dispatch_model(name, ns, week=3, enable_paged_attention=not args.disable_paged_attention)
+    return dispatch_model(name, ns, week=3, enable_paged_attention=not args.disable_paged_attention, max_context=args.max_context)
+
+
+def _rope_scaling_arg(spec: str) -> dict:
+    from .rope_scaling import parse_cli
+
+    try:
+        return parse_cli(spec)
+    except ValueError as exc:
+        raise argparse.ArgumentTypeError(str(exc)) from None
+
+
+def _positive_int(text: str) -> int:
+    try:
+        value = int(text)
+    except ValueError:
+        value = 0
+    if value <= 0:
+        raise argparse.ArgumentTypeError(f"expected a positive integer (got {text!r})")
+    return value
 
 
 def parse_lora_specs(lora, synthetic_lora):
@@ -308,6 +331,10 @@ def main(argv=None) -> int:
         p.add_argument("--prompt", default="Give me a short introduction to large language models.")
         p.add_argument("--prompt-ids", default=None, help="comma-separated token ids (';' between requests for `batch`)")
         p.add_argument("--loader", choices=["week2", "week3"], default="week3")
+        p.add_argument("--rope-scaling", type=_rope_scaling_arg, default=None, metavar="yarn:FACTOR[:ORIGINAL]",
+                       help="static YaRN RoPE scaling of the --synthetic model (a checkpoint states its own in config.json)")
+        p.add_argument("--max-context", type=_positive_int, default=None, metavar="N",
+                       help="context window of the decode / prefill graphs (default 8192); refused if its KV pages do not fit the GPU")
         p.add_argument("--device", default="cuda:0")
         p.add_argument("--disable-paged-attention", action="store_true")
         p.add_argument("--enable-thinking", action="store_true")
@@ -351,6 +378,10 @@ def main(argv=None) -> int:
     args = ap.parse_args(argv)
     if not args.model and not args.synthetic:
         ap.error("--model or --synthetic is required")
+    if args.rope_scaling is not None and not args.synthetic:
+        ap.error("--rope-scaling applies to --synthetic; a checkpoint's config.json states its own rope_scaling")
+    if args.command == "batch" and args.max_context is not None and args.max_seq_len > args.max_context:
+        ap.error(f"--max-seq-len {args.max_seq_len} exceeds --max-context {args.max_context}")
     if args.logprobs is not None and not 0 <= args.logprobs <= 20:
         ap.error("--logprobs must be in [0, 20]")
     return args.fn(args)

@@ -358,7 +358,8 @@ class DecodeEngine(_GraphEngine):
         # is the TMA + wgmma streaming kernel (attention_prefill_tc.cu).
         self._attention_fused = self.fused and DecodeEngine.fused_attention_applies(model, self.B * self.max_seq_len)
         if self._attention_fused:
-            self._rope_inv_freq = ext.rope_inv_freq_table(self.D, attn0.rope.base, self.device)
+            # the model's scaled table when it has one (every site reads it); else the fused kernel's own unscaled table
+            self._rope_inv_freq = attn0.rope.inv_freq if attn0.rope.inv_freq is not None else ext.rope_inv_freq_table(self.D, attn0.rope.base, self.device)
             self._attn_ws = torch.empty(ext.decode_attention_fused_workspace(self.B, self.Hq, self.Hkv, rows_per_request=rows_per_request),
                                         dtype=torch.float32, device=self.device)
         # Row variants: the scheduler fills slots from index 0 (batch.py:220-226), so while few requests are live the
@@ -477,8 +478,8 @@ class DecodeEngine(_GraphEngine):
             v = _proj(h, at.wv).view(B, Hkv, 1, D)
             q = ext.rms_norm(q, at.q_norm._weight_as(x.dtype, x.device), at.q_norm.eps)
             k = ext.rms_norm(k, at.k_norm._weight_as(x.dtype, x.device), at.k_norm.eps)
-            q = ext.rope(q, self.offsets, at.rope.dims, at.rope.base, at.rope.traditional)
-            k = ext.rope(k, self.offsets, at.rope.dims, at.rope.base, at.rope.traditional)
+            q = at.rope(q, self.offsets)
+            k = at.rope(k, self.offsets)
             ext.paged_cache_append_decode(pool._key_pages, pool._value_pages, k.view(B, Hkv, 1, D), v, self.tables[i], self.context_lens)
             y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
@@ -539,7 +540,7 @@ class DecodeEngine(_GraphEngine):
             # projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel, q|k|v is never written
             q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
                                             at.k_norm._weight_as(h.dtype, h.device), offsets, self.tables[i][:R], context_lens,
-                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps)
+                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)
             y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             return y.view(R, Hq * D)
@@ -559,7 +560,7 @@ class DecodeEngine(_GraphEngine):
                                                   pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
                                                   self.max_seq_len, workspace=self._attn_ws)
             q = ext.decode_qk_norm_rope_append(qkv, qw, kw, offsets, self.tables[i][:R], context_lens, pool._key_pages, pool._value_pages,
-                                               Hq, Hkv, at.rope.base, at.q_norm.eps)
+                                               Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)
             y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             return y.view(R, Hq * D)
@@ -584,7 +585,7 @@ class DecodeEngine(_GraphEngine):
             else:
                 q = ext.decode_qk_norm_rope_append(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                    self.offsets, self.tables[i], self.context_lens, pool._key_pages, pool._value_pages,
-                                                   Hq, Hkv, at.rope.base, at.q_norm.eps)
+                                                   Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)
                 y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
                                         at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             x = ext.quantized_matmul_fused(at.wo.scales, at.wo.biases, at.wo.weight, y.view(B, Hq * D), residual=x, epilogue=ext.EPI_RESIDUAL)
@@ -1285,6 +1286,10 @@ class PrefillEngine(_GraphEngine):
         self.replays = 0
         self.kernels_per_chunk = 0
         self._packed = model.packed_layers()
+        # A window above 8,192 keys (a long prefix): the chunk's attention splits the prefix's key range over more CTAs and
+        # merges the partials into the token-major output; windows up to 8,192 keep the unsplit launch (no workspace).
+        ws = ext.paged_attention_token_major_workspace(self.Hq, L, model.page_size, self.max_pages)
+        self._attn_ws = torch.empty(ws, dtype=torch.uint8, device=self.device) if ws else None
         if self.lora is not None:  # one id per chunk, broadcast to its rows (padding rows carry it too: they are never stored)
             self._alloc_adapter_ids(L, -1)
 
@@ -1304,22 +1309,22 @@ class PrefillEngine(_GraphEngine):
         if self.L <= 128:  # projection + q/k norm + RoPE + append: the split-reduction planes feed the second kernel
             q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
                                             at.k_norm._weight_as(h.dtype, h.device), self.offsets, self.tables[i], self.ctxs,
-                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, chunk=True)  # [Hq, L, D]
+                                            pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, chunk=True, inv_freq=at.rope.inv_freq)  # [Hq, L, D]
         else:
             q = ext.chunk_qk_norm_rope_append(_proj(h, pk.qkv), at.q_norm._weight_as(h.dtype, h.device), at.k_norm._weight_as(h.dtype, h.device),
                                               self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
-                                              Hq, Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
+                                              Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)  # [Hq, L, D]
         return ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
-                                               True, Hkv, Hq)
+                                               True, Hkv, Hq, workspace=self._attn_ws)
 
     def _qkv_attention(self, i, block, qkv):
         """``_attention`` from q|k|v rows the adapters were already added to (LoRA engines, any chunk length)."""
         at, pool = block.self_attn, self.model.page_pools[i]
         q = ext.chunk_qk_norm_rope_append(qkv, at.q_norm._weight_as(qkv.dtype, qkv.device), at.k_norm._weight_as(qkv.dtype, qkv.device),
                                           self.offsets, self.tables[i], self.ctxs, pool._key_pages, pool._value_pages,
-                                          self.Hq, self.Hkv, at.rope.base, at.q_norm.eps)  # [Hq, L, D]
+                                          self.Hq, self.Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)  # [Hq, L, D]
         return ext.paged_attention_token_major(q, pool._key_pages, pool._value_pages, self.tables[i:i + 1], self.ctx_after, at.scale,
-                                               True, self.Hkv, self.Hq)
+                                               True, self.Hkv, self.Hq, workspace=self._attn_ws)
 
     def _forward(self) -> None:
         m, L = self.model, self.L

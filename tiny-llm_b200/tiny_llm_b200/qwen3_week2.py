@@ -22,6 +22,7 @@ from .kv_cache import TinyKvCache
 from .layer_norm import RMSNorm
 from .positional_encoding import RoPE
 from .quantize import QuantizedWeights, dequantize_linear, quantized_linear
+from .rope_scaling import parse_rope_scaling
 from .week2_kernels import FastRMSNorm, FastRoPE, decode_attention_custom, swiglu
 
 WEEK2_CHECKPOINTS = (
@@ -201,6 +202,8 @@ class Qwen3ModelWeek2:
 
         self.checkpoint = checkpoint
         args = mlx_model.args
+        if parse_rope_scaling(getattr(args, "rope_scaling", None), args.max_position_embeddings) is not None:
+            raise ValueError("the Week 2 model does not implement RoPE scaling (YaRN); load this config with Qwen3ModelWeek3")
         self.num_hidden_layers = args.num_hidden_layers
         self.hidden_size = args.hidden_size
         self.vocab_size = args.vocab_size

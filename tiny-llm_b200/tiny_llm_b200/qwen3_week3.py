@@ -23,6 +23,7 @@ from .kv_cache import TinyKvCache
 from .moe import Moe
 from .paged_kv_cache import TinyKvPagedCache, TinyKvPagedPool
 from .quantize import QuantizedWeights, quantized_linear
+from .rope_scaling import parse_rope_scaling, rope_inv_freq
 from .week2_kernels import (
     FastRMSNorm,
     FastRoPE,
@@ -31,6 +32,26 @@ from .week2_kernels import (
     scaled_dot_product_attention,
     swiglu,
 )
+
+
+def kv_reservation_pages(window: int, page_size: int, batch_size: int = 1) -> int:
+    """Pages per layer a decode engine of ``batch_size`` slots and context window ``window`` reserves."""
+    return (batch_size + 1) * (-(-window // page_size)) + 1
+
+
+def kv_reservation_bytes(layers: int, num_kv_heads: int, head_dim: int, page_size: int, window: int, batch_size: int = 1,
+                         dtype_bytes: int = 2) -> int:
+    """Bytes of bf16 K and V pages for ``kv_reservation_pages`` pages in each of ``layers`` layers."""
+    page_bytes = 2 * num_kv_heads * page_size * head_dim * dtype_bytes
+    return layers * kv_reservation_pages(window, page_size, batch_size) * page_bytes
+
+
+def check_kv_reservation(need: int, free: int, window: int, batch_size: int) -> None:
+    """Refuse a reservation of ``need`` bytes that does not fit ``free`` bytes."""
+    if need > free:
+        gib = 1 << 30
+        raise MemoryError(f"context window {window} for {batch_size} slot(s) needs {need} bytes ({need / gib:.2f} GiB) of KV pages, "
+                          f"but only {max(free, 0)} bytes ({max(free, 0) / gib:.2f} GiB) of device memory are free")
 
 
 class Qwen3MultiHeadAttention:
@@ -52,15 +73,22 @@ class Qwen3MultiHeadAttention:
         theta: int = 1000000,
         rms_norm_eps: float = 1e-5,
         use_paged_attention: bool = True,
+        rope_inv_freq: torch.Tensor | None = None,
+        rope_mscale: float = 1.0,
     ):
+        """``rope_inv_freq``: the model's scaled RoPE table (``rope_scaling.rope_inv_freq``), None for plain RoPE.
+        ``rope_mscale``: YaRN's ``m``; q and k are each scaled by it, which is folded into ``scale`` as ``m^2`` (so
+        every engine, which reads ``scale``, applies it and the K pages hold unscaled keys)."""
         assert num_heads % num_kv_heads == 0, f"num_heads {num_heads} must be divisible by num_kv_heads {num_kv_heads}"
         self.hidden_size = hidden_size
         self.num_heads = num_heads
         self.num_kv_heads = num_kv_heads
         self.head_dim = head_dim
         self.scale = head_dim**-0.5
+        if rope_mscale != 1.0:
+            self.scale *= rope_mscale * rope_mscale
         self.wq, self.wk, self.wv, self.wo = wq, wk, wv, wo
-        self.rope = FastRoPE(head_dim, max_seq_len, theta)
+        self.rope = FastRoPE(head_dim, max_seq_len, theta, inv_freq=rope_inv_freq)
         self.q_norm = FastRMSNorm(head_dim, q_norm, eps=rms_norm_eps)
         self.k_norm = FastRMSNorm(head_dim, k_norm, eps=rms_norm_eps)
         self.use_paged_attention = use_paged_attention
@@ -153,6 +181,8 @@ class Qwen3TransformerBlock:
         max_seq_len: int = 32768,
         theta: int = 1000000,
         use_paged_attention: bool = True,
+        rope_inv_freq: torch.Tensor | None = None,
+        rope_mscale: float = 1.0,
     ):
         self.num_attention_heads = num_attention_heads
         self.hidden_size = hidden_size
@@ -174,6 +204,8 @@ class Qwen3TransformerBlock:
             theta=theta,
             rms_norm_eps=rms_norm_eps,
             use_paged_attention=use_paged_attention,
+            rope_inv_freq=rope_inv_freq,
+            rope_mscale=rope_mscale,
         )
 
     def __call__(self, x, offset, cache: TinyKvCache, mask=None, lora=None):
@@ -196,7 +228,8 @@ def is_qwen3_moe_sparse_layer(args: Any, layer_idx: int) -> bool:
 class Qwen3ModelWeek3:
     """qwen3_week3.py:218-338."""
 
-    def __init__(self, mlx_model: Any, page_size: int = 128, enable_paged_attention: bool = True):
+    def __init__(self, mlx_model: Any, page_size: int = 128, enable_paged_attention: bool = True, max_context: int | None = None):
+        """``max_context``: the graph engines' context window (``set_max_context``); None keeps the default 8,192."""
         args = mlx_model.args
         self.num_hidden_layers = args.num_hidden_layers
         self.hidden_size = args.hidden_size
@@ -215,6 +248,14 @@ class Qwen3ModelWeek3:
             weight=packed(mlx_model.model.embed_tokens),
             use_custom_kernel=True,
         )
+        # One RoPE frequency table for the whole model when the config scales RoPE (YaRN): every site - operator path,
+        # decode, prefill and verify graphs - reads this tensor, so keys written at prefill and queries rotated at
+        # decode use identical angles.  None: plain RoPE, every site keeps its inline base^(-i/half).
+        self.rope_scaling = parse_rope_scaling(getattr(args, "rope_scaling", None), args.max_position_embeddings)
+        self.rope_inv_freq = None
+        if self.rope_scaling is not None:
+            self.rope_inv_freq = rope_inv_freq(args.head_dim, args.rope_theta, self.rope_scaling, self.embedding.weight.scales.device)
+        mscale = 1.0 if self.rope_scaling is None else self.rope_scaling.mscale
         self.layers_inner = []
         for index, layer in enumerate(mlx_model.model.layers[: self.num_hidden_layers]):
             attn = layer.self_attn
@@ -255,6 +296,8 @@ class Qwen3ModelWeek3:
                     max_seq_len=args.max_position_embeddings,
                     theta=args.rope_theta,
                     use_paged_attention=enable_paged_attention,
+                    rope_inv_freq=self.rope_inv_freq,
+                    rope_mscale=mscale,
                 )
             )
         self.norm = FastRMSNorm(args.hidden_size, weight=mlx_model.model.norm.weight, eps=args.rms_norm_eps)
@@ -277,6 +320,44 @@ class Qwen3ModelWeek3:
         self._paged = enable_paged_attention
         self.prefix_cache = None  # prefix_cache.PrefixCache over page_pools, once enable_prefix_cache() is called
         self.adapters = None  # lora.AdapterSet, once load_adapters() is called
+        if max_context is not None:
+            self.set_max_context(max_context)
+
+    @property
+    def max_context(self) -> int:
+        """The graph engines' context window: the longest request a decode, prefill or verify graph holds (requests
+        beyond it run operator by operator).  Backed by ``decode_graph_max_seq_len``."""
+        return self.decode_graph_max_seq_len
+
+    def set_max_context(self, tokens: int, batch_size: int = 1, device=None) -> None:
+        """Set the graph engines' context window to ``tokens`` (rounded up to whole pages).  A decode engine of
+        ``batch_size`` slots reserves ``(B + 1) * ceil(W / page) + 1`` pages per layer; a window whose reservation does
+        not fit the device's free memory is refused here, before anything is allocated or captured.  Only before the
+        first graph engine exists: captured graphs do not change their page tables."""
+        tokens = int(tokens)
+        if tokens <= 0:
+            raise ValueError(f"max_context must be positive (got {tokens})")
+        if self._decode_engines or self._prefill_engines or self._verify_engines:
+            raise RuntimeError("set_max_context: call it before the first decode, prefill or verify graph engine exists")
+        window = -(-tokens // self.page_size) * self.page_size
+        self._check_reservation(window, batch_size, device)
+        self.decode_graph_max_seq_len = window
+
+    def kv_reservation_bytes(self, window: int, batch_size: int = 1) -> int:
+        """Bytes of K and V pages a ``batch_size``-slot decode engine with context window ``window`` reserves."""
+        attn = self.layers_inner[0].self_attn
+        return kv_reservation_bytes(self.num_hidden_layers, attn.num_kv_heads, attn.head_dim, self.page_size, window, batch_size)
+
+    def _check_reservation(self, window: int, batch_size: int, device=None) -> None:
+        """Refuse (``MemoryError``, with the bytes needed) a decode-engine page reservation that does not fit the
+        device's free memory.  Slabs that already hold enough pages need nothing; a growing slab is allocated whole
+        while the old one is still alive, so the whole new size must be free."""
+        dev = torch.device(device if device is not None else self.embedding.weight.scales.device)
+        pages = kv_reservation_pages(window, self.page_size, batch_size)
+        if dev.type != "cuda" or all(p.capacity >= pages for p in self.page_pools):
+            return
+        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        check_kv_reservation(self.kv_reservation_bytes(window, batch_size), free, window, batch_size)
 
     def create_kv_cache(self) -> list[TinyKvCache]:
         """One logical cache per layer, all sharing that layer's pool."""
@@ -339,6 +420,7 @@ class Qwen3ModelWeek3:
         key = (batch_size, limit)
         if key not in self._decode_engines:
             dev = device if device is not None else self.embedding.weight.scales.device
+            self._check_reservation(limit, batch_size, dev)
             engine = DecodeEngine(self, batch_size, limit, dev)
             engine.reserve_pools((batch_size + 1) * engine.max_pages + 1)
             self._decode_engines[key] = engine
@@ -489,6 +571,41 @@ class Qwen3ModelWeek3:
             engine.prefill_chunk(inputs.reshape(-1), off, cache, adapter_id=adapter_id)
         return logits.clone()
 
+    # Operator-path calls are run as they come up to ONE_CALL_MAX_TOKENS rows while every activation and logits tensor
+    # stays below 2^31 elements (the kernels index elements with 32-bit ints there).  A longer prompt - a 131,072-token
+    # prefill under YaRN - is run as consecutive PREFILL_PIECE_TOKENS-row calls on the same cache: chunked prefill.
+    ONE_CALL_MAX_TOKENS = 32768
+    PREFILL_PIECE_TOKENS = 8192
+
+    def _needs_pieces(self, B: int, L: int, logits_to_keep: int | None) -> bool:
+        args = self.mlx_model.args
+        attn = self.layers_inner[0].self_attn
+        width = max(args.hidden_size, attn.num_heads * attn.head_dim, args.intermediate_size,
+                    getattr(args, "moe_intermediate_size", 0) * getattr(args, "num_experts_per_tok", 0))
+        keep = L if logits_to_keep is None else min(logits_to_keep, L)
+        return L > self.PREFILL_PIECE_TOKENS and (L > self.ONE_CALL_MAX_TOKENS or B * L * width >= 2**31 or B * keep * self.vocab_size >= 2**31)
+
+    def _prefill_in_pieces(self, inputs, offset, cache, logits_to_keep, adapter_ids):
+        """``self(inputs, ...)`` as consecutive calls of at most ``PREFILL_PIECE_TOKENS`` rows; returns the same rows."""
+        L = inputs.shape[1]
+        keep = L if logits_to_keep is None else logits_to_keep
+        if keep <= 0:
+            raise ValueError("logits_to_keep must be positive")
+        outs = []
+        for a in range(0, L, self.PREFILL_PIECE_TOKENS):
+            b = min(a + self.PREFILL_PIECE_TOKENS, L)
+            want = min(b - a, max(0, b - (L - keep)))  # rows of this piece among the last `keep`
+            if isinstance(offset, int):
+                off = offset + a
+            elif isinstance(offset, torch.Tensor):
+                off = offset + a
+            else:
+                off = [int(o) + a for o in offset]
+            out = self(inputs[:, a:b], off, cache, logits_to_keep=max(want, 1), adapter_ids=adapter_ids)
+            if want:
+                outs.append(out[:, -want:])
+        return outs[0] if len(outs) == 1 else torch.cat(outs, dim=1)
+
     def __call__(self, inputs, offset, cache: list[TinyKvCache], logits_to_keep: int | None = None, adapter_ids=None):
         """``adapter_ids``: one ``AdapterSet`` id per batch row (-1: the base model), after ``load_adapters``."""
         ids = self._adapter_rows(adapter_ids, inputs.shape[0])
@@ -498,6 +615,8 @@ class Qwen3ModelWeek3:
             out = self._graph_prefill(inputs, offset, cache, logits_to_keep, -1 if ids is None else ids[0])
             if out is not None:
                 return out
+        if inputs.dim() == 2 and self._needs_pieces(inputs.shape[0], inputs.shape[1], logits_to_keep):
+            return self._prefill_in_pieces(inputs, offset, cache, logits_to_keep, adapter_ids)
         h = self.embedding(inputs)
         row_ids = None if ids is None else self.adapters.row_ids(ids, inputs.shape[1])
         for index, (block, layer_cache) in enumerate(zip(self.layers_inner, cache)):

@@ -42,12 +42,20 @@ CONFIGS = {
 
 
 def make_args(name_or_dims, **overrides) -> SimpleNamespace:
+    """``rope_scaling`` (an override): a ``config.json`` entry such as ``{"rope_type": "yarn", "factor": 4.0,
+    "original_max_position_embeddings": 32768}``, checked by ``rope_scaling.parse_rope_scaling``; None is left out."""
     dims = dict(CONFIGS[name_or_dims]) if isinstance(name_or_dims, str) else dict(name_or_dims)
     dims.setdefault("rms_norm_eps", 1e-6)
     dims.setdefault("max_position_embeddings", 40960)
     dims.setdefault("rope_theta", 1000000)
     dims.setdefault("tie_word_embeddings", True)
     dims.update(overrides)
+    if dims.get("rope_scaling") is None:
+        dims.pop("rope_scaling", None)
+    else:
+        from .rope_scaling import parse_rope_scaling
+
+        dims["rope_scaling"] = parse_rope_scaling(dims["rope_scaling"], dims["max_position_embeddings"]).to_config()
     if dims.get("num_experts", 0) > 0:  # Qwen3-MoE keys (mlx_lm qwen3_moe.ModelArgs)
         dims.setdefault("num_experts_per_tok", 8)
         dims.setdefault("moe_intermediate_size", dims["intermediate_size"])

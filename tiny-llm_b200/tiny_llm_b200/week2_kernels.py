@@ -42,13 +42,15 @@ class FastRMSNorm:
 
 class FastRoPE:
     """week2_kernels.py:22-53 - ``offset`` may be an int, one int per batch
-    row, a 0-d tensor or a ``[B]`` tensor."""
+    row, a 0-d tensor or a ``[B]`` tensor.  ``inv_freq``: a float64 ``[dims / 2]`` device table of a scaled RoPE
+    (``rope_scaling.rope_inv_freq``) that replaces ``base``; None rotates by ``base^(-i / (dims / 2))``."""
 
-    def __init__(self, dims: int, seq_len: int, base: int = 10000, traditional: bool = False):
+    def __init__(self, dims: int, seq_len: int, base: int = 10000, traditional: bool = False, inv_freq: torch.Tensor | None = None):
         self.dims = dims
         self.seq_len = seq_len
         self.base = base
         self.traditional = traditional
+        self.inv_freq = inv_freq
 
     def __call__(self, x: torch.Tensor, offset: int | list[int] | torch.Tensor = 0) -> torch.Tensor:
         batch = x.shape[0]
@@ -64,6 +66,8 @@ class FastRoPE:
             raise ValueError("FastRoPE needs one offset per batch row")
         else:
             offsets = offset.to(device=x.device, dtype=torch.int32)
+        if self.inv_freq is not None:
+            return tiny_llm_ext_b200.rope_table(x.contiguous(), offsets.contiguous(), self.dims, self.inv_freq, self.traditional)
         return tiny_llm_ext_b200.rope(x.contiguous(), offsets.contiguous(), self.dims, self.base, self.traditional)
 
 
