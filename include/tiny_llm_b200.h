@@ -568,6 +568,29 @@ int tl_set_pdl(int enabled);
 int tl_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                       int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, void *stream);
 
+/* Prompt-lookup proposals (DESIGN.md section 14).  history (int32, device, `capacity` entries) holds s[0..length);
+ * the call first appends the n_appended (0..TL_NGRAM_MAX_APPEND) ids at `appended` (HOST memory: they travel as
+ * kernel arguments, no copy) so that s = s[0..L), L = length + n_appended <= capacity, then searches it:
+ *   c(e), e in [0, L-2]: the largest t <= min(n_max, e + 1) with s[e-t+1..e] == s[L-t..L-1] (0 if s[e] != s[L-1]);
+ *   e* maximises (c(e), e) over the e with c(e) >= n_min (the longest match, then the latest);
+ *   p_t = s'[e* + 1 + t], t < k, s' = s followed by p (a continuation past s repeats the matched period).
+ * out (int32, device, [2 + k]) receives c(e*), e*, p_0..p_{k-1}; with no match 0, -1 and k times -1.
+ * state (int32, device, TL_NGRAM_STATE_WORDS, 8-byte aligned, zeroed once by the caller) carries the cross-CTA
+ * reduction, which the call leaves zeroed, and the one-hot rows last written.  onehot (optional, dtype [k, vocab],
+ * device, filled with -inf once by the caller, used with one state only): the previous call's rows are cleared to
+ * -inf and row t gets 0 at p_t, so it holds exactly the current proposals as point masses (all -inf with no match),
+ * in O(k) writes.  1 <= k <= TL_NGRAM_MAX_K, 1 <= n_min <= n_max <= TL_NGRAM_MAX_N, and with onehot
+ * 1 <= vocab <= TL_NGRAM_MAX_VOCAB (the vocabularies tl_speculative_sample takes).  grid: the number of CTAs, 0 for
+ * ceil((L - 1) / TL_NGRAM_TILE); the outputs do not depend on it.  One launch, no synchronisation: graph-capturable. */
+#define TL_NGRAM_MAX_K 7
+#define TL_NGRAM_MAX_N 8
+#define TL_NGRAM_MAX_APPEND 8
+#define TL_NGRAM_TILE 1024
+#define TL_NGRAM_STATE_WORDS 12
+#define TL_NGRAM_MAX_VOCAB TL_SPECULATIVE_SAMPLE_MAX_VOCAB
+int tl_ngram_propose(int32_t *history, int capacity, int length, const int32_t *appended, int n_appended, int k, int n_min,
+                     int n_max, int32_t *out, int32_t *state, void *onehot, int vocab, int dtype, int grid, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

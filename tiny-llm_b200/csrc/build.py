@@ -36,6 +36,7 @@ SOURCES = [
     "decode_attention_fused.cu",
     "sampling.cu",
     "spec_sample.cu",
+    "ngram.cu",
     "logprobs.cu",
     "constrained.cu",
     "moe.cu",

@@ -458,6 +458,26 @@ int tl_log_rows(const void *src, void *dst, const int32_t *out_index, int capaci
     return launch_log_rows(src, dst, out_index, capacity, bytes, as_stream(stream));
 }
 
+int tl_ngram_propose(int32_t *history, int capacity, int length, const int32_t *appended, int n_appended, int k, int n_min, int n_max,
+                     int32_t *out, int32_t *state, void *onehot, int vocab, int dtype, int grid, void *stream) {
+    if (k < 1 || k > TL_NGRAM_MAX_K) return fail(TL_EINVAL, "ngram_propose: k must be in [1, %d]", TL_NGRAM_MAX_K);
+    if (n_min < 1 || n_min > n_max || n_max > TL_NGRAM_MAX_N)
+        return fail(TL_EINVAL, "ngram_propose: need 1 <= n_min <= n_max <= %d", TL_NGRAM_MAX_N);
+    if (n_appended < 0 || n_appended > TL_NGRAM_MAX_APPEND)
+        return fail(TL_EINVAL, "ngram_propose: at most %d appended tokens", TL_NGRAM_MAX_APPEND);
+    if (length < 0 || capacity < 0 || static_cast<long long>(length) + n_appended > capacity)
+        return fail(TL_EINVAL, "ngram_propose: %d + %d tokens exceed the history's capacity %d", length, n_appended, capacity);
+    if (grid < 0) return fail(TL_EINVAL, "ngram_propose: grid must be >= 0");
+    if (!history || !out || !state || (n_appended > 0 && !appended)) return fail(TL_EINVAL, "ngram_propose: null pointer");
+    if (reinterpret_cast<uintptr_t>(state) % 8 != 0) return fail(TL_EINVAL, "ngram_propose: state must be 8-byte aligned");
+    if (onehot) {
+        if (!float_dtype(dtype)) return fail(TL_EDTYPE, "ngram_propose: expected float32, float16, or bfloat16");
+        if (vocab < 1 || vocab > TL_NGRAM_MAX_VOCAB) return fail(TL_EINVAL, "ngram_propose: vocab must be in [1, %d]", TL_NGRAM_MAX_VOCAB);
+    }
+    return launch_ngram_propose(history, length, appended, n_appended, k, n_min, n_max, out, state, onehot, vocab, dtype, grid,
+                                as_stream(stream));
+}
+
 int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                               const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks, uint32_t *reach,
                               void *stream) {

@@ -66,6 +66,11 @@ int launch_speculative_sample(const void *target, const void *draft, const int32
                               int rows, int vocab, int dtype, cudaStream_t st);
 int launch_log_rows(const void *src, void *dst, const int32_t *out_index, int capacity, long long bytes, cudaStream_t st);
 
+// ngram.cu: prompt-lookup proposals, one launch over ngram_propose_grid CTAs unless `grid` > 0
+int ngram_propose_grid(int length, int n_appended);
+int launch_ngram_propose(int32_t *history, int length, const int32_t *appended, int n_appended, int k, int n_min, int n_max, int32_t *out,
+                         int32_t *state, void *onehot, int vocab, int dtype, int grid, cudaStream_t st);
+
 int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                           int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, cudaStream_t st);
 

@@ -51,6 +51,12 @@ __all__ = [
     "speculative_sample",
     "SPECULATIVE_SAMPLE_MAX_VOCAB",
     "log_rows",
+    "ngram_propose",
+    "NGRAM_MAX_K",
+    "NGRAM_MAX_N",
+    "NGRAM_MAX_APPEND",
+    "NGRAM_TILE",
+    "NGRAM_STATE_WORDS",
     "constraint_token_masks",
     "logprobs",
     "LOGPROBS_MAX_N",
@@ -117,6 +123,7 @@ _SIGNATURES = {
     "tl_sample": (_I, [_VP] * 7 + [_I] * 3 + [_VP]),
     "tl_speculative_sample": (_I, [_VP] * 9 + [_I] * 3 + [_VP]),
     "tl_log_rows": (_I, [_VP] * 3 + [_I, _LL, _VP]),
+    "tl_ngram_propose": (_I, [_VP, _I, _I, _VP] + [_I] * 4 + [_VP] * 3 + [_I] * 3 + [_VP]),
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
@@ -834,6 +841,52 @@ def log_rows(src, dst, out_index, stream=None):
     _gpu("log_rows", src, dst, out_index)
     _check(_lib.tl_log_rows(src.data_ptr(), dst.data_ptr(), out_index.data_ptr(), dst.shape[0], src.numel() * src.element_size(),
                             _stream_ptr(stream, src)))
+
+
+NGRAM_MAX_K = 7
+NGRAM_MAX_N = 8
+NGRAM_MAX_APPEND = 8
+NGRAM_TILE = 1024
+NGRAM_STATE_WORDS = 12
+
+
+def ngram_propose(history, length, appended, k, n_min, n_max, out, state, onehot=None, grid=0, stream=None):
+    """Prompt-lookup proposals (``tl_ngram_propose``, DESIGN.md section 14): append the host ids ``appended`` (at most
+    ``NGRAM_MAX_APPEND``, passed by value) to ``history`` (int32 ``[capacity]``, holding ``length`` tokens), then
+    write into ``out`` (int32 ``[2 + k]``) the longest-then-latest match length c (0: no match), its end e (-1) and the
+    k tokens that followed it (-1s).  ``state`` (int32 ``[NGRAM_STATE_WORDS]``, zeroed once) belongs to one history
+    and one ``onehot`` (``[k, vocab]`` float, filled with -inf once), whose rows then hold exactly 0 at each current
+    proposal and -inf elsewhere.  ``grid`` > 0 fixes the number of CTAs (the result does not depend on it).  No host
+    synchronisation: the call captures into a CUDA graph.  Returns ``out``."""
+    appended = [int(t) for t in appended]
+    if not isinstance(k, int) or not 1 <= k <= NGRAM_MAX_K:
+        raise RuntimeError(f"ngram_propose: k must be in [1, {NGRAM_MAX_K}]")
+    if not (isinstance(n_min, int) and isinstance(n_max, int) and 1 <= n_min <= n_max <= NGRAM_MAX_N):
+        raise RuntimeError(f"ngram_propose: need 1 <= n_min <= n_max <= {NGRAM_MAX_N}")
+    if len(appended) > NGRAM_MAX_APPEND:
+        raise RuntimeError(f"ngram_propose: at most {NGRAM_MAX_APPEND} appended tokens")
+    if history.dtype != torch.int32 or history.dim() != 1:
+        raise RuntimeError("ngram_propose: history must be int32 [capacity]")
+    if not (isinstance(length, int) and 0 <= length and length + len(appended) <= history.shape[0]):
+        raise RuntimeError(f"ngram_propose: {length} + {len(appended)} tokens exceed the history's capacity {history.shape[0]}")
+    if out.dtype != torch.int32 or tuple(out.shape) != (2 + k,):
+        raise RuntimeError(f"ngram_propose: out must be int32 [{2 + k}]")
+    if state.dtype != torch.int32 or tuple(state.shape) != (NGRAM_STATE_WORDS,):
+        raise RuntimeError(f"ngram_propose: state must be int32 [{NGRAM_STATE_WORDS}]")
+    named = dict(history=history, out=out, state=state)
+    vocab, dtype = 0, 0
+    if onehot is not None:
+        if onehot.dtype not in _FLOATS or onehot.dim() != 2 or onehot.shape[0] != k:
+            raise RuntimeError(f"ngram_propose: onehot must be float [{k}, vocab]")
+        vocab, dtype = onehot.shape[1], _DTYPE_CODE[onehot.dtype]
+        named["onehot"] = onehot
+    _contig("ngram_propose", **named)
+    _gpu("ngram_propose", *named.values())
+    ids = (ctypes.c_int32 * NGRAM_MAX_APPEND)(*appended)
+    _check(_lib.tl_ngram_propose(history.data_ptr(), history.shape[0], length, ids, len(appended), k, n_min, n_max, out.data_ptr(),
+                                 state.data_ptr(), None if onehot is None else onehot.data_ptr(), vocab, dtype, grid,
+                                 _stream_ptr(stream, history)))
+    return out
 
 
 def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None):

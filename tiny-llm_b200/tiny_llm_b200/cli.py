@@ -14,6 +14,8 @@ see checkpoint.py; there is no hub download here).
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3 --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
         (speculative sampling: the same ids as the seeded sampled run without the draft)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-lookup 4 --prompt-lookup-ngram 2:3 --prompt-ids 5,17,3,9,5,17
+        (prompt-lookup speculative decoding: proposals from the request's own tokens, same ids as greedy)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
         (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
     python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
@@ -185,13 +187,17 @@ def cmd_generate(args) -> int:
     ids = _prompt_ids(args, tokenizer, args.prompt)
     sampler = sampling = None
     penalties = _penalties(args)
-    if (args.draft_model or args.draft_synthetic) and args.regex is not None:
+    drafted = bool(args.draft_model or args.draft_synthetic)
+    speculative = drafted or args.prompt_lookup is not None
+    if drafted and args.prompt_lookup is not None:
+        raise SystemExit("give one proposer: a draft (--draft-model / --draft-synthetic) or --prompt-lookup, not both")
+    if speculative and args.regex is not None:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --regex")
     constraint = _constraint(args, model, tokenizer, device)
     if constraint is not None:
         penalties["constraint"] = constraint
     if args.sampler_temp != 0 or penalties:
-        if device.type == "cuda" or penalties or args.draft_model or args.draft_synthetic:  # the seeded kernel
+        if device.type == "cuda" or penalties or speculative:  # the seeded kernel
             sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed, **penalties)
         else:
             sampler = make_sampler(args.sampler_temp, top_p=args.sampler_top_p, top_k=args.sampler_top_k)
@@ -208,8 +214,8 @@ def cmd_generate(args) -> int:
     eos = getattr(tokenizer, "eos_token_id", None)
     if constraint is not None and args.synthetic:
         eos = constraint.vocabulary.eos_ids[0]
-    if args.draft_model or args.draft_synthetic:
-        from .generate import speculative_generate_ids
+    if speculative:
+        from .generate import _check_prompt_lookup, prompt_lookup_generate_ids, speculative_generate_ids
 
         if args.adapter is not None or getattr(model, "adapters", None) is not None:
             raise SystemExit("speculative decoding does not take adapters: drop --lora / --synthetic-lora / --adapter")
@@ -220,13 +226,28 @@ def cmd_generate(args) -> int:
             raise SystemExit("speculative decoding does not report log-probabilities: drop --logprobs")
         if args.draft_model and args.draft_synthetic:
             raise SystemExit("give one draft: --draft-model or --draft-synthetic, not both")
+        eos_ids = () if eos is None else (eos,)
+        if args.prompt_lookup is not None:
+            try:
+                ngram = _check_prompt_lookup(args.prompt_lookup, [int(n) for n in args.prompt_lookup_ngram.split(":")])
+            except ValueError as exc:
+                raise SystemExit(f"--prompt-lookup K --prompt-lookup-ngram MIN:MAX: {exc}") from None
+            produced, stats = prompt_lookup_generate_ids(model, ids, args.max_new_tokens, proposal_length=args.prompt_lookup,
+                                                         ngram=ngram, eos_token_ids=eos_ids, device=device, on_token=emit,
+                                                         sampling=sampling)
+            proposed, accepted = sum(p for p, _ in stats), sum(a for _, a in stats)
+            matched = sum(1 for p, _ in stats if p)
+            print(f"\nspeculative: {len(stats)} rounds, {accepted}/{proposed} proposals accepted"
+                  + (f" ({accepted / proposed:.2f})" if proposed else "") + f", {matched} rounds matched", file=sys.stderr)
+            print()
+            return 0
         draft_args = argparse.Namespace(**{**vars(args), "model": args.draft_model, "synthetic": args.draft_synthetic})
         draft_ns, draft_tokenizer, draft_name = _load(draft_args, device)
         if tokenizer is not None and draft_tokenizer is not None and tokenizer.get_vocab() != draft_tokenizer.get_vocab():
             raise SystemExit("draft and target tokenizers use different token ids")
         draft = _model(args, draft_ns, draft_name)
         produced, stats = speculative_generate_ids(draft, model, ids, args.max_new_tokens, proposal_length=args.proposal_length,
-                                                   eos_token_ids=() if eos is None else (eos,), device=device, on_token=emit,
+                                                   eos_token_ids=eos_ids, device=device, on_token=emit,
                                                    sampling=sampling)
         proposed, accepted = sum(p for p, _ in stats), sum(a for _, a in stats)
         print(f"\nspeculative: {len(stats)} rounds, {accepted}/{proposed} proposals accepted"
@@ -368,6 +389,10 @@ def main(argv=None) -> int:
     sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
     sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")
     sub.choices["generate"].add_argument("--proposal-length", type=int, default=4, help="draft tokens proposed per round")
+    sub.choices["generate"].add_argument("--prompt-lookup", type=int, default=None, metavar="K",
+                                         help="prompt-lookup speculative decoding: K (1..7) proposals per round from the request's own tokens")
+    sub.choices["generate"].add_argument("--prompt-lookup-ngram", default="2:3", metavar="MIN:MAX",
+                                         help="suffix lengths prompt lookup matches (1 <= MIN <= MAX <= 8)")
     sub.choices["batch"].add_argument("--prompts-file", default=None)
     sub.choices["batch"].add_argument("--batch-size", type=int, default=5)
     sub.choices["batch"].add_argument("--prefill-step", type=int, default=128)

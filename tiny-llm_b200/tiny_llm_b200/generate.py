@@ -116,9 +116,10 @@ class _GenericRunner:
     the draft keeps the logits row each proposal was drawn from, and ``verify`` returns ``tl_speculative_sample``'s
     tokens on the target's T rows in place of the argmax predictions (DESIGN.md section 8d)."""
 
-    def __init__(self, model, draft_model, device, sampling=None):
+    def __init__(self, model, draft_model, device, sampling=None, proposer=None):
         self.model, self.draft_model, self.device = model, draft_model, device
         self.sampling = sampling
+        self.proposer = proposer  # prompt lookup (draft_model None): an ``NgramProposer`` or a stand-in
         self._draft_rows: list = []
 
     def round_fits(self, offset: int, k: int) -> bool:
@@ -155,6 +156,16 @@ class _GenericRunner:
                 break
         return out
 
+    def propose(self, committed, token):
+        """Prompt lookup: the proposer's k proposals after ``token`` as host ids, or None when the history has no match.
+        Sampled, the draft rows are the proposer's one-hot rows: q is the point mass at each proposal."""
+        match, ids, _, onehot = self.proposer(committed, token)
+        if not match:
+            return None
+        if self.sampling is not None:
+            self._draft_rows = list(onehot.split(1))
+        return ids
+
     def verify(self, token, proposals, offset, cache) -> tuple[list[int], list[int]]:
         """(target predictions for rows [token, *proposals], the proposals as host ids)."""
         ids = [token, *proposals]
@@ -185,8 +196,18 @@ class _GraphRunner(_GenericRunner):
         """The graph engines hold ``decode_graph_max_seq_len`` tokens; ``model(...)`` leaves its decode graph at the same
         limit.  A round appends up to ``offset + k + 1`` tokens to either cache (k proposals, the verify rows, the draft's
         catch-up), so past that point the protocol continues target-only through ``model(...)``, as greedy does."""
-        limit = min(self.model.decode_graph_max_seq_len, self.draft_model.decode_graph_max_seq_len)
+        limit = min(m.decode_graph_max_seq_len for m in (self.model, self.draft_model) if m is not None)
         return offset + k + 1 <= limit
+
+    def propose(self, committed, token):
+        """Prompt lookup: the proposals as the proposer's device tensor, which the verify graph reads device to device
+        (the host ids came back with the match length in the proposer's one read)."""
+        match, _, proposals, onehot = self.proposer(committed, token)
+        if not match:
+            return None
+        if self.sampling is not None:
+            self._draft_rows = onehot  # a buffer of fixed address: one sampled verify graph per k
+        return proposals
 
     def draft(self, token, offset, cache, k, eos):
         engine = self.draft_model.decode_engine(1, self.draft_model.decode_graph_max_seq_len)
@@ -209,11 +230,11 @@ def _graph_runner_applies(model, draft_model, device, k) -> bool:
 
     if not (1 <= k <= 7) or not (device is None or torch.device(device).type == "cuda"):
         return False
-    return all(isinstance(m, Qwen3ModelWeek3) and m.verify_applies() for m in (model, draft_model))
+    return all(isinstance(m, Qwen3ModelWeek3) and m.verify_applies() for m in (model, draft_model) if m is not None)
 
 
 def _rewind(cache, n: int) -> None:
-    if n:
+    if n and cache is not None:
         for layer in cache:
             layer.rewind(n)
 
@@ -229,14 +250,19 @@ def _check_offset(cache, expected: int, what: str) -> None:
 
 def _speculate(runner, model, draft_model, prompt_ids, max_new_tokens, proposal_length, eos, emit):
     """The reference protocol on token ids.  ``emit(ids)`` receives each accepted run; returns the per-round
-    (proposed, accepted) counts.  Every page of both caches goes back to its pool on return or on an exception."""
+    (proposed, accepted) counts.  Every page of both caches goes back to its pool on return or on an exception.
+    With ``draft_model`` None the proposals come from ``runner.propose`` (prompt lookup): there is no draft cache, and
+    a round whose history has no match is one target step, recorded as (0, 0)."""
     stats: list[tuple[int, int]] = []
     produced = [0]
+    committed = list(prompt_ids) if draft_model is None else None  # the proposer's view: prompt + emitted ids
 
     def out(ids) -> bool:  # emit up to the budget; True once it is spent
         ids = list(ids)[: max_new_tokens - produced[0]]
         if ids:
             produced[0] += len(ids)
+            if committed is not None:
+                committed.extend(ids)
             emit(ids)
         return produced[0] >= max_new_tokens
 
@@ -259,21 +285,36 @@ def _speculate(runner, model, draft_model, prompt_ids, max_new_tokens, proposal_
         if proposal_length == 0 or not runner.round_fits(offset, proposal_length):
             target_only(token, offset)
             return stats
-        draft_cache = draft_model.create_kv_cache()
-        draft_token = runner.prefill(draft_model, prompt_ids, draft_cache)
-        _check_offset(draft_cache, offset, "draft")
-        if draft_token in eos:
-            target_only(token, offset)
-            return stats
+        if draft_model is not None:
+            draft_cache = draft_model.create_kv_cache()
+            draft_token = runner.prefill(draft_model, prompt_ids, draft_cache)
+            _check_offset(draft_cache, offset, "draft")
+            if draft_token in eos:
+                target_only(token, offset)
+                return stats
         while True:
             if not runner.round_fits(offset, proposal_length):  # past the graph engines' length: target-only, as greedy
                 target_only(token, offset)
                 return stats
-            proposals = runner.draft(token, offset, draft_cache, proposal_length, eos)
+            if draft_cache is None:
+                proposals = runner.propose(committed, token)
+                if proposals is None:  # no match: one target step
+                    stats.append((0, 0))
+                    if out([token]):
+                        return stats
+                    token = runner.target_step(token, offset, cache)
+                    offset += 1
+                    _check_offset(cache, offset, "target")
+                    if token in eos:
+                        return stats
+                    continue
+            else:
+                proposals = runner.draft(token, offset, draft_cache, proposal_length, eos)
             predictions, drafted = runner.verify(token, proposals, offset, cache)
             n = len(drafted)  # tokens appended to the draft cache; the target appended n + 1
             _check_offset(cache, offset + n + 1, "target")
-            _check_offset(draft_cache, offset + n, "draft")
+            if draft_cache is not None:
+                _check_offset(draft_cache, offset + n, "draft")
             aligned = [token, *predictions[:-1]]
             checked = [token, *drafted]
             stop = None  # (index, terminal)
@@ -290,7 +331,8 @@ def _speculate(runner, model, draft_model, prompt_ids, max_new_tokens, proposal_
                 _rewind(cache, n + 1 - i)
                 _rewind(draft_cache, n - i)
                 _check_offset(cache, offset + i, "target")
-                _check_offset(draft_cache, offset + i, "draft")
+                if draft_cache is not None:
+                    _check_offset(draft_cache, offset + i, "draft")
                 if out(aligned[:i]) or terminal:
                     return stats
                 token = aligned[i]
@@ -305,8 +347,9 @@ def _speculate(runner, model, draft_model, prompt_ids, max_new_tokens, proposal_
             token = predictions[-1]
             if token in eos:
                 return stats
-            runner.draft(checked[-1], offset - 1, draft_cache, 1, ())  # the draft catches up on its last proposal
-            _check_offset(draft_cache, offset, "draft")
+            if draft_cache is not None:
+                runner.draft(checked[-1], offset - 1, draft_cache, 1, ())  # the draft catches up on its last proposal
+                _check_offset(draft_cache, offset, "draft")
     finally:
         _release_kv_cache(draft_cache)
         _release_kv_cache(cache)
@@ -363,6 +406,99 @@ def speculative_generate_ids(draft_model, model, prompt_ids, max_new_tokens: int
                 on_token(int(t))
 
     stats = _speculate(runner, model, draft_model, prompt_ids, max_new_tokens, proposal_length, eos, emit)
+    return produced, stats
+
+
+# ------------------------------------------------------------------ prompt lookup --
+# The proposals are the tokens that followed the latest, longest earlier occurrence of the history's last n tokens
+# (``tl_ngram_propose``, DESIGN.md section 14): no second model, no second cache and no draft pass.  The rounds are
+# ``_speculate``'s with ``draft_model`` None.
+
+
+class NgramProposer:
+    """Prompt lookup's proposer for one request.  The history (prompt, emitted ids, pending token) lives in a device
+    buffer: the prompt is uploaded once, and each call appends the ids emitted since the previous call as kernel
+    arguments, runs one ``ngram_propose`` launch and reads back the match length and the k proposals (one small
+    device->host read).  With ``onehot_dtype`` the proposer also keeps the ``[k, vocab]`` one-hot rows of its current
+    proposals (the draft distribution of the sampled verify pass) at a fixed address, in the model's logits dtype."""
+
+    def __init__(self, model, prompt_ids, k: int, ngram, device=None, sampled: bool = False, capacity: int = 0):
+        from extensions_b200 import tiny_llm_ext_b200 as ext
+
+        self._ext = ext
+        scales = model.embedding.weight.scales  # the activation dtype: that of the verify pass's logits
+        device = scales.device if device is None else device
+        self.k, (self.n_min, self.n_max) = k, ngram
+        prompt = torch.as_tensor([int(t) for t in prompt_ids], dtype=torch.int32)
+        self.length = prompt.numel()
+        self.history = torch.empty(max(capacity, self.length + ext.NGRAM_MAX_APPEND), dtype=torch.int32, device=device)
+        self.history[: self.length].copy_(prompt)
+        self.out = torch.empty(2 + k, dtype=torch.int32, device=device)
+        self.state = torch.zeros(ext.NGRAM_STATE_WORDS, dtype=torch.int32, device=device)
+        self.onehot = None
+        if sampled:
+            self.onehot = torch.full((k, model.vocab_size), float("-inf"), dtype=scales.dtype, device=device)
+
+    def __call__(self, committed, token):
+        """-> (match length, host proposals, device proposals [k], one-hot rows or None) for the history
+        ``committed + [token]``, of which the first ``self.length`` ids are already on the device."""
+        new = [*committed[self.length :], int(token)]
+        if self.length + len(new) > self.history.numel():  # grow by doubling, device to device
+            grown = torch.empty(2 * (self.length + len(new)), dtype=torch.int32, device=self.history.device)
+            grown[: self.length].copy_(self.history[: self.length])
+            self.history = grown
+        self._ext.ngram_propose(self.history, self.length, new, self.k, self.n_min, self.n_max, self.out, self.state, self.onehot)
+        self.length += len(new)
+        host = self.out.tolist()  # the round's one added device->host read
+        return host[0], host[2:] if host[0] else [], self.out[2:], self.onehot
+
+
+def _check_prompt_lookup(proposal_length, ngram) -> tuple[int, int]:
+    if not isinstance(proposal_length, int) or isinstance(proposal_length, bool) or not 1 <= proposal_length <= 7:
+        raise ValueError("proposal_length must be an integer in [1, 7] for prompt lookup")
+    try:
+        n_min, n_max = (int(n) for n in ngram)
+    except (TypeError, ValueError):
+        raise ValueError("ngram must be a pair (n_min, n_max)") from None
+    if not 1 <= n_min <= n_max <= 8 or any(isinstance(n, bool) or int(n) != n for n in ngram):
+        raise ValueError("ngram must satisfy 1 <= n_min <= n_max <= 8")
+    return n_min, n_max
+
+
+def prompt_lookup_generate_ids(model, prompt_ids, max_new_tokens: int, proposal_length: int = 4, ngram=(2, 3), eos_token_ids=(),
+                               device=None, on_token=None, sampling=None):
+    """Speculative generation of ``model`` whose proposals come from the request's own tokens (prompt lookup): each round
+    proposes the ``proposal_length`` tokens that followed the latest occurrence of the longest suffix of the history
+    of ``ngram = (n_min, n_max)`` tokens, on the device (``NgramProposer``), and verifies them with ``_speculate``'s
+    protocol.  A round with no match is one target step.  Returns ``(ids, stats)`` with per-round ``(proposed,
+    accepted)`` counts, ``(0, 0)`` for a round without a match.  CUDA Week-3 models verify in one captured graph per
+    round, reading the proposals device to device; MoE models and other devices verify through ``model(...)``.
+    Greedy (``sampling`` None or temperature 0), the ids equal ``greedy_generate_ids(model, ...)`` token for token.
+    Sampled, the draft distribution is the point mass at each proposal, so ``tl_speculative_sample`` accepts proposal
+    d with probability p_d and otherwise draws from p restricted to i != d: each emitted token is distributed as the
+    target's ``tl_sample`` draw at its position, but the ids need not equal ``greedy_generate_ids(model,
+    sampling=...)``'s (the acceptance and residual draws use their own Philox streams).  Constraints, penalties and
+    min-p are refused with ``ValueError``, as are ``proposal_length`` outside [1, 7] and ``ngram`` outside
+    ``1 <= n_min <= n_max <= 8``."""
+    ngram = _check_prompt_lookup(proposal_length, ngram)
+    sampling = _spec_sampling(sampling, None)
+    prompt_ids = [int(t) for t in prompt_ids]
+    if not prompt_ids:
+        raise ValueError("prompt must encode to at least one token")
+    eos = {int(t) for t in eos_token_ids}
+    fast = _graph_runner_applies(model, None, device, proposal_length)
+    capacity = len(prompt_ids) + min(max(max_new_tokens, 0), 1 << 16) + 8
+    proposer = NgramProposer(model, prompt_ids, proposal_length, ngram, device, sampling is not None, capacity)
+    runner = (_GraphRunner if fast else _GenericRunner)(model, None, device, sampling, proposer=proposer)
+    produced: list[int] = []
+
+    def emit(ids):
+        for t in ids:
+            produced.append(int(t))
+            if on_token is not None:
+                on_token(int(t))
+
+    stats = _speculate(runner, model, None, prompt_ids, max_new_tokens, proposal_length, eos, emit)
     return produced, stats
 
 
