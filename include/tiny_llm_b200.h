@@ -591,6 +591,27 @@ int tl_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offs
 int tl_ngram_propose(int32_t *history, int capacity, int length, const int32_t *appended, int n_appended, int k, int n_min,
                      int n_max, int32_t *out, int32_t *state, void *onehot, int vocab, int dtype, int grid, void *stream);
 
+/* Beam search's cross-beam selection (DESIGN.md section 15).  top_lp (float32) and top_ids (int32), device, [rows, n],
+ * are tl_logprobs' top-n lists of `rows` logits rows, n = num_beams + num_eos; cum (float32, device, num_beams
+ * entries) holds the rows' cumulative log-probabilities.  Candidate (r, k) scores s = fl(cum[r] + top_lp[r, k]); one
+ * with id -1, or whose s is -inf or NaN, is never taken.  The takeable candidates are walked in the order (s
+ * descending, r ascending, k ascending), p their position: an EOS id (eos_ids, HOST memory, passed by value) at
+ * p < num_beams finishes a hypothesis, one at p >= num_beams is skipped, and any other id becomes a live beam while
+ * fewer than num_beams are live.  result (int32, device, TL_BEAM_RESULT_WORDS) receives
+ *   [0] live count, [1] finished count,
+ *   [2 + j], [10 + j], [18 + j]: live beam j's parent row, token and new cum (float32 bits), in walk order,
+ *   [26 + f], [34 + f], [42 + f], [50 + f]: finished f's parent row, EOS id, sum (float32 bits) and walk position.
+ * cum is rewritten in place after every input is read: [0, live) the live beams' sums, [live, num_beams) -inf (an
+ * idle row of a later step is then never taken).  1 <= num_beams <= TL_BEAM_MAX_WIDTH, 1 <= rows <= num_beams,
+ * 0 <= num_eos <= TL_BEAM_MAX_EOS distinct non-negative ids, n == num_beams + num_eos.  One launch, no
+ * synchronisation: graph-capturable. */
+#define TL_BEAM_MAX_WIDTH 8
+#define TL_BEAM_MAX_EOS 4
+#define TL_BEAM_MAX_N (TL_BEAM_MAX_WIDTH + TL_BEAM_MAX_EOS)
+#define TL_BEAM_RESULT_WORDS (2 + 7 * TL_BEAM_MAX_WIDTH)
+int tl_beam_select(const float *top_lp, const int32_t *top_ids, float *cum, int rows, int n, int num_beams, const int32_t *eos_ids,
+                   int num_eos, int32_t *result, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

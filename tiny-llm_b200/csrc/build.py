@@ -37,6 +37,7 @@ SOURCES = [
     "sampling.cu",
     "spec_sample.cu",
     "ngram.cu",
+    "beam.cu",
     "logprobs.cu",
     "constrained.cu",
     "moe.cu",

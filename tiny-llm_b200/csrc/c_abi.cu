@@ -478,6 +478,21 @@ int tl_ngram_propose(int32_t *history, int capacity, int length, const int32_t *
                                 as_stream(stream));
 }
 
+int tl_beam_select(const float *top_lp, const int32_t *top_ids, float *cum, int rows, int n, int num_beams, const int32_t *eos_ids,
+                   int num_eos, int32_t *result, void *stream) {
+    if (num_beams < 1 || num_beams > TL_BEAM_MAX_WIDTH) return fail(TL_EINVAL, "beam_select: num_beams must be in [1, %d]", TL_BEAM_MAX_WIDTH);
+    if (num_eos < 0 || num_eos > TL_BEAM_MAX_EOS) return fail(TL_EINVAL, "beam_select: at most %d EOS ids", TL_BEAM_MAX_EOS);
+    if (rows < 1 || rows > num_beams) return fail(TL_EINVAL, "beam_select: rows must be in [1, num_beams = %d]", num_beams);
+    if (n != num_beams + num_eos) return fail(TL_EINVAL, "beam_select: n must be num_beams + num_eos = %d", num_beams + num_eos);
+    if (!top_lp || !top_ids || !cum || !result || (num_eos > 0 && !eos_ids)) return fail(TL_EINVAL, "beam_select: null pointer");
+    for (int e = 0; e < num_eos; ++e) {
+        if (eos_ids[e] < 0) return fail(TL_EINVAL, "beam_select: EOS ids must be non-negative");
+        for (int f = 0; f < e; ++f)
+            if (eos_ids[f] == eos_ids[e]) return fail(TL_EINVAL, "beam_select: EOS id %d given twice", eos_ids[e]);
+    }
+    return launch_beam_select(top_lp, top_ids, cum, rows, n, num_beams, eos_ids, num_eos, result, as_stream(stream));
+}
+
 int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                               const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks, uint32_t *reach,
                               void *stream) {

@@ -71,6 +71,10 @@ int ngram_propose_grid(int length, int n_appended);
 int launch_ngram_propose(int32_t *history, int length, const int32_t *appended, int n_appended, int k, int n_min, int n_max, int32_t *out,
                          int32_t *state, void *onehot, int vocab, int dtype, int grid, cudaStream_t st);
 
+// beam.cu: beam search's cross-beam selection, one CTA
+int launch_beam_select(const float *top_lp, const int32_t *top_ids, float *cum, int rows, int n, int width, const int32_t *eos_ids,
+                       int num_eos, int32_t *result, cudaStream_t st);
+
 int launch_decode_advance(int32_t *tokens, const int32_t *next_tokens, int32_t *offsets, int32_t *context_lens,
                           int32_t *out_log, int32_t *step_counter, int batch, int log_capacity, cudaStream_t st);
 

@@ -52,6 +52,7 @@ __all__ = [
     "SPECULATIVE_SAMPLE_MAX_VOCAB",
     "log_rows",
     "ngram_propose",
+    "beam_select",
     "NGRAM_MAX_K",
     "NGRAM_MAX_N",
     "NGRAM_MAX_APPEND",
@@ -124,6 +125,7 @@ _SIGNATURES = {
     "tl_speculative_sample": (_I, [_VP] * 9 + [_I] * 3 + [_VP]),
     "tl_log_rows": (_I, [_VP] * 3 + [_I, _LL, _VP]),
     "tl_ngram_propose": (_I, [_VP, _I, _I, _VP] + [_I] * 4 + [_VP] * 3 + [_I] * 3 + [_VP]),
+    "tl_beam_select": (_I, [_VP] * 3 + [_I] * 3 + [_VP, _I, _VP, _VP]),
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
@@ -886,6 +888,45 @@ def ngram_propose(history, length, appended, k, n_min, n_max, out, state, onehot
     _check(_lib.tl_ngram_propose(history.data_ptr(), history.shape[0], length, ids, len(appended), k, n_min, n_max, out.data_ptr(),
                                  state.data_ptr(), None if onehot is None else onehot.data_ptr(), vocab, dtype, grid,
                                  _stream_ptr(stream, history)))
+    return out
+
+
+BEAM_MAX_WIDTH = 8
+BEAM_MAX_EOS = 4
+BEAM_RESULT_WORDS = 2 + 7 * BEAM_MAX_WIDTH
+
+
+def beam_select(top_lp, top_ids, cum, num_beams, eos_ids, out, stream=None):
+    """Beam search's cross-beam selection (``tl_beam_select``, DESIGN.md section 15) over ``tl_logprobs``' top-N lists
+    ``top_lp`` float32 / ``top_ids`` int32 ``[rows, N]`` of ``rows <= num_beams`` rows, ``N = num_beams + len(eos_ids)``,
+    and the rows' cumulative log-probabilities ``cum`` (float32 ``[num_beams]``, device), which the launch rewrites in
+    place with the live beams' sums (-inf past them).  The EOS ids travel as kernel arguments.  Writes the packed result
+    into ``out`` (int32 ``[BEAM_RESULT_WORDS]``): live and finished counts, the live beams' (parent, token, cum bits) and
+    the finished records' (parent, EOS id, sum bits, walk position).  No host synchronisation: the call captures into a
+    CUDA graph.  Returns ``out``."""
+    eos = [int(t) for t in eos_ids]
+    if not isinstance(num_beams, int) or isinstance(num_beams, bool) or not 1 <= num_beams <= BEAM_MAX_WIDTH:
+        raise RuntimeError(f"beam_select: num_beams must be in [1, {BEAM_MAX_WIDTH}]")
+    if len(eos) > BEAM_MAX_EOS:
+        raise RuntimeError(f"beam_select: at most {BEAM_MAX_EOS} EOS ids")
+    n = num_beams + len(eos)
+    if top_lp.dtype != torch.float32 or top_lp.dim() != 2 or top_lp.shape[1] != n:
+        raise RuntimeError(f"beam_select: top_lp must be float32 [rows, {n}]")
+    rows = top_lp.shape[0]
+    if not 1 <= rows <= num_beams:
+        raise RuntimeError(f"beam_select: rows must be in [1, {num_beams}]")
+    if top_ids.dtype != torch.int32 or tuple(top_ids.shape) != (rows, n):
+        raise RuntimeError(f"beam_select: top_ids must be int32 [{rows}, {n}]")
+    if cum.dtype != torch.float32 or tuple(cum.shape) != (num_beams,):
+        raise RuntimeError(f"beam_select: cum must be float32 [{num_beams}]")
+    if out.dtype != torch.int32 or tuple(out.shape) != (BEAM_RESULT_WORDS,):
+        raise RuntimeError(f"beam_select: out must be int32 [{BEAM_RESULT_WORDS}]")
+    named = dict(top_lp=top_lp, top_ids=top_ids, cum=cum, out=out)
+    _contig("beam_select", **named)
+    _gpu("beam_select", *named.values())
+    ids = (ctypes.c_int32 * BEAM_MAX_EOS)(*eos)
+    _check(_lib.tl_beam_select(top_lp.data_ptr(), top_ids.data_ptr(), cum.data_ptr(), rows, n, num_beams, ids, len(eos), out.data_ptr(),
+                               _stream_ptr(stream, top_lp)))
     return out
 
 

@@ -16,6 +16,8 @@ see checkpoint.py; there is no hub download here).
         (speculative sampling: the same ids as the seeded sampled run without the draft)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-lookup 4 --prompt-lookup-ngram 2:3 --prompt-ids 5,17,3,9,5,17
         (prompt-lookup speculative decoding: proposals from the request's own tokens, same ids as greedy)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --num-beams 4 --num-return-sequences 2
+        (beam search: the returned hypotheses with their scores, best first)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
         (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
     python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
@@ -187,6 +189,8 @@ def cmd_generate(args) -> int:
     ids = _prompt_ids(args, tokenizer, args.prompt)
     sampler = sampling = None
     penalties = _penalties(args)
+    if args.num_beams is not None:
+        return _beam_search(args, model, tokenizer, ids, penalties, device)
     drafted = bool(args.draft_model or args.draft_synthetic)
     speculative = drafted or args.prompt_lookup is not None
     if drafted and args.prompt_lookup is not None:
@@ -262,6 +266,34 @@ def cmd_generate(args) -> int:
         print("logprobs (raw model distribution):")
         _print_logprobs(entries, tokenizer)
     return 0 if produced is not None else 1
+
+
+def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
+    """``generate --num-beams W``: one line per returned hypothesis (rank, score, sum of log-probabilities, length,
+    finished or not), then its text (its ids for ``--prompt-ids`` runs)."""
+    from .generate import beam_search_ids
+
+    refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("penalties or --min-p", bool(penalties)),
+               ("--regex", args.regex is not None), ("--logprobs", args.logprobs is not None),
+               ("adapters", args.adapter is not None or getattr(model, "adapters", None) is not None),
+               ("a draft", bool(args.draft_model or args.draft_synthetic)), ("--prompt-lookup", args.prompt_lookup is not None)]
+    for what, given in refused:
+        if given:
+            raise SystemExit(f"beam search is deterministic and takes no {what}: drop it or --num-beams")
+    eos = getattr(tokenizer, "eos_token_id", None)
+    try:
+        hyps = beam_search_ids(model, ids, args.max_new_tokens, num_beams=args.num_beams, length_penalty=args.length_penalty,
+                               early_stopping=args.early_stopping, num_return_sequences=args.num_return_sequences,
+                               eos_token_ids=() if eos is None else (eos,), device=device)
+    except ValueError as exc:
+        raise SystemExit(f"--num-beams: {exc}") from None
+    for rank, h in enumerate(hyps):
+        state = "finished" if h.finished else "unfinished"
+        print(f"beam {rank}: score {h.score:.6f}  sum_logprob {h.sum_logprob:.6f}  length {len(h.ids) + int(h.finished)}  {state}")
+    for rank, h in enumerate(hyps):
+        text = " ".join(str(t) for t in h.ids) if tokenizer is None or args.prompt_ids else tokenizer.decode(h.ids)
+        print(f"[{rank}] {text}")
+    return 0
 
 
 def cmd_batch(args) -> int:
@@ -389,6 +421,14 @@ def main(argv=None) -> int:
     sub.choices["generate"].add_argument("--draft-model", default=None, help="checkpoint directory of a draft model: speculative decoding")
     sub.choices["generate"].add_argument("--draft-synthetic", default=None, help="random-weight draft of a named shape (seed 0, as --synthetic)")
     sub.choices["generate"].add_argument("--proposal-length", type=int, default=4, help="draft tokens proposed per round")
+    sub.choices["generate"].add_argument("--num-beams", type=int, default=None, metavar="W",
+                                         help="deterministic beam search with W (1..8) beams; prints every returned hypothesis")
+    sub.choices["generate"].add_argument("--length-penalty", type=float, default=1.0,
+                                         help="beam search: a hypothesis of L tokens scores sum_logprob / L**A")
+    sub.choices["generate"].add_argument("--early-stopping", action="store_true",
+                                         help="beam search: stop as soon as num_beams hypotheses have finished")
+    sub.choices["generate"].add_argument("--num-return-sequences", type=int, default=1, metavar="N",
+                                         help="beam search: hypotheses to return (1..W)")
     sub.choices["generate"].add_argument("--prompt-lookup", type=int, default=None, metavar="K",
                                          help="prompt-lookup speculative decoding: K (1..7) proposals per round from the request's own tokens")
     sub.choices["generate"].add_argument("--prompt-lookup-ngram", default="2:3", metavar="MIN:MAX",

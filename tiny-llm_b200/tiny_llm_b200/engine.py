@@ -417,6 +417,13 @@ class DecodeEngine(_GraphEngine):
         self._con_host = None
         self._con_dev = None
         self._con_key = None
+        # beam_step(): the greedy step body, then tl_logprobs' top N = B + E of every row into fixed buffers and
+        # tl_beam_select, one graph per EOS tuple (the ids are kernel arguments, and they fix N); the beams' cumulative
+        # log-probabilities live in beam_cum, which the select rewrites in place; all on first use
+        self._graph_beam: dict = {}
+        self._beam_bufs: dict = {}
+        self.beam_cum = None
+        self.kernels_per_beam_step = 0
         if self.lora is not None:
             if rows_per_request != 1 or not self.fused:
                 raise ValueError("a model with adapters runs one row per slot on the fused decode step")
@@ -618,6 +625,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_con = {}
         self._graph_keep = None
         self._graph_spec = {}
+        self._graph_beam = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -667,6 +675,44 @@ class DecodeEngine(_GraphEngine):
             self._set_idle()
             self.step_counter.zero_()
             self._graph_keep = self._graph_of(keep_step, pool=self._graph.pool(), warmups=1)
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def beam_buffers(self, eos_ids: tuple):
+        """The fixed buffers of the beam step for ``eos_ids``: the beams' ``cum`` (float32 ``[B]``, shared by every EOS
+        tuple), ``tl_logprobs``' outputs ``[1, B(, N)]`` with their zero ``out_index``, and the packed select result."""
+        if self.beam_cum is None:
+            self.beam_cum = torch.zeros(self.B, dtype=torch.float32, device=self.device)
+        bufs = self._beam_bufs.get(eos_ids)
+        if bufs is None:
+            B, N, dev = self.B, self.B + len(eos_ids), self.device
+            lp = (torch.empty((1, B), dtype=torch.float32, device=dev), torch.empty((1, B), dtype=torch.float32, device=dev),
+                  torch.empty((1, B), dtype=torch.int32, device=dev), torch.empty((1, B, N), dtype=torch.int32, device=dev),
+                  torch.empty((1, B, N), dtype=torch.float32, device=dev))
+            bufs = self._beam_bufs[eos_ids] = (lp, torch.zeros(1, dtype=torch.int32, device=dev),
+                                                 torch.zeros(ext.BEAM_RESULT_WORDS, dtype=torch.int32, device=dev))
+        return bufs
+
+    def _ensure_beam_graph(self, eos_ids: tuple) -> None:
+        """Capture the beam step for ``eos_ids`` (same conditions as ``_ensure_sample_graph``).  Its warm-up runs the
+        select once, so ``beam_cum`` is kept aside and put back."""
+        if eos_ids in self._graph_beam:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+        lp, index, result = self.beam_buffers(eos_ids)
+        N = self.B + len(eos_ids)
+
+        def beam_step():
+            forward()
+            ext.logprobs(self.logits, None, None, N, out=lp, out_index=index)
+            ext.beam_select(lp[4][0], lp[3][0], self.beam_cum, self.B, eos_ids, result)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            kept = self.beam_cum.clone()
+            self._set_idle()
+            self._graph_beam[eos_ids] = self._graph_of(beam_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_beam_step = self._launches
+            self.beam_cum.copy_(kept)
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
     def _ensure_penalized_graph(self) -> None:
@@ -1140,6 +1186,27 @@ class DecodeEngine(_GraphEngine):
             return out
         _, lp, rank, ids, top = self._lp_log
         return out, (lp[:steps], rank[:steps], ids[:steps], top[:steps])
+
+
+    def beam_step(self, tokens, offsets, caches, eos_ids: tuple):
+        """One step of beam search over the B slots (``generate.beam_search_ids``): append ``tokens`` at ``offsets`` to
+        the slots' caches (``caches`` as for ``step``; an empty slot takes token 0 at offset 0 and its ``beam_cum`` entry
+        must be -inf), then choose the next beams from every row's top ``B + len(eos_ids)`` tokens and ``beam_cum``.
+        Returns the packed ``tl_beam_select`` result (int32 ``[BEAM_RESULT_WORDS]``, device), overwritten by the next
+        call; ``beam_cum`` then holds the new beams' sums."""
+        B = self.B
+        self._host_write_begin()
+        ctx = self._advance_host(caches, 1)
+        self._ensure_graph()
+        self.beam_buffers(eos_ids)
+        self._ensure_beam_graph(eos_ids)
+        self.meta_np[0:B] = tokens
+        self.meta_np[B : 2 * B] = offsets
+        self.meta_np[2 * B : 3 * B] = ctx
+        self._upload()
+        self._graph_beam[eos_ids].replay()
+        self.graph_replays += 1
+        return self._beam_bufs[eos_ids][2]
 
 
 class VerifyEngine(DecodeEngine):

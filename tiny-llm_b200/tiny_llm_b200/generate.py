@@ -3,9 +3,16 @@
 
 from __future__ import annotations
 
+import math
+from dataclasses import dataclass
+
+import numpy as np
 import torch
 
+from extensions_b200 import tiny_llm_ext_b200
+
 from .batch import greedy_tokens
+from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, token_logprobs
 from .lora import adapter_ids_of
 from .sampler import sample_tokens, token_state_row
@@ -547,3 +554,201 @@ def speculative_generate(draft_model, model, draft_tokenizer, tokenizer, prompt:
     text = detokenizer.text
     print(text)
     return text
+
+
+# ------------------------------------------------------------------ beam search --
+# Each step scores every live beam's top W + E tokens, ``tl_logprobs``' top-N lists, and ``tl_beam_select`` walks the
+# candidates of all beams in one order (DESIGN.md section 15).  Beam j decodes in slot j of a W-row step; a parent's
+# first child takes over the parent's caches and the others fork them (``paged_kv_cache.fork``: shared full pages, a
+# copied tail page).
+
+
+@dataclass
+class BeamHypothesis:
+    """One result of ``beam_search_ids``: the generated ids (an ending EOS is not included), the sum of their
+    log-probabilities (with the EOS's), ``sum_logprob / L**length_penalty`` with L the length including the EOS, and
+    whether the hypothesis ended in an EOS (False: cut by ``max_new_tokens``)."""
+
+    ids: list
+    sum_logprob: float
+    score: float
+    finished: bool
+
+
+def unpack_beam_result(words):
+    """The packed ``tl_beam_select`` result (``BEAM_RESULT_WORDS`` int32 words) as ``(live, finished)``: live beams
+    ``(parent, token, cum)`` and finished records ``(parent, eos id, sum, walk position)``, in walk order."""
+    w = np.asarray(words, dtype=np.int32)
+    f = w.view(np.float32)
+    M = tiny_llm_ext_b200.BEAM_MAX_WIDTH
+    a, b = 2, 2 + 3 * M
+    live = [(int(w[a + j]), int(w[a + M + j]), float(f[a + 2 * M + j])) for j in range(int(w[0]))]
+    finished = [(int(w[b + j]), int(w[b + M + j]), float(f[b + 2 * M + j]), int(w[b + 3 * M + j])) for j in range(int(w[1]))]
+    return live, finished
+
+
+def _beam_score(total: float, length: int, length_penalty: float) -> float:
+    return float(total) / (float(length) ** length_penalty)
+
+
+class _BeamRunner:
+    """Beam search's model actions through ``model(...)`` (any paged model, any device): a step is one call over the W
+    slots (``BatchingKvCache`` per layer) and eager ``logprobs`` + ``beam_select`` launches on its W rows."""
+
+    def __init__(self, model, width: int, eos: tuple, device):
+        self.model, self.W, self.eos, self.device = model, width, eos, device
+        self.N = width + len(eos)
+        self.cum = self.result = None
+
+    def _buffers(self, device):
+        if self.cum is None:
+            self.cum = torch.zeros(self.W, dtype=torch.float32, device=device)
+            self.result = torch.zeros(tiny_llm_ext_b200.BEAM_RESULT_WORDS, dtype=torch.int32, device=device)
+
+    def _select(self, rows):
+        _, _, _, ids, top = tiny_llm_ext_b200.logprobs(rows.contiguous(), None, None, self.N)
+        tiny_llm_ext_b200.beam_select(top, ids, self.cum, self.W, self.eos, self.result)
+        return self.result.tolist()  # the step's one device->host read
+
+    def first(self, row):
+        """Select from the prompt's last logits row ``[1, V]`` with ``cum = [0]``."""
+        self._buffers(row.device)
+        self.cum.zero_()
+        return self._select(row)
+
+    def step(self, tokens, offsets, caches):
+        y = torch.as_tensor(tokens, dtype=torch.int32, device=self.device).view(self.W, 1)
+        logits = self.model(y, list(offsets), caches, logits_to_keep=1)
+        return self._select(logits[:, -1, :])
+
+
+class _BeamGraphRunner(_BeamRunner):
+    """CUDA Week-3 models: every step after the first is one replay of the W-slot decode engine's beam step graph
+    (``DecodeEngine.beam_step``), whose ``beam_cum`` the first, eager select writes."""
+
+    def __init__(self, model, width: int, eos: tuple, device):
+        super().__init__(model, width, eos, device)
+        self.engine = model.decode_engine(width, model.decode_graph_max_seq_len)
+        _, _, self.result = self.engine.beam_buffers(eos)
+        self.cum = self.engine.beam_cum
+
+    def step(self, tokens, offsets, caches):
+        return self.engine.beam_step(tokens, offsets, caches, self.eos).tolist()
+
+
+def _beam_graph_applies(model, device, tokens: int) -> bool:
+    from .qwen3_week3 import Qwen3ModelWeek3
+
+    return (isinstance(model, Qwen3ModelWeek3) and model._paged and model.use_decode_graph is not False
+            and getattr(model, "adapters", None) is None and torch.device(device).type == "cuda"
+            and tokens <= model.decode_graph_max_seq_len)
+
+
+def _check_beam_args(num_beams, length_penalty, num_return_sequences, max_new_tokens, eos) -> None:
+    width, max_eos = tiny_llm_ext_b200.BEAM_MAX_WIDTH, tiny_llm_ext_b200.BEAM_MAX_EOS
+    if not isinstance(num_beams, int) or isinstance(num_beams, bool) or not 1 <= num_beams <= width:
+        raise ValueError(f"num_beams must be an integer in [1, {width}]")
+    if len(eos) > max_eos:
+        raise ValueError(f"beam search takes at most {max_eos} EOS ids")
+    if (not isinstance(num_return_sequences, int) or isinstance(num_return_sequences, bool)
+            or not 1 <= num_return_sequences <= num_beams):
+        raise ValueError("num_return_sequences must be an integer in [1, num_beams]")
+    if not math.isfinite(float(length_penalty)):
+        raise ValueError("length_penalty must be finite")
+    if not isinstance(max_new_tokens, int) or max_new_tokens < 0:
+        raise ValueError("max_new_tokens must be a non-negative integer")
+
+
+def beam_search_ids(model, prompt_ids, max_new_tokens: int, num_beams: int = 4, length_penalty: float = 1.0,
+                    early_stopping: bool = False, num_return_sequences: int = 1, eos_token_ids=(), device=None):
+    """Deterministic beam search of ``num_beams`` (1..8) beams (DESIGN.md section 15; ``tests/beam_ref.py`` states the
+    rule in plain loops).  Each step walks every live beam's top ``num_beams + len(eos_token_ids)`` tokens in the order
+    (score descending, beam, rank): an EOS among the first ``num_beams`` finishes a hypothesis, other tokens become the
+    next beams.  A hypothesis of L tokens (its EOS included) scores ``sum_logprob / L**length_penalty``; at most
+    ``num_beams`` finished ones are kept.  The search ends when no beam is left, when ``num_beams`` are kept and
+    ``early_stopping`` is set or no live beam's score beats the worst kept one, or after ``max_new_tokens`` steps, when
+    the live beams join the pool unfinished.  Returns the best ``num_return_sequences`` ``BeamHypothesis``, best first.
+    With ``num_beams=1`` and ``early_stopping=True`` the ids are ``greedy_generate_ids``'.
+    CUDA Week-3 models whose decode graph window holds prompt + ``max_new_tokens`` run each step as one replay of the
+    W-slot beam step graph; other paged models run the same protocol through ``model(...)``.  Refused with
+    ``ValueError`` before any work: ``num_beams`` outside 1..8, more than 4 EOS ids, ``num_return_sequences`` outside
+    1..num_beams, a non-finite ``length_penalty``, a negative ``max_new_tokens``, an empty prompt and non-paged caches."""
+    eos = tuple(dict.fromkeys(int(t) for t in eos_token_ids))
+    _check_beam_args(num_beams, length_penalty, num_return_sequences, max_new_tokens, eos)
+    prompt = [int(t) for t in prompt_ids]
+    if not prompt:
+        raise ValueError("prompt must encode to at least one token")
+    from .paged_kv_cache import TinyKvPagedCache, fork
+
+    cache = model.create_kv_cache()
+    if not all(isinstance(c, TinyKvPagedCache) for c in cache):
+        _release_kv_cache(cache)
+        raise ValueError("beam search needs paged KV caches (the Week-3 model)")
+    if max_new_tokens == 0:
+        _release_kv_cache(cache)
+        return []
+    W, alpha = num_beams, float(length_penalty)
+    if device is None:
+        scales = getattr(getattr(getattr(model, "embedding", None), "weight", None), "scales", None)
+        device = None if scales is None else scales.device
+    graph = device is not None and _beam_graph_applies(model, device, len(prompt) + max_new_tokens)
+    runner = (_BeamGraphRunner if graph else _BeamRunner)(model, W, eos, device)
+    kept: list = []  # (hypothesis, (step, walk position)), best first, at most W
+
+    def keep(hyp, order):
+        kept.append((hyp, order))
+        kept.sort(key=lambda h: (-h[0].score, h[1]))
+        del kept[W:]
+
+    beams: list = []  # (per-layer caches, ids) of the live beams, beam j in slot j
+    try:
+        logits = model(torch.as_tensor(prompt, dtype=torch.int32, device=device)[None], 0, cache, logits_to_keep=1)
+        words = runner.first(logits[:, -1, :])
+        beams, cache = [(cache, [])], None
+        slots = [BatchingKvCache(W) for _ in range(len(beams[0][0]))]
+        step = 0
+        while True:
+            live, finished = unpack_beam_result(words)
+            for parent, _, total, pos in finished:
+                ids = beams[parent][1]
+                keep(BeamHypothesis(list(ids), total, _beam_score(total, len(ids) + 1, alpha), True), (step, pos))
+            step += 1
+            if not live:
+                break
+            if len(kept) == W and (early_stopping or max(_beam_score(c, len(beams[p][1]) + 1, alpha) for p, _, c in live) <= kept[-1][0].score):
+                break
+            if step == max_new_tokens:
+                for j, (p, tok, c) in enumerate(live):
+                    ids = [*beams[p][1], tok]
+                    keep(BeamHypothesis(ids, c, _beam_score(c, len(ids), alpha), False), (max_new_tokens, j))
+                break
+            children: dict = {}
+            for p, _, _ in live:
+                children[p] = children.get(p, 0) + 1
+            for i, (caches, ids) in enumerate(beams):  # before the forks: the pages held stay within W beams' worth
+                if i not in children:
+                    _release_kv_cache(caches)
+                    beams[i] = (None, ids)
+            extra = [p for p in children if children[p] > 1]
+            forks = dict(zip(extra, fork([(beams[p][0], children[p] - 1) for p in extra])))
+            taken: set = set()
+            new = []
+            for p, tok, _ in live:
+                if p in taken:
+                    caches = forks[p].pop()
+                else:
+                    taken.add(p)
+                    caches = beams[p][0]
+                new.append((caches, [*beams[p][1], tok]))
+            beams = new
+            tokens, offsets = [0] * W, [0] * W
+            for j, (caches, ids) in enumerate(beams):
+                tokens[j], offsets[j] = ids[-1], len(prompt) + len(ids) - 1
+            for layer, slot in enumerate(slots):
+                slot.kv_caches = [beams[j][0][layer] if j < len(beams) else None for j in range(W)]
+            words = runner.step(tokens, offsets, slots)
+    finally:
+        _release_kv_cache(cache)
+        for caches, _ in beams:
+            _release_kv_cache(caches)
+    return [h for h, _ in kept[:num_return_sequences]]

@@ -18,6 +18,10 @@ back to the free list only when the last reference is dropped.  A write may only
 land in a page its writer alone references, and in a page the index holds as a
 partial node only at or beyond the indexed length (``check_write``).  Without an
 index no page is ever shared and every path above is unchanged.
+
+Beam search (``generate.beam_search_ids``) shares pages the same way: ``fork``
+gives a request's copies its full pages by reference and a private copy of its
+partly filled tail page, so no beam ever writes a page another beam holds.
 """
 
 from __future__ import annotations
@@ -636,3 +640,58 @@ class TinyKvPagedCache(TinyKvCache):
         self.page_ids.clear()
         lens.clear()
         self.offset = 0
+
+
+# ---- shared pages: copy on write and forks -----------------------------------------
+def adopt_with_copies(caches, pages, tokens: int, tails, copies: list) -> None:
+    """Start each fresh per-layer cache of ``caches`` on ``tokens`` tokens (``TinyKvPagedCache.adopt_prefix``): a
+    reference on each full page of ``pages[layer]`` and, when ``tokens`` reaches past them, a private page whose first
+    slots are copied from ``tails[layer]``.  The copy records ``(layer, source, destination, slots)`` are appended to
+    ``copies`` for one ``copy_pages`` call."""
+    P = caches[0].page_size
+    for layer, cache in enumerate(caches):
+        full = pages[layer]
+        dst = cache.adopt_prefix(full, [P] * len(full), tokens)
+        if dst is not None:
+            copies.append((layer, tails[layer], dst, tokens - P * len(full)))
+
+
+def copy_pages(pools, copies) -> None:
+    """Enqueue every copy record over the layers' slabs: one ``paged_cache_copy_prefix`` call, which splits into
+    launches of 128 records.  Stream order puts each copy ahead of every later write to its source page."""
+    if copies:
+        tiny_llm_ext_b200.paged_cache_copy_prefix([p._key_pages for p in pools], [p._value_pages for p in pools], copies)
+
+
+def fork(requests) -> list:
+    """For each ``(caches, n)`` of ``requests`` (a request's per-layer caches, all on the same pools): ``n`` new
+    per-layer caches that hold what ``caches`` holds.  Full pages are shared by reference; the partly filled tail page
+    is copied into a private page for each new cache (a tail that ends on a page boundary needs no copy).  All layers
+    of all new caches are copied by one ``copy_pages`` call.  Returns one list of new caches per request; on an
+    exception every page taken so far is given back."""
+    made: list = []
+    copies: list = []
+    pools = None
+    try:
+        for caches, n in requests:
+            pools = [c.pool for c in caches]
+            tokens = caches[0].offset  # settles appends the decode engine deferred
+            P = caches[0].page_size
+            full = tokens // P
+            pages = [c.page_ids[:full] for c in caches]
+            tails = [c.page_ids[full] if tokens % P else None for c in caches]
+            kids = []
+            made.append(kids)
+            for _ in range(n):
+                kid = [TinyKvPagedCache(pool) for pool in pools]
+                kids.append(kid)
+                adopt_with_copies(kid, pages, tokens, tails, copies)
+        if pools is not None:
+            copy_pages(pools, copies)
+    except BaseException:
+        for kids in made:
+            for kid in kids:
+                for c in kid:
+                    c.release()
+        raise
+    return made

@@ -27,7 +27,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass, field
 
-from extensions_b200 import tiny_llm_ext_b200
+from .paged_kv_cache import adopt_with_copies, copy_pages
 
 
 class _Node:
@@ -127,19 +127,16 @@ class PrefixCache:
         copy launch.  Returns the reused length, the offset the request prefills from."""
         if match.reused == 0:
             return 0
-        P = self.page_size
         cow = match.cow
         if cow is not None:  # pinned while the destinations are allocated, so no eviction can take the source
             for layer, pool in enumerate(self.pools):
                 pool.share_page(cow.pages[layer])
         try:
             copies = []
-            for layer, cache in enumerate(caches):
-                dst = cache.adopt_prefix([n.pages[layer] for n in match.shared], [P] * len(match.shared), match.reused)
-                if dst is not None:
-                    copies.append((layer, cow.pages[layer], dst, match.cow_slots))
-            if copies:
-                tiny_llm_ext_b200.paged_cache_copy_prefix([p._key_pages for p in self.pools], [p._value_pages for p in self.pools], copies)
+            pages = [[n.pages[layer] for n in match.shared] for layer in range(len(caches))]
+            tails = [None if cow is None else cow.pages[layer] for layer in range(len(caches))]
+            adopt_with_copies(caches, pages, match.reused, tails, copies)
+            copy_pages(self.pools, copies)
         finally:
             if cow is not None:  # the copy is enqueued ahead of every later write to the source page
                 for layer, pool in enumerate(self.pools):
