@@ -181,6 +181,21 @@ int tl_paged_attention_token_major_split(const void *q, const void *key_pages, c
                                          const int32_t *context_lens, void *out, int rows, int L, int num_pages, int page_size, int max_pages,
                                          float scale, int is_causal, int num_kv_heads, int num_heads, void *workspace, size_t workspace_bytes,
                                          void *stream);
+/* Shared-prefix decode attention: the result of tl_paged_attention at L = 1, causal, for every slot on its own block
+ * table, computed with each group's shared pages streamed once for all its query rows.  q, out [batch * Hq, 1, 128]
+ * bf16; pages, block_table [batch, max_pages] and context_lens [batch] as tl_paged_attention.  groups: num_groups
+ * int32 triples (first_slot, count, shared_pages) on the device; slots first_slot .. first_slot + count - 1 hold the
+ * same page ids in their first shared_pages table entries (not checked) and each row's context covers them.  Entries
+ * with count 0 are unused; slots in no group, and groups with shared_pages 0, attend all their keys in the suffix pass.
+ * groups_host: the same triples in host memory, checked here: groups in [0, batch), not overlapping, count * Hq / Hkv
+ * <= 128, 0 <= shared_pages <= max_pages.  bf16, D = 128, page_size a multiple of 64.  The launch grid and split
+ * counts depend only on (batch, heads, page_size, max_pages): one captured graph serves every grouping.  Three
+ * launches (prefix pass, suffix pass, merge); workspace of tl_shared_prefix_attention_workspace bytes. */
+size_t tl_shared_prefix_attention_workspace(int batch, int num_heads, int num_kv_heads, int page_size, int max_pages);
+int tl_shared_prefix_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                               const int32_t *context_lens, const int32_t *groups, const int32_t *groups_host, int num_groups,
+                               void *out, int batch, int D, int num_pages, int page_size, int max_pages, float scale,
+                               int num_kv_heads, int num_heads, int dtype, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- CUDA extension behind the same per-op semantics ---------------------
  * Device-driven K/V append for a decode batch (the batched form of

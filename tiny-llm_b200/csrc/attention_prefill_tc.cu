@@ -70,8 +70,27 @@ struct TcArgs {
     int splits, tiles_per_split;
     int out_token_major;  // out[(b, l, head), :] instead of [(b, head, l), :] (the layout the o-projection takes); split: the merge writes it
     float *ws_o, *ws_m, *ws_l;
+    // Shared-prefix attention (TC_PREFIX / TC_SUFFIX, L = 1): group descriptors (first_slot, count, shared_pages) x
+    // num_groups; the partial of split s of row r goes to slot r * split_stride + split_base + s.
+    const int32_t *groups;
+    int num_groups, split_base, split_stride;
 };
 
+// TC_PLAIN: tl_paged_attention.  TC_PREFIX: one CTA per (group, KV head, split) over the group's shared pages, its 128
+// MMA rows the count x G query rows of the group's slots (slot-major), unmasked.  TC_SUFFIX: one CTA per (slot, KV head,
+// split) over the slot's keys after its group's shared pages, as TC_PLAIN at L = 1 otherwise.
+enum { TC_PLAIN = 0, TC_PREFIX = 1, TC_SUFFIX = 2 };
+
+// The group of slot b: (first_slot, count, shared_pages), or (b, 1, 0) when no group with shared pages holds it.
+__device__ __forceinline__ int3 tc_group_of(const int32_t *groups, int num_groups, int b) {
+    for (int i = 0; i < num_groups; ++i) {
+        const int f = groups[3 * i], c = groups[3 * i + 1], sp = groups[3 * i + 2];
+        if (c > 0 && sp > 0 && b >= f && b < f + c) return make_int3(f, c, sp);
+    }
+    return make_int3(b, 1, 0);
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const TcArgs a) {
@@ -83,18 +102,24 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int qb = static_cast<int>(gridDim.x) / a.splits - 1 - static_cast<int>(blockIdx.x) / a.splits;  // long (late) query blocks first
     const int kvh = blockIdx.y, b = blockIdx.z;
     const int q0 = qb * a.RH;
+    const int cap = a.max_pages * a.page_size;
+    int3 grp = make_int3(b, 1, 0);
+    if (MODE != TC_PLAIN) grp = tc_group_of(a.groups, a.num_groups, b);
+    if (MODE == TC_PREFIX && grp.x != b) return;  // the group's first slot covers its rows
     // The causal shift uses the whole context, the block table clamps afterwards (attention_decode.cu).
     const int ctx = a.context_lens[b];
-    const int cap = a.max_pages * a.page_size;
-    // keys any row of this CTA may see: [0, key_end)
+    // keys any row of this CTA may see: [0, key_end); the prefix pass sees the shared pages, the suffix pass what follows
     const int last_row = min(q0 + a.RH, a.L) - 1;
-    const int key_end = ctx <= 0 ? 0 : min(a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx, cap);
+    const int shared_keys = min(grp.z * a.page_size, cap);
+    const int key_end = MODE == TC_PREFIX ? shared_keys
+                        : ctx <= 0 ? 0 : min(a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx, cap);
     const int all_tiles = (key_end + TC_BN - 1) / TC_BN;
+    const int tile_lo = MODE == TC_SUFFIX ? min(shared_keys / TC_BN, all_tiles) : 0;
     // Split-KV: the launch fixes the NUMBER of splits from the block table's width (the grid of a captured graph cannot
     // follow the context), the tiles are dealt out here from the request's real length, so a request far below the
     // bound still keeps all its splits busy.
-    const int tps = a.splits > 1 ? max((all_tiles + a.splits - 1) / a.splits, 1) : a.tiles_per_split;
-    const int t0 = min(split * tps, all_tiles);
+    const int tps = a.splits > 1 ? max((all_tiles - tile_lo + a.splits - 1) / a.splits, 1) : a.tiles_per_split;
+    const int t0 = tile_lo + min(split * tps, all_tiles - tile_lo);
     const int n_tiles = min(tps, all_tiles - t0);  // this CTA: global tiles t0 .. t0 + n_tiles - 1
 
     const uint32_t q_base = g_smem_u32(tsm + TC_Q_OFF);
@@ -129,8 +154,13 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             const int head0 = b * a.Hq + kvh * a.G;
             if (g_elect_one()) {
                 g_mbar_expect_tx(q_full, TC_Q_BYTES);
-                g_tma_load_3d(q_base, &tmap_q, 0, q0, head0, q_full);
-                g_tma_load_3d(q_base + TC_Q_BYTES / 2, &tmap_q, 64, q0, head0, q_full);
+                if (MODE == TC_PREFIX) {  // 4-D map [D, G, Hkv, B], box 64 x G x 1 x RH: row = slot * G + head
+                    g_tma_load_4d(q_base, &tmap_q, 0, 0, kvh, b, q_full);
+                    g_tma_load_4d(q_base + TC_Q_BYTES / 2, &tmap_q, 64, 0, kvh, b, q_full);
+                } else {
+                    g_tma_load_3d(q_base, &tmap_q, 0, q0, head0, q_full);
+                    g_tma_load_3d(q_base + TC_Q_BYTES / 2, &tmap_q, 64, q0, head0, q_full);
+                }
             }
             __syncwarp();
             const int32_t *table = a.block_table + static_cast<size_t>(b) * a.max_pages;
@@ -164,11 +194,20 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         // columns 8 j + 2 (t % 4) + {0, 1} of each (wgmma accumulator layout, wgmma.cuh).
         const int wg = wg_idx - 1;
         const int t = threadIdx.x & 127;
+        // TC_PREFIX: l = the row's slot inside the group (a row past the group's count is not written)
         int lq[2], g[2], l[2], limit[2];
         bool row_valid[2];
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
             const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * rr;  // MMA row 0..127
+            if (MODE == TC_PREFIX) {  // row = (slot grp.x + s, head g) of the group; every shared key precedes every row
+                l[rr] = r / a.G;
+                g[rr] = r - l[rr] * a.G, lq[rr] = 0;
+                const int c = l[rr] < grp.y ? a.context_lens[b + l[rr]] : 0;
+                row_valid[rr] = c > 0;
+                limit[rr] = !row_valid[rr] ? -1 : min(c, key_end) - 1;
+                continue;
+            }
             g[rr] = r / a.RH, lq[rr] = r - g[rr] * a.RH;                   // query head of the KV group, position inside the block
             l[rr] = q0 + lq[rr];
             row_valid[rr] = l[rr] < a.L && ctx > 0;
@@ -275,11 +314,12 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             float lt = l_sum[rr];
             lt += __shfl_xor_sync(0xffffffffu, lt, 1);
             lt += __shfl_xor_sync(0xffffffffu, lt, 2);
-            if (l[rr] >= a.L) continue;
-            const size_t out_row = static_cast<size_t>(b * a.Hq + kvh * a.G + g[rr]) * a.L + l[rr];
+            if (l[rr] >= (MODE == TC_PREFIX ? grp.y : a.L)) continue;
+            const size_t out_row = MODE == TC_PREFIX ? static_cast<size_t>(b + l[rr]) * a.Hq + kvh * a.G + g[rr]
+                                                     : static_cast<size_t>(b * a.Hq + kvh * a.G + g[rr]) * a.L + l[rr];
             const int col = 2 * (lane & 3);
-            if (a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
-                const size_t slot = out_row * a.splits + split;
+            if (MODE != TC_PLAIN || a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
+                const size_t slot = out_row * a.split_stride + a.split_base + split;
                 float *po = a.ws_o + slot * TC_D;
 #pragma unroll
                 for (int c8 = 0; c8 < TC_D / 8; ++c8)
@@ -320,6 +360,23 @@ bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_
 // masking stays per row inside a split; a split past a row's last visible key leaves an empty partial (m = -1e30, l = 0)
 // that the merge weights by zero.  The split count comes from the block table's width and the tiles are dealt out from
 // the real context inside the kernel, so a row's result does not depend on the graph's grid.
+// Split count: the one that minimises waves x (tiles per CTA + fixed cost) + merge launch, in units of one 64-key tile,
+// with one CTA slot per SM, ~3 tiles of fixed cost per CTA (set-up, Q load, epilogue) and 2 + splits / 4 for the merge
+// launch (it reads one partial per split and row).  base: CTAs per split; at most max_splits.
+static int tc_wave_splits(long long base, long long max_tiles, long long max_splits) {
+    const long long slots = sm_count();
+    long long best = 1, best_cost = -1;
+    for (long long sp = 1; sp <= max_splits && sp <= (max_tiles > 1 ? max_tiles : 1); ++sp) {
+        const long long tps = (max_tiles + sp - 1) / sp;
+        const long long real = (max_tiles + tps - 1) / tps;
+        if (real != sp) continue;
+        const long long waves = (base * sp + slots - 1) / slots;
+        const long long cost = 4 * waves * (tps + 3) + (sp > 1 ? 8 + sp : 0);  // x 4: quarter-tile units
+        if (best_cost < 0 || cost < best_cost) best_cost = cost, best = sp;
+    }
+    return static_cast<int>(best);
+}
+
 size_t paged_token_major_workspace(int rows, int L, int page_size, int max_pages) {
     if (static_cast<long long>(max_pages) * page_size <= PREFILL_SPLIT_MIN_KEYS) return 0;
     return static_cast<size_t>(rows) * L * PAGED_MAX_SPLITS * (TC_D + 2) * sizeof(float);
@@ -337,6 +394,13 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     a.tiles_per_page = page_size / TC_BN;
     a.scale_log2 = scale * TC_LOG2E;
     a.is_causal = is_causal;
+    static bool configured = false;
+    if (!configured) {
+        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
+            cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_PLAIN>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+            return fail(TL_ECUDA, "paged_attention: cannot raise shared memory limit");
+        configured = true;
+    }
     CUtensorMap mq, mk, mv;
     {
         const cuuint64_t dims[3] = {TC_D, static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(rows)};
@@ -349,37 +413,19 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
         if (int e = tc_map(&mk, kp, 4, dims, box)) return e;
         if (int e = tc_map(&mv, vp, 4, dims, box)) return e;
     }
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(paged_prefill_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
-            cudaFuncSetAttribute(paged_prefill_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
-            return fail(TL_ECUDA, "paged_attention: cannot raise shared memory limit");
-        configured = true;
-    }
     const int q_blocks = (L + a.RH - 1) / a.RH;
     const long long max_tiles = (static_cast<long long>(max_pages) * page_size + TC_BN - 1) / TC_BN;
     a.out_token_major = out_token_major ? 1 : 0;
     a.splits = 1;
+    a.split_stride = 1;
     a.tiles_per_split = static_cast<int>(max_tiles < 1 ? 1 : max_tiles);
     if (allow_split && ws != nullptr && (!out_token_major || static_cast<long long>(max_pages) * page_size > PREFILL_SPLIT_MIN_KEYS)) {
-        // Split count: the one that minimises waves x (tiles per CTA + fixed cost) + merge launch, in units of one 64-key
-        // tile, with one CTA slot per SM, ~3 tiles of fixed cost per CTA (set-up, Q load, epilogue) and 2 + splits / 4
-        // for the merge launch (it reads one partial per split and row).
-        const long long base = static_cast<long long>(q_blocks) * num_kv_heads * B;
-        const long long slots = sm_count();
         const size_t rows_total = static_cast<size_t>(rows) * L;
-        long long best = 1, best_cost = -1;
-        for (long long sp = 1; sp <= PAGED_MAX_SPLITS && sp <= (max_tiles > 1 ? max_tiles : 1); ++sp) {
-            const long long tps = (max_tiles + sp - 1) / sp;
-            const long long real = (max_tiles + tps - 1) / tps;
-            if (real != sp) continue;
-            if (sp > 1 && ws_bytes < rows_total * sp * (TC_D + 2) * sizeof(float)) break;
-            const long long waves = (base * sp + slots - 1) / slots;
-            const long long cost = 4 * waves * (tps + 3) + (sp > 1 ? 8 + sp : 0);  // x 4: quarter-tile units
-            if (best_cost < 0 || cost < best_cost) best_cost = cost, best = sp;
-        }
+        const long long fit = static_cast<long long>(ws_bytes / (rows_total * (TC_D + 2) * sizeof(float)));  // splits the workspace holds
+        const int best = tc_wave_splits(static_cast<long long>(q_blocks) * num_kv_heads * B, max_tiles,
+                                        fit < PAGED_MAX_SPLITS ? fit : PAGED_MAX_SPLITS);
         if (best > 1) {
-            a.splits = static_cast<int>(best), a.tiles_per_split = static_cast<int>((max_tiles + best - 1) / best);
+            a.splits = a.split_stride = best, a.tiles_per_split = static_cast<int>((max_tiles + best - 1) / best);
             a.ws_o = static_cast<float *>(ws);
             a.ws_m = a.ws_o + rows_total * best * TC_D;
             a.ws_l = a.ws_m + rows_total * best;
@@ -387,11 +433,83 @@ int launch_paged_prefill_tc(const void *q, const void *kp, const void *vp, const
     }
     dim3 grid(q_blocks * a.splits, num_kv_heads, B);
     if (grid.y > 65535 || grid.z > 65535) return fail(TL_EINVAL, "paged_attention: too many heads / requests for one launch");
-    cudaError_t le = launch_chained(paged_prefill_tc_kernel, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
+    cudaError_t le = launch_chained(paged_prefill_tc_kernel<TC_PLAIN>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
     if (le != cudaSuccess) return fail(TL_ECUDA, "paged_attention: launch failed: %s", cudaGetErrorString(le));
     TL_LAUNCH_CHECK("paged_prefill_tc");
     if (a.splits > 1) return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, rows * L, a.splits, st, L, num_heads, out_token_major);
     return TL_OK;
+}
+
+// ---------------------------------------------------------------- shared-prefix attention --
+// The split counts follow from the engine's shapes alone (one captured graph serves every grouping): the prefix pass
+// sizes its splits by the wave model for one group over the whole table, the suffix pass for every slot over the whole
+// table (a slot in no group attends all its keys there); the two share the PAGED_MAX_SPLITS slots of a row.
+void shared_prefix_splits(int batch, int num_kv_heads, int page_size, int max_pages, int *prefix, int *suffix) {
+    const long long max_tiles = static_cast<long long>(max_pages) * page_size / TC_BN;
+    *prefix = tc_wave_splits(num_kv_heads, max_tiles, PAGED_MAX_SPLITS / 2);
+    *suffix = tc_wave_splits(static_cast<long long>(batch) * num_kv_heads, max_tiles, PAGED_MAX_SPLITS - *prefix);
+}
+
+size_t shared_prefix_workspace(int batch, int num_heads, int num_kv_heads, int page_size, int max_pages) {
+    int sp, ss;
+    shared_prefix_splits(batch, num_kv_heads, page_size, max_pages, &sp, &ss);
+    return static_cast<size_t>(batch) * num_heads * (sp + ss) * (TC_D + 2) * sizeof(float);
+}
+
+int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl,
+                                   const int32_t *groups, int num_groups, void *out, int batch, int num_pages, int page_size,
+                                   int max_pages, float scale, int num_kv_heads, int num_heads, void *ws, cudaStream_t st) {
+    const int G = num_heads / num_kv_heads;
+    int sp, ss;
+    shared_prefix_splits(batch, num_kv_heads, page_size, max_pages, &sp, &ss);
+    const size_t rows_total = static_cast<size_t>(batch) * num_heads;
+    TcArgs a{};
+    a.block_table = bt, a.context_lens = cl, a.out = static_cast<bf16 *>(out);
+    a.L = 1, a.Hq = num_heads, a.Hkv = num_kv_heads, a.G = G, a.RH = TC_BM / G;
+    a.page_size = page_size, a.max_pages = max_pages, a.num_pages = num_pages;
+    a.tiles_per_page = page_size / TC_BN;
+    a.scale_log2 = scale * TC_LOG2E;
+    a.is_causal = 1;
+    a.groups = groups, a.num_groups = num_groups;
+    a.split_stride = sp + ss;
+    a.ws_o = static_cast<float *>(ws);
+    a.ws_m = a.ws_o + rows_total * a.split_stride * TC_D;
+    a.ws_l = a.ws_m + rows_total * a.split_stride;
+    const int max_tiles = max_pages * page_size / TC_BN;
+    static bool configured = false;
+    if (!configured) {
+        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_PREFIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess ||
+            cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_SUFFIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
+            return fail(TL_ECUDA, "shared_prefix_attention: cannot raise shared memory limit");
+        configured = true;
+    }
+    CUtensorMap mq4, mq3, mk, mv;
+    {
+        const cuuint64_t dims[4] = {TC_D, static_cast<cuuint64_t>(G), static_cast<cuuint64_t>(num_kv_heads), static_cast<cuuint64_t>(batch)};
+        const cuuint32_t box[4] = {64, static_cast<cuuint32_t>(G), 1, static_cast<cuuint32_t>(a.RH)};
+        if (int e = tc_map(&mq4, q, 4, dims, box)) return e;
+    }
+    {
+        const cuuint64_t dims[3] = {TC_D, 1, static_cast<cuuint64_t>(rows_total)};
+        const cuuint32_t box[3] = {64, static_cast<cuuint32_t>(a.RH), static_cast<cuuint32_t>(G)};
+        if (int e = tc_map(&mq3, q, 3, dims, box)) return e;
+    }
+    {
+        const cuuint64_t dims[4] = {TC_D, static_cast<cuuint64_t>(page_size), static_cast<cuuint64_t>(num_kv_heads), static_cast<cuuint64_t>(num_pages)};
+        const cuuint32_t box[4] = {64, TC_BN, 1, 1};
+        if (int e = tc_map(&mk, kp, 4, dims, box)) return e;
+        if (int e = tc_map(&mv, vp, 4, dims, box)) return e;
+    }
+    a.splits = sp, a.split_base = 0, a.tiles_per_split = (max_tiles + sp - 1) / sp;
+    cudaError_t le = launch_chained(paged_prefill_tc_kernel<TC_PREFIX>, dim3(sp, num_kv_heads, batch), dim3(TC_THREADS), TC_SMEM_BYTES, st,
+                                    mq4, mk, mv, a);
+    if (le != cudaSuccess) return fail(TL_ECUDA, "shared_prefix_attention: launch failed: %s", cudaGetErrorString(le));
+    TL_LAUNCH_CHECK("shared_prefix_attention_prefix");
+    a.splits = ss, a.split_base = sp, a.tiles_per_split = (max_tiles + ss - 1) / ss;
+    le = launch_chained(paged_prefill_tc_kernel<TC_SUFFIX>, dim3(ss, num_kv_heads, batch), dim3(TC_THREADS), TC_SMEM_BYTES, st, mq3, mk, mv, a);
+    if (le != cudaSuccess) return fail(TL_ECUDA, "shared_prefix_attention: launch failed: %s", cudaGetErrorString(le));
+    TL_LAUNCH_CHECK("shared_prefix_attention_suffix");
+    return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, static_cast<int>(rows_total), sp + ss, st, 1, num_heads, false);
 }
 
 }  // namespace tl

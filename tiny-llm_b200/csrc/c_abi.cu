@@ -6,6 +6,7 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <vector>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -384,6 +385,44 @@ int tl_paged_attention_token_major_split(const void *q, const void *key_pages, c
         return fail(TL_EINVAL, "paged_attention_token_major: needs the wgmma kernel (bf16, D = 128, pages a multiple of 64 slots)");
     return launch_paged_prefill_tc(q, key_pages, value_pages, block_table, context_lens, out, rows, L, num_pages, page_size, max_pages, scale,
                                    is_causal, num_kv_heads, num_heads, workspace != nullptr, workspace, workspace_bytes, as_stream(stream), true);
+}
+
+size_t tl_shared_prefix_attention_workspace(int batch, int num_heads, int num_kv_heads, int page_size, int max_pages) {
+    if (batch <= 0 || num_heads <= 0 || num_kv_heads <= 0 || page_size <= 0 || max_pages <= 0) return 0;
+    return shared_prefix_workspace(batch, num_heads, num_kv_heads, page_size, max_pages);
+}
+
+int tl_shared_prefix_attention(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                               const int32_t *context_lens, const int32_t *groups, const int32_t *groups_host, int num_groups,
+                               void *out, int batch, int D, int num_pages, int page_size, int max_pages, float scale,
+                               int num_kv_heads, int num_heads, int dtype, void *workspace, size_t workspace_bytes, void *stream) {
+    if (dtype != TL_BF16) return fail(TL_EDTYPE, "shared_prefix_attention: bfloat16 only");
+    if (D != PAGED_D) return fail(TL_EINVAL, "shared_prefix_attention: head dimension must be %d", PAGED_D);
+    if (num_heads <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0 || 128 % (num_heads / num_kv_heads) != 0)
+        return fail(TL_EINVAL, "shared_prefix_attention: num_heads / num_kv_heads must be a whole divisor of 128");
+    if (batch <= 0 || num_pages <= 0 || max_pages <= 0 || page_size <= 0 || page_size % 64 != 0)
+        return fail(TL_EINVAL, "shared_prefix_attention: bad shape (page_size must be a multiple of 64)");
+    if (num_groups < 0 || num_groups > batch) return fail(TL_EINVAL, "shared_prefix_attention: num_groups must be in [0, batch]");
+    if (!q || !key_pages || !value_pages || !block_table || !context_lens || !out || !workspace || (num_groups > 0 && (!groups || !groups_host)))
+        return fail(TL_EINVAL, "shared_prefix_attention: null pointer");
+    const int G = num_heads / num_kv_heads;
+    std::vector<char> taken(batch, 0);
+    for (int i = 0; i < num_groups; ++i) {
+        const int f = groups_host[3 * i], c = groups_host[3 * i + 1], sp = groups_host[3 * i + 2];
+        if (c == 0) continue;
+        if (c < 0 || f < 0 || f > batch - c) return fail(TL_EINVAL, "shared_prefix_attention: group %d leaves the slots [0, %d)", i, batch);
+        if (static_cast<long long>(c) * G > 128)
+            return fail(TL_EINVAL, "shared_prefix_attention: group %d has %d x %d query rows, more than 128", i, c, G);
+        if (sp < 0 || sp > max_pages) return fail(TL_EINVAL, "shared_prefix_attention: group %d shares %d pages, outside [0, %d]", i, sp, max_pages);
+        for (int b = f; b < f + c; ++b) {
+            if (taken[b]) return fail(TL_EINVAL, "shared_prefix_attention: slot %d is in two groups", b);
+            taken[b] = 1;
+        }
+    }
+    if (workspace_bytes < shared_prefix_workspace(batch, num_heads, num_kv_heads, page_size, max_pages))
+        return fail(TL_EINVAL, "shared_prefix_attention: workspace too small");
+    return launch_shared_prefix_attention(q, key_pages, value_pages, block_table, context_lens, groups, num_groups, out, batch, num_pages,
+                                          page_size, max_pages, scale, num_kv_heads, num_heads, workspace, as_stream(stream));
 }
 
 // ------------------------------------------------------------------ misc --

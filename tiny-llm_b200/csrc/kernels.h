@@ -179,6 +179,13 @@ int launch_paged_gqa_merge(const float *ws_o, const float *ws_m, const float *ws
 // more than this many keys: every shape below it keeps the unsplit launch and its bits.
 constexpr long long PREFILL_SPLIT_MIN_KEYS = 8192;
 size_t paged_token_major_workspace(int rows, int L, int page_size, int max_pages);
+// Shared-prefix decode attention (tl_shared_prefix_attention): the wgmma kernel's prefix pass over each group's shared
+// pages, its suffix pass over every slot's remaining keys, and paged_gqa_merge_kernel over both passes' partials.
+void shared_prefix_splits(int batch, int num_kv_heads, int page_size, int max_pages, int *prefix, int *suffix);
+size_t shared_prefix_workspace(int batch, int num_heads, int num_kv_heads, int page_size, int max_pages);
+int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl,
+                                   const int32_t *groups, int num_groups, void *out, int batch, int num_pages, int page_size,
+                                   int max_pages, float scale, int num_kv_heads, int num_heads, void *ws, cudaStream_t st);
 
 // attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the wgmma kernel does not take)
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,

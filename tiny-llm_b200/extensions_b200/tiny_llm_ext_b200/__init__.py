@@ -82,6 +82,8 @@ __all__ = [
     "LoraSite",
     "lora_apply",
     "lora_apply_route",
+    "shared_prefix_attention",
+    "shared_prefix_attention_workspace",
 ]
 
 _HERE = Path(__file__).resolve().parent
@@ -159,6 +161,8 @@ _SIGNATURES = {
     "tl_moe_combine": (_I, [_VP] * 4 + [_F, _VP, _VP] + [_I] * 4 + [_VP]),
     "tl_lora_apply_route": (_I, [_I, _I, _VP]),
     "tl_lora_apply": (_I, [_VP] * 6 + [_I, _I, _VP]),
+    "tl_shared_prefix_attention_workspace": (_SZ, [_I] * 5),
+    "tl_shared_prefix_attention": (_I, [_VP] * 7 + [_I, _VP] + [_I] * 5 + [_F] + [_I] * 3 + [_VP, _SZ, _VP]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -1148,6 +1152,48 @@ def quantized_matmul_route(M, N, K, lda, prologue, fused, use_simdgroup, dtype, 
                                           _DTYPE_CODE[dtype], addr(a), addr(b), addr(scales), addr(biases), *map(ctypes.byref, facts))
     _check(min(code, 0))
     return (code, *(f.value for f in facts))
+
+
+def shared_prefix_attention_workspace(batch: int, num_heads: int, num_kv_heads: int, page_size: int, max_pages: int) -> int:
+    """Bytes of workspace ``shared_prefix_attention`` takes for these shapes (its split partials)."""
+    return int(_lib.tl_shared_prefix_attention_workspace(int(batch), int(num_heads), int(num_kv_heads), int(page_size), int(max_pages)))
+
+
+def shared_prefix_attention(query, key_pages, value_pages, block_table, context_lens, groups, groups_host, scale, num_kv_heads, num_heads,
+                            workspace=None, stream=None):
+    """Decode attention (L = 1, causal) of ``batch`` slots where groups of consecutive slots share their leading pages
+    (``tl_shared_prefix_attention``, DESIGN.md section 16): each group's shared pages are streamed once for all its
+    query rows, every row then attends its own keys after them, and the partials are merged.  The result is
+    ``paged_attention(..., is_causal=True)``'s up to the order of the sums.  ``groups``: int32 ``[num_groups, 3]``
+    ``(first_slot, count, shared_pages)`` on the device (rows with count 0 unused); ``groups_host``: the same on the
+    host, checked by the C entry.  ``workspace``: a byte buffer of ``shared_prefix_attention_workspace`` bytes (a
+    fresh one when None)."""
+    op = "shared_prefix_attention"
+    if query.dtype != torch.bfloat16 or key_pages.dtype != torch.bfloat16 or value_pages.dtype != torch.bfloat16:
+        raise RuntimeError(f"{op}: q, key_pages and value_pages must be bfloat16")
+    if query.dim() != 3 or query.shape[1] != 1 or key_pages.dim() != 4 or key_pages.shape != value_pages.shape:
+        raise RuntimeError(f"{op}: q must be [B * H_q, 1, D] and the page tensors [P, H_kv, page_size, D]")
+    if groups.dtype != torch.int32 or groups.dim() != 2 or groups.shape[1] != 3 or tuple(groups_host.shape) != tuple(groups.shape):
+        raise RuntimeError(f"{op}: groups must be int32 [num_groups, 3] with a host copy of the same shape")
+    if groups_host.dtype != torch.int32 or groups_host.is_cuda or not groups_host.is_contiguous():
+        raise RuntimeError(f"{op}: groups_host must be a contiguous int32 CPU tensor")
+    batch = query.shape[0] // int(num_heads)
+    _int32(op, batch, context_lens=context_lens)
+    _block_table(op, block_table, batch)
+    _gpu(op, query, key_pages, value_pages, block_table, context_lens, groups)
+    _contig(op, query=query, key_pages=key_pages, value_pages=value_pages, block_table=block_table, context_lens=context_lens, groups=groups)
+    P, _, page_size, D = key_pages.shape
+    max_pages = block_table.shape[1]
+    need = shared_prefix_attention_workspace(batch, num_heads, num_kv_heads, page_size, max_pages)
+    if workspace is None:
+        workspace = _workspace(max(need, 1), query.device)
+    out = torch.empty_like(query)
+    _check(_lib.tl_shared_prefix_attention(query.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), block_table.data_ptr(),
+                                           context_lens.data_ptr(), groups.data_ptr(), groups_host.data_ptr(), groups.shape[0], out.data_ptr(),
+                                           batch, D, P, page_size, max_pages, float(scale), int(num_kv_heads), int(num_heads),
+                                           _DTYPE_CODE[query.dtype], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+                                           _stream_ptr(stream, query)))
+    return out
 
 
 def paged_attention_token_major_workspace(rows: int, L: int, page_size: int, max_pages: int) -> int:

@@ -8,8 +8,8 @@ from .basics import linear, silu, softmax
 from .batch import ContinuousBatcher, Request, batch_generate
 from .checkpoint import load_checkpoint, load_tokenizer, save_checkpoint
 from .embedding import Embedding, QuantizedEmbedding
-from .generate import (BeamHypothesis, beam_search_ids, greedy_generate_ids, prompt_lookup_generate_ids, simple_generate_with_kv_cache,
-                       speculative_generate, speculative_generate_ids)
+from .generate import (BeamHypothesis, ParallelSample, beam_search_ids, greedy_generate_ids, parallel_sample_ids, prompt_lookup_generate_ids,
+                       simple_generate_with_kv_cache, speculative_generate, speculative_generate_ids)
 from .kv_cache import BatchingKvCache, TinyKvCache, TinyKvFullCache
 from .layer_norm import RMSNorm
 from .moe import Moe, grouped_expert_linear, route_topk

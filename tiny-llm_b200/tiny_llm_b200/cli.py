@@ -20,6 +20,8 @@ see checkpoint.py; there is no hub download here).
         (beam search: the returned hypotheses with their scores, best first)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logprobs 5
         (each generated token's log-probability, rank and 5 most likely alternatives, after the text)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --num-samples 4 --sampler-temp 0.8 --seed 3
+        (parallel sampling: 4 seeded samples from one prefill, sample j uses seed + j)
     python -m tiny_llm_b200.cli score    --model /path/to/ckpt --prompt "The capital of France is Paris." [--logprobs 3]
         (teacher-forced log-probability of every prompt token and the prompt's perplexity)
     python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3,8;5,17,3,9" --prefix-cache
@@ -190,7 +192,11 @@ def cmd_generate(args) -> int:
     sampler = sampling = None
     penalties = _penalties(args)
     if args.num_beams is not None:
+        if args.num_samples is not None:
+            raise SystemExit("give --num-beams or --num-samples, not both")
         return _beam_search(args, model, tokenizer, ids, penalties, device)
+    if args.num_samples is not None:
+        return _parallel_sample(args, model, tokenizer, ids, penalties, device)
     drafted = bool(args.draft_model or args.draft_synthetic)
     speculative = drafted or args.prompt_lookup is not None
     if drafted and args.prompt_lookup is not None:
@@ -266,6 +272,41 @@ def cmd_generate(args) -> int:
         print("logprobs (raw model distribution):")
         _print_logprobs(entries, tokenizer)
     return 0 if produced is not None else 1
+
+
+def _parallel_sample(args, model, tokenizer, ids, penalties, device) -> int:
+    """``generate --num-samples N``: N seeded samples of the prompt from one prefill (sample j draws with seed
+    ``--seed + j``); per sample one line with its seed, finish reason and length, then its text (its ids for
+    ``--prompt-ids`` runs), then its log-probabilities with ``--logprobs``."""
+    from .generate import parallel_sample_ids, sample_seed
+    from .sampler import SamplingParams
+
+    refused = [("adapters", args.adapter is not None or getattr(model, "adapters", None) is not None),
+               ("a draft", bool(args.draft_model or args.draft_synthetic)), ("--prompt-lookup", args.prompt_lookup is not None)]
+    for what, given in refused:
+        if given:
+            raise SystemExit(f"parallel sampling takes no {what}: drop it or --num-samples")
+    if device.type != "cuda":  # without --num-samples a CPU run draws through make_sampler, which has no per-sample seeds
+        raise SystemExit("parallel sampling draws with the seeded CUDA sampling kernel: it needs a CUDA --device")
+    constraint = _constraint(args, model, tokenizer, device)
+    if constraint is not None:
+        penalties["constraint"] = constraint
+    sampling = SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed, **penalties)
+    eos = getattr(tokenizer, "eos_token_id", None)
+    if constraint is not None and args.synthetic:
+        eos = constraint.vocabulary.eos_ids[0]
+    try:
+        samples = parallel_sample_ids(model, [ids], args.num_samples, sampling, args.max_new_tokens,
+                                      eos_token_ids=() if eos is None else (eos,), logprobs=args.logprobs, device=device)[0]
+    except ValueError as exc:
+        raise SystemExit(f"--num-samples: {exc}") from None
+    for j, s in enumerate(samples):
+        print(f"sample {j}: seed {sample_seed(args.seed, j)}, {s.finish_reason}, {len(s.ids)} tokens")
+        print(" ".join(str(t) for t in s.ids) if tokenizer is None else tokenizer.decode(s.ids))
+        if s.logprobs is not None:
+            print("logprobs (raw model distribution):")
+            _print_logprobs(s.logprobs, tokenizer)
+    return 0
 
 
 def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
@@ -429,6 +470,8 @@ def main(argv=None) -> int:
                                          help="beam search: stop as soon as num_beams hypotheses have finished")
     sub.choices["generate"].add_argument("--num-return-sequences", type=int, default=1, metavar="N",
                                          help="beam search: hypotheses to return (1..W)")
+    sub.choices["generate"].add_argument("--num-samples", type=int, default=None, metavar="N",
+                                         help="N (1..16) seeded samples of the prompt from one prefill on a CUDA device; sample j uses seed + j")
     sub.choices["generate"].add_argument("--prompt-lookup", type=int, default=None, metavar="K",
                                          help="prompt-lookup speculative decoding: K (1..7) proposals per round from the request's own tokens")
     sub.choices["generate"].add_argument("--prompt-lookup-ngram", default="2:3", metavar="MIN:MAX",

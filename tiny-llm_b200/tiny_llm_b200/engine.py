@@ -45,6 +45,36 @@ from .paged_kv_cache import TinyKvPagedCache
 # the launch count, bounds the step.
 FUSED_ATTENTION_MAX_SLOT_TOKENS = 16384
 
+# Grouped decode attention (tl_shared_prefix_attention, DESIGN.md section 16) replaces the step's attention for a group
+# of COUNT slots sharing SHARED_TOKENS prompt tokens only where tools/parallel_sample_bench.py measured it faster.
+SHARED_PREFIX_MIN_COUNT = 2
+SHARED_PREFIX_MIN_TOKENS = 1024
+
+
+def shared_prefix_attention_applies(count: int, shared_tokens: int, model) -> bool:
+    """Whether a group of ``count`` slots that share ``shared_tokens`` leading tokens decodes with grouped attention:
+    the kernel's conditions (bf16, head_dim 128, pages a multiple of 64 slots, ``count x G <= 128``) and the measured
+    rule (DESIGN.md section 16)."""
+    attn0 = model.layers_inner[0].self_attn
+    G = attn0.num_heads // attn0.num_kv_heads
+    if (attn0.head_dim != 128 or model.page_size % 64 != 0 or 128 % G != 0 or count * G > 128
+            or model.embedding.weight.scales.dtype != torch.bfloat16):
+        return False
+    return count >= SHARED_PREFIX_MIN_COUNT and shared_tokens >= SHARED_PREFIX_MIN_TOKENS
+
+
+def shared_run(tables, first: int, count: int, write_from: int, page_size: int) -> int:
+    """Leading pages that slots ``first .. first + count - 1`` share in every layer of ``tables`` ([layers, B,
+    max_pages] page ids), stopping before the page holding position ``write_from`` (the first a slot may still write).
+    Forks share the same run in every layer; a group whose layers disagree is refused with ``ValueError``."""
+    limit = max(write_from, 0) // page_size
+    rows = np.asarray(tables)[:, first : first + count, :limit]
+    same = (rows == rows[:, :1, :]).all(axis=1) & (rows[:, 0, :] >= 0)  # [layers, limit]
+    runs = [int(np.argmin(r)) if not r.all() else limit for r in same]
+    if len(set(runs)) != 1:
+        raise ValueError(f"slots {first}..{first + count - 1} do not share the same pages in every layer")
+    return runs[0]
+
 
 def _concat_weights(parts):
     """Stack packed projections along the output dimension (one launch instead of
@@ -424,6 +454,14 @@ class DecodeEngine(_GraphEngine):
         self._beam_bufs: dict = {}
         self.beam_cum = None
         self.kernels_per_beam_step = 0
+        # decode_on_device(groups=...): grouped twins of the sampled step (with and without logprobs), whose attention is
+        # q/k norm + RoPE + append then tl_shared_prefix_attention over the (first_slot, count, shared_pages) descriptors
+        # of the call; one graph per logprobs N (None: none), all on first use
+        self._graph_grp: dict = {}
+        self._grp_host = None
+        self._grp_dev = None
+        self._grp_ws = None
+        self.kernels_per_grouped_step = 0
         if self.lora is not None:
             if rows_per_request != 1 or not self.fused:
                 raise ValueError("a model with adapters runs one row per slot on the fused decode step")
@@ -506,7 +544,7 @@ class DecodeEngine(_GraphEngine):
         self.logits.copy_(logits)
 
     def _forward_fused(self, rows: int | None = None, sampled: bool = False, penalized: bool = False, constrained: bool = False,
-                       spec_draft=None) -> None:
+                       spec_draft=None, grouped: bool = False) -> None:
         """Same step in ~7 launches per layer: norm / SwiGLU / residual folded into
         the streaming projections, q/k norm + RoPE + K/V append in one kernel.
         Every rounding point of the operator-by-operator sequence is kept.
@@ -520,10 +558,10 @@ class DecodeEngine(_GraphEngine):
             x = _normed(_lora_layers(m, x, self.adapter_ids[:R], self._qkv_attention(R)), m.norm)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x)
         elif self.B > 8:
-            h = _swap_ab_layers(m, x, self._swap_ab_attention(R))
+            h = _swap_ab_layers(m, x, self._swap_ab_attention(R, grouped))
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, h)
         else:
-            x = self._matvec_layers(x)
+            x = self._matvec_layers(x, grouped)
             logits = ext.quantized_matmul_fused(head.scales, head.biases, head.weight, x, m.norm._weight_as(x.dtype, x.device),
                                                 prologue=ext.PRO_RMSNORM, eps=m.norm.eps)
         self._next_tokens(logits, R, sampled, penalized, constrained, spec_draft)
@@ -531,14 +569,21 @@ class DecodeEngine(_GraphEngine):
             self.logits = torch.zeros((self.rows, logits.shape[-1]), dtype=logits.dtype, device=logits.device)
         self.logits[:R].copy_(logits)
 
-    def _swap_ab_attention(self, R: int):
-        """The attention of ``_swap_ab_layers`` for the first ``R`` slots."""
+    def _grouped_attention(self, i: int, at, q):
+        """``tl_shared_prefix_attention`` of all B slots over the descriptors of the call (layer ``i``)."""
+        pool = self.model.page_pools[i]
+        return ext.shared_prefix_attention(q.view(self.B * self.Hq, 1, self.D), pool._key_pages, pool._value_pages, self.tables[i],
+                                           self.context_lens, self._grp_dev, self._grp_host, at.scale, self.Hkv, self.Hq,
+                                           workspace=self._grp_ws)
+
+    def _swap_ab_attention(self, R: int, grouped: bool = False):
+        """The attention of ``_swap_ab_layers`` for the first ``R`` slots (``grouped``: all B, shared-prefix attention)."""
         m, Hq, Hkv, D = self.model, self.Hq, self.Hkv, self.D
         offsets, context_lens = self.offsets[:R], self.context_lens[:R]
 
         def attention(i, block, h):
             at, pk, pool = block.self_attn, self._packed[i], m.page_pools[i]
-            if self._attention_fused:
+            if self._attention_fused and not grouped:
                 qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h)
                 return ext.decode_attention_fused(qkv, at.q_norm._weight_as(h.dtype, h.device), at.k_norm._weight_as(h.dtype, h.device),
                                                   offsets, self.tables[i][:R], context_lens, self._rope_inv_freq,
@@ -548,6 +593,8 @@ class DecodeEngine(_GraphEngine):
             q = ext.qkv_project_rope_append(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, h, at.q_norm._weight_as(h.dtype, h.device),
                                             at.k_norm._weight_as(h.dtype, h.device), offsets, self.tables[i][:R], context_lens,
                                             pool._key_pages, pool._value_pages, Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)
+            if grouped:
+                return self._grouped_attention(i, at, q).view(R, Hq * D)
             y = ext.paged_attention(q.view(R * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i][:R], context_lens,
                                     at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             return y.view(R, Hq * D)
@@ -574,9 +621,10 @@ class DecodeEngine(_GraphEngine):
 
         return attention
 
-    def _matvec_layers(self, x):
+    def _matvec_layers(self, x, grouped: bool = False):
         """The layer stack for at most 8 slots on the streaming matvec kernel, with RMSNorm as its prologue and the
-        residual add as its epilogue; returns the residual stream before the final norm."""
+        residual add as its epilogue; returns the residual stream before the final norm.  ``grouped``: the attention is
+        q/k norm + RoPE + append and ``tl_shared_prefix_attention``."""
         m = self.model
         B, Hq, Hkv, D = x.shape[0], self.Hq, self.Hkv, self.D
         for i, block in enumerate(m.layers_inner):
@@ -584,7 +632,7 @@ class DecodeEngine(_GraphEngine):
             ln1, ln2 = block.input_layernorm, block.post_attention_layernorm
             qkv = ext.quantized_matmul_fused(pk.qkv.scales, pk.qkv.biases, pk.qkv.weight, x, ln1._weight_as(x.dtype, x.device),
                                              prologue=ext.PRO_RMSNORM, eps=ln1.eps)
-            if self._attention_fused:
+            if self._attention_fused and not grouped:
                 y = ext.decode_attention_fused(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                self.offsets, self.tables[i], self.context_lens, self._rope_inv_freq,
                                                pool._key_pages, pool._value_pages, Hq, Hkv, at.q_norm.eps, at.scale,
@@ -593,8 +641,11 @@ class DecodeEngine(_GraphEngine):
                 q = ext.decode_qk_norm_rope_append(qkv, at.q_norm._weight_as(x.dtype, x.device), at.k_norm._weight_as(x.dtype, x.device),
                                                    self.offsets, self.tables[i], self.context_lens, pool._key_pages, pool._value_pages,
                                                    Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)
-                y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
-                                        at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
+                if grouped:
+                    y = self._grouped_attention(i, at, q)
+                else:
+                    y = ext.paged_attention(q.view(B * Hq, 1, D), pool._key_pages, pool._value_pages, self.tables[i], self.context_lens,
+                                            at.scale, is_causal=True, num_kv_heads=Hkv, num_heads=Hq)
             x = ext.quantized_matmul_fused(at.wo.scales, at.wo.biases, at.wo.weight, y.view(B, Hq * D), residual=x, epilogue=ext.EPI_RESIDUAL)
             if isinstance(block.mlp, Moe):
                 x = _moe_mlp(block.mlp, x, ln2=ln2)
@@ -626,6 +677,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_keep = None
         self._graph_spec = {}
         self._graph_beam = {}
+        self._graph_grp = {}
         if self._rows_per_request > 1:  # a verify pass: no self-advancing loop, no row variants
             self.kernels_per_step = self._launches
             return
@@ -714,6 +766,55 @@ class DecodeEngine(_GraphEngine):
             self.kernels_per_beam_step = self._launches
             self.beam_cum.copy_(kept)
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _ensure_grouped_graph(self, max_n: int | None) -> None:
+        """Capture the grouped twin of the sampled step, with one ``tl_logprobs`` launch when ``max_n`` is given (same
+        conditions as ``_ensure_sample_graph``; the descriptors are all-unused during the warm-up)."""
+        if self._grp_host is None:
+            self._grp_host = torch.zeros((self.B, 3), dtype=torch.int32, pin_memory=True)
+            self._grp_dev = self._grp_host.to(self.device, copy=True)
+            nbytes = ext.shared_prefix_attention_workspace(self.B, self.Hq, self.Hkv, self.page_size, self.max_pages)
+            self._grp_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        if max_n in self._graph_grp:
+            return
+        forward = self._forward_fused
+
+        def grouped_step():
+            forward(sampled=True, grouped=True)
+            if max_n is not None:
+                ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self._grp_host.zero_()
+            self._grp_dev.zero_()
+            self.step_counter.zero_()
+            self._graph_grp[max_n] = self._graph_of(grouped_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_grouped_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _group_descriptors(self, groups, offsets) -> list:
+        """``(first_slot, count, shared_pages)`` of each group of ``groups`` (``(first_slot, count)`` pairs), from the
+        host block tables after this call's pages are allocated; ``shared_pages`` is 0 where the selection rule
+        (``shared_prefix_attention_applies``) keeps the plain attention.  Malformed groups raise ``ValueError``."""
+        taken = [False] * self.B
+        out = []
+        for first, count in groups:
+            first, count = int(first), int(count)
+            if count < 1 or first < 0 or first + count > self.B:
+                raise ValueError(f"group ({first}, {count}) leaves the engine's {self.B} slots")
+            if any(taken[first : first + count]):
+                raise ValueError(f"group ({first}, {count}) overlaps another group")
+            taken[first : first + count] = [True] * count
+            if self._recs[first] is None or any(self._recs[b] is None for b in range(first, first + count)):
+                raise ValueError(f"group ({first}, {count}) holds an idle slot")
+            pages = shared_run(self.tables_np, first, count, min(int(offsets[b]) for b in range(first, first + count)), self.page_size)
+            if not shared_prefix_attention_applies(count, pages * self.page_size, self.model):
+                pages = 0
+            out.append((first, count, pages))
+        return out
 
     def _ensure_penalized_graph(self) -> None:
         """Capture the penalised sampled self-advancing step (same conditions as ``_ensure_sample_graph``; the warm-up
@@ -1082,7 +1183,7 @@ class DecodeEngine(_GraphEngine):
         return self.logits.view(B, 1, self.V), self.next_tokens
 
     def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None, adapter_ids=None,
-                         keep_logits: bool = False):
+                         keep_logits: bool = False, groups=None):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
@@ -1102,7 +1203,13 @@ class DecodeEngine(_GraphEngine):
         ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above.
         ``keep_logits=True`` (plain ``sampling``: no penalty, constraint or logprobs) replays the sampled step with one
         more launch that keeps each step's logits rows, and returns ``(tokens, logits [steps, B, V])``, a device view of
-        the engine's log (overwritten by the next call): the rows a speculative draft's proposals were drawn from."""
+        the engine's log (overwritten by the next call): the rows a speculative draft's proposals were drawn from.
+        ``groups`` (``(first_slot, count)`` pairs of slots forked from one prompt, ``paged_kv_cache.fork``): for the
+        plain sampled step, with or without logprobs, on a fused engine without adapters, the leading full pages every
+        layer of a group's slots shares are attended once for all its rows (``tl_shared_prefix_attention``) wherever
+        ``shared_prefix_attention_applies``; every other call, and a call where no group qualifies, replays the graph
+        it would without ``groups``.  Groups that leave the slots, overlap, hold an idle slot or whose layers do not
+        share the same pages raise ``ValueError``."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         if keep_logits:
@@ -1131,6 +1238,13 @@ class DecodeEngine(_GraphEngine):
         self._host_write_begin()
         ctx = self._advance_host(caches, steps)
         self._ensure_graph()
+        descriptors = None
+        if groups is not None:
+            descriptors = self._group_descriptors(groups, offsets)
+            plain = (sampling is not None and not penalized and not constrained and not keep_logits and self.fused
+                     and self.lora is None and self._rows_per_request == 1)
+            if not plain or not any(d[2] for d in descriptors):
+                descriptors = None
         self._adapters_of_call(adapter_ids)
         if penalized:
             self._alloc_penalties()
@@ -1142,6 +1256,14 @@ class DecodeEngine(_GraphEngine):
                 self._alloc_logprobs(max(top_n))
                 self._set_top_n(top_n)
             self._ensure_constrained_graph(penalized, None if top_n is None else max(top_n))
+        elif descriptors is not None:
+            if top_n is not None:
+                self._alloc_logprobs(max(top_n))
+                self._set_top_n(top_n)
+            self._ensure_grouped_graph(None if top_n is None else max(top_n))
+            self._grp_host.zero_()
+            for j, d in enumerate(descriptors):
+                self._grp_host[j] = torch.tensor(d, dtype=torch.int32)
         elif top_n is not None:
             self._ensure_logprobs_graph(sampling is not None, max(top_n), penalized)
             self._set_top_n(top_n)
@@ -1162,6 +1284,8 @@ class DecodeEngine(_GraphEngine):
         self.meta_np[2 * B : 3 * B] = ctx
         if constrained:
             graph = self._graph_con[(penalized, None if top_n is None else max(top_n))]
+        elif descriptors is not None:
+            graph = self._graph_grp[None if top_n is None else max(top_n)]
         elif top_n is not None:
             graph = self._graph_lp[(sampling is not None, penalized)]
         elif penalized:
@@ -1174,6 +1298,9 @@ class DecodeEngine(_GraphEngine):
         self._stream.wait_stream(cur)
         with torch.cuda.stream(self._stream):
             self._upload()
+            if descriptors is not None:
+                self._grp_dev.copy_(self._grp_host, non_blocking=True)
+                self._upload_event.record()
             self.step_counter.zero_()
             for i in range(steps):
                 graph.replay()

@@ -13,7 +13,7 @@ from extensions_b200 import tiny_llm_ext_b200
 
 from .batch import greedy_tokens
 from .kv_cache import BatchingKvCache
-from .logprobs import _check_n, token_logprobs
+from .logprobs import _check_n, _host_rows, entries_from_host, token_logprobs
 from .lora import adapter_ids_of
 from .sampler import sample_tokens, token_state_row
 
@@ -752,3 +752,173 @@ def beam_search_ids(model, prompt_ids, max_new_tokens: int, num_beams: int = 4, 
         for caches, _ in beams:
             _release_kv_cache(caches)
     return [h for h, _ in kept[:num_return_sequences]]
+
+
+# ------------------------------------------------------------------ parallel sampling --
+# n seeded samples of each prompt from one prefill: the prompt's cache is forked n - 1 ways (``paged_kv_cache.fork``),
+# prompt i's samples decode in slots i*n .. i*n+n-1 of one P*n-slot step, and each such range is a group of
+# ``DecodeEngine.decode_on_device(groups=...)``, whose shared prompt pages are attended once per step (DESIGN.md
+# section 16).
+
+PARALLEL_MAX_SAMPLES = 16  # n x G <= 128 for every Qwen3 head ratio up to G = 8
+PARALLEL_MAX_SLOTS = 64
+PARALLEL_ROUND = 16  # decode steps between two reads of the tokens
+
+
+@dataclass
+class ParallelSample:
+    """One sample of ``parallel_sample_ids``: the generated ids (an ending EOS is not included), ``"stop"`` (an EOS)
+    or ``"length"`` (``max_new_tokens``), and one ``TokenLogprobs`` per id when logprobs were asked for (else None)."""
+
+    ids: list
+    finish_reason: str
+    logprobs: list | None = None
+
+
+def sample_seed(seed: int, j: int) -> int:
+    """The seed of sample ``j`` of a request seeded ``seed``: ``(seed + j) mod 2**64`` (the CLI's "request i uses
+    seed + i"), as the signed 64-bit value ``SamplingParams`` holds."""
+    v = (int(seed) + int(j)) % (1 << 64)
+    return v - (1 << 64) if v >= (1 << 63) else v
+
+
+def _check_parallel_args(model, prompts, num_samples, sampling, max_new_tokens, logprobs, adapter) -> list:
+    from .sampler import SamplingParams
+
+    if adapter is not None:
+        raise ValueError("parallel sampling takes no adapter")
+    if not isinstance(num_samples, int) or isinstance(num_samples, bool) or not 1 <= num_samples <= PARALLEL_MAX_SAMPLES:
+        raise ValueError(f"num_samples must be an integer in [1, {PARALLEL_MAX_SAMPLES}]")
+    if not prompts or len(prompts) * num_samples > PARALLEL_MAX_SLOTS:
+        raise ValueError(f"prompts x num_samples must be in [1, {PARALLEL_MAX_SLOTS}]")
+    if any(len(p) == 0 for p in prompts):
+        raise ValueError("prompt must encode to at least one token")
+    if not isinstance(max_new_tokens, int) or isinstance(max_new_tokens, bool) or max_new_tokens < 0:
+        raise ValueError("max_new_tokens must be a non-negative integer")
+    if logprobs is not None:
+        _check_n(logprobs)
+    per = [sampling] * len(prompts) if isinstance(sampling, SamplingParams) else list(sampling)
+    if len(per) != len(prompts) or not all(isinstance(p, SamplingParams) for p in per):
+        raise ValueError("sampling must be one SamplingParams or one per prompt")
+    if num_samples > 1 and any(p.temperature == 0 for p in per):
+        raise ValueError("temperature 0 is greedy: every sample would be the same; give num_samples=1")
+    return per
+
+
+def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_tokens: int, eos_token_ids=(), logprobs=None, device=None,
+                        adapter=None):
+    """``num_samples`` independent seeded samples of each prompt of ``prompts`` (lists of ids) from one prefill each.
+    Sample j of a prompt draws with ``replace(sampling, seed=(seed + j) mod 2**64)`` (``sampling``: one
+    ``SamplingParams`` or one per prompt), so it is the ``greedy_generate_ids(sampling=...)`` run of that seed.  Each
+    sample ends at its first EOS (not returned) or after ``max_new_tokens``.  Returns one list per prompt of
+    ``num_samples`` ``ParallelSample``.
+    The prompt's cache is forked ``num_samples - 1`` ways; all samples decode together, in rounds of
+    ``decode_on_device`` on a CUDA Week-3 model whose graph window holds the prompt and budget (with grouped attention
+    over each prompt's shared pages where ``shared_prefix_attention_applies``), else through ``model(...)``.  Every
+    page goes back to its pool on return and on an exception.  Refused with ``ValueError`` before any work:
+    ``num_samples`` outside 1..16, more than 64 samples in all, an empty prompt, a negative budget, non-paged caches,
+    temperature 0 with ``num_samples > 1`` and an ``adapter``."""
+    from dataclasses import replace
+
+    from .paged_kv_cache import TinyKvPagedCache, fork
+    from .sampler import token_state_row
+
+    prompts = [[int(t) for t in p] for p in prompts]
+    per = _check_parallel_args(model, prompts, num_samples, sampling, max_new_tokens, logprobs, adapter)
+    probe = model.create_kv_cache()
+    paged = all(isinstance(c, TinyKvPagedCache) for c in probe)
+    _release_kv_cache(probe)
+    if not paged:
+        raise ValueError("parallel sampling needs paged KV caches (the Week-3 model)")
+    n, P = num_samples, len(prompts)
+    eos = {int(t) for t in eos_token_ids}
+    params = [replace(per[i], seed=sample_seed(per[i].seed, j)) for i in range(P) for j in range(n)]
+    out = [[ParallelSample([], "length", [] if logprobs is not None else None) for _ in range(n)] for _ in range(P)]
+    if max_new_tokens == 0:
+        return out
+    if device is None:
+        scales = getattr(getattr(getattr(model, "embedding", None), "weight", None), "scales", None)
+        device = None if scales is None else scales.device
+    longest = max(len(p) for p in prompts) + max_new_tokens
+    graph = device is not None and _beam_graph_applies(model, device, longest)
+    slots: list = [None] * (P * n)  # per-layer caches of each sample
+    done = [False] * (P * n)
+    penalized = any(p.penalized for p in params)
+    constrained = any(p.constraint is not None for p in params)
+    state = constraints = None
+
+    def take(b, token, entry) -> None:
+        if done[b]:
+            return
+        s = out[b // n][b % n]
+        if token in eos:
+            done[b], s.finish_reason = True, "stop"
+            return
+        s.ids.append(int(token))
+        if entry is not None:
+            s.logprobs.append(entry)
+        if len(s.ids) >= max_new_tokens:
+            done[b] = True
+
+    try:
+        firsts = []
+        for i, prompt in enumerate(prompts):
+            cache = model.create_kv_cache()
+            slots[i * n] = cache
+            logits = model(torch.as_tensor(prompt, dtype=torch.int32, device=device)[None], 0, cache, logits_to_keep=1)
+            rows = logits[:, -1, :].expand(n, -1).contiguous()
+            st = con = None
+            if penalized:
+                st = torch.stack([token_state_row(torch.as_tensor(prompt), [], rows.shape[-1], device=rows.device)] * n)
+            if constrained:
+                con = torch.stack([params[i * n + j].constraint.descriptor() if params[i * n + j].constraint is not None
+                                   else torch.zeros(5, dtype=torch.int64) for j in range(n)]).to(rows.device)
+            tok = sample_tokens(rows, params[i * n : i * n + n], [len(prompt)] * n, st, con)
+            ent = token_logprobs(rows, tok, logprobs) if logprobs is not None else [None] * n
+            firsts.append((tok.tolist(), ent, st, con))
+            if n > 1:
+                slots[i * n + 1 : i * n + n] = fork([(cache, n - 1)])[0]
+        tokens = [0] * (P * n)
+        for i, (tok, ent, st, con) in enumerate(firsts):
+            for j in range(n):
+                tokens[i * n + j] = tok[j]
+                take(i * n + j, tok[j], ent[j])
+        if not graph:
+            state = torch.cat([f[2] for f in firsts]) if penalized else None
+            constraints = torch.cat([f[3] for f in firsts]) if constrained else None
+        offsets = [len(prompts[b // n]) for b in range(P * n)]
+        batch = [BatchingKvCache(P * n) for _ in range(len(slots[0]))]
+        for layer, slot in enumerate(batch):
+            slot.kv_caches = [slots[b][layer] for b in range(P * n)]
+        groups = [(i * n, n) for i in range(P)] if n > 1 else None
+        engine = model.decode_engine(P * n, model.decode_graph_max_seq_len) if graph else None
+        while not all(done):
+            steps = min(PARALLEL_ROUND, max_new_tokens - min(len(out[b // n][b % n].ids) for b in range(P * n) if not done[b]))
+            if graph:
+                history = None
+                if penalized or constrained:
+                    history = [(prompts[b // n], out[b // n][b % n].ids) for b in range(P * n)]
+                got = engine.decode_on_device(tokens, offsets, batch, steps, sampling=params, logprobs=logprobs, history=history, groups=groups)
+                ids, lp = (got, None) if logprobs is None else got
+                host = ids.tolist()  # the round's device->host read
+                lp_host = None if lp is None else [_host_rows(ids[s], *[t[s] for t in lp]) for s in range(steps)]
+                for s in range(steps):
+                    ent = entries_from_host(*lp_host[s]) if lp_host is not None else [None] * (P * n)
+                    for b in range(P * n):
+                        take(b, host[s][b], ent[b])
+                tokens = host[-1]
+                offsets = [o + steps for o in offsets]
+            else:
+                for _ in range(steps):
+                    y = torch.as_tensor(tokens, dtype=torch.int32, device=device).view(P * n, 1)
+                    rows = model(y, list(offsets), batch, logits_to_keep=1)[:, -1, :]
+                    tok = sample_tokens(rows, params, [o + 1 for o in offsets], state, constraints)
+                    ent = token_logprobs(rows, tok, logprobs) if logprobs is not None else [None] * (P * n)
+                    tokens = tok.tolist()
+                    for b in range(P * n):
+                        take(b, tokens[b], ent[b])
+                    offsets = [o + 1 for o in offsets]
+    finally:
+        for caches in slots:
+            _release_kv_cache(caches)
+    return out
