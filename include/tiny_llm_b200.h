@@ -196,6 +196,26 @@ int tl_shared_prefix_attention(const void *q, const void *key_pages, const void 
                                const int32_t *context_lens, const int32_t *groups, const int32_t *groups_host, int num_groups,
                                void *out, int batch, int D, int num_pages, int page_size, int max_pages, float scale,
                                int num_kv_heads, int num_heads, int dtype, void *workspace, size_t workspace_bytes, void *stream);
+/* Segment-causal attention for packed prefill (embedding passes): one request whose L rows are several prompts laid
+ * end to end, each row's K/V already appended at slot = row through the one block-table row block_table [max_pages].
+ * Row l sees exactly the keys segment_start[l] <= key <= l (segment_start: int32 [L] on the device, the first row of
+ * l's prompt); a row with segment_start[l] > l (padding) sees nothing and its output is 0.  A CTA skips the key tiles
+ * before the smallest segment_start of its rows.  q [Hq, L, 128] (the chunk form's layout), out [L, Hq * 128]
+ * token-major; bf16 or fp16 q / pages / out, 16-byte aligned; page_size a multiple of 64; Hq / Hkv divides 128;
+ * L <= max_pages * page_size.  One launch, no workspace, no synchronisation (capturable). */
+int tl_paged_attention_segments(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                const int32_t *segment_start, void *out, int L, int D, int num_pages, int page_size, int max_pages, float scale,
+                                int num_kv_heads, int num_heads, int dtype, void *stream);
+/* Pooled embeddings of packed hidden states (DESIGN.md section 17).  hidden [rows, hidden_size] and norm_weight
+ * [hidden_size] bf16 or fp16; segment_start int32 [num_segments + 1] on the device, segment s = rows
+ * segment_start[s] .. segment_start[s + 1] - 1.  Each pooled row is RMS-normalised exactly as tl_rms_norm does it
+ * (same bits); TL_EMBED_LAST takes the segment's last row, TL_EMBED_MEAN the fp32 mean of its normalised,
+ * dtype-rounded rows summed in row order.  The result is truncated to the first `dimensions` features and, with
+ * normalize, divided by its fp32 L2 norm (a zero vector stays zero).  out: fp32 [num_segments, dimensions].  An
+ * empty segment gives zeros.  hidden_size <= TL_EMBED_MAX_HIDDEN. */
+enum { TL_EMBED_LAST = 0, TL_EMBED_MEAN = 1, TL_EMBED_MAX_HIDDEN = 12288 };
+int tl_embed_pool(const void *hidden, const void *norm_weight, float eps, const int32_t *segment_start, int num_segments, int rows, int hidden_size,
+                  int dimensions, int pooling, int normalize, float *out, int dtype, void *stream);
 
 /* ---- CUDA extension behind the same per-op semantics ---------------------
  * Device-driven K/V append for a decode batch (the batched form of

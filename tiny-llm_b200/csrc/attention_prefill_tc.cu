@@ -74,12 +74,16 @@ struct TcArgs {
     // num_groups; the partial of split s of row r goes to slot r * split_stride + split_base + s.
     const int32_t *groups;
     int num_groups, split_base, split_stride;
+    // Segment-causal attention (TC_SEGMENT, one packed request): row l sees the keys segment_start[l] <= key <= l.
+    const int32_t *segment_start;
 };
 
 // TC_PLAIN: tl_paged_attention.  TC_PREFIX: one CTA per (group, KV head, split) over the group's shared pages, its 128
 // MMA rows the count x G query rows of the group's slots (slot-major), unmasked.  TC_SUFFIX: one CTA per (slot, KV head,
-// split) over the slot's keys after its group's shared pages, as TC_PLAIN at L = 1 otherwise.
-enum { TC_PLAIN = 0, TC_PREFIX = 1, TC_SUFFIX = 2 };
+// split) over the slot's keys after its group's shared pages, as TC_PLAIN at L = 1 otherwise.  TC_SEGMENT: TC_PLAIN's
+// causal token-major prefill of one request whose L rows are packed prompts: row l also masks the keys before
+// segment_start[l], and a CTA starts at the tile holding the smallest segment_start of its rows.
+enum { TC_PLAIN = 0, TC_PREFIX = 1, TC_SUFFIX = 2, TC_SEGMENT = 3 };
 
 // The group of slot b: (first_slot, count, shared_pages), or (b, 1, 0) when no group with shared pages holds it.
 __device__ __forceinline__ int3 tc_group_of(const int32_t *groups, int num_groups, int b) {
@@ -90,7 +94,7 @@ __device__ __forceinline__ int3 tc_group_of(const int32_t *groups, int num_group
     return make_int3(b, 1, 0);
 }
 
-template <int MODE>
+template <int MODE, typename T = bf16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const TcArgs a) {
@@ -104,17 +108,22 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int q0 = qb * a.RH;
     const int cap = a.max_pages * a.page_size;
     int3 grp = make_int3(b, 1, 0);
-    if (MODE != TC_PLAIN) grp = tc_group_of(a.groups, a.num_groups, b);
+    if (MODE == TC_PREFIX || MODE == TC_SUFFIX) grp = tc_group_of(a.groups, a.num_groups, b);
     if (MODE == TC_PREFIX && grp.x != b) return;  // the group's first slot covers its rows
     // The causal shift uses the whole context, the block table clamps afterwards (attention_decode.cu).
-    const int ctx = a.context_lens[b];
+    const int ctx = MODE == TC_SEGMENT ? a.L : a.context_lens[b];  // TC_SEGMENT: the packed rows are the whole context
     // keys any row of this CTA may see: [0, key_end); the prefix pass sees the shared pages, the suffix pass what follows
     const int last_row = min(q0 + a.RH, a.L) - 1;
     const int shared_keys = min(grp.z * a.page_size, cap);
     const int key_end = MODE == TC_PREFIX ? shared_keys
                         : ctx <= 0 ? 0 : min(a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx, cap);
     const int all_tiles = (key_end + TC_BN - 1) / TC_BN;
-    const int tile_lo = MODE == TC_SUFFIX ? min(shared_keys / TC_BN, all_tiles) : 0;
+    int seg_lo = 0;  // TC_SEGMENT: the smallest segment start of this CTA's rows
+    if (MODE == TC_SEGMENT) {
+        seg_lo = key_end;
+        for (int r = q0; r <= last_row; ++r) seg_lo = min(seg_lo, max(a.segment_start[r], 0));
+    }
+    const int tile_lo = MODE == TC_SUFFIX ? min(shared_keys / TC_BN, all_tiles) : MODE == TC_SEGMENT ? min(seg_lo / TC_BN, all_tiles) : 0;
     // Split-KV: the launch fixes the NUMBER of splits from the block table's width (the grid of a captured graph cannot
     // follow the context), the tiles are dealt out here from the request's real length, so a request far below the
     // bound still keeps all its splits busy.
@@ -195,7 +204,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         const int wg = wg_idx - 1;
         const int t = threadIdx.x & 127;
         // TC_PREFIX: l = the row's slot inside the group (a row past the group's count is not written)
-        int lq[2], g[2], l[2], limit[2];
+        int lq[2], g[2], l[2], limit[2], lo[2] = {0, 0};  // lo: TC_SEGMENT's first visible key
         bool row_valid[2];
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
@@ -213,6 +222,10 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             row_valid[rr] = l[rr] < a.L && ctx > 0;
             // last key this row may see (bottom-right causal alignment, paged_attention.metal:411)
             limit[rr] = !row_valid[rr] ? -1 : min(a.is_causal ? min(ctx - 1, l[rr] + (ctx - a.L)) : ctx - 1, cap - 1);
+            if (MODE == TC_SEGMENT && row_valid[rr]) {
+                lo[rr] = max(a.segment_start[l[rr]], 0);
+                if (lo[rr] > limit[rr]) row_valid[rr] = false, limit[rr] = -1;  // an empty segment (a padding row): output 0
+            }
         }
         float o[TC_D / 2];
 #pragma unroll
@@ -228,7 +241,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             const int pid = table[lp];
             const bool page_ok = pid >= 0 && pid < a.num_pages;
             // ---- S = Q K_j^T: both operands K-major, two 64-wide halves of the head dimension
-            float sc[TC_BN / 2];
+            float sc[TC_BN / 2];  // fp32 scores
 #pragma unroll
             for (int i = 0; i < TC_BN / 2; ++i) sc[i] = 0.f;
             g_mbar_wait(k_full + 8 * s, ph);
@@ -239,7 +252,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 #pragma unroll
                 for (int k = 0; k < TC_D / 16; ++k) {
                     const uint32_t half = k >> 2, kk = k & 3;
-                    Wgmma<bf16, TC_BN>::ss(sc, g_wgmma_desc(q_wg + half * (TC_Q_BYTES / 2) + 32 * kk, 16, 1024),
+                    Wgmma<T, TC_BN>::ss(sc, g_wgmma_desc(q_wg + half * (TC_Q_BYTES / 2) + 32 * kk, 16, 1024),
                                            g_wgmma_desc(kb + half * (TC_KV_TILE / 2) + 32 * kk, 16, 1024), k > 0 ? 1u : 0u);
                 }
             }
@@ -253,6 +266,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int visible = page_ok ? min(limit[rr] - key0 + 1, TC_BN) : 0;  // keys [0, visible) of the tile
+                const int first = lo[rr] - key0;                                        // TC_SEGMENT: and not below first
                 // raw maximum (the scale is positive, so it commutes with max); masking only on boundary tiles
                 float raw_max = -CUDART_INF_F;
 #pragma unroll
@@ -260,7 +274,8 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         float &v = sc[4 * c8 + 2 * rr + e];
-                        if (visible < TC_BN && 8 * c8 + 2 * (lane & 3) + e >= visible) v = -CUDART_INF_F;  // exp2 gives exactly 0
+                        const int c = 8 * c8 + 2 * (lane & 3) + e;
+                        if (MODE == TC_SEGMENT ? (c >= visible || c < first) : (visible < TC_BN && c >= visible)) v = -CUDART_INF_F;  // exp2 gives exactly 0
                         raw_max = fmaxf(raw_max, v);
                     }
                 raw_max = fmaxf(raw_max, __shfl_xor_sync(0xffffffffu, raw_max, 1));
@@ -288,7 +303,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
                     const float p1 = tc_ex2(fmaf(sc[4 * c8 + 2 * rr + 1], a.scale_log2, -m_eff));
                     tile_sum += p0 + p1;
                     // K step c8 / 2: registers {row r0, keys +0..7}, {r0 + 8, +0..7}, {r0, +8..15}, {r0 + 8, +8..15}
-                    pa[c8 >> 1][2 * (c8 & 1) + rr] = pack2<bf16>(p0, p1);
+                    pa[c8 >> 1][2 * (c8 & 1) + rr] = pack2<T>(p0, p1);
                 }
                 l_sum[rr] += tile_sum;
             }
@@ -300,7 +315,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
                 const uint32_t vb = v_base + s * TC_KV_TILE;
 #pragma unroll
                 for (int k = 0; k < TC_BN / 16; ++k)  // 16 keys = two 8-row groups of 128 B
-                    Wgmma<bf16, TC_D, 1>::rs(o, pa[k], g_wgmma_desc(vb + k * 2048, TC_KV_TILE / 2, 1024), 1u);
+                    Wgmma<T, TC_D, 1>::rs(o, pa[k], g_wgmma_desc(vb + k * 2048, TC_KV_TILE / 2, 1024), 1u);
             }
             wgmma_commit();
             wgmma_wait<0>();
@@ -318,7 +333,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             const size_t out_row = MODE == TC_PREFIX ? static_cast<size_t>(b + l[rr]) * a.Hq + kvh * a.G + g[rr]
                                                      : static_cast<size_t>(b * a.Hq + kvh * a.G + g[rr]) * a.L + l[rr];
             const int col = 2 * (lane & 3);
-            if (MODE != TC_PLAIN || a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
+            if (MODE == TC_PREFIX || MODE == TC_SUFFIX || a.splits > 1) {  // unnormalised partial for the merge kernel (attention_decode.cu: paged_gqa_merge_kernel)
                 const size_t slot = out_row * a.split_stride + a.split_base + split;
                 float *po = a.ws_o + slot * TC_D;
 #pragma unroll
@@ -330,10 +345,10 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
                 }
             } else {
                 const float inv = (lt == 0.f || !row_valid[rr]) ? 0.f : 1.0f / lt;
-                bf16 *dst = a.out + (a.out_token_major ? (static_cast<size_t>(b) * a.L + l[rr]) * a.Hq + (kvh * a.G + g[rr]) : out_row) * TC_D;
+                T *dst = reinterpret_cast<T *>(a.out) + (a.out_token_major ? (static_cast<size_t>(b) * a.L + l[rr]) * a.Hq + (kvh * a.G + g[rr]) : out_row) * TC_D;
 #pragma unroll
                 for (int c8 = 0; c8 < TC_D / 8; ++c8)
-                    *reinterpret_cast<uint32_t *>(dst + 8 * c8 + col) = pack2<bf16>(o[4 * c8 + 2 * rr] * inv, o[4 * c8 + 2 * rr + 1] * inv);
+                    *reinterpret_cast<uint32_t *>(dst + 8 * c8 + col) = pack2<T>(o[4 * c8 + 2 * rr] * inv, o[4 * c8 + 2 * rr + 1] * inv);
             }
         }
     }
@@ -341,9 +356,10 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
 
 // ---------------------------------------------------------------- host side --
 // bf16 Q / K / V with the 128-byte swizzle (the K-major wgmma layout), 256-byte L2 promotion.
-static int tc_map(CUtensorMap *out, const void *ptr, int rank, const cuuint64_t *dims, const cuuint32_t *box) {
-    return cached_tensor_map(out, ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, dims, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "paged_attention");
+static int tc_map(CUtensorMap *out, const void *ptr, int rank, const cuuint64_t *dims, const cuuint32_t *box,
+                  CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+    return cached_tensor_map(out, ptr, dtype, rank, dims, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                             "paged_attention");
 }
 
 bool paged_prefill_tc_supported(int L, int num_pages, int page_size, int num_kv_heads, int num_heads) {
@@ -510,6 +526,60 @@ int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp
     if (le != cudaSuccess) return fail(TL_ECUDA, "shared_prefix_attention: launch failed: %s", cudaGetErrorString(le));
     TL_LAUNCH_CHECK("shared_prefix_attention_suffix");
     return launch_paged_gqa_merge(a.ws_o, a.ws_m, a.ws_l, out, static_cast<int>(rows_total), sp + ss, st, 1, num_heads, false);
+}
+
+// ---------------------------------------------------------------- segment-causal attention --
+// One packed request of L rows (B = 1, the chunk form's q [Hq, L, D] and token-major out [L, Hq * D]) whose keys are its
+// own rows 0 .. L - 1: row l sees segment_start[l] <= key <= l.  Unsplit (a pass of L <= 8,192 rows spans at most as
+// many keys): the q-block grid of launch_paged_prefill_tc at B = 1.
+template <typename T>
+static int launch_segment_t(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
+                            int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, CUtensorMapDataType dt,
+                            cudaStream_t st) {
+    static bool configured = false;
+    if (!configured) {
+        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_SEGMENT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
+            return fail(TL_ECUDA, "paged_attention_segments: cannot raise shared memory limit");
+        configured = true;
+    }
+    TcArgs a{};
+    a.block_table = bt, a.context_lens = nullptr, a.out = static_cast<bf16 *>(out);
+    a.L = L, a.Hq = num_heads, a.Hkv = num_kv_heads, a.G = num_heads / num_kv_heads, a.RH = TC_BM / a.G;
+    a.page_size = page_size, a.max_pages = max_pages, a.num_pages = num_pages;
+    a.tiles_per_page = page_size / TC_BN;
+    a.scale_log2 = scale * TC_LOG2E;
+    a.is_causal = 1;
+    a.splits = a.split_stride = 1;
+    a.tiles_per_split = (max_pages * page_size + TC_BN - 1) / TC_BN;
+    a.out_token_major = 1;
+    a.segment_start = seg;
+    CUtensorMap mq, mk, mv;
+    {
+        const cuuint64_t dims[3] = {TC_D, static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(num_heads)};
+        const cuuint32_t box[3] = {64, static_cast<cuuint32_t>(a.RH), static_cast<cuuint32_t>(a.G)};
+        if (int e = tc_map(&mq, q, 3, dims, box, dt)) return e;
+    }
+    {
+        const cuuint64_t dims[4] = {TC_D, static_cast<cuuint64_t>(page_size), static_cast<cuuint64_t>(num_kv_heads), static_cast<cuuint64_t>(num_pages)};
+        const cuuint32_t box[4] = {64, TC_BN, 1, 1};
+        if (int e = tc_map(&mk, kp, 4, dims, box, dt)) return e;
+        if (int e = tc_map(&mv, vp, 4, dims, box, dt)) return e;
+    }
+    const dim3 grid((L + a.RH - 1) / a.RH, num_kv_heads, 1);
+    cudaError_t le = launch_chained(paged_prefill_tc_kernel<TC_SEGMENT, T>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
+    if (le != cudaSuccess) return fail(TL_ECUDA, "paged_attention_segments: launch failed: %s", cudaGetErrorString(le));
+    TL_LAUNCH_CHECK("paged_attention_segments");
+    return TL_OK;
+}
+
+int launch_paged_attention_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
+                                    int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, int dtype,
+                                    cudaStream_t st) {
+    if (dtype == TL_F16)
+        return launch_segment_t<__half>(q, kp, vp, bt, seg, out, L, num_pages, page_size, max_pages, scale, num_kv_heads, num_heads,
+                                        CU_TENSOR_MAP_DATA_TYPE_FLOAT16, st);
+    return launch_segment_t<bf16>(q, kp, vp, bt, seg, out, L, num_pages, page_size, max_pages, scale, num_kv_heads, num_heads,
+                                  CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, st);
 }
 
 }  // namespace tl

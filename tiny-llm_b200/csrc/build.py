@@ -42,6 +42,7 @@ SOURCES = [
     "constrained.cu",
     "moe.cu",
     "lora.cu",
+    "embed.cu",
     "tma.cu",
 ]
 

@@ -425,6 +425,39 @@ int tl_shared_prefix_attention(const void *q, const void *key_pages, const void 
                                           page_size, max_pages, scale, num_kv_heads, num_heads, workspace, as_stream(stream));
 }
 
+int tl_paged_attention_segments(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                const int32_t *segment_start, void *out, int L, int D, int num_pages, int page_size, int max_pages, float scale,
+                                int num_kv_heads, int num_heads, int dtype, void *stream) {
+    if (dtype != TL_BF16 && dtype != TL_F16) return fail(TL_EDTYPE, "paged_attention_segments: expected float16 or bfloat16");
+    if (D != PAGED_D) return fail(TL_EINVAL, "paged_attention_segments: head dimension must be %d", PAGED_D);
+    if (num_heads <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0 || 128 % (num_heads / num_kv_heads) != 0)
+        return fail(TL_EINVAL, "paged_attention_segments: num_heads / num_kv_heads must be a whole divisor of 128");
+    if (L < 0 || num_pages <= 0 || max_pages <= 0 || page_size <= 0 || page_size % 64 != 0)
+        return fail(TL_EINVAL, "paged_attention_segments: bad shape (page_size must be a multiple of 64)");
+    if (static_cast<long long>(L) > static_cast<long long>(max_pages) * page_size)
+        return fail(TL_EINVAL, "paged_attention_segments: %d rows do not fit the block table's %d pages", L, max_pages);
+    if (L == 0) return TL_OK;
+    if (!q || !key_pages || !value_pages || !block_table || !segment_start || !out)
+        return fail(TL_EINVAL, "paged_attention_segments: null pointer");
+    if (!aligned16(q) || !aligned16(key_pages) || !aligned16(value_pages) || !aligned16(out))
+        return fail(TL_EINVAL, "paged_attention_segments: q, pages and out must be 16-byte aligned");
+    return launch_paged_attention_segments(q, key_pages, value_pages, block_table, segment_start, out, L, num_pages, page_size, max_pages, scale,
+                                           num_kv_heads, num_heads, dtype, as_stream(stream));
+}
+
+int tl_embed_pool(const void *hidden, const void *norm_weight, float eps, const int32_t *segment_start, int num_segments, int rows, int hidden_size,
+                  int dimensions, int pooling, int normalize, float *out, int dtype, void *stream) {
+    if (dtype != TL_BF16 && dtype != TL_F16) return fail(TL_EDTYPE, "embed_pool: expected float16 or bfloat16");
+    if (num_segments < 0 || rows < 0 || hidden_size <= 0 || hidden_size > TL_EMBED_MAX_HIDDEN)
+        return fail(TL_EINVAL, "embed_pool: bad shape (hidden size must be in [1, %d])", TL_EMBED_MAX_HIDDEN);
+    if (dimensions < 1 || dimensions > hidden_size) return fail(TL_EINVAL, "embed_pool: dimensions must be in [1, %d]", hidden_size);
+    if (pooling != TL_EMBED_LAST && pooling != TL_EMBED_MEAN) return fail(TL_EINVAL, "embed_pool: pooling must be TL_EMBED_LAST or TL_EMBED_MEAN");
+    if (num_segments == 0) return TL_OK;
+    if (!hidden || !norm_weight || !segment_start || !out) return fail(TL_EINVAL, "embed_pool: null pointer");
+    return launch_embed_pool(hidden, norm_weight, eps, segment_start, num_segments, rows, hidden_size, dimensions, pooling == TL_EMBED_MEAN,
+                             normalize != 0, out, dtype, as_stream(stream));
+}
+
 // ------------------------------------------------------------------ misc --
 size_t tl_argmax_workspace(int rows, int vocab) { return argmax_workspace(rows, vocab); }
 

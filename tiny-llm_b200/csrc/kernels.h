@@ -186,6 +186,14 @@ size_t shared_prefix_workspace(int batch, int num_heads, int num_kv_heads, int p
 int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl,
                                    const int32_t *groups, int num_groups, void *out, int batch, int num_pages, int page_size,
                                    int max_pages, float scale, int num_kv_heads, int num_heads, void *ws, cudaStream_t st);
+// Segment-causal attention of one packed request (tl_paged_attention_segments): bf16 or fp16 (dtype), unsplit.
+int launch_paged_attention_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
+                                    int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, int dtype,
+                                    cudaStream_t st);
+
+// embed.cu
+int launch_embed_pool(const void *x, const void *w, float eps, const int32_t *seg, int n, int rows, int H, int d, int mean, int normalize,
+                      float *out, int dtype, cudaStream_t st);
 
 // attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the wgmma kernel does not take)
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,

@@ -84,6 +84,8 @@ __all__ = [
     "lora_apply_route",
     "shared_prefix_attention",
     "shared_prefix_attention_workspace",
+    "paged_attention_segments",
+    "embed_pool",
 ]
 
 _HERE = Path(__file__).resolve().parent
@@ -163,6 +165,8 @@ _SIGNATURES = {
     "tl_lora_apply": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_shared_prefix_attention_workspace": (_SZ, [_I] * 5),
     "tl_shared_prefix_attention": (_I, [_VP] * 7 + [_I, _VP] + [_I] * 5 + [_F] + [_I] * 3 + [_VP, _SZ, _VP]),
+    "tl_paged_attention_segments": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
+    "tl_embed_pool": (_I, [_VP, _VP, _F, _VP] + [_I] * 6 + [_VP, _I, _VP]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -1231,6 +1235,60 @@ def paged_attention_token_major(query, key_pages, value_pages, block_table, cont
     y = paged_attention(query, key_pages, value_pages, block_table, context_lens, scale, is_causal=is_causal, num_kv_heads=num_kv_heads,
                         num_heads=num_heads, stream=stream)
     return y.view(B, num_heads, L, D).transpose(1, 2).reshape(B * L, num_heads * D)
+
+
+def paged_attention_segments(query, key_pages, value_pages, block_table, segment_start, scale, num_kv_heads, num_heads, stream=None):
+    """Segment-causal prefill attention of one packed request (``tl_paged_attention_segments``, DESIGN.md section 17):
+    ``query`` [Hq, L, 128] (``chunk_qk_norm_rope_append``'s output) -> ``[L, Hq * 128]`` token-major, row ``l`` seeing
+    the keys ``segment_start[l] <= key <= l`` through the one block-table row ``block_table`` [max_pages]; a row with
+    ``segment_start[l] > l`` gives zeros.  bf16 or fp16; page size a multiple of 64, Hq / Hkv dividing 128."""
+    op = "paged_attention_segments"
+    if query.dim() != 3 or key_pages.dim() != 4 or key_pages.shape != value_pages.shape:
+        raise RuntimeError(f"{op}: q must be [H_q, L, D] and the page tensors [P, H_kv, page_size, D]")
+    if query.dtype not in _HALF or key_pages.dtype != query.dtype or value_pages.dtype != query.dtype:
+        raise RuntimeError(f"{op}: q, key_pages and value_pages must share one dtype, float16 or bfloat16")
+    Hq, L, D = query.shape
+    if Hq != num_heads or key_pages.shape[1] != num_kv_heads:
+        raise RuntimeError(f"{op}: q must hold num_heads heads and the pages num_kv_heads")
+    _int32(op, L, segment_start=segment_start)
+    _block_table(op, block_table, None)
+    _gpu(op, query, key_pages, value_pages, block_table, segment_start)
+    _contig(op, query=query, key_pages=key_pages, value_pages=value_pages, block_table=block_table, segment_start=segment_start)
+    P, _, page_size, _ = key_pages.shape
+    out = torch.empty((L, Hq * D), dtype=query.dtype, device=query.device)
+    _check(_lib.tl_paged_attention_segments(query.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), block_table.data_ptr(),
+                                            segment_start.data_ptr(), out.data_ptr(), L, D, P, page_size, block_table.shape[0], float(scale),
+                                            int(num_kv_heads), int(num_heads), _DTYPE_CODE[query.dtype], _stream_ptr(stream, query)))
+    return out
+
+
+EMBED_POOLING = {"last": 0, "mean": 1}
+
+
+def embed_pool(hidden, norm_weight, eps, segment_start, pooling="last", dimensions=None, normalize=True, stream=None):
+    """Pooled embeddings of packed hidden states (``tl_embed_pool``, DESIGN.md section 17): ``hidden`` [rows, H] bf16 or
+    fp16, segments ``segment_start[s] .. segment_start[s + 1] - 1`` (int32 ``[n + 1]``).  Each pooled row is
+    ``rms_norm(row, norm_weight, eps)`` bit for bit; ``pooling`` "last" takes the segment's last row, "mean" the fp32
+    mean of its normalised rows; the first ``dimensions`` features (all when None) are kept and, with ``normalize``,
+    divided by their L2 norm.  Returns fp32 ``[n, dimensions]``."""
+    op = "embed_pool"
+    if pooling not in EMBED_POOLING:
+        raise ValueError(f"{op}: pooling must be one of {sorted(EMBED_POOLING)}, got {pooling!r}")
+    if hidden.dim() != 2 or hidden.dtype not in _HALF or norm_weight.dtype != hidden.dtype or tuple(norm_weight.shape) != (hidden.shape[1],):
+        raise RuntimeError(f"{op}: hidden must be float16 or bfloat16 [rows, H] with a norm weight [H] of its dtype")
+    rows, H = hidden.shape
+    d = H if dimensions is None else int(dimensions)
+    if not 1 <= d <= H:
+        raise ValueError(f"{op}: dimensions must be in [1, {H}], got {d}")
+    if segment_start.dtype != torch.int32 or segment_start.dim() != 1 or segment_start.shape[0] < 1:
+        raise RuntimeError(f"{op}: segment_start must be int32 [n + 1]")
+    _gpu(op, hidden, norm_weight, segment_start)
+    _contig(op, hidden=hidden, norm_weight=norm_weight, segment_start=segment_start)
+    n = segment_start.shape[0] - 1
+    out = torch.empty((n, d), dtype=torch.float32, device=hidden.device)
+    _check(_lib.tl_embed_pool(hidden.data_ptr(), norm_weight.data_ptr(), float(eps), segment_start.data_ptr(), n, rows, H, d,
+                              EMBED_POOLING[pooling], int(bool(normalize)), out.data_ptr(), _DTYPE_CODE[hidden.dtype], _stream_ptr(stream, hidden)))
+    return out
 
 
 def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight, norm_eps, stream=None):

@@ -7,6 +7,7 @@ from .attention import paged_attention, scaled_dot_product_attention_grouped, sc
 from .basics import linear, silu, softmax
 from .batch import ContinuousBatcher, Request, batch_generate
 from .checkpoint import load_checkpoint, load_tokenizer, save_checkpoint
+from .embed import embed_ids
 from .embedding import Embedding, QuantizedEmbedding
 from .generate import (BeamHypothesis, ParallelSample, beam_search_ids, greedy_generate_ids, parallel_sample_ids, prompt_lookup_generate_ids,
                        simple_generate_with_kv_cache, speculative_generate, speculative_generate_ids)

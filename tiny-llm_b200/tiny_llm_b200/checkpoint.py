@@ -9,7 +9,8 @@ checkpoint directory is ``config.json`` + ``model*.safetensors`` whose tensors
 are named ``model.layers.{i}.self_attn.q_proj.{weight,scales,biases}`` ... with
 ``weight`` packed uint32 ``[out, in/8]`` in exactly the nibble order
 ``dequantize_weights`` decodes (quantize.py:103-121), so loading is a rename into
-``SimpleNamespace``s: no tensor is transformed.
+``SimpleNamespace``s: no tensor is transformed.  Embedding checkpoints (Qwen3-Embedding) save the bare ``Qwen3Model``:
+the same tensors without the ``model.`` prefix and without ``lm_head``; they load too.
 
 ``save_checkpoint`` writes the same layout (used by the tests to round-trip a
 synthetic model, and handy for producing fixtures); there is no network here, so
@@ -65,6 +66,10 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
     if scaling is not None:
         args.rope_scaling = scaling.to_config()
     tensors = _read_tensors(path)
+    # Qwen3Model naming (embedding checkpoints): embed_tokens.*, layers.{i}.*, norm.*, no lm_head
+    root = "model." if "model.embed_tokens.weight" in tensors or "embed_tokens.weight" not in tensors else ""
+    if not root and "lm_head.weight" not in tensors:
+        args.tie_word_embeddings = True  # no head of its own: the model embeds, its logits are the tied embedding's
 
     def take(name: str) -> torch.Tensor:
         if name not in tensors:
@@ -84,13 +89,13 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
 
     layers = []
     for i in range(args.num_hidden_layers):
-        base = f"model.layers.{i}"
+        base = f"{root}layers.{i}"
         attn = SimpleNamespace(**{n: linear(f"{base}.self_attn.{n}") for n in _LINEARS["self_attn"]},
                                q_norm=norm(f"{base}.self_attn.q_norm"), k_norm=norm(f"{base}.self_attn.k_norm"))
         mlp = SimpleNamespace(**{n: linear(f"{base}.mlp.{n}") for n in _LINEARS["mlp"]})
         layers.append(SimpleNamespace(self_attn=attn, mlp=mlp, input_layernorm=norm(f"{base}.input_layernorm"),
                                       post_attention_layernorm=norm(f"{base}.post_attention_layernorm")))
-    model = SimpleNamespace(args=args, model=SimpleNamespace(embed_tokens=linear("model.embed_tokens"), layers=layers, norm=norm("model.norm")))
+    model = SimpleNamespace(args=args, model=SimpleNamespace(embed_tokens=linear(f"{root}embed_tokens"), layers=layers, norm=norm(f"{root}norm")))
     if not args.tie_word_embeddings:
         model.lm_head = linear("lm_head")
     return model

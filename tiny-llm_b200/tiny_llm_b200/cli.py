@@ -31,6 +31,8 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli batch --synthetic tiny-d128 --synthetic-lora a=16 --synthetic-lora b=8:1 \
         --prompt-ids "5,17,3;5,17,3;5,17,3" --adapters "a;;b"
         (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
+    python -m tiny_llm_b200.cli embed --synthetic tiny-d128 --prompt-ids "5,17,3;9,2,4,8" --dimensions 64 [--pooling mean] [--out e.npy]
+        (one pooled, L2-normalised embedding per prompt from packed prefill passes; --append-eos for Qwen3-Embedding)
 """
 
 from __future__ import annotations
@@ -414,6 +416,54 @@ def cmd_score(args) -> int:
     return 0
 
 
+def embed_inputs(args, tokenizer) -> list[list[int]]:
+    """The token ids ``embed`` runs: ``--prompt-ids`` ("1,2;3,4"), else the ``--prompt`` texts and the lines of
+    ``--prompts-file`` encoded by the tokenizer; ``--append-eos`` ends each with the tokenizer's EOS id (what
+    Qwen3-Embedding's last-token pooling expects)."""
+    if args.prompt_ids:
+        prompts = [[int(t) for t in part.split(",") if t.strip()] for part in args.prompt_ids.split(";")]
+    else:
+        texts = list(args.prompt or [])
+        if args.prompts_file:
+            with open(args.prompts_file, encoding="utf-8") as f:
+                texts += [line.rstrip("\n") for line in f if line.strip()]
+        if not texts:
+            raise SystemExit("embed needs --prompt-ids, --prompt or --prompts-file")
+        if tokenizer is None:
+            raise SystemExit("text prompts need the checkpoint's tokenizer files; use --prompt-ids")
+        prompts = [list(tokenizer.encode(t, add_special_tokens=False)) for t in texts]
+    if args.append_eos:
+        eos = None if tokenizer is None else tokenizer.eos_token_id
+        if eos is None:
+            raise SystemExit("--append-eos needs a tokenizer with an EOS id")
+        prompts = [p + [int(eos)] for p in prompts]
+    for i, p in enumerate(prompts):
+        if not p:
+            raise SystemExit(f"prompt {i} is empty")
+    return prompts
+
+
+def cmd_embed(args) -> int:
+    from .embed import embed_ids
+
+    device = torch.device(args.device)
+    ns, tokenizer, name = _load(args, device)
+    model = _model(args, ns, name)
+    prompts = embed_inputs(args, tokenizer)
+    try:
+        out = embed_ids(model, prompts, pooling=args.pooling, normalize=not args.no_normalize, dimensions=args.dimensions,
+                        max_tokens=args.max_tokens, device=device).cpu()
+    except ValueError as exc:
+        raise SystemExit(f"embed: {exc}") from None
+    for i, row in enumerate(out):
+        print(f"[{i}] {len(prompts[i])} tokens, {row.numel()} dims, norm {row.norm().item():.6f}: " + " ".join(f"{v:.6f}" for v in row.tolist()))
+    if args.out:
+        import numpy as np
+
+        np.save(args.out, out.numpy())
+    return 0
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="tiny_llm_b200.cli")
     sub = ap.add_subparsers(dest="command", required=True)
@@ -476,6 +526,20 @@ def main(argv=None) -> int:
                                          help="prompt-lookup speculative decoding: K (1..7) proposals per round from the request's own tokens")
     sub.choices["generate"].add_argument("--prompt-lookup-ngram", default="2:3", metavar="MIN:MAX",
                                          help="suffix lengths prompt lookup matches (1 <= MIN <= MAX <= 8)")
+    p = sub.add_parser("embed")
+    p.set_defaults(fn=cmd_embed, loader="week3", rope_scaling=None, max_context=None, disable_paged_attention=False, logprobs=None)
+    p.add_argument("--model", default=None, help="checkpoint directory (Qwen3 or Qwen3-Embedding, MLX 4-bit)")
+    p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny-d128, qwen3-0.6b, qwen3-4b) instead of --model")
+    p.add_argument("--prompt", action="append", default=None, help="a text to embed (repeatable; needs the tokenizer)")
+    p.add_argument("--prompts-file", default=None, help="one text per line")
+    p.add_argument("--prompt-ids", default=None, help="comma-separated token ids, ';' between prompts")
+    p.add_argument("--append-eos", action="store_true", help="end every prompt with the tokenizer's EOS id")
+    p.add_argument("--pooling", choices=["last", "mean"], default="last")
+    p.add_argument("--dimensions", type=_positive_int, default=None, metavar="N", help="keep the first N features (default: all)")
+    p.add_argument("--no-normalize", action="store_true", help="skip the L2 normalisation")
+    p.add_argument("--max-tokens", type=_positive_int, default=8192, metavar="N", help="rows per packed pass (a multiple of 128)")
+    p.add_argument("--out", default=None, metavar="FILE.npy", help="also save the [n, d] float32 embeddings")
+    p.add_argument("--device", default="cuda:0")
     sub.choices["batch"].add_argument("--prompts-file", default=None)
     sub.choices["batch"].add_argument("--batch-size", type=int, default=5)
     sub.choices["batch"].add_argument("--prefill-step", type=int, default=128)
