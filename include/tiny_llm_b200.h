@@ -92,12 +92,25 @@ size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_sim
 int tl_quantized_matmul(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
                         int N, int K, int dtype, int use_simdgroup, int use_split_k, void *workspace,
                         size_t workspace_bytes, void *stream);
+/* W8A16: every entry that takes packed weights has a *_bits sibling whose `bits` (after dtype) is 4 or 8; the entry
+ * without the suffix is its bits = 4 form.  8-bit weights are MLX affine at group 128: b [K, N/4] u32, code i of a word
+ * = (w >> 8i) & 255, scales/biases [K, N/128], weight = code * scale + bias.  Kernel choice, row thresholds and
+ * workspace sizes are those of 4 bits.  Any other `bits` is TL_EINVAL (the two workspace queries return 0 for it). */
+int tl_quantized_matmul_route_bits(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, int bits, const void *a,
+                                   const void *b, const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass,
+                                   int *units);
+size_t tl_quantized_matmul_workspace_bits(int M, int N, int K, int dtype, int bits, int use_simdgroup, int use_split_k);
+int tl_quantized_matmul_bits(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
+                             int bits, int use_simdgroup, int use_split_k, void *workspace, size_t workspace_bytes, void *stream);
 
 /* Replaces quantized_embedding (tiny_llm_ext.h:40-41, quantized_matmul.cpp:82-101,
  * :242-273).  indices int32/uint32 [tokens] (bit pattern), weight [vocab, dim/8] u32,
  * scales/biases [vocab, dim/128], out [tokens, dim]. */
 int tl_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight,
                            void *out, int tokens, int vocab, int dim, int dtype, void *stream);
+/* weight [vocab, dim * bits / 32] u32; at 8 bits 8-byte aligned. */
+int tl_quantized_embedding_bits(const void *indices, const void *scales, const void *biases, const void *weight, void *out, int tokens, int vocab,
+                                int dim, int dtype, int bits, void *stream);
 
 /* ---- fused model kernels (week2_kernels.cpp:36-84, :104-211) ------------- */
 /* x [rows, dim], weight [dim], out [rows, dim]:  x * rsqrt(mean(x^2)+eps) * w */
@@ -382,6 +395,10 @@ size_t tl_quantized_matmul_fused_workspace(int M, int N, int K, int lda, int pro
 int tl_quantized_matmul_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0,
                               const void *p1, const void *residual, int M, int N, int K, int lda, int prologue,
                               int epilogue, float eps, int dtype, void *workspace, size_t workspace_bytes, void *stream);
+size_t tl_quantized_matmul_fused_workspace_bits(int M, int N, int K, int lda, int prologue, int dtype, int bits);
+int tl_quantized_matmul_fused_bits(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
+                                   const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype, int bits,
+                                   void *workspace, size_t workspace_bytes, void *stream);
 /* out = residual + projection(p0) and, in the same call, normed_out = rms_norm(out, norm_weight, norm_eps): the
  * residual-stream projections (o, down) of qwen3_week3.py:204-206 followed by the RMSNorm that opens the next block
  * (:195-199).  Same rounding points as tl_quantized_matmul_fused(TL_EPI_RESIDUAL) then tl_rms_norm; with a split
@@ -390,6 +407,9 @@ int tl_quantized_matmul_fused(const void *scales, const void *biases, const void
 int tl_quantized_matmul_residual_norm(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *residual,
                                       const void *norm_weight, void *normed_out, int M, int N, int K, float norm_eps, int dtype, void *workspace,
                                       size_t workspace_bytes, void *stream);
+int tl_quantized_matmul_residual_norm_bits(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *residual,
+                                           const void *norm_weight, void *normed_out, int M, int N, int K, float norm_eps, int dtype, int bits,
+                                           void *workspace, size_t workspace_bytes, void *stream);
 /* q|k|v projection of `rows` activation rows (p0 [rows, N], packed weight rows = q heads | k heads | v heads) followed by
  * per-head q/k RMSNorm + RoPE + K/V append (tl_decode_qk_norm_rope_append, or its chunk form when chunk != 0).  With a
  * split reduction (9..128 rows) the partial planes feed the second kernel directly and q|k|v is never materialised;
@@ -404,6 +424,17 @@ int tl_qkv_project_rope_append_table(const void *scales, const void *biases, con
                                      const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
                                      int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
                                      int dtype, void *workspace, size_t workspace_bytes, void *stream, const double *inv_freq);
+int tl_qkv_project_rope_append_bits(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                    const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                    const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                    int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
+                                    int dtype, int bits, void *workspace, size_t workspace_bytes, void *stream);
+int tl_qkv_project_rope_append_table_bits(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                          const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                          const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                          int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages,
+                                          int chunk, int dtype, int bits, void *workspace, size_t workspace_bytes, void *stream,
+                                          const double *inv_freq);
 /* Decode step, L == 1: per-head q/k RMSNorm + RoPE + K/V append in one launch.
  * qkv [B, (Hq + 2*Hkv) * D] (q heads | k heads | v heads); q_out [B, Hq, D];
  * K/V rows land in the page slot of token context_lens[b]-1 (rows with context

@@ -120,15 +120,32 @@ int tl_device_info(int *sms, int *major, int *minor) {
 }
 
 // ------------------------------------------------------------ W4A16 ------
-size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_simdgroup, int /*use_split_k*/) {
+// Every entry that takes packed weights has a *_bits sibling for 4- or 8-bit codes (group 128 at both widths); the
+// entry without the suffix is its bits = 4 form.  The kernel choice does not depend on the width.
+static bool bad_bits(int bits) { return bits != 4 && bits != 8; }
+#define TL_CHECK_BITS(op) \
+    if (bad_bits(bits)) return fail(TL_EINVAL, op ": bits must be 4 or 8 (got %d)", bits)
+
+size_t tl_quantized_matmul_workspace(int M, int N, int K, int dtype, int use_simdgroup, int use_split_k) {
+    return tl_quantized_matmul_workspace_bits(M, N, K, dtype, 4, use_simdgroup, use_split_k);
+}
+
+size_t tl_quantized_matmul_workspace_bits(int M, int N, int K, int dtype, int bits, int use_simdgroup, int /*use_split_k*/) {
+    if (bad_bits(bits)) return 0;  // the launch refuses the width
     if (w4a16_path(M, N, K, dtype, use_simdgroup, false, TL_PRO_NONE, N) == W4Path::SKINNY) return w4a16_skinny_workspace(M, N, K);
     return 0;
 }
 
 int tl_quantized_matmul(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N,
-                        int K, int dtype, int use_simdgroup, int /*use_split_k*/, void *workspace, size_t workspace_bytes,
+                        int K, int dtype, int use_simdgroup, int use_split_k, void *workspace, size_t workspace_bytes,
                         void *stream) {
+    return tl_quantized_matmul_bits(scales, biases, a, b, out, M, N, K, dtype, 4, use_simdgroup, use_split_k, workspace, workspace_bytes, stream);
+}
+
+int tl_quantized_matmul_bits(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
+                             int bits, int use_simdgroup, int /*use_split_k*/, void *workspace, size_t workspace_bytes, void *stream) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    TL_CHECK_BITS("quantized_matmul");
     if (M < 0 || N <= 0 || K < 0) return fail(TL_EINVAL, "quantized_matmul: negative dimension");
     if (N % 128 != 0) return fail(TL_EINVAL, "quantized_matmul: N must be divisible by group_size");
     if (!scales || !biases || !a || !b || !out) {
@@ -137,22 +154,30 @@ int tl_quantized_matmul(const void *scales, const void *biases, const void *a, c
     }
     cudaStream_t st = as_stream(stream);
     switch (w4a16_path(M, N, K, dtype, use_simdgroup, false, TL_PRO_NONE, N)) {
-        case W4Path::VANILLA: return launch_w4a16_vanilla(scales, biases, a, b, out, M, N, K, dtype, st);
+        case W4Path::VANILLA: return launch_w4a16_vanilla(scales, biases, a, b, out, M, N, K, dtype, st, bits);
         case W4Path::SKINNY:
-            return launch_w4a16_skinny(scales, biases, a, b, out, nullptr, M, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st);
-        case W4Path::TILES: return launch_w4a16_tiles(scales, biases, a, b, out, M, N, K, dtype, st);
+            return launch_w4a16_skinny(scales, biases, a, b, out, nullptr, M, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st, nullptr, 0.f,
+                                       nullptr, nullptr, nullptr, bits);
+        case W4Path::TILES: return launch_w4a16_tiles(scales, biases, a, b, out, M, N, K, dtype, st, bits);
         case W4Path::STREAM: break;
     }
-    return launch_w4a16_fused(scales, biases, b, out, a, nullptr, nullptr, M, N, K, N, TL_PRO_NONE, TL_EPI_NONE, 0.f, dtype, st);
+    return launch_w4a16_fused(scales, biases, b, out, a, nullptr, nullptr, M, N, K, N, TL_PRO_NONE, TL_EPI_NONE, 0.f, dtype, st, bits);
 }
 
 int tl_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight, void *out,
                            int tokens, int vocab, int dim, int dtype, void *stream) {
-    if (tokens < 0 || vocab <= 0 || dim <= 0 || dim % 128 != 0)
-        return fail(TL_EINVAL, "quantized_embedding: expected 4-bit weights with group size 128");
+    return tl_quantized_embedding_bits(indices, scales, biases, weight, out, tokens, vocab, dim, dtype, 4, stream);
+}
+
+int tl_quantized_embedding_bits(const void *indices, const void *scales, const void *biases, const void *weight, void *out, int tokens, int vocab,
+                                int dim, int dtype, int bits, void *stream) {
+    if (tokens < 0 || vocab <= 0 || dim <= 0 || dim % 128 != 0 || bad_bits(bits))
+        return fail(TL_EINVAL, bits == 4 ? "quantized_embedding: expected 4-bit weights with group size 128"
+                                         : "quantized_embedding: expected 4- or 8-bit weights with group size 128");
     if (tokens == 0) return TL_OK;
     if (!indices || !scales || !biases || !weight || !out) return fail(TL_EINVAL, "quantized_embedding: null pointer");
-    return launch_quantized_embedding(indices, scales, biases, weight, out, tokens, vocab, dim, dtype, as_stream(stream));
+    if (bits == 8 && (reinterpret_cast<uintptr_t>(weight) & 7u) != 0) return fail(TL_EINVAL, "quantized_embedding: 8-bit weight must be 8-byte aligned");
+    return launch_quantized_embedding(indices, scales, biases, weight, out, tokens, vocab, dim, dtype, as_stream(stream), bits);
 }
 
 // ----------------------------------------------------- fused model ops ----
@@ -591,7 +616,15 @@ int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n
 
 int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, const void *a, const void *b,
                               const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass, int *units) {
+    return tl_quantized_matmul_route_bits(M, N, K, lda, prologue, fused, use_simdgroup, dtype, 4, a, b, scales, biases, splits, gb_per_split,
+                                          rows_per_pass, units);
+}
+
+int tl_quantized_matmul_route_bits(int M, int N, int K, int lda, int prologue, int fused, int use_simdgroup, int dtype, int bits, const void *a,
+                                   const void *b, const void *scales, const void *biases, int *splits, int *gb_per_split, int *rows_per_pass,
+                                   int *units) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    TL_CHECK_BITS("quantized_matmul_route");
     if (M < 0 || N <= 0 || K < 0 || lda < N || N % 128 != 0) return fail(TL_EINVAL, "quantized_matmul_route: bad shape");
     if (prologue < TL_PRO_NONE || prologue > TL_PRO_SWIGLU || (!fused && (prologue != TL_PRO_NONE || lda != N)))
         return fail(TL_EINVAL, "quantized_matmul_route: a prologue or a row stride needs a fused form");
@@ -604,7 +637,7 @@ int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fu
         else
             s = 1, gbps = N / 128;
     } else if (path == W4Path::STREAM) {
-        if (int e = w4a16_stream_plan(M, N, K, lda, a, nullptr, b, scales, biases, &rpp, &u)) return e;
+        if (int e = w4a16_stream_plan(M, N, K, lda, a, nullptr, b, scales, biases, &rpp, &u, bits)) return e;
     }
     if (splits) *splits = s;
     if (gb_per_split) *gb_per_split = gbps;
@@ -620,6 +653,11 @@ int tl_quantized_matmul_route(int M, int N, int K, int lda, int prologue, int fu
 }
 
 size_t tl_quantized_matmul_fused_workspace(int M, int N, int K, int lda, int prologue, int dtype) {
+    return tl_quantized_matmul_fused_workspace_bits(M, N, K, lda, prologue, dtype, 4);
+}
+
+size_t tl_quantized_matmul_fused_workspace_bits(int M, int N, int K, int lda, int prologue, int dtype, int bits) {
+    if (bad_bits(bits)) return 0;  // the launch refuses the width
     if (w4a16_path(M, N, K, dtype, true, true, prologue, lda) == W4Path::SKINNY) return w4a16_skinny_workspace(M, N, K);
     return 0;
 }
@@ -627,7 +665,15 @@ size_t tl_quantized_matmul_fused_workspace(int M, int N, int K, int lda, int pro
 int tl_quantized_matmul_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0,
                               const void *p1, const void *residual, int M, int N, int K, int lda, int prologue,
                               int epilogue, float eps, int dtype, void *workspace, size_t workspace_bytes, void *stream) {
+    return tl_quantized_matmul_fused_bits(scales, biases, b, out, p0, p1, residual, M, N, K, lda, prologue, epilogue, eps, dtype, 4, workspace,
+                                          workspace_bytes, stream);
+}
+
+int tl_quantized_matmul_fused_bits(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
+                                   const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype, int bits,
+                                   void *workspace, size_t workspace_bytes, void *stream) {
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    TL_CHECK_BITS("quantized_matmul_fused");
     if (M < 0 || N <= 0 || K < 0 || lda < N) return fail(TL_EINVAL, "quantized_matmul_fused: bad shape");
     if (N % 128 != 0) return fail(TL_EINVAL, "quantized_matmul: N must be divisible by group_size");
     if (prologue < TL_PRO_NONE || prologue > TL_PRO_SWIGLU || epilogue < TL_EPI_NONE || epilogue > TL_EPI_SWIGLU_PAIRS)
@@ -638,16 +684,25 @@ int tl_quantized_matmul_fused(const void *scales, const void *biases, const void
     if (!scales || !biases || !b || !out || !p0 || (prologue != TL_PRO_NONE && !p1) || (epilogue == TL_EPI_RESIDUAL && !residual))
         return fail(TL_EINVAL, "quantized_matmul_fused: null pointer");
     if (w4a16_path(M, N, K, dtype, true, true, prologue, lda) == W4Path::SKINNY)
-        return launch_w4a16_skinny(scales, biases, p0, b, out, residual, M, N, K, epilogue, dtype, workspace, workspace_bytes, as_stream(stream));
+        return launch_w4a16_skinny(scales, biases, p0, b, out, residual, M, N, K, epilogue, dtype, workspace, workspace_bytes, as_stream(stream), nullptr,
+                                   0.f, nullptr, nullptr, nullptr, bits);
     return launch_w4a16_fused(scales, biases, b, out, p0, p1, residual, M, N, K, lda, prologue, epilogue, eps, dtype,
-                              as_stream(stream));
+                              as_stream(stream), bits);
 }
 
 int tl_quantized_matmul_residual_norm(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *residual,
                                       const void *norm_weight, void *normed_out, int M, int N, int K, float norm_eps, int dtype, void *workspace,
                                       size_t workspace_bytes, void *stream) {
+    return tl_quantized_matmul_residual_norm_bits(scales, biases, b, out, p0, residual, norm_weight, normed_out, M, N, K, norm_eps, dtype, 4,
+                                                  workspace, workspace_bytes, stream);
+}
+
+int tl_quantized_matmul_residual_norm_bits(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *residual,
+                                           const void *norm_weight, void *normed_out, int M, int N, int K, float norm_eps, int dtype, int bits,
+                                           void *workspace, size_t workspace_bytes, void *stream) {
     if (!norm_weight || !normed_out) return fail(TL_EINVAL, "quantized_matmul_residual_norm: null pointer");
     if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
+    TL_CHECK_BITS("quantized_matmul_residual_norm");
     if (M < 0 || N <= 0 || K < 0 || N % 128 != 0) return fail(TL_EINVAL, "quantized_matmul_residual_norm: bad shape");
     if (M == 0 || K == 0) return TL_OK;
     if (!scales || !biases || !b || !out || !p0 || !residual) return fail(TL_EINVAL, "quantized_matmul_residual_norm: null pointer");
@@ -655,9 +710,10 @@ int tl_quantized_matmul_residual_norm(const void *scales, const void *biases, co
     int rc;
     if (w4a16_path(M, N, K, dtype, true, true, TL_PRO_NONE, N) == W4Path::SKINNY)
         rc = launch_w4a16_skinny(scales, biases, p0, b, out, residual, M, N, K, TL_EPI_RESIDUAL, dtype, workspace, workspace_bytes, as_stream(stream),
-                                 norm_weight, norm_eps, normed_out, &norm_done);
+                                 norm_weight, norm_eps, normed_out, &norm_done, nullptr, bits);
     else
-        rc = launch_w4a16_fused(scales, biases, b, out, p0, nullptr, residual, M, N, K, N, TL_PRO_NONE, TL_EPI_RESIDUAL, 0.f, dtype, as_stream(stream));
+        rc = launch_w4a16_fused(scales, biases, b, out, p0, nullptr, residual, M, N, K, N, TL_PRO_NONE, TL_EPI_RESIDUAL, 0.f, dtype, as_stream(stream),
+                                bits);
     if (rc != TL_OK || norm_done) return rc;
     return launch_rms_norm(out, norm_weight, normed_out, M, K, norm_eps, dtype, as_stream(stream));
 }
@@ -666,9 +722,19 @@ int tl_qkv_project_rope_append(const void *scales, const void *biases, const voi
                                const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table, const int32_t *context_lens, void *q_out,
                                void *key_pages, void *value_pages, int rows, int N, int num_heads, int num_kv_heads, int head_dim, float base, float eps,
                                int num_pages, int page_size, int max_pages, int chunk, int dtype, void *workspace, size_t workspace_bytes, void *stream) {
-    return tl_qkv_project_rope_append_table(scales, biases, b, p0, qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens, q_out,
-                                            key_pages, value_pages, rows, N, num_heads, num_kv_heads, head_dim, base, eps, num_pages, page_size,
-                                            max_pages, chunk, dtype, workspace, workspace_bytes, stream, nullptr);
+    return tl_qkv_project_rope_append_table_bits(scales, biases, b, p0, qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens,
+                                                 q_out, key_pages, value_pages, rows, N, num_heads, num_kv_heads, head_dim, base, eps, num_pages,
+                                                 page_size, max_pages, chunk, dtype, 4, workspace, workspace_bytes, stream, nullptr);
+}
+
+int tl_qkv_project_rope_append_bits(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                    const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                    const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                    int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
+                                    int dtype, int bits, void *workspace, size_t workspace_bytes, void *stream) {
+    return tl_qkv_project_rope_append_table_bits(scales, biases, b, p0, qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens,
+                                                 q_out, key_pages, value_pages, rows, N, num_heads, num_kv_heads, head_dim, base, eps, num_pages,
+                                                 page_size, max_pages, chunk, dtype, bits, workspace, workspace_bytes, stream, nullptr);
 }
 
 int tl_qkv_project_rope_append_table(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
@@ -676,7 +742,19 @@ int tl_qkv_project_rope_append_table(const void *scales, const void *biases, con
                                      const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
                                      int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages, int chunk,
                                      int dtype, void *workspace, size_t workspace_bytes, void *stream, const double *inv_freq) {
+    return tl_qkv_project_rope_append_table_bits(scales, biases, b, p0, qkv_scratch, q_norm_weight, k_norm_weight, offsets, block_table, context_lens,
+                                                 q_out, key_pages, value_pages, rows, N, num_heads, num_kv_heads, head_dim, base, eps, num_pages,
+                                                 page_size, max_pages, chunk, dtype, 4, workspace, workspace_bytes, stream, inv_freq);
+}
+
+int tl_qkv_project_rope_append_table_bits(const void *scales, const void *biases, const void *b, const void *p0, void *qkv_scratch,
+                                          const void *q_norm_weight, const void *k_norm_weight, const int32_t *offsets, const int32_t *block_table,
+                                          const int32_t *context_lens, void *q_out, void *key_pages, void *value_pages, int rows, int N, int num_heads,
+                                          int num_kv_heads, int head_dim, float base, float eps, int num_pages, int page_size, int max_pages,
+                                          int chunk, int dtype, int bits, void *workspace, size_t workspace_bytes, void *stream,
+                                          const double *inv_freq) {
     if (dtype != TL_BF16) return fail(TL_EDTYPE, "qkv_project_rope_append: bfloat16 required");
+    TL_CHECK_BITS("qkv_project_rope_append");
     if (rows < 0 || N <= 0 || N % 128 != 0 || num_heads <= 0 || num_kv_heads <= 0 || head_dim <= 0 || head_dim % 2 != 0 || head_dim > 512 || num_pages <= 0 ||
         page_size <= 0 || max_pages <= 0)
         return fail(TL_EINVAL, "qkv_project_rope_append: bad shape");
@@ -690,10 +768,10 @@ int tl_qkv_project_rope_append_table(const void *scales, const void *biases, con
     int rc;
     if (w4a16_path(rows, N, K, dtype, true, true, TL_PRO_NONE, N) == W4Path::SKINNY && qkv_planes_rope_supported(num_heads, num_kv_heads, head_dim, dtype))
         rc = launch_w4a16_skinny(scales, biases, p0, b, qkv_scratch, nullptr, rows, N, K, TL_EPI_NONE, dtype, workspace, workspace_bytes, st, nullptr, 0.f,
-                                 nullptr, nullptr, &planes);
+                                 nullptr, nullptr, &planes, bits);
     else
-        rc = tl_quantized_matmul_fused(scales, biases, b, qkv_scratch, p0, nullptr, nullptr, rows, N, K, N, TL_PRO_NONE, TL_EPI_NONE, 0.f, dtype,
-                                       workspace, workspace_bytes, stream);
+        rc = tl_quantized_matmul_fused_bits(scales, biases, b, qkv_scratch, p0, nullptr, nullptr, rows, N, K, N, TL_PRO_NONE, TL_EPI_NONE, 0.f, dtype,
+                                            bits, workspace, workspace_bytes, stream);
     if (rc != TL_OK) return rc;
     if (planes > 1)  // the split-reduction planes go straight into the norm / RoPE / append kernel: q|k|v is never written
         return launch_qkv_planes_rope_append(static_cast<const float *>(workspace), planes, q_norm_weight, k_norm_weight, offsets, block_table,

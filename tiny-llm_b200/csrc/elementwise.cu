@@ -348,13 +348,13 @@ int launch_add(const void *a, const void *b, void *out, long long n, int dtype, 
 }
 
 // ------------------------------------------------------ W4 embedding rows --
-// One thread per packed word: 8 codes -> 8 outputs (one 128-bit store).
+// One thread per 8 codes (one packed word; two at 8 bits) -> 8 outputs (one 128-bit store).
 // value = float(code) * scale + bias, rounded once (quantized_matmul.metal:83-88).
-template <typename T>
+template <typename T, int BITS = 4>
 __global__ void quantized_embedding_kernel(const int32_t *__restrict__ indices, const T *__restrict__ scales,
                                            const T *__restrict__ biases, const uint32_t *__restrict__ weight,
                                            T *__restrict__ out, int tokens, int vocab, int dim, bool vec_store) {
-    const int words = dim / 8;
+    const int words = dim / 8;  // 8-code chunks per row
     const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (idx >= static_cast<long long>(tokens) * words) return;
     const int token = static_cast<int>(idx / words);
@@ -365,12 +365,21 @@ __global__ void quantized_embedding_kernel(const int32_t *__restrict__ indices, 
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = 0.f;
     } else {
-        const uint32_t packed = weight[static_cast<size_t>(row) * words + wcol];
-        const size_t g = static_cast<size_t>(row) * (dim / 128) + wcol / 16;
-        const float s = to_f(scales[g]);
-        const float b = to_f(biases[g]);
+        if constexpr (BITS == 8) {
+            const uint2 packed = reinterpret_cast<const uint2 *>(weight)[static_cast<size_t>(row) * words + wcol];
+            const size_t g = static_cast<size_t>(row) * (dim / 128) + wcol / 16;
+            const float s = to_f(scales[g]);
+            const float b = to_f(biases[g]);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = static_cast<float>((packed >> (4 * j)) & 0xFu) * s + b;
+            for (int j = 0; j < 8; ++j) v[j] = static_cast<float>(((j < 4 ? packed.x : packed.y) >> (8 * (j & 3))) & 0xFFu) * s + b;
+        } else {
+            const uint32_t packed = weight[static_cast<size_t>(row) * words + wcol];
+            const size_t g = static_cast<size_t>(row) * (dim / 128) + wcol / 16;
+            const float s = to_f(scales[g]);
+            const float b = to_f(biases[g]);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[j] = static_cast<float>((packed >> (4 * j)) & 0xFu) * s + b;
+        }
     }
     T *dst = out + static_cast<size_t>(token) * dim + wcol * 8;
     if (vec_store) {
@@ -384,13 +393,13 @@ __global__ void quantized_embedding_kernel(const int32_t *__restrict__ indices, 
     }
 }
 
-template <typename T>
+template <typename T, int BITS>
 static int embedding_t(const void *indices, const void *scales, const void *biases, const void *weight, void *out,
                        int tokens, int vocab, int dim, cudaStream_t st) {
     const long long total = static_cast<long long>(tokens) * (dim / 8);
     if (total == 0) return TL_OK;
     const int threads = 256;
-    quantized_embedding_kernel<T><<<static_cast<unsigned>(ceil_div_ll(total, threads)), threads, 0, st>>>(
+    quantized_embedding_kernel<T, BITS><<<static_cast<unsigned>(ceil_div_ll(total, threads)), threads, 0, st>>>(
         static_cast<const int32_t *>(indices), static_cast<const T *>(scales), static_cast<const T *>(biases),
         static_cast<const uint32_t *>(weight), static_cast<T *>(out), tokens, vocab, dim, aligned16(out));
     TL_LAUNCH_CHECK("quantized_embedding");
@@ -398,10 +407,14 @@ static int embedding_t(const void *indices, const void *scales, const void *bias
 }
 
 int launch_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight,
-                               void *out, int tokens, int vocab, int dim, int dtype, cudaStream_t st) {
+                               void *out, int tokens, int vocab, int dim, int dtype, cudaStream_t st, int bits) {
     switch (dtype) {
-        case TL_F16: return embedding_t<__half>(indices, scales, biases, weight, out, tokens, vocab, dim, st);
-        case TL_BF16: return embedding_t<__nv_bfloat16>(indices, scales, biases, weight, out, tokens, vocab, dim, st);
+        case TL_F16:
+            return bits == 8 ? embedding_t<__half, 8>(indices, scales, biases, weight, out, tokens, vocab, dim, st)
+                             : embedding_t<__half, 4>(indices, scales, biases, weight, out, tokens, vocab, dim, st);
+        case TL_BF16:
+            return bits == 8 ? embedding_t<__nv_bfloat16, 8>(indices, scales, biases, weight, out, tokens, vocab, dim, st)
+                             : embedding_t<__nv_bfloat16, 4>(indices, scales, biases, weight, out, tokens, vocab, dim, st);
     }
     return fail(TL_EDTYPE, "quantized_embedding: scales and biases must have the same 16-bit dtype");
 }

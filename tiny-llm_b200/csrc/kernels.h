@@ -22,7 +22,7 @@ int launch_rope_inv_freq(double *out, int half, float base, cudaStream_t st);
 int launch_swiglu(const void *gate, const void *up, void *out, long long n, int dtype, cudaStream_t st);
 int launch_add(const void *a, const void *b, void *out, long long n, int dtype, cudaStream_t st);
 int launch_quantized_embedding(const void *indices, const void *scales, const void *biases, const void *weight,
-                               void *out, int tokens, int vocab, int dim, int dtype, cudaStream_t st);
+                               void *out, int tokens, int vocab, int dim, int dtype, cudaStream_t st, int bits = 4);
 int launch_paged_cache_update(void *pages, const void *values, int heads, int page_size, int head_dim, int length,
                               int page_id, int start, int dtype, cudaStream_t st);
 int launch_paged_cache_append_chunk(void *key_pages, void *value_pages, const void *keys, const void *values,
@@ -89,14 +89,14 @@ int launch_decode_qk_norm_rope_append(const void *qkv, const void *q_norm_w, con
 // p0/p1 in elements) and epilogue (0 none; 1 out = residual + result); and the scalar control kernel.
 int launch_w4a16_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
                        const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype,
-                       cudaStream_t st);
+                       cudaStream_t st, int bits = 4);
 void set_use_pdl(bool on);
 bool use_pdl();
 int launch_w4a16_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
-                         int N, int K, int dtype, cudaStream_t st);
+                         int N, int K, int dtype, cudaStream_t st, int bits = 4);
 // Rows per pass and 128-column groups per unit of the streaming kernel, or TL_EINVAL for operands it cannot take.
 int w4a16_stream_plan(int M, int N, int K, int lda, const void *p0, const void *p1, const void *b, const void *scales, const void *biases,
-                      int *rows_per_pass, int *units);
+                      int *rows_per_pass, int *units, int bits = 4);
 
 // w4a16_skinny.cu (swap-AB wgmma GEMM: split reduction for 9 <= M <= 128, 128-token tiles for prefill)
 // Split count of the reduction; *gb_per_split (optional) receives the 128-wide group blocks of each split.
@@ -106,11 +106,11 @@ size_t w4a16_skinny_workspace(int M, int N, int K);
 // whether the launch did it (split reduction, K <= 4096) or the caller still has to run rms_norm
 int launch_w4a16_skinny(const void *scales, const void *biases, const void *a, const void *b, void *out, const void *residual, int M, int N,
                         int K, int epilogue, int dtype, void *ws, size_t ws_bytes, cudaStream_t st, const void *norm_w = nullptr,
-                        float norm_eps = 0.f, void *normed = nullptr, bool *norm_done = nullptr, int *planes_out = nullptr);
+                        float norm_eps = 0.f, void *normed = nullptr, bool *norm_done = nullptr, int *planes_out = nullptr, int bits = 4);
 // planes_out (optional): with a split reduction the launch stops after the GEMM (partial planes [splits][M][K] fp32 in the
 // workspace, *planes_out = splits) and the caller's fused kernel adds them; *planes_out = 1 means `out` is complete
 int launch_w4a16_tiles(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
-                       cudaStream_t st);
+                       cudaStream_t st, int bits = 4);
 // Grouped expert GEMM over expert-sorted rows (MoE; tl_moe_grouped_matmul): K % 128 == 0, splits == 1
 int launch_w4a16_grouped(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets, const int32_t *tiles,
                          const int32_t *out_index, int R, int E, int N, int K, int epilogue, int nt, int max_tiles, int dtype, cudaStream_t st);

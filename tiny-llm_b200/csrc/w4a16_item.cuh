@@ -167,6 +167,83 @@ __device__ __forceinline__ void w4_consume(const W4Unit<U> &un, const uint4 *act
     }
 }
 
+// ---- 8-bit codes (W8A16).  A 128-column group is 128 bytes of a row; lane t holds bytes 32t..32t+31 of rows g and
+// g + 8 (two 128-bit loads each), i.e. the 8-element activation chunks 4t..4t+3 of the group - the chunks its W4 twin
+// holds as words 4t..4t+3 - so the staged activations (w4_stage) serve both widths unchanged.
+// bf16 holds 128 + q exactly only for q < 128, so each code is split q = 16 h + l and both nibbles go through the exact
+// W4 operand: per 8-byte chunk two PRMTs regroup the bytes as (e0, e4, e1, e5) / (e2, e6, e3, e7), eight LOP3s (five
+// shifts) give the nibble pairs in the k-slot order of the W4 extraction, and four MMAs accumulate sum(l a) and
+// sum(h a) separately in fp32.  Per HBM byte that is W4's LOP3 and MMA count.  Combination per group, in fp32:
+//   acc += scale * (16 * d_h + d_l) + bias * asum        (16 * d_h is exact; weights are never rounded to T)
+// A unit is one group (pairs of groups would spill).
+struct W8Unit {
+    uint4 w[4];
+    uint32_t sb;
+};
+
+__device__ __forceinline__ void w8_load(W8Unit &un, const unsigned char *p0, const unsigned char *p8, const unsigned char *psb) {
+    un.w[0] = ldg_stream(p0);
+    un.w[1] = ldg_stream(p0 + 16);
+    un.w[2] = ldg_stream(p8);
+    un.w[3] = ldg_stream(p8 + 16);
+    unsigned short v;
+    asm volatile("ld.global.nc.u16 %0, [%1];" : "=h"(v) : "l"(psb));
+    un.sb = v;
+}
+
+template <typename T, int MP>
+__device__ __forceinline__ void w8_consume(const W8Unit &un, const uint4 *actp, const float *asump, int g,
+                                           float (&acc)[(MP + 7) / 8][4]) {
+    constexpr int MT = (MP + 7) / 8;
+    const uint32_t mask = k_w4_mask;
+    const uint32_t magic = W4Num<T>::MAGIC;
+    const float s0 = W4Num<T>::lo(__shfl_sync(0xffffffffu, un.sb, g));
+    const float s8 = W4Num<T>::lo(__shfl_sync(0xffffffffu, un.sb, g + 8));
+    const float b0 = W4Num<T>::lo(__shfl_sync(0xffffffffu, un.sb, g + 16));
+    const float b8 = W4Num<T>::lo(__shfl_sync(0xffffffffu, un.sb, g + 24));
+    const uint32_t x0[8] = {un.w[0].x, un.w[0].y, un.w[0].z, un.w[0].w, un.w[1].x, un.w[1].y, un.w[1].z, un.w[1].w};
+    const uint32_t x1[8] = {un.w[2].x, un.w[2].y, un.w[2].z, un.w[2].w, un.w[3].x, un.w[3].y, un.w[3].z, un.w[3].w};
+    float dl[MT][4], dh[MT][4];
+    float2 as[MT];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) as[mt] = *reinterpret_cast<const float2 *>(asump + mt * 8);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        // bytes (e0..e3 | e4..e7) of chunk j -> (e0, e1, e4, e5) and (e2, e3, e6, e7): nibble pairs (e0, e4), (e1, e5), ...
+        const uint32_t r01 = __byte_perm(x0[2 * j], x0[2 * j + 1], 0x5410), r23 = __byte_perm(x0[2 * j], x0[2 * j + 1], 0x7632);
+        const uint32_t q01 = __byte_perm(x1[2 * j], x1[2 * j + 1], 0x5410), q23 = __byte_perm(x1[2 * j], x1[2 * j + 1], 0x7632);
+        const uint32_t a0 = w4_lop(r01, mask, magic), a1 = w4_lop(r01 >> 8, mask, magic);
+        const uint32_t a2 = w4_lop(r23, mask, magic), a3 = w4_lop(r23 >> 8, mask, magic);
+        const uint32_t c0 = w4_lop(q01, mask, magic), c1 = w4_lop(q01 >> 8, mask, magic);
+        const uint32_t c2 = w4_lop(q23, mask, magic), c3 = w4_lop(q23 >> 8, mask, magic);
+        const uint32_t h0 = w4_lop(r01 >> 4, mask, magic), h1 = w4_lop(r01 >> 12, mask, magic);
+        const uint32_t h2 = w4_lop(r23 >> 4, mask, magic), h3 = w4_lop(r23 >> 12, mask, magic);
+        const uint32_t k0 = w4_lop(q01 >> 4, mask, magic), k1 = w4_lop(q01 >> 12, mask, magic);
+        const uint32_t k2 = w4_lop(q23 >> 4, mask, magic), k3 = w4_lop(q23 >> 12, mask, magic);
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+            const uint4 bf = actp[j * MP * 4 + mt * 32];
+            if (j == 0) {
+                const float n0 = as[mt].x * W4Num<T>::NEG_OFFSET, n1 = as[mt].y * W4Num<T>::NEG_OFFSET;
+                W4Num<T>::mma_c(dl[mt], a0, c0, a1, c1, bf.x, bf.y, n0, n1);
+                W4Num<T>::mma_c(dh[mt], h0, k0, h1, k1, bf.x, bf.y, n0, n1);
+            } else {
+                W4Num<T>::mma(dl[mt], a0, c0, a1, c1, bf.x, bf.y);
+                W4Num<T>::mma(dh[mt], h0, k0, h1, k1, bf.x, bf.y);
+            }
+            W4Num<T>::mma(dl[mt], a2, c2, a3, c3, bf.z, bf.w);
+            W4Num<T>::mma(dh[mt], h2, k2, h3, k3, bf.z, bf.w);
+        }
+    }
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+        acc[mt][0] = fmaf(b0, as[mt].x, fmaf(s0, fmaf(16.f, dh[mt][0], dl[mt][0]), acc[mt][0]));
+        acc[mt][1] = fmaf(b0, as[mt].y, fmaf(s0, fmaf(16.f, dh[mt][1], dl[mt][1]), acc[mt][1]));
+        acc[mt][2] = fmaf(b8, as[mt].x, fmaf(s8, fmaf(16.f, dh[mt][2], dl[mt][2]), acc[mt][2]));
+        acc[mt][3] = fmaf(b8, as[mt].y, fmaf(s8, fmaf(16.f, dh[mt][3], dl[mt][3]), acc[mt][3]));
+    }
+}
+
 // This lane's base pointers into the staged activations (group 0).
 template <int MP>
 __device__ __forceinline__ const uint4 *w4_act_lane(const uint4 *act, int g, int t) {

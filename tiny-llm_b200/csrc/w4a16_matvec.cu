@@ -15,6 +15,8 @@
 // bias * asum" factorisation (:515-521) applied once per 128-wide group in fp32.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 #include "w4a16_item.cuh"
@@ -86,14 +88,19 @@ struct StreamArgs {
 
 
 // MP: activation rows per pass padded to a power of two (template: shared-memory offsets of the
-// B fragments become immediates).  U: 128-column groups per unit (2 when N % 256 == 0).
-template <typename T, int MP, int U>
+// B fragments become immediates).  U: 128-column groups per unit (2 when N % 256 == 0; always 1 at 8 bits).
+// BITS: 4, or 8 (b [K, N/4]: code i of a word = (w >> 8i) & 255; the unit and consumer of w4a16_item.cuh's W8 form).
+template <typename T, int MP, int U, int BITS = 4>
 __global__ void __launch_bounds__(S5_WARPS * 32, 1) w4a16_stream5_kernel(const StreamArgs args) {
+    static_assert(BITS == 4 || (BITS == 8 && U == 1), "8-bit units hold one group");
+    using Unit = std::conditional_t<BITS == 8, W8Unit, W4Unit<U>>;
     constexpr int NW = S5_WARPS;
     constexpr int NT = NW * 32;
     constexpr int MT = (MP + 7) / 8;
     constexpr int MPA = w4_mpa(MP);
-    constexpr int DEPTH = (MP <= 8 ? S5_DEPTH_SMALL : (MP == 16 ? 3 : 2));  // units per warp in the register pipeline
+    // units per warp in the register pipeline (an 8-bit unit is twice a 4-bit one: at 32 rows one unit, the bytes in flight
+    // of two 4-bit units, keeps it free of spills)
+    constexpr int DEPTH = (MP <= 8 ? S5_DEPTH_SMALL : (MP == 16 ? 3 : (BITS == 8 ? 1 : 2)));
     constexpr int ENTRY = 16 * 8 * MT;                                      // floats per (chunk, warp) partial sum
     extern __shared__ __align__(128) unsigned char smem5_raw[];
     __shared__ int warp_begin[NW + 1];
@@ -128,34 +135,37 @@ __global__ void __launch_bounds__(S5_WARPS * 32, 1) w4a16_stream5_kernel(const S
     // ---- load cursor (runs DEPTH units ahead of the consumer)
     const unsigned char *bbytes = reinterpret_cast<const unsigned char *>(args.b);
     const unsigned char *sbtable = reinterpret_cast<const unsigned char *>(lane < 16 ? args.scales : args.biases);
-    const size_t row_bytes = static_cast<size_t>(N) / 2;
+    const size_t row_bytes = static_cast<size_t>(N) / (8 / BITS);
     const unsigned char *l_p0, *l_p8, *l_sb;
     int l_i = begin, l_chunk = begin / P;
     int l_u = begin - l_chunk * P;
     auto chunk_ptrs = [&]() {  // rows past K are clamped: loaded, multiplied, never stored
         const int base = r0 + l_chunk * 16;
         const int q0 = min(base + g, K - 1), q8 = min(base + g + 8, K - 1), qs = min(base + (lane & 15), K - 1);
-        l_p0 = bbytes + q0 * row_bytes + l_u * (U * 64) + t * 16;
-        l_p8 = bbytes + q8 * row_bytes + l_u * (U * 64) + t * 16;
+        l_p0 = bbytes + q0 * row_bytes + l_u * (U * 16 * BITS) + t * 4 * BITS;
+        l_p8 = bbytes + q8 * row_bytes + l_u * (U * 16 * BITS) + t * 4 * BITS;
         l_sb = sbtable + (static_cast<size_t>(qs) * G + l_u * U) * 2;
     };
     chunk_ptrs();
-    auto load_next = [&](W4Unit<U> &un) {
+    auto load_next = [&](Unit &un) {
         if (l_i < end) {
-            w4_load<U>(un, l_p0, l_p8, l_sb);
+            if constexpr (BITS == 8)
+                w8_load(un, l_p0, l_p8, l_sb);
+            else
+                w4_load<U>(un, l_p0, l_p8, l_sb);
             l_i += 1;
             if (++l_u == P) {
                 l_u = 0;
                 l_chunk += 1;
                 chunk_ptrs();
             } else {
-                l_p0 += U * 64;
-                l_p8 += U * 64;
+                l_p0 += U * 16 * BITS;
+                l_p8 += U * 16 * BITS;
                 l_sb += U * 2;
             }
         }
     };
-    W4Unit<U> buf[DEPTH];
+    Unit buf[DEPTH];
 #pragma unroll
     for (int k = 0; k < DEPTH; ++k) load_next(buf[k]);  // in flight before the activations exist
     TL_TRACE_STAMP(11);
@@ -203,7 +213,10 @@ __global__ void __launch_bounds__(S5_WARPS * 32, 1) w4a16_stream5_kernel(const S
 #pragma unroll
         for (int k = 0; k < DEPTH; ++k) {
             if (i + k < end) {  // warp-uniform; k is a compile-time register index
-                w4_consume<T, MP, U>(buf[k], actp, asump, g, acc);
+                if constexpr (BITS == 8)
+                    w8_consume<T, MP>(buf[k], actp, asump, g, acc);
+                else
+                    w4_consume<T, MP, U>(buf[k], actp, asump, g, acc);
                 load_next(buf[k]);
                 actp += U * w4_act_group_stride<MP>();
                 asump += U * w4_asum_group_stride<MP>();
@@ -305,7 +318,7 @@ static int stream5_grid(int K) {
 // shared memory) and 128-column groups per unit (2 when N % 256 == 0, the scale/bias rows are 4-byte aligned and at
 // most 16 rows are streamed: 32 rows x pairs would spill).  The launch and tl_quantized_matmul_route both use it.
 int w4a16_stream_plan(int M, int N, int K, int lda, const void *p0, const void *p1, const void *b, const void *scales, const void *biases,
-                      int *rows_per_pass, int *units) {
+                      int *rows_per_pass, int *units, int bits) {
     if (!aligned16(p0) || !aligned16(b) || (p1 && !aligned16(p1)) || (lda % 8) != 0)
         return fail(TL_EINVAL, "quantized_matmul: operands must be 16-byte aligned");
     if (K >= (1 << 24)) return fail(TL_EINVAL, "quantized_matmul: more than 2^24 output features");
@@ -316,18 +329,18 @@ int w4a16_stream_plan(int M, int N, int K, int lda, const void *p0, const void *
     if (stream5_smem_bytes(N, K, rpp, grid_x) > S5_SMEM_MAX)
         return fail(TL_EINVAL, "quantized_matmul: activations do not fit in shared memory (N=%d, K=%d, rows=%d)", N, K, rpp);
     *rows_per_pass = rpp;
-    *units = pairs && M <= 16 ? 2 : 1;
+    *units = bits == 4 && pairs && M <= 16 ? 2 : 1;
     return TL_OK;
 }
 
-template <typename T, int MP, int U>
+template <typename T, int MP, int U, int BITS>
 static int stream5_launch(StreamArgs args, cudaStream_t st) {
     const int grid_x = stream5_grid(args.K);
     const size_t smem = stream5_smem_bytes(args.N, args.K, MP, grid_x);
     const size_t limit = S5_SMEM_MAX;
     static bool configured = false;  // per process: one device per process (DESIGN.md section 5)
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(w4a16_stream5_kernel<T, MP, U>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaError_t e = cudaFuncSetAttribute(w4a16_stream5_kernel<T, MP, U, BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              static_cast<int>(limit));
         if (e != cudaSuccess) return fail(TL_ECUDA, "quantized_matmul: cannot raise shared memory limit: %s", cudaGetErrorString(e));
         configured = true;
@@ -342,36 +355,37 @@ static int stream5_launch(StreamArgs args, cudaStream_t st) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = g_use_pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, w4a16_stream5_kernel<T, MP, U>, args);
+    cudaError_t e = cudaLaunchKernelEx(&cfg, w4a16_stream5_kernel<T, MP, U, BITS>, args);
     if (e != cudaSuccess) return fail(TL_ECUDA, "w4a16_stream5: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("w4a16_stream5");
     return TL_OK;
 }
 
-template <typename T, int U>
+template <typename T, int U, int BITS>
 static int stream5_u(StreamArgs args, cudaStream_t st) {
     switch (args.rows_per_pass) {
-        case 1: return stream5_launch<T, 1, U>(args, st);
-        case 2: return stream5_launch<T, 2, U>(args, st);
-        case 4: return stream5_launch<T, 4, U>(args, st);
-        case 8: return stream5_launch<T, 8, U>(args, st);
-        case 16: return stream5_launch<T, 16, U>(args, st);
-        default: return stream5_launch<T, 32, U>(args, st);
+        case 1: return stream5_launch<T, 1, U, BITS>(args, st);
+        case 2: return stream5_launch<T, 2, U, BITS>(args, st);
+        case 4: return stream5_launch<T, 4, U, BITS>(args, st);
+        case 8: return stream5_launch<T, 8, U, BITS>(args, st);
+        case 16: return stream5_launch<T, 16, U, BITS>(args, st);
+        default: return stream5_launch<T, 32, U, BITS>(args, st);
     }
 }
 
 template <typename T>
-static int stream5_t(StreamArgs args, cudaStream_t st) {
+static int stream5_t(StreamArgs args, int bits, cudaStream_t st) {
     int units = 1;
     if (int e = w4a16_stream_plan(args.M, args.N, args.K, args.lda, args.p0, args.p1, args.b, args.scales, args.biases, &args.rows_per_pass,
-                                  &units))
+                                  &units, bits))
         return e;
-    return units == 2 ? stream5_u<T, 2>(args, st) : stream5_u<T, 1>(args, st);
+    if (bits == 8) return stream5_u<T, 1, 8>(args, st);
+    return units == 2 ? stream5_u<T, 2, 4>(args, st) : stream5_u<T, 1, 4>(args, st);
 }
 
 int launch_w4a16_fused(const void *scales, const void *biases, const void *b, void *out, const void *p0, const void *p1,
                        const void *residual, int M, int N, int K, int lda, int prologue, int epilogue, float eps, int dtype,
-                       cudaStream_t st) {
+                       cudaStream_t st, int bits) {
     if (M == 0 || K == 0) return TL_OK;
     StreamArgs args{};
     args.scales = scales, args.biases = biases, args.b = static_cast<const uint32_t *>(b), args.out = out;
@@ -379,8 +393,8 @@ int launch_w4a16_fused(const void *scales, const void *biases, const void *b, vo
     args.M = M, args.N = N, args.K = K, args.lda = lda;
     args.prologue = prologue, args.epilogue = epilogue, args.eps = eps;
     switch (dtype) {
-        case TL_F16: return stream5_t<__half>(args, st);
-        case TL_BF16: return stream5_t<__nv_bfloat16>(args, st);
+        case TL_F16: return stream5_t<__half>(args, bits, st);
+        case TL_BF16: return stream5_t<__nv_bfloat16>(args, bits, st);
     }
     return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
 }
@@ -388,15 +402,16 @@ int launch_w4a16_fused(const void *scales, const void *biases, const void *b, vo
 // ---------------------------------------------------------------------------
 // Scalar control kernel: one thread per output, the literal arithmetic of
 // quantized_matmul_vanilla_w4a16_g128 (quantized_matmul.metal:8-56):
-//   sum += (float(code) * scale + bias) * float(a), codes in nibble order.
-template <typename T>
+//   sum += (float(code) * scale + bias) * float(a), codes in nibble (8 bits: byte) order.
+template <typename T, int BITS = 4>
 __global__ void w4a16_vanilla_kernel(const T *__restrict__ scales, const T *__restrict__ biases,
                                      const T *__restrict__ a, const uint32_t *__restrict__ b, T *__restrict__ out,
                                      int M, int N, int K) {
+    constexpr int PER = 32 / BITS;  // codes per word
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int i = blockIdx.y;
     if (k >= K || i >= M) return;
-    const int words = N / 8;
+    const int words = N / PER;
     const int G = N / 128;
     const uint32_t *brow = b + static_cast<size_t>(k) * words;
     const T *arow = a + static_cast<size_t>(i) * N;
@@ -404,32 +419,33 @@ __global__ void w4a16_vanilla_kernel(const T *__restrict__ scales, const T *__re
     for (int grp = 0; grp < G; ++grp) {
         const float s = to_f(scales[static_cast<size_t>(k) * G + grp]);
         const float c = to_f(biases[static_cast<size_t>(k) * G + grp]);
-        for (int w = 0; w < 16; ++w) {
-            const uint32_t packed = brow[grp * 16 + w];
-            const T *av = arow + grp * 128 + w * 8;
+        for (int w = 0; w < 128 / PER; ++w) {
+            const uint32_t packed = brow[grp * (128 / PER) + w];
+            const T *av = arow + grp * 128 + w * PER;
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                sum += (static_cast<float>((packed >> (4 * j)) & 0xFu) * s + c) * to_f(av[j]);
+            for (int j = 0; j < PER; ++j)
+                sum += (static_cast<float>((packed >> (BITS * j)) & ((1u << BITS) - 1u)) * s + c) * to_f(av[j]);
         }
     }
     out[static_cast<size_t>(i) * K + k] = from_f<T>(sum);
 }
 
+template <typename T, int BITS>
+static void vanilla_t(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, dim3 grid,
+                      cudaStream_t st) {
+    w4a16_vanilla_kernel<T, BITS><<<grid, 128, 0, st>>>(static_cast<const T *>(scales), static_cast<const T *>(biases), static_cast<const T *>(a),
+                                                       static_cast<const uint32_t *>(b), static_cast<T *>(out), M, N, K);
+}
+
 int launch_w4a16_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, int M,
-                         int N, int K, int dtype, cudaStream_t st) {
+                         int N, int K, int dtype, cudaStream_t st, int bits) {
     if (M == 0 || K == 0) return TL_OK;
     dim3 grid(ceil_div(K, 128), M);
     if (dtype == TL_BF16)
-        w4a16_vanilla_kernel<__nv_bfloat16><<<grid, 128, 0, st>>>(
-            static_cast<const __nv_bfloat16 *>(scales), static_cast<const __nv_bfloat16 *>(biases),
-            static_cast<const __nv_bfloat16 *>(a), static_cast<const uint32_t *>(b), static_cast<__nv_bfloat16 *>(out),
-            M, N, K);
+        bits == 8 ? vanilla_t<__nv_bfloat16, 8>(scales, biases, a, b, out, M, N, K, grid, st)
+                  : vanilla_t<__nv_bfloat16, 4>(scales, biases, a, b, out, M, N, K, grid, st);
     else if (dtype == TL_F16)
-        w4a16_vanilla_kernel<__half><<<grid, 128, 0, st>>>(static_cast<const __half *>(scales),
-                                                            static_cast<const __half *>(biases),
-                                                            static_cast<const __half *>(a),
-                                                            static_cast<const uint32_t *>(b),
-                                                            static_cast<__half *>(out), M, N, K);
+        bits == 8 ? vanilla_t<__half, 8>(scales, biases, a, b, out, M, N, K, grid, st) : vanilla_t<__half, 4>(scales, biases, a, b, out, M, N, K, grid, st);
     else
         return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
     TL_LAUNCH_CHECK("w4a16_vanilla");

@@ -21,6 +21,16 @@
 //                      quantized_matmul.metal:183-194) and stores them in the K-major 128-byte-swizzled layout
 //                      wgmma reads; then the warpgroup issues eight wgmma m64nNTk16 (fp32 accumulators in
 //                      registers) and dequantises the next block while they run (two A stages per warpgroup).
+//
+// 8-bit codes (BITS = 8, b [K, N/4], code i of a word = (w >> 8i) & 255): a 128-byte box row holds ONE group, so a box
+// is one group block and is released after it.  Thread (row, half) reads 64 bytes = 64 codes.  The dequantiser keeps the
+// W4 rounding point, T(code * scale + bias) rounded once by one HFMA2 from the exact code:
+//   fp16: PRMT (0x64, q) -> 1024 + q, exact for every byte; HSUB2 -> q;
+//   bf16: 128 + q is exact only below q = 128, so PRMT (0x4B0000, q) -> fp32 2^23 + q, FADD -> q in fp32; q has at most
+//         8 significant bits, so the high halves of two such floats (one PRMT) are the bf16 codes, exactly.
+// Instruction budget per 64 codes (one thread, one block): fp16 32 PRMT + 32 HSUB2 + 32 HFMA2 (96); bf16 96 PRMT + 64 FADD
+// + 32 HFMA2 (192), against W4's 32 LOP3 + 24 SHF + 32 HSUB2 + 32 HFMA2 + 16 PRMT (136).  Per byte of weights that is
+// 1.5 (fp16) and 3.0 (bf16) instructions at 8 bits against 4.25 at 4 bits; per MMA, 0.7x and 1.4x of W4.
 #include <type_traits>
 
 #include "common.cuh"
@@ -84,9 +94,11 @@ struct SkNum<__half> {
 // GROUPED (MoE experts): the activation rows are sorted by expert; CTA row blockIdx.y is entry blockIdx.y of the tile
 // table (expert e, first sorted row), its weights are rows e K + tile * 128 of the stacked [E K, N / 8] experts, rows
 // past the expert's segment are computed and not stored, and CTAs past the table's count exit.  splits == 1.
-template <typename T, int NT, bool GROUPED = false>
+template <typename T, int NT, bool GROUPED = false, int BITS = 4>
 __global__ void __launch_bounds__(SK_THREADS, 1)
 w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const SkArgs args) {
+    static_assert(BITS == 4 || (BITS == 8 && !GROUPED), "8-bit codes: dense projections only");
+    constexpr int PG = BITS == 4 ? SK_PG : 1;  // group blocks per packed box
     using Smem = SkSmem<NT>;
     constexpr int PSTAGES = Smem::PSTAGES;
     constexpr int BSTAGES = Smem::BSTAGES;
@@ -138,14 +150,14 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 
     if (warp == 0) {
         // ------------------------------------------------ TMA producer: packed weights, one 128-row x 128-byte box per two group blocks
-        const int n_box = (n_gb + SK_PG - 1) / SK_PG;
+        const int n_box = (n_gb + PG - 1) / PG;
         int ps = 0;
         uint32_t ph = 1;  // producer side: the first pass through the ring does not wait
         for (int i = 0; i < n_box; ++i) {
             g_mbar_wait(p_empty + 8 * ps, ph);
             if (g_elect_one()) {
                 g_mbar_expect_tx(p_full + 8 * ps, SK_PACKED_BYTES);  // columns past the row end are zero-filled and still counted
-                g_tma_load_2d(p_base + ps * SK_PACKED_BYTES, &tmap_w, (gb0 + i * SK_PG) * (SK_GB / 2), wrow0, p_full + 8 * ps);
+                g_tma_load_2d(p_base + ps * SK_PACKED_BYTES, &tmap_w, (gb0 + i * PG) * (SK_GB * BITS / 8), wrow0, p_full + 8 * ps);
             }
             __syncwarp();
             if (++ps == PSTAGES) ps = 0, ph ^= 1u;
@@ -200,31 +212,62 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             // row `frow` of the box: 128 bytes = 8 chunks of 16 B, chunk c stored at (c ^ (row & 7)) by the TMA swizzle;
             // group block i is bytes [64 (i % 2), + 64), this thread's half of it 32 bytes = 64 codes
             const unsigned char *src = p_row + ps * SK_PACKED_BYTES;
-            const uint32_t c0 = static_cast<uint32_t>(4 * (i & 1) + 2 * half);
-            const uint4 lo = *reinterpret_cast<const uint4 *>(src + ((c0 ^ swz) << 4));
-            const uint4 hi = *reinterpret_cast<const uint4 *>(src + (((c0 + 1) ^ swz) << 4));
             uint32_t outw[32];
-            const uint32_t wv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+            if constexpr (BITS == 8) {
+                // this thread's half of the group: chunks 4 half .. 4 half + 3 of the row, codes in byte order
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                uint32_t p[4];
+                for (int c = 0; c < 4; ++c) {
+                    const uint4 v4 = *reinterpret_cast<const uint4 *>(src + (((static_cast<uint32_t>(4 * half + c)) ^ swz) << 4));
+                    const uint32_t wv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    uint32_t bits;  // (128 + code_q, 128 + code_{q+4}) in one LOP3: ((w >> 4q) & 0x000F000F) | magic
-                    asm("lop3.b32 %0, %1, 0x000F000F, %2, 0xEA;" : "=r"(bits) : "r"(wv[j] >> (4 * q)), "r"(magic));
-                    V2 code = __hsub2(*reinterpret_cast<V2 *>(&bits), offset2);
-                    V2 v = __hfma2(code, s2, b2);                                   // code * scale + bias, one rounding
-                    p[q] = *reinterpret_cast<uint32_t *>(&v);
+                    for (int j = 0; j < 4; ++j) {
+                        if constexpr (std::is_same<T, __half>::value) {
+#pragma unroll
+                            for (int q = 0; q < 2; ++q) {
+                                uint32_t bits = __byte_perm(wv[j], 0x64646464u, q == 0 ? 0x4140 : 0x4342);  // (1024 + c_2q, 1024 + c_2q+1)
+                                V2 code = __hsub2(*reinterpret_cast<V2 *>(&bits), offset2);
+                                V2 v = __hfma2(code, s2, b2);
+                                outw[8 * c + 2 * j + q] = *reinterpret_cast<uint32_t *>(&v);
+                            }
+                        } else {
+                            uint32_t f[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) f[q] = __float_as_uint(__uint_as_float(__byte_perm(wv[j], 0x4B000000u, 0x7440 | q)) - 8388608.f);
+#pragma unroll
+                            for (int q = 0; q < 2; ++q) {
+                                uint32_t bits = __byte_perm(f[2 * q], f[2 * q + 1], 0x7632);  // (c_2q, c_2q+1) in bf16
+                                V2 v = __hfma2(*reinterpret_cast<V2 *>(&bits), s2, b2);
+                                outw[8 * c + 2 * j + q] = *reinterpret_cast<uint32_t *>(&v);
+                            }
+                        }
+                    }
                 }
-                outw[4 * j + 0] = __byte_perm(p[0], p[1], 0x5410);  // (e0, e1)
-                outw[4 * j + 1] = __byte_perm(p[2], p[3], 0x5410);  // (e2, e3)
-                outw[4 * j + 2] = __byte_perm(p[0], p[1], 0x7632);  // (e4, e5)
-                outw[4 * j + 3] = __byte_perm(p[2], p[3], 0x7632);  // (e6, e7)
+            } else {
+                const uint32_t c0 = static_cast<uint32_t>(4 * (i & 1) + 2 * half);
+                const uint4 lo = *reinterpret_cast<const uint4 *>(src + ((c0 ^ swz) << 4));
+                const uint4 hi = *reinterpret_cast<const uint4 *>(src + (((c0 + 1) ^ swz) << 4));
+                const uint32_t wv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    uint32_t p[4];
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        uint32_t bits;  // (128 + code_q, 128 + code_{q+4}) in one LOP3: ((w >> 4q) & 0x000F000F) | magic
+                        asm("lop3.b32 %0, %1, 0x000F000F, %2, 0xEA;" : "=r"(bits) : "r"(wv[j] >> (4 * q)), "r"(magic));
+                        V2 code = __hsub2(*reinterpret_cast<V2 *>(&bits), offset2);
+                        V2 v = __hfma2(code, s2, b2);                                   // code * scale + bias, one rounding
+                        p[q] = *reinterpret_cast<uint32_t *>(&v);
+                    }
+                    outw[4 * j + 0] = __byte_perm(p[0], p[1], 0x5410);  // (e0, e1)
+                    outw[4 * j + 1] = __byte_perm(p[2], p[3], 0x5410);  // (e2, e3)
+                    outw[4 * j + 2] = __byte_perm(p[0], p[1], 0x7632);  // (e4, e5)
+                    outw[4 * j + 3] = __byte_perm(p[2], p[3], 0x7632);  // (e6, e7)
+                }
             }
             // The box is released only now: the arithmetic above consumed the loaded words, so this warp's
             // shared-memory reads of the box have completed (mbarrier operations are not ordered behind loads).
             __syncwarp();
-            g_mbar_arrive_if(p_empty + 8 * ps, lane == 0 && ((i & 1) || i + 1 == n_gb));
+            g_mbar_arrive_if(p_empty + 8 * ps, lane == 0 && (PG == 1 || (i & 1) || i + 1 == n_gb));
             // A stage s was last read by the MMAs of block i - 2, complete since wgmma_wait<1> of block i - 1
             unsigned char *dst = a_row + s * SK_A_BYTES;
 #pragma unroll
@@ -248,7 +291,7 @@ w4a16_skinny_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             wgmma_reg_fence(acc);
             g_mbar_arrive_if(b_empty + 8 * prev_bs, i > 0 && t == 0);
             prev_bs = bs;
-            if ((i & 1) || i + 1 == n_gb)
+            if (PG == 1 || (i & 1) || i + 1 == n_gb)
                 if (++ps == PSTAGES) ps = 0, php ^= 1u;
             if (++bs == BSTAGES) bs = 0, phb ^= 1u;
         }
@@ -437,14 +480,14 @@ size_t w4a16_skinny_workspace(int M, int N, int K) {
     return splits > 1 ? static_cast<size_t>(splits) * M * K * sizeof(float) : 0;
 }
 
-// Tensor maps of the activations a [M, N] (16-bit, [nt tokens x 64] boxes) and of the packed weights b [K, N/2] (bytes,
-// 128 rows x 128-byte boxes), both with the 128-byte swizzle wgmma reads.
+// Tensor maps of the activations a [M, N] (16-bit, [nt tokens x 64] boxes) and of the packed weights b [K, N * bits / 8]
+// (bytes, 128 rows x 128-byte boxes), both with the 128-byte swizzle wgmma reads.
 template <typename T>
-static int sk_maps(CUtensorMap *ma, CUtensorMap *mw, const void *a, const void *b, int M, int N, int K, int nt) {
+static int sk_maps(CUtensorMap *ma, CUtensorMap *mw, const void *a, const void *b, int M, int N, int K, int nt, int bits = 4) {
     const CUtensorMapDataType dt = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     const cuuint64_t a_dims[2] = {static_cast<cuuint64_t>(N), static_cast<cuuint64_t>(M)};
     const cuuint32_t a_box[2] = {SK_KB, static_cast<cuuint32_t>(nt)};
-    const cuuint64_t w_dims[2] = {static_cast<cuuint64_t>(N) / 2, static_cast<cuuint64_t>(K)};
+    const cuuint64_t w_dims[2] = {static_cast<cuuint64_t>(N) * bits / 8, static_cast<cuuint64_t>(K)};
     const cuuint32_t w_box[2] = {SK_PG * SK_GB / 2, SK_FEAT};
     if (int e = cached_tensor_map(ma, a, dt, 2, a_dims, a_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "quantized_matmul"))
         return e;
@@ -452,10 +495,10 @@ static int sk_maps(CUtensorMap *ma, CUtensorMap *mw, const void *a, const void *
                              "quantized_matmul");
 }
 
-template <typename T, int NT, bool GROUPED = false>
+template <typename T, int NT, bool GROUPED = false, int BITS = 4>
 static int skinny_launch(const CUtensorMap &ma, const CUtensorMap &mw, const SkArgs &args, dim3 grid, cudaStream_t st) {
     constexpr size_t smem = SkSmem<NT>::BYTES;
-    auto *kernel = w4a16_skinny_kernel<T, NT, GROUPED>;
+    auto *kernel = w4a16_skinny_kernel<T, NT, GROUPED, BITS>;
     static bool configured = false;
     if (!configured) {
         if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess ||
@@ -472,7 +515,7 @@ static int skinny_launch(const CUtensorMap &ma, const CUtensorMap &mw, const SkA
 template <typename T>
 static int skinny_t(const void *scales, const void *biases, const void *a, const void *b, void *out, const void *residual, int M, int N, int K,
                     int epilogue, void *ws, size_t ws_bytes, const void *norm_w, float norm_eps, void *normed, bool *norm_done, cudaStream_t st,
-                    int *planes_out) {
+                    int *planes_out, int bits) {
     if (!aligned16(a) || !aligned16(b)) return fail(TL_EINVAL, "quantized_matmul: a and b must be 16-byte aligned");
     const int NT = M <= 16 ? 16 : (M <= 32 ? 32 : (M <= 64 ? 64 : 128));
     const int tiles = (K + SK_FEAT - 1) / SK_FEAT;
@@ -484,14 +527,23 @@ static int skinny_t(const void *scales, const void *biases, const void *a, const
         return fail(TL_EWORKSPACE, "quantized_matmul: workspace too small (%zu < %zu)", ws_bytes, w4a16_skinny_workspace(M, N, K));
     args.partials = static_cast<float *>(ws);
     CUtensorMap ma, mw;
-    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, NT)) return e;
+    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, NT, bits)) return e;
     const dim3 grid(tiles * args.splits);
     int rc;
-    switch (NT) {
-        case 16: rc = skinny_launch<T, 16>(ma, mw, args, grid, st); break;
-        case 32: rc = skinny_launch<T, 32>(ma, mw, args, grid, st); break;
-        case 64: rc = skinny_launch<T, 64>(ma, mw, args, grid, st); break;
-        default: rc = skinny_launch<T, 128>(ma, mw, args, grid, st); break;
+    if (bits == 8) {
+        switch (NT) {
+            case 16: rc = skinny_launch<T, 16, false, 8>(ma, mw, args, grid, st); break;
+            case 32: rc = skinny_launch<T, 32, false, 8>(ma, mw, args, grid, st); break;
+            case 64: rc = skinny_launch<T, 64, false, 8>(ma, mw, args, grid, st); break;
+            default: rc = skinny_launch<T, 128, false, 8>(ma, mw, args, grid, st); break;
+        }
+    } else {
+        switch (NT) {
+            case 16: rc = skinny_launch<T, 16>(ma, mw, args, grid, st); break;
+            case 32: rc = skinny_launch<T, 32>(ma, mw, args, grid, st); break;
+            case 64: rc = skinny_launch<T, 64>(ma, mw, args, grid, st); break;
+            default: rc = skinny_launch<T, 128>(ma, mw, args, grid, st); break;
+        }
     }
     if (planes_out != nullptr) {  // the caller adds the planes itself (fused consumer); 1 = `out` holds the finished result
         *planes_out = args.splits;
@@ -518,7 +570,7 @@ static int skinny_t(const void *scales, const void *biases, const void *a, const
 
 int launch_w4a16_skinny(const void *scales, const void *biases, const void *a, const void *b, void *out, const void *residual, int M, int N,
                         int K, int epilogue, int dtype, void *ws, size_t ws_bytes, cudaStream_t st, const void *norm_w, float norm_eps, void *normed,
-                        bool *norm_done, int *planes_out) {
+                        bool *norm_done, int *planes_out, int bits) {
     bool unused = false;
     if (norm_done == nullptr) norm_done = &unused;
     *norm_done = false;
@@ -526,32 +578,33 @@ int launch_w4a16_skinny(const void *scales, const void *biases, const void *a, c
     if (epilogue == SK_EPI_SWIGLU_PAIRS && K % 16 != 0) return fail(TL_EINVAL, "quantized_matmul: interleaved gate|up rows need K %% 16 == 0");
     if (dtype == TL_BF16)
         return skinny_t<__nv_bfloat16>(scales, biases, a, b, out, residual, M, N, K, epilogue, ws, ws_bytes, norm_w, norm_eps, normed, norm_done, st,
-                                       planes_out);
+                                       planes_out, bits);
     if (dtype == TL_F16)
-        return skinny_t<__half>(scales, biases, a, b, out, residual, M, N, K, epilogue, ws, ws_bytes, norm_w, norm_eps, normed, norm_done, st, planes_out);
+        return skinny_t<__half>(scales, biases, a, b, out, residual, M, N, K, epilogue, ws, ws_bytes, norm_w, norm_eps, normed, norm_done, st, planes_out,
+                                bits);
     return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
 }
 
 // Prefill GEMM (any M): 128-token tiles along grid.y, the whole reduction per CTA, the epilogue in the kernel.
 template <typename T>
-static int tiles_t(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, cudaStream_t st) {
+static int tiles_t(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, cudaStream_t st, int bits) {
     if (!aligned16(a) || !aligned16(b)) return fail(TL_EINVAL, "quantized_matmul: a and b must be 16-byte aligned");
     SkArgs args{};
     args.scales = scales, args.biases = biases, args.out = out;
     args.M = M, args.N = N, args.K = K, args.epilogue = SK_EPI_NONE;
     args.splits = 1, args.gb_per_split = N / SK_GB;
     CUtensorMap ma, mw;
-    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, 128)) return e;
+    if (int e = sk_maps<T>(&ma, &mw, a, b, M, N, K, 128, bits)) return e;
     const dim3 grid((K + SK_FEAT - 1) / SK_FEAT, (M + 127) / 128);
     if (grid.y > 65535) return fail(TL_EINVAL, "quantized_matmul: too many rows for one launch");
-    return skinny_launch<T, 128>(ma, mw, args, grid, st);
+    return bits == 8 ? skinny_launch<T, 128, false, 8>(ma, mw, args, grid, st) : skinny_launch<T, 128>(ma, mw, args, grid, st);
 }
 
 int launch_w4a16_tiles(const void *scales, const void *biases, const void *a, const void *b, void *out, int M, int N, int K, int dtype,
-                       cudaStream_t st) {
+                       cudaStream_t st, int bits) {
     if (M == 0 || K == 0) return TL_OK;
-    if (dtype == TL_BF16) return tiles_t<__nv_bfloat16>(scales, biases, a, b, out, M, N, K, st);
-    if (dtype == TL_F16) return tiles_t<__half>(scales, biases, a, b, out, M, N, K, st);
+    if (dtype == TL_BF16) return tiles_t<__nv_bfloat16>(scales, biases, a, b, out, M, N, K, st, bits);
+    if (dtype == TL_F16) return tiles_t<__half>(scales, biases, a, b, out, M, N, K, st, bits);
     return fail(TL_EDTYPE, "quantized_matmul: scales must be float16 or bfloat16");
 }
 

@@ -107,6 +107,9 @@ _SIGNATURES = {
     "tl_quantized_matmul_workspace": (_SZ, [_I] * 6),
     "tl_quantized_matmul": (_I, [_VP] * 5 + [_I] * 6 + [_VP, _SZ, _VP]),
     "tl_quantized_embedding": (_I, [_VP] * 5 + [_I] * 4 + [_VP]),
+    "tl_quantized_matmul_workspace_bits": (_SZ, [_I] * 7),
+    "tl_quantized_matmul_bits": (_I, [_VP] * 5 + [_I] * 7 + [_VP, _SZ, _VP]),
+    "tl_quantized_embedding_bits": (_I, [_VP] * 5 + [_I] * 5 + [_VP]),
     "tl_rms_norm": (_I, [_VP] * 3 + [_I, _I, _F, _I, _VP]),
     "tl_rope": (_I, [_VP] * 3 + [_I] * 5 + [_F, _I, _I, _VP]),
     "tl_rope_table": (_I, [_VP] * 3 + [_I] * 5 + [_F, _I, _I, _VP, _VP]),
@@ -136,6 +139,8 @@ _SIGNATURES = {
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_qkv_project_rope_append_table": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP, _VP]),
+    "tl_qkv_project_rope_append_bits": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 6 + [_VP, _SZ, _VP]),
+    "tl_qkv_project_rope_append_table_bits": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 6 + [_VP, _SZ, _VP, _VP]),
     "tl_paged_attention_token_major": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
     "tl_paged_attention_token_major_workspace": (_SZ, [_I] * 4),
     "tl_paged_attention_token_major_split": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP, _SZ, _VP]),
@@ -143,6 +148,10 @@ _SIGNATURES = {
     "tl_quantized_matmul_route": (_I, [_I] * 8 + [_VP] * 4 + [ctypes.POINTER(_I)] * 4),
     "tl_quantized_matmul_fused": (_I, [_VP] * 7 + [_I] * 6 + [_F, _I, _VP, _SZ, _VP]),
     "tl_quantized_matmul_residual_norm": (_I, [_VP] * 8 + [_I] * 3 + [_F, _I, _VP, _SZ, _VP]),
+    "tl_quantized_matmul_fused_workspace_bits": (_SZ, [_I] * 7),
+    "tl_quantized_matmul_route_bits": (_I, [_I] * 9 + [_VP] * 4 + [ctypes.POINTER(_I)] * 4),
+    "tl_quantized_matmul_fused_bits": (_I, [_VP] * 7 + [_I] * 6 + [_F, _I, _I, _VP, _SZ, _VP]),
+    "tl_quantized_matmul_residual_norm_bits": (_I, [_VP] * 8 + [_I] * 3 + [_F, _I, _I, _VP, _SZ, _VP]),
     "tl_decode_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
     "tl_decode_qk_norm_rope_append_table": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP, _VP]),
     "tl_chunk_qk_norm_rope_append": (_I, [_VP] * 9 + [_I] * 4 + [_F, _F] + [_I] * 4 + [_VP]),
@@ -298,7 +307,7 @@ def quantized_matmul(
     use_split_k=False,
     stream=None,
 ):
-    """``a [M,N] @ dequant(b [K,N/8]).T -> [M,K]`` (bindings.cpp:16-33)."""
+    """``a [M,N] @ dequant(b [K,N*bits/32]).T -> [M,K]`` (bindings.cpp:16-33); ``bits`` is 4 or 8."""
     if scales.dtype not in _HALF:
         raise RuntimeError("quantized_matmul: scales must be float16 or bfloat16")
     if scales.dtype != biases.dtype:
@@ -311,8 +320,8 @@ def quantized_matmul(
         raise RuntimeError("quantized_matmul: a must be a 2D array")
     if b.dim() != 2:
         raise RuntimeError("quantized_matmul: b must be a 2D array")
-    if bits != 4:
-        raise RuntimeError("quantized_matmul: bits must be 4")
+    if bits not in (4, 8):
+        raise RuntimeError("quantized_matmul: bits must be 4 or 8")
     if group_size != 128:
         raise RuntimeError("quantized_matmul: group_size must be 128")
     if not transpose_b:
@@ -325,7 +334,7 @@ def quantized_matmul(
         raise RuntimeError("quantized_matmul: a columns must be divisible by group_size")
     if scales.shape[1] != a.shape[1] // group_size:
         raise RuntimeError("quantized_matmul: scales must have one column per input group")
-    if b.shape[1] != a.shape[1] // 8:
+    if b.shape[1] != a.shape[1] * bits // 32:
         raise RuntimeError("quantized_matmul: a must have the same number of columns as b")
     _gpu("quantized_matmul", scales, biases, a, b)
     _contig("quantized_matmul", a=a, b=b, scales=scales, biases=biases)
@@ -333,11 +342,11 @@ def quantized_matmul(
     K = b.shape[0]
     out = torch.empty((M, K), dtype=a.dtype, device=a.device)
     code = _DTYPE_CODE[a.dtype]
-    ws_bytes = _lib.tl_quantized_matmul_workspace(M, N, K, code, int(use_simdgroup), int(use_split_k))
+    ws_bytes = _lib.tl_quantized_matmul_workspace_bits(M, N, K, code, int(bits), int(use_simdgroup), int(use_split_k))
     ws = _zero_workspace(ws_bytes, a.device)
     _check(
-        _lib.tl_quantized_matmul(
-            scales.data_ptr(), biases.data_ptr(), a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, code,
+        _lib.tl_quantized_matmul_bits(
+            scales.data_ptr(), biases.data_ptr(), a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, code, int(bits),
             int(use_simdgroup), int(use_split_k), None if ws is None else ws.data_ptr(), ws_bytes,
             _stream_ptr(stream, a),
         )
@@ -346,23 +355,24 @@ def quantized_matmul(
 
 
 def quantized_embedding(indices, scales, biases, weight, group_size, bits, stream=None):
-    """Row gather + dequantise (bindings.cpp:34-35)."""
+    """Row gather + dequantise (bindings.cpp:34-35); ``bits`` is 4 or 8."""
     if indices.dtype not in _PACKED or weight.dtype not in _PACKED:
         raise RuntimeError("quantized_embedding: indices and weight must use 32-bit integers")
     if scales.dtype != biases.dtype or scales.dtype not in _HALF:
         raise RuntimeError("quantized_embedding: scales and biases must have the same 16-bit dtype")
-    if group_size != 128 or bits != 4 or scales.shape != biases.shape:
-        raise RuntimeError("quantized_embedding: expected 4-bit weights with group size 128")
-    dim = weight.shape[1] * 8
+    if group_size != 128 or bits not in (4, 8) or scales.shape != biases.shape:
+        raise RuntimeError("quantized_embedding: expected 4-bit weights with group size 128" if bits == 4 else
+                           "quantized_embedding: expected 4- or 8-bit weights with group size 128")
+    dim = weight.shape[1] * 32 // bits
     if scales.shape[0] != weight.shape[0] or scales.shape[1] != dim // group_size:
         raise RuntimeError("quantized_embedding: incompatible parameter shapes")
     _gpu("quantized_embedding", indices, scales, biases, weight)
     _contig("quantized_embedding", indices=indices, scales=scales, biases=biases, weight=weight)
     out = torch.empty((*indices.shape, dim), dtype=scales.dtype, device=scales.device)
     _check(
-        _lib.tl_quantized_embedding(
+        _lib.tl_quantized_embedding_bits(
             indices.data_ptr(), scales.data_ptr(), biases.data_ptr(), weight.data_ptr(), out.data_ptr(),
-            indices.numel(), weight.shape[0], dim, _DTYPE_CODE[scales.dtype], _stream_ptr(stream, scales),
+            indices.numel(), weight.shape[0], dim, _DTYPE_CODE[scales.dtype], int(bits), _stream_ptr(stream, scales),
         )
     )
     return out
@@ -1098,17 +1108,25 @@ PRO_NONE, PRO_RMSNORM, PRO_SWIGLU = 0, 1, 2
 EPI_NONE, EPI_RESIDUAL, EPI_SWIGLU_PAIRS = 0, 1, 2
 
 
+def packed_bits(b, N: int):
+    """Code width of packed weights ``b [K, N * bits / 32]`` over ``N`` inputs, ``32 * b.shape[1] / N``: 4 or 8, else
+    None (the fused functions refuse it)."""
+    bits, rem = divmod(32 * b.shape[1], N) if N > 0 else (0, 1)
+    return bits if rem == 0 and bits in (4, 8) else None
+
+
 def quantized_matmul_fused(scales, biases, b, p0, p1=None, residual=None, prologue=PRO_NONE, epilogue=EPI_NONE, eps=0.0,
                            out=None, stream=None):
     """Decode projection with the neighbouring element-wise operator folded in
     (``include/tiny_llm_b200.h``): ``p0`` is ``[M, N]`` (row stride ``p0.stride(0)``),
-    ``b`` ``[K, N/8]``; bit-identical to the unfused operator sequence."""
+    ``b`` ``[K, N/8]`` (4-bit codes) or ``[K, N/4]`` (8-bit); bit-identical to the unfused operator sequence."""
     if p0.dim() != 2 or b.dim() != 2 or p0.stride(1) != 1:
         raise RuntimeError("quantized_matmul_fused: p0 must be 2D with unit inner stride")
     M, N = p0.shape
     K = b.shape[0]
-    if b.shape[1] * 8 != N or tuple(scales.shape) != (K, N // 128) or scales.shape != biases.shape:
-        raise RuntimeError("quantized_matmul_fused: incompatible parameter shapes")
+    bits = packed_bits(b, N)
+    if bits is None or tuple(scales.shape) != (K, N // 128) or scales.shape != biases.shape:
+        raise RuntimeError("quantized_matmul_fused: incompatible parameter shapes (b must hold 4- or 8-bit codes: [K, N/8] or [K, N/4])")
     if scales.dtype not in _HALF or p0.dtype != scales.dtype or biases.dtype != scales.dtype:
         raise RuntimeError("quantized_matmul: a must be the same dtype as scales")
     _gpu("quantized_matmul_fused", scales, biases, b, p0)
@@ -1125,13 +1143,13 @@ def quantized_matmul_fused(scales, biases, b, p0, p1=None, residual=None, prolog
     if out is None:
         out = torch.empty((M, K // 2 if epilogue == EPI_SWIGLU_PAIRS else K), dtype=p0.dtype, device=p0.device)
     code = _DTYPE_CODE[p0.dtype]
-    ws_bytes = _lib.tl_quantized_matmul_fused_workspace(M, N, K, lda, int(prologue), code)
+    ws_bytes = _lib.tl_quantized_matmul_fused_workspace_bits(M, N, K, lda, int(prologue), code, bits)
     ws = _zero_workspace(ws_bytes, p0.device)
     _check(
-        _lib.tl_quantized_matmul_fused(
+        _lib.tl_quantized_matmul_fused_bits(
             scales.data_ptr(), biases.data_ptr(), b.data_ptr(), out.data_ptr(), p0.data_ptr(),
             None if p1 is None else p1.data_ptr(), None if residual is None else residual.data_ptr(), M, N, K, lda,
-            int(prologue), int(epilogue), float(eps), code, None if ws is None else ws.data_ptr(), ws_bytes,
+            int(prologue), int(epilogue), float(eps), code, bits, None if ws is None else ws.data_ptr(), ws_bytes,
             _stream_ptr(stream, p0),
         )
     )
@@ -1141,19 +1159,20 @@ def quantized_matmul_fused(scales, biases, b, p0, p1=None, residual=None, prolog
 W4_VANILLA, W4_STREAM, W4_SKINNY, W4_TILES = 0, 1, 2, 3
 
 
-def quantized_matmul_route(M, N, K, lda, prologue, fused, use_simdgroup, dtype, a, b, scales, biases):
+def quantized_matmul_route(M, N, K, lda, prologue, fused, use_simdgroup, dtype, a, b, scales, biases, bits=4):
     """The kernel a W4A16 projection runs, decided without launching or reading anything: ``(route, splits,
     gb_per_split, rows_per_pass, units)`` with ``route`` one of ``W4_VANILLA`` / ``W4_STREAM`` / ``W4_SKINNY`` /
     ``W4_TILES`` (``include/tiny_llm_b200.h`` documents the other fields).  ``fused`` selects the rule of
     ``quantized_matmul_fused`` / ``quantized_matmul_residual_norm``.  ``a``, ``b``, ``scales`` and ``biases`` are tensors
-    or plain addresses: only their alignment counts.  ``dtype`` is a torch dtype."""
+    or plain addresses: only their alignment counts.  ``dtype`` is a torch dtype; ``bits`` (4 or 8) the code width."""
 
     def addr(x):
         return x.data_ptr() if isinstance(x, torch.Tensor) else int(x)
 
     facts = [_I() for _ in range(4)]
-    code = _lib.tl_quantized_matmul_route(int(M), int(N), int(K), int(lda), int(prologue), int(bool(fused)), int(bool(use_simdgroup)),
-                                          _DTYPE_CODE[dtype], addr(a), addr(b), addr(scales), addr(biases), *map(ctypes.byref, facts))
+    code = _lib.tl_quantized_matmul_route_bits(int(M), int(N), int(K), int(lda), int(prologue), int(bool(fused)), int(bool(use_simdgroup)),
+                                               _DTYPE_CODE[dtype], int(bits), addr(a), addr(b), addr(scales), addr(biases),
+                                               *map(ctypes.byref, facts))
     _check(min(code, 0))
     return (code, *(f.value for f in facts))
 
@@ -1299,8 +1318,9 @@ def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight,
         raise RuntimeError("quantized_matmul_residual_norm: p0 must be contiguous [M, N]")
     M, N = p0.shape
     K = b.shape[0]
-    if b.shape[1] * 8 != N or tuple(scales.shape) != (K, N // 128) or scales.shape != biases.shape:
-        raise RuntimeError("quantized_matmul_fused: incompatible parameter shapes")
+    bits = packed_bits(b, N)
+    if bits is None or tuple(scales.shape) != (K, N // 128) or scales.shape != biases.shape:
+        raise RuntimeError("quantized_matmul_fused: incompatible parameter shapes (b must hold 4- or 8-bit codes: [K, N/8] or [K, N/4])")
     if scales.dtype not in _HALF or p0.dtype != scales.dtype or biases.dtype != scales.dtype or norm_weight.dtype != scales.dtype:
         raise RuntimeError("quantized_matmul: a must be the same dtype as scales")
     if tuple(residual.shape) != (M, K) or not residual.is_contiguous() or residual.dtype != p0.dtype:
@@ -1312,12 +1332,12 @@ def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight,
     out = torch.empty((M, K), dtype=p0.dtype, device=p0.device)
     normed = torch.empty_like(out)
     code = _DTYPE_CODE[p0.dtype]
-    ws_bytes = _lib.tl_quantized_matmul_fused_workspace(M, N, K, N, int(PRO_NONE), code)
+    ws_bytes = _lib.tl_quantized_matmul_fused_workspace_bits(M, N, K, N, int(PRO_NONE), code, bits)
     ws = _zero_workspace(ws_bytes, p0.device)
     _check(
-        _lib.tl_quantized_matmul_residual_norm(
+        _lib.tl_quantized_matmul_residual_norm_bits(
             scales.data_ptr(), biases.data_ptr(), b.data_ptr(), out.data_ptr(), p0.data_ptr(), residual.data_ptr(), norm_weight.data_ptr(),
-            normed.data_ptr(), M, N, K, float(norm_eps), code, None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, p0),
+            normed.data_ptr(), M, N, K, float(norm_eps), code, bits, None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, p0),
         )
     )
     return out, normed
@@ -1397,7 +1417,8 @@ def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight,
     rows, N = p0.shape
     P, Hkv, page_size, D = key_pages.shape
     K = b.shape[0]
-    if K != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads or b.shape[1] * 8 != N:
+    bits = packed_bits(b, N)
+    if K != (num_heads + 2 * num_kv_heads) * D or Hkv != num_kv_heads or bits is None:
         raise RuntimeError("qkv_project_rope_append: weight rows must be (Hq + 2*Hkv) * D")
     if (p0.dtype != torch.bfloat16 or key_pages.dtype != p0.dtype or value_pages.dtype != p0.dtype or scales.dtype != p0.dtype
             or biases.dtype != p0.dtype or not p0.is_contiguous()):
@@ -1413,14 +1434,14 @@ def qkv_project_rope_append(scales, biases, b, p0, q_norm_weight, k_norm_weight,
     scratch = torch.empty((rows, K), dtype=p0.dtype, device=p0.device)
     q_out = torch.empty((num_heads, rows, D) if chunk else (rows, num_heads, D), dtype=p0.dtype, device=p0.device)
     code = _DTYPE_CODE[p0.dtype]
-    ws_bytes = _lib.tl_quantized_matmul_fused_workspace(rows, N, K, N, int(PRO_NONE), code)
+    ws_bytes = _lib.tl_quantized_matmul_fused_workspace_bits(rows, N, K, N, int(PRO_NONE), code, bits)
     ws = _zero_workspace(ws_bytes, p0.device)
     max_pages = block_table.shape[-1]
     args = (scales.data_ptr(), biases.data_ptr(), b.data_ptr(), p0.data_ptr(), scratch.data_ptr(), q_norm_weight.data_ptr(), k_norm_weight.data_ptr(),
             offsets.data_ptr(), block_table.data_ptr(), context_lens.data_ptr(), q_out.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(),
-            rows, N, int(num_heads), int(num_kv_heads), D, float(base), float(eps), P, page_size, max_pages, int(bool(chunk)), code,
+            rows, N, int(num_heads), int(num_kv_heads), D, float(base), float(eps), P, page_size, max_pages, int(bool(chunk)), code, bits,
             None if ws is None else ws.data_ptr(), ws_bytes, _stream_ptr(stream, p0))
-    _check(_lib.tl_qkv_project_rope_append(*args) if inv_freq is None else _lib.tl_qkv_project_rope_append_table(*args, inv_freq.data_ptr()))
+    _check(_lib.tl_qkv_project_rope_append_bits(*args) if inv_freq is None else _lib.tl_qkv_project_rope_append_table_bits(*args, inv_freq.data_ptr()))
     return q_out
 
 

@@ -53,6 +53,7 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
     config = json.loads((path / "config.json").read_text())
     quant = config.get("quantization") or config.get("quantization_config") or {}
     group_size, bits = int(quant.get("group_size", 128)), int(quant.get("bits", 4))
+    _check_quantization(quant, group_size, bits)
     if "head_dim" not in config:
         config["head_dim"] = config["hidden_size"] // config["num_attention_heads"]
     config.setdefault("tie_word_embeddings", True)
@@ -82,7 +83,11 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
             weight = weight.view(torch.uint32)
         if weight.dtype != torch.uint32:
             raise ValueError(f"{prefix}.weight is {weight.dtype}: expected packed uint32 (a {bits}-bit MLX checkpoint)")
-        return SimpleNamespace(weight=weight, scales=take(prefix + ".scales"), biases=take(prefix + ".biases"), group_size=group_size, bits=bits)
+        scales = take(prefix + ".scales")
+        if weight.dim() != 2 or scales.dim() != 2 or weight.shape[1] * 32 // bits != scales.shape[1] * group_size or (weight.shape[1] * 32) % bits:
+            raise ValueError(f"{prefix}: packed weight {tuple(weight.shape)} and scales {tuple(scales.shape)} do not match {bits}-bit codes "
+                             f"at group {group_size} (weight.shape[1] * 32 / bits must equal scales.shape[1] * {group_size})")
+        return SimpleNamespace(weight=weight, scales=scales, biases=take(prefix + ".biases"), group_size=group_size, bits=bits)
 
     def norm(prefix: str) -> SimpleNamespace:
         return SimpleNamespace(weight=take(prefix + ".weight"))
@@ -101,8 +106,20 @@ def load_checkpoint(path, device="cpu") -> SimpleNamespace:
     return model
 
 
+def _check_quantization(quant: dict, group_size: int, bits: int) -> None:
+    """The projection kernels take MLX affine 4- or 8-bit codes at group 128, one width for the whole model."""
+    if bits not in (4, 8):
+        raise ValueError(f"quantization.bits = {bits}: only 4- and 8-bit checkpoints are supported")
+    if group_size != 128:
+        raise ValueError(f"quantization.group_size = {group_size}: only group size 128 is supported (convert with --q-group-size 128)")
+    for key, value in quant.items():  # mlx-lm writes per-layer overrides as {"<layer path>": {"group_size", "bits"}}
+        if isinstance(value, dict) and (int(value.get("bits", bits)) != bits or int(value.get("group_size", group_size)) != group_size):
+            raise ValueError(f"quantization override for {key!r} ({value}) differs from the global {bits} bits / group {group_size}: "
+                             "mixed per-layer quantisation is not supported")
+
+
 def save_checkpoint(model_ns: SimpleNamespace, path) -> None:
-    """Write ``model_ns`` in the MLX 4-bit layout (config.json + model.safetensors)."""
+    """Write ``model_ns`` in the MLX layout of its width (config.json + model.safetensors)."""
     from safetensors.torch import save_file
 
     path = Path(path)

@@ -49,7 +49,8 @@ def _load(args, device):
 
     if args.synthetic:
         extra = {} if args.rope_scaling is None else {"rope_scaling": args.rope_scaling}
-        return (synthetic_qwen3(args.synthetic, seed=0, device=device, realistic=args.synthetic.startswith("tiny"), **extra), None,
+        return (synthetic_qwen3(args.synthetic, seed=0, device=device, realistic=args.synthetic.startswith("tiny"), bits=args.synthetic_bits,
+                                **extra), None,
                 "Qwen/Qwen3-synthetic")
     ns = load_checkpoint(args.model, device=device)
     tokenizer = None
@@ -472,6 +473,8 @@ def main(argv=None) -> int:
         p.set_defaults(fn=fn)
         p.add_argument("--model", default=None, help="checkpoint directory (config.json + *.safetensors [+ tokenizer files])")
         p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny, tiny-d128, qwen3-0.6b, qwen3-4b) instead of --model")
+        p.add_argument("--synthetic-bits", type=int, choices=(4, 8), default=4,
+                       help="code width of the --synthetic weights, and of a --draft-synthetic draft's (MLX affine, group 128)")
         p.add_argument("--prompt", default="Give me a short introduction to large language models.")
         p.add_argument("--prompt-ids", default=None, help="comma-separated token ids (';' between requests for `batch`)")
         p.add_argument("--loader", choices=["week2", "week3"], default="week3")
@@ -528,8 +531,9 @@ def main(argv=None) -> int:
                                          help="suffix lengths prompt lookup matches (1 <= MIN <= MAX <= 8)")
     p = sub.add_parser("embed")
     p.set_defaults(fn=cmd_embed, loader="week3", rope_scaling=None, max_context=None, disable_paged_attention=False, logprobs=None)
-    p.add_argument("--model", default=None, help="checkpoint directory (Qwen3 or Qwen3-Embedding, MLX 4-bit)")
+    p.add_argument("--model", default=None, help="checkpoint directory (Qwen3 or Qwen3-Embedding, MLX 4- or 8-bit)")
     p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny-d128, qwen3-0.6b, qwen3-4b) instead of --model")
+    p.add_argument("--synthetic-bits", type=int, choices=(4, 8), default=4, help="code width of the --synthetic weights (MLX affine, group 128)")
     p.add_argument("--prompt", action="append", default=None, help="a text to embed (repeatable; needs the tokenizer)")
     p.add_argument("--prompts-file", default=None, help="one text per line")
     p.add_argument("--prompt-ids", default=None, help="comma-separated token ids, ';' between prompts")
@@ -552,6 +556,8 @@ def main(argv=None) -> int:
         ap.error("--model or --synthetic is required")
     if args.rope_scaling is not None and not args.synthetic:
         ap.error("--rope-scaling applies to --synthetic; a checkpoint's config.json states its own rope_scaling")
+    if args.synthetic_bits != 4 and not args.synthetic:
+        ap.error("--synthetic-bits applies to --synthetic; a checkpoint's config.json states its own quantization")
     if args.command == "batch" and args.max_context is not None and args.max_seq_len > args.max_context:
         ap.error(f"--max-seq-len {args.max_seq_len} exceeds --max-context {args.max_context}")
     if args.logprobs is not None and not 0 <= args.logprobs <= 20:

@@ -22,6 +22,8 @@ from .quantize import QuantizedWeights, as_packed_i32, quantized_linear
 
 
 def _experts(w: QuantizedWeights, op: str) -> tuple[int, int, int]:
+    if w.bits == 8:
+        raise ValueError(f"{op}: Qwen3-MoE with 8-bit weights is not supported (there is no 8-bit grouped expert GEMM); use a 4-bit checkpoint")
     if w.weight.dim() != 3 or w.scales.dim() != 3 or w.group_size != 128 or w.bits != 4 or w.biases is None:
         raise ValueError(f"{op}: expert weights must be 4-bit / group 128 [E, out, in/8] with scales and biases [E, out, in/128]")
     E, out_dim, words = w.weight.shape

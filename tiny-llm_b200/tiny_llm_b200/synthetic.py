@@ -1,4 +1,4 @@
-"""Synthetic Qwen3-shaped W4A16 checkpoints in the ``mlx_model`` duck type.
+"""Synthetic Qwen3-shaped W4A16 (and W8A16) checkpoints in the ``mlx_model`` duck type.
 
 There is no network here, so benchmarks and tests run on random weights of the
 right architecture (SURVEY.md section 8d).  The object mirrors what
@@ -21,6 +21,7 @@ import torch
 
 GROUP_SIZE = 128
 BITS = 4
+SUPPORTED_BITS = (4, 8)  # MLX affine widths the projection kernels take, both at GROUP_SIZE
 
 # Published Qwen3 dense configs (hidden, layers, heads, kv heads, head dim, mlp).
 CONFIGS = {
@@ -85,20 +86,49 @@ def quantize_w4(weight: torch.Tensor, group_size: int = GROUP_SIZE):
     return words.view(torch.uint32), scale_b.squeeze(-1).contiguous(), bias_b.squeeze(-1).contiguous()
 
 
-def _random_layer(out_dim: int, in_dim: int, gen: torch.Generator) -> SimpleNamespace:
+def quantize_affine(weight: torch.Tensor, bits: int, group_size: int = GROUP_SIZE):
+    """Affine min/max quantiser at ``bits`` (4 or 8): (packed uint32 [K, N * bits / 32], scales, biases), code ``j`` of
+    a word in bits ``[bits * j, bits * (j + 1))`` - the layout ``dequantize_weights`` decodes.  At 4 bits it computes
+    what ``quantize_w4`` does."""
+    if bits not in SUPPORTED_BITS:
+        raise ValueError(f"quantize_affine: bits must be 4 or 8, got {bits}")
+    K, N = weight.shape
+    assert N % group_size == 0
+    top = (1 << bits) - 1
+    groups = weight.to(torch.float32).reshape(K, N // group_size, group_size)
+    lo = groups.amin(dim=-1, keepdim=True)
+    hi = groups.amax(dim=-1, keepdim=True)
+    scale_b = ((hi - lo) / float(top)).clamp_min(1e-8).to(torch.bfloat16)
+    bias_b = lo.to(torch.bfloat16)
+    codes = torch.round((groups - bias_b.to(torch.float32)) / scale_b.to(torch.float32)).clamp_(0, top).to(torch.int64)
+    return pack_codes(codes.reshape(K, N), bits), scale_b.squeeze(-1).contiguous(), bias_b.squeeze(-1).contiguous()
+
+
+def pack_codes(codes: torch.Tensor, bits: int) -> torch.Tensor:
+    """Integer codes [K, N] in ``[0, 2**bits)`` -> packed uint32 [K, N * bits / 32] (code j of a word at bit ``bits * j``)."""
+    K, N = codes.shape
+    per = 32 // bits
+    shifts = torch.arange(0, 32, bits, dtype=torch.int64)
+    words = (codes.to(torch.int64).reshape(K, N // per, per) << shifts).sum(dim=-1)  # < 2^32
+    return torch.where(words >= 2**31, words - 2**32, words).to(torch.int32).view(torch.uint32)
+
+
+def _random_layer(out_dim: int, in_dim: int, gen: torch.Generator, bits: int = BITS) -> SimpleNamespace:
     """Random codes + signed scales; dequantised weights ~ N(0, 1/in_dim)
-    (value = (q-7.5)*s + e with q uniform: var = 22.25*sigma^2)."""
+    (value = (q - c)*s + e with q uniform on [0, 2c]: 4 bits c = 7.5, var = 22.25*sigma^2; 8 bits c = 127.5 and
+    s scaled by 15/255, the same weight distribution)."""
     sigma = 1.0 / (4.717 * in_dim**0.5)
-    words = torch.randint(-(2**31), 2**31, (out_dim, in_dim // 8), dtype=torch.int64, generator=gen).to(torch.int32)
-    scales = (torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * sigma).to(torch.bfloat16)
-    biases = (-7.5 * scales.to(torch.float32) + torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * sigma).to(torch.bfloat16)
-    return SimpleNamespace(weight=words.view(torch.uint32), scales=scales, biases=biases, group_size=GROUP_SIZE, bits=BITS)
+    centre, step = (7.5, 1.0) if bits == 4 else (127.5, 15.0 / 255.0)
+    words = torch.randint(-(2**31), 2**31, (out_dim, in_dim * bits // 32), dtype=torch.int64, generator=gen).to(torch.int32)
+    scales = (torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * (sigma * step)).to(torch.bfloat16)
+    biases = (-centre * scales.to(torch.float32) + torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * sigma).to(torch.bfloat16)
+    return SimpleNamespace(weight=words.view(torch.uint32), scales=scales, biases=biases, group_size=GROUP_SIZE, bits=bits)
 
 
-def _quantized_layer(out_dim: int, in_dim: int, gen: torch.Generator, std: float) -> SimpleNamespace:
+def _quantized_layer(out_dim: int, in_dim: int, gen: torch.Generator, std: float, bits: int = BITS) -> SimpleNamespace:
     dense = torch.randn(out_dim, in_dim, generator=gen) * std
-    words, scales, biases = quantize_w4(dense)
-    return SimpleNamespace(weight=words, scales=scales, biases=biases, group_size=GROUP_SIZE, bits=BITS)
+    words, scales, biases = quantize_w4(dense) if bits == 4 else quantize_affine(dense, bits)
+    return SimpleNamespace(weight=words, scales=scales, biases=biases, group_size=GROUP_SIZE, bits=bits)
 
 
 def _norm_weight(dim: int, gen: torch.Generator) -> SimpleNamespace:
@@ -109,32 +139,34 @@ def _empty_norm(dim: int, device) -> SimpleNamespace:
     return SimpleNamespace(weight=torch.empty((dim,), dtype=torch.bfloat16, device=device))
 
 
-def _empty_layer(out_dim: int, in_dim: int, device) -> SimpleNamespace:
+def _empty_layer(out_dim: int, in_dim: int, device, bits: int = BITS) -> SimpleNamespace:
     return SimpleNamespace(
-        weight=torch.empty((out_dim, in_dim // 8), dtype=torch.int32, device=device).view(torch.uint32),
+        weight=torch.empty((out_dim, in_dim * bits // 32), dtype=torch.int32, device=device).view(torch.uint32),
         scales=torch.empty((out_dim, in_dim // GROUP_SIZE), dtype=torch.bfloat16, device=device),
         biases=torch.empty((out_dim, in_dim // GROUP_SIZE), dtype=torch.bfloat16, device=device),
         group_size=GROUP_SIZE,
-        bits=BITS,
+        bits=bits,
     )
 
 
 def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realistic: bool = False, empty: bool = False,
-                    **overrides) -> SimpleNamespace:
+                    bits: int = BITS, **overrides) -> SimpleNamespace:
     """Random Qwen3-shaped model.  ``realistic=True`` quantises Gaussian dense
-    weights with ``quantize_w4`` (slow, for small models); the default draws
+    weights with ``quantize_w4`` (``quantize_affine`` at 8 bits; slow, for small models); the default draws
     codes/scales directly, which is what the 4B-sized benchmarks use.
     ``empty=True`` only allocates (uninitialised, directly on ``device``): the
-    receive side of the data-parallel weight broadcast."""
+    receive side of the data-parallel weight broadcast.  ``bits``: 4 or 8 (MLX affine, group 128)."""
+    if bits not in SUPPORTED_BITS:
+        raise ValueError(f"synthetic_qwen3: bits must be 4 or 8, got {bits}")
     args = make_args(name_or_dims, **overrides)
     gen = torch.Generator().manual_seed(seed)
 
     def layer(out_dim: int, in_dim: int) -> SimpleNamespace:
         if empty:
-            return _empty_layer(out_dim, in_dim, device)
+            return _empty_layer(out_dim, in_dim, device, bits)
         if realistic:
-            return _quantized_layer(out_dim, in_dim, gen, std=in_dim**-0.5)
-        return _random_layer(out_dim, in_dim, gen)
+            return _quantized_layer(out_dim, in_dim, gen, std=in_dim**-0.5, bits=bits)
+        return _random_layer(out_dim, in_dim, gen, bits)
 
     def norm(dim: int) -> SimpleNamespace:
         return _empty_norm(dim, device) if empty else _norm_weight(dim, gen)
@@ -145,7 +177,7 @@ def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realis
         stacked = {key: torch.stack([getattr(p, key).view(torch.int32) if key == "weight" else getattr(p, key) for p in parts])
                    for key in ("weight", "scales", "biases")}
         stacked["weight"] = stacked["weight"].view(torch.uint32)
-        return SimpleNamespace(**stacked, group_size=GROUP_SIZE, bits=BITS)
+        return SimpleNamespace(**stacked, group_size=GROUP_SIZE, bits=bits)
 
     def mlp(index: int) -> SimpleNamespace:
         sparse = (getattr(args, "num_experts", 0) > 0 and index not in args.mlp_only_layers
@@ -217,12 +249,12 @@ def named_tensors(node, prefix=""):
         yield prefix[:-1], node
 
 
-def weight_stream_bytes(args) -> int:
+def weight_stream_bytes(args, bits: int = BITS) -> int:
     """Packed bytes one decode token must stream (projections of every layer +
-    tied head): 0.53125 B per weight = N/2 codes + 4 B of scale/bias per 128
-    (book/src/week2-03-quantize-model.md:179-181)."""
+    tied head): 0.53125 B per weight at 4 bits = N/2 codes + 4 B of scale/bias per 128
+    (book/src/week2-03-quantize-model.md:179-181); 1.03125 B at 8 bits."""
     q_width = args.num_attention_heads * args.head_dim
     kv_width = args.num_key_value_heads * args.head_dim
     per_layer = args.hidden_size * (q_width + 2 * kv_width) + q_width * args.hidden_size + 3 * args.hidden_size * args.intermediate_size
     weights = args.num_hidden_layers * per_layer + args.vocab_size * args.hidden_size
-    return weights * 17 // 32
+    return weights * 17 // 32 if bits == 4 else weights * 33 // 32
