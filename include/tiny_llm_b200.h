@@ -229,6 +229,32 @@ int tl_paged_attention_segments(const void *q, const void *key_pages, const void
 enum { TL_EMBED_LAST = 0, TL_EMBED_MEAN = 1, TL_EMBED_MAX_HIDDEN = 12288 };
 int tl_embed_pool(const void *hidden, const void *norm_weight, float eps, const int32_t *segment_start, int num_segments, int rows, int hidden_size,
                   int dimensions, int pooling, int normalize, float *out, int dtype, void *stream);
+/* Prefixed-segment attention for packed reranking passes (DESIGN.md section 19): tl_paged_attention_segments with one
+ * more visible key range per row.  Row l sees exactly the keys in [prefix_start[l], prefix_end[l]) and in
+ * [segment_start[l], l].  prefix_start / prefix_end: int32 [L] on the device; precondition prefix_end[l] <=
+ * segment_start[l] (a larger prefix_end is cut there); prefix_start[l] == prefix_end[l] is an empty prefix.  A padding
+ * row has an empty prefix and segment_start[l] > l (L): its output is 0.  A CTA visits the key tiles of the hull of
+ * its rows' prefix ranges, then those from its rows' smallest segment start to its last row, and skips the tiles
+ * between; skipped and masked keys change no bit of the result.  Masked K/V slots are multiplied by zero
+ * probabilities, so every slot the block table reaches must hold finite values.  Other arguments, layouts and checks
+ * as tl_paged_attention_segments. */
+int tl_paged_attention_prefixed_segments(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                         const int32_t *segment_start, const int32_t *prefix_start, const int32_t *prefix_end, void *out, int L,
+                                         int D, int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads,
+                                         int dtype, void *stream);
+/* Selected-token logits of packed hidden states (DESIGN.md section 19), in place of the LM head.  hidden [rows,
+ * hidden_size] and norm_weight [hidden_size] bf16 or fp16; row_index int32 [n] and token_ids int32 [m] on the device,
+ * 1 <= m <= TL_SELECT_MAX_IDS.  The LM head (or the tied embedding) is MLX affine at group 128: weight [vocab,
+ * hidden_size * bits / 32] u32, scales / biases [vocab, hidden_size / 128] of the hidden dtype, bits 4 or 8.  Row
+ * row_index[i] is RMS-normalised exactly as tl_rms_norm does it; the logit of token_ids[j] is the fp32 sum, in a fixed
+ * order, of the normalised row times the weights T(code * scale + bias), rounded to the hidden dtype T.  logits [n, m]
+ * fp32 (T-rounded values) and logprobs [n, m] fp32, the log-softmax over the m logits of a row.  Valid ranges:
+ * 0 <= row_index[i] < rows, 0 <= token_ids[j] < vocab; an index outside gives NaN in what it touches and reads
+ * nothing.  hidden_size a multiple of 128, at most TL_EMBED_MAX_HIDDEN.  One launch, no workspace. */
+enum { TL_SELECT_MAX_IDS = 32 };
+int tl_select_logits(const void *hidden, const void *norm_weight, float eps, const int32_t *row_index, int n, int rows, int hidden_size,
+                     const void *weight, const void *scales, const void *biases, int vocab, int bits, const int32_t *token_ids, int m,
+                     float *logits, float *logprobs, int dtype, void *stream);
 
 /* ---- CUDA extension behind the same per-op semantics ---------------------
  * Device-driven K/V append for a decode batch (the batched form of

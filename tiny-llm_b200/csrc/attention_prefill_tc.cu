@@ -76,14 +76,23 @@ struct TcArgs {
     int num_groups, split_base, split_stride;
     // Segment-causal attention (TC_SEGMENT, one packed request): row l sees the keys segment_start[l] <= key <= l.
     const int32_t *segment_start;
+    // Prefixed-segment attention (TC_PREFIXED): row l also sees the keys prefix_start[l] <= key < prefix_end[l].
+    const int32_t *prefix_start, *prefix_end;
 };
 
 // TC_PLAIN: tl_paged_attention.  TC_PREFIX: one CTA per (group, KV head, split) over the group's shared pages, its 128
 // MMA rows the count x G query rows of the group's slots (slot-major), unmasked.  TC_SUFFIX: one CTA per (slot, KV head,
 // split) over the slot's keys after its group's shared pages, as TC_PLAIN at L = 1 otherwise.  TC_SEGMENT: TC_PLAIN's
 // causal token-major prefill of one request whose L rows are packed prompts: row l also masks the keys before
-// segment_start[l], and a CTA starts at the tile holding the smallest segment_start of its rows.
-enum { TC_PLAIN = 0, TC_PREFIX = 1, TC_SUFFIX = 2, TC_SEGMENT = 3 };
+// segment_start[l], and a CTA starts at the tile holding the smallest segment_start of its rows.  TC_PREFIXED:
+// TC_SEGMENT plus one more visible range per row, [prefix_start[l], prefix_end[l]) with prefix_end[l] <= segment_start[l]
+// (a reranking pass: a query's prefix, then its documents, DESIGN.md section 19).  A CTA first walks the tiles of the
+// hull of its rows' prefix ranges, then its segment tiles as TC_SEGMENT does, and skips every tile between them: the
+// documents of one query lie one after another behind their prefix, so without the skip the last one's rows would walk
+// all their siblings' tiles.  A tile whose keys a row masks adds exact zeros to it (p = exp2(-inf) = 0, no rescale), so
+// the skip changes no bit; the masked K/V slots are multiplied by p = 0, which holds because every pool slot is finite
+// (zero-initialised, or written by an earlier pass).
+enum { TC_PLAIN = 0, TC_PREFIX = 1, TC_SUFFIX = 2, TC_SEGMENT = 3, TC_PREFIXED = 4 };
 
 // The group of slot b: (first_slot, count, shared_pages), or (b, 1, 0) when no group with shared pages holds it.
 __device__ __forceinline__ int3 tc_group_of(const int32_t *groups, int num_groups, int b) {
@@ -111,25 +120,40 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     if (MODE == TC_PREFIX || MODE == TC_SUFFIX) grp = tc_group_of(a.groups, a.num_groups, b);
     if (MODE == TC_PREFIX && grp.x != b) return;  // the group's first slot covers its rows
     // The causal shift uses the whole context, the block table clamps afterwards (attention_decode.cu).
-    const int ctx = MODE == TC_SEGMENT ? a.L : a.context_lens[b];  // TC_SEGMENT: the packed rows are the whole context
+    const int ctx = MODE == TC_SEGMENT || MODE == TC_PREFIXED ? a.L : a.context_lens[b];  // the packed rows are the whole context
     // keys any row of this CTA may see: [0, key_end); the prefix pass sees the shared pages, the suffix pass what follows
     const int last_row = min(q0 + a.RH, a.L) - 1;
     const int shared_keys = min(grp.z * a.page_size, cap);
     const int key_end = MODE == TC_PREFIX ? shared_keys
                         : ctx <= 0 ? 0 : min(a.is_causal ? min(ctx, max(ctx - a.L + last_row + 1, 0)) : ctx, cap);
     const int all_tiles = (key_end + TC_BN - 1) / TC_BN;
-    int seg_lo = 0;  // TC_SEGMENT: the smallest segment start of this CTA's rows
-    if (MODE == TC_SEGMENT) {
+    int seg_lo = 0;  // TC_SEGMENT / TC_PREFIXED: the smallest segment start of this CTA's rows
+    if (MODE == TC_SEGMENT || MODE == TC_PREFIXED) {
         seg_lo = key_end;
         for (int r = q0; r <= last_row; ++r) seg_lo = min(seg_lo, max(a.segment_start[r], 0));
     }
-    const int tile_lo = MODE == TC_SUFFIX ? min(shared_keys / TC_BN, all_tiles) : MODE == TC_SEGMENT ? min(seg_lo / TC_BN, all_tiles) : 0;
+    const int tile_lo = MODE == TC_SUFFIX ? min(shared_keys / TC_BN, all_tiles)
+                        : MODE == TC_SEGMENT || MODE == TC_PREFIXED ? min(seg_lo / TC_BN, all_tiles) : 0;
+    // TC_PREFIXED: the tiles pre_t0 .. pre_t0 + pre_n - 1 of the hull of the rows' prefix ranges come first (those at or
+    // past tile_lo are segment tiles already); rows with an empty segment (padding) do not count.
+    int pre_t0 = 0, pre_n = 0;
+    if (MODE == TC_PREFIXED) {
+        int p_lo = key_end, p_hi = 0;
+        for (int r = q0; r <= last_row; ++r) {
+            const int ps = max(a.prefix_start[r], 0), pe = min(a.prefix_end[r], key_end);
+            if (ps < pe && a.segment_start[r] <= r) p_lo = min(p_lo, ps), p_hi = max(p_hi, pe);
+        }
+        pre_t0 = p_lo / TC_BN;
+        pre_n = max(min((p_hi + TC_BN - 1) / TC_BN, tile_lo) - pre_t0, 0);
+    }
     // Split-KV: the launch fixes the NUMBER of splits from the block table's width (the grid of a captured graph cannot
     // follow the context), the tiles are dealt out here from the request's real length, so a request far below the
     // bound still keeps all its splits busy.
     const int tps = a.splits > 1 ? max((all_tiles - tile_lo + a.splits - 1) / a.splits, 1) : a.tiles_per_split;
     const int t0 = tile_lo + min(split * tps, all_tiles - tile_lo);
-    const int n_tiles = min(tps, all_tiles - t0);  // this CTA: global tiles t0 .. t0 + n_tiles - 1
+    const int n_tiles = min(tps, all_tiles - t0) + pre_n;  // this CTA: global tiles t0 .. t0 + n_tiles - 1 (after the prefix tiles)
+    // the global tile of this CTA's j-th tile
+    auto tile_of = [&](int j) { return MODE != TC_PREFIXED ? t0 + j : j < pre_n ? pre_t0 + j : t0 + j - pre_n; };
 
     const uint32_t q_base = g_smem_u32(tsm + TC_Q_OFF);
     const uint32_t k_base = g_smem_u32(tsm + TC_K_OFF), v_base = g_smem_u32(tsm + TC_V_OFF);
@@ -176,10 +200,11 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             int s = 0;
             uint32_t ph = 1;  // producer side: first pass through the ring does not wait
             for (int j = 0; j < n_tiles; ++j) {
-                const int lp = (t0 + j) / a.tiles_per_page;
+                const int tile = tile_of(j);
+                const int lp = tile / a.tiles_per_page;
                 int pid = table[lp];
                 if (pid < 0 || pid >= a.num_pages) pid = a.num_pages;  // outside the tensor: the TMA unit writes zeros
-                const int slot0 = (t0 + j - lp * a.tiles_per_page) * TC_BN;
+                const int slot0 = (tile - lp * a.tiles_per_page) * TC_BN;
                 g_mbar_wait(k_empty + 8 * s, ph);
                 if (g_elect_one()) {
                     g_mbar_expect_tx(k_full + 8 * s, TC_KV_TILE);
@@ -205,6 +230,7 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         const int t = threadIdx.x & 127;
         // TC_PREFIX: l = the row's slot inside the group (a row past the group's count is not written)
         int lq[2], g[2], l[2], limit[2], lo[2] = {0, 0};  // lo: TC_SEGMENT's first visible key
+        int pst[2] = {0, 0}, pen[2] = {0, 0};               // TC_PREFIXED: the prefix range [pst, pen)
         bool row_valid[2];
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
@@ -222,9 +248,10 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             row_valid[rr] = l[rr] < a.L && ctx > 0;
             // last key this row may see (bottom-right causal alignment, paged_attention.metal:411)
             limit[rr] = !row_valid[rr] ? -1 : min(a.is_causal ? min(ctx - 1, l[rr] + (ctx - a.L)) : ctx - 1, cap - 1);
-            if (MODE == TC_SEGMENT && row_valid[rr]) {
+            if ((MODE == TC_SEGMENT || MODE == TC_PREFIXED) && row_valid[rr]) {
                 lo[rr] = max(a.segment_start[l[rr]], 0);
                 if (lo[rr] > limit[rr]) row_valid[rr] = false, limit[rr] = -1;  // an empty segment (a padding row): output 0
+                else if (MODE == TC_PREFIXED) pst[rr] = max(a.prefix_start[l[rr]], 0), pen[rr] = min(a.prefix_end[l[rr]], lo[rr]);
             }
         }
         float o[TC_D / 2];
@@ -237,7 +264,8 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         int s = 0;
         uint32_t ph = 0;
         for (int j = 0; j < n_tiles; ++j) {
-            const int lp = (t0 + j) / a.tiles_per_page;
+            const int tile = tile_of(j);
+            const int lp = tile / a.tiles_per_page;
             const int pid = table[lp];
             const bool page_ok = pid >= 0 && pid < a.num_pages;
             // ---- S = Q K_j^T: both operands K-major, two 64-wide halves of the head dimension
@@ -261,12 +289,13 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             wgmma_reg_fence(sc);
             if (t == 0) g_mbar_arrive(k_empty + 8 * s);  // K stage reusable: this warpgroup's MMAs have read it
             // ---- softmax of the tile: sc[4 c8 + 2 rr + e] = S[row rr, key 8 c8 + 2 (t % 4) + e]
-            const int key0 = (t0 + j) * TC_BN;
+            const int key0 = tile * TC_BN;
             uint32_t pa[TC_BN / 16][4];  // bf16 probabilities as the A operand of the four P V K steps
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int visible = page_ok ? min(limit[rr] - key0 + 1, TC_BN) : 0;  // keys [0, visible) of the tile
                 const int first = lo[rr] - key0;                                        // TC_SEGMENT: and not below first
+                const int pfirst = pst[rr] - key0, pend = page_ok ? pen[rr] - key0 : 0;  // TC_PREFIXED: or in [pfirst, pend)
                 // raw maximum (the scale is positive, so it commutes with max); masking only on boundary tiles
                 float raw_max = -CUDART_INF_F;
 #pragma unroll
@@ -275,7 +304,9 @@ paged_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
                     for (int e = 0; e < 2; ++e) {
                         float &v = sc[4 * c8 + 2 * rr + e];
                         const int c = 8 * c8 + 2 * (lane & 3) + e;
-                        if (MODE == TC_SEGMENT ? (c >= visible || c < first) : (visible < TC_BN && c >= visible)) v = -CUDART_INF_F;  // exp2 gives exactly 0
+                        const bool masked = MODE == TC_PREFIXED ? (c >= visible || c < first) && (c < pfirst || c >= pend)
+                                            : MODE == TC_SEGMENT ? (c >= visible || c < first) : (visible < TC_BN && c >= visible);
+                        if (masked) v = -CUDART_INF_F;  // exp2 gives exactly 0
                         raw_max = fmaxf(raw_max, v);
                     }
                 raw_max = fmaxf(raw_max, __shfl_xor_sync(0xffffffffu, raw_max, 1));
@@ -530,16 +561,17 @@ int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp
 
 // ---------------------------------------------------------------- segment-causal attention --
 // One packed request of L rows (B = 1, the chunk form's q [Hq, L, D] and token-major out [L, Hq * D]) whose keys are its
-// own rows 0 .. L - 1: row l sees segment_start[l] <= key <= l.  Unsplit (a pass of L <= 8,192 rows spans at most as
-// many keys): the q-block grid of launch_paged_prefill_tc at B = 1.
-template <typename T>
-static int launch_segment_t(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
-                            int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, CUtensorMapDataType dt,
-                            cudaStream_t st) {
+// own rows 0 .. L - 1: row l sees segment_start[l] <= key <= l (TC_SEGMENT), and also prefix_start[l] <= key <
+// prefix_end[l] (TC_PREFIXED).  Unsplit (a pass of L <= 8,192 rows spans at most as many keys): the q-block grid of
+// launch_paged_prefill_tc at B = 1.
+template <int MODE, typename T>
+static int launch_segment_t(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, const int32_t *pre_start,
+                            const int32_t *pre_end, void *out, int L, int num_pages, int page_size, int max_pages, float scale,
+                            int num_kv_heads, int num_heads, CUtensorMapDataType dt, cudaStream_t st, const char *op) {
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<TC_SEGMENT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
-            return fail(TL_ECUDA, "paged_attention_segments: cannot raise shared memory limit");
+        if (cudaFuncSetAttribute(paged_prefill_tc_kernel<MODE, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
+            return fail(TL_ECUDA, "%s: cannot raise shared memory limit", op);
         configured = true;
     }
     TcArgs a{};
@@ -553,6 +585,7 @@ static int launch_segment_t(const void *q, const void *kp, const void *vp, const
     a.tiles_per_split = (max_pages * page_size + TC_BN - 1) / TC_BN;
     a.out_token_major = 1;
     a.segment_start = seg;
+    a.prefix_start = pre_start, a.prefix_end = pre_end;
     CUtensorMap mq, mk, mv;
     {
         const cuuint64_t dims[3] = {TC_D, static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(num_heads)};
@@ -566,20 +599,32 @@ static int launch_segment_t(const void *q, const void *kp, const void *vp, const
         if (int e = tc_map(&mv, vp, 4, dims, box, dt)) return e;
     }
     const dim3 grid((L + a.RH - 1) / a.RH, num_kv_heads, 1);
-    cudaError_t le = launch_chained(paged_prefill_tc_kernel<TC_SEGMENT, T>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
-    if (le != cudaSuccess) return fail(TL_ECUDA, "paged_attention_segments: launch failed: %s", cudaGetErrorString(le));
-    TL_LAUNCH_CHECK("paged_attention_segments");
+    cudaError_t le = launch_chained(paged_prefill_tc_kernel<MODE, T>, grid, dim3(TC_THREADS), TC_SMEM_BYTES, st, mq, mk, mv, a);
+    if (le != cudaSuccess) return fail(TL_ECUDA, "%s: launch failed: %s", op, cudaGetErrorString(le));
+    TL_LAUNCH_CHECK(op);
     return TL_OK;
 }
 
 int launch_paged_attention_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
                                     int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, int dtype,
                                     cudaStream_t st) {
+    const char *op = "paged_attention_segments";
     if (dtype == TL_F16)
-        return launch_segment_t<__half>(q, kp, vp, bt, seg, out, L, num_pages, page_size, max_pages, scale, num_kv_heads, num_heads,
-                                        CU_TENSOR_MAP_DATA_TYPE_FLOAT16, st);
-    return launch_segment_t<bf16>(q, kp, vp, bt, seg, out, L, num_pages, page_size, max_pages, scale, num_kv_heads, num_heads,
-                                  CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, st);
+        return launch_segment_t<TC_SEGMENT, __half>(q, kp, vp, bt, seg, nullptr, nullptr, out, L, num_pages, page_size, max_pages, scale,
+                                                    num_kv_heads, num_heads, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, st, op);
+    return launch_segment_t<TC_SEGMENT, bf16>(q, kp, vp, bt, seg, nullptr, nullptr, out, L, num_pages, page_size, max_pages, scale,
+                                              num_kv_heads, num_heads, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, st, op);
+}
+
+int launch_paged_attention_prefixed_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg,
+                                             const int32_t *pre_start, const int32_t *pre_end, void *out, int L, int num_pages, int page_size,
+                                             int max_pages, float scale, int num_kv_heads, int num_heads, int dtype, cudaStream_t st) {
+    const char *op = "paged_attention_prefixed_segments";
+    if (dtype == TL_F16)
+        return launch_segment_t<TC_PREFIXED, __half>(q, kp, vp, bt, seg, pre_start, pre_end, out, L, num_pages, page_size, max_pages, scale,
+                                                     num_kv_heads, num_heads, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, st, op);
+    return launch_segment_t<TC_PREFIXED, bf16>(q, kp, vp, bt, seg, pre_start, pre_end, out, L, num_pages, page_size, max_pages, scale,
+                                               num_kv_heads, num_heads, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, st, op);
 }
 
 }  // namespace tl

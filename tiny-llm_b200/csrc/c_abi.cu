@@ -483,6 +483,44 @@ int tl_embed_pool(const void *hidden, const void *norm_weight, float eps, const 
                              normalize != 0, out, dtype, as_stream(stream));
 }
 
+int tl_paged_attention_prefixed_segments(const void *q, const void *key_pages, const void *value_pages, const int32_t *block_table,
+                                         const int32_t *segment_start, const int32_t *prefix_start, const int32_t *prefix_end, void *out, int L,
+                                         int D, int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads,
+                                         int dtype, void *stream) {
+    const char *op = "paged_attention_prefixed_segments";
+    if (dtype != TL_BF16 && dtype != TL_F16) return fail(TL_EDTYPE, "%s: expected float16 or bfloat16", op);
+    if (D != PAGED_D) return fail(TL_EINVAL, "%s: head dimension must be %d", op, PAGED_D);
+    if (num_heads <= 0 || num_kv_heads <= 0 || num_heads % num_kv_heads != 0 || 128 % (num_heads / num_kv_heads) != 0)
+        return fail(TL_EINVAL, "%s: num_heads / num_kv_heads must be a whole divisor of 128", op);
+    if (L < 0 || num_pages <= 0 || max_pages <= 0 || page_size <= 0 || page_size % 64 != 0)
+        return fail(TL_EINVAL, "%s: bad shape (page_size must be a multiple of 64)", op);
+    if (static_cast<long long>(L) > static_cast<long long>(max_pages) * page_size)
+        return fail(TL_EINVAL, "%s: %d rows do not fit the block table's %d pages", op, L, max_pages);
+    if (L == 0) return TL_OK;
+    if (!q || !key_pages || !value_pages || !block_table || !segment_start || !prefix_start || !prefix_end || !out)
+        return fail(TL_EINVAL, "%s: null pointer", op);
+    if (!aligned16(q) || !aligned16(key_pages) || !aligned16(value_pages) || !aligned16(out))
+        return fail(TL_EINVAL, "%s: q, pages and out must be 16-byte aligned", op);
+    return launch_paged_attention_prefixed_segments(q, key_pages, value_pages, block_table, segment_start, prefix_start, prefix_end, out, L,
+                                                    num_pages, page_size, max_pages, scale, num_kv_heads, num_heads, dtype, as_stream(stream));
+}
+
+int tl_select_logits(const void *hidden, const void *norm_weight, float eps, const int32_t *row_index, int n, int rows, int hidden_size,
+                     const void *weight, const void *scales, const void *biases, int vocab, int bits, const int32_t *token_ids, int m,
+                     float *logits, float *logprobs, int dtype, void *stream) {
+    if (dtype != TL_BF16 && dtype != TL_F16) return fail(TL_EDTYPE, "select_logits: expected float16 or bfloat16");
+    if (bits != 4 && bits != 8) return fail(TL_EINVAL, "select_logits: bits must be 4 or 8, got %d", bits);
+    if (m < 1 || m > TL_SELECT_MAX_IDS) return fail(TL_EINVAL, "select_logits: %d token ids, expected 1 to %d", m, TL_SELECT_MAX_IDS);
+    if (hidden_size <= 0 || hidden_size > TL_EMBED_MAX_HIDDEN || hidden_size % 128 != 0)
+        return fail(TL_EINVAL, "select_logits: hidden size %d is not a multiple of 128 in [128, %d]", hidden_size, TL_EMBED_MAX_HIDDEN);
+    if (n < 0 || rows < 0 || vocab <= 0) return fail(TL_EINVAL, "select_logits: bad shape");
+    if (n == 0) return TL_OK;
+    if (!hidden || !norm_weight || !row_index || !weight || !scales || !biases || !token_ids || !logits || !logprobs)
+        return fail(TL_EINVAL, "select_logits: null pointer");
+    return launch_select_logits(hidden, norm_weight, eps, row_index, n, rows, hidden_size, weight, scales, biases, vocab, bits, token_ids, m,
+                                logits, logprobs, dtype, as_stream(stream));
+}
+
 // ------------------------------------------------------------------ misc --
 size_t tl_argmax_workspace(int rows, int vocab) { return argmax_workspace(rows, vocab); }
 

@@ -190,10 +190,17 @@ int launch_shared_prefix_attention(const void *q, const void *kp, const void *vp
 int launch_paged_attention_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg, void *out, int L,
                                     int num_pages, int page_size, int max_pages, float scale, int num_kv_heads, int num_heads, int dtype,
                                     cudaStream_t st);
+// Prefixed-segment attention (tl_paged_attention_prefixed_segments): TC_SEGMENT plus a prefix key range per row.
+int launch_paged_attention_prefixed_segments(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *seg,
+                                             const int32_t *pre_start, const int32_t *pre_end, void *out, int L, int num_pages, int page_size,
+                                             int max_pages, float scale, int num_kv_heads, int num_heads, int dtype, cudaStream_t st);
 
 // embed.cu
 int launch_embed_pool(const void *x, const void *w, float eps, const int32_t *seg, int n, int rows, int H, int d, int mean, int normalize,
                       float *out, int dtype, cudaStream_t st);
+int launch_select_logits(const void *x, const void *w, float eps, const int32_t *row_idx, int n, int rows, int H, const void *wq,
+                         const void *scales, const void *biases, int V, int bits, const int32_t *ids, int m, float *logits, float *logprobs,
+                         int dtype, cudaStream_t st);
 
 // attention_prefill.cu (mma.sync flash prefill: fallback for page sizes / head ratios the wgmma kernel does not take)
 int launch_paged_prefill_fa(const void *q, const void *kp, const void *vp, const int32_t *bt, const int32_t *cl, void *out, int rows,

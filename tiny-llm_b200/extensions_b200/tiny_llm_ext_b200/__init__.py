@@ -86,6 +86,9 @@ __all__ = [
     "shared_prefix_attention_workspace",
     "paged_attention_segments",
     "embed_pool",
+    "paged_attention_prefixed_segments",
+    "select_logits",
+    "SELECT_MAX_IDS",
 ]
 
 _HERE = Path(__file__).resolve().parent
@@ -176,6 +179,8 @@ _SIGNATURES = {
     "tl_shared_prefix_attention": (_I, [_VP] * 7 + [_I, _VP] + [_I] * 5 + [_F] + [_I] * 3 + [_VP, _SZ, _VP]),
     "tl_paged_attention_segments": (_I, [_VP] * 6 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
     "tl_embed_pool": (_I, [_VP, _VP, _F, _VP] + [_I] * 6 + [_VP, _I, _VP]),
+    "tl_paged_attention_prefixed_segments": (_I, [_VP] * 8 + [_I] * 5 + [_F] + [_I] * 3 + [_VP]),
+    "tl_select_logits": (_I, [_VP, _VP, _F, _VP] + [_I] * 3 + [_VP] * 3 + [_I, _I, _VP, _I, _VP, _VP, _I, _VP]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -1308,6 +1313,72 @@ def embed_pool(hidden, norm_weight, eps, segment_start, pooling="last", dimensio
     _check(_lib.tl_embed_pool(hidden.data_ptr(), norm_weight.data_ptr(), float(eps), segment_start.data_ptr(), n, rows, H, d,
                               EMBED_POOLING[pooling], int(bool(normalize)), out.data_ptr(), _DTYPE_CODE[hidden.dtype], _stream_ptr(stream, hidden)))
     return out
+
+
+def paged_attention_prefixed_segments(query, key_pages, value_pages, block_table, segment_start, prefix_start, prefix_end, scale,
+                                      num_kv_heads, num_heads, stream=None):
+    """Prefixed-segment prefill attention of one packed request (``tl_paged_attention_prefixed_segments``, DESIGN.md
+    section 19): ``paged_attention_segments`` where row ``l`` also sees the keys ``prefix_start[l] <= key <
+    prefix_end[l]`` (int32 ``[L]`` each, ``prefix_end[l] <= segment_start[l]``; equal bounds: no prefix)."""
+    op = "paged_attention_prefixed_segments"
+    if query.dim() != 3 or key_pages.dim() != 4 or key_pages.shape != value_pages.shape:
+        raise RuntimeError(f"{op}: q must be [H_q, L, D] and the page tensors [P, H_kv, page_size, D]")
+    if query.dtype not in _HALF or key_pages.dtype != query.dtype or value_pages.dtype != query.dtype:
+        raise RuntimeError(f"{op}: q, key_pages and value_pages must share one dtype, float16 or bfloat16")
+    Hq, L, D = query.shape
+    if Hq != num_heads or key_pages.shape[1] != num_kv_heads:
+        raise RuntimeError(f"{op}: q must hold num_heads heads and the pages num_kv_heads")
+    _int32(op, L, segment_start=segment_start, prefix_start=prefix_start, prefix_end=prefix_end)
+    _block_table(op, block_table, None)
+    _gpu(op, query, key_pages, value_pages, block_table, segment_start, prefix_start, prefix_end)
+    _contig(op, query=query, key_pages=key_pages, value_pages=value_pages, block_table=block_table, segment_start=segment_start,
+            prefix_start=prefix_start, prefix_end=prefix_end)
+    P, _, page_size, _ = key_pages.shape
+    out = torch.empty((L, Hq * D), dtype=query.dtype, device=query.device)
+    _check(_lib.tl_paged_attention_prefixed_segments(query.data_ptr(), key_pages.data_ptr(), value_pages.data_ptr(), block_table.data_ptr(),
+                                                     segment_start.data_ptr(), prefix_start.data_ptr(), prefix_end.data_ptr(), out.data_ptr(), L,
+                                                     D, P, page_size, block_table.shape[0], float(scale), int(num_kv_heads), int(num_heads),
+                                                     _DTYPE_CODE[query.dtype], _stream_ptr(stream, query)))
+    return out
+
+
+SELECT_MAX_IDS = 32
+
+
+def select_logits(hidden, norm_weight, eps, row_index, weight, scales, biases, token_ids, stream=None):
+    """Selected-token logits (``tl_select_logits``, DESIGN.md section 19): rows ``row_index`` (int32 ``[n]``) of
+    ``hidden`` [rows, H] (bf16 or fp16) RMS-normalised with ``norm_weight`` bit for bit as ``rms_norm``, then the
+    logits of ``token_ids`` (int32 ``[m]``, 1 <= m <= 32) under the packed MLX affine head ``weight`` [V, H * bits / 32]
+    u32 with ``scales`` / ``biases`` [V, H / 128] (group 128; the width, 4 or 8 bits, follows from ``weight``'s shape).
+    Returns fp32 ``(logits [n, m], logprobs [n, m])``: the logits rounded to the hidden dtype, and their log-softmax
+    over the m ids."""
+    op = "select_logits"
+    if hidden.dim() != 2 or hidden.dtype not in _HALF or norm_weight.dtype != hidden.dtype or tuple(norm_weight.shape) != (hidden.shape[1],):
+        raise RuntimeError(f"{op}: hidden must be float16 or bfloat16 [rows, H] with a norm weight [H] of its dtype")
+    rows, H = hidden.shape
+    if H % 128 != 0:
+        raise RuntimeError(f"{op}: the hidden size must be a multiple of 128 (group 128), got {H}")
+    if weight.dim() != 2 or weight.dtype not in _PACKED or weight.shape[1] * 32 % H != 0 or weight.shape[1] * 32 // H not in (4, 8):
+        raise RuntimeError(f"{op}: weight must be packed 4- or 8-bit codes [V, H * bits / 32] (int32 or uint32)")
+    bits = weight.shape[1] * 32 // H
+    V = weight.shape[0]
+    if scales.dtype != hidden.dtype or biases.dtype != hidden.dtype or tuple(scales.shape) != (V, H // 128) or scales.shape != biases.shape:
+        raise RuntimeError(f"{op}: scales and biases must be [V, H / 128] of the hidden dtype")
+    _int32(op, row_index=row_index, token_ids=token_ids)
+    if row_index.dim() != 1 or token_ids.dim() != 1:
+        raise RuntimeError(f"{op}: row_index and token_ids must be 1-D")
+    m = token_ids.shape[0]
+    if not 1 <= m <= SELECT_MAX_IDS:
+        raise RuntimeError(f"{op}: 1 to {SELECT_MAX_IDS} token ids, got {m}")
+    _gpu(op, hidden, norm_weight, row_index, weight, scales, biases, token_ids)
+    _contig(op, hidden=hidden, norm_weight=norm_weight, row_index=row_index, weight=weight, scales=scales, biases=biases, token_ids=token_ids)
+    n = row_index.shape[0]
+    logits = torch.empty((n, m), dtype=torch.float32, device=hidden.device)
+    logprobs = torch.empty((n, m), dtype=torch.float32, device=hidden.device)
+    _check(_lib.tl_select_logits(hidden.data_ptr(), norm_weight.data_ptr(), float(eps), row_index.data_ptr(), n, rows, H, weight.data_ptr(),
+                                 scales.data_ptr(), biases.data_ptr(), V, bits, token_ids.data_ptr(), m, logits.data_ptr(), logprobs.data_ptr(),
+                                 _DTYPE_CODE[hidden.dtype], _stream_ptr(stream, hidden)))
+    return logits, logprobs
 
 
 def quantized_matmul_residual_norm(scales, biases, b, p0, residual, norm_weight, norm_eps, stream=None):

@@ -8,6 +8,7 @@ from .basics import linear, silu, softmax
 from .batch import ContinuousBatcher, Request, batch_generate
 from .checkpoint import load_checkpoint, load_tokenizer, save_checkpoint
 from .embed import embed_ids
+from .rerank import rerank_ids, split_shared_prefix
 from .embedding import Embedding, QuantizedEmbedding
 from .generate import (BeamHypothesis, ParallelSample, beam_search_ids, greedy_generate_ids, parallel_sample_ids, prompt_lookup_generate_ids,
                        simple_generate_with_kv_cache, speculative_generate, speculative_generate_ids)

@@ -33,6 +33,8 @@ see checkpoint.py; there is no hub download here).
         (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
     python -m tiny_llm_b200.cli embed --synthetic tiny-d128 --prompt-ids "5,17,3;9,2,4,8" --dimensions 64 [--pooling mean] [--out e.npy]
         (one pooled, L2-normalised embedding per prompt from packed prefill passes; --append-eos for Qwen3-Embedding)
+    python -m tiny_llm_b200.cli rerank --synthetic tiny-d128 --prefix-ids "5,17,3" --document-ids "9,2;4,8,1" --true-id 10 --false-id 11
+        (one Qwen3-Reranker relevance score per document; with --model: --query, --document / --documents-file, --instruction)
 """
 
 from __future__ import annotations
@@ -465,6 +467,60 @@ def cmd_embed(args) -> int:
     return 0
 
 
+def rerank_inputs(args, tokenizer):
+    """``(prefix, documents, true_id, false_id)`` for ``rerank``.  With ``--document-ids`` ("a,b;c,d"): the documents'
+    ids after ``--prefix-ids``.  Otherwise each ``--document`` and line of ``--documents-file`` is put into the
+    Qwen3-Reranker template with ``--query`` and ``--instruction``, each pair is tokenised whole, and the longest
+    shared leading run of ids becomes the prefix.  ``--true-id`` / ``--false-id`` default to the tokenizer's "yes" and
+    "no"."""
+    from .rerank import rerank_prompt, split_shared_prefix
+
+    def ids(text):
+        return [int(t) for t in text.split(",") if t.strip()]
+
+    if args.document_ids:
+        prefix = ids(args.prefix_ids or "")
+        docs = [ids(part) for part in args.document_ids.split(";")]
+    else:
+        texts = list(args.document or [])
+        if args.documents_file:
+            with open(args.documents_file, encoding="utf-8") as f:
+                texts += [line.rstrip("\n") for line in f if line.strip()]
+        if not texts or args.query is None:
+            raise SystemExit("rerank needs --document-ids, or --query with --document or --documents-file")
+        if tokenizer is None:
+            raise SystemExit("text queries and documents need the checkpoint's tokenizer files; use --prefix-ids / --document-ids")
+        prompts = [list(tokenizer.encode(rerank_prompt(args.query, t, args.instruction), add_special_tokens=False)) for t in texts]
+        prefix, docs = split_shared_prefix(prompts)
+    for i, d in enumerate(docs):
+        if not d:
+            raise SystemExit(f"document {i} is empty")
+    true_id, false_id = args.true_id, args.false_id
+    if true_id is None or false_id is None:
+        if tokenizer is None:
+            raise SystemExit("--true-id and --false-id are needed without the checkpoint's tokenizer")
+        true_id = tokenizer.convert_tokens_to_ids("yes") if true_id is None else true_id
+        false_id = tokenizer.convert_tokens_to_ids("no") if false_id is None else false_id
+    return prefix, docs, int(true_id), int(false_id)
+
+
+def cmd_rerank(args) -> int:
+    from .rerank import rerank_ids
+
+    device = torch.device(args.device)
+    ns, tokenizer, name = _load(args, device)
+    model = _model(args, ns, name)
+    prefix, docs, true_id, false_id = rerank_inputs(args, tokenizer)
+    try:
+        scores = rerank_ids(model, [(prefix, docs)], true_id, false_id, max_tokens=args.max_tokens, device=device)[0].cpu()
+    except ValueError as exc:
+        raise SystemExit(f"rerank: {exc}") from None
+    print(f"shared prefix: {len(prefix)} tokens")
+    for i, (doc, score) in enumerate(zip(docs, scores.tolist())):
+        print(f"[{i}] {len(doc)} tokens: {score:.6f}")
+    return 0
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="tiny_llm_b200.cli")
     sub = ap.add_subparsers(dest="command", required=True)
@@ -543,6 +599,21 @@ def main(argv=None) -> int:
     p.add_argument("--no-normalize", action="store_true", help="skip the L2 normalisation")
     p.add_argument("--max-tokens", type=_positive_int, default=8192, metavar="N", help="rows per packed pass (a multiple of 128)")
     p.add_argument("--out", default=None, metavar="FILE.npy", help="also save the [n, d] float32 embeddings")
+    p.add_argument("--device", default="cuda:0")
+    p = sub.add_parser("rerank")
+    p.set_defaults(fn=cmd_rerank, loader="week3", rope_scaling=None, max_context=None, disable_paged_attention=False, logprobs=None)
+    p.add_argument("--model", default=None, help="checkpoint directory (Qwen3 or Qwen3-Reranker, MLX 4- or 8-bit)")
+    p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny-d128, qwen3-0.6b, qwen3-4b) instead of --model")
+    p.add_argument("--synthetic-bits", type=int, choices=(4, 8), default=4, help="code width of the --synthetic weights (MLX affine, group 128)")
+    p.add_argument("--query", default=None, help="the query text (needs the tokenizer)")
+    p.add_argument("--document", action="append", default=None, help="a document text (repeatable)")
+    p.add_argument("--documents-file", default=None, help="one document text per line")
+    p.add_argument("--instruction", default=None, help="the task instruction (default: Qwen3-Reranker's web-search one)")
+    p.add_argument("--prefix-ids", default=None, help="comma-separated token ids shared by every prompt")
+    p.add_argument("--document-ids", default=None, help="comma-separated token ids of each prompt's rest, ';' between documents")
+    p.add_argument("--true-id", type=int, default=None, help="the id whose probability is the score (default: the tokenizer's \"yes\")")
+    p.add_argument("--false-id", type=int, default=None, help="the competing id (default: the tokenizer's \"no\")")
+    p.add_argument("--max-tokens", type=_positive_int, default=8192, metavar="N", help="rows per packed pass (a multiple of 128)")
     p.add_argument("--device", default="cuda:0")
     sub.choices["batch"].add_argument("--prompts-file", default=None)
     sub.choices["batch"].add_argument("--batch-size", type=int, default=5)

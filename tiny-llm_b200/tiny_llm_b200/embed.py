@@ -77,22 +77,29 @@ def pass_layout(lengths, max_tokens: int):
     return offsets, ctxs, seg, bounds
 
 
-def _check_model(model, device) -> None:
+def _check_model(model, device, op: str = "embed") -> None:
+    """Refuse, for the packed passes of ``op``, the models ``run_packed_pass`` does not run."""
     if any(isinstance(block.mlp, Moe) for block in model.layers_inner):
-        raise ValueError("embed: Qwen3-MoE models are not supported")
+        raise ValueError(f"{op}: Qwen3-MoE models are not supported")
     if model.adapters is not None:
-        raise ValueError("embed: models with adapters loaded are not supported")
+        raise ValueError(f"{op}: models with adapters loaded are not supported")
     if not PrefillEngine.supported(model, device):
-        raise ValueError("embed: needs a CUDA device, bf16 weights, head dimension 128 (non-traditional RoPE over the whole head), "
+        raise ValueError(f"{op}: needs a CUDA device, bf16 weights, head dimension 128 (non-traditional RoPE over the whole head), "
                          "a page size that is a multiple of 64 and a head ratio that divides 128")
 
 
-def _run_pass(model, ids, lengths, max_tokens, pooling, normalize, dimensions, device) -> torch.Tensor:
-    """One packed pass: the pooled rows of its prompts, in order."""
+def run_packed_pass(model, max_tokens, tokens, offsets, ctxs, arrays, attend, head, device):
+    """One packed pass of ``max_tokens`` rows through the layer stack, with pages borrowed from the model's pools for
+    the pass and returned in a ``finally``.  ``tokens``, ``offsets`` (RoPE positions) and ``ctxs`` (post-append lengths:
+    row r appends its K/V at slot r, 0 appends nothing) are per-row int32 host arrays; ``arrays`` further int32 host
+    arrays uploaded with them in one copy.  ``attend(q, attn, pool, table, views)`` is a layer's attention on its
+    ``[Hq, T, D]`` queries, ``head(x, views)`` turns the final ``[T, H]`` hidden state into the result; ``views`` are the
+    device copies of ``arrays``.  The rest - embedding, norms, projections, K/V append - is the > 128-row branch of
+    ``engine.PrefillEngine._forward``."""
     n_pages = -(-max_tokens // model.page_size)
     layers = model.layers_inner
     attn0 = layers[0].self_attn
-    Hq, Hkv, D = attn0.num_heads, attn0.num_kv_heads, attn0.head_dim
+    Hkv, D = attn0.num_kv_heads, attn0.head_dim
     caches = []
     try:
         for pool in model.page_pools:
@@ -102,17 +109,15 @@ def _run_pass(model, ids, lengths, max_tokens, pooling, normalize, dimensions, d
             cache = TinyKvPagedCache(pool)
             caches.append(cache)
             cache.append_slots(max_tokens)
-        offsets, ctxs, seg, bounds = pass_layout(lengths, max_tokens)
-        tokens = np.zeros(max_tokens, dtype=np.int32)
-        for p, s in zip(ids, bounds[0::2]):
-            tokens[s:s + len(p)] = p
         tables = np.stack([np.asarray(c.page_ids, dtype=np.int32) for c in caches])
-        meta = torch.from_numpy(np.concatenate([tokens, offsets, ctxs, seg, bounds, tables.reshape(-1)])).to(device)
         T = max_tokens
-        tok, off, ctx, segs = meta[0:T].view(1, T), meta[T:2 * T], meta[2 * T:3 * T], meta[3 * T:4 * T]
-        nb = bounds.shape[0]
-        bnd = meta[4 * T:4 * T + nb]
-        tab = meta[4 * T + nb:].view(len(caches), n_pages)
+        meta = torch.from_numpy(np.concatenate([tokens, offsets, ctxs, *arrays, tables.reshape(-1)]).astype(np.int32, copy=False)).to(device)
+        tok, off, ctx = meta[0:T].view(1, T), meta[T:2 * T], meta[2 * T:3 * T]
+        views, at_ = [], 3 * T
+        for arr in arrays:
+            views.append(meta[at_:at_ + len(arr)])
+            at_ += len(arr)
+        tab = meta[at_:].view(len(caches), n_pages)
 
         emb = model.embedding.weight
         x = ext.quantized_embedding(tok, emb.scales, emb.biases, emb.weight, emb.group_size, emb.bits).view(T, -1)
@@ -122,17 +127,32 @@ def _run_pass(model, ids, lengths, max_tokens, pooling, normalize, dimensions, d
             h = _normed(x, block.input_layernorm)
             q = ext.chunk_qk_norm_rope_append(_proj(h, packed[i].qkv), at.q_norm._weight_as(h.dtype, h.device),
                                               at.k_norm._weight_as(h.dtype, h.device), off, tab[i], ctx, pool._key_pages, pool._value_pages,
-                                              Hq, Hkv, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)  # [Hq, T, D]
-            a = ext.paged_attention_segments(q, pool._key_pages, pool._value_pages, tab[i], segs, at.scale, Hkv, Hq)
+                                              at.num_heads, at.num_kv_heads, at.rope.base, at.q_norm.eps, inv_freq=at.rope.inv_freq)  # [Hq, T, D]
+            a = attend(q, at, pool, tab[i], views)
             x = ext.add(x, _proj(a, at.wo))
             h = _normed(x, block.post_attention_layernorm)
             x = ext.add(x, _proj(ext.swiglu(_proj(h, mlp.w_gate), _proj(h, mlp.w_up)), mlp.w_down))
-        # segment s of embed_pool = bounds[2s] .. bounds[2s + 1]: pool every other segment (the gaps are padding)
-        out = ext.embed_pool(x, model.norm._weight_as(x.dtype, x.device), model.norm.eps, bnd, pooling, dimensions, normalize)
-        return out[0::2]
+        return head(x, views)
     finally:
         for cache in caches:
             cache.release()
+
+
+def _run_pass(model, ids, lengths, max_tokens, pooling, normalize, dimensions, device) -> torch.Tensor:
+    """One packed pass: the pooled rows of its prompts, in order."""
+    offsets, ctxs, seg, bounds = pass_layout(lengths, max_tokens)
+    tokens = np.zeros(max_tokens, dtype=np.int32)
+    for p, s in zip(ids, bounds[0::2]):
+        tokens[s:s + len(p)] = p
+
+    def attend(q, at, pool, table, views):
+        return ext.paged_attention_segments(q, pool._key_pages, pool._value_pages, table, views[0], at.scale, at.num_kv_heads, at.num_heads)
+
+    def head(x, views):
+        # segment s of embed_pool = bounds[2s] .. bounds[2s + 1]: pool every other segment (the gaps are padding)
+        return ext.embed_pool(x, model.norm._weight_as(x.dtype, x.device), model.norm.eps, views[1], pooling, dimensions, normalize)[0::2]
+
+    return run_packed_pass(model, max_tokens, tokens, offsets, ctxs, [seg, bounds], attend, head, device)
 
 
 def embed_ids(model, prompts, pooling: str = "last", normalize: bool = True, dimensions: int | None = None, max_tokens: int = 8192,
