@@ -561,7 +561,7 @@ int tl_decode_attention_fused_rows(const void *qkv, const void *q_norm_weight, c
                                    int head_dim, float eps, float scale, int num_pages, int page_size, int max_pages,
                                    int max_context, int dtype, void *stream);
 /* ---- Qwen3-MoE sparse block (moe.py:36-89 of the reference) ----------------
- * One layer runs: router projection (tl_quantized_matmul*), tl_moe_topk, tl_moe_group, tl_moe_gather,
+ * One layer runs: router projection (tl_quantized_matmul*, or tl_moe_router for 8-bit group-64 routers), tl_moe_topk, tl_moe_group, tl_moe_gather,
  * tl_moe_grouped_matmul (gate|up, EPI_SWIGLU_PAIRS, sorted output), tl_moe_grouped_matmul (down, scattered back to
  * the original row order with out_index = perm), tl_moe_combine.  All are capture-safe: outputs are sized by
  * R = T * k rows and E experts, nothing synchronises and no count is read by the host.  Rounding (DESIGN.md):
@@ -599,6 +599,18 @@ int tl_moe_grouped_matmul(const void *scales, const void *biases, const void *b,
  * or a negative TL_E* code for arguments the launch rejects. */
 enum { TL_MOE_CONTROL = 0, TL_MOE_WGMMA = 1 };
 int tl_moe_grouped_matmul_route(int T, int k, int E, int N, int K, int epilogue, int dtype, const void *a, const void *b, int *nt, int *max_tiles);
+/* Router projection of a router stored as MLX affine 8-bit codes at group 64 (the group-128 projection entries take
+ * the others): w uint32 [E, H / 4] (code j of a word in bits [8 j, 8 j + 8)), scales / biases [E, H / 64] and x [T, H]
+ * of one 16-bit dtype, logits [T, E]:
+ *   logits[t, e] = T(sum over groups g, in a fixed order, of fp32 scale[e, g] * sum_k code[e, k] a[t, k]
+ *                                                             + bias[e, g] * sum_k a[t, k])      (k in group g)
+ * i.e. sum_k (scale * code + bias) * a in fp32, rounded once.  With norm_weight [H] (else NULL) a = the row's RMSNorm
+ * T(x * rsqrt(mean(x^2) + eps) * w), bit for bit tl_rms_norm's output; without it a = x.  E <= 256, H % 64 == 0,
+ * 0 <= T <= TL_MOE_ROUTER_MAX_ROWS; x, w and norm_weight 16-byte aligned.  A row's logits depend only on that row.
+ * Other arguments: TL_EINVAL. */
+#define TL_MOE_ROUTER_MAX_ROWS (1 << 19)
+int tl_moe_router(const void *x, const void *norm_weight, float eps, const void *w, const void *scales, const void *biases, void *logits, int T,
+                  int E, int H, int dtype, void *stream);
 /* out [T, H] = T(residual + T(sum_fp32 over j < k of T(y[t k + j] * scores[t, j]))) (no residual: the sum alone);
  * y [T k, H] in original row order.  With norm_weight, normed_out = the RMSNorm of out (H <= 4096). */
 int tl_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_weight, float eps, void *out, void *normed_out,

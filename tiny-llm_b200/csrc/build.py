@@ -41,6 +41,7 @@ SOURCES = [
     "logprobs.cu",
     "constrained.cu",
     "moe.cu",
+    "moe_router.cu",
     "lora.cu",
     "embed.cu",
     "tma.cu",

@@ -1021,6 +1021,19 @@ int tl_moe_combine(const void *y, const void *scores, const void *residual, cons
     return launch_moe_combine(y, scores, residual, norm_weight, eps, out, normed_out, T, k, H, dtype, as_stream(stream));
 }
 
+int tl_moe_router(const void *x, const void *norm_weight, float eps, const void *w, const void *scales, const void *biases, void *logits, int T,
+                  int E, int H, int dtype, void *stream) {
+    if (dtype != TL_F16 && dtype != TL_BF16) return fail(TL_EINVAL, "moe_router: x must be float16 or bfloat16");
+    if (T < 0 || T > TL_MOE_ROUTER_MAX_ROWS) return fail(TL_EINVAL, "moe_router: rows must be in [0, %d] (got %d)", TL_MOE_ROUTER_MAX_ROWS, T);
+    if (E <= 0 || E > TL_MOE_MAX_EXPERTS) return fail(TL_EINVAL, "moe_router: 1 to %d experts (got %d)", TL_MOE_MAX_EXPERTS, E);
+    if (H <= 0 || H % 64 != 0) return fail(TL_EINVAL, "moe_router: the hidden size must be a positive multiple of 64 (got %d)", H);
+    if (T == 0) return TL_OK;
+    if (!x || !w || !scales || !biases || !logits) return fail(TL_EINVAL, "moe_router: null pointer");
+    if (!aligned16(x) || !aligned16(w) || (norm_weight && !aligned16(norm_weight)))
+        return fail(TL_EINVAL, "moe_router: x, the codes and the norm weight must be 16-byte aligned");
+    return launch_moe_router(x, norm_weight, eps, w, scales, biases, logits, T, E, H, dtype, as_stream(stream));
+}
+
 int tl_lora_apply_route(int M, int dtype, const tl_lora_site *site) { return lora_route(M, dtype, site); }
 
 int tl_lora_apply(const void *x, void *const *y, const void *const *residual, const long long *ldy, const int32_t *adapter_ids,

@@ -127,6 +127,9 @@ int launch_moe_gather(const void *x, const int32_t *perm, const void *norm_w, fl
                       cudaStream_t st);
 int launch_moe_combine(const void *y, const void *scores, const void *residual, const void *norm_w, float eps, void *out, void *normed, int T,
                        int k, int H, int dtype, cudaStream_t st);
+// moe_router.cu (8-bit group-64 router projection, optional RMSNorm prologue: norm_w null or [H])
+int launch_moe_router(const void *x, const void *norm_w, float eps, const void *w, const void *scales, const void *biases, void *out, int T,
+                      int E, int H, int dtype, cudaStream_t st);
 int launch_moe_grouped_vanilla(const void *scales, const void *biases, const void *a, const void *b, void *out, const int32_t *offsets,
                                const int32_t *out_index, int R, int E, int N, int K, int epilogue, int dtype, cudaStream_t st);
 

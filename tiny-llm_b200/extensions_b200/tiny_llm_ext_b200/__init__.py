@@ -79,6 +79,8 @@ __all__ = [
     "moe_grouped_matmul",
     "moe_grouped_matmul_route",
     "moe_combine",
+    "moe_router",
+    "MOE_ROUTER_GROUP",
     "LoraSite",
     "lora_apply",
     "lora_apply_route",
@@ -173,6 +175,7 @@ _SIGNATURES = {
     "tl_moe_grouped_matmul_route": (_I, [_I] * 7 + [_VP] * 2 + [ctypes.POINTER(_I)] * 2),
     "tl_moe_grouped_matmul": (_I, [_VP] * 8 + [_I] * 7 + [_VP]),
     "tl_moe_combine": (_I, [_VP] * 4 + [_F, _VP, _VP] + [_I] * 4 + [_VP]),
+    "tl_moe_router": (_I, [_VP, _VP, _F] + [_VP] * 4 + [_I] * 4 + [_VP]),
     "tl_lora_apply_route": (_I, [_I, _I, _VP]),
     "tl_lora_apply": (_I, [_VP] * 6 + [_I, _I, _VP]),
     "tl_shared_prefix_attention_workspace": (_SZ, [_I] * 5),
@@ -1738,6 +1741,39 @@ def moe_combine(y, scores, residual=None, norm_weight=None, eps=0.0, stream=None
 
 
 LORA_MAX_SEGMENTS, LORA_MAX_RANK, LORA_MAX_ADAPTERS = 3, 64, 32
+MOE_ROUTER_GROUP = 64  # group size of the 8-bit routers moe_router takes
+
+
+def moe_router(x, weight, scales, biases, norm_weight=None, eps=0.0, stream=None):
+    """Router logits ``[T, E]`` of an MLX affine 8-bit router at group 64 (``tl_moe_router``): ``x [T, H]`` (bf16 or
+    fp16), ``weight`` packed codes ``[E, H / 4]`` (int32 or uint32), ``scales`` / ``biases [E, H / 64]`` of x's dtype;
+    ``sum_k (scale * code + bias) * a`` in fp32, rounded once.  With ``norm_weight [H]``, ``a`` is the row's RMSNorm,
+    bit for bit ``rms_norm(x, norm_weight, eps)``; else ``a = x``."""
+    op = "moe_router"
+    if x.dim() != 2 or x.dtype not in _HALF:
+        raise RuntimeError(f"{op}: x must be float16 or bfloat16 [T, H]")
+    T, H = x.shape
+    if H <= 0 or H % MOE_ROUTER_GROUP:
+        raise RuntimeError(f"{op}: the hidden size must be a positive multiple of {MOE_ROUTER_GROUP}, got {H}")
+    if weight.dim() != 2 or weight.dtype not in _PACKED or weight.shape[1] * 4 != H:
+        raise RuntimeError(f"{op}: weight must be packed 8-bit codes [E, H / 4] = [E, {H // 4}] (int32 or uint32), got {tuple(weight.shape)}")
+    E = weight.shape[0]
+    if E <= 0 or E > MOE_MAX_EXPERTS:
+        raise RuntimeError(f"{op}: 1 to {MOE_MAX_EXPERTS} experts (got {E})")
+    G = H // MOE_ROUTER_GROUP
+    if scales.dtype != x.dtype or biases.dtype != x.dtype or tuple(scales.shape) != (E, G) or scales.shape != biases.shape:
+        raise RuntimeError(f"{op}: scales and biases must be [E, H / 64] = [{E}, {G}] of x's dtype")
+    if norm_weight is not None and (norm_weight.dtype != x.dtype or tuple(norm_weight.shape) != (H,)):
+        raise RuntimeError(f"{op}: norm weight must be [H] in the dtype of x")
+    extra = {} if norm_weight is None else {"norm_weight": norm_weight}
+    _gpu(op, x, weight, scales, biases, *extra.values())
+    _contig(op, x=x, weight=weight, scales=scales, biases=biases, **extra)
+    out = torch.empty((T, E), dtype=x.dtype, device=x.device)
+    _check(_lib.tl_moe_router(x.data_ptr(), None if norm_weight is None else norm_weight.data_ptr(), float(eps), weight.data_ptr(),
+                              scales.data_ptr(), biases.data_ptr(), out.data_ptr(), T, E, H, _DTYPE_CODE[x.dtype], _stream_ptr(stream, x)))
+    return out
+
+
 LORA_RANKS = (8, 16, 32, 64)
 LORA_ROWS, LORA_TILES = 0, 1
 

@@ -6,6 +6,7 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli generate --model /path/to/Qwen3-4B-MLX-4bit --prompt "..." [--loader week3]
     python -m tiny_llm_b200.cli batch    --model /path/to/ckpt --prompts-file prompts.txt --batch-size 5
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --max-new-tokens 8   (no files needed)
+    python -m tiny_llm_b200.cli generate --model /path/to/Qwen3-30B-A3B-MLX-4bit --prompt "..."   (Qwen3-MoE; --synthetic tiny-moe-d128 without files)
     python -m tiny_llm_b200.cli batch    --synthetic tiny-d128 --prompt-ids "5,17,3;9,2,4" --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
         (seeded sampling with the tl_sample kernel: the same seed gives the same tokens)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --sampler-temp 0.7 --presence-penalty 1.5 --min-p 0.05
@@ -41,8 +42,12 @@ from __future__ import annotations
 
 import argparse
 import sys
+from pathlib import Path
 
 import torch
+
+
+TOKENIZER_FILES = ("tokenizer.json", "tokenizer_config.json", "vocab.json", "tokenizer.model")
 
 
 def _load(args, device):
@@ -56,6 +61,10 @@ def _load(args, device):
                 "Qwen/Qwen3-synthetic")
     ns = load_checkpoint(args.model, device=device)
     tokenizer = None
+    if not any((Path(args.model) / f).exists() for f in TOKENIZER_FILES):
+        # transformers would build an empty-vocabulary tokenizer from config.json alone and print every token as ""
+        print(f"(no tokenizer files in {args.model}: token ids are printed)", file=sys.stderr)
+        return ns, None, "Qwen/Qwen3-" + str(args.model)
     try:
         tokenizer = load_tokenizer(args.model)
     except Exception as exc:  # token-id mode still works without tokenizer files
@@ -528,7 +537,8 @@ def main(argv=None) -> int:
         p = sub.add_parser(name)
         p.set_defaults(fn=fn)
         p.add_argument("--model", default=None, help="checkpoint directory (config.json + *.safetensors [+ tokenizer files])")
-        p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny, tiny-d128, qwen3-0.6b, qwen3-4b) instead of --model")
+        p.add_argument("--synthetic", default=None, help="random weights of a named shape (tiny, tiny-d128, qwen3-0.6b, qwen3-4b; Qwen3-MoE: "
+                       "tiny-moe-d128, qwen3-30b-a3b) instead of --model")
         p.add_argument("--synthetic-bits", type=int, choices=(4, 8), default=4,
                        help="code width of the --synthetic weights, and of a --draft-synthetic draft's (MLX affine, group 128)")
         p.add_argument("--prompt", default="Give me a short introduction to large language models.")

@@ -38,7 +38,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200 as ext
 
 from .kv_cache import BatchingKvCache
-from .moe import Moe
+from .moe import Moe, router_logits
 from .paged_kv_cache import TinyKvPagedCache
 
 # Decode attention runs as one fused launch while slots x max_seq_len stays within this: beyond it the K/V stream, not
@@ -125,12 +125,11 @@ def _moe_mlp(moe, x, h=None, ln2=None, nxt=None):
     (the matvec stack) the router projection takes ``ln2`` as its prologue and the gather applies it to each row.  With
     ``nxt`` (the next RMSNorm) the combine also returns its output, as ``(x, h)``.  Every row is routed, idle slots and
     padding rows included: a row's result depends only on that row."""
-    w = moe.w_router
     if h is None:
         norm = (ln2._weight_as(x.dtype, x.device), ln2.eps)
-        logits = ext.quantized_matmul_fused(w.scales, w.biases, w.weight, x, norm[0], prologue=ext.PRO_RMSNORM, eps=norm[1])
+        logits = router_logits(x, moe.w_router, norm=norm)
     else:
-        norm, logits = None, _proj(h, w)
+        norm, logits = None, router_logits(h, moe.w_router, projection=_proj)
     _, ids, scores = ext.moe_topk(logits, moe.num_experts_per_tok, moe.norm_topk_prob)
     return moe.experts(x if h is None else h, ids, scores, residual=x, gather_norm=norm,
                        next_norm=None if nxt is None else (nxt._weight_as(x.dtype, x.device), nxt.eps))

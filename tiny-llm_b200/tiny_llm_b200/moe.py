@@ -5,7 +5,7 @@ leading expert axis (``weight [E, out, in/8]``, ``scales``/``biases [E, out, in/
 layout).  A layer is one fixed launch sequence that never reads a count back to the host, so it can be captured in
 a CUDA graph:
 
-    router projection -> moe_topk -> moe_group -> moe_gather -> grouped gate|up (SwiGLU epilogue, sorted rows)
+    router projection (router_logits) -> moe_topk -> moe_group -> moe_gather -> grouped gate|up (SwiGLU epilogue, sorted rows)
     -> grouped down (scattered back to token order) -> moe_combine
 
 Rounding follows the reference's operator sequence, except that SwiGLU is the project's ``swiglu`` arithmetic on the
@@ -61,9 +61,30 @@ def grouped_expert_linear(x: torch.Tensor, w_experts: QuantizedWeights, expert_i
     return out.reshape(*lead, K)
 
 
+ROUTER_G64 = (8, ext.MOE_ROUTER_GROUP)  # (bits, group_size) of the routers mlx_lm stores apart from the model's setting
+
+
+def _check_router(w: QuantizedWeights) -> None:
+    if w.group_size == ext.MOE_ROUTER_GROUP and (w.bits, w.group_size) != ROUTER_G64:
+        raise ValueError(f"Moe: a group-{w.group_size} router must have 8-bit codes (got {w.bits} bits)")
+
+
+def router_logits(h: torch.Tensor, w: QuantizedWeights, norm=None, projection=quantized_linear) -> torch.Tensor:
+    """Router logits ``[..., E]`` of the rows ``h [..., H]``: the one place that picks the router's kernel.  An 8-bit
+    group-64 router (``ROUTER_G64``) runs ``ext.moe_router``; any other runs ``projection(h, w)`` (the caller's
+    projection launch), or with ``norm = (weight, eps)`` the streaming projection with the RMSNorm prologue.  With
+    ``norm``, ``h`` is not yet normalised; both forms give the bits of ``rms_norm`` followed by the projection."""
+    if (w.bits, w.group_size) == ROUTER_G64:
+        rows = h.reshape(-1, h.shape[-1]).contiguous()
+        return ext.moe_router(rows, w.weight, w.scales, w.biases, *(norm or ())).reshape(*h.shape[:-1], -1)
+    if norm is not None:
+        return ext.quantized_matmul_fused(w.scales, w.biases, w.weight, h, norm[0], prologue=ext.PRO_RMSNORM, eps=norm[1])
+    return projection(h, w)
+
+
 def route_topk(x: torch.Tensor, w_router: QuantizedWeights, top_k: int, norm_topk_prob: bool = False):
     """moe.py:36-49 - ``(probs [..., E], ids [..., k], scores [..., k])``; ids in descending order of probability."""
-    logits = quantized_linear(x, w_router)
+    logits = router_logits(x, w_router)
     *lead, E = logits.shape
     probs, ids, scores = ext.moe_topk(logits.reshape(-1, E).contiguous(), int(top_k), norm_topk_prob)
     return probs.reshape(*lead, E), ids.reshape(*lead, top_k), scores.reshape(*lead, top_k)
@@ -89,6 +110,7 @@ class Moe:
         self.w_down = w_down
         self.num_experts_per_tok = num_experts_per_tok
         self.norm_topk_prob = norm_topk_prob
+        _check_router(w_router)
         E, inter, hidden = _experts(w_gate, "Moe")
         if _experts(w_up, "Moe") != (E, inter, hidden) or _experts(w_down, "Moe") != (E, hidden, inter):
             raise ValueError("Moe: gate / up must be [E, I, H] and down [E, H, I] experts")

@@ -57,13 +57,29 @@ def make_args(name_or_dims, **overrides) -> SimpleNamespace:
         from .rope_scaling import parse_rope_scaling
 
         dims["rope_scaling"] = parse_rope_scaling(dims["rope_scaling"], dims["max_position_embeddings"]).to_config()
-    if dims.get("num_experts", 0) > 0:  # Qwen3-MoE keys (mlx_lm qwen3_moe.ModelArgs)
+    moe_defaults(dims)
+    return SimpleNamespace(**dims)
+
+
+MOE_KEYS = ("num_experts", "num_experts_per_tok", "moe_intermediate_size", "norm_topk_prob", "decoder_sparse_step", "mlp_only_layers")
+
+
+def moe_defaults(dims: dict) -> dict:
+    """Fill the Qwen3-MoE keys a config with ``num_experts > 0`` leaves out (mlx_lm qwen3_moe.ModelArgs), in place; the
+    loader applies the same defaults to ``config.json``."""
+    if dims.get("num_experts", 0) > 0:
         dims.setdefault("num_experts_per_tok", 8)
         dims.setdefault("moe_intermediate_size", dims["intermediate_size"])
         dims.setdefault("norm_topk_prob", True)
         dims.setdefault("decoder_sparse_step", 1)
         dims.setdefault("mlp_only_layers", [])
-    return SimpleNamespace(**dims)
+    return dims
+
+
+def is_sparse_layer(args, index: int) -> bool:
+    """qwen3_week3.is_qwen3_moe_sparse_layer, for code that must not import the model."""
+    return (getattr(args, "num_experts", 0) > 0 and index not in getattr(args, "mlp_only_layers", [])
+            and (index + 1) % getattr(args, "decoder_sparse_step", 1) == 0)
 
 
 def quantize_w4(weight: torch.Tensor, group_size: int = GROUP_SIZE):
@@ -113,22 +129,22 @@ def pack_codes(codes: torch.Tensor, bits: int) -> torch.Tensor:
     return torch.where(words >= 2**31, words - 2**32, words).to(torch.int32).view(torch.uint32)
 
 
-def _random_layer(out_dim: int, in_dim: int, gen: torch.Generator, bits: int = BITS) -> SimpleNamespace:
+def _random_layer(out_dim: int, in_dim: int, gen: torch.Generator, bits: int = BITS, group_size: int = GROUP_SIZE) -> SimpleNamespace:
     """Random codes + signed scales; dequantised weights ~ N(0, 1/in_dim)
     (value = (q - c)*s + e with q uniform on [0, 2c]: 4 bits c = 7.5, var = 22.25*sigma^2; 8 bits c = 127.5 and
     s scaled by 15/255, the same weight distribution)."""
     sigma = 1.0 / (4.717 * in_dim**0.5)
     centre, step = (7.5, 1.0) if bits == 4 else (127.5, 15.0 / 255.0)
     words = torch.randint(-(2**31), 2**31, (out_dim, in_dim * bits // 32), dtype=torch.int64, generator=gen).to(torch.int32)
-    scales = (torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * (sigma * step)).to(torch.bfloat16)
-    biases = (-centre * scales.to(torch.float32) + torch.randn(out_dim, in_dim // GROUP_SIZE, generator=gen) * sigma).to(torch.bfloat16)
-    return SimpleNamespace(weight=words.view(torch.uint32), scales=scales, biases=biases, group_size=GROUP_SIZE, bits=bits)
+    scales = (torch.randn(out_dim, in_dim // group_size, generator=gen) * (sigma * step)).to(torch.bfloat16)
+    biases = (-centre * scales.to(torch.float32) + torch.randn(out_dim, in_dim // group_size, generator=gen) * sigma).to(torch.bfloat16)
+    return SimpleNamespace(weight=words.view(torch.uint32), scales=scales, biases=biases, group_size=group_size, bits=bits)
 
 
-def _quantized_layer(out_dim: int, in_dim: int, gen: torch.Generator, std: float, bits: int = BITS) -> SimpleNamespace:
+def _quantized_layer(out_dim: int, in_dim: int, gen: torch.Generator, std: float, bits: int = BITS, group_size: int = GROUP_SIZE) -> SimpleNamespace:
     dense = torch.randn(out_dim, in_dim, generator=gen) * std
-    words, scales, biases = quantize_w4(dense) if bits == 4 else quantize_affine(dense, bits)
-    return SimpleNamespace(weight=words, scales=scales, biases=biases, group_size=GROUP_SIZE, bits=bits)
+    words, scales, biases = quantize_w4(dense) if bits == 4 and group_size == GROUP_SIZE else quantize_affine(dense, bits, group_size)
+    return SimpleNamespace(weight=words, scales=scales, biases=biases, group_size=group_size, bits=bits)
 
 
 def _norm_weight(dim: int, gen: torch.Generator) -> SimpleNamespace:
@@ -139,34 +155,41 @@ def _empty_norm(dim: int, device) -> SimpleNamespace:
     return SimpleNamespace(weight=torch.empty((dim,), dtype=torch.bfloat16, device=device))
 
 
-def _empty_layer(out_dim: int, in_dim: int, device, bits: int = BITS) -> SimpleNamespace:
+def _empty_layer(out_dim: int, in_dim: int, device, bits: int = BITS, group_size: int = GROUP_SIZE) -> SimpleNamespace:
     return SimpleNamespace(
         weight=torch.empty((out_dim, in_dim * bits // 32), dtype=torch.int32, device=device).view(torch.uint32),
-        scales=torch.empty((out_dim, in_dim // GROUP_SIZE), dtype=torch.bfloat16, device=device),
-        biases=torch.empty((out_dim, in_dim // GROUP_SIZE), dtype=torch.bfloat16, device=device),
-        group_size=GROUP_SIZE,
+        scales=torch.empty((out_dim, in_dim // group_size), dtype=torch.bfloat16, device=device),
+        biases=torch.empty((out_dim, in_dim // group_size), dtype=torch.bfloat16, device=device),
+        group_size=group_size,
         bits=bits,
     )
 
 
 def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realistic: bool = False, empty: bool = False,
-                    bits: int = BITS, **overrides) -> SimpleNamespace:
+                    bits: int = BITS, router_bits: int | None = None, router_group_size: int | None = None, **overrides) -> SimpleNamespace:
     """Random Qwen3-shaped model.  ``realistic=True`` quantises Gaussian dense
     weights with ``quantize_w4`` (``quantize_affine`` at 8 bits; slow, for small models); the default draws
     codes/scales directly, which is what the 4B-sized benchmarks use.
     ``empty=True`` only allocates (uninitialised, directly on ``device``): the
-    receive side of the data-parallel weight broadcast.  ``bits``: 4 or 8 (MLX affine, group 128)."""
+    receive side of the data-parallel weight broadcast.  ``bits``: 4 or 8 (MLX affine, group 128).
+    ``router_bits`` / ``router_group_size`` (Qwen3-MoE): the width and group of every sparse layer's router
+    (``mlp.gate``) when it differs from the model's; 8 and 64 give the layout mlx_lm converts qwen3_moe routers to.
+    None keeps the model's setting (and every draw of the model without them)."""
     if bits not in SUPPORTED_BITS:
         raise ValueError(f"synthetic_qwen3: bits must be 4 or 8, got {bits}")
+    router_bits = bits if router_bits is None else router_bits
+    router_group_size = GROUP_SIZE if router_group_size is None else router_group_size
+    if router_bits not in SUPPORTED_BITS or router_group_size not in (64, GROUP_SIZE):
+        raise ValueError(f"synthetic_qwen3: router bits must be 4 or 8 and its group 64 or 128, got {router_bits} / {router_group_size}")
     args = make_args(name_or_dims, **overrides)
     gen = torch.Generator().manual_seed(seed)
 
-    def layer(out_dim: int, in_dim: int) -> SimpleNamespace:
+    def layer(out_dim: int, in_dim: int, width: int = bits, group_size: int = GROUP_SIZE) -> SimpleNamespace:
         if empty:
-            return _empty_layer(out_dim, in_dim, device, bits)
+            return _empty_layer(out_dim, in_dim, device, width, group_size)
         if realistic:
-            return _quantized_layer(out_dim, in_dim, gen, std=in_dim**-0.5, bits=bits)
-        return _random_layer(out_dim, in_dim, gen, bits)
+            return _quantized_layer(out_dim, in_dim, gen, std=in_dim**-0.5, bits=width, group_size=group_size)
+        return _random_layer(out_dim, in_dim, gen, width, group_size)
 
     def norm(dim: int) -> SimpleNamespace:
         return _empty_norm(dim, device) if empty else _norm_weight(dim, gen)
@@ -180,12 +203,10 @@ def synthetic_qwen3(name_or_dims="qwen3-4b", seed: int = 0, device="cpu", realis
         return SimpleNamespace(**stacked, group_size=GROUP_SIZE, bits=bits)
 
     def mlp(index: int) -> SimpleNamespace:
-        sparse = (getattr(args, "num_experts", 0) > 0 and index not in args.mlp_only_layers
-                  and (index + 1) % args.decoder_sparse_step == 0)  # qwen3_week3.is_qwen3_moe_sparse_layer
-        if sparse:
+        if is_sparse_layer(args, index):
             inter = args.moe_intermediate_size
             return SimpleNamespace(
-                gate=layer(args.num_experts, args.hidden_size),
+                gate=layer(args.num_experts, args.hidden_size, router_bits, router_group_size),
                 switch_mlp=SimpleNamespace(gate_proj=experts(inter, args.hidden_size), up_proj=experts(inter, args.hidden_size),
                                            down_proj=experts(args.hidden_size, inter)),
             )
