@@ -367,6 +367,28 @@ int tl_sample_constrained(const void *logits, const float *temperature, const in
                           const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                           const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab,
                           int dtype, void *stream);
+/* JSON mode (DESIGN.md section 20): a byte-level pushdown automaton over RFC 8259 `ws object ws`, with at most
+ * TL_JSON_MAX_DEPTH open containers and at most TL_JSON_MAX_WS_RUN consecutive whitespace bytes.  A JSON row is a
+ * tl_constraint_row with num_states = 1 whose mask is the row's own uint32 [2, ceil(vocab / 32)] buffer (row 0: this
+ * step's mask, written by tl_json_token_masks; row 1: EOS only) and whose dfa is an all-zero int32 [1, 256] table, so
+ * tl_sample_constrained keeps state 0 for a token with bytes and moves to 1 (terminal) on EOS.  Its automaton state is
+ * two int64 words per row:
+ *   word 0         the container stack: bit d set iff the container at depth d + 1 is an array;
+ *   word 1         bits 0-6 depth, 8-12 lexer state, 16-21 current whitespace run, 24-26 and 27-29 the lexer state's
+ *                  progress (UTF-8 bytes to go and the next byte's range, hex digits to go, literal and index),
+ *                  30 the open string is a key, 32 the row is in JSON mode, 33 terminal (after EOS).
+ * Lexer state 7 is "closed": the top-level object has closed and only whitespace and EOS may follow. */
+#define TL_JSON_MAX_DEPTH 64
+#define TL_JSON_MAX_WS_RUN 32
+/* Row 0 of every JSON row's mask (rows with bit 32 set and bit 33 clear; others are not touched), in one launch: bit t
+ * iff token t has bytes and walking them from the row's state stays in the language within both caps, or t has no
+ * bytes, the text is complete and bit t of the row's mask row 1 is set.  The vocabulary is the row's descriptor's
+ * token_offsets / token_bytes.  Deterministic, no atomics. */
+int tl_json_token_masks(const tl_constraint_row *constraints, const int64_t *json_states, int rows, int vocab, void *stream);
+/* After the draw: for JSON rows with positions[r] > 0 and not terminal, the state becomes the walk of tokens[r]'s
+ * bytes, or terminal when the token has no bytes (EOS).  Other rows are unchanged. */
+int tl_json_advance(const tl_constraint_row *constraints, int64_t *json_states, const int32_t *tokens, const int32_t *positions, int rows,
+                    void *stream);
 /* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
  * launch, one cluster of CTAs per row (DESIGN.md section 8a).
  *

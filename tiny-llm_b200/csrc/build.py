@@ -40,6 +40,7 @@ SOURCES = [
     "beam.cu",
     "logprobs.cu",
     "constrained.cu",
+    "json.cu",
     "moe.cu",
     "moe_router.cu",
     "lora.cu",

@@ -638,6 +638,19 @@ int tl_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num
                                          as_stream(stream));
 }
 
+int tl_json_token_masks(const tl_constraint_row *constraints, const int64_t *json_states, int rows, int vocab, void *stream) {
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "json_token_masks: bad shape");
+    if (rows > 0 && (!constraints || !json_states)) return fail(TL_EINVAL, "json_token_masks: null pointer");
+    return launch_json_token_masks(constraints, json_states, rows, vocab, as_stream(stream));
+}
+
+int tl_json_advance(const tl_constraint_row *constraints, int64_t *json_states, const int32_t *tokens, const int32_t *positions, int rows,
+                    void *stream) {
+    if (rows < 0) return fail(TL_EINVAL, "json_advance: bad shape");
+    if (rows > 0 && (!constraints || !json_states || !tokens || !positions)) return fail(TL_EINVAL, "json_advance: null pointer");
+    return launch_json_advance(constraints, json_states, tokens, positions, rows, as_stream(stream));
+}
+
 int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
                 int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
                 void *stream) {

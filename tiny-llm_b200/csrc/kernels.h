@@ -53,6 +53,10 @@ int launch_sample_constrained(const void *logits, const float *temperature, cons
 int launch_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                                   const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks,
                                   uint32_t *reach, cudaStream_t st);
+// json.cu
+int launch_json_token_masks(const tl_constraint_row *constraints, const int64_t *states, int rows, int vocab, cudaStream_t st);
+int launch_json_advance(const tl_constraint_row *constraints, int64_t *states, const int32_t *tokens, const int32_t *positions, int rows,
+                        cudaStream_t st);
 // logprobs.cu: same cluster plan as sampling.cu
 constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
 int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,

@@ -59,6 +59,9 @@ __all__ = [
     "NGRAM_TILE",
     "NGRAM_STATE_WORDS",
     "constraint_token_masks",
+    "json_token_masks",
+    "json_advance",
+    "JSON_STATE_WORDS",
     "logprobs",
     "LOGPROBS_MAX_N",
     "decode_advance",
@@ -141,6 +144,8 @@ _SIGNATURES = {
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
+    "tl_json_token_masks": (_I, [_VP, _VP, _I, _I, _VP]),
+    "tl_json_advance": (_I, [_VP] * 4 + [_I, _VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_qkv_project_rope_append_table": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP, _VP]),
@@ -1020,6 +1025,44 @@ def sample_constrained(logits, temperature, top_k, top_p, seed, positions, const
                                       positions.data_ptr(), *ptr, constraints.data_ptr(), out.data_ptr(), rows, vocab,
                                       _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
+
+
+JSON_STATE_WORDS = 2  # int64 words of one JSON row's automaton state (include/tiny_llm_b200.h)
+
+
+def _json_rows(op, constraints, json_states):
+    if constraints.dtype != torch.int64 or constraints.dim() != 2 or constraints.shape[1] != CONSTRAINT_ROW_WORDS:
+        raise RuntimeError(f"{op}: constraints must be int64 [rows, {CONSTRAINT_ROW_WORDS}]")
+    rows = constraints.shape[0]
+    if json_states.dtype != torch.int64 or tuple(json_states.shape) != (rows, JSON_STATE_WORDS):
+        raise RuntimeError(f"{op}: json_states must be int64 [{rows}, {JSON_STATE_WORDS}]")
+    return rows
+
+
+def json_token_masks(constraints, json_states, vocab, stream=None):
+    """Row 0 of each JSON row's mask buffer (``tl_json_token_masks``): ``constraints`` int64 ``[rows, 5]``
+    descriptors, ``json_states`` int64 ``[rows, 2]`` automaton states; rows not in JSON mode, or terminal, are not
+    touched.  Writes through the descriptors' mask pointers; returns nothing."""
+    rows = _json_rows("json_token_masks", constraints, json_states)
+    if isinstance(vocab, bool) or not isinstance(vocab, int) or vocab <= 0:
+        raise RuntimeError("json_token_masks: vocab must be a positive int")
+    _contig("json_token_masks", constraints=constraints, json_states=json_states)
+    _gpu("json_token_masks", constraints, json_states)
+    _check(_lib.tl_json_token_masks(constraints.data_ptr(), json_states.data_ptr(), rows, vocab, _stream_ptr(stream, constraints)))
+
+
+def json_advance(constraints, json_states, tokens, positions, stream=None):
+    """Advance each JSON row's automaton state by its drawn token (``tl_json_advance``), for rows with
+    ``positions > 0``; ``tokens`` and ``positions`` int32 ``[rows]``."""
+    rows = _json_rows("json_advance", constraints, json_states)
+    for name, t in (("tokens", tokens), ("positions", positions)):
+        if t.dtype != torch.int32 or tuple(t.shape) != (rows,):
+            raise RuntimeError(f"json_advance: {name} must be int32 [{rows}]")
+    named = dict(constraints=constraints, json_states=json_states, tokens=tokens, positions=positions)
+    _contig("json_advance", **named)
+    _gpu("json_advance", *named.values())
+    _check(_lib.tl_json_advance(constraints.data_ptr(), json_states.data_ptr(), tokens.data_ptr(), positions.data_ptr(), rows,
+                                _stream_ptr(stream, constraints)))
 
 
 def constraint_token_masks(dfa, accept, token_offsets, token_bytes, eos_ids, stream=None):

@@ -25,6 +25,7 @@ from extensions_b200 import tiny_llm_ext_b200
 from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, token_logprobs
 from .lora import adapter_ids_of
+from .json_mode import ConstraintRows
 from .sampler import any_constrained, any_penalized, sample_tokens, sampling_per_request, token_state_row
 
 
@@ -67,7 +68,7 @@ class Request:
     ``SamplingParams``) draws the request's tokens with the seeded ``tl_sample``
     kernel; None keeps them greedy.  A penalised ``sampling`` draws the first
     token against the prompt-only token state (``token_state_row``).  A constrained ``sampling`` draws the first token
-    under the start state of ``constraint_row``, its one-row descriptor, which that launch advances.  ``logprobs``
+    under the start state of ``constraint_row``, its one-row ``ConstraintRows``, which that launch advances.  ``logprobs``
     (an int N) records one ``TokenLogprobs`` per generated token in
     ``logprob_entries``."""
 
@@ -91,7 +92,7 @@ class Request:
         self.sampling = sampling
         self.logprobs = logprobs
         self.logprob_entries: list = []
-        self.constraint_row = None  # int64 [1, 5] tl_constraint_row, made with the first token's draw
+        self.constraint_row = None  # one-row ConstraintRows, made with the first token's draw
         self.model = model
         if isinstance(prompt, str):
             ids = tokenizer.encode(prompt, add_special_tokens=False)
@@ -149,7 +150,7 @@ class Request:
                     if self.sampling.penalized:
                         state = token_state_row(self.prefill_tokens, [], logits.shape[-1], device=logits.device)[None]
                     if self.sampling.constraint is not None:
-                        self.constraint_row = self.sampling.constraint.descriptor()[None]
+                        self.constraint_row = ConstraintRows.build([self.sampling], logits.shape[-1], logits.device)
                     token = sample_tokens(logits, [self.sampling], [total], state, self.constraint_row)
                 if self.logprobs is not None:
                     entry = token_logprobs(logits, token, self.logprobs)[0]
@@ -233,8 +234,9 @@ class ContinuousBatcher:
     prompt and the first token, and every decode step with a penalised slot is one ``tl_sample_penalized`` launch over
     all slots (idle slots at position 0, so their rows do not change); the kernel counts each drawn token.
 
-    Constrained requests (``SamplingParams.constraint``) keep their automaton state in one int64 ``[batch_size, 5]``
-    slab of ``tl_constraint_row`` descriptors, allocated when the first of them enters a slot.  Admission copies the
+    Constrained requests (``SamplingParams.constraint``) keep their automaton state in one ``ConstraintRows`` of
+    ``batch_size`` rows (``tl_constraint_row`` descriptors, plus JSON states and mask buffers once a JSON request
+    enters), allocated when the first of them enters a slot.  Admission copies the
     request's row (advanced by its prefill draw) into the slot on the device; idle and unconstrained slots hold zero
     rows.  Every decode step with a constrained slot is one ``tl_sample_constrained`` launch over all slots.
 
@@ -287,7 +289,7 @@ class ContinuousBatcher:
         self.peak_active_requests = 0
         self.peak_live_pages = 0
         self.token_state: torch.Tensor | None = None  # [batch_size, vocab] int32, on first penalised admission
-        self.constraint_rows: torch.Tensor | None = None  # [batch_size, 5] int64, on first constrained admission
+        self.constraint_rows: ConstraintRows | None = None  # batch_size rows, on first constrained admission
         self.prefix_cache = model.enable_prefix_cache() if prefix_cache else None
         self.reused_tokens: dict[int, int] = {}
         self.reused_total = 0
@@ -342,16 +344,17 @@ class ContinuousBatcher:
         token_state_row(request.prefill_tokens, [request.next_token], self.token_state.shape[1], out=self.token_state[slot])
 
     def _admit_constraint(self, request: Request, slot: int) -> None:
-        """Copy the request's constraint descriptor into the slot's row (a device copy), or zero the row."""
+        """Copy the request's constraint row into the slot's row (a device copy of its state), or clear the row.  The
+        JSON state and mask buffers are allocated with the first JSON request."""
         if self.constraint_rows is None:
             if request.constraint_row is None:
                 return
-            self.constraint_rows = torch.zeros((self.batch_size, request.constraint_row.shape[1]), dtype=torch.int64,
-                                               device=request.constraint_row.device)
+            src = request.constraint_row
+            self.constraint_rows = ConstraintRows(self.batch_size, src.vocab, src.device, src.has_json)
         if request.constraint_row is None:
-            self.constraint_rows[slot].zero_()
+            self.constraint_rows.clear_row(slot)
         else:
-            self.constraint_rows[slot].copy_(request.constraint_row[0])
+            self.constraint_rows.copy_row(slot, request.constraint_row)
 
     def _budget_spent(self, request: Request) -> bool:
         if self.max_new_tokens is None:
@@ -467,7 +470,7 @@ class ContinuousBatcher:
                     for table in self.kv_cache:
                         table.remove_request(i)
                     if self.constraint_rows is not None:
-                        self.constraint_rows[i].zero_()
+                        self.constraint_rows.clear_row(i)
                     self.results.append((request.prompt_idx, text))
                     self.slot_adapter_ids[i] = -1
                     self.slots[i] = None

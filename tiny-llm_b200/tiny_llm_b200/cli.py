@@ -29,6 +29,8 @@ see checkpoint.py; there is no hub download here).
         (requests share the KV pages of a common prompt prefix; reused tokens per request and cache stats after the text)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --regex "[0-9]{4}-[0-9]{2}-[0-9]{2}"
         (every generated token keeps the text inside the pattern's language; EOS ends it once it is a match)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --json
+        (the generated text is one JSON object: every prefix can still complete, EOS only once it has closed)
     python -m tiny_llm_b200.cli batch --synthetic tiny-d128 --synthetic-lora a=16 --synthetic-lora b=8:1 \
         --prompt-ids "5,17,3;5,17,3;5,17,3" --adapters "a;;b"
         (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
@@ -169,24 +171,30 @@ def _penalties(args) -> dict:
 
 
 def _constraint(args, model, tokenizer, device):
-    """The ``TokenConstraint`` of ``--regex`` over the checkpoint tokenizer's vocabulary (the synthetic vocabulary with
-    ``--synthetic``), or None."""
-    if args.regex is None:
+    """The ``TokenConstraint`` of ``--regex`` or the ``JsonConstraint`` of ``--json`` over the checkpoint tokenizer's
+    vocabulary (the synthetic vocabulary with ``--synthetic``), or None."""
+    if args.regex is not None and args.json:
+        raise SystemExit("give --regex or --json, not both")
+    if args.regex is None and not args.json:
         return None
     from .constrained import TokenConstraint, TokenVocabulary
+    from .json_mode import JsonConstraint
 
+    flag = "--regex" if args.regex is not None else "--json"
     if device.type != "cuda":
-        raise SystemExit("--regex runs on the CUDA sampling kernel: use a cuda --device")
+        raise SystemExit(f"{flag} runs on the CUDA sampling kernel: use a cuda --device")
     if args.synthetic:
         vocabulary = TokenVocabulary.synthetic(model.vocab_size)
     elif tokenizer is None:
-        raise SystemExit("--regex needs the checkpoint's tokenizer files (or --synthetic)")
+        raise SystemExit(f"{flag} needs the checkpoint's tokenizer files (or --synthetic)")
     else:
         vocabulary = TokenVocabulary.from_tokenizer(tokenizer, model.vocab_size)
     try:
+        if args.json:
+            return JsonConstraint(vocabulary, device=device)
         return TokenConstraint.compile(args.regex, vocabulary, device=device)
     except ValueError as exc:
-        raise SystemExit(f"--regex: {exc}")
+        raise SystemExit(f"{flag}: {exc}")
 
 
 def _adapter_kw(args, key: str) -> dict:
@@ -217,6 +225,8 @@ def cmd_generate(args) -> int:
         raise SystemExit("give one proposer: a draft (--draft-model / --draft-synthetic) or --prompt-lookup, not both")
     if speculative and args.regex is not None:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --regex")
+    if speculative and args.json:
+        raise SystemExit("speculative decoding is greedy and unconstrained: drop --json")
     constraint = _constraint(args, model, tokenizer, device)
     if constraint is not None:
         penalties["constraint"] = constraint
@@ -329,7 +339,7 @@ def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
     from .generate import beam_search_ids
 
     refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("penalties or --min-p", bool(penalties)),
-               ("--regex", args.regex is not None), ("--logprobs", args.logprobs is not None),
+               ("--regex", args.regex is not None), ("--json", args.json), ("--logprobs", args.logprobs is not None),
                ("adapters", args.adapter is not None or getattr(model, "adapters", None) is not None),
                ("a draft", bool(args.draft_model or args.draft_synthetic)), ("--prompt-lookup", args.prompt_lookup is not None)]
     for what, given in refused:
@@ -566,6 +576,8 @@ def main(argv=None) -> int:
                                        help="keep tokens at least this fraction as likely as the top one (0: off)")
         sub.choices[name].add_argument("--regex", default=None, metavar="PATTERN",
                                        help="constrain the generated text to fullmatch PATTERN (re.ASCII semantics over UTF-8 bytes)")
+        sub.choices[name].add_argument("--json", action="store_true",
+                                       help="constrain the generated text to one JSON object (RFC 8259; depth <= 64, whitespace runs <= 32)")
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")

@@ -37,6 +37,7 @@ import torch
 
 from extensions_b200 import tiny_llm_ext_b200 as ext
 
+from .json_mode import ConstraintRows, JsonConstraint
 from .kv_cache import BatchingKvCache
 from .moe import Moe, router_logits
 from .paged_kv_cache import TinyKvPagedCache
@@ -436,6 +437,13 @@ class DecodeEngine(_GraphEngine):
         # states the launches advance; all on first use
         self._graph_con: dict = {}
         self.kernels_per_constrained_step = 0
+        # decode_on_device(sampling=<with a JSON-mode slot>): one graph per (penalised, logprobs N or None), the
+        # constrained step between tl_json_token_masks and tl_json_advance over a B-row ConstraintRows (descriptors,
+        # JSON states and mask buffers; regex and plain slots ride along); all on first use
+        self._graph_json: dict = {}
+        self.kernels_per_json_step = 0
+        self._json_tab = None
+        self._json_key = None
         # decode_on_device(sampling=..., keep_logits=True): the sampled step plus one tl_log_rows launch that keeps the
         # step's logits rows in a [capacity, B, V] log at the step counter (a speculative draft's q rows); on first use
         self._graph_keep = None
@@ -483,7 +491,9 @@ class DecodeEngine(_GraphEngine):
         """The step's token per row: ``tl_argmax``, or (the sampled graph) ``tl_sample`` with the per-slot parameters at
         position ``context_lens``, the index of the token being drawn, or (the penalised graph) ``tl_sample_penalized``
         over ``token_counts``, or (a constrained graph) ``tl_sample_constrained`` over the slot descriptors, or (the
-        sampled verify graph, ``spec_draft`` the draft's logits rows) ``tl_speculative_sample`` on the proposals."""
+        sampled verify graph, ``spec_draft`` the draft's logits rows) ``tl_speculative_sample`` on the proposals.
+        ``constrained == "json"`` (the JSON graph) draws over the JSON table's descriptors, between the JSON rows' mask
+        launch and their state advance."""
         if spec_draft is not None:
             ext.speculative_sample(logits, spec_draft, self.tokens[1:R], *self._spec_params, self.context_lens[:R], out=self.next_tokens[:R])
             return
@@ -492,8 +502,14 @@ class DecodeEngine(_GraphEngine):
             if penalized:
                 p = self._pen_dev.view(torch.float32).view(4, self.B)
                 pen = (p[0, :R], p[1, :R], p[2, :R], p[3, :R], self.token_counts[:R])
+            tab = self._json_tab if constrained == "json" else None
+            if tab is not None:
+                ext.json_token_masks(tab.descriptors[:R], tab.json_states[:R], self.V)
+            descriptors = self._con_dev.view(self.B, -1)[:R] if tab is None else tab.descriptors[:R]
             tokens = ext.sample_constrained(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
-                                            self.context_lens[:R], self._con_dev.view(self.B, -1)[:R], *pen)
+                                            self.context_lens[:R], descriptors, *pen)
+            if tab is not None:
+                ext.json_advance(tab.descriptors[:R], tab.json_states[:R], tokens, self.context_lens[:R])
         elif penalized:
             pen = self._pen_dev.view(torch.float32).view(4, self.B)
             tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
@@ -673,6 +689,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_pen = None
         self._graph_lp = {}
         self._graph_con = {}
+        self._graph_json = {}
         self._graph_keep = None
         self._graph_spec = {}
         self._graph_beam = {}
@@ -861,6 +878,7 @@ class DecodeEngine(_GraphEngine):
             B, cap, dev = self.B, self.log_capacity, self.device
             self._graph_lp = {}
             self._graph_con = {k: g for k, g in self._graph_con.items() if k[1] is None}
+            self._graph_json = {k: g for k, g in self._graph_json.items() if k[1] is None}
             self._lp_max_n = max_n
             self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
                             torch.zeros((cap, B), dtype=torch.int32, device=dev), torch.zeros((cap, B, max_n), dtype=torch.int32, device=dev),
@@ -891,6 +909,57 @@ class DecodeEngine(_GraphEngine):
             self._graph_con[(penalized, max_n)] = self._graph_of(constrained_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_constrained_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _ensure_json_graph(self, penalized: bool, max_n: int | None) -> None:
+        """Capture the JSON-mode step: the constrained step with the JSON rows' masks before the draw and their advance
+        after it (the warm-up runs at context 0, so it advances no state).  One graph per (penalized, max_n)."""
+        if (penalized, max_n) in self._graph_json:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def json_step():
+            forward(sampled=True, penalized=penalized, constrained="json")
+            if max_n is not None:
+                ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()
+            self._graph_json[(penalized, max_n)] = self._graph_of(json_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_json_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_json_constraints(self, per: list, history) -> None:
+        """The JSON table's rows for the slots' constraints (JSON, regex or none), as ``_set_constraints`` sets the
+        descriptors: a slot with a ``history`` entry starts from the host walk of its generated ids (refused when they
+        leave the language), a slot with a new constraint from the start state, and every other constrained slot
+        keeps its device state."""
+        from .json_mode import JsonConstraint
+
+        B = self.B
+        cons = [None if p is None else p.constraint for p in per]
+        if history is not None:
+            history = list(history)
+            if len(history) != B:
+                raise ValueError(f"history must hold one (prompt_ids, generated_ids) or None per slot ({B})")
+        walked = {}
+        for b, c in enumerate(cons):
+            if c is None or history is None or history[b] is None:
+                continue
+            state = c.walk(history[b][1]) if isinstance(c, JsonConstraint) else c.walk(c.start_state, history[b][1])
+            if state is None or (not isinstance(c, JsonConstraint) and state < 0):
+                raise ValueError(f"slot {b}: its generated ids leave the constraint's language")
+            walked[b] = state
+        key = tuple(cons)
+        if self._json_key is not None and all(x is y for x, y in zip(key, self._json_key)) and not walked:
+            return
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)  # the previous call's replays read the table
+        for b, c in enumerate(cons):
+            if b in walked or self._json_key is None or self._json_key[b] is not c or c is None:
+                self._json_tab.set_row(b, c, walked.get(b))
+        self._json_key = key
 
     def _set_constraints(self, per: list, history) -> None:
         """Upload the slot descriptors when the slots' constraints change or ``history`` is given.  A slot whose
@@ -1198,7 +1267,9 @@ class DecodeEngine(_GraphEngine):
         With a constrained slot (``SamplingParams.constraint``) the step is ``tl_sample_constrained`` over the engine's
         slot descriptors, captured on first use per (penalised, logprobs); each launch advances the slots' automaton
         states.  ``history`` also sets a constrained slot's state to the walk of its generated ids; without it a slot
-        keeps its state while its constraint stays the same and starts at the start state otherwise.
+        keeps its state while its constraint stays the same and starts at the start state otherwise.  With a JSON-mode
+        slot (``JsonConstraint``) the step is a graph of its own: the JSON rows' masks, the constrained draw and their
+        state advance, with the same rules for ``history``.
         ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above.
         ``keep_logits=True`` (plain ``sampling``: no penalty, constraint or logprobs) replays the sampled step with one
         more launch that keeps each step's logits rows, and returns ``(tokens, logits [steps, B, V])``, a device view of
@@ -1247,7 +1318,15 @@ class DecodeEngine(_GraphEngine):
         self._adapters_of_call(adapter_ids)
         if penalized:
             self._alloc_penalties()
-        if constrained:
+        json = constrained and any(isinstance(p.constraint, JsonConstraint) for p in per if p is not None)
+        if json:
+            if self._json_tab is None:
+                self._json_tab = ConstraintRows(B, self.V, self.device, json=True)
+            if top_n is not None:
+                self._alloc_logprobs(max(top_n))
+                self._set_top_n(top_n)
+            self._ensure_json_graph(penalized, None if top_n is None else max(top_n))
+        elif constrained:
             if self._con_dev is None:
                 self._con_host = torch.zeros(5 * B, dtype=torch.int64, pin_memory=True)
                 self._con_dev = self._con_host.to(self.device, copy=True)
@@ -1276,12 +1355,16 @@ class DecodeEngine(_GraphEngine):
             self._set_sampling(sampling)
         if penalized:
             self._set_penalties(self._per_slot_sampling(sampling), history)
-        if constrained:
+        if json:
+            self._set_json_constraints(self._per_slot_sampling(sampling), history)
+        elif constrained:
             self._set_constraints(self._per_slot_sampling(sampling), history)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
-        if constrained:
+        if json:
+            graph = self._graph_json[(penalized, None if top_n is None else max(top_n))]
+        elif constrained:
             graph = self._graph_con[(penalized, None if top_n is None else max(top_n))]
         elif descriptors is not None:
             graph = self._graph_grp[None if top_n is None else max(top_n)]

@@ -12,6 +12,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200
 
 from .batch import greedy_tokens
+from .json_mode import ConstraintRows
 from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, _host_rows, entries_from_host, token_logprobs
 from .lora import adapter_ids_of
@@ -67,7 +68,7 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
                 if sampling.penalized and state is None:
                     state = token_state_row(prompt, [], logits.shape[-1], device=logits.device)[None]
                 if sampling.constraint is not None and constraints is None:
-                    constraints = sampling.constraint.descriptor()[None]
+                    constraints = ConstraintRows.build([sampling], logits.shape[-1], logits.device)
                 token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state, constraints)
             elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])
@@ -871,8 +872,7 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
             if penalized:
                 st = torch.stack([token_state_row(torch.as_tensor(prompt), [], rows.shape[-1], device=rows.device)] * n)
             if constrained:
-                con = torch.stack([params[i * n + j].constraint.descriptor() if params[i * n + j].constraint is not None
-                                   else torch.zeros(5, dtype=torch.int64) for j in range(n)]).to(rows.device)
+                con = ConstraintRows.build(params[i * n : i * n + n], rows.shape[-1], rows.device)
             tok = sample_tokens(rows, params[i * n : i * n + n], [len(prompt)] * n, st, con)
             ent = token_logprobs(rows, tok, logprobs) if logprobs is not None else [None] * n
             firsts.append((tok.tolist(), ent, st, con))
@@ -885,7 +885,7 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
                 take(i * n + j, tok[j], ent[j])
         if not graph:
             state = torch.cat([f[2] for f in firsts]) if penalized else None
-            constraints = torch.cat([f[3] for f in firsts]) if constrained else None
+            constraints = ConstraintRows.concat([f[3] for f in firsts]) if constrained else None
         offsets = [len(prompts[b // n]) for b in range(P * n)]
         batch = [BatchingKvCache(P * n) for _ in range(len(slots[0]))]
         for layer, slot in enumerate(batch):

@@ -53,7 +53,8 @@ class SamplingParams:
 
     ``constraint`` (a ``TokenConstraint``, ``tl_sample_constrained``, DESIGN.md section 8c) restricts every draw to the
     tokens that keep the text a prefix of the pattern's language (EOS once it is a match); greedy under a constraint is
-    ``SamplingParams(0.0, constraint=c)``.  With a mask that allows every token the draw is the unconstrained one."""
+    ``SamplingParams(0.0, constraint=c)``.  With a mask that allows every token the draw is the unconstrained one.
+    A ``JsonConstraint`` (JSON mode, DESIGN.md section 20) restricts the text to one JSON object the same way."""
 
     temperature: float
     top_k: int | None = None
@@ -94,8 +95,9 @@ class SamplingParams:
             raise ValueError(f"min_p must be a number in [0, 1], got {m!r}")
         if self.constraint is not None:
             from .constrained import TokenConstraint
+            from .json_mode import JsonConstraint
 
-            if not isinstance(self.constraint, TokenConstraint):
+            if not isinstance(self.constraint, (TokenConstraint, JsonConstraint)):
                 raise ValueError(f"constraint must be None or a TokenConstraint, got {type(self.constraint).__name__}")
 
     @property
@@ -177,7 +179,9 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
     When a row is penalised the launch is ``tl_sample_penalized`` over ``state`` (int32 ``[rows, vocab]``, required
     then), which it updates at the drawn tokens of the rows with position > 0.  When a row carries a constraint the
     launch is ``tl_sample_constrained`` over ``constraints`` (int64 ``[rows, 5]`` descriptor rows, required then: the
-    constrained rows' ``TokenConstraint.descriptor``, zero rows elsewhere), whose states it advances likewise."""
+    constrained rows' ``TokenConstraint.descriptor``, zero rows elsewhere), whose states it advances likewise.
+    ``constraints`` may also be a ``ConstraintRows`` (required for JSON rows): its JSON rows' masks are written before
+    the draw and their states advanced after it."""
     from extensions_b200 import tiny_llm_ext_b200 as ext
 
     temperature, top_k, top_p, seed = sampling_tensors(params, logits.device)
@@ -193,7 +197,16 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
             if state is None:
                 raise ValueError("a penalised SamplingParams needs the request's token state")
             pen = (*penalty_tensors(params, logits.device), state)
-        return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
+        from .json_mode import ConstraintRows, JsonConstraint
+
+        if not isinstance(constraints, ConstraintRows):
+            if any(p is not None and isinstance(p.constraint, JsonConstraint) for p in params):
+                raise ValueError("a JSON-mode SamplingParams needs the request's ConstraintRows")
+            return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
+        constraints.before_draw(len(params))
+        tokens = ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints.descriptors[:len(params)], *pen)
+        constraints.after_draw(tokens, pos)
+        return tokens
     if not any_penalized(params):
         return ext.sample(logits.contiguous(), temperature, top_k, top_p, seed, pos)
     if state is None:

@@ -4,8 +4,10 @@
   launch (CUDA events, median of 20);
 * ``tl_sample_constrained`` (every row masked, bf16 logits, temperature 0.7, top-p 0.9, top-k 50) against ``tl_sample``
   on the same rows, at 1, 8 and 64 rows (CUDA events over 200 launches);
-* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+``, at B = 1 and B = 8 on Qwen3-4B-shaped
-  synthetic weights, context 128 + steps, alternated in one process.
+* JSON mode's ``tl_json_token_masks`` per call at 1, 8 and 64 rows, every row inside a string value (nearly every
+  token walks its whole length) and every row at a value position (most tokens fail on their first byte);
+* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+`` and under JSON mode, at B = 1 and B = 8 on
+  Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
 
   python tools/constrained_bench.py [--out tools_out/constrained_bench.json]
 """
@@ -28,6 +30,7 @@ from sample_bench import card, timed  # noqa: E402
 from tiny_llm_b200 import BatchingKvCache, Qwen3ModelWeek3, SamplingParams  # noqa: E402
 from tiny_llm_b200.constrained import TokenConstraint, TokenVocabulary, compile_dfa  # noqa: E402
 from tiny_llm_b200.engine import DecodeEngine  # noqa: E402
+from tiny_llm_b200.json_mode import ConstraintRows, JsonConstraint, JsonWalker  # noqa: E402
 from tiny_llm_b200.sampler import sampling_tensors  # noqa: E402
 from tiny_llm_b200.synthetic import synthetic_qwen3  # noqa: E402
 
@@ -83,8 +86,27 @@ def kernel_table(c) -> dict:
     return out
 
 
-def decode_rates(model, c, B, ctx=128, steps=64, rounds=3) -> dict:
-    msl = ctx + 2 * (rounds + 1) * steps + 64
+def json_mask_table(jc) -> dict:
+    out = {}
+    for rows in (1, 8, 64):
+        res = {}
+        for where, text in (("in_string", b'{"name": "abc'), ("at_value", b'{"name": ')):
+            w = JsonWalker()
+            w.walk(text)
+            tab = ConstraintRows(rows, V, DEV, json=True)
+            for r in range(rows):
+                tab.set_row(r, jc, w)
+            res[where] = timed(lambda: ext.json_token_masks(tab.descriptors, tab.json_states, V))
+        out[rows] = res
+        print(f"json masks, rows {rows}: " + ", ".join(f"{k} {v:.1f} us" for k, v in res.items()), flush=True)
+    return out
+
+
+def decode_rates(model, c, jc, B, ctx=128, steps=64, rounds=3) -> dict:
+    modes = {"sampled": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1),
+             "constrained": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=c),
+             "json": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=jc)}
+    msl = ctx + len(modes) * (rounds + 1) * steps + 64
     engine = DecodeEngine(model, B, msl, DEV)
     engine.reserve_pools()
     tables = [BatchingKvCache(max_active_requests=B, max_seq_len=msl) for _ in range(model.num_hidden_layers)]
@@ -93,8 +115,6 @@ def decode_rates(model, c, B, ctx=128, steps=64, rounds=3) -> dict:
         for cc, t in zip(cache, tables):
             cc.append_slots(ctx)
             t.add_request(cc, b)
-    modes = {"sampled": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1),
-             "constrained": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=c)}
     offsets, tokens = [ctx] * B, [1] * B
     times = {m: [] for m in modes}
     for r in range(rounds + 1):
@@ -109,13 +129,16 @@ def decode_rates(model, c, B, ctx=128, steps=64, rounds=3) -> dict:
             if r:  # round 0 captures the graphs
                 times[mode].append(a.elapsed_time(b))
     res = {m: B * steps * len(v) / (sum(v) / 1e3) for m, v in times.items()}
-    res["kernels_per_step"] = {"sampled": engine.kernels_per_sampled_step, "constrained": engine.kernels_per_constrained_step}
+    res["kernels_per_step"] = {"sampled": engine.kernels_per_sampled_step, "constrained": engine.kernels_per_constrained_step,
+                               "json": engine.kernels_per_json_step}
     for t in tables:  # the next engine reserves its pages from the same pools
         for cc in t.kv_caches:
             if cc is not None:
                 cc.release()
     print(f"B {B}: sampled {res['sampled']:.1f} tok/s, constrained {res['constrained']:.1f} tok/s "
-          f"({(res['constrained'] / res['sampled'] - 1) * 100:+.2f} %)", flush=True)
+          f"({(res['constrained'] / res['sampled'] - 1) * 100:+.2f} %), json {res['json']:.1f} tok/s "
+          f"({(res['json'] / res['sampled'] - 1) * 100:+.2f} % against sampled, {(res['json'] / res['constrained'] - 1) * 100:+.2f} % "
+          "against [a-z ]+)", flush=True)
     return res
 
 
@@ -131,9 +154,11 @@ def main() -> None:
     result["compile"] = compile_table(vocab)
     c = TokenConstraint.compile(PATTERNS["words"], vocab, device=DEV)
     result["kernels_us"] = kernel_table(c)
+    jc = JsonConstraint(vocab, device=DEV)
+    result["json_masks_us"] = json_mask_table(jc)
     ns = synthetic_qwen3("qwen3-4b", seed=0, device=DEV)
     model = Qwen3ModelWeek3(ns, page_size=64)
-    result["decode"] = {B: decode_rates(model, c, B) for B in (1, 8)}
+    result["decode"] = {B: decode_rates(model, c, jc, B) for B in (1, 8)}
     if args.out:
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
         Path(args.out).write_text(json.dumps(result, indent=1))
