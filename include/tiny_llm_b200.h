@@ -389,6 +389,44 @@ int tl_json_token_masks(const tl_constraint_row *constraints, const int64_t *jso
  * bytes, or terminal when the token has no bytes (EOS).  Other rows are unchanged. */
 int tl_json_advance(const tl_constraint_row *constraints, int64_t *json_states, const int32_t *tokens, const int32_t *positions, int rows,
                     void *stream);
+/* JSON Schema structured outputs (DESIGN.md section 21): a byte-level pushdown automaton compiled from a schema into
+ * one table blob per schema (json_schema.py writes it; 16-byte aligned):
+ *   int32 num_states S, num_classes C, blob bytes, num_actions A;  uint8 class_of[256];
+ *   uint32 info[S]      bit 0 whitespace counts here, bit 1 accepting, bits 8-15 need (stack entries the cheapest
+ *                       completion from the state still pushes);
+ *   uint32 actions[A]   bits 0-1 kind (0 checked shift, 1 call, 2 return, 3 return and reprocess the byte), 2-16
+ *                       target, 17-31 return;
+ *   uint16 trans[S, C]  0 fail, 1-0x7FFF a plain shift to that state (its need is at most the source's, so the depth
+ *                       cap holds unchecked), 0x8000 | a action a.
+ * State 0 is dead.  A schema row is a tl_constraint_row exactly like a JSON row (num_states 1, its own uint32
+ * [2, ceil(vocab / 32)] mask buffer, the all-zero dfa).  Its automaton state is TL_SCHEMA_STATE_WORDS int64 words:
+ *   word 0         the row's table blob (0: not a schema row);
+ *   word 1         bits 0-14 state, 16-21 depth (stack entries), 24-29 current whitespace run, 32 the row is in schema
+ *                  mode, 33 terminal (after EOS);
+ *   words 2-9      the stack of return states, 16 bits each, entry k at word 2 + k / 4, bits 16 (k % 4); entries at
+ *                  or above the depth are 0.
+ * A byte in a state: look up the entry; a reprocess entry pops the return state and looks the byte up there.  In a
+ * whitespace state the run grows on whitespace (at most TL_JSON_MAX_WS_RUN); any other byte resets it.  A checked
+ * shift to t needs depth + need(t) <= TL_SCHEMA_MAX_DEPTH, a call (t, r) depth + 1 + need(t) and depth + need(r)
+ * within it. */
+#define TL_SCHEMA_MAX_DEPTH 32
+#define TL_SCHEMA_MAX_ITEMS 64
+#define TL_SCHEMA_MAX_STATES 32767
+#define TL_SCHEMA_MAX_TABLE_BYTES (1 << 22)
+#define TL_SCHEMA_SMEM_BYTES (47 * 1024)
+#define TL_SCHEMA_STATE_WORDS 10
+/* Row 0 of every schema row's mask (rows with bit 32 of word 1 set and bit 33 clear; others are not touched), in one
+ * launch: bit t iff token t has bytes and walking them from the row's state stays in the language, or t has no bytes,
+ * the text is complete (accepting state, depth 0) and bit t of the row's mask row 1 is set.  smem_bytes (a multiple of
+ * 16, at most TL_SCHEMA_SMEM_BYTES) is the dynamic shared memory of each CTA: a row's blob is staged there when it
+ * fits and read through L1/L2 otherwise, with the same result (size it to the largest blob that fits, or 0).
+ * Deterministic, no atomics. */
+int tl_schema_token_masks(const tl_constraint_row *constraints, const int64_t *schema_states, int rows, int vocab, int smem_bytes,
+                          void *stream);
+/* After the draw: for schema rows with positions[r] > 0 and not terminal, the state becomes the walk of tokens[r]'s
+ * bytes (the dead state when it leaves the language), or terminal when the token has no bytes (EOS). */
+int tl_schema_advance(const tl_constraint_row *constraints, int64_t *schema_states, const int32_t *tokens, const int32_t *positions,
+                      int rows, void *stream);
 /* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
  * launch, one cluster of CTAs per row (DESIGN.md section 8a).
  *

@@ -41,6 +41,7 @@ SOURCES = [
     "logprobs.cu",
     "constrained.cu",
     "json.cu",
+    "json_schema.cu",
     "moe.cu",
     "moe_router.cu",
     "lora.cu",

@@ -651,6 +651,21 @@ int tl_json_advance(const tl_constraint_row *constraints, int64_t *json_states, 
     return launch_json_advance(constraints, json_states, tokens, positions, rows, as_stream(stream));
 }
 
+int tl_schema_token_masks(const tl_constraint_row *constraints, const int64_t *schema_states, int rows, int vocab, int smem_bytes,
+                          void *stream) {
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "schema_token_masks: bad shape");
+    if (smem_bytes < 0 || smem_bytes > TL_SCHEMA_SMEM_BYTES || smem_bytes % 16) return fail(TL_EINVAL, "schema_token_masks: bad smem_bytes");
+    if (rows > 0 && (!constraints || !schema_states)) return fail(TL_EINVAL, "schema_token_masks: null pointer");
+    return launch_schema_token_masks(constraints, schema_states, rows, vocab, smem_bytes, as_stream(stream));
+}
+
+int tl_schema_advance(const tl_constraint_row *constraints, int64_t *schema_states, const int32_t *tokens, const int32_t *positions,
+                      int rows, void *stream) {
+    if (rows < 0) return fail(TL_EINVAL, "schema_advance: bad shape");
+    if (rows > 0 && (!constraints || !schema_states || !tokens || !positions)) return fail(TL_EINVAL, "schema_advance: null pointer");
+    return launch_schema_advance(constraints, schema_states, tokens, positions, rows, as_stream(stream));
+}
+
 int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,
                 int32_t *target_rank, int32_t *top_ids, float *top_lp, int rows, int vocab, int max_n, int out_capacity, int dtype,
                 void *stream) {

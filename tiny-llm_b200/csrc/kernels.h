@@ -57,6 +57,11 @@ int launch_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int
 int launch_json_token_masks(const tl_constraint_row *constraints, const int64_t *states, int rows, int vocab, cudaStream_t st);
 int launch_json_advance(const tl_constraint_row *constraints, int64_t *states, const int32_t *tokens, const int32_t *positions, int rows,
                         cudaStream_t st);
+// json_schema.cu
+int launch_schema_token_masks(const tl_constraint_row *constraints, const int64_t *states, int rows, int vocab, int smem_bytes,
+                              cudaStream_t st);
+int launch_schema_advance(const tl_constraint_row *constraints, int64_t *states, const int32_t *tokens, const int32_t *positions,
+                          int rows, cudaStream_t st);
 // logprobs.cu: same cluster plan as sampling.cu
 constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
 int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,

@@ -62,6 +62,9 @@ __all__ = [
     "json_token_masks",
     "json_advance",
     "JSON_STATE_WORDS",
+    "schema_token_masks",
+    "schema_advance",
+    "SCHEMA_STATE_WORDS",
     "logprobs",
     "LOGPROBS_MAX_N",
     "decode_advance",
@@ -146,6 +149,8 @@ _SIGNATURES = {
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
     "tl_json_token_masks": (_I, [_VP, _VP, _I, _I, _VP]),
     "tl_json_advance": (_I, [_VP] * 4 + [_I, _VP]),
+    "tl_schema_token_masks": (_I, [_VP, _VP, _I, _I, _I, _VP]),
+    "tl_schema_advance": (_I, [_VP] * 4 + [_I, _VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_qkv_project_rope_append_table": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP, _VP]),
@@ -1063,6 +1068,49 @@ def json_advance(constraints, json_states, tokens, positions, stream=None):
     _gpu("json_advance", *named.values())
     _check(_lib.tl_json_advance(constraints.data_ptr(), json_states.data_ptr(), tokens.data_ptr(), positions.data_ptr(), rows,
                                 _stream_ptr(stream, constraints)))
+
+
+SCHEMA_STATE_WORDS = 10  # int64 words of one JSON Schema row's automaton state (include/tiny_llm_b200.h)
+SCHEMA_SMEM_BYTES = 47 * 1024  # TL_SCHEMA_SMEM_BYTES: the largest table blob a masks launch stages in shared memory
+
+
+def _schema_rows(op, constraints, schema_states):
+    if constraints.dtype != torch.int64 or constraints.dim() != 2 or constraints.shape[1] != CONSTRAINT_ROW_WORDS:
+        raise RuntimeError(f"{op}: constraints must be int64 [rows, {CONSTRAINT_ROW_WORDS}]")
+    rows = constraints.shape[0]
+    if schema_states.dtype != torch.int64 or tuple(schema_states.shape) != (rows, SCHEMA_STATE_WORDS):
+        raise RuntimeError(f"{op}: schema_states must be int64 [{rows}, {SCHEMA_STATE_WORDS}]")
+    return rows
+
+
+def schema_token_masks(constraints, schema_states, vocab, smem_bytes=0, stream=None):
+    """Row 0 of each JSON Schema row's mask buffer (``tl_schema_token_masks``): ``constraints`` int64 ``[rows, 5]``
+    descriptors, ``schema_states`` int64 ``[rows, 10]`` automaton states (word 0 the row's table blob); rows not in
+    schema mode, or terminal, are not touched.  ``smem_bytes``: the shared memory that stages blobs up to that size
+    (``ConstraintRows.schema_smem_bytes``).  Writes through the descriptors' mask pointers; returns nothing."""
+    rows = _schema_rows("schema_token_masks", constraints, schema_states)
+    if isinstance(vocab, bool) or not isinstance(vocab, int) or vocab <= 0:
+        raise RuntimeError("schema_token_masks: vocab must be a positive int")
+    if isinstance(smem_bytes, bool) or not isinstance(smem_bytes, int) or not 0 <= smem_bytes <= SCHEMA_SMEM_BYTES or smem_bytes % 16:
+        raise RuntimeError(f"schema_token_masks: smem_bytes must be a multiple of 16 in [0, {SCHEMA_SMEM_BYTES}]")
+    _contig("schema_token_masks", constraints=constraints, schema_states=schema_states)
+    _gpu("schema_token_masks", constraints, schema_states)
+    _check(_lib.tl_schema_token_masks(constraints.data_ptr(), schema_states.data_ptr(), rows, vocab, smem_bytes,
+                                      _stream_ptr(stream, constraints)))
+
+
+def schema_advance(constraints, schema_states, tokens, positions, stream=None):
+    """Advance each JSON Schema row's automaton state by its drawn token (``tl_schema_advance``), for rows with
+    ``positions > 0``; ``tokens`` and ``positions`` int32 ``[rows]``."""
+    rows = _schema_rows("schema_advance", constraints, schema_states)
+    for name, t in (("tokens", tokens), ("positions", positions)):
+        if t.dtype != torch.int32 or tuple(t.shape) != (rows,):
+            raise RuntimeError(f"schema_advance: {name} must be int32 [{rows}]")
+    named = dict(constraints=constraints, schema_states=schema_states, tokens=tokens, positions=positions)
+    _contig("schema_advance", **named)
+    _gpu("schema_advance", *named.values())
+    _check(_lib.tl_schema_advance(constraints.data_ptr(), schema_states.data_ptr(), tokens.data_ptr(), positions.data_ptr(), rows,
+                                  _stream_ptr(stream, constraints)))
 
 
 def constraint_token_masks(dfa, accept, token_offsets, token_bytes, eos_ids, stream=None):

@@ -350,7 +350,7 @@ class ContinuousBatcher:
             if request.constraint_row is None:
                 return
             src = request.constraint_row
-            self.constraint_rows = ConstraintRows(self.batch_size, src.vocab, src.device, src.has_json)
+            self.constraint_rows = ConstraintRows(self.batch_size, src.vocab, src.device, src.has_json, src.has_schema)
         if request.constraint_row is None:
             self.constraint_rows.clear_row(slot)
         else:

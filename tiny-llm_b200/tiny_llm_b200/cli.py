@@ -31,6 +31,9 @@ see checkpoint.py; there is no hub download here).
         (every generated token keeps the text inside the pattern's language; EOS ends it once it is a match)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --json
         (the generated text is one JSON object: every prefix can still complete, EOS only once it has closed)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 \
+        --json-schema '{"type": "object", "properties": {"name": {"type": "string"}}, "required": ["name"]}'
+        (one JSON object that validates against the schema, keys in the schema's order; FILE_OR_INLINE_JSON)
     python -m tiny_llm_b200.cli batch --synthetic tiny-d128 --synthetic-lora a=16 --synthetic-lora b=8:1 \
         --prompt-ids "5,17,3;5,17,3;5,17,3" --adapters "a;;b"
         (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
@@ -171,16 +174,28 @@ def _penalties(args) -> dict:
 
 
 def _constraint(args, model, tokenizer, device):
-    """The ``TokenConstraint`` of ``--regex`` or the ``JsonConstraint`` of ``--json`` over the checkpoint tokenizer's
-    vocabulary (the synthetic vocabulary with ``--synthetic``), or None."""
+    """The ``TokenConstraint`` of ``--regex``, the ``JsonConstraint`` of ``--json`` or the ``JsonSchemaConstraint`` of
+    ``--json-schema`` over the checkpoint tokenizer's vocabulary (the synthetic vocabulary with ``--synthetic``), or
+    None."""
+    schema_text = args.json_schema
+    given = [f for f, on in (("--regex", args.regex is not None), ("--json", args.json), ("--json-schema", schema_text is not None)) if on]
     if args.regex is not None and args.json:
         raise SystemExit("give --regex or --json, not both")
-    if args.regex is None and not args.json:
+    if len(given) > 1:
+        raise SystemExit(f"give one of {', '.join(given)}, not several")
+    if not given:
         return None
     from .constrained import TokenConstraint, TokenVocabulary
     from .json_mode import JsonConstraint
+    from .json_schema import JsonSchemaConstraint, load_schema_arg
 
-    flag = "--regex" if args.regex is not None else "--json"
+    flag = given[0]
+    schema = None
+    if schema_text is not None:
+        try:
+            schema = load_schema_arg(schema_text)
+        except (OSError, ValueError) as exc:
+            raise SystemExit(f"--json-schema: not a JSON schema file or inline JSON object: {exc}")
     if device.type != "cuda":
         raise SystemExit(f"{flag} runs on the CUDA sampling kernel: use a cuda --device")
     if args.synthetic:
@@ -192,6 +207,8 @@ def _constraint(args, model, tokenizer, device):
     try:
         if args.json:
             return JsonConstraint(vocabulary, device=device)
+        if schema is not None:
+            return JsonSchemaConstraint(schema, vocabulary, device=device)
         return TokenConstraint.compile(args.regex, vocabulary, device=device)
     except ValueError as exc:
         raise SystemExit(f"{flag}: {exc}")
@@ -227,6 +244,8 @@ def cmd_generate(args) -> int:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --regex")
     if speculative and args.json:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --json")
+    if speculative and args.json_schema is not None:
+        raise SystemExit("speculative decoding is greedy and unconstrained: drop --json-schema")
     constraint = _constraint(args, model, tokenizer, device)
     if constraint is not None:
         penalties["constraint"] = constraint
@@ -339,7 +358,8 @@ def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
     from .generate import beam_search_ids
 
     refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("penalties or --min-p", bool(penalties)),
-               ("--regex", args.regex is not None), ("--json", args.json), ("--logprobs", args.logprobs is not None),
+               ("--regex", args.regex is not None), ("--json", args.json),
+               ("--json-schema", args.json_schema is not None), ("--logprobs", args.logprobs is not None),
                ("adapters", args.adapter is not None or getattr(model, "adapters", None) is not None),
                ("a draft", bool(args.draft_model or args.draft_synthetic)), ("--prompt-lookup", args.prompt_lookup is not None)]
     for what, given in refused:
@@ -578,6 +598,9 @@ def main(argv=None) -> int:
                                        help="constrain the generated text to fullmatch PATTERN (re.ASCII semantics over UTF-8 bytes)")
         sub.choices[name].add_argument("--json", action="store_true",
                                        help="constrain the generated text to one JSON object (RFC 8259; depth <= 64, whitespace runs <= 32)")
+        sub.choices[name].add_argument("--json-schema", default=None, metavar="FILE_OR_INLINE_JSON",
+                                       help="constrain the generated text to one JSON object that validates against this JSON Schema "
+                                            "(keys in the schema's order; DESIGN.md section 21 lists the keywords)")
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")

@@ -38,6 +38,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200 as ext
 
 from .json_mode import ConstraintRows, JsonConstraint
+from .json_schema import JsonSchemaConstraint
 from .kv_cache import BatchingKvCache
 from .moe import Moe, router_logits
 from .paged_kv_cache import TinyKvPagedCache
@@ -444,6 +445,13 @@ class DecodeEngine(_GraphEngine):
         self.kernels_per_json_step = 0
         self._json_tab = None
         self._json_key = None
+        # decode_on_device(sampling=<with a JSON Schema slot>): one graph per (penalised, logprobs N or None, any JSON
+        # slot), the constrained step between the schema (and JSON) rows' masks and their advances over a B-row
+        # ConstraintRows of its own; all on first use
+        self._graph_schema: dict = {}
+        self.kernels_per_schema_step = 0
+        self._schema_tab = None
+        self._schema_key = None
         # decode_on_device(sampling=..., keep_logits=True): the sampled step plus one tl_log_rows launch that keeps the
         # step's logits rows in a [capacity, B, V] log at the step counter (a speculative draft's q rows); on first use
         self._graph_keep = None
@@ -493,7 +501,9 @@ class DecodeEngine(_GraphEngine):
         over ``token_counts``, or (a constrained graph) ``tl_sample_constrained`` over the slot descriptors, or (the
         sampled verify graph, ``spec_draft`` the draft's logits rows) ``tl_speculative_sample`` on the proposals.
         ``constrained == "json"`` (the JSON graph) draws over the JSON table's descriptors, between the JSON rows' mask
-        launch and their state advance."""
+        launch and their state advance; ``constrained == "schema"`` (the schema graph) likewise over the schema table,
+        with the schema rows' launches (and the JSON rows' when the table holds any); the masks launch stages the tables
+        in the shared memory the table held at capture."""
         if spec_draft is not None:
             ext.speculative_sample(logits, spec_draft, self.tokens[1:R], *self._spec_params, self.context_lens[:R], out=self.next_tokens[:R])
             return
@@ -502,14 +512,18 @@ class DecodeEngine(_GraphEngine):
             if penalized:
                 p = self._pen_dev.view(torch.float32).view(4, self.B)
                 pen = (p[0, :R], p[1, :R], p[2, :R], p[3, :R], self.token_counts[:R])
-            tab = self._json_tab if constrained == "json" else None
-            if tab is not None:
+            tab = self._json_tab if constrained == "json" else self._schema_tab if constrained == "schema" else None
+            if tab is not None and tab.has_json:
                 ext.json_token_masks(tab.descriptors[:R], tab.json_states[:R], self.V)
+            if tab is not None and tab.has_schema:
+                ext.schema_token_masks(tab.descriptors[:R], tab.schema_states[:R], self.V, tab.schema_smem_bytes)
             descriptors = self._con_dev.view(self.B, -1)[:R] if tab is None else tab.descriptors[:R]
             tokens = ext.sample_constrained(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
                                             self.context_lens[:R], descriptors, *pen)
-            if tab is not None:
+            if tab is not None and tab.has_json:
                 ext.json_advance(tab.descriptors[:R], tab.json_states[:R], tokens, self.context_lens[:R])
+            if tab is not None and tab.has_schema:
+                ext.schema_advance(tab.descriptors[:R], tab.schema_states[:R], tokens, self.context_lens[:R])
         elif penalized:
             pen = self._pen_dev.view(torch.float32).view(4, self.B)
             tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
@@ -690,6 +704,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_lp = {}
         self._graph_con = {}
         self._graph_json = {}
+        self._graph_schema = {}
         self._graph_keep = None
         self._graph_spec = {}
         self._graph_beam = {}
@@ -879,6 +894,7 @@ class DecodeEngine(_GraphEngine):
             self._graph_lp = {}
             self._graph_con = {k: g for k, g in self._graph_con.items() if k[1] is None}
             self._graph_json = {k: g for k, g in self._graph_json.items() if k[1] is None}
+            self._graph_schema = {k: g for k, g in self._graph_schema.items() if k[1] is None}
             self._lp_max_n = max_n
             self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
                             torch.zeros((cap, B), dtype=torch.int32, device=dev), torch.zeros((cap, B, max_n), dtype=torch.int32, device=dev),
@@ -931,7 +947,29 @@ class DecodeEngine(_GraphEngine):
             self.kernels_per_json_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
-    def _set_json_constraints(self, per: list, history) -> None:
+    def _ensure_schema_graph(self, penalized: bool, max_n: int | None, json: bool) -> None:
+        """Capture the JSON Schema step: the constrained step with the schema rows' masks before the draw and their
+        advance after it, and the JSON rows' too when ``json`` (the warm-up runs at context 0, so it advances no
+        state).  One graph per (penalized, max_n, json)."""
+        if (penalized, max_n, json) in self._graph_schema:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def schema_step():
+            forward(sampled=True, penalized=penalized, constrained="schema")
+            if max_n is not None:
+                ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()
+            self._graph_schema[(penalized, max_n, json)] = self._graph_of(schema_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_schema_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_json_constraints(self, per: list, history, schema: bool = False) -> None:
         """The JSON table's rows for the slots' constraints (JSON, regex or none), as ``_set_constraints`` sets the
         descriptors: a slot with a ``history`` entry starts from the host walk of its generated ids (refused when they
         leave the language), a slot with a new constraint from the start state, and every other constrained slot
@@ -948,18 +986,23 @@ class DecodeEngine(_GraphEngine):
         for b, c in enumerate(cons):
             if c is None or history is None or history[b] is None:
                 continue
-            state = c.walk(history[b][1]) if isinstance(c, JsonConstraint) else c.walk(c.start_state, history[b][1])
-            if state is None or (not isinstance(c, JsonConstraint) and state < 0):
+            rows = isinstance(c, (JsonConstraint, JsonSchemaConstraint))
+            state = c.walk(history[b][1]) if rows else c.walk(c.start_state, history[b][1])
+            if state is None or (not rows and state < 0):
                 raise ValueError(f"slot {b}: its generated ids leave the constraint's language")
             walked[b] = state
         key = tuple(cons)
-        if self._json_key is not None and all(x is y for x, y in zip(key, self._json_key)) and not walked:
+        tab, old = (self._schema_tab, self._schema_key) if schema else (self._json_tab, self._json_key)
+        if old is not None and all(x is y for x, y in zip(key, old)) and not walked:
             return
         torch.cuda.current_stream(self.device).wait_stream(self._stream)  # the previous call's replays read the table
         for b, c in enumerate(cons):
-            if b in walked or self._json_key is None or self._json_key[b] is not c or c is None:
-                self._json_tab.set_row(b, c, walked.get(b))
-        self._json_key = key
+            if b in walked or old is None or old[b] is not c or c is None:
+                tab.set_row(b, c, walked.get(b))
+        if schema:
+            self._schema_key = key
+        else:
+            self._json_key = key
 
     def _set_constraints(self, per: list, history) -> None:
         """Upload the slot descriptors when the slots' constraints change or ``history`` is given.  A slot whose
@@ -1269,7 +1312,8 @@ class DecodeEngine(_GraphEngine):
         states.  ``history`` also sets a constrained slot's state to the walk of its generated ids; without it a slot
         keeps its state while its constraint stays the same and starts at the start state otherwise.  With a JSON-mode
         slot (``JsonConstraint``) the step is a graph of its own: the JSON rows' masks, the constrained draw and their
-        state advance, with the same rules for ``history``.
+        state advance, with the same rules for ``history``.  With a JSON Schema slot (``JsonSchemaConstraint``) the
+        step is the schema graph kind, which runs the schema rows' (and any JSON rows') masks and advances.
         ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above.
         ``keep_logits=True`` (plain ``sampling``: no penalty, constraint or logprobs) replays the sampled step with one
         more launch that keeps each step's logits rows, and returns ``(tokens, logits [steps, B, V])``, a device view of
@@ -1319,7 +1363,18 @@ class DecodeEngine(_GraphEngine):
         if penalized:
             self._alloc_penalties()
         json = constrained and any(isinstance(p.constraint, JsonConstraint) for p in per if p is not None)
-        if json:
+        schema = constrained and any(isinstance(p.constraint, JsonSchemaConstraint) for p in per if p is not None)
+        if schema:
+            if self._schema_tab is None:
+                self._schema_tab = ConstraintRows(B, self.V, self.device, json=json, schema=True)
+            if json:
+                self._schema_tab.ensure_json()
+            if top_n is not None:
+                self._alloc_logprobs(max(top_n))
+                self._set_top_n(top_n)
+            self._set_json_constraints(self._per_slot_sampling(sampling), history, schema=True)
+            self._ensure_schema_graph(penalized, None if top_n is None else max(top_n), self._schema_tab.has_json)
+        elif json:
             if self._json_tab is None:
                 self._json_tab = ConstraintRows(B, self.V, self.device, json=True)
             if top_n is not None:
@@ -1355,14 +1410,18 @@ class DecodeEngine(_GraphEngine):
             self._set_sampling(sampling)
         if penalized:
             self._set_penalties(self._per_slot_sampling(sampling), history)
-        if json:
+        if schema:
+            pass  # the schema table's rows are set above, before its graph is captured, which sizes its masks launch
+        elif json:
             self._set_json_constraints(self._per_slot_sampling(sampling), history)
         elif constrained:
             self._set_constraints(self._per_slot_sampling(sampling), history)
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
-        if json:
+        if schema:
+            graph = self._graph_schema[(penalized, None if top_n is None else max(top_n), self._schema_tab.has_json)]
+        elif json:
             graph = self._graph_json[(penalized, None if top_n is None else max(top_n))]
         elif constrained:
             graph = self._graph_con[(penalized, None if top_n is None else max(top_n))]

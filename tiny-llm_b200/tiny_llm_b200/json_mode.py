@@ -358,26 +358,32 @@ class JsonConstraint:
 
 # -------------------------------------------------------------------------------------------- per-row tables --
 class ConstraintRows:
-    """The constraint tables of one draw's rows, for any mix of regex, JSON and unconstrained ``SamplingParams``:
-    ``descriptors`` int64 ``[R, 5]`` ``tl_constraint_row``s and, when a row is in JSON mode, ``json_states`` int64
-    ``[R, 2]`` (zero rows: not JSON) and ``json_masks`` int32 ``[R, 2, ceil(V / 32)]`` (row 0 this step's mask, row
-    1 EOS only).  ``sample`` runs the masks launch, ``tl_sample_constrained`` and the advance; regex rows advance inside
-    the draw as before."""
+    """The constraint tables of one draw's rows, for any mix of regex, JSON, JSON Schema and unconstrained
+    ``SamplingParams``: ``descriptors`` int64 ``[R, 5]`` ``tl_constraint_row``s and, when a row is in JSON mode,
+    ``json_states`` int64 ``[R, 2]`` (zero rows: not JSON), when a row is under a ``JsonSchemaConstraint``,
+    ``schema_states`` int64 ``[R, 10]`` (zero rows: not a schema row), and for either ``json_masks`` int32
+    ``[R, 2, ceil(V / 32)]`` (row 0 this step's mask, row 1 EOS only).  ``sample`` runs the masks launches,
+    ``tl_sample_constrained`` and the advances; regex rows advance inside the draw as before."""
 
-    def __init__(self, rows: int, vocab: int, device, json: bool):
+    def __init__(self, rows: int, vocab: int, device, json: bool, schema: bool = False):
         self.rows, self.vocab, self.device = rows, vocab, torch.device(device)
         self.descriptors = torch.zeros((rows, 5), dtype=torch.int64, device=device)
-        self.json_states = self.json_masks = None
-        self._json_constraints: list = [None] * rows
+        self.json_states = self.json_masks = self.schema_states = None
+        self.schema_smem_bytes = 0  # shared memory of the schema masks launch: the largest schema blob that fits
+        self._json_constraints: list = [None] * rows  # the row's JsonConstraint or JsonSchemaConstraint
         if json:
-            self.json_states = torch.zeros((rows, STATE_WORDS), dtype=torch.int64, device=device)
-            self.json_masks = torch.zeros((rows, 2, (vocab + 31) // 32), dtype=torch.int32, device=device)
+            self.ensure_json()
+        if schema:
+            self.ensure_schema()
 
     @classmethod
     def build(cls, params, vocab: int, device) -> ConstraintRows:
         """Rows at their constraints' start states, one per entry of ``params`` (None: unconstrained)."""
+        from .json_schema import JsonSchemaConstraint
+
         cons = [None if p is None else p.constraint for p in params]
-        out = cls(len(cons), vocab, device, any(isinstance(c, JsonConstraint) for c in cons))
+        out = cls(len(cons), vocab, device, any(isinstance(c, JsonConstraint) for c in cons),
+                  any(isinstance(c, JsonSchemaConstraint) for c in cons))
         for r, c in enumerate(cons):
             out.set_row(r, c)
         return out
@@ -386,7 +392,7 @@ class ConstraintRows:
     def concat(cls, tables: list) -> ConstraintRows:
         """One table of the rows of ``tables`` in order (device copies of their states)."""
         t0 = tables[0]
-        out = cls(sum(t.rows for t in tables), t0.vocab, t0.device, any(t.has_json for t in tables))
+        out = cls(sum(t.rows for t in tables), t0.vocab, t0.device, any(t.has_json for t in tables), any(t.has_schema for t in tables))
         r = 0
         for t in tables:
             for s in range(t.rows):
@@ -398,44 +404,86 @@ class ConstraintRows:
     def has_json(self) -> bool:
         return self.json_states is not None
 
+    @property
+    def has_schema(self) -> bool:
+        return self.schema_states is not None
+
+    def _ensure_masks(self) -> None:
+        if self.json_masks is None:
+            self.json_masks = torch.zeros((self.rows, 2, (self.vocab + 31) // 32), dtype=torch.int32, device=self.device)
+
     def ensure_json(self) -> None:
         if self.json_states is None:
             self.json_states = torch.zeros((self.rows, STATE_WORDS), dtype=torch.int64, device=self.device)
-            self.json_masks = torch.zeros((self.rows, 2, (self.vocab + 31) // 32), dtype=torch.int32, device=self.device)
+            self._ensure_masks()
+
+    def ensure_schema(self) -> None:
+        from .json_schema import SCHEMA_STATE_WORDS
+
+        if self.schema_states is None:
+            self.schema_states = torch.zeros((self.rows, SCHEMA_STATE_WORDS), dtype=torch.int64, device=self.device)
+            self._ensure_masks()
+
+    def _zero_states(self, r: int, keep=None) -> None:
+        for states in (self.json_states, self.schema_states):
+            if states is not None and states is not keep:
+                states[r].zero_()
 
     def set_row(self, r: int, constraint, state=None) -> None:
-        """Row ``r`` under ``constraint`` (None: unconstrained) at ``state`` (a regex state, or a ``JsonWalker``;
-        default the start)."""
+        """Row ``r`` under ``constraint`` (None: unconstrained) at ``state`` (a regex state, a ``JsonWalker`` or a
+        ``SchemaWalker``; default the start)."""
         from .constrained import descriptor_values
+        from .json_schema import JsonSchemaConstraint
 
         if isinstance(constraint, JsonConstraint):
             self.ensure_json()
+            self._zero_states(r, keep=self.json_states)
             w = JsonWalker() if state is None else state
             self.json_masks[r, 1].copy_(constraint.eos_row)
             self.json_states[r].copy_(torch.tensor(w.words(), dtype=torch.int64))
             self.descriptors[r].copy_(torch.tensor(self._json_descriptor(r, constraint, 1 if w.terminal else 0), dtype=torch.int64))
+        elif isinstance(constraint, JsonSchemaConstraint):
+            self.ensure_schema()
+            self._zero_states(r, keep=self.schema_states)
+            w = constraint.start() if state is None else state
+            self.json_masks[r, 1].copy_(constraint.eos_row)
+            self.schema_states[r].copy_(torch.tensor(constraint.words(w), dtype=torch.int64))
+            self._fit_schema(constraint)
+            self.descriptors[r].copy_(torch.tensor(self._json_descriptor(r, constraint, 1 if w.terminal else 0), dtype=torch.int64))
         else:
-            if self.json_states is not None:
-                self.json_states[r].zero_()
+            self._zero_states(r)
             self.descriptors[r].copy_(torch.tensor(descriptor_values(constraint, 0 if state is None else state), dtype=torch.int64))
-        self._json_constraints[r] = constraint if isinstance(constraint, JsonConstraint) else None
+        self._json_constraints[r] = constraint if isinstance(constraint, (JsonConstraint, JsonSchemaConstraint)) else None
 
-    def _json_descriptor(self, r: int, c: JsonConstraint, state: int) -> list[int]:
+    def _fit_schema(self, c) -> None:
+        from .json_schema import SCHEMA_SMEM_BYTES
+
+        n = int(c.compiled.blob.size)
+        if n <= SCHEMA_SMEM_BYTES:
+            self.schema_smem_bytes = max(self.schema_smem_bytes, n)
+
+    def _json_descriptor(self, r: int, c, state: int) -> list[int]:
         packed = 1 | (state << 32)  # num_states 1, state 0 (or 1, terminal)
         return [self.json_masks[r].data_ptr(), c.dfa.data_ptr(), c.token_offsets.data_ptr(), c.token_bytes.data_ptr(), packed]
 
     def copy_row(self, r: int, src: ConstraintRows, s: int = 0) -> None:
-        """Row ``r`` takes row ``s`` of ``src`` (a device copy of its state; the descriptor is rebuilt for JSON rows,
-        whose mask pointer is per table)."""
+        """Row ``r`` takes row ``s`` of ``src`` (a device copy of its state; the descriptor is rebuilt for JSON and
+        schema rows, whose mask pointer is per table)."""
         c = src._json_constraints[s]
         if c is None:
-            if self.json_states is not None:
-                self.json_states[r].zero_()
+            self._zero_states(r)
             self.descriptors[r].copy_(src.descriptors[s])
             self._json_constraints[r] = None
             return
-        self.ensure_json()
-        self.json_states[r].copy_(src.json_states[s])
+        if isinstance(c, JsonConstraint):
+            self.ensure_json()
+            self._zero_states(r, keep=self.json_states)
+            self.json_states[r].copy_(src.json_states[s])
+        else:
+            self.ensure_schema()
+            self._zero_states(r, keep=self.schema_states)
+            self.schema_states[r].copy_(src.schema_states[s])
+            self._fit_schema(c)
         self.json_masks[r].copy_(src.json_masks[s])
         self.descriptors[r, :4].copy_(torch.tensor(self._json_descriptor(r, c, 0)[:4], dtype=torch.int64))
         self.descriptors[r, 4].copy_(src.descriptors[s, 4])  # num_states and the terminal flag
@@ -443,29 +491,41 @@ class ConstraintRows:
 
     def clear_row(self, r: int) -> None:
         self.descriptors[r].zero_()
-        if self.json_states is not None:
-            self.json_states[r].zero_()
+        self._zero_states(r)
         self._json_constraints[r] = None
 
     def before_draw(self, rows: int | None = None) -> None:
-        """This step's masks of the JSON rows among the first ``rows`` (default all)."""
+        """This step's masks of the JSON and schema rows among the first ``rows`` (default all)."""
         from extensions_b200 import tiny_llm_ext_b200 as ext
 
+        n = self.rows if rows is None else rows
         if self.json_states is not None:
-            n = self.rows if rows is None else rows
             ext.json_token_masks(self.descriptors[:n], self.json_states[:n], self.vocab)
+        if self.schema_states is not None:
+            ext.schema_token_masks(self.descriptors[:n], self.schema_states[:n], self.vocab, self.schema_smem_bytes)
 
     def after_draw(self, tokens: torch.Tensor, positions: torch.Tensor) -> None:
-        """Advance the JSON rows by their drawn ``tokens`` (rows with ``positions > 0``)."""
+        """Advance the JSON and schema rows by their drawn ``tokens`` (rows with ``positions > 0``)."""
         from extensions_b200 import tiny_llm_ext_b200 as ext
 
+        n = tokens.shape[0]
         if self.json_states is not None:
-            n = tokens.shape[0]
             ext.json_advance(self.descriptors[:n], self.json_states[:n], tokens, positions)
+        if self.schema_states is not None:
+            ext.schema_advance(self.descriptors[:n], self.schema_states[:n], tokens, positions)
 
     def walkers(self) -> list:
-        """The host mirror of each row's JSON state (None for rows not in JSON mode); one device read."""
-        if self.json_states is None:
-            return [None] * self.rows
-        words = self.json_states.tolist()
-        return [None if c is None else JsonWalker(w) for c, w in zip(self._json_constraints, words)]
+        """The host mirror of each row's JSON or schema state (None for other rows); one device read per kind."""
+        from .json_schema import SchemaWalker
+
+        jw = self.json_states.tolist() if self.json_states is not None else None
+        sw = self.schema_states.tolist() if self.schema_states is not None else None
+        out = []
+        for r, c in enumerate(self._json_constraints):
+            if c is None:
+                out.append(None)
+            elif isinstance(c, JsonConstraint):
+                out.append(JsonWalker(jw[r]))
+            else:
+                out.append(SchemaWalker(c.compiled, sw[r]))
+        return out

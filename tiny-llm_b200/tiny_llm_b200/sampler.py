@@ -54,7 +54,8 @@ class SamplingParams:
     ``constraint`` (a ``TokenConstraint``, ``tl_sample_constrained``, DESIGN.md section 8c) restricts every draw to the
     tokens that keep the text a prefix of the pattern's language (EOS once it is a match); greedy under a constraint is
     ``SamplingParams(0.0, constraint=c)``.  With a mask that allows every token the draw is the unconstrained one.
-    A ``JsonConstraint`` (JSON mode, DESIGN.md section 20) restricts the text to one JSON object the same way."""
+    A ``JsonConstraint`` (JSON mode, DESIGN.md section 20) restricts the text to one JSON object the same way, and a
+    ``JsonSchemaConstraint`` (DESIGN.md section 21) to one JSON object that validates against a schema."""
 
     temperature: float
     top_k: int | None = None
@@ -96,8 +97,9 @@ class SamplingParams:
         if self.constraint is not None:
             from .constrained import TokenConstraint
             from .json_mode import JsonConstraint
+            from .json_schema import JsonSchemaConstraint
 
-            if not isinstance(self.constraint, (TokenConstraint, JsonConstraint)):
+            if not isinstance(self.constraint, (TokenConstraint, JsonConstraint, JsonSchemaConstraint)):
                 raise ValueError(f"constraint must be None or a TokenConstraint, got {type(self.constraint).__name__}")
 
     @property
@@ -198,10 +200,13 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
                 raise ValueError("a penalised SamplingParams needs the request's token state")
             pen = (*penalty_tensors(params, logits.device), state)
         from .json_mode import ConstraintRows, JsonConstraint
+        from .json_schema import JsonSchemaConstraint
 
         if not isinstance(constraints, ConstraintRows):
             if any(p is not None and isinstance(p.constraint, JsonConstraint) for p in params):
                 raise ValueError("a JSON-mode SamplingParams needs the request's ConstraintRows")
+            if any(p is not None and isinstance(p.constraint, JsonSchemaConstraint) for p in params):
+                raise ValueError("a JSON-schema SamplingParams needs the request's ConstraintRows")
             return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
         constraints.before_draw(len(params))
         tokens = ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints.descriptors[:len(params)], *pen)

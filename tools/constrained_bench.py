@@ -6,8 +6,11 @@
   on the same rows, at 1, 8 and 64 rows (CUDA events over 200 launches);
 * JSON mode's ``tl_json_token_masks`` per call at 1, 8 and 64 rows, every row inside a string value (nearly every
   token walks its whole length) and every row at a value position (most tokens fail on their first byte);
-* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+`` and under JSON mode, at B = 1 and B = 8 on
-  Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
+* JSON Schema's ``tl_schema_token_masks`` per call at 1, 8 and 64 rows under ``SCHEMA`` (11 properties, a nested
+  array of objects, an enum, a pattern and a recursive ``$ref``), beside ``tl_json_token_masks`` on the same text in
+  the same process, inside a string value and at a value position;
+* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+``, under JSON mode and under ``SCHEMA``, at B = 1
+  and B = 8 on Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
 
   python tools/constrained_bench.py [--out tools_out/constrained_bench.json]
 """
@@ -31,6 +34,7 @@ from tiny_llm_b200 import BatchingKvCache, Qwen3ModelWeek3, SamplingParams  # no
 from tiny_llm_b200.constrained import TokenConstraint, TokenVocabulary, compile_dfa  # noqa: E402
 from tiny_llm_b200.engine import DecodeEngine  # noqa: E402
 from tiny_llm_b200.json_mode import ConstraintRows, JsonConstraint, JsonWalker  # noqa: E402
+from tiny_llm_b200.json_schema import SCHEMA_SMEM_BYTES, JsonSchemaConstraint  # noqa: E402
 from tiny_llm_b200.sampler import sampling_tensors  # noqa: E402
 from tiny_llm_b200.synthetic import synthetic_qwen3  # noqa: E402
 
@@ -102,10 +106,59 @@ def json_mask_table(jc) -> dict:
     return out
 
 
-def decode_rates(model, c, jc, B, ctx=128, steps=64, rounds=3) -> dict:
+SCHEMA = {
+    "type": "object",
+    "properties": {
+        "name": {"type": "string"},
+        "age": {"type": "integer"},
+        "email": {"type": "string", "pattern": "^[a-z]{1,16}@[a-z]{1,12}\\.com$"},
+        "status": {"enum": ["active", "inactive", "pending", None]},
+        "score": {"type": "number"},
+        "nickname": {"type": ["string", "null"]},
+        "tags": {"type": "array", "items": {"type": "string"}, "maxItems": 8},
+        "address": {"type": "object", "properties": {"street": {"type": "string"}, "city": {"type": "string"}, "zip": {"type": "string"}},
+                    "required": ["street", "city"]},
+        "orders": {"type": "array", "items": {"type": "object", "properties": {"id": {"type": "integer"}, "qty": {"type": "integer"},
+                                                                                "note": {"type": "string"}}, "required": ["id", "qty"]}},
+        "comments": {"type": "array", "items": {"$ref": "#/$defs/comment"}},
+        "active": {"type": "boolean"},
+    },
+    "required": ["name", "age", "status"],
+    "$defs": {"comment": {"type": "object", "properties": {"text": {"type": "string"}, "replies": {"type": "array", "items": {"$ref": "#/$defs/comment"}}},
+                          "required": ["text"]}},
+}
+
+
+def schema_mask_table(sc, jc) -> dict:
+    """``tl_schema_token_masks`` under SCHEMA beside ``tl_json_token_masks`` on the same text, alternated per size."""
+    out = {"blob_bytes": int(sc.compiled.blob.size), "staged": bool(sc.compiled.blob.size <= SCHEMA_SMEM_BYTES),
+           "states": sc.compiled.num_states, "classes": sc.compiled.num_classes}
+    print(f"schema tables: {out['states']} states, {out['classes']} byte classes, {out['blob_bytes']} bytes "
+          f"({'staged in' if out['staged'] else 'read around'} shared memory)", flush=True)
+    for rows in (1, 8, 64):
+        res = {}
+        for where, text in (("in_string", b'{"name": "abc'), ("at_value", b'{"name": ')):
+            w = sc.start()
+            assert w.walk(text)
+            jw = JsonWalker()
+            jw.walk(text)
+            tab = ConstraintRows(rows, V, DEV, json=False, schema=True)
+            jtab = ConstraintRows(rows, V, DEV, json=True)
+            for r in range(rows):
+                tab.set_row(r, sc, w)
+                jtab.set_row(r, jc, jw)
+            res[f"schema_{where}"] = timed(lambda: ext.schema_token_masks(tab.descriptors, tab.schema_states, V))
+            res[f"json_{where}"] = timed(lambda: ext.json_token_masks(jtab.descriptors, jtab.json_states, V))
+        out[rows] = res
+        print(f"schema vs json masks, rows {rows}: " + ", ".join(f"{k} {v:.1f} us" for k, v in res.items()), flush=True)
+    return out
+
+
+def decode_rates(model, c, jc, sc, B, ctx=128, steps=64, rounds=3) -> dict:
     modes = {"sampled": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1),
              "constrained": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=c),
-             "json": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=jc)}
+             "json": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=jc),
+             "schema": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=sc)}
     msl = ctx + len(modes) * (rounds + 1) * steps + 64
     engine = DecodeEngine(model, B, msl, DEV)
     engine.reserve_pools()
@@ -130,7 +183,7 @@ def decode_rates(model, c, jc, B, ctx=128, steps=64, rounds=3) -> dict:
                 times[mode].append(a.elapsed_time(b))
     res = {m: B * steps * len(v) / (sum(v) / 1e3) for m, v in times.items()}
     res["kernels_per_step"] = {"sampled": engine.kernels_per_sampled_step, "constrained": engine.kernels_per_constrained_step,
-                               "json": engine.kernels_per_json_step}
+                               "json": engine.kernels_per_json_step, "schema": engine.kernels_per_schema_step}
     for t in tables:  # the next engine reserves its pages from the same pools
         for cc in t.kv_caches:
             if cc is not None:
@@ -138,7 +191,7 @@ def decode_rates(model, c, jc, B, ctx=128, steps=64, rounds=3) -> dict:
     print(f"B {B}: sampled {res['sampled']:.1f} tok/s, constrained {res['constrained']:.1f} tok/s "
           f"({(res['constrained'] / res['sampled'] - 1) * 100:+.2f} %), json {res['json']:.1f} tok/s "
           f"({(res['json'] / res['sampled'] - 1) * 100:+.2f} % against sampled, {(res['json'] / res['constrained'] - 1) * 100:+.2f} % "
-          "against [a-z ]+)", flush=True)
+          f"against [a-z ]+), schema {res['schema']:.1f} tok/s ({(res['schema'] / res['json'] - 1) * 100:+.2f} % against json)", flush=True)
     return res
 
 
@@ -156,9 +209,11 @@ def main() -> None:
     result["kernels_us"] = kernel_table(c)
     jc = JsonConstraint(vocab, device=DEV)
     result["json_masks_us"] = json_mask_table(jc)
+    sc = JsonSchemaConstraint(SCHEMA, vocab, device=DEV)
+    result["schema_masks_us"] = schema_mask_table(sc, jc)
     ns = synthetic_qwen3("qwen3-4b", seed=0, device=DEV)
     model = Qwen3ModelWeek3(ns, page_size=64)
-    result["decode"] = {B: decode_rates(model, c, jc, B) for B in (1, 8)}
+    result["decode"] = {B: decode_rates(model, c, jc, sc, B) for B in (1, 8)}
     if args.out:
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
         Path(args.out).write_text(json.dumps(result, indent=1))
