@@ -9,6 +9,8 @@ in float64 from the exact inputs, on the inputs' device, and return besides the 
     smax[r]   = max over keys with p_j > 0 of |mask_j| + scale * sum_d |q_d k_jd|     bounds |s_j| and its fp32 error
     nvis[r]   = number of keys the row sees                        bounds the length of fp32 accumulation chains
 
+``masked_reference`` takes an explicit key mask instead (``segment_visible`` builds the one of the segment-causal and
+prefixed-segment entry points) and also returns V1, the sum of |v| over the visible keys.
 ``error_bound`` turns them into an elementwise tolerance (its docstring has the derivation).  ``check_needles``
 compares a kernel with the reference on needle queries (``needle_queries``): a query that is a scaled copy of one key
 puts almost all the probability on that key, so whether the kernel saw the key changes the output by O(1).
@@ -124,7 +126,67 @@ def dense_reference(q, k, v, mask, scale, causal, has_mask, num_heads, num_kv_he
     return out.reshape(rows, L, D), A.reshape(rows, L, D), smax.reshape(rows, L), nvis
 
 
-def error_bound(ref, A, smax, nvis, D, out_dtype, p_rounded):
+def masked_reference(q, k, v, visible, scale, num_kv_heads):
+    """Attention over an explicit key mask: q [Hq, L, D]; k / v [Hkv, S, D] in logical key order; visible bool
+    [Hq or 1, L, S].  Returns (out, A, smax, nvis) as ``paged_reference`` does, plus V1 [Hq, L, D] = the sum of |v_jd|
+    over the keys the row sees (the scale of P's absolute rounding floor, ``error_bound(p_dtype=float16)``).  Float64
+    on q's device, chunked over rows so that L = S = 8192 fits."""
+    Hq, L, D = q.shape
+    S = k.shape[1]
+    G = Hq // num_kv_heads
+    dev = q.device
+    Q = q.to(F64).reshape(num_kv_heads, G, L, D)
+    K, V = k.to(dev).to(F64)[:, None], v.to(dev).to(F64)[:, None]  # [Hkv, 1, S, D]
+    Kt, Ka, Va = K.transpose(-1, -2), K.abs().transpose(-1, -2), V.abs()
+    vis = visible.to(dev)
+    out = torch.zeros(Hq, L, D, dtype=F64, device=dev)
+    A, V1 = torch.zeros_like(out), torch.zeros_like(out)
+    smax = torch.zeros(Hq, L, dtype=F64, device=dev)
+    nvis = torch.zeros(Hq, L, dtype=torch.int64, device=dev)
+    chunk = max(1, (1 << 25) // (Hq * max(S, 1)))
+    for l0 in range(0, L, chunk):
+        l1 = min(L, l0 + chunk)
+        ok = vis[:, l0:l1].expand(Hq, l1 - l0, S).reshape(num_kv_heads, G, l1 - l0, S)
+        s = (scale * (Q[:, :, l0:l1] @ Kt)).masked_fill(~ok, float("-inf"))
+        absum = abs(scale) * (Q[:, :, l0:l1].abs() @ Ka)
+        o = torch.empty(num_kv_heads, G, l1 - l0, D, dtype=F64, device=dev)
+        a = torch.empty_like(o)
+        sm = torch.empty(num_kv_heads, G, l1 - l0, dtype=F64, device=dev)
+        _softmax_stats(s, absum, V, o, a, sm)
+        out[:, l0:l1] = o.reshape(Hq, l1 - l0, D)
+        A[:, l0:l1] = a.reshape(Hq, l1 - l0, D)
+        smax[:, l0:l1] = sm.reshape(Hq, l1 - l0)
+        V1[:, l0:l1] = (ok.to(F64) @ Va).reshape(Hq, l1 - l0, D)
+        nvis[:, l0:l1] = ok.sum(dim=-1).reshape(Hq, l1 - l0)
+    return out, A, smax, nvis, V1
+
+
+def live_keys(block_table, num_pages, page_size, S):
+    """[S] bool: key j's page id block_table[j // page_size] is in [0, num_pages)."""
+    ids = block_table.to(torch.int64).reshape(-1).cpu()[torch.arange(S) // page_size]
+    return (ids >= 0) & (ids < num_pages)
+
+
+def segment_visible(segment_start, key_live, prefix_start=None, prefix_end=None):
+    """[1, L, L] bool: the keys row l of ``tl_paged_attention_segments`` (prefix_start None) or
+    ``tl_paged_attention_prefixed_segments`` sees over one packed request whose keys are its L rows.  With
+    lo = max(segment_start[l], 0): nothing when segment_start[l] > l; else [lo, l] and, prefixed, [max(prefix_start[l], 0),
+    min(prefix_end[l], lo)); never a key whose page is not live (``live_keys``)."""
+    seg = torch.as_tensor(segment_start, dtype=torch.int64).cpu()
+    L = seg.shape[0]
+    row = torch.arange(L)[:, None]
+    key = torch.arange(L)[None, :]
+    lo = seg.clamp(min=0)[:, None]
+    own = seg[:, None] <= row
+    vis = (key >= lo) & (key <= row)
+    if prefix_start is not None:
+        ps = torch.as_tensor(prefix_start, dtype=torch.int64).cpu().clamp(min=0)[:, None]
+        pe = torch.minimum(torch.as_tensor(prefix_end, dtype=torch.int64).cpu()[:, None], lo)
+        vis = vis | ((key >= ps) & (key < pe))
+    return (vis & own & key_live[None, :])[None]
+
+
+def error_bound(ref, A, smax, nvis, D, out_dtype, p_rounded, *, p_dtype=torch.bfloat16, V1=None):
     """Elementwise bound on |kernel - ref| for a kernel that computes scores and the softmax in fp32.
 
     Scores.  A score is a sum of D products; in fp32 (bf16 x bf16 products are exact, an MMA may truncate each
@@ -135,7 +197,13 @@ def error_bound(ref, A, smax, nvis, D, out_dtype, p_rounded):
     by a factor in [e^-2delta, e^2delta], so the output moves by at most eps_s A with eps_s = e^(2 delta) - 1.
 
     P.  The tensor-core kernels (mma.sync flash, wgmma) round P to bf16 for P V while the row sum uses the unrounded
-    P: at most 2^-8 A (bf16 unit roundoff, ``p_rounded``).
+    P: at most 2^-8 A (bf16 unit roundoff, ``p_rounded``).  The fp16 form of the wgmma kernel (``p_dtype`` float16)
+    rounds P to fp16, whose range ends where bf16's does not: in the units the row is finally normalised with, its
+    largest p is >= 1 (the kept maximum lies at most 2^8 below the row's maximum and never above it; a rescale only
+    scales earlier terms down), an fp16 p below 2^-14 is subnormal and one below 2^-25 rounds to 0.  So each p is off by
+    at most 2^-11 p + 2^-25, and since sum p >= 1 the output by at most 2^-11 A + 2^-25 V1, V1 = sum over the visible
+    keys of |v_jd| (``masked_reference``).  Example: a key at the row maximum with v_d = 0 and 4,000 keys 18 nats lower
+    with v_d = 1 give ref_d = 6e-5 while every p of those keys (2^-26) rounds to 0.
 
     Accumulation.  O and the row sum are fp32 sums; no kernel adds more than nvis / 4 + 64 terms in one sequential
     chain (the row-wise and dense kernels' four warps are the narrowest split), each addition off by <= 2^-24
@@ -148,9 +216,16 @@ def error_bound(ref, A, smax, nvis, D, out_dtype, p_rounded):
     delta = (2 * D + 16) * 2.0**-24 * smax + 2.0**-20
     eps_s = torch.expm1(2 * delta)
     n_acc = (nvis.to(F64) / 4 + 64) * 2.0**-23
-    u_p = 2.0**-8 if p_rounded else 0.0
+    u_p = UNIT_ROUNDOFF[p_dtype] if p_rounded else 0.0
     u_out = UNIT_ROUNDOFF[out_dtype] + 2.0**-23
-    return u_out * ref.abs() + (u_p + eps_s + n_acc)[..., None] * A
+    tol = u_out * ref.abs() + (u_p + eps_s + n_acc)[..., None] * A
+    if p_rounded and p_dtype == torch.float16:
+        if V1 is None:
+            raise ValueError("error_bound: fp16 P needs V1, the sum of |v| over the visible keys")
+        tol = tol + 2.0**-25 * V1
+    elif p_rounded and p_dtype != torch.bfloat16:
+        raise ValueError(f"error_bound: no bound for P rounded to {p_dtype}")
+    return tol
 
 
 def assert_within(got, ref, tol, what):
