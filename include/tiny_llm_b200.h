@@ -427,6 +427,49 @@ int tl_schema_token_masks(const tl_constraint_row *constraints, const int64_t *s
  * bytes (the dead state when it leaves the language), or terminal when the token has no bytes (EOS). */
 int tl_schema_advance(const tl_constraint_row *constraints, int64_t *schema_states, const int32_t *tokens, const int32_t *positions,
                       int rows, void *stream);
+/* Grammar-constrained generation (DESIGN.md section 23): a byte-level pushdown automaton compiled from a GBNF grammar
+ * into one table blob per grammar (grammar.py writes it; 16-byte aligned):
+ *   int32 num_states S (ids 0..S-1, 0 dead), num_classes C, blob bytes, action words A;  uint8 class_of[256];
+ *   uint32 info[S]      bit 0 the state's rule may end here, bits 8-15 need (stack entries the cheapest completion
+ *                       from the state still pushes);
+ *   uint32 trans[S, C]  0 no action, else bits 0-23 the first action word in acts, bits 24-31 the action count;
+ *   uint32 acts[A]      per action one word (bits 0-14 target, 16-21 pushes k, 24-31 peak: the most stack entries the
+ *                       chain's cheapest completion holds above the current depth), then ceil(k / 2) words of 16-bit
+ *                       return states, bottom first, low half first.
+ * A grammar row is a tl_constraint_row exactly like a JSON row (num_states 1, its own uint32 [2, ceil(vocab / 32)] mask
+ * buffer, the all-zero dfa).  Its state is a set of at most TL_GRAMMAR_MAX_PARSES parses in TL_GRAMMAR_STATE_WORDS
+ * int64 words:
+ *   word 0         the row's table blob (0: not a grammar row);
+ *   word 1         bits 0-3 the parse count n, 32 the row is in grammar mode, 33 terminal (after EOS), 34 failed (a
+ *                  drawn token was not allowed);
+ *   words 2-9      parse p < n: bits 0-14 state, 16-21 depth; others 0;
+ *   words 10-73    the return stacks, 16 bits each: entry k of parse p at uint16 index p * TL_GRAMMAR_MAX_DEPTH + k;
+ *                  entries at or above a parse's depth are 0.
+ * A byte over the set: for each parse in order, each action of its state on the byte's class (in table order) whose
+ * depth + peak <= TL_GRAMMAR_MAX_DEPTH makes a parse (target, stack + pushes), kept unless an equal (state, depth,
+ * stack) parse was made before; then, while the state's rule may end and the depth is above 0, the return state is
+ * popped and its actions are taken the same way.  The byte fails when no parse is made or when a parse beyond
+ * TL_GRAMMAR_MAX_PARSES would be kept.  The text is complete when some parse, popping through states whose rule may
+ * end, reaches depth 0 in such a state. */
+#define TL_GRAMMAR_MAX_STATES 32767
+#define TL_GRAMMAR_MAX_DEPTH 32
+#define TL_GRAMMAR_MAX_PARSES 8
+#define TL_GRAMMAR_MAX_TABLE_BYTES (1 << 22)
+#define TL_GRAMMAR_SMEM_BYTES (46 * 1024)
+#define TL_GRAMMAR_STATE_WORDS 74
+/* Row 0 of every grammar row's mask (rows with bit 32 of word 1 set and bit 33 clear; others are not touched), in one
+ * launch: bit t iff token t has bytes and walking them from the row's parse set never fails, or t has no bytes, the
+ * text is complete and bit t of the row's mask row 1 is set.  smem_bytes (a multiple of 16, at most
+ * TL_GRAMMAR_SMEM_BYTES) is the dynamic shared memory of each CTA: a row's blob is staged there when it fits and read
+ * through L1/L2 otherwise, with the same result.  Deterministic, no atomics. */
+int tl_grammar_token_masks(const tl_constraint_row *constraints, const int64_t *grammar_states, int rows, int vocab, int smem_bytes,
+                           void *stream);
+/* After the draw: for grammar rows with positions[r] > 0, neither terminal nor failed, the parse set becomes the walk of
+ * tokens[r]'s bytes, or terminal when the token has no bytes, is an EOS id (bit set in the row's mask row 1) and the
+ * text is complete.  A token that is not allowed (drawn only when the row allows none) leaves n = 0, every parse and
+ * stack word 0 and the failed bit set; callers must refuse such a row. */
+int tl_grammar_advance(const tl_constraint_row *constraints, int64_t *grammar_states, const int32_t *tokens, const int32_t *positions,
+                       int rows, int vocab, void *stream);
 /* Log-probabilities of logits [rows, vocab] (rows <= 65535, vocab <= 409,600; fp32, fp16 or bf16 read as fp32), one
  * launch, one cluster of CTAs per row (DESIGN.md section 8a).
  *

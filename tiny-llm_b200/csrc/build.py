@@ -42,6 +42,7 @@ SOURCES = [
     "constrained.cu",
     "json.cu",
     "json_schema.cu",
+    "grammar.cu",
     "logit_controls.cu",
     "moe.cu",
     "moe_router.cu",

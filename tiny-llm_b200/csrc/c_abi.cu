@@ -666,6 +666,21 @@ int tl_schema_advance(const tl_constraint_row *constraints, int64_t *schema_stat
     return launch_schema_advance(constraints, schema_states, tokens, positions, rows, as_stream(stream));
 }
 
+int tl_grammar_token_masks(const tl_constraint_row *constraints, const int64_t *grammar_states, int rows, int vocab, int smem_bytes,
+                           void *stream) {
+    if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "grammar_token_masks: bad shape");
+    if (smem_bytes < 0 || smem_bytes > TL_GRAMMAR_SMEM_BYTES || smem_bytes % 16) return fail(TL_EINVAL, "grammar_token_masks: bad smem_bytes");
+    if (rows > 0 && (!constraints || !grammar_states)) return fail(TL_EINVAL, "grammar_token_masks: null pointer");
+    return launch_grammar_token_masks(constraints, grammar_states, rows, vocab, smem_bytes, as_stream(stream));
+}
+
+int tl_grammar_advance(const tl_constraint_row *constraints, int64_t *grammar_states, const int32_t *tokens, const int32_t *positions,
+                       int rows, int vocab, void *stream) {
+    if (rows < 0 || vocab <= 0) return fail(TL_EINVAL, "grammar_advance: bad shape");
+    if (rows > 0 && (!constraints || !grammar_states || !tokens || !positions)) return fail(TL_EINVAL, "grammar_advance: null pointer");
+    return launch_grammar_advance(constraints, grammar_states, tokens, positions, rows, vocab, as_stream(stream));
+}
+
 int tl_logit_controls(const void *logits, const tl_control_row *controls, const int32_t *positions, const int32_t *tokens,
                       int32_t *tails, float *out, int rows, int vocab, int dtype, void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "logit_controls: expected float32, float16, or bfloat16");

@@ -62,6 +62,11 @@ int launch_schema_token_masks(const tl_constraint_row *constraints, const int64_
                               cudaStream_t st);
 int launch_schema_advance(const tl_constraint_row *constraints, int64_t *states, const int32_t *tokens, const int32_t *positions,
                           int rows, cudaStream_t st);
+// grammar.cu
+int launch_grammar_token_masks(const tl_constraint_row *constraints, const int64_t *states, int rows, int vocab, int smem_bytes,
+                               cudaStream_t st);
+int launch_grammar_advance(const tl_constraint_row *constraints, int64_t *states, const int32_t *tokens, const int32_t *positions,
+                           int rows, int vocab, cudaStream_t st);
 // logit_controls.cu
 int launch_logit_controls(const void *logits, const tl_control_row *controls, const int32_t *positions, const int32_t *tokens,
                           int32_t *tails, float *out, int rows, int vocab, int dtype, cudaStream_t st);

@@ -68,6 +68,9 @@ __all__ = [
     "schema_token_masks",
     "schema_advance",
     "SCHEMA_STATE_WORDS",
+    "grammar_token_masks",
+    "grammar_advance",
+    "GRAMMAR_STATE_WORDS",
     "logprobs",
     "LOGPROBS_MAX_N",
     "decode_advance",
@@ -155,6 +158,8 @@ _SIGNATURES = {
     "tl_json_advance": (_I, [_VP] * 4 + [_I, _VP]),
     "tl_schema_token_masks": (_I, [_VP, _VP, _I, _I, _I, _VP]),
     "tl_schema_advance": (_I, [_VP] * 4 + [_I, _VP]),
+    "tl_grammar_token_masks": (_I, [_VP, _VP, _I, _I, _I, _VP]),
+    "tl_grammar_advance": (_I, [_VP] * 4 + [_I, _I, _VP]),
     "tl_logprobs": (_I, [_VP] * 9 + [_I] * 5 + [_VP]),
     "tl_qkv_project_rope_append": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP]),
     "tl_qkv_project_rope_append_table": (_I, [_VP] * 13 + [_I] * 5 + [_F, _F] + [_I] * 5 + [_VP, _SZ, _VP, _VP]),
@@ -1145,6 +1150,52 @@ def schema_advance(constraints, schema_states, tokens, positions, stream=None):
     _gpu("schema_advance", *named.values())
     _check(_lib.tl_schema_advance(constraints.data_ptr(), schema_states.data_ptr(), tokens.data_ptr(), positions.data_ptr(), rows,
                                   _stream_ptr(stream, constraints)))
+
+
+GRAMMAR_STATE_WORDS = 74  # int64 words of one grammar row's parse set (include/tiny_llm_b200.h)
+GRAMMAR_SMEM_BYTES = 46 * 1024  # TL_GRAMMAR_SMEM_BYTES: the largest table blob a masks launch stages in shared memory
+
+
+def _grammar_rows(op, constraints, grammar_states):
+    if constraints.dtype != torch.int64 or constraints.dim() != 2 or constraints.shape[1] != CONSTRAINT_ROW_WORDS:
+        raise RuntimeError(f"{op}: constraints must be int64 [rows, {CONSTRAINT_ROW_WORDS}]")
+    rows = constraints.shape[0]
+    if grammar_states.dtype != torch.int64 or tuple(grammar_states.shape) != (rows, GRAMMAR_STATE_WORDS):
+        raise RuntimeError(f"{op}: grammar_states must be int64 [{rows}, {GRAMMAR_STATE_WORDS}]")
+    return rows
+
+
+def grammar_token_masks(constraints, grammar_states, vocab, smem_bytes=0, stream=None):
+    """Row 0 of each grammar row's mask buffer (``tl_grammar_token_masks``): ``constraints`` int64 ``[rows, 5]``
+    descriptors, ``grammar_states`` int64 ``[rows, 74]`` parse sets (word 0 the row's table blob); rows not in grammar
+    mode, or terminal, are not touched.  ``smem_bytes``: the shared memory that stages blobs up to that size
+    (``ConstraintRows.grammar_smem_bytes``).  Writes through the descriptors' mask pointers; returns nothing."""
+    rows = _grammar_rows("grammar_token_masks", constraints, grammar_states)
+    if isinstance(vocab, bool) or not isinstance(vocab, int) or vocab <= 0:
+        raise RuntimeError("grammar_token_masks: vocab must be a positive int")
+    if isinstance(smem_bytes, bool) or not isinstance(smem_bytes, int) or not 0 <= smem_bytes <= GRAMMAR_SMEM_BYTES or smem_bytes % 16:
+        raise RuntimeError(f"grammar_token_masks: smem_bytes must be a multiple of 16 in [0, {GRAMMAR_SMEM_BYTES}]")
+    _contig("grammar_token_masks", constraints=constraints, grammar_states=grammar_states)
+    _gpu("grammar_token_masks", constraints, grammar_states)
+    _check(_lib.tl_grammar_token_masks(constraints.data_ptr(), grammar_states.data_ptr(), rows, vocab, smem_bytes,
+                                       _stream_ptr(stream, constraints)))
+
+
+def grammar_advance(constraints, grammar_states, tokens, positions, vocab, stream=None):
+    """Advance each grammar row's parse set by its drawn token (``tl_grammar_advance``), for rows with
+    ``positions > 0``; ``tokens`` and ``positions`` int32 ``[rows]``.  A token the row did not allow sets the row's
+    failed bit (bit 34 of word 1)."""
+    rows = _grammar_rows("grammar_advance", constraints, grammar_states)
+    if isinstance(vocab, bool) or not isinstance(vocab, int) or vocab <= 0:
+        raise RuntimeError("grammar_advance: vocab must be a positive int")
+    for name, t in (("tokens", tokens), ("positions", positions)):
+        if t.dtype != torch.int32 or tuple(t.shape) != (rows,):
+            raise RuntimeError(f"grammar_advance: {name} must be int32 [{rows}]")
+    named = dict(constraints=constraints, grammar_states=grammar_states, tokens=tokens, positions=positions)
+    _contig("grammar_advance", **named)
+    _gpu("grammar_advance", *named.values())
+    _check(_lib.tl_grammar_advance(constraints.data_ptr(), grammar_states.data_ptr(), tokens.data_ptr(), positions.data_ptr(), rows,
+                                   vocab, _stream_ptr(stream, constraints)))
 
 
 def constraint_token_masks(dfa, accept, token_offsets, token_bytes, eos_ids, stream=None):

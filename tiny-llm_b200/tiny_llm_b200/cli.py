@@ -36,6 +36,8 @@ see checkpoint.py; there is no hub download here).
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 \
         --json-schema '{"type": "object", "properties": {"name": {"type": "string"}}, "required": ["name"]}'
         (one JSON object that validates against the schema, keys in the schema's order; FILE_OR_INLINE_JSON)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --grammar 'root ::= [0-9]+ ("+" [0-9]+)*'
+        (the generated text stays in the language of a GBNF grammar; FILE_OR_INLINE grammar text)
     python -m tiny_llm_b200.cli batch --synthetic tiny-d128 --synthetic-lora a=16 --synthetic-lora b=8:1 \
         --prompt-ids "5,17,3;5,17,3;5,17,3" --adapters "a;;b"
         (one resident base model, each request under the LoRA adapter it names: --lora NAME=DIR loads a PEFT directory)
@@ -211,9 +213,14 @@ def _controls(args) -> dict:
 
 
 def _constraint(args, model, tokenizer, device):
-    """The ``TokenConstraint`` of ``--regex``, the ``JsonConstraint`` of ``--json`` or the ``JsonSchemaConstraint`` of
-    ``--json-schema`` over the checkpoint tokenizer's vocabulary (the synthetic vocabulary with ``--synthetic``), or
-    None."""
+    """The ``TokenConstraint`` of ``--regex``, the ``JsonConstraint`` of ``--json``, the ``JsonSchemaConstraint`` of
+    ``--json-schema`` or the ``GrammarConstraint`` of ``--grammar`` over the checkpoint tokenizer's vocabulary (the
+    synthetic vocabulary with ``--synthetic``), or None."""
+    grammar_text = getattr(args, "grammar", None)
+    if grammar_text is not None and (args.regex is not None or args.json or args.json_schema is not None):
+        raise SystemExit("--grammar takes no --regex, --json or --json-schema: give one constraint")
+    if grammar_text is not None:
+        return _grammar_constraint(args, grammar_text, model, tokenizer, device)
     schema_text = args.json_schema
     given = [f for f, on in (("--regex", args.regex is not None), ("--json", args.json), ("--json-schema", schema_text is not None)) if on]
     if args.regex is not None and args.json:
@@ -251,6 +258,28 @@ def _constraint(args, model, tokenizer, device):
         raise SystemExit(f"{flag}: {exc}")
 
 
+def _grammar_constraint(args, text: str, model, tokenizer, device):
+    from .constrained import TokenVocabulary
+    from .grammar import GrammarConstraint, load_grammar_arg
+
+    try:
+        grammar = load_grammar_arg(text)
+    except (OSError, UnicodeDecodeError) as exc:
+        raise SystemExit(f"--grammar: not a grammar file or inline GBNF grammar: {exc}")
+    if device.type != "cuda":
+        raise SystemExit("--grammar runs on the CUDA sampling kernel: use a cuda --device")
+    if args.synthetic:
+        vocabulary = TokenVocabulary.synthetic(model.vocab_size)
+    elif tokenizer is None:
+        raise SystemExit("--grammar needs the checkpoint's tokenizer files (or --synthetic)")
+    else:
+        vocabulary = TokenVocabulary.from_tokenizer(tokenizer, model.vocab_size)
+    try:
+        return GrammarConstraint(grammar, vocabulary, device=device)
+    except ValueError as exc:
+        raise SystemExit(f"--grammar: {exc}")
+
+
 def _adapter_kw(args, key: str) -> dict:
     """``{key: name}`` for ``--adapter NAME`` (nothing without it, so models that take no adapters run as before)."""
     return {} if args.adapter is None else {key: args.adapter}
@@ -286,8 +315,12 @@ def cmd_generate(args) -> int:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --json")
     if speculative and args.json_schema is not None:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --json-schema")
+    if speculative and args.grammar is not None:
+        raise SystemExit("speculative decoding and prompt lookup are greedy and unconstrained: drop --grammar")
     if speculative and controls:
         raise SystemExit("speculative decoding takes no --logit-bias, --allowed-token-ids, --bad-words or --min-tokens")
+    if controls and args.grammar is not None:
+        raise SystemExit("--logit-bias, --allowed-token-ids, --bad-words and --min-tokens take no --grammar")
     constraint = _constraint(args, model, tokenizer, device)
     if constraint is not None:
         if controls:
@@ -409,7 +442,8 @@ def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
 
     refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("penalties or --min-p", bool(penalties)),
                ("--regex", args.regex is not None), ("--json", args.json),
-               ("--json-schema", args.json_schema is not None), ("--logprobs", args.logprobs is not None),
+               ("--json-schema", args.json_schema is not None), ("--grammar", args.grammar is not None),
+               ("--logprobs", args.logprobs is not None),
                ("adapters", args.adapter is not None or getattr(model, "adapters", None) is not None),
                ("a draft", bool(args.draft_model or args.draft_synthetic)), ("--prompt-lookup", args.prompt_lookup is not None)]
     for what, given in refused:
@@ -451,6 +485,8 @@ def cmd_batch(args) -> int:
     sampling = None
     penalties = _penalties(args)
     controls = _controls(args)
+    if controls and args.grammar is not None:
+        raise SystemExit("--logit-bias, --allowed-token-ids, --bad-words and --min-tokens take no --grammar")
     constraint = _constraint(args, model, tokenizer, device)
     if constraint is not None:
         if controls:
@@ -668,6 +704,9 @@ def main(argv=None) -> int:
         sub.choices[name].add_argument("--json-schema", default=None, metavar="FILE_OR_INLINE_JSON",
                                        help="constrain the generated text to one JSON object that validates against this JSON Schema "
                                             "(keys in the schema's order; DESIGN.md section 21 lists the keywords)")
+        sub.choices[name].add_argument("--grammar", default=None, metavar="FILE_OR_INLINE",
+                                       help="constrain the generated text to the language of this GBNF grammar (a file, or the "
+                                            "grammar text itself when it holds '::='; start rule root; DESIGN.md section 23)")
     for name in ("generate", "batch", "score"):
         sub.choices[name].add_argument("--logprobs", type=int, default=None, metavar="N",
                                        help="print each token's log-probability, rank and N most likely alternatives (N <= 20)")

@@ -38,6 +38,7 @@ import torch
 from extensions_b200 import tiny_llm_ext_b200 as ext
 
 from .json_mode import ConstraintRows, JsonConstraint
+from .grammar import GrammarConstraint
 from .json_schema import JsonSchemaConstraint
 from .kv_cache import BatchingKvCache
 from .moe import Moe, router_logits
@@ -452,6 +453,13 @@ class DecodeEngine(_GraphEngine):
         self.kernels_per_schema_step = 0
         self._schema_tab = None
         self._schema_key = None
+        # decode_on_device(sampling=<with a grammar slot>): one graph per (penalised, logprobs N or None, any JSON slot,
+        # any schema slot), the constrained step between the grammar (and JSON and schema) rows' masks and their
+        # advances over a B-row ConstraintRows of its own; all on first use
+        self._graph_grammar: dict = {}
+        self.kernels_per_grammar_step = 0
+        self._grammar_tab = None
+        self._grammar_key = None
         # decode_on_device(sampling=<with logits controls>): one graph per (penalised, logprobs N or None), the sampled
         # (or penalised) step with one tl_logit_controls launch before the draw, over a B-row ControlRows whose history
         # tails the launches advance, into a [B, V] fp32 buffer the draw reads; all on first use
@@ -512,7 +520,8 @@ class DecodeEngine(_GraphEngine):
         ``constrained == "json"`` (the JSON graph) draws over the JSON table's descriptors, between the JSON rows' mask
         launch and their state advance; ``constrained == "schema"`` (the schema graph) likewise over the schema table,
         with the schema rows' launches (and the JSON rows' when the table holds any); the masks launch stages the tables
-        in the shared memory the table held at capture.  ``controlled`` (the controlled graphs) first turns the rows into
+        in the shared memory the table held at capture.  ``constrained == "grammar"`` (the grammar graph) likewise over
+        the grammar table, with the grammar rows' launches and the JSON and schema rows' when the table holds any.  ``controlled`` (the controlled graphs) first turns the rows into
         their controlled fp32 rows with ``tl_logit_controls`` and draws from those; ``self.logits`` keeps the raw rows."""
         if controlled:
             tab = self._ctl_tab
@@ -525,11 +534,13 @@ class DecodeEngine(_GraphEngine):
             if penalized:
                 p = self._pen_dev.view(torch.float32).view(4, self.B)
                 pen = (p[0, :R], p[1, :R], p[2, :R], p[3, :R], self.token_counts[:R])
-            tab = self._json_tab if constrained == "json" else self._schema_tab if constrained == "schema" else None
+            tab = {"json": self._json_tab, "schema": self._schema_tab, "grammar": self._grammar_tab}.get(constrained)
             if tab is not None and tab.has_json:
                 ext.json_token_masks(tab.descriptors[:R], tab.json_states[:R], self.V)
             if tab is not None and tab.has_schema:
                 ext.schema_token_masks(tab.descriptors[:R], tab.schema_states[:R], self.V, tab.schema_smem_bytes)
+            if tab is not None and tab.has_grammar:
+                ext.grammar_token_masks(tab.descriptors[:R], tab.grammar_states[:R], self.V, tab.grammar_smem_bytes)
             descriptors = self._con_dev.view(self.B, -1)[:R] if tab is None else tab.descriptors[:R]
             tokens = ext.sample_constrained(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
                                             self.context_lens[:R], descriptors, *pen)
@@ -537,6 +548,8 @@ class DecodeEngine(_GraphEngine):
                 ext.json_advance(tab.descriptors[:R], tab.json_states[:R], tokens, self.context_lens[:R])
             if tab is not None and tab.has_schema:
                 ext.schema_advance(tab.descriptors[:R], tab.schema_states[:R], tokens, self.context_lens[:R])
+            if tab is not None and tab.has_grammar:
+                ext.grammar_advance(tab.descriptors[:R], tab.grammar_states[:R], tokens, self.context_lens[:R], self.V)
         elif penalized:
             pen = self._pen_dev.view(torch.float32).view(4, self.B)
             tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
@@ -718,6 +731,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_con = {}
         self._graph_json = {}
         self._graph_schema = {}
+        self._graph_grammar = {}
         self._graph_ctl = {}
         self._graph_keep = None
         self._graph_spec = {}
@@ -909,6 +923,7 @@ class DecodeEngine(_GraphEngine):
             self._graph_con = {k: g for k, g in self._graph_con.items() if k[1] is None}
             self._graph_json = {k: g for k, g in self._graph_json.items() if k[1] is None}
             self._graph_schema = {k: g for k, g in self._graph_schema.items() if k[1] is None}
+            self._graph_grammar = {k: g for k, g in self._graph_grammar.items() if k[1] is None}
             self._graph_ctl = {k: g for k, g in self._graph_ctl.items() if k[1] is None}
             self._lp_max_n = max_n
             self._lp_log = (torch.zeros((cap, B), dtype=torch.float32, device=dev), torch.zeros((cap, B), dtype=torch.float32, device=dev),
@@ -1045,7 +1060,29 @@ class DecodeEngine(_GraphEngine):
             self.kernels_per_schema_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
-    def _set_json_constraints(self, per: list, history, schema: bool = False) -> None:
+    def _ensure_grammar_graph(self, penalized: bool, max_n: int | None, json: bool, schema: bool) -> None:
+        """Capture the grammar step: the constrained step with the grammar rows' masks before the draw and their
+        advance after it, and the JSON and schema rows' too when ``json`` / ``schema`` (the warm-up runs at context 0,
+        so it advances no state).  One graph per (penalized, max_n, json, schema)."""
+        if (penalized, max_n, json, schema) in self._graph_grammar:
+            return
+        forward = self._forward_fused if self.fused else self._forward_unfused
+
+        def grammar_step():
+            forward(sampled=True, penalized=penalized, constrained="grammar")
+            if max_n is not None:
+                ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
+            ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
+
+        with torch.cuda.stream(self._stream):
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._set_idle()
+            self.step_counter.zero_()
+            self._graph_grammar[(penalized, max_n, json, schema)] = self._graph_of(grammar_step, pool=self._graph.pool(), warmups=1)
+            self.kernels_per_grammar_step = self._launches
+        torch.cuda.current_stream(self.device).wait_stream(self._stream)
+
+    def _set_json_constraints(self, per: list, history, schema: bool = False, grammar: bool = False) -> None:
         """The JSON table's rows for the slots' constraints (JSON, regex or none), as ``_set_constraints`` sets the
         descriptors: a slot with a ``history`` entry starts from the host walk of its generated ids (refused when they
         leave the language), a slot with a new constraint from the start state, and every other constrained slot
@@ -1062,20 +1099,25 @@ class DecodeEngine(_GraphEngine):
         for b, c in enumerate(cons):
             if c is None or history is None or history[b] is None:
                 continue
-            rows = isinstance(c, (JsonConstraint, JsonSchemaConstraint))
+            rows = isinstance(c, (JsonConstraint, JsonSchemaConstraint, GrammarConstraint))
             state = c.walk(history[b][1]) if rows else c.walk(c.start_state, history[b][1])
             if state is None or (not rows and state < 0):
                 raise ValueError(f"slot {b}: its generated ids leave the constraint's language")
             walked[b] = state
         key = tuple(cons)
-        tab, old = (self._schema_tab, self._schema_key) if schema else (self._json_tab, self._json_key)
+        if grammar:
+            tab, old = self._grammar_tab, self._grammar_key
+        else:
+            tab, old = (self._schema_tab, self._schema_key) if schema else (self._json_tab, self._json_key)
         if old is not None and all(x is y for x, y in zip(key, old)) and not walked:
             return
         torch.cuda.current_stream(self.device).wait_stream(self._stream)  # the previous call's replays read the table
         for b, c in enumerate(cons):
             if b in walked or old is None or old[b] is not c or c is None:
                 tab.set_row(b, c, walked.get(b))
-        if schema:
+        if grammar:
+            self._grammar_key = key
+        elif schema:
             self._schema_key = key
         else:
             self._json_key = key
@@ -1389,7 +1431,11 @@ class DecodeEngine(_GraphEngine):
         keeps its state while its constraint stays the same and starts at the start state otherwise.  With a JSON-mode
         slot (``JsonConstraint``) the step is a graph of its own: the JSON rows' masks, the constrained draw and their
         state advance, with the same rules for ``history``.  With a JSON Schema slot (``JsonSchemaConstraint``) the
-        step is the schema graph kind, which runs the schema rows' (and any JSON rows') masks and advances.
+        step is the schema graph kind, which runs the schema rows' (and any JSON rows') masks and advances.  With a
+        grammar slot (``GrammarConstraint``, DESIGN.md section 23) the step is the grammar graph kind, which runs the
+        grammar rows' (and any JSON and schema rows') masks and advances; ``history`` sets a grammar slot's parse set to
+        the walk of its generated ids, and a slot whose parses went past the parse cap raises ``ValueError`` after the
+        replays.
         ``adapter_ids`` (LoRA engines): one ``AdapterSet`` id per slot as in ``step``, for every graph kind above.
         ``keep_logits=True`` (plain ``sampling``: no penalty, constraint or logprobs) replays the sampled step with one
         more launch that keeps each step's logits rows, and returns ``(tokens, logits [steps, B, V])``, a device view of
@@ -1412,6 +1458,8 @@ class DecodeEngine(_GraphEngine):
             from .sampler import any_constrained, any_penalized
 
             per = None if sampling is None else self._per_slot_sampling(sampling)
+            if per is not None and any(p is not None and p.grammar for p in per):
+                raise ValueError("keep_logits takes plain sampling: no grammar constraint")
             if per is None or logprobs is not None or any_penalized(per) or any_constrained(per):
                 raise ValueError("keep_logits takes plain sampling: no penalties, min-p, constraint or logprobs")
             if any(p is not None and p.controls for p in per):
@@ -1430,6 +1478,8 @@ class DecodeEngine(_GraphEngine):
 
             per = self._per_slot_sampling(sampling)
             penalized, constrained, controlled = any_penalized(per), any_constrained(per), any_controlled(per)
+            if controlled and any(p is not None and p.grammar for p in per):
+                raise ValueError("logits controls take no grammar: no slot may carry a grammar beside a controlled slot")
             if controlled and constrained:
                 raise ValueError("logits controls take no constraint: no slot may carry one beside a controlled slot")
             if controlled:
@@ -1452,7 +1502,20 @@ class DecodeEngine(_GraphEngine):
             self._alloc_penalties()
         json = constrained and any(isinstance(p.constraint, JsonConstraint) for p in per if p is not None)
         schema = constrained and any(isinstance(p.constraint, JsonSchemaConstraint) for p in per if p is not None)
-        if schema:
+        grammar = constrained and any(p.grammar for p in per if p is not None)
+        if grammar:
+            if self._grammar_tab is None:
+                self._grammar_tab = ConstraintRows(B, self.V, self.device, json=json, schema=schema, grammar=True)
+            if json:
+                self._grammar_tab.ensure_json()
+            if schema:
+                self._grammar_tab.ensure_schema()
+            if top_n is not None:
+                self._alloc_logprobs(max(top_n))
+                self._set_top_n(top_n)
+            self._set_json_constraints(self._per_slot_sampling(sampling), history, grammar=True)
+            self._ensure_grammar_graph(penalized, None if top_n is None else max(top_n), self._grammar_tab.has_json, self._grammar_tab.has_schema)
+        elif schema:
             if self._schema_tab is None:
                 self._schema_tab = ConstraintRows(B, self.V, self.device, json=json, schema=True)
             if json:
@@ -1504,8 +1567,8 @@ class DecodeEngine(_GraphEngine):
             self._set_sampling(sampling)
         if penalized:
             self._set_penalties(self._per_slot_sampling(sampling), history)
-        if schema:
-            pass  # the schema table's rows are set above, before its graph is captured, which sizes its masks launch
+        if grammar or schema:
+            pass  # the grammar and schema tables' rows are set above, before their graph is captured, which sizes the masks launches
         elif json:
             self._set_json_constraints(self._per_slot_sampling(sampling), history)
         elif constrained:
@@ -1513,7 +1576,10 @@ class DecodeEngine(_GraphEngine):
         self.meta_np[0:B] = tokens
         self.meta_np[B : 2 * B] = offsets
         self.meta_np[2 * B : 3 * B] = ctx
-        if schema:
+        if grammar:
+            tab = self._grammar_tab
+            graph = self._graph_grammar[(penalized, None if top_n is None else max(top_n), tab.has_json, tab.has_schema)]
+        elif schema:
             graph = self._graph_schema[(penalized, None if top_n is None else max(top_n), self._schema_tab.has_json)]
         elif json:
             graph = self._graph_json[(penalized, None if top_n is None else max(top_n))]
@@ -1543,6 +1609,8 @@ class DecodeEngine(_GraphEngine):
                 graph.replay()
         cur.wait_stream(self._stream)
         self.graph_replays += steps
+        if grammar:
+            self._grammar_tab.check_grammar_rows()
         out = self.out_log[: steps * B].view(steps, B)
         if keep_logits:
             return out, self._logits_log[:steps]
@@ -1659,6 +1727,8 @@ class VerifyEngine(DecodeEngine):
         T = self.T
         spec = sampling is not None
         if spec:
+            if sampling.grammar:
+                raise ValueError("the sampled verify pass takes no grammar constraint")
             if sampling.penalized or sampling.constraint is not None:
                 raise ValueError("the sampled verify pass takes plain sampling: no penalties, min-p or constraint")
             if draft_logits is None or tuple(draft_logits.shape) != (T - 1, self.V) or not draft_logits.is_contiguous():

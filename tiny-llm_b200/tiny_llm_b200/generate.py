@@ -379,6 +379,10 @@ def _check_proposal_length(proposal_length) -> None:
 
 def _spec_sampling(sampling, constraint):
     """The ``SamplingParams`` speculative decoding samples with (None: greedy), refusing what it does not take."""
+    from .grammar import GrammarConstraint
+
+    if isinstance(constraint, GrammarConstraint):
+        raise ValueError("speculative decoding is greedy and unconstrained: it takes no grammar")
     if constraint is not None:
         raise ValueError("speculative decoding is greedy and unconstrained: it takes no constraint")
     if sampling is None:
@@ -387,6 +391,8 @@ def _spec_sampling(sampling, constraint):
 
     if not isinstance(sampling, SamplingParams):
         raise ValueError(f"sampling must be None or a SamplingParams, got {type(sampling).__name__}")
+    if sampling.grammar:
+        raise ValueError("speculative decoding and prompt lookup are unconstrained: sampling must carry no grammar")
     if sampling.constraint is not None:
         raise ValueError("speculative decoding is unconstrained: sampling must carry no constraint")
     if sampling.penalized:

@@ -358,32 +358,37 @@ class JsonConstraint:
 
 # -------------------------------------------------------------------------------------------- per-row tables --
 class ConstraintRows:
-    """The constraint tables of one draw's rows, for any mix of regex, JSON, JSON Schema and unconstrained
+    """The constraint tables of one draw's rows, for any mix of regex, JSON, JSON Schema, grammar and unconstrained
     ``SamplingParams``: ``descriptors`` int64 ``[R, 5]`` ``tl_constraint_row``s and, when a row is in JSON mode,
     ``json_states`` int64 ``[R, 2]`` (zero rows: not JSON), when a row is under a ``JsonSchemaConstraint``,
-    ``schema_states`` int64 ``[R, 10]`` (zero rows: not a schema row), and for either ``json_masks`` int32
+    ``schema_states`` int64 ``[R, 10]`` (zero rows: not a schema row), when a row is under a ``GrammarConstraint``,
+    ``grammar_states`` int64 ``[R, 74]`` (zero rows: not a grammar row), and for any of them ``json_masks`` int32
     ``[R, 2, ceil(V / 32)]`` (row 0 this step's mask, row 1 EOS only).  ``sample`` runs the masks launches,
     ``tl_sample_constrained`` and the advances; regex rows advance inside the draw as before."""
 
-    def __init__(self, rows: int, vocab: int, device, json: bool, schema: bool = False):
+    def __init__(self, rows: int, vocab: int, device, json: bool, schema: bool = False, grammar: bool = False):
         self.rows, self.vocab, self.device = rows, vocab, torch.device(device)
         self.descriptors = torch.zeros((rows, 5), dtype=torch.int64, device=device)
-        self.json_states = self.json_masks = self.schema_states = None
+        self.json_states = self.json_masks = self.schema_states = self.grammar_states = None
         self.schema_smem_bytes = 0  # shared memory of the schema masks launch: the largest schema blob that fits
-        self._json_constraints: list = [None] * rows  # the row's JsonConstraint or JsonSchemaConstraint
+        self.grammar_smem_bytes = 0  # likewise for the grammar masks launch
+        self._json_constraints: list = [None] * rows  # the row's JsonConstraint, JsonSchemaConstraint or GrammarConstraint
         if json:
             self.ensure_json()
         if schema:
             self.ensure_schema()
+        if grammar:
+            self.ensure_grammar()
 
     @classmethod
     def build(cls, params, vocab: int, device) -> ConstraintRows:
         """Rows at their constraints' start states, one per entry of ``params`` (None: unconstrained)."""
+        from .grammar import GrammarConstraint
         from .json_schema import JsonSchemaConstraint
 
         cons = [None if p is None else p.constraint for p in params]
         out = cls(len(cons), vocab, device, any(isinstance(c, JsonConstraint) for c in cons),
-                  any(isinstance(c, JsonSchemaConstraint) for c in cons))
+                  any(isinstance(c, JsonSchemaConstraint) for c in cons), any(isinstance(c, GrammarConstraint) for c in cons))
         for r, c in enumerate(cons):
             out.set_row(r, c)
         return out
@@ -392,7 +397,8 @@ class ConstraintRows:
     def concat(cls, tables: list) -> ConstraintRows:
         """One table of the rows of ``tables`` in order (device copies of their states)."""
         t0 = tables[0]
-        out = cls(sum(t.rows for t in tables), t0.vocab, t0.device, any(t.has_json for t in tables), any(t.has_schema for t in tables))
+        out = cls(sum(t.rows for t in tables), t0.vocab, t0.device, any(t.has_json for t in tables), any(t.has_schema for t in tables),
+                  any(t.has_grammar for t in tables))
         r = 0
         for t in tables:
             for s in range(t.rows):
@@ -407,6 +413,10 @@ class ConstraintRows:
     @property
     def has_schema(self) -> bool:
         return self.schema_states is not None
+
+    @property
+    def has_grammar(self) -> bool:
+        return self.grammar_states is not None
 
     def _ensure_masks(self) -> None:
         if self.json_masks is None:
@@ -424,15 +434,23 @@ class ConstraintRows:
             self.schema_states = torch.zeros((self.rows, SCHEMA_STATE_WORDS), dtype=torch.int64, device=self.device)
             self._ensure_masks()
 
+    def ensure_grammar(self) -> None:
+        from .grammar import GRAMMAR_STATE_WORDS
+
+        if self.grammar_states is None:
+            self.grammar_states = torch.zeros((self.rows, GRAMMAR_STATE_WORDS), dtype=torch.int64, device=self.device)
+            self._ensure_masks()
+
     def _zero_states(self, r: int, keep=None) -> None:
-        for states in (self.json_states, self.schema_states):
+        for states in (self.json_states, self.schema_states, self.grammar_states):
             if states is not None and states is not keep:
                 states[r].zero_()
 
     def set_row(self, r: int, constraint, state=None) -> None:
-        """Row ``r`` under ``constraint`` (None: unconstrained) at ``state`` (a regex state, a ``JsonWalker`` or a
-        ``SchemaWalker``; default the start)."""
+        """Row ``r`` under ``constraint`` (None: unconstrained) at ``state`` (a regex state, a ``JsonWalker``, a
+        ``SchemaWalker`` or a ``GrammarWalker``; default the start)."""
         from .constrained import descriptor_values
+        from .grammar import GrammarConstraint
         from .json_schema import JsonSchemaConstraint
 
         if isinstance(constraint, JsonConstraint):
@@ -450,10 +468,18 @@ class ConstraintRows:
             self.schema_states[r].copy_(torch.tensor(constraint.words(w), dtype=torch.int64))
             self._fit_schema(constraint)
             self.descriptors[r].copy_(torch.tensor(self._json_descriptor(r, constraint, 1 if w.terminal else 0), dtype=torch.int64))
+        elif isinstance(constraint, GrammarConstraint):
+            self.ensure_grammar()
+            self._zero_states(r, keep=self.grammar_states)
+            w = constraint.start() if state is None else state
+            self.json_masks[r, 1].copy_(constraint.eos_row)
+            self.grammar_states[r].copy_(torch.tensor(constraint.words(w), dtype=torch.int64))
+            self._fit_grammar(constraint)
+            self.descriptors[r].copy_(torch.tensor(self._json_descriptor(r, constraint, 1 if w.terminal else 0), dtype=torch.int64))
         else:
             self._zero_states(r)
             self.descriptors[r].copy_(torch.tensor(descriptor_values(constraint, 0 if state is None else state), dtype=torch.int64))
-        self._json_constraints[r] = constraint if isinstance(constraint, (JsonConstraint, JsonSchemaConstraint)) else None
+        self._json_constraints[r] = constraint if isinstance(constraint, (JsonConstraint, JsonSchemaConstraint, GrammarConstraint)) else None
 
     def _fit_schema(self, c) -> None:
         from .json_schema import SCHEMA_SMEM_BYTES
@@ -461,6 +487,13 @@ class ConstraintRows:
         n = int(c.compiled.blob.size)
         if n <= SCHEMA_SMEM_BYTES:
             self.schema_smem_bytes = max(self.schema_smem_bytes, n)
+
+    def _fit_grammar(self, c) -> None:
+        from .grammar import GRAMMAR_SMEM_BYTES
+
+        n = int(c.compiled.blob.size)
+        if n <= GRAMMAR_SMEM_BYTES:
+            self.grammar_smem_bytes = max(self.grammar_smem_bytes, n)
 
     def _json_descriptor(self, r: int, c, state: int) -> list[int]:
         packed = 1 | (state << 32)  # num_states 1, state 0 (or 1, terminal)
@@ -475,10 +508,17 @@ class ConstraintRows:
             self.descriptors[r].copy_(src.descriptors[s])
             self._json_constraints[r] = None
             return
+        from .grammar import GrammarConstraint
+
         if isinstance(c, JsonConstraint):
             self.ensure_json()
             self._zero_states(r, keep=self.json_states)
             self.json_states[r].copy_(src.json_states[s])
+        elif isinstance(c, GrammarConstraint):
+            self.ensure_grammar()
+            self._zero_states(r, keep=self.grammar_states)
+            self.grammar_states[r].copy_(src.grammar_states[s])
+            self._fit_grammar(c)
         else:
             self.ensure_schema()
             self._zero_states(r, keep=self.schema_states)
@@ -495,7 +535,7 @@ class ConstraintRows:
         self._json_constraints[r] = None
 
     def before_draw(self, rows: int | None = None) -> None:
-        """This step's masks of the JSON and schema rows among the first ``rows`` (default all)."""
+        """This step's masks of the JSON, schema and grammar rows among the first ``rows`` (default all)."""
         from extensions_b200 import tiny_llm_ext_b200 as ext
 
         n = self.rows if rows is None else rows
@@ -503,9 +543,12 @@ class ConstraintRows:
             ext.json_token_masks(self.descriptors[:n], self.json_states[:n], self.vocab)
         if self.schema_states is not None:
             ext.schema_token_masks(self.descriptors[:n], self.schema_states[:n], self.vocab, self.schema_smem_bytes)
+        if self.grammar_states is not None:
+            ext.grammar_token_masks(self.descriptors[:n], self.grammar_states[:n], self.vocab, self.grammar_smem_bytes)
 
     def after_draw(self, tokens: torch.Tensor, positions: torch.Tensor) -> None:
-        """Advance the JSON and schema rows by their drawn ``tokens`` (rows with ``positions > 0``)."""
+        """Advance the JSON, schema and grammar rows by their drawn ``tokens`` (rows with ``positions > 0``).  A grammar
+        row whose drawn token was not allowed raises ``ValueError`` (``check_grammar_rows``)."""
         from extensions_b200 import tiny_llm_ext_b200 as ext
 
         n = tokens.shape[0]
@@ -513,19 +556,38 @@ class ConstraintRows:
             ext.json_advance(self.descriptors[:n], self.json_states[:n], tokens, positions)
         if self.schema_states is not None:
             ext.schema_advance(self.descriptors[:n], self.schema_states[:n], tokens, positions)
+        if self.grammar_states is not None:
+            ext.grammar_advance(self.descriptors[:n], self.grammar_states[:n], tokens, positions, self.vocab)
+            self.check_grammar_rows(n)
+
+    def check_grammar_rows(self, rows: int | None = None) -> None:
+        """Raise ``ValueError`` when a grammar row among the first ``rows`` (default all) has its failed bit set: its
+        parses went past the parse cap, no token was allowed and the draw's fallback token left the grammar."""
+        if self.grammar_states is None:
+            return
+        from .grammar import GRAMMAR_MAX_PARSES, failed_rows
+
+        bad = failed_rows(self.grammar_states[: self.rows if rows is None else rows])
+        if bad:
+            raise ValueError(f"grammar: row {bad[0]} has no allowed token: every continuation keeps more than "
+                             f"GRAMMAR_MAX_PARSES = {GRAMMAR_MAX_PARSES} parses live, so the text cannot stay in the grammar")
 
     def walkers(self) -> list:
         """The host mirror of each row's JSON or schema state (None for other rows); one device read per kind."""
+        from .grammar import GrammarConstraint, GrammarWalker
         from .json_schema import SchemaWalker
 
         jw = self.json_states.tolist() if self.json_states is not None else None
         sw = self.schema_states.tolist() if self.schema_states is not None else None
+        gw = self.grammar_states.tolist() if self.grammar_states is not None else None
         out = []
         for r, c in enumerate(self._json_constraints):
             if c is None:
                 out.append(None)
             elif isinstance(c, JsonConstraint):
                 out.append(JsonWalker(jw[r]))
+            elif isinstance(c, GrammarConstraint):
+                out.append(GrammarWalker(c.compiled, gw[r]))
             else:
                 out.append(SchemaWalker(c.compiled, sw[r]))
         return out

@@ -55,7 +55,8 @@ class SamplingParams:
     tokens that keep the text a prefix of the pattern's language (EOS once it is a match); greedy under a constraint is
     ``SamplingParams(0.0, constraint=c)``.  With a mask that allows every token the draw is the unconstrained one.
     A ``JsonConstraint`` (JSON mode, DESIGN.md section 20) restricts the text to one JSON object the same way, and a
-    ``JsonSchemaConstraint`` (DESIGN.md section 21) to one JSON object that validates against a schema.
+    ``JsonSchemaConstraint`` (DESIGN.md section 21) to one JSON object that validates against a schema, and a
+    ``GrammarConstraint`` (DESIGN.md section 23) to the language of a GBNF grammar.
 
     Logits controls (``tl_logit_controls``, DESIGN.md section 22), each off at its default and refused together with a
     ``constraint``: ``logit_bias`` (a mapping token id -> finite bias in [-100, 100], at most 1024 entries) adds its
@@ -111,13 +112,16 @@ class SamplingParams:
             from .constrained import TokenConstraint
             from .json_mode import JsonConstraint
             from .json_schema import JsonSchemaConstraint
+            from .grammar import GrammarConstraint
 
-            if not isinstance(self.constraint, (TokenConstraint, JsonConstraint, JsonSchemaConstraint)):
+            if not isinstance(self.constraint, (TokenConstraint, JsonConstraint, JsonSchemaConstraint, GrammarConstraint)):
                 raise ValueError(f"constraint must be None or a TokenConstraint, got {type(self.constraint).__name__}")
         from .logit_controls import normalized_controls
 
         for name, value in normalized_controls(self).items():
             object.__setattr__(self, name, value)
+        if self.controls and self.grammar:
+            raise ValueError("logit_bias, allowed_token_ids, bad_words_ids and min_tokens take no grammar constraint")
         if self.controls and self.constraint is not None:
             raise ValueError("logit_bias, allowed_token_ids, bad_words_ids and min_tokens take no constraint")
 
@@ -125,6 +129,13 @@ class SamplingParams:
     def controls(self) -> bool:
         """Whether the request needs ``tl_logit_controls``: a logit bias, an allow-list, banned sequences or min_tokens."""
         return self.logit_bias is not None or self.allowed_token_ids is not None or self.bad_words_ids is not None or self.min_tokens > 0
+
+    @property
+    def grammar(self) -> bool:
+        """Whether the request carries a ``GrammarConstraint``."""
+        from .grammar import GrammarConstraint
+
+        return isinstance(self.constraint, GrammarConstraint)
 
     @property
     def penalized(self) -> bool:
@@ -210,8 +221,8 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
     then), which it updates at the drawn tokens of the rows with position > 0.  When a row carries a constraint the
     launch is ``tl_sample_constrained`` over ``constraints`` (int64 ``[rows, 5]`` descriptor rows, required then: the
     constrained rows' ``TokenConstraint.descriptor``, zero rows elsewhere), whose states it advances likewise.
-    ``constraints`` may also be a ``ConstraintRows`` (required for JSON rows): its JSON rows' masks are written before
-    the draw and their states advanced after it.
+    ``constraints`` may also be a ``ConstraintRows`` (required for JSON, schema and grammar rows): those rows' masks are
+    written before the draw and their states advanced after it.
     When a row carries logits controls, ``tl_logit_controls`` first turns every row into its fp32 controlled row
     (uncontrolled rows are copied exactly) over ``controls`` (a ``ControlRows`` of at least ``rows`` rows, required
     then), appending ``tokens`` (the step's input token per row) to its history tails, and the draw runs on those rows.
@@ -246,6 +257,8 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
                 raise ValueError("a JSON-mode SamplingParams needs the request's ConstraintRows")
             if any(p is not None and isinstance(p.constraint, JsonSchemaConstraint) for p in params):
                 raise ValueError("a JSON-schema SamplingParams needs the request's ConstraintRows")
+            if any(p is not None and p.grammar for p in params):
+                raise ValueError("a grammar SamplingParams needs the request's ConstraintRows")
             return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
         constraints.before_draw(len(params))
         tokens = ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints.descriptors[:len(params)], *pen)

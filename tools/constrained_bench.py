@@ -9,8 +9,12 @@
 * JSON Schema's ``tl_schema_token_masks`` per call at 1, 8 and 64 rows under ``SCHEMA`` (11 properties, a nested
   array of objects, an enum, a pattern and a recursive ``$ref``), beside ``tl_json_token_masks`` on the same text in
   the same process, inside a string value and at a value position;
-* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+``, under JSON mode and under ``SCHEMA``, at B = 1
-  and B = 8 on Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one process.
+* the grammar kernel's ``tl_grammar_token_masks`` per call at 1, 8 and 64 rows: the expression grammar (inside a
+  number, at a term), ``JSON_GBNF`` (JSON as a GBNF grammar) beside ``tl_schema_token_masks`` under ``SCHEMA`` and
+  ``tl_json_token_masks`` on the same text, and ``EIGHT`` with eight parses live;
+* ``decode_on_device`` tok/s, sampled against sampled under ``[a-z ]+``, under JSON mode, under ``SCHEMA`` and under the
+  expression grammar, at B = 1 and B = 8 on Qwen3-4B-shaped synthetic weights, context 128 + steps, alternated in one
+  process.
 
   python tools/constrained_bench.py [--out tools_out/constrained_bench.json]
 """
@@ -33,6 +37,7 @@ from sample_bench import card, timed  # noqa: E402
 from tiny_llm_b200 import BatchingKvCache, Qwen3ModelWeek3, SamplingParams  # noqa: E402
 from tiny_llm_b200.constrained import TokenConstraint, TokenVocabulary, compile_dfa  # noqa: E402
 from tiny_llm_b200.engine import DecodeEngine  # noqa: E402
+from tiny_llm_b200.grammar import GRAMMAR_SMEM_BYTES, GrammarConstraint  # noqa: E402
 from tiny_llm_b200.json_mode import ConstraintRows, JsonConstraint, JsonWalker  # noqa: E402
 from tiny_llm_b200.json_schema import SCHEMA_SMEM_BYTES, JsonSchemaConstraint  # noqa: E402
 from tiny_llm_b200.sampler import sampling_tensors  # noqa: E402
@@ -154,11 +159,66 @@ def schema_mask_table(sc, jc) -> dict:
     return out
 
 
-def decode_rates(model, c, jc, sc, B, ctx=128, steps=64, rounds=3) -> dict:
+EXPR = '''root ::= expr
+expr ::= term | term "+" expr
+term ::= num | "(" expr ")"
+num  ::= [0-9]+'''
+JSON_GBNF = r'''root   ::= object
+value  ::= object | array | string | number | "true" | "false" | "null"
+object ::= "{" ws ( string ":" ws value ( "," ws string ":" ws value )* )? "}" ws
+array  ::= "[" ws ( value ( "," ws value )* )? "]" ws
+string ::= "\"" ( [^"\\\x00-\x1F] | "\\" ( ["\\/bfnrt] | "u" [0-9a-fA-F]{4} ) )* "\"" ws
+number ::= "-"? ( "0" | [1-9] [0-9]* ) ( "." [0-9]+ )? ( [eE] [-+]? [0-9]+ )? ws
+ws     ::= [ \t\n]{0,8}'''
+EIGHT = ('root ::= "ab" tail\ntail ::= ' + " | ".join(f"r{k}" for k in range(1, 9)) + "\n"
+         + "\n".join(f'r{k} ::= "x" r{k} "{k}" | "z"' for k in range(1, 9)))
+
+
+def grammar_mask_table(vocab, sc, jc) -> dict:
+    """``tl_grammar_token_masks`` for three grammars, and the schema and JSON-mode kernels on JSON_GBNF's texts."""
+    gs = {"expr": GrammarConstraint(EXPR, vocab, device=DEV), "json_gbnf": GrammarConstraint(JSON_GBNF, vocab, device=DEV),
+          "eight": GrammarConstraint(EIGHT, vocab, device=DEV)}
+    out = {"tables": {k: {"states": g.compiled.num_states, "classes": g.compiled.num_classes, "blob_bytes": int(g.compiled.blob.size),
+                          "staged": bool(g.compiled.blob.size <= GRAMMAR_SMEM_BYTES)} for k, g in gs.items()}}
+    print(f"grammar tables: {out['tables']}", flush=True)
+    cases = [("expr_in_number", "expr", b"(12+(3"), ("expr_at_term", "expr", b"(12+"),
+             ("json_gbnf_in_string", "json_gbnf", b'{"name": "abc'), ("json_gbnf_at_value", "json_gbnf", b'{"name": '),
+             ("eight_parses", "eight", b"abxx")]
+    for rows in (1, 8, 64):
+        res = {}
+        for name, key, text in cases:
+            g = gs[key]
+            w = g.start()
+            assert w.walk(text), text
+            tab = ConstraintRows(rows, V, DEV, json=False, grammar=True)
+            for r in range(rows):
+                tab.set_row(r, g, w)
+            res[f"grammar_{name}"] = timed(lambda: ext.grammar_token_masks(tab.descriptors, tab.grammar_states, V, tab.grammar_smem_bytes))
+            res[f"parses_{name}"] = len(w.parses)
+        for where, text in (("in_string", b'{"name": "abc'), ("at_value", b'{"name": ')):
+            w = sc.start()
+            assert w.walk(text)
+            jw = JsonWalker()
+            jw.walk(text)
+            tab = ConstraintRows(rows, V, DEV, json=False, schema=True)
+            jtab = ConstraintRows(rows, V, DEV, json=True)
+            for r in range(rows):
+                tab.set_row(r, sc, w)
+                jtab.set_row(r, jc, jw)
+            res[f"schema_{where}"] = timed(lambda: ext.schema_token_masks(tab.descriptors, tab.schema_states, V, tab.schema_smem_bytes))
+            res[f"json_{where}"] = timed(lambda: ext.json_token_masks(jtab.descriptors, jtab.json_states, V))
+        out[rows] = res
+        print(f"grammar masks, rows {rows}: " + ", ".join(f"{k} {v:.1f} us" if isinstance(v, float) else f"{k} {v}" for k, v in res.items()),
+              flush=True)
+    return out
+
+
+def decode_rates(model, c, jc, sc, gc, B, ctx=128, steps=64, rounds=3) -> dict:
     modes = {"sampled": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1),
              "constrained": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=c),
              "json": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=jc),
-             "schema": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=sc)}
+             "schema": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=sc),
+             "grammar": SamplingParams(0.7, top_k=50, top_p=0.9, seed=1, constraint=gc)}
     msl = ctx + len(modes) * (rounds + 1) * steps + 64
     engine = DecodeEngine(model, B, msl, DEV)
     engine.reserve_pools()
@@ -183,7 +243,8 @@ def decode_rates(model, c, jc, sc, B, ctx=128, steps=64, rounds=3) -> dict:
                 times[mode].append(a.elapsed_time(b))
     res = {m: B * steps * len(v) / (sum(v) / 1e3) for m, v in times.items()}
     res["kernels_per_step"] = {"sampled": engine.kernels_per_sampled_step, "constrained": engine.kernels_per_constrained_step,
-                               "json": engine.kernels_per_json_step, "schema": engine.kernels_per_schema_step}
+                               "json": engine.kernels_per_json_step, "schema": engine.kernels_per_schema_step,
+                               "grammar": engine.kernels_per_grammar_step}
     for t in tables:  # the next engine reserves its pages from the same pools
         for cc in t.kv_caches:
             if cc is not None:
@@ -191,7 +252,8 @@ def decode_rates(model, c, jc, sc, B, ctx=128, steps=64, rounds=3) -> dict:
     print(f"B {B}: sampled {res['sampled']:.1f} tok/s, constrained {res['constrained']:.1f} tok/s "
           f"({(res['constrained'] / res['sampled'] - 1) * 100:+.2f} %), json {res['json']:.1f} tok/s "
           f"({(res['json'] / res['sampled'] - 1) * 100:+.2f} % against sampled, {(res['json'] / res['constrained'] - 1) * 100:+.2f} % "
-          f"against [a-z ]+), schema {res['schema']:.1f} tok/s ({(res['schema'] / res['json'] - 1) * 100:+.2f} % against json)", flush=True)
+          f"against [a-z ]+), schema {res['schema']:.1f} tok/s ({(res['schema'] / res['json'] - 1) * 100:+.2f} % against json), "
+          f"grammar {res['grammar']:.1f} tok/s ({(res['grammar'] / res['sampled'] - 1) * 100:+.2f} % against sampled)", flush=True)
     return res
 
 
@@ -211,9 +273,11 @@ def main() -> None:
     result["json_masks_us"] = json_mask_table(jc)
     sc = JsonSchemaConstraint(SCHEMA, vocab, device=DEV)
     result["schema_masks_us"] = schema_mask_table(sc, jc)
+    result["grammar_masks_us"] = grammar_mask_table(vocab, sc, jc)
+    gc = GrammarConstraint(EXPR, vocab, device=DEV)
     ns = synthetic_qwen3("qwen3-4b", seed=0, device=DEV)
     model = Qwen3ModelWeek3(ns, page_size=64)
-    result["decode"] = {B: decode_rates(model, c, jc, sc, B) for B in (1, 8)}
+    result["decode"] = {B: decode_rates(model, c, jc, sc, gc, B) for B in (1, 8)}
     if args.out:
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
         Path(args.out).write_text(json.dumps(result, indent=1))
