@@ -305,6 +305,19 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
 int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                         const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                         const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* tl_sample_penalized with XTC (DESIGN.md section 24): xtc_threshold and xtc_probability, per-row f32 device arrays
+ * (both NULL: tl_sample_penalized, bit for bit).  For a row with temperature > 0, a finite maximum and probability q > 0, let K be
+ * the keep set above, e_i = fl(expf(fl(fl(x_i - m) / T)) * 2^40) rounded to an integer for i in K, S their (exact,
+ * integer) sum, and A = {i in K : (double)e_i >= (double)theta * (double)S}.  u = (2 (w >> 9) + 1) 2^-24 with w word
+ * 0 of Philox4x32-10 at counter (0, position, 3, 0) under the seed key (counter word 2 is the stream: 0 the draw,
+ * 1 acceptance, 2 residual, 3 XTC).  When u < q and |A| >= 2, every i in A with x_i > min over A of x leaves K
+ * (ties at that minimum stay), and the draw runs on the smaller set.  |e_i / S - p_i| stays below 2^-20 for the
+ * exact softmax p over K (expf's 2 ulp, the 2^-40 rounding of each term), so A agrees with {p_i >= theta} for every
+ * i whose p_i lies farther than 2^-20 from theta.  Temperature 0 is unaffected. */
+int tl_sample_penalized_xtc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                            const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                            int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
 /* Speculative sampling (DESIGN.md section 8d): the rejection rule over one verify pass of T = k + 1 rows
  * (1 <= T <= 65535, vocab <= TL_SPECULATIVE_SAMPLE_MAX_VOCAB).  target [T, vocab] are the target's logits rows,
  * draft [k, vocab] the draft's rows each proposal proposals[j] (int32, device) was drawn from, the parameters per row
@@ -367,6 +380,12 @@ int tl_sample_constrained(const void *logits, const float *temperature, const in
                           const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                           const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab,
                           int dtype, void *stream);
+/* tl_sample_constrained with xtc_threshold and xtc_probability as tl_sample_penalized_xtc takes them (both NULL, or
+ * both given with the penalty arrays): K, S and A are taken over the allowed entries only. */
+int tl_sample_constrained_xtc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
 /* JSON mode (DESIGN.md section 20): a byte-level pushdown automaton over RFC 8259 `ws object ws`, with at most
  * TL_JSON_MAX_DEPTH open containers and at most TL_JSON_MAX_WS_RUN consecutive whitespace bytes.  A JSON row is a
  * tl_constraint_row with num_states = 1 whose mask is the row's own uint32 [2, ceil(vocab / 32)] buffer (row 0: this
@@ -864,6 +883,38 @@ typedef struct tl_control_row {
  * synchronisation; a row's y does not depend on its index or on the row count.  Out-of-range ids in data are ignored. */
 int tl_logit_controls(const void *logits, const tl_control_row *controls, const int32_t *positions, const int32_t *tokens,
                       int32_t *tails, float *out, int rows, int vocab, int dtype, void *stream);
+
+/* DRY, "don't repeat yourself" (DESIGN.md section 24).  One descriptor per row, in device memory (528 bytes):
+ *   flags           TL_DRY_ON for a DRY row (0: the row is left alone);
+ *   allowed_length  a >= 1, the longest repeat that goes unpenalised;
+ *   last_n          N: the window is h_lo .. h_{n-1}, lo = 0 for N = 0, else max(0, n - N);
+ *   num_breakers    the count of ids in breakers (sorted ascending, at most TL_DRY_MAX_BREAKERS);
+ *   penalty         P[k] = fl32(m b^k) for k = 0 .. TL_DRY_MAX_MATCH - a, computed in double by the host.
+ * TL_DRY_MAX_MATCH caps the match length: at b = 1.75 and m = 1 the penalty passes 10^15 at k = 62 already, so a
+ * longer match changes nothing a sampler could see; the cap bounds a match's reads at 64 ids per end. */
+#define TL_DRY_ON 1
+#define TL_DRY_MAX_MATCH 64
+#define TL_DRY_MAX_BREAKERS 64
+typedef struct tl_dry_row {
+    int32_t flags;
+    int32_t allowed_length;
+    int32_t last_n;
+    int32_t num_breakers;
+    int32_t breakers[TL_DRY_MAX_BREAKERS];
+    float penalty[TL_DRY_MAX_MATCH];
+} tl_dry_row;
+/* The DRY penalty on the fp32 rows x [rows, vocab] (in place; tl_logit_controls' output), one launch, one cluster of
+ * CTAs per row splitting the row's history ends.  For a DRY row with 1 <= n = positions[r] <= capacity the history is
+ * h_0 .. h_{n-2} = history[r, 0 .. n-2] and h_{n-1} = tokens[r] (the step's input token).  Unless h_{n-1} is a breaker,
+ * for every end lo <= e <= n - 2 whose next id t = h_{e+1} is not a breaker, l(e) is the largest l <= TL_DRY_MAX_MATCH
+ * with e - i >= lo, h_{e-i} = h_{n-1-i} and h_{n-1-i} not a breaker for every i < l; l*(t) the maximum over the ends
+ * followed by t.  Every t with l*(t) >= a becomes fl32(x_t - P[l*(t) - a]), or -inf when that P is +inf (NaN stays).
+ * The launch then writes history[r, n - 1] = tokens[r].  Rows at position 0 (idle slots, capture warm-ups), rows past
+ * capacity and rows with flags 0 are left alone.  scratch (fp32 [rows, capacity]) holds each end's candidate between
+ * the read and the write phases; every candidate is computed from the unpenalised row and the row keeps the least of
+ * them, so the result is deterministic.  No host synchronisation. */
+int tl_dry_penalty(float *x, const tl_dry_row *dry, const int32_t *positions, const int32_t *tokens, int32_t *history, float *scratch,
+                   int rows, int vocab, int capacity, void *stream);
 
 #ifdef __cplusplus
 }

@@ -44,6 +44,7 @@ SOURCES = [
     "json_schema.cu",
     "grammar.cu",
     "logit_controls.cu",
+    "dry.cu",
     "moe.cu",
     "moe_router.cu",
     "lora.cu",

@@ -546,6 +546,14 @@ int tl_sample(const void *logits, const float *temperature, const int32_t *top_k
 int tl_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                         const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                         const float *min_p, int32_t *state, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
+    return tl_sample_penalized_xtc(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, nullptr,
+                                   nullptr, out_tokens, rows, vocab, dtype, stream);
+}
+
+int tl_sample_penalized_xtc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                            const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                            int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_penalized: expected float32, float16, or bfloat16");
     if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_penalized: bad shape");
     if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
@@ -553,14 +561,23 @@ int tl_sample_penalized(const void *logits, const float *temperature, const int3
     if (!logits || !temperature || !top_k || !top_p || !seed || !positions || !repetition || !presence || !frequency || !min_p || !state ||
         !out_tokens)
         return fail(TL_EINVAL, "sample_penalized: null pointer");
+    if (!xtc_threshold != !xtc_probability) return fail(TL_EINVAL, "sample_penalized: give both XTC arrays or neither");
     return launch_sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
-                                   out_tokens, rows, vocab, dtype, as_stream(stream));
+                                   xtc_threshold, xtc_probability, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
 int tl_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                           const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                           const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab,
                           int dtype, void *stream) {
+    return tl_sample_constrained_xtc(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
+                                     nullptr, nullptr, constraints, out_tokens, rows, vocab, dtype, stream);
+}
+
+int tl_sample_constrained_xtc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_constrained: expected float32, float16, or bfloat16");
     if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_constrained: bad shape");
     if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
@@ -569,8 +586,10 @@ int tl_sample_constrained(const void *logits, const float *temperature, const in
         return fail(TL_EINVAL, "sample_constrained: null pointer");
     const int given = !!repetition + !!presence + !!frequency + !!min_p + !!state;
     if (given != 0 && given != 5) return fail(TL_EINVAL, "sample_constrained: give every penalty array and the state, or none");
+    if (!xtc_threshold != !xtc_probability || (xtc_threshold && !state))
+        return fail(TL_EINVAL, "sample_constrained: give both XTC arrays, with the penalty arrays, or neither");
     return launch_sample_constrained(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
-                                     constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
+                                     xtc_threshold, xtc_probability, constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
 int tl_speculative_sample(const void *target, const void *draft, const int32_t *proposals, const float *temperature,
@@ -688,6 +707,14 @@ int tl_logit_controls(const void *logits, const tl_control_row *controls, const 
     if (rows == 0) return TL_OK;
     if (!logits || !controls || !positions || !tokens || !tails || !out) return fail(TL_EINVAL, "logit_controls: null pointer");
     return launch_logit_controls(logits, controls, positions, tokens, tails, out, rows, vocab, dtype, as_stream(stream));
+}
+
+int tl_dry_penalty(float *x, const tl_dry_row *dry, const int32_t *positions, const int32_t *tokens, int32_t *history, float *scratch,
+                   int rows, int vocab, int capacity, void *stream) {
+    if (rows < 0 || rows > 65535 || vocab <= 0 || capacity <= 0) return fail(TL_EINVAL, "dry_penalty: bad shape");
+    if (rows == 0) return TL_OK;
+    if (!x || !dry || !positions || !tokens || !history || !scratch) return fail(TL_EINVAL, "dry_penalty: null pointer");
+    return launch_dry_penalty(x, dry, positions, tokens, history, scratch, rows, vocab, capacity, as_stream(stream));
 }
 
 int tl_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *target_lp,

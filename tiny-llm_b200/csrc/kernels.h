@@ -44,11 +44,12 @@ int launch_sample(const void *logits, const float *temperature, const int32_t *t
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                            const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability, int32_t *out,
+                            int rows, int vocab, int dtype, cudaStream_t st);
 int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                              const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype,
-                              cudaStream_t st);
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
 // constrained.cu
 int launch_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                                   const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks,
@@ -70,6 +71,9 @@ int launch_grammar_advance(const tl_constraint_row *constraints, int64_t *states
 // logit_controls.cu
 int launch_logit_controls(const void *logits, const tl_control_row *controls, const int32_t *positions, const int32_t *tokens,
                           int32_t *tails, float *out, int rows, int vocab, int dtype, cudaStream_t st);
+// dry.cu
+int launch_dry_penalty(float *x, const tl_dry_row *dry, const int32_t *positions, const int32_t *tokens, int32_t *history, float *scratch,
+                       int rows, int vocab, int capacity, cudaStream_t st);
 // logprobs.cu: same cluster plan as sampling.cu
 constexpr int LOGPROBS_MAX_N = TL_LOGPROBS_MAX_N;
 int launch_logprobs(const void *logits, const int32_t *targets, const int32_t *top_n, const int32_t *out_index, float *lse, float *lp,

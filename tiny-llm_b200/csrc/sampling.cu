@@ -30,6 +30,12 @@
 // the wait.  For a row with a mask, the staged entries of disallowed tokens become NaN after the penalty rewrite:
 // NaN entries are never counted, weighed, kept or drawn, so every later step runs on the allowed entries alone.  Rank 0
 // walks the drawn token's bytes through the DFA and writes the row's new state, for rows with position > 0.
+//
+// The XTC forms (XTC, DESIGN.md section 24) add one step after the keep threshold: with probability q, drawn from
+// Philox stream 3 at the row's position, the kept entries whose share of the kept mass is at least theta, all but the
+// least likely of them, become NaN when there are two or more.  Two integer passes over the staged slice (the kept
+// mass, then the count and minimum key of the entries at or above theta's share) decide it, so every CTA of the
+// cluster drops the same entries.
 #include <cooperative_groups.h>
 
 #include <climits>
@@ -49,6 +55,11 @@ struct Penalties {
     const float *repetition, *presence, *frequency, *min_p;
     int32_t *state;
     int svec;  // the state rows are 16-byte aligned (vocab % 4 == 0 and an aligned base)
+};
+
+// Per-row arrays of the XTC forms.  Unused (all null) by the others.
+struct Xtc {
+    const float *threshold, *probability;
 };
 
 constexpr int32_t STATE_PROMPT = 1 << 30;
@@ -86,12 +97,12 @@ __device__ __forceinline__ int constraint_lowest(const tl_constraint_row &c, int
     return 0;
 }
 
-template <typename T, int LEVELS, bool PEN, bool MASK>
+template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restrict__ logits, const float *__restrict__ temperature,
                                                                 const int32_t *__restrict__ top_k, const float *__restrict__ top_p,
                                                                 const int64_t *__restrict__ seed, const int32_t *__restrict__ positions,
                                                                 int32_t *__restrict__ out, int vocab, int slice, int vec, Penalties pen,
-                                                                tl_constraint_row *con) {
+                                                                tl_constraint_row *con, Xtc xtc) {
     extern __shared__ float4 smem_dyn[];
     float *xs = reinterpret_cast<float *>(smem_dyn);
     __shared__ unsigned int h_count[2][BINS];  // double-buffered: level l + 2 reuses l's buffer after all remote reads of it
@@ -210,6 +221,55 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     const uint32_t pos = static_cast<uint32_t>(positions[row]);
     const uint64_t sd = static_cast<uint64_t>(seed[row]);
     const uint32_t k0 = static_cast<uint32_t>(sd), k1 = static_cast<uint32_t>(sd >> 32);
+    if constexpr (XTC) {
+        __shared__ unsigned long long x_mass;
+        __shared__ unsigned int x_count, x_min, x_hi;
+        const uint4 w = philox4x32_10(make_uint4(0u, pos, 3u, 0u), k0, k1);
+        const float u = static_cast<float>(2u * (w.x >> 9) + 1u) * 5.9604644775390625e-8f;
+        if (u < xtc.probability[row]) {  // the same decision in every CTA of the cluster
+            if (threadIdx.x == 0) x_mass = 0, x_count = 0, x_min = UINT_MAX;
+            __syncthreads();
+            // e_i = exp((x_i - m) / T) in 2^-40 fixed point: integer sums, exact in any order
+            unsigned long long s = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v && order_key(v) >= tau) s += __float2ull_rn(expf(__fdiv_rn(__fsub_rn(v, m), temp)) * MASS_SCALE);
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == 0 && s) atomicAdd(&x_mass, s);
+            cluster.sync();
+            unsigned long long total = 0;
+            for (int r = 0; r < C; ++r) total += *cluster.map_shared_rank(&x_mass, r);
+            const double thr = static_cast<double>(xtc.threshold[row]) * static_cast<double>(total);
+            unsigned int c = 0, lowest = UINT_MAX;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v && order_key(v) >= tau &&
+                    static_cast<double>(__float2ull_rn(expf(__fdiv_rn(__fsub_rn(v, m), temp)) * MASS_SCALE)) >= thr)
+                    ++c, lowest = min(lowest, order_key(v));
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                c += __shfl_xor_sync(0xffffffffu, c, o);
+                lowest = min(lowest, __shfl_xor_sync(0xffffffffu, lowest, o));
+            }
+            if (lane == 0 && c) atomicAdd(&x_count, c), atomicMin(&x_min, lowest);
+            cluster.sync();
+            if (threadIdx.x == 0) {
+                unsigned int cnt = 0, lo = UINT_MAX;
+                for (int r = 0; r < C; ++r) cnt += *cluster.map_shared_rank(&x_count, r), lo = min(lo, *cluster.map_shared_rank(&x_min, r));
+                x_hi = cnt >= 2 ? lo : UINT_MAX;  // ties at the least likely value stay
+            }
+            __syncthreads();
+            const uint32_t hi = x_hi;
+            if (hi != UINT_MAX) {
+                for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS)
+                    if (xs[i] == xs[i] && order_key(xs[i]) > hi) xs[i] = NAN;
+                __syncthreads();
+            }
+        }
+    }
     mine = Best{-INFINITY, INT_MAX};
     TL_ROW_GUMBEL_PASS(0u);
     mine = warp_best(mine);
@@ -235,13 +295,13 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     cluster.sync();
 }
 
-template <typename T, int LEVELS, bool PEN, bool MASK>
+template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC>
 int launch_sample_t(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                     const int32_t *positions, int32_t *out, int rows, int vocab, int cluster, int slice, int vec, const Penalties &pen,
-                    tl_constraint_row *con, cudaStream_t st) {
+                    tl_constraint_row *con, const Xtc &xtc, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
+        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN, MASK, XTC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
             return fail(TL_ECUDA, "sample: cannot raise shared memory limit");
         configured = true;
     }
@@ -261,16 +321,16 @@ int launch_sample_t(const void *logits, const float *temperature, const int32_t 
     cfg.numAttrs = use_pdl() ? 2 : 1;
     const T *x = static_cast<const T *>(logits);
     cudaError_t e =
-        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN, MASK>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen, con);
+        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN, MASK, XTC>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen, con, xtc);
     if (e != cudaSuccess) return fail(TL_ECUDA, "sample: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("sample");
     return TL_OK;
 }
 
-template <bool PEN, bool MASK>
+template <bool PEN, bool MASK, bool XTC = false>
 int launch_sample_any(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                       const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, const Penalties &pen, tl_constraint_row *con,
-                      cudaStream_t st) {
+                      cudaStream_t st, const Xtc &xtc = Xtc{}) {
     if (rows == 0) return TL_OK;
     int cluster = 0, slice = 0;
     if (int e = sample_plan(vocab, &cluster, &slice)) return e;
@@ -278,16 +338,16 @@ int launch_sample_any(const void *logits, const float *temperature, const int32_
     const int vec = (vocab % per16 == 0 && aligned16(logits)) ? 1 : 0;
     switch (dtype) {
         case TL_F32:
-            return launch_sample_t<float, 4, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice, vec,
-                                                        pen, con, st);
+            return launch_sample_t<float, 4, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
+                                                             vec, pen, con, xtc, st);
         case TL_F16:
-            return launch_sample_t<__half, 4, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
-                                                         vec, pen, con, st);
+            return launch_sample_t<__half, 4, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
+                                                              slice, vec, pen, con, xtc, st);
         case TL_BF16:  // a raw bf16 value's key has 16 significant bits: two levels.  A penalty rewrites the staged values
                        // (x / r, x * r, x - f c, x - pres) into arbitrary fp32 values: four levels, or tau would stop
                        // at a 16-bit prefix and keep every entry of its bucket below x_(k) or v*
-            return launch_sample_t<__nv_bfloat16, PEN ? 4 : 2, PEN, MASK>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
-                                                                 slice, vec, pen, con, st);
+            return launch_sample_t<__nv_bfloat16, PEN ? 4 : 2, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab,
+                                                                      cluster, slice, vec, pen, con, xtc, st);
         default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
     }
 }
@@ -312,19 +372,26 @@ int launch_sample(const void *logits, const float *temperature, const int32_t *t
 
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                            const float *min_p, int32_t *state, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability, int32_t *out,
+                            int rows, int vocab, int dtype, cudaStream_t st) {
     const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    if (xtc_threshold)
+        return launch_sample_any<true, false, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, nullptr, st,
+                                                    Xtc{xtc_threshold, xtc_probability});
     return launch_sample_any<true, false>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, nullptr, st);
 }
 
 int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                              const float *min_p, int32_t *state, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype,
-                              cudaStream_t st) {
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
     if (!state)
         return launch_sample_any<false, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{},
                                               constraints, st);
     const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    if (xtc_threshold)
+        return launch_sample_any<true, true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, constraints,
+                                                   st, Xtc{xtc_threshold, xtc_probability});
     return launch_sample_any<true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, constraints, st);
 }
 

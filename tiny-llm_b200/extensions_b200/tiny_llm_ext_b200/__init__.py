@@ -51,6 +51,8 @@ __all__ = [
     "logit_controls",
     "CONTROL_ROW_WORDS",
     "CONTROL_TAIL",
+    "dry_penalty",
+    "DRY_ROW_WORDS",
     "speculative_sample",
     "SPECULATIVE_SAMPLE_MAX_VOCAB",
     "log_rows",
@@ -152,7 +154,10 @@ _SIGNATURES = {
     "tl_beam_select": (_I, [_VP] * 3 + [_I] * 3 + [_VP, _I, _VP, _VP]),
     "tl_sample_penalized": (_I, [_VP] * 12 + [_I] * 3 + [_VP]),
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
+    "tl_sample_penalized_xtc": (_I, [_VP] * 14 + [_I] * 3 + [_VP]),
+    "tl_sample_constrained_xtc": (_I, [_VP] * 15 + [_I] * 3 + [_VP]),
     "tl_logit_controls": (_I, [_VP] * 6 + [_I] * 3 + [_VP]),
+    "tl_dry_penalty": (_I, [_VP] * 6 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
     "tl_json_token_masks": (_I, [_VP, _VP, _I, _I, _VP]),
     "tl_json_advance": (_I, [_VP] * 4 + [_I, _VP]),
@@ -975,11 +980,27 @@ def beam_select(top_lp, top_ids, cum, num_beams, eos_ids, out, stream=None):
     return out
 
 
-def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None):
+def _xtc_arrays(op, rows, xtc_threshold, xtc_probability):
+    """The XTC pointers (None, None) or both arrays checked as float32 [rows]."""
+    if xtc_threshold is None and xtc_probability is None:
+        return None, None
+    if xtc_threshold is None or xtc_probability is None:
+        raise RuntimeError(f"{op}: give both XTC arrays or neither")
+    for name, t in (("xtc_threshold", xtc_threshold), ("xtc_probability", xtc_probability)):
+        if t.dtype != torch.float32 or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"{op}: {name} must be float32 [{rows}]")
+    _contig(op, xtc_threshold=xtc_threshold, xtc_probability=xtc_probability)
+    _gpu(op, xtc_threshold, xtc_probability)
+    return xtc_threshold.data_ptr(), xtc_probability.data_ptr()
+
+
+def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None,
+                     xtc_threshold=None, xtc_probability=None):
     """``sample`` with token-history penalties and min-p (``tl_sample_penalized``) -> int32 ``[rows]``.  Further
     per-row device arrays: ``repetition``, ``presence``, ``frequency`` and ``min_p`` float32 ``[rows]``, and ``state``
     int32 ``[rows, vocab]`` (bit 30: token in the prompt, bits 0-29: times drawn), read, and for rows with
-    ``positions > 0`` incremented at the drawn token."""
+    ``positions > 0`` incremented at the drawn token.  ``xtc_threshold`` and ``xtc_probability`` (float32 ``[rows]``,
+    both or neither) add XTC (DESIGN.md section 24)."""
     if logits.dtype not in _FLOATS or logits.dim() != 2:
         raise RuntimeError("sample_penalized: expected 2D float logits")
     rows, vocab = logits.shape
@@ -994,10 +1015,12 @@ def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetit
                  presence=presence, frequency=frequency, min_p=min_p, state=state)
     _contig("sample_penalized", **named)
     _gpu("sample_penalized", *named.values())
+    xtc = _xtc_arrays("sample_penalized", rows, xtc_threshold, xtc_probability)
     out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
-    _check(_lib.tl_sample_penalized(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
-                                    positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(), min_p.data_ptr(),
-                                    state.data_ptr(), out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+    _check(_lib.tl_sample_penalized_xtc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                        positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(),
+                                        min_p.data_ptr(), state.data_ptr(), *xtc, out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype],
+                                        _stream_ptr(stream, logits)))
     return out
 
 
@@ -1005,11 +1028,12 @@ CONSTRAINT_ROW_WORDS = 5  # int64 words of one tl_constraint_row (40 bytes)
 
 
 def sample_constrained(logits, temperature, top_k, top_p, seed, positions, constraints, repetition=None, presence=None, frequency=None,
-                       min_p=None, state=None, stream=None):
+                       min_p=None, state=None, stream=None, xtc_threshold=None, xtc_probability=None):
     """``sample`` (no penalty arrays) or ``sample_penalized`` (all of them) restricted per row to the tokens of its
     constraint (``tl_sample_constrained``) -> int32 ``[rows]``.  ``constraints`` int64 ``[rows, 5]``: one
     ``tl_constraint_row`` per row (all zero: unconstrained), whose state the launch advances for rows with
-    ``positions > 0``."""
+    ``positions > 0``.  ``xtc_threshold`` and ``xtc_probability`` as ``sample_penalized`` takes them, with the penalty
+    arrays."""
     if logits.dtype not in _FLOATS or logits.dim() != 2:
         raise RuntimeError("sample_constrained: expected 2D float logits")
     rows, vocab = logits.shape
@@ -1033,10 +1057,13 @@ def sample_constrained(logits, temperature, top_k, top_p, seed, positions, const
         named.update(repetition=repetition, presence=presence, frequency=frequency, min_p=min_p, state=state)
     _contig("sample_constrained", **named)
     _gpu("sample_constrained", *named.values())
+    xtc = _xtc_arrays("sample_constrained", rows, xtc_threshold, xtc_probability)
+    if xtc[0] is not None and state is None:
+        raise RuntimeError("sample_constrained: XTC needs the penalty arrays and the state")
     out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
     ptr = [None if t is None else t.data_ptr() for t in pen]
-    _check(_lib.tl_sample_constrained(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
-                                      positions.data_ptr(), *ptr, constraints.data_ptr(), out.data_ptr(), rows, vocab,
+    _check(_lib.tl_sample_constrained_xtc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                          positions.data_ptr(), *ptr, *xtc, constraints.data_ptr(), out.data_ptr(), rows, vocab,
                                       _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
 
@@ -1069,6 +1096,34 @@ def logit_controls(logits, controls, positions, tokens, tails, out=None, stream=
     _check(_lib.tl_logit_controls(logits.data_ptr(), controls.data_ptr(), positions.data_ptr(), tokens.data_ptr(), tails.data_ptr(),
                                   out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
     return out
+
+
+DRY_ROW_WORDS = 4 + 64 + 64  # int32 words of one tl_dry_row (flags .. num_breakers, breakers, penalty table)
+
+
+def dry_penalty(x, dry, positions, tokens, history, scratch, stream=None):
+    """The DRY penalty (``tl_dry_penalty``, DESIGN.md section 24) applied in place to the fp32 rows ``x [rows, vocab]``
+    -> ``x``.  ``dry`` int32 ``[rows, DRY_ROW_WORDS]``: one ``tl_dry_row`` per row (all zero: left alone);
+    ``positions`` int32 ``[rows]``, the index of the token drawn next (the history length n); ``tokens`` int32
+    ``[rows]``, the step's input token h_{n-1}; ``history`` int32 ``[rows, capacity]``, whose entries 0 .. n-2 are
+    read and entry n-1 written with the input token; ``scratch`` float32 ``[rows, capacity]``."""
+    if x.dtype != torch.float32 or x.dim() != 2:
+        raise RuntimeError("dry_penalty: x must be 2D float32")
+    rows, vocab = x.shape
+    if dry.dtype != torch.int32 or tuple(dry.shape) != (rows, DRY_ROW_WORDS):
+        raise RuntimeError(f"dry_penalty: dry must be int32 [{rows}, {DRY_ROW_WORDS}]")
+    _int32("dry_penalty", rows, positions=positions, tokens=tokens)
+    if history.dtype != torch.int32 or history.dim() != 2 or history.shape[0] != rows or history.shape[1] < 1:
+        raise RuntimeError(f"dry_penalty: history must be int32 [{rows}, capacity]")
+    capacity = history.shape[1]
+    if scratch.dtype != torch.float32 or tuple(scratch.shape) != (rows, capacity):
+        raise RuntimeError(f"dry_penalty: scratch must be float32 [{rows}, {capacity}]")
+    named = dict(x=x, dry=dry, positions=positions, tokens=tokens, history=history, scratch=scratch)
+    _contig("dry_penalty", **named)
+    _gpu("dry_penalty", *named.values())
+    _check(_lib.tl_dry_penalty(x.data_ptr(), dry.data_ptr(), positions.data_ptr(), tokens.data_ptr(), history.data_ptr(), scratch.data_ptr(),
+                               rows, vocab, capacity, _stream_ptr(stream, x)))
+    return x
 
 
 JSON_STATE_WORDS = 2  # int64 words of one JSON row's automaton state (include/tiny_llm_b200.h)

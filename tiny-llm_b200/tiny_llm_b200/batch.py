@@ -155,7 +155,7 @@ class Request:
                         self.constraint_row = ConstraintRows.build([self.sampling], logits.shape[-1], logits.device)
                     controls = None
                     if self.sampling.controls:
-                        controls = ControlRows(1, logits.shape[-1], logits.device)
+                        controls = ControlRows(1, logits.shape[-1], logits.device, history_capacity=total)
                         controls.set_row(0, self.sampling, self.prompt_list, (), () if self.eos_token_id is None else (self.eos_token_id,))
                     token = sample_tokens(logits, [self.sampling], [total], state, self.constraint_row, controls, self.prefill_tokens[-1:])
                 if self.logprobs is not None:
@@ -381,7 +381,8 @@ class ContinuousBatcher:
         if self.control_rows is None:
             if not controlled:
                 return
-            self.control_rows = ControlRows(self.batch_size, self.model.vocab_size, request.prefill_tokens.device)
+            self.control_rows = ControlRows(self.batch_size, self.model.vocab_size, request.prefill_tokens.device,
+                                            history_capacity=self.max_seq_len + 1)
         if controlled:
             eos = () if request.eos_token_id is None else (request.eos_token_id,)
             self.control_rows.set_row(slot, request.sampling, request.prompt_list, [request.next_token], eos)

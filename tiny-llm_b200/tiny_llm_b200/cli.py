@@ -13,6 +13,8 @@ see checkpoint.py; there is no hub download here).
         (token-history penalties and min-p; with --sampler-temp 0 the greedy token of the penalised logits)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --logit-bias 42:5 --bad-words "7,8;9"
         (logits controls: a per-token bias, banned sequences; also --allowed-token-ids and --min-tokens)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --sampler-temp 0.8 --dry-multiplier 0.8 --xtc-probability 0.5
+        (DRY penalises tokens that extend a verbatim repeat; XTC drops the most likely choices with a seeded probability)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3 --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
@@ -50,6 +52,7 @@ see checkpoint.py; there is no hub download here).
 from __future__ import annotations
 
 import argparse
+import json
 import sys
 from pathlib import Path
 
@@ -204,6 +207,52 @@ def parse_controls(logit_bias=None, allowed_token_ids=None, bad_words=None, min_
     return out
 
 
+def parse_dry_xtc(dry_multiplier=0.0, dry_base=1.75, dry_allowed_length=2, dry_penalty_last_n=0, dry_sequence_breakers=None,
+                  xtc_threshold=0.1, xtc_probability=0.0, tokenizer=None) -> dict:
+    """The ``SamplingParams`` DRY and XTC fields of the flags (an empty dict when both samplers are off).
+    ``--dry-sequence-breakers`` is either ids (``"13,198"``) or a JSON list of strings (``'["\\n", ":"]'``); a string
+    becomes the last id of the tokenizer's encoding of ``"a" + s`` (text-generation-webui's rule), so it needs a
+    tokenizer.  Malformed values raise ``ValueError``."""
+    out = {}
+    if dry_multiplier:
+        out.update(dry_multiplier=dry_multiplier, dry_base=dry_base, dry_allowed_length=dry_allowed_length,
+                   dry_penalty_last_n=dry_penalty_last_n)
+        if dry_sequence_breakers:
+            text = dry_sequence_breakers.strip()
+            if text.startswith("["):
+                try:
+                    strings = json.loads(text)
+                except json.JSONDecodeError:
+                    raise ValueError("--dry-sequence-breakers must be ids ID,ID or a JSON list of strings") from None
+                if not isinstance(strings, list) or not all(isinstance(s, str) and s for s in strings):
+                    raise ValueError("--dry-sequence-breakers must be ids ID,ID or a JSON list of strings")
+                if strings and tokenizer is None:
+                    raise ValueError("--dry-sequence-breakers strings need a tokenizer: give ids with --synthetic")
+                ids = []
+                for s in strings:
+                    enc = tokenizer.encode("a" + s, add_special_tokens=False)
+                    if enc:
+                        ids.append(int(enc[-1]))
+                out["dry_sequence_breakers"] = ids
+            else:
+                try:
+                    out["dry_sequence_breakers"] = [int(t) for t in text.split(",") if t.strip()]
+                except ValueError:
+                    raise ValueError("--dry-sequence-breakers must be ids ID,ID or a JSON list of strings") from None
+    if xtc_probability:
+        out.update(xtc_probability=xtc_probability, xtc_threshold=xtc_threshold)
+    return out
+
+
+def _dry_xtc(args, tokenizer) -> dict:
+    """The DRY and XTC fields of ``--dry-*`` and ``--xtc-*``."""
+    try:
+        return parse_dry_xtc(args.dry_multiplier, args.dry_base, args.dry_allowed_length, args.dry_penalty_last_n,
+                             args.dry_sequence_breakers, args.xtc_threshold, args.xtc_probability, tokenizer)
+    except ValueError as exc:
+        raise SystemExit(str(exc)) from None
+
+
 def _controls(args) -> dict:
     """The logits-control fields of ``--logit-bias``, ``--allowed-token-ids``, ``--bad-words`` and ``--min-tokens``."""
     try:
@@ -297,6 +346,9 @@ def cmd_generate(args) -> int:
     sampler = sampling = None
     penalties = _penalties(args)
     controls = _controls(args)
+    dry_xtc = _dry_xtc(args, tokenizer)
+    if dry_xtc and (args.num_beams is not None or args.num_samples is not None):
+        raise SystemExit("beam search and parallel sampling take no --dry-multiplier or --xtc-probability")
     if controls and (args.num_beams is not None or args.num_samples is not None):
         raise SystemExit("beam search and parallel sampling take no --logit-bias, --allowed-token-ids, --bad-words or --min-tokens")
     if args.num_beams is not None:
@@ -317,6 +369,8 @@ def cmd_generate(args) -> int:
         raise SystemExit("speculative decoding is greedy and unconstrained: drop --json-schema")
     if speculative and args.grammar is not None:
         raise SystemExit("speculative decoding and prompt lookup are greedy and unconstrained: drop --grammar")
+    if speculative and dry_xtc:
+        raise SystemExit("speculative decoding and prompt lookup take no --dry-multiplier or --xtc-probability")
     if speculative and controls:
         raise SystemExit("speculative decoding takes no --logit-bias, --allowed-token-ids, --bad-words or --min-tokens")
     if controls and args.grammar is not None:
@@ -327,6 +381,7 @@ def cmd_generate(args) -> int:
             raise SystemExit("--logit-bias, --allowed-token-ids, --bad-words and --min-tokens take no --regex, --json or --json-schema")
         penalties["constraint"] = constraint
     penalties.update(controls)
+    penalties.update(dry_xtc)
     if args.sampler_temp != 0 or penalties:
         if device.type == "cuda" or penalties or speculative:  # the seeded kernel
             try:
@@ -493,6 +548,7 @@ def cmd_batch(args) -> int:
             raise SystemExit("--logit-bias, --allowed-token-ids, --bad-words and --min-tokens take no --regex, --json or --json-schema")
         penalties["constraint"] = constraint
     penalties.update(controls)
+    penalties.update(_dry_xtc(args, tokenizer))
     if args.sampler_temp != 0 or penalties:  # request i draws with seed `--seed + i`
         try:
             sampling = [SamplingParams(args.sampler_temp, top_k=args.sampler_top_k, top_p=args.sampler_top_p, seed=args.seed + i, **penalties)
@@ -697,6 +753,17 @@ def main(argv=None) -> int:
                                        help="never complete these token sequences (split by ';'); a single id is banned outright")
         sub.choices[name].add_argument("--min-tokens", type=int, default=0, metavar="N",
                                        help="hold back EOS until N tokens have been generated")
+        sub.choices[name].add_argument("--dry-multiplier", type=float, default=0.0,
+                                       help="DRY: penalise tokens that extend a verbatim repeat of the history (0: off)")
+        sub.choices[name].add_argument("--dry-base", type=float, default=1.75, help="DRY: the penalty's growth per repeated token (> 1)")
+        sub.choices[name].add_argument("--dry-allowed-length", type=int, default=2, help="DRY: the longest repeat left alone (>= 1)")
+        sub.choices[name].add_argument("--dry-penalty-last-n", type=int, default=0, help="DRY: the window of recent tokens (0: all)")
+        sub.choices[name].add_argument("--dry-sequence-breakers", default=None, metavar="ID,ID or JSON",
+                                       help='DRY: ids, or a JSON list of strings such as \'["\\n", ":"]\', that no repeat runs through')
+        sub.choices[name].add_argument("--xtc-threshold", type=float, default=0.1,
+                                       help="XTC: tokens at least this likely are the top choices (in (0, 1])")
+        sub.choices[name].add_argument("--xtc-probability", type=float, default=0.0,
+                                       help="XTC: the chance per draw of excluding all top choices but the least likely (0: off)")
         sub.choices[name].add_argument("--regex", default=None, metavar="PATTERN",
                                        help="constrain the generated text to fullmatch PATTERN (re.ASCII semantics over UTF-8 bytes)")
         sub.choices[name].add_argument("--json", action="store_true",

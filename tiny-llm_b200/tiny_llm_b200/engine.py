@@ -47,6 +47,10 @@ from .paged_kv_cache import TinyKvPagedCache
 # Decode attention runs as one fused launch while slots x max_seq_len stays within this: beyond it the K/V stream, not
 # the launch count, bounds the step.
 FUSED_ATTENTION_MAX_SLOT_TOKENS = 16384
+# decode_on_device's graph-kind flags beyond True: ``penalized == XTC`` draws with XTC (DESIGN.md section 24),
+# ``controlled == DRY`` adds one tl_dry_penalty launch after tl_logit_controls
+XTC = "xtc"
+DRY = "dry"
 
 # Grouped decode attention (tl_shared_prefix_attention, DESIGN.md section 16) replaces the step's attention for a group
 # of COUNT slots sharing SHARED_TOKENS prompt tokens only where tools/parallel_sample_bench.py measured it faster.
@@ -426,9 +430,10 @@ class DecodeEngine(_GraphEngine):
         self._lp_key = None
         self.kernels_per_logprobs_step = 0
         # decode_on_device(sampling=<penalised>): the penalised sampled graph, the per-slot token state [B, V] it reads and
-        # counts into, and the penalty parameters in their own pinned block (repetition | presence | frequency | min_p
-        # f32, B each), all on first use
+        # counts into, and the penalty parameters in their own pinned block (repetition | presence | frequency | min_p |
+        # xtc_threshold | xtc_probability, f32, B each), all on first use; the XTC twin (penalized == XTC) likewise
         self._graph_pen = None
+        self._graph_pen_xtc = None
         self.kernels_per_penalized_step = 0
         self.token_counts = None
         self._pen_host = None
@@ -467,7 +472,7 @@ class DecodeEngine(_GraphEngine):
         self.kernels_per_controlled_step = 0
         self._ctl_tab = None
         self._ctl_y = None
-        self._ctl_key = None
+        self._ctl_key = None  # with a DRY slot (controlled == DRY) the graph adds one tl_dry_penalty launch
         # decode_on_device(sampling=..., keep_logits=True): the sampled step plus one tl_log_rows launch that keeps the
         # step's logits rows in a [capacity, B, V] log at the step counter (a speculative draft's q rows); on first use
         self._graph_keep = None
@@ -526,13 +531,19 @@ class DecodeEngine(_GraphEngine):
         if controlled:
             tab = self._ctl_tab
             logits = ext.logit_controls(logits, tab.descriptors[:R], self.context_lens[:R], self.tokens[:R], tab.tails[:R], out=self._ctl_y[:R])
+            if controlled == DRY:
+                ext.dry_penalty(logits, tab.dry.table[:R], self.context_lens[:R], self.tokens[:R], tab.dry.history[:R], tab.dry.scratch[:R])
+        xtc = {}
+        if penalized == XTC:
+            p = self._pen_dev.view(torch.float32).view(6, self.B)
+            xtc = dict(xtc_threshold=p[4, :R], xtc_probability=p[5, :R])
         if spec_draft is not None:
             ext.speculative_sample(logits, spec_draft, self.tokens[1:R], *self._spec_params, self.context_lens[:R], out=self.next_tokens[:R])
             return
         if constrained:
             pen = ()
             if penalized:
-                p = self._pen_dev.view(torch.float32).view(4, self.B)
+                p = self._pen_dev.view(torch.float32).view(6, self.B)
                 pen = (p[0, :R], p[1, :R], p[2, :R], p[3, :R], self.token_counts[:R])
             tab = {"json": self._json_tab, "schema": self._schema_tab, "grammar": self._grammar_tab}.get(constrained)
             if tab is not None and tab.has_json:
@@ -543,7 +554,7 @@ class DecodeEngine(_GraphEngine):
                 ext.grammar_token_masks(tab.descriptors[:R], tab.grammar_states[:R], self.V, tab.grammar_smem_bytes)
             descriptors = self._con_dev.view(self.B, -1)[:R] if tab is None else tab.descriptors[:R]
             tokens = ext.sample_constrained(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
-                                            self.context_lens[:R], descriptors, *pen)
+                                            self.context_lens[:R], descriptors, *pen, **xtc)
             if tab is not None and tab.has_json:
                 ext.json_advance(tab.descriptors[:R], tab.json_states[:R], tokens, self.context_lens[:R])
             if tab is not None and tab.has_schema:
@@ -551,9 +562,9 @@ class DecodeEngine(_GraphEngine):
             if tab is not None and tab.has_grammar:
                 ext.grammar_advance(tab.descriptors[:R], tab.grammar_states[:R], tokens, self.context_lens[:R], self.V)
         elif penalized:
-            pen = self._pen_dev.view(torch.float32).view(4, self.B)
+            pen = self._pen_dev.view(torch.float32).view(6, self.B)
             tokens = ext.sample_penalized(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
-                                          self.context_lens[:R], pen[0, :R], pen[1, :R], pen[2, :R], pen[3, :R], self.token_counts[:R])
+                                          self.context_lens[:R], pen[0, :R], pen[1, :R], pen[2, :R], pen[3, :R], self.token_counts[:R], **xtc)
         elif sampled:
             tokens = ext.sample(logits, self._samp_temperature[:R], self._samp_top_k[:R], self._samp_top_p[:R], self._samp_seed[:R],
                                 self.context_lens[:R])
@@ -727,6 +738,7 @@ class DecodeEngine(_GraphEngine):
         self._graphs = {self.B: self._graph}
         self._graph_sample = None  # captured again on first use, over the current slabs
         self._graph_pen = None
+        self._graph_pen_xtc = None
         self._graph_lp = {}
         self._graph_con = {}
         self._graph_json = {}
@@ -875,22 +887,26 @@ class DecodeEngine(_GraphEngine):
             out.append((first, count, pages))
         return out
 
-    def _ensure_penalized_graph(self) -> None:
-        """Capture the penalised sampled self-advancing step (same conditions as ``_ensure_sample_graph``; the warm-up
-        runs at context 0, so it counts nothing)."""
-        if self._graph_pen is not None:
+    def _ensure_penalized_graph(self, penalized=True) -> None:
+        """Capture the penalised sampled self-advancing step (``penalized == XTC``: with XTC; same conditions as
+        ``_ensure_sample_graph``; the warm-up runs at context 0, so it counts nothing)."""
+        if (self._graph_pen_xtc if penalized == XTC else self._graph_pen) is not None:
             return
         forward = self._forward_fused if self.fused else self._forward_unfused
 
         def penalized_step():
-            forward(sampled=True, penalized=True)
+            forward(sampled=True, penalized=penalized)
             ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
 
         with torch.cuda.stream(self._stream):
             self._stream.wait_stream(torch.cuda.current_stream(self.device))
             self._set_idle()
-            self._graph_pen = self._graph_of(penalized_step, pool=self._graph.pool(), warmups=1)
-            self.kernels_per_penalized_step = self._launches
+            graph = self._graph_of(penalized_step, pool=self._graph.pool(), warmups=1)
+            if penalized == XTC:
+                self._graph_pen_xtc = graph
+            else:
+                self._graph_pen = graph
+                self.kernels_per_penalized_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
     def _ensure_logprobs_graph(self, sampled: bool, max_n: int, penalized: bool = False) -> None:
@@ -934,17 +950,18 @@ class DecodeEngine(_GraphEngine):
                 self._lp_dev = self._lp_host.to(self.device, copy=True)
             self._lp_key = None
 
-    def _ensure_controlled_graph(self, penalized: bool, max_n: int | None) -> None:
+    def _ensure_controlled_graph(self, penalized: bool, max_n: int | None, controlled=True) -> None:
         """Capture the sampled (``penalized``: penalised) self-advancing step with one ``tl_logit_controls`` launch before
-        the draw and one ``tl_logprobs`` launch on the raw logits when ``max_n`` is given (same conditions as
-        ``_ensure_sample_graph``; the warm-up runs at context 0, so it appends to no tail).  One graph per
-        (penalized, max_n)."""
-        if (penalized, max_n) in self._graph_ctl:
+        the draw (``controlled == DRY``: then one ``tl_dry_penalty`` launch) and one ``tl_logprobs`` launch on the raw
+        logits when ``max_n`` is given (same conditions as ``_ensure_sample_graph``; the warm-up runs at context 0, so it
+        appends to no tail or history).  One graph per (penalized, max_n), and per (penalized, max_n, DRY) with DRY."""
+        key = (penalized, max_n) if controlled is True else (penalized, max_n, controlled)
+        if key in self._graph_ctl:
             return
         forward = self._forward_fused if self.fused else self._forward_unfused
 
         def controlled_step():
-            forward(sampled=True, penalized=penalized, controlled=True)
+            forward(sampled=True, penalized=penalized, controlled=controlled)
             if max_n is not None:
                 ext.logprobs(self.logits, self.next_tokens, self._lp_dev, max_n, out=self._lp_log, out_index=self.step_counter)
             ext.decode_advance(self.tokens, self.next_tokens, self.offsets, self.context_lens, self.out_log, self.step_counter)
@@ -953,7 +970,7 @@ class DecodeEngine(_GraphEngine):
             self._stream.wait_stream(torch.cuda.current_stream(self.device))
             self._set_idle()
             self.step_counter.zero_()
-            self._graph_ctl[(penalized, max_n)] = self._graph_of(controlled_step, pool=self._graph.pool(), warmups=1)
+            self._graph_ctl[key] = self._graph_of(controlled_step, pool=self._graph.pool(), warmups=1)
             self.kernels_per_controlled_step = self._launches
         torch.cuda.current_stream(self.device).wait_stream(self._stream)
 
@@ -978,7 +995,7 @@ class DecodeEngine(_GraphEngine):
         from .logit_controls import ControlRows
 
         if self._ctl_tab is None:
-            self._ctl_tab = ControlRows(self.B, self.V, self.device)
+            self._ctl_tab = ControlRows(self.B, self.V, self.device, history_capacity=self.max_seq_len)
             self._ctl_y = torch.empty((self.B, self.V), dtype=torch.float32, device=self.device)
             self._ctl_key = [None] * self.B
         history = None if history is None else list(history)
@@ -1176,13 +1193,13 @@ class DecodeEngine(_GraphEngine):
         """The token counts and the penalty block, on first use (before the penalised graphs are captured over them)."""
         if self.token_counts is None:
             self.token_counts = torch.zeros((self.B, self.V), dtype=torch.int32, device=self.device)
-            self._pen_host = torch.zeros(16 * self.B, dtype=torch.uint8, pin_memory=True)
+            self._pen_host = torch.zeros(24 * self.B, dtype=torch.uint8, pin_memory=True)
             self._pen_dev = self._pen_host.to(self.device, copy=True)
 
     def _set_penalties(self, per: list, history) -> None:
         """Rebuild the token-count rows ``history`` gives (per slot ``(prompt_ids, generated_ids)`` or None: keep the
         row) and upload the penalty parameters if they changed."""
-        from .sampler import penalty_tensors, token_state_row
+        from .sampler import penalty_tensors, token_state_row, xtc_tensors
 
         B = self.B
         if history is not None:
@@ -1198,10 +1215,10 @@ class DecodeEngine(_GraphEngine):
             return
         self._host_write_begin()
         host = self._pen_host.numpy()
-        for j, t in enumerate(penalty_tensors(per, "cpu")):
+        for j, t in enumerate((*penalty_tensors(per, "cpu"), *xtc_tensors(per, "cpu"))):
             host[4 * B * j : 4 * B * (j + 1)] = t.numpy().view(np.uint8)
         self._upload_meta(self._pen_dev, self._pen_host)
-        self.h2d_bytes += 16 * B
+        self.h2d_bytes += 24 * B
         self._pen_key = key
 
     def _set_sampling(self, sampling) -> None:
@@ -1460,6 +1477,10 @@ class DecodeEngine(_GraphEngine):
             per = None if sampling is None else self._per_slot_sampling(sampling)
             if per is not None and any(p is not None and p.grammar for p in per):
                 raise ValueError("keep_logits takes plain sampling: no grammar constraint")
+            if per is not None and any(p is not None and p.xtc for p in per):
+                raise ValueError("keep_logits takes plain sampling: no XTC (xtc_probability)")
+            if per is not None and any(p is not None and p.dry for p in per):
+                raise ValueError("keep_logits takes plain sampling: no DRY (dry_multiplier)")
             if per is None or logprobs is not None or any_penalized(per) or any_constrained(per):
                 raise ValueError("keep_logits takes plain sampling: no penalties, min-p, constraint or logprobs")
             if any(p is not None and p.controls for p in per):
@@ -1478,6 +1499,10 @@ class DecodeEngine(_GraphEngine):
 
             per = self._per_slot_sampling(sampling)
             penalized, constrained, controlled = any_penalized(per), any_constrained(per), any_controlled(per)
+            if any(p is not None and p.xtc for p in per):
+                penalized = XTC
+            if any(p is not None and p.dry for p in per):
+                controlled = DRY
             if controlled and any(p is not None and p.grammar for p in per):
                 raise ValueError("logits controls take no grammar: no slot may carry a grammar beside a controlled slot")
             if controlled and constrained:
@@ -1537,7 +1562,7 @@ class DecodeEngine(_GraphEngine):
             if top_n is not None:
                 self._alloc_logprobs(max(top_n))
                 self._set_top_n(top_n)
-            self._ensure_controlled_graph(penalized, None if top_n is None else max(top_n))
+            self._ensure_controlled_graph(penalized, None if top_n is None else max(top_n), controlled)
         elif constrained:
             if self._con_dev is None:
                 self._con_host = torch.zeros(5 * B, dtype=torch.int64, pin_memory=True)
@@ -1558,7 +1583,7 @@ class DecodeEngine(_GraphEngine):
             self._ensure_logprobs_graph(sampling is not None, max(top_n), penalized)
             self._set_top_n(top_n)
         elif penalized:
-            self._ensure_penalized_graph()
+            self._ensure_penalized_graph(penalized)
         elif keep_logits:
             self._ensure_keep_graph(steps)
         elif sampling is not None:
@@ -1584,7 +1609,7 @@ class DecodeEngine(_GraphEngine):
         elif json:
             graph = self._graph_json[(penalized, None if top_n is None else max(top_n))]
         elif controlled:
-            graph = self._graph_ctl[(penalized, None if top_n is None else max(top_n))]
+            graph = self._graph_ctl[(penalized, None if top_n is None else max(top_n)) + (() if controlled is True else (controlled,))]
         elif constrained:
             graph = self._graph_con[(penalized, None if top_n is None else max(top_n))]
         elif descriptors is not None:
@@ -1592,7 +1617,7 @@ class DecodeEngine(_GraphEngine):
         elif top_n is not None:
             graph = self._graph_lp[(sampling is not None, penalized)]
         elif penalized:
-            graph = self._graph_pen
+            graph = self._graph_pen_xtc if penalized == XTC else self._graph_pen
         elif keep_logits:
             graph = self._graph_keep
         else:
@@ -1729,6 +1754,10 @@ class VerifyEngine(DecodeEngine):
         if spec:
             if sampling.grammar:
                 raise ValueError("the sampled verify pass takes no grammar constraint")
+            if sampling.xtc:
+                raise ValueError("the sampled verify pass takes no XTC: xtc_probability must be 0")
+            if sampling.dry:
+                raise ValueError("the sampled verify pass takes no DRY: dry_multiplier must be 0")
             if sampling.penalized or sampling.constraint is not None:
                 raise ValueError("the sampled verify pass takes plain sampling: no penalties, min-p or constraint")
             if draft_logits is None or tuple(draft_logits.shape) != (T - 1, self.V) or not draft_logits.is_contiguous():

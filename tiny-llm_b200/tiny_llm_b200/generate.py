@@ -76,7 +76,7 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
                 if sampling.constraint is not None and constraints is None:
                     constraints = ConstraintRows.build([sampling], logits.shape[-1], logits.device)
                 if sampling.controls and controls is None:
-                    controls = ControlRows(1, logits.shape[-1], logits.device)
+                    controls = ControlRows(1, logits.shape[-1], logits.device, history_capacity=len(ids) + max_new_tokens)
                     controls.set_row(0, sampling, ids, (), () if eos_token_id is None else (eos_token_id,))
                 token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state, constraints, controls, tokens[-1:])
             elif sampler is None:
@@ -395,6 +395,10 @@ def _spec_sampling(sampling, constraint):
         raise ValueError("speculative decoding and prompt lookup are unconstrained: sampling must carry no grammar")
     if sampling.constraint is not None:
         raise ValueError("speculative decoding is unconstrained: sampling must carry no constraint")
+    if sampling.xtc:
+        raise ValueError("speculative decoding and prompt lookup take no XTC: xtc_probability must be 0")
+    if sampling.dry:
+        raise ValueError("speculative decoding and prompt lookup take no DRY: dry_multiplier must be 0")
     if sampling.penalized:
         raise ValueError("speculative sampling takes temperature, top-k and top-p only: no penalties or min-p")
     if sampling.controls:
@@ -818,6 +822,8 @@ def _check_parallel_args(model, prompts, num_samples, sampling, max_new_tokens, 
     per = [sampling] * len(prompts) if isinstance(sampling, SamplingParams) else list(sampling)
     if len(per) != len(prompts) or not all(isinstance(p, SamplingParams) for p in per):
         raise ValueError("sampling must be one SamplingParams or one per prompt")
+    if any(p.dry for p in per):
+        raise ValueError("parallel sampling takes no DRY: dry_multiplier must be 0")
     if any(p.controls for p in per):
         raise ValueError("parallel sampling takes no logit_bias, allowed_token_ids, bad_words_ids or min_tokens")
     if num_samples > 1 and any(p.temperature == 0 for p in per):

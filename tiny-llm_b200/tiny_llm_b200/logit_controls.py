@@ -163,19 +163,33 @@ def unpack_row(header, data, vocab: int) -> dict:
 class ControlRows:
     """The ``tl_logit_controls`` table of ``rows`` rows on ``device``: ``descriptors`` (int64 ``[rows, ROW_WORDS]``,
     zero rows uncontrolled) and ``tails`` (int32 ``[rows, TAIL]``), plus each controlled row's packed words, which the
-    table keeps alive while its descriptor points at them."""
+    table keeps alive while its descriptor points at them.  ``dry`` is the ``tl_dry_penalty`` table beside it
+    (``dry.DryRows`` of ``history_capacity`` ids per row), allocated when the first DRY row is written."""
 
-    def __init__(self, rows: int, vocab: int, device):
+    def __init__(self, rows: int, vocab: int, device, history_capacity: int | None = None):
         self.rows, self.vocab, self.device = rows, vocab, torch.device(device)
         self.descriptors = torch.zeros((rows, ROW_WORDS), dtype=torch.int64, device=self.device)
         self.tails = torch.full((rows, TAIL), -1, dtype=torch.int32, device=self.device)
         self._data: list = [None] * rows
+        self.history_capacity = history_capacity
+        self.dry = None
+
+    def _set_dry(self, r: int, p, history_ids) -> None:
+        from .dry import DryRows
+
+        if p is not None and p.dry and self.dry is None:
+            if not self.history_capacity:
+                raise ValueError("a DRY request needs a history capacity: this loop allocated none")
+            self.dry = DryRows(self.rows, self.history_capacity, self.device)
+        if self.dry is not None:
+            self.dry.set_row(r, p, history_ids)
 
     def set_row(self, r: int, p, prompt_ids, generated_ids=(), eos_ids=()) -> int:
         """Write request ``p``'s row ``r`` from its history; returns the step's input token (the last history id).  An
         uncontrolled ``p`` clears the row."""
         tail, last = history_tail(prompt_ids, generated_ids)
         header, words = pack_row(p, self.vocab, eos_ids, len(prompt_ids))
+        self._set_dry(r, p, [*prompt_ids, *generated_ids])
         if not header[0]:
             self.clear_row(r)
             return last
@@ -193,16 +207,19 @@ class ControlRows:
         self.descriptors[r].zero_()
         self.tails[r].fill_(-1)
         self._data[r] = None
+        if self.dry is not None:
+            self.dry.clear_row(r)
 
     def row_data(self, r: int):
         return self._data[r]
 
 
-def control_rows(params, vocab: int, device, eos_ids=(), histories=None) -> tuple[ControlRows, list[int]]:
+def control_rows(params, vocab: int, device, eos_ids=(), histories=None, history_capacity=None) -> tuple[ControlRows, list[int]]:
     """One ``ControlRows`` row per entry of ``params`` (``SamplingParams`` or None), each from its history
     ``(prompt_ids, generated_ids)`` in ``histories`` -> ``(rows, input tokens)``: the launch's ``tokens`` argument for
-    the row's next draw (the last history id of each row; 0 for rows without a history)."""
-    table = ControlRows(len(params), vocab, device)
+    the row's next draw (the last history id of each row; 0 for rows without a history).  DRY rows need
+    ``history_capacity``."""
+    table = ControlRows(len(params), vocab, device, history_capacity)
     if histories is None:
         histories = [None] * len(params)
     if len(histories) != len(params):

@@ -65,7 +65,15 @@ class SamplingParams:
     other ids are the request's most recent tokens (prompt, then generated ids); ``min_tokens`` sends the EOS ids to
     -inf until that many tokens have been generated.  The draw, greedy included, runs on the controlled row.  They are
     stored normalised: ``logit_bias`` as ``((id, bias), ...)`` sorted by id, ``allowed_token_ids`` as a sorted tuple of
-    distinct ids and ``bad_words_ids`` as a tuple of tuples, so a ``SamplingParams`` stays hashable."""
+    distinct ids and ``bad_words_ids`` as a tuple of tuples, so a ``SamplingParams`` stays hashable.
+
+    DRY (``tl_dry_penalty``, DESIGN.md section 24), a logits control run after the others: with ``dry_multiplier``
+    m > 0, a token that would extend a repeat of an earlier span of the history (prompt, then generated ids) of
+    length l >= ``dry_allowed_length`` a loses ``m * dry_base ** (l - a)`` (b > 1), l capped at 64 and taken over
+    the last ``dry_penalty_last_n`` tokens (0: all of them); a repeat never runs through a
+    ``dry_sequence_breakers`` id (at most 64, stored as a sorted tuple).  XTC (the penalised form, DESIGN.md section
+    24): with probability ``xtc_probability`` per draw, every kept token whose probability is at least
+    ``xtc_threshold`` but the least likely of them is excluded, when there are two or more."""
 
     temperature: float
     top_k: int | None = None
@@ -80,6 +88,13 @@ class SamplingParams:
     allowed_token_ids: object = None
     bad_words_ids: object = None
     min_tokens: int = 0
+    dry_multiplier: float = 0.0
+    dry_base: float = 1.75
+    dry_allowed_length: int = 2
+    dry_penalty_last_n: int = 0
+    dry_sequence_breakers: object = ()
+    xtc_threshold: float = 0.1
+    xtc_probability: float = 0.0
 
     def __post_init__(self):
         t = self.temperature
@@ -108,6 +123,20 @@ class SamplingParams:
         m = self.min_p
         if not real(m) or not 0 <= m <= 1:
             raise ValueError(f"min_p must be a number in [0, 1], got {m!r}")
+        q = self.xtc_probability
+        if not real(q) or not 0 <= q <= 1:
+            raise ValueError(f"xtc_probability must be a number in [0, 1], got {q!r}")
+        th = self.xtc_threshold
+        if not real(th) or not 0 < th <= 1:
+            raise ValueError(f"xtc_threshold must be a number in (0, 1], got {th!r}")
+        object.__setattr__(self, "xtc_probability", float(q))
+        object.__setattr__(self, "xtc_threshold", float(th))
+        from .dry import normalized_dry
+
+        for name, value in normalized_dry(self).items():
+            object.__setattr__(self, name, value)
+        if self.dry and self.constraint is not None:
+            raise ValueError("dry_multiplier takes no constraint")
         if self.constraint is not None:
             from .constrained import TokenConstraint
             from .json_mode import JsonConstraint
@@ -128,7 +157,18 @@ class SamplingParams:
     @property
     def controls(self) -> bool:
         """Whether the request needs ``tl_logit_controls``: a logit bias, an allow-list, banned sequences or min_tokens."""
-        return self.logit_bias is not None or self.allowed_token_ids is not None or self.bad_words_ids is not None or self.min_tokens > 0
+        return (self.logit_bias is not None or self.allowed_token_ids is not None or self.bad_words_ids is not None or self.min_tokens > 0
+                or self.dry)
+
+    @property
+    def dry(self) -> bool:
+        """Whether the request needs ``tl_dry_penalty`` (DRY is on: ``dry_multiplier > 0``)."""
+        return self.dry_multiplier > 0
+
+    @property
+    def xtc(self) -> bool:
+        """Whether the draw runs XTC (``xtc_probability > 0``)."""
+        return self.xtc_probability > 0
 
     @property
     def grammar(self) -> bool:
@@ -139,8 +179,9 @@ class SamplingParams:
 
     @property
     def penalized(self) -> bool:
-        """Whether the request needs ``tl_sample_penalized``: a penalty or min-p is on."""
-        return self.repetition_penalty != 1 or self.presence_penalty != 0 or self.frequency_penalty != 0 or self.min_p > 0
+        """Whether the request needs ``tl_sample_penalized``: a penalty, min-p or XTC is on."""
+        return (self.repetition_penalty != 1 or self.presence_penalty != 0 or self.frequency_penalty != 0 or self.min_p > 0
+                or self.xtc)
 
 
 GREEDY = SamplingParams(0.0)
@@ -177,6 +218,14 @@ def any_controlled(params) -> bool:
     return any(p is not None and p.controls for p in params)
 
 
+def any_dry(params) -> bool:
+    return any(p is not None and p.dry for p in params)
+
+
+def any_xtc(params) -> bool:
+    return any(p is not None and p.xtc for p in params)
+
+
 def any_constrained(params) -> bool:
     return any(p is not None and p.constraint is not None for p in params)
 
@@ -187,6 +236,14 @@ def penalty_tensors(params, device) -> tuple[torch.Tensor, ...]:
     params = [GREEDY if p is None else p for p in params]
     return tuple(torch.tensor([float(getattr(p, name)) for p in params], dtype=torch.float32, device=device)
                  for name in ("repetition_penalty", "presence_penalty", "frequency_penalty", "min_p"))
+
+
+def xtc_tensors(params, device) -> tuple[torch.Tensor, ...]:
+    """The per-row XTC arrays (threshold, probability) ``ext.sample_penalized`` and ``ext.sample_constrained`` take
+    beside ``penalty_tensors``' (None: greedy, XTC off)."""
+    params = [GREEDY if p is None else p for p in params]
+    return tuple(torch.tensor([float(getattr(p, name)) for p in params], dtype=torch.float32, device=device)
+                 for name in ("xtc_threshold", "xtc_probability"))
 
 
 STATE_PROMPT = 1 << 30  # token state: bit 30 marks a prompt token, bits 0-29 count the draws
@@ -226,6 +283,8 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
     When a row carries logits controls, ``tl_logit_controls`` first turns every row into its fp32 controlled row
     (uncontrolled rows are copied exactly) over ``controls`` (a ``ControlRows`` of at least ``rows`` rows, required
     then), appending ``tokens`` (the step's input token per row) to its history tails, and the draw runs on those rows.
+    When a row has DRY on, ``tl_dry_penalty`` then penalises those rows in place over ``controls.dry`` and appends
+    ``tokens`` to its histories.  XTC rows pass the ``xtc_tensors`` to the penalised or constrained draw.
     Rows of other requests may carry a constraint in the same launch: the constrained draw then runs on their exact
     fp32 copies, which draws the tokens it draws on the raw rows (a request never carries both)."""
     from extensions_b200 import tiny_llm_ext_b200 as ext
@@ -238,6 +297,13 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
         n = len(params)
         tok = torch.as_tensor(tokens, dtype=torch.int32).reshape(-1).to(logits.device)
         logits = ext.logit_controls(logits.contiguous(), controls.descriptors[:n], pos, tok, controls.tails[:n])
+        if any_dry(params):
+            if controls.dry is None:
+                raise ValueError("a SamplingParams with DRY needs its history in the ControlRows")
+            ext.dry_penalty(logits, controls.dry.table[:n], pos, tok, controls.dry.history[:n], controls.dry.scratch[:n])
+    xtc = {}
+    if any_xtc(params):
+        xtc = dict(zip(("xtc_threshold", "xtc_probability"), xtc_tensors(params, logits.device)))
     if any_constrained(params):
         if constraints is None:
             raise ValueError("a constrained SamplingParams needs the request's constraint descriptor")
@@ -259,13 +325,14 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
                 raise ValueError("a JSON-schema SamplingParams needs the request's ConstraintRows")
             if any(p is not None and p.grammar for p in params):
                 raise ValueError("a grammar SamplingParams needs the request's ConstraintRows")
-            return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen)
+            return ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints, *pen, **xtc)
         constraints.before_draw(len(params))
-        tokens = ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints.descriptors[:len(params)], *pen)
+        tokens = ext.sample_constrained(logits.contiguous(), temperature, top_k, top_p, seed, pos, constraints.descriptors[:len(params)], *pen,
+                                        **xtc)
         constraints.after_draw(tokens, pos)
         return tokens
     if not any_penalized(params):
         return ext.sample(logits.contiguous(), temperature, top_k, top_p, seed, pos)
     if state is None:
         raise ValueError("a penalised SamplingParams needs the request's token state")
-    return ext.sample_penalized(logits.contiguous(), temperature, top_k, top_p, seed, pos, *penalty_tensors(params, logits.device), state)
+    return ext.sample_penalized(logits.contiguous(), temperature, top_k, top_p, seed, pos, *penalty_tensors(params, logits.device), state, **xtc)
