@@ -331,7 +331,7 @@ def _pow2(t):
 
 
 def exact_probes(M, N, K, dtype, g, positions, *, prologue=PRO_NONE, epilogue=EPI_NONE, residual=False, group_rows=True, lda=None,
-                 weights=None):
+                 weights=None, bits=4):
     """Weights and needle activations on which every path is bit-exact.
 
     scales: powers of two 2^-(5 + (k + 2 grp) % 3), so neighbouring rows and neighbouring groups differ; biases -c s with
@@ -348,15 +348,30 @@ def exact_probes(M, N, K, dtype, g, positions, *, prologue=PRO_NONE, epilogue=EP
         w = 2^8): every gate output is 0 or >= 32, where silu(g) = g in fp32 and to 2^-45 in float64, and g * up has at
         most 8 significant bits (|g up| <= 240^2 < 65504).
       residual: s 2^e times an integer in -60..60, with the result still exact (at most 7 bits).
+    bits=8 (b [K, N/4], code i of a word in bits 8i..8i+7): codes are random bytes, c is in 0..255, so every weight
+    (q - c) s has at most 8 significant bits (exact in bf16, unchanged by the tensor-core rounding).  Every needle
+    column cycles through the codes 0, 127, 128 and 255 over the feature rows (PROBE_CODES8: the bf16 128 + q trap, both
+    nibbles, both bytes halves).  What changes to keep every sum a T number:
+      multi-entry rows put their two extra entries at offsets +36 and +76 of the group (the needle's column modulo 4,
+        so the same code) with opposite signs: they cancel exactly, and a kernel that misreads either column does not;
+      SWIGLU_PAIRS: needles +2^6 (after RMSNORM: w = 2^5); a needle column's code depends on its group only, gate rows
+        take c = q or q - c >= 64 (gates 0 or >= 32), up rows q - c in {0, +-1, .., +-32}: g * up has at most 8 bits;
+      residual: s 2^e times an integer r chosen per output so that |r| and |r + acc / (s 2^e)| stay below 256.
     positions: the reduction positions to cover (probe_positions); rows past them repeat from the start.
     weights: (words, scales, biases) of an earlier probe of the same form, to keep."""
     G = N // 128
+    wide = bits == 8
     pairs = epilogue == EPI_SWIGLU_PAIRS
+    top = 2.0**6 if wide else 2.0**9  # pairs needle
+    extra = (36, 76) if wide else (37, 77)
     kk = torch.arange(K)[:, None]
     gg = torch.arange(G)[None, :]
     s = _pow2(-(5 + (kk + 2 * gg) % 3)).expand(K, G).contiguous()
     if weights is not None:  # new activations for the same weights
         words, scales, biases = weights
+    elif wide:
+        words, c = _probe_codes8(K, N, g, positions, pairs, extra)
+        scales, biases = s.to(dtype), (-c * s).to(dtype)
     else:
         c = torch.randint(0, 16, (K, G), generator=g)
         if pairs:
@@ -382,10 +397,10 @@ def exact_probes(M, N, K, dtype, g, positions, *, prologue=PRO_NONE, epilogue=EP
         i += 1
         ent = [first]
         if multi and m % 2 == 1:  # two more entries in the same group, at other offsets
-            ent += [first - first % 128 + (first + d) % 128 for d in (37, 77)]
+            ent += [first - first % 128 + (first + d) % 128 for d in extra]
         rows.append(ent)
         if pairs:
-            mag.append(2.0**9)
+            mag.append(top)
         elif len(ent) > 1 or prologue == PRO_RMSNORM:
             mag.append(1.0)
         else:
@@ -399,18 +414,23 @@ def exact_probes(M, N, K, dtype, g, positions, *, prologue=PRO_NONE, epilogue=EP
     if prologue == PRO_SWIGLU:
         p0 = torch.randn(M, lda, generator=g) * 4
         p1 = torch.zeros(M, lda)
+    avals = []  # the exact prologue output at each entry
     for m, ent in enumerate(rows):
-        for n in ent:
-            v = sign() * mag[m]
+        vals = [sign() * mag[m] for _ in ent]
+        if wide and len(ent) == 3:
+            vals[2] = -vals[1]  # the two extra entries cancel
+        for n, v in zip(ent, vals):
             if prologue == PRO_SWIGLU:
                 p0[m, n], p1[m, n] = 32.0, v / 32.0
             elif prologue == PRO_RMSNORM:
                 p0[m, n] = 1.0 if pairs else v
             else:
                 p0[m, n] = v
+        avals.append(vals)
     if prologue == PRO_RMSNORM:
-        # norm weights: a = 2 w = 2^-1 .. 2^1 (2^9 everywhere for the pairs epilogue)
-        p1 = (torch.full((N,), 2.0**8) if pairs else _pow2(torch.arange(N) % 3 - 2)).to(dtype)
+        # norm weights: a = 2 w = 2^-1 .. 2^1 (the pairs needle everywhere for the pairs epilogue)
+        p1 = (torch.full((N,), top / 2) if pairs else _pow2(torch.arange(N) % 3 - 2)).to(dtype)
+        avals = [[(1.0 if pairs else v) * 2.0 * float(p1[n]) for n, v in zip(ent, vals)] for ent, vals in zip(rows, avals)]
         v = torch.tensor(1.0 / N, dtype=torch.float32)
         eps32 = (torch.tensor(0.25, dtype=F64) - v.to(F64)).to(torch.float32)
         assert float(eps32 + v) == 0.25
@@ -422,9 +442,56 @@ def exact_probes(M, N, K, dtype, g, positions, *, prologue=PRO_NONE, epilogue=EP
     res = None
     if residual:
         grp = torch.tensor([ent[0] // 128 for ent in rows])
-        unit = s[:, grp].T * torch.tensor(mag)[:, None]  # [M, K]
-        res = (torch.randint(-60, 61, (M, K), generator=g) * unit).to(dtype)
+        if not wide:
+            unit = s[:, grp].T * torch.tensor(mag)[:, None]  # [M, K]
+            res = (torch.randint(-60, 61, (M, K), generator=g) * unit).to(dtype)
+        else:
+            amin = torch.tensor([min(abs(v) for v in vals) for vals in avals], dtype=F64)
+            unit = s[:, grp].T.to(F64) * amin[:, None]
+            acc = _probe_acc8(words, scales, biases, rows, avals, K)
+            A = torch.round(acc / unit)
+            assert bool((A * unit == acc).all()) and bool((A.abs() <= 255).all())
+            lo, hi = torch.clamp(A - 255, min=-255), torch.clamp(A + 255, max=255)
+            total = lo + torch.floor(torch.rand(M, K, generator=g, dtype=F64) * (hi - lo + 1))
+            res = ((total - A) * unit).to(dtype)
     return Probe(words, scales, biases, p0, p1, res, eps, rows)
+
+
+PROBE_CODES8 = (0, 127, 128, 255)
+
+
+def _probe_codes8(K, N, g, positions, pairs, extra):
+    """8-bit probe codes (see exact_probes): (words [K, N/4] int32, c [K, N/128] int64)."""
+    G = N // 128
+    codes = torch.randint(0, 256, (K, N), dtype=torch.uint8, generator=g)
+    cols = set(positions)
+    if not pairs:  # the columns multi-entry rows may reach
+        cols |= {p - p % 128 + (p + d) % 128 for p in positions for d in extra}
+    cols = torch.tensor(sorted(cols), dtype=torch.int64)
+    k = torch.arange(K)[:, None]
+    probe = torch.tensor(PROBE_CODES8, dtype=torch.uint8)
+    if pairs:
+        codes[:, cols] = probe[(k + cols // 128) % 4]
+        q = probe[(k + torch.arange(G)[None, :]) % 4].to(torch.int64)  # every needle code of row k, group grp
+        c_gate = (torch.rand(K, G, generator=g) * torch.clamp(q - 63, min=1)).to(torch.int64)  # q - c >= 64, or c = q = 0
+        j = torch.randint(0, 6, (K, G), generator=g)
+        d = torch.where(torch.randint(0, 4, (K, G), generator=g) == 0, 0, 2**j)
+        c_up = torch.where(q >= 128, q - d, q + d)  # q - c = +-d, c in 0..255
+        c = torch.where(((torch.arange(K) % 16) < 8)[:, None], c_gate, c_up)
+    else:
+        codes[:, cols] = probe[(k + cols) % 4]
+        c = torch.randint(0, 256, (K, G), generator=g)
+    return codes.view(torch.int32), c
+
+
+def _probe_acc8(words, scales, biases, rows, avals, K):
+    """Exact float64 projection [M, K] of the probe activations (entries ``rows`` with values ``avals``)."""
+    acc = torch.zeros(len(rows), K, dtype=F64)
+    for m, (ent, vals) in enumerate(zip(rows, avals)):
+        for n, v in zip(ent, vals):
+            q = ((words[:, n // 4].to(torch.int64) & 0xFFFFFFFF) >> (8 * (n % 4))) & 255
+            acc[m] += (q.to(F64) * scales[:, n // 128].to(F64) + biases[:, n // 128].to(F64)).cpu() * v
+    return acc
 
 
 def probe_reference(probe, W, *, prologue=PRO_NONE, epilogue=EPI_NONE, norm_weight=None, norm_eps=0.0):

@@ -4,8 +4,8 @@ Rounding points are those of 4 bits (include/tiny_llm_b200.h): weights exact on 
 T(code * scale + bias) rounded once on the wgmma kernels, the same prologues and epilogues.  What changes is the
 streaming kernel's factorisation: each code is split q = 16 h + l and the group dot product is
 scale * (16 d_h + d_l) + bias * asum, where d_h and d_l are the W4 shifted-code sums over nibbles.  ``error_bound``
-accounts for it (its docstring has the derivation).  ``exact_probes8`` builds inputs on which every kernel's arithmetic
-is exact, with codes 0, 127, 128 and 255 in every needle column.
+accounts for it (its docstring has the derivation).  The exact probes are ``w4a16_ref.exact_probes(..., bits=8)``: every
+kernel's arithmetic is exact on them, with codes 0, 127, 128 and 255 in every needle column.
 """
 
 from __future__ import annotations
@@ -30,7 +30,7 @@ def _load_w4a16_ref():
 
 wr = _load_w4a16_ref()
 F64 = torch.float64
-PROBE_CODES = (0, 127, 128, 255)
+PROBE_CODES = wr.PROBE_CODES8
 # The streaming bound's scale coefficient at 8 bits over the W4 one (see error_bound): 17 nibble sums plus a chain of
 # codes up to 255 instead of 15 stay below 18 times the W4 coefficient for every chain length and shift.
 STREAM8_SCALE = 18.0
@@ -93,37 +93,3 @@ def embedding_ref(words, scales, biases, ids):
     out = torch.zeros(ids.numel(), G * 128, dtype=scales.dtype, device=words.device)
     out[valid] = table[ids[valid]]
     return out
-
-
-def exact_probes8(M, N, K, dtype, g, positions, residual=False):
-    """Inputs on which every W8 kernel is exact: every code of the needle columns cycles through 0, 127, 128 and 255
-    (over the rows) and is random elsewhere; scales are powers of two 2^-e (e in 0..3) and biases -c 2^-e (c in
-    0..127), so a weight (q - c) 2^-e has |q - c| <= 255: at most 8 significant bits, exact in bf16 and fp16 alike.
-    Each activation row holds one needle +-2^-j at a position from ``positions`` (rows cycle through them) and zeros
-    elsewhere, so an output is one exact product.  Returns (words, scales, biases, p0, residual or None, want [M, K]
-    float64)."""
-    G = N // 128
-    codes = torch.randint(0, 256, (K, N), generator=g)
-    probe = torch.tensor(PROBE_CODES)
-    for p in positions:
-        codes[:, p] = probe[(torch.arange(K) + p) % 4]
-    e = torch.randint(0, 4, (K, G), generator=g)
-    scales = torch.ldexp(torch.ones(K, G), -e)
-    c = torch.randint(0, 128, (K, G), generator=g)
-    biases = -c.to(torch.float32) * scales
-    p0 = torch.zeros(M, N)
-    cols = []
-    for m in range(M):
-        p = positions[m % len(positions)]
-        p0[m, p] = (-1.0) ** m * 2.0 ** -(m % 3)
-        cols.append(p)
-    words = pack_codes8(codes)
-    scales_t, biases_t, p0_t = scales.to(dtype), biases.to(dtype), p0.to(dtype)
-    W = weights8(words, scales_t, biases_t, rounded=False)
-    want = p0_t.to(F64) @ W.w.T
-    res = None
-    if residual:
-        res = torch.ldexp(torch.randint(-64, 64, (M, K), generator=g).to(torch.float32), torch.tensor(-4)).to(dtype)
-        want = wr.round_to(res.to(F64) + wr.round_to(want, dtype), dtype)
-    assert torch.equal(wr.round_to(want, dtype), want), "probe outputs must be representable in T"
-    return words, scales_t, biases_t, p0_t, res, want
