@@ -318,6 +318,26 @@ int tl_sample_penalized_xtc(const void *logits, const float *temperature, const 
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                             const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
                             int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* tl_sample_penalized_xtc with the truncation samplers (DESIGN.md section 25): typical_p, top_n_sigma, mirostat_tau and
+ * mirostat_eta, per-row f32 device arrays, and mirostat_mu, a per-row f32 device array read and written (all NULL:
+ * tl_sample_penalized_xtc, bit for bit; any of them NULL when no row of the launch uses it).  For a row with temperature
+ * > 0 and a finite maximum m (z_i = fl(x_i - m), e_i the 2^-40 fixed-point masses as tl_sample_penalized_xtc defines
+ * them):
+ *   top-n-sigma  n = top_n_sigma > 0: tau also bounds x >= m - n sigma, sigma the population standard deviation of the
+ *                row's finite entries (sums in double, the bound rounded up to fp32);
+ *   typical      0 < p = typical_p < 1: over the keep set K and its T = 1 masses, d_i = |z_bar - z_i| with
+ *                z_bar = sum e_i z_i / sum e_i; K keeps the entries whose d (rounded to fp32) is at most the smallest
+ *                d* with mass(d <= d*) >= p S_K, the others become NaN; XTC then runs on what is left;
+ *   Mirostat     mirostat_tau > 0 (mirostat_eta and mirostat_mu then required): top-k, top-p, min-p, top-n-sigma,
+ *                typical and XTC are ignored; with e_i at the row's temperature over the non-NaN entries and S their
+ *                sum, the row keeps {(double)e_i >= min(S 2^-mu, 2^40)} (the maximum always), draws among them, and
+ *                for rows with position > 0 writes mu' = fl32(mu - eta (log2 S_K - log2 e_token - tau)) in double.
+ * Temperature 0 and a non-finite maximum are unaffected, and leave mu alone. */
+int tl_sample_penalized_trunc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                              float *mirostat_mu, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
 /* Speculative sampling (DESIGN.md section 8d): the rejection rule over one verify pass of T = k + 1 rows
  * (1 <= T <= 65535, vocab <= TL_SPECULATIVE_SAMPLE_MAX_VOCAB).  target [T, vocab] are the target's logits rows,
  * draft [k, vocab] the draft's rows each proposal proposals[j] (int32, device) was drawn from, the parameters per row
@@ -386,6 +406,14 @@ int tl_sample_constrained_xtc(const void *logits, const float *temperature, cons
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                               const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
                               tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream);
+/* tl_sample_constrained_xtc with the truncation arrays as tl_sample_penalized_trunc takes them (with the penalty arrays):
+ * every sum and keep set is taken over the allowed entries only. */
+int tl_sample_constrained_trunc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                                const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                                const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                                const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                                float *mirostat_mu, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype,
+                                void *stream);
 /* JSON mode (DESIGN.md section 20): a byte-level pushdown automaton over RFC 8259 `ws object ws`, with at most
  * TL_JSON_MAX_DEPTH open containers and at most TL_JSON_MAX_WS_RUN consecutive whitespace bytes.  A JSON row is a
  * tl_constraint_row with num_states = 1 whose mask is the row's own uint32 [2, ceil(vocab / 32)] buffer (row 0: this

@@ -554,6 +554,16 @@ int tl_sample_penalized_xtc(const void *logits, const float *temperature, const 
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                             const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
                             int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
+    return tl_sample_penalized_trunc(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
+                                     xtc_threshold, xtc_probability, nullptr, nullptr, nullptr, nullptr, nullptr, out_tokens, rows, vocab,
+                                     dtype, stream);
+}
+
+int tl_sample_penalized_trunc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                              const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                              const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                              const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                              float *mirostat_mu, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_penalized: expected float32, float16, or bfloat16");
     if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_penalized: bad shape");
     if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
@@ -562,8 +572,11 @@ int tl_sample_penalized_xtc(const void *logits, const float *temperature, const 
         !out_tokens)
         return fail(TL_EINVAL, "sample_penalized: null pointer");
     if (!xtc_threshold != !xtc_probability) return fail(TL_EINVAL, "sample_penalized: give both XTC arrays or neither");
+    if (mirostat_tau && (!mirostat_eta || !mirostat_mu))
+        return fail(TL_EINVAL, "sample_penalized: Mirostat needs mirostat_eta and mirostat_mu beside mirostat_tau");
     return launch_sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
-                                   xtc_threshold, xtc_probability, out_tokens, rows, vocab, dtype, as_stream(stream));
+                                   xtc_threshold, xtc_probability, typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu,
+                                   out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
 int tl_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
@@ -578,6 +591,17 @@ int tl_sample_constrained_xtc(const void *logits, const float *temperature, cons
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                               const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
                               tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype, void *stream) {
+    return tl_sample_constrained_trunc(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
+                                       xtc_threshold, xtc_probability, nullptr, nullptr, nullptr, nullptr, nullptr, constraints, out_tokens,
+                                       rows, vocab, dtype, stream);
+}
+
+int tl_sample_constrained_trunc(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
+                                const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
+                                const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                                const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                                float *mirostat_mu, tl_constraint_row *constraints, int32_t *out_tokens, int rows, int vocab, int dtype,
+                                void *stream) {
     if (!float_dtype(dtype)) return fail(TL_EDTYPE, "sample_constrained: expected float32, float16, or bfloat16");
     if (rows < 0 || rows > 65535 || vocab <= 0) return fail(TL_EINVAL, "sample_constrained: bad shape");
     if (int e = sample_plan(vocab, nullptr, nullptr)) return e;
@@ -588,8 +612,13 @@ int tl_sample_constrained_xtc(const void *logits, const float *temperature, cons
     if (given != 0 && given != 5) return fail(TL_EINVAL, "sample_constrained: give every penalty array and the state, or none");
     if (!xtc_threshold != !xtc_probability || (xtc_threshold && !state))
         return fail(TL_EINVAL, "sample_constrained: give both XTC arrays, with the penalty arrays, or neither");
+    if ((typical_p || top_n_sigma || mirostat_tau) && !state)
+        return fail(TL_EINVAL, "sample_constrained: typical, top-n-sigma and Mirostat need the penalty arrays and the state");
+    if (mirostat_tau && (!mirostat_eta || !mirostat_mu))
+        return fail(TL_EINVAL, "sample_constrained: Mirostat needs mirostat_eta and mirostat_mu beside mirostat_tau");
     return launch_sample_constrained(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state,
-                                     xtc_threshold, xtc_probability, constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
+                                     xtc_threshold, xtc_probability, typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu,
+                                     constraints, out_tokens, rows, vocab, dtype, as_stream(stream));
 }
 
 int tl_speculative_sample(const void *target, const void *draft, const int32_t *proposals, const float *temperature,

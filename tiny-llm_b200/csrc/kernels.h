@@ -44,12 +44,15 @@ int launch_sample(const void *logits, const float *temperature, const int32_t *t
                   const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability, int32_t *out,
-                            int rows, int vocab, int dtype, cudaStream_t st);
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                            const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                            float *mirostat_mu, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
 int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                               const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
-                              tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st);
+                              const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                              float *mirostat_mu, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype,
+                              cudaStream_t st);
 // constrained.cu
 int launch_constraint_token_masks(const int32_t *dfa, const uint8_t *accept, int num_states, const int32_t *token_offsets,
                                   const uint8_t *token_bytes, int vocab, const int32_t *eos_ids, int num_eos, uint32_t *masks,

@@ -36,6 +36,13 @@
 // least likely of them, become NaN when there are two or more.  Two integer passes over the staged slice (the kept
 // mass, then the count and minimum key of the entries at or above theta's share) decide it, so every CTA of the
 // cluster drops the same entries.
+//
+// The truncation forms (TRUNC, DESIGN.md section 25; always with XTC's code, which they skip when no XTC array is
+// given) add top-n-sigma, locally typical sampling and Mirostat 2.0 after min-p.  Top-n-sigma is two fixed-order double
+// reductions (mean, then squared deviations) and one more lower bound on tau.  Typical sums the kept T = 1 masses and
+// sum e_i z_i, runs up to four radix levels over the key of d_i = |z_bar - z_i| ascending in the same bins, and sends
+// the kept entries above the boundary d to NaN.  Mirostat sums the tempered masses, sends every entry below S 2^-mu to
+// NaN, sums the rest, and after the draw rank 0 reads the token's value over distributed shared memory to update mu.
 #include <cooperative_groups.h>
 
 #include <climits>
@@ -60,6 +67,13 @@ struct Penalties {
 // Per-row arrays of the XTC forms.  Unused (all null) by the others.
 struct Xtc {
     const float *threshold, *probability;
+};
+
+// Per-row arrays of the truncation forms (DESIGN.md section 25); any of them may be null when no row uses it.  Mirostat
+// is on for a row with mirostat_tau > 0, and mu (fp32, one per row) is then read and, at position > 0, written.
+struct Trunc {
+    const float *typical_p, *top_n_sigma, *mirostat_tau, *mirostat_eta;
+    float *mu;
 };
 
 constexpr int32_t STATE_PROMPT = 1 << 30;
@@ -97,12 +111,45 @@ __device__ __forceinline__ int constraint_lowest(const tl_constraint_row &c, int
     return 0;
 }
 
-template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC>
+// TRUNC: the cluster totals of a pair of per-thread partial sums, added in one fixed order (each thread's entries, a
+// warp butterfly, the warps in order, the ranks in order), so every CTA of the cluster gets the same bits in every
+// launch; integer pairs give the same total in any order.  `pub` is published to the other CTAs: each reduction of a
+// launch uses a slot of its own, since a slower CTA may still read the previous one after this CTA went on.
+template <typename V>
+struct Pair {
+    V a, b;
+};
+template <typename V>
+__device__ __forceinline__ Pair<V> cluster_sum(cg::cluster_group &cluster, Pair<V> p, Pair<V> *w, Pair<V> *pub, Pair<V> *res, int C) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) p.a += __shfl_xor_sync(0xffffffffu, p.a, o), p.b += __shfl_xor_sync(0xffffffffu, p.b, o);
+    if (lane == 0) w[warp] = p;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        Pair<V> s{0, 0};
+        for (int i = 0; i < SAMPLE_WARPS; ++i) s.a += w[i].a, s.b += w[i].b;
+        *pub = s;
+    }
+    cluster.sync();
+    if (threadIdx.x == 0) {
+        Pair<V> t{0, 0};
+        for (int r = 0; r < C; ++r) {
+            const Pair<V> q = *cluster.map_shared_rank(pub, r);
+            t.a += q.a, t.b += q.b;
+        }
+        *res = t;
+    }
+    __syncthreads();
+    return *res;
+}
+
+template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC, bool TRUNC = false>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restrict__ logits, const float *__restrict__ temperature,
                                                                 const int32_t *__restrict__ top_k, const float *__restrict__ top_p,
                                                                 const int64_t *__restrict__ seed, const int32_t *__restrict__ positions,
                                                                 int32_t *__restrict__ out, int vocab, int slice, int vec, Penalties pen,
-                                                                tl_constraint_row *con, Xtc xtc) {
+                                                                tl_constraint_row *con, Xtc xtc, Trunc trn) {
     extern __shared__ float4 smem_dyn[];
     float *xs = reinterpret_cast<float *>(smem_dyn);
     __shared__ unsigned int h_count[2][BINS];  // double-buffered: level l + 2 reuses l's buffer after all remote reads of it
@@ -221,12 +268,147 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     const uint32_t pos = static_cast<uint32_t>(positions[row]);
     const uint64_t sd = static_cast<uint64_t>(seed[row]);
     const uint32_t k0 = static_cast<uint32_t>(sd), k1 = static_cast<uint32_t>(sd >> 32);
+    // ---- 2b. truncation (TRUNC, DESIGN.md section 25): top-n-sigma joins tau, typical sends the kept entries it drops
+    //      to NaN, and Mirostat replaces the keep set with its own (NaN outside it, tau = 0)
+    // (nothing of it stays in registers across the draw: rank 0 reads mu, S_K and the parameters again to update mu)
+    __shared__ unsigned long long s_miro_kept;  // Mirostat: the kept mass S_K (unused by the other forms)
+    if constexpr (TRUNC) {
+        __shared__ Pair<double> tr_wd[SAMPLE_WARPS], tr_pd[2], tr_rd;
+        __shared__ Pair<unsigned long long> tr_wu[SAMPLE_WARPS], tr_pu[3], tr_ru;
+        __shared__ uint32_t s_dprefix;
+        __shared__ unsigned long long s_dbelow;
+        __shared__ double s_dwant;
+        const bool miro = trn.mirostat_tau && trn.mirostat_tau[row] > 0.f;
+        const float nsig = trn.top_n_sigma && !miro ? trn.top_n_sigma[row] : 0.f;
+        const float typ = trn.typical_p && !miro ? trn.typical_p[row] : 1.f;
+        if (nsig > 0.f) {  // x >= m - n sigma over the finite entries (population sigma), the bound rounded up to fp32
+            double sx = 0, cnt = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (isfinite(v)) sx += v, cnt += 1;
+            }
+            const Pair<double> t1 = cluster_sum(cluster, Pair<double>{sx, cnt}, tr_wd, &tr_pd[0], &tr_rd, C);
+            const double mean = t1.a / t1.b;
+            double sq = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (isfinite(v)) sq += (static_cast<double>(v) - mean) * (static_cast<double>(v) - mean);
+            }
+            const Pair<double> t2 = cluster_sum(cluster, Pair<double>{sq, 0.0}, tr_wd, &tr_pd[1], &tr_rd, C);
+            const double bound = static_cast<double>(m) - static_cast<double>(nsig) * sqrt(t2.a / t1.b);
+            tau = max(tau, order_key(__double2float_ru(bound)));
+        }
+        if (typ > 0.f && typ < 1.f) {
+            // the T = 1 masses of the keep set K: S_K and sum e_i z_i (z_i = x_i - m, 2^-4 fixed point, signed), so
+            // z_bar = sum p_i z_i and d_i = |z_bar - z_i| = |-ln p_i - H|
+            unsigned long long se = 0, sz = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v && order_key(v) >= tau) {
+                    const unsigned long long e = __float2ull_rn(expf(v - m) * MASS_SCALE);
+                    se += e;
+                    if (e) sz += static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(e) * static_cast<double>(v - m) * 16.0));
+                }
+            }
+            const Pair<unsigned long long> tk = cluster_sum(cluster, Pair<unsigned long long>{se, sz}, tr_wu, &tr_pu[0], &tr_ru, C);
+            const double zbar = static_cast<double>(static_cast<long long>(tk.b)) * 0.0625 / static_cast<double>(tk.a);
+            // every CTA has read the keep threshold's bins (the barrier above): both buffers are free again
+            for (int i = threadIdx.x; i < 2 * BINS; i += SAMPLE_THREADS) (&h_count[0][0])[i] = 0, (&h_mass[0][0])[i] = 0;
+            if (threadIdx.x == 0) s_dprefix = 0, s_dbelow = 0, s_dwant = static_cast<double>(typ) * static_cast<double>(tk.a);
+            __syncthreads();
+            // d* = the smallest key of d with mass(key <= d*) >= typical_p S_K: 4 radix levels, ascending
+            for (int level = 0; level < 4; ++level) {
+                const int buf = level & 1;
+                const int shift = 24 - 8 * level;
+                const uint32_t prefix = s_dprefix;
+                for (int base = warp * 32; base < n; base += SAMPLE_THREADS) {
+                    const int i = base + lane;
+                    int bin = -1;
+                    unsigned long long e = 0;
+                    if (i < n) {
+                        const float v = xs[i];
+                        if (v == v && order_key(v) >= tau) {
+                            const uint32_t dk = __float_as_uint(__double2float_rn(fabs(zbar - static_cast<double>(v - m))));
+                            if (level == 0 || (dk >> (shift + 8)) == (prefix >> (shift + 8))) {
+                                bin = static_cast<int>((dk >> shift) & 0xffu);
+                                e = __float2ull_rn(expf(v - m) * MASS_SCALE);
+                            }
+                        }
+                    }
+                    bin_add(h_count[buf], h_mass[buf], bin, e, true);
+                }
+                cluster.sync();
+                if (threadIdx.x < BINS) {
+                    unsigned long long s = 0;
+                    for (int r = 0; r < C; ++r) s += *cluster.map_shared_rank(&h_mass[buf][threadIdx.x], r);
+                    t_mass[threadIdx.x] = s;
+                }
+                for (int i = threadIdx.x; i < BINS; i += SAMPLE_THREADS) h_count[buf ^ 1][i] = 0, h_mass[buf ^ 1][i] = 0;
+                __syncthreads();
+                if (warp == 0) {  // lane owns bins 8 lane .. 8 lane + 7; prefix sums from bin 0 up
+                    unsigned long long s[8], ls = 0;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) s[j] = t_mass[8 * lane + j], ls += s[j];
+                    unsigned long long incl = ls;
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, o);
+                        if (lane >= o) incl += up;
+                    }
+                    const double want = s_dwant;  // typical_p S_K
+                    unsigned long long below = s_dbelow + (incl - ls);
+                    int hit = -1;
+                    unsigned long long hit_below = 0;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        if (hit < 0 && static_cast<double>(below + s[j]) >= want) hit = 8 * lane + j, hit_below = below;
+                        below += s[j];
+                    }
+                    const unsigned hb = __ballot_sync(0xffffffffu, hit >= 0);
+                    // the crossing bin adds mass, so it holds an entry; no crossing cannot happen (want < S_K)
+                    if (hb && lane == __ffs(hb) - 1) s_dprefix = prefix | (static_cast<uint32_t>(hit) << shift), s_dbelow = hit_below;
+                }
+                __syncthreads();
+            }
+            const uint32_t dstar = s_dprefix;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v && order_key(v) >= tau && __float_as_uint(__double2float_rn(fabs(zbar - static_cast<double>(v - m)))) > dstar)
+                    xs[i] = NAN;
+            }
+            __syncthreads();
+        }
+        if (miro) {  // keep {e_i >= S 2^-mu} at the row's temperature, the maximum always (its e is 2^40)
+            const float mu = trn.mu[row];
+            unsigned long long se = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v) se += __float2ull_rn(expf(__fdiv_rn(__fsub_rn(v, m), temp)) * MASS_SCALE);
+            }
+            const unsigned long long S = cluster_sum(cluster, Pair<unsigned long long>{se, 0ull}, tr_wu, &tr_pu[1], &tr_ru, C).a;
+            const double thr = fmin(static_cast<double>(S) * exp2(-static_cast<double>(mu)), static_cast<double>(MASS_SCALE));
+            unsigned long long sk = 0;
+            for (int i = threadIdx.x; i < n; i += SAMPLE_THREADS) {
+                const float v = xs[i];
+                if (v == v) {
+                    const unsigned long long e = __float2ull_rn(expf(__fdiv_rn(__fsub_rn(v, m), temp)) * MASS_SCALE);
+                    if (static_cast<double>(e) >= thr)
+                        sk += e;
+                    else
+                        xs[i] = NAN;
+                }
+            }
+            const unsigned long long kept = cluster_sum(cluster, Pair<unsigned long long>{sk, 0ull}, tr_wu, &tr_pu[2], &tr_ru, C).a;
+            if (threadIdx.x == 0) s_miro_kept = kept;
+            tau = 0;
+        }
+    }
     if constexpr (XTC) {
         __shared__ unsigned long long x_mass;
         __shared__ unsigned int x_count, x_min, x_hi;
         const uint4 w = philox4x32_10(make_uint4(0u, pos, 3u, 0u), k0, k1);
         const float u = static_cast<float>(2u * (w.x >> 9) + 1u) * 5.9604644775390625e-8f;
-        if (u < xtc.probability[row]) {  // the same decision in every CTA of the cluster
+        if ((!TRUNC || (xtc.probability && !(trn.mirostat_tau && trn.mirostat_tau[row] > 0.f))) && u < xtc.probability[row]) {  // the same decision in every CTA of the cluster
             if (threadIdx.x == 0) x_mass = 0, x_count = 0, x_min = UINT_MAX;
             __syncthreads();
             // e_i = exp((x_i - m) / T) in 2^-40 fixed point: integer sums, exact in any order
@@ -283,7 +465,9 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
     if (rank == 0 && threadIdx.x == 0) {
         Best d{-INFINITY, INT_MAX};
         for (int r = 0; r < C; ++r) d = better(d, *cluster.map_shared_rank(&pub_draw, r));
-        const int token = d.i == INT_MAX ? best.i : d.i;  // the row maximum is always kept: INT_MAX cannot happen
+        // the row maximum is always kept: INT_MAX cannot happen (TRUNC reads it back from shared memory rather than keep
+        // a register across its passes)
+        const int token = d.i == INT_MAX ? (TRUNC ? row_max.i : best.i) : d.i;
         out[row] = token;
         if constexpr (PEN) {
             if (positions[row] > 0) pen.state[static_cast<size_t>(row) * vocab + token] += 1;
@@ -291,17 +475,27 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const T *__restr
         if constexpr (MASK) {
             if (con[row].mask && positions[row] > 0) con[row].state = constraint_advance(con[row], token);
         }
+        if constexpr (TRUNC) {  // mu' = mu - eta (s - tau), s = log2 S_K - log2 e_token: the surprise over the kept mass
+            if (trn.mirostat_tau && trn.mirostat_tau[row] > 0.f && positions[row] > 0) {
+                const int owner = token / slice;
+                const float xt = *cluster.map_shared_rank(xs + (token - owner * slice), owner);
+                const unsigned long long et = __float2ull_rn(expf(__fdiv_rn(__fsub_rn(xt, m), temp)) * MASS_SCALE);
+                const double s = log2(static_cast<double>(s_miro_kept)) - log2(static_cast<double>(et));
+                trn.mu[row] = static_cast<float>(static_cast<double>(trn.mu[row]) -
+                                                 static_cast<double>(trn.mirostat_eta[row]) * (s - static_cast<double>(trn.mirostat_tau[row])));
+            }
+        }
     }
     cluster.sync();
 }
 
-template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC>
+template <typename T, int LEVELS, bool PEN, bool MASK, bool XTC, bool TRUNC>
 int launch_sample_t(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                     const int32_t *positions, int32_t *out, int rows, int vocab, int cluster, int slice, int vec, const Penalties &pen,
-                    tl_constraint_row *con, const Xtc &xtc, cudaStream_t st) {
+                    tl_constraint_row *con, const Xtc &xtc, const Trunc &trn, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN, MASK, XTC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
+        if (cudaFuncSetAttribute(sample_kernel<T, LEVELS, PEN, MASK, XTC, TRUNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SAMPLE_MAX_SMEM) != cudaSuccess)
             return fail(TL_ECUDA, "sample: cannot raise shared memory limit");
         configured = true;
     }
@@ -321,16 +515,16 @@ int launch_sample_t(const void *logits, const float *temperature, const int32_t 
     cfg.numAttrs = use_pdl() ? 2 : 1;
     const T *x = static_cast<const T *>(logits);
     cudaError_t e =
-        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN, MASK, XTC>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen, con, xtc);
+        cudaLaunchKernelEx(&cfg, sample_kernel<T, LEVELS, PEN, MASK, XTC, TRUNC>, x, temperature, top_k, top_p, seed, positions, out, vocab, slice, vec, pen, con, xtc, trn);
     if (e != cudaSuccess) return fail(TL_ECUDA, "sample: launch failed: %s", cudaGetErrorString(e));
     TL_LAUNCH_CHECK("sample");
     return TL_OK;
 }
 
-template <bool PEN, bool MASK, bool XTC = false>
+template <bool PEN, bool MASK, bool XTC = false, bool TRUNC = false>
 int launch_sample_any(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                       const int32_t *positions, int32_t *out, int rows, int vocab, int dtype, const Penalties &pen, tl_constraint_row *con,
-                      cudaStream_t st, const Xtc &xtc = Xtc{}) {
+                      cudaStream_t st, const Xtc &xtc = Xtc{}, const Trunc &trn = Trunc{}) {
     if (rows == 0) return TL_OK;
     int cluster = 0, slice = 0;
     if (int e = sample_plan(vocab, &cluster, &slice)) return e;
@@ -338,16 +532,16 @@ int launch_sample_any(const void *logits, const float *temperature, const int32_
     const int vec = (vocab % per16 == 0 && aligned16(logits)) ? 1 : 0;
     switch (dtype) {
         case TL_F32:
-            return launch_sample_t<float, 4, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
-                                                             vec, pen, con, xtc, st);
+            return launch_sample_t<float, 4, PEN, MASK, XTC, TRUNC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster, slice,
+                                                             vec, pen, con, xtc, trn, st);
         case TL_F16:
-            return launch_sample_t<__half, 4, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
-                                                              slice, vec, pen, con, xtc, st);
+            return launch_sample_t<__half, 4, PEN, MASK, XTC, TRUNC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, cluster,
+                                                              slice, vec, pen, con, xtc, trn, st);
         case TL_BF16:  // a raw bf16 value's key has 16 significant bits: two levels.  A penalty rewrites the staged values
                        // (x / r, x * r, x - f c, x - pres) into arbitrary fp32 values: four levels, or tau would stop
                        // at a 16-bit prefix and keep every entry of its bucket below x_(k) or v*
-            return launch_sample_t<__nv_bfloat16, PEN ? 4 : 2, PEN, MASK, XTC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab,
-                                                                      cluster, slice, vec, pen, con, xtc, st);
+            return launch_sample_t<__nv_bfloat16, PEN ? 4 : 2, PEN, MASK, XTC, TRUNC>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab,
+                                                                      cluster, slice, vec, pen, con, xtc, trn, st);
         default: return fail(TL_EDTYPE, "sample: expected float32, float16, or bfloat16");
     }
 }
@@ -372,9 +566,14 @@ int launch_sample(const void *logits, const float *temperature, const int32_t *t
 
 int launch_sample_penalized(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                             const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
-                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability, int32_t *out,
-                            int rows, int vocab, int dtype, cudaStream_t st) {
+                            const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
+                            const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                            float *mirostat_mu, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
     const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    if (typical_p || top_n_sigma || mirostat_tau)
+        return launch_sample_any<true, false, true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, nullptr,
+                                                          st, Xtc{xtc_threshold, xtc_probability},
+                                                          Trunc{typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu});
     if (xtc_threshold)
         return launch_sample_any<true, false, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, nullptr, st,
                                                     Xtc{xtc_threshold, xtc_probability});
@@ -384,11 +583,16 @@ int launch_sample_penalized(const void *logits, const float *temperature, const 
 int launch_sample_constrained(const void *logits, const float *temperature, const int32_t *top_k, const float *top_p, const int64_t *seed,
                               const int32_t *positions, const float *repetition, const float *presence, const float *frequency,
                               const float *min_p, int32_t *state, const float *xtc_threshold, const float *xtc_probability,
-                              tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
+                              const float *typical_p, const float *top_n_sigma, const float *mirostat_tau, const float *mirostat_eta,
+                              float *mirostat_mu, tl_constraint_row *constraints, int32_t *out, int rows, int vocab, int dtype, cudaStream_t st) {
     if (!state)
         return launch_sample_any<false, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, Penalties{},
                                               constraints, st);
     const Penalties pen{repetition, presence, frequency, min_p, state, (vocab % 4 == 0 && aligned16(state)) ? 1 : 0};
+    if (typical_p || top_n_sigma || mirostat_tau)
+        return launch_sample_any<true, true, true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen,
+                                                         constraints, st, Xtc{xtc_threshold, xtc_probability},
+                                                         Trunc{typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu});
     if (xtc_threshold)
         return launch_sample_any<true, true, true>(logits, temperature, top_k, top_p, seed, positions, out, rows, vocab, dtype, pen, constraints,
                                                    st, Xtc{xtc_threshold, xtc_probability});

@@ -156,6 +156,8 @@ _SIGNATURES = {
     "tl_sample_constrained": (_I, [_VP] * 13 + [_I] * 3 + [_VP]),
     "tl_sample_penalized_xtc": (_I, [_VP] * 14 + [_I] * 3 + [_VP]),
     "tl_sample_constrained_xtc": (_I, [_VP] * 15 + [_I] * 3 + [_VP]),
+    "tl_sample_penalized_trunc": (_I, [_VP] * 19 + [_I] * 3 + [_VP]),
+    "tl_sample_constrained_trunc": (_I, [_VP] * 20 + [_I] * 3 + [_VP]),
     "tl_logit_controls": (_I, [_VP] * 6 + [_I] * 3 + [_VP]),
     "tl_dry_penalty": (_I, [_VP] * 6 + [_I] * 3 + [_VP]),
     "tl_constraint_token_masks": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP]),
@@ -994,13 +996,34 @@ def _xtc_arrays(op, rows, xtc_threshold, xtc_probability):
     return xtc_threshold.data_ptr(), xtc_probability.data_ptr()
 
 
+def _trunc_arrays(op, rows, typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu):
+    """The truncation pointers (None when no array is given) with each given array checked as float32 [rows]."""
+    named = dict(typical_p=typical_p, top_n_sigma=top_n_sigma, mirostat_tau=mirostat_tau, mirostat_eta=mirostat_eta,
+                 mirostat_mu=mirostat_mu)
+    if all(t is None for t in named.values()):
+        return None
+    if mirostat_tau is not None and (mirostat_eta is None or mirostat_mu is None):
+        raise RuntimeError(f"{op}: Mirostat needs mirostat_eta and mirostat_mu beside mirostat_tau")
+    given = {name: t for name, t in named.items() if t is not None}
+    for name, t in given.items():
+        if t.dtype != torch.float32 or t.dim() != 1 or t.shape[0] != rows:
+            raise RuntimeError(f"{op}: {name} must be float32 [{rows}]")
+    _contig(op, **given)
+    _gpu(op, *given.values())
+    return [None if t is None else t.data_ptr() for t in named.values()]
+
+
 def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetition, presence, frequency, min_p, state, stream=None,
-                     xtc_threshold=None, xtc_probability=None):
+                     xtc_threshold=None, xtc_probability=None, typical_p=None, top_n_sigma=None, mirostat_tau=None, mirostat_eta=None,
+                     mirostat_mu=None):
     """``sample`` with token-history penalties and min-p (``tl_sample_penalized``) -> int32 ``[rows]``.  Further
     per-row device arrays: ``repetition``, ``presence``, ``frequency`` and ``min_p`` float32 ``[rows]``, and ``state``
     int32 ``[rows, vocab]`` (bit 30: token in the prompt, bits 0-29: times drawn), read, and for rows with
     ``positions > 0`` incremented at the drawn token.  ``xtc_threshold`` and ``xtc_probability`` (float32 ``[rows]``,
-    both or neither) add XTC (DESIGN.md section 24)."""
+    both or neither) add XTC (DESIGN.md section 24).  ``typical_p``, ``top_n_sigma``, ``mirostat_tau`` and
+    ``mirostat_eta`` (float32 ``[rows]``, each optional) add the truncation samplers (``tl_sample_penalized_trunc``,
+    DESIGN.md section 25); with ``mirostat_tau`` (rows with tau > 0 run Mirostat 2.0) ``mirostat_eta`` and
+    ``mirostat_mu`` (float32 ``[rows]``, read and, for rows with ``positions > 0``, updated) are required."""
     if logits.dtype not in _FLOATS or logits.dim() != 2:
         raise RuntimeError("sample_penalized: expected 2D float logits")
     rows, vocab = logits.shape
@@ -1016,7 +1039,14 @@ def sample_penalized(logits, temperature, top_k, top_p, seed, positions, repetit
     _contig("sample_penalized", **named)
     _gpu("sample_penalized", *named.values())
     xtc = _xtc_arrays("sample_penalized", rows, xtc_threshold, xtc_probability)
+    trunc = _trunc_arrays("sample_penalized", rows, typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu)
     out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
+    if trunc is not None:
+        _check(_lib.tl_sample_penalized_trunc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                              positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(),
+                                              min_p.data_ptr(), state.data_ptr(), *xtc, *trunc, out.data_ptr(), rows, vocab,
+                                              _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+        return out
     _check(_lib.tl_sample_penalized_xtc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
                                         positions.data_ptr(), repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(),
                                         min_p.data_ptr(), state.data_ptr(), *xtc, out.data_ptr(), rows, vocab, _DTYPE_CODE[logits.dtype],
@@ -1028,12 +1058,13 @@ CONSTRAINT_ROW_WORDS = 5  # int64 words of one tl_constraint_row (40 bytes)
 
 
 def sample_constrained(logits, temperature, top_k, top_p, seed, positions, constraints, repetition=None, presence=None, frequency=None,
-                       min_p=None, state=None, stream=None, xtc_threshold=None, xtc_probability=None):
+                       min_p=None, state=None, stream=None, xtc_threshold=None, xtc_probability=None, typical_p=None, top_n_sigma=None,
+                       mirostat_tau=None, mirostat_eta=None, mirostat_mu=None):
     """``sample`` (no penalty arrays) or ``sample_penalized`` (all of them) restricted per row to the tokens of its
     constraint (``tl_sample_constrained``) -> int32 ``[rows]``.  ``constraints`` int64 ``[rows, 5]``: one
     ``tl_constraint_row`` per row (all zero: unconstrained), whose state the launch advances for rows with
-    ``positions > 0``.  ``xtc_threshold`` and ``xtc_probability`` as ``sample_penalized`` takes them, with the penalty
-    arrays."""
+    ``positions > 0``.  ``xtc_threshold`` and ``xtc_probability``, and the truncation arrays, as ``sample_penalized``
+    takes them, with the penalty arrays."""
     if logits.dtype not in _FLOATS or logits.dim() != 2:
         raise RuntimeError("sample_constrained: expected 2D float logits")
     rows, vocab = logits.shape
@@ -1060,8 +1091,16 @@ def sample_constrained(logits, temperature, top_k, top_p, seed, positions, const
     xtc = _xtc_arrays("sample_constrained", rows, xtc_threshold, xtc_probability)
     if xtc[0] is not None and state is None:
         raise RuntimeError("sample_constrained: XTC needs the penalty arrays and the state")
+    trunc = _trunc_arrays("sample_constrained", rows, typical_p, top_n_sigma, mirostat_tau, mirostat_eta, mirostat_mu)
+    if trunc is not None and state is None:
+        raise RuntimeError("sample_constrained: typical, top-n-sigma and Mirostat need the penalty arrays and the state")
     out = torch.empty((rows,), dtype=torch.int32, device=logits.device)
     ptr = [None if t is None else t.data_ptr() for t in pen]
+    if trunc is not None:
+        _check(_lib.tl_sample_constrained_trunc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
+                                                positions.data_ptr(), *ptr, *xtc, *trunc, constraints.data_ptr(), out.data_ptr(), rows, vocab,
+                                                _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))
+        return out
     _check(_lib.tl_sample_constrained_xtc(logits.data_ptr(), temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(),
                                           positions.data_ptr(), *ptr, *xtc, constraints.data_ptr(), out.data_ptr(), rows, vocab,
                                       _DTYPE_CODE[logits.dtype], _stream_ptr(stream, logits)))

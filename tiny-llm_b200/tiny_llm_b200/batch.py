@@ -27,7 +27,8 @@ from .logprobs import _check_n, token_logprobs
 from .lora import adapter_ids_of
 from .json_mode import ConstraintRows
 from .logit_controls import ControlRows
-from .sampler import any_constrained, any_controlled, any_penalized, sample_tokens, sampling_per_request, token_state_row
+from .sampler import (any_constrained, any_controlled, any_penalized, mirostat_start, sample_tokens, sampling_per_request,
+                      token_state_row)
 
 
 def greedy_tokens(logits: torch.Tensor) -> torch.Tensor:
@@ -94,6 +95,7 @@ class Request:
         self.logprobs = logprobs
         self.logprob_entries: list = []
         self.constraint_row = None  # one-row ConstraintRows, made with the first token's draw
+        self.mirostat_mu = None  # Mirostat: the request's mu [1] (f32, device), 2 tau before its first token's draw
         self.model = model
         if isinstance(prompt, str):
             ids = tokenizer.encode(prompt, add_special_tokens=False)
@@ -157,7 +159,10 @@ class Request:
                     if self.sampling.controls:
                         controls = ControlRows(1, logits.shape[-1], logits.device, history_capacity=total)
                         controls.set_row(0, self.sampling, self.prompt_list, (), () if self.eos_token_id is None else (self.eos_token_id,))
-                    token = sample_tokens(logits, [self.sampling], [total], state, self.constraint_row, controls, self.prefill_tokens[-1:])
+                    if self.sampling.mirostat:
+                        self.mirostat_mu = torch.full((1,), mirostat_start(self.sampling), dtype=torch.float32, device=logits.device)
+                    mu = {} if self.mirostat_mu is None else {"mirostat_mu": self.mirostat_mu}
+                    token = sample_tokens(logits, [self.sampling], [total], state, self.constraint_row, controls, self.prefill_tokens[-1:], **mu)
                 if self.logprobs is not None:
                     entry = token_logprobs(logits, token, self.logprobs)[0]
         self.offset += chunk
@@ -308,6 +313,7 @@ class ContinuousBatcher:
         self.token_state: torch.Tensor | None = None  # [batch_size, vocab] int32, on first penalised admission
         self.constraint_rows: ConstraintRows | None = None  # batch_size rows, on first constrained admission
         self.control_rows: ControlRows | None = None  # batch_size rows, on first controlled admission
+        self.mirostat_mu: torch.Tensor | None = None  # [batch_size] f32, each Mirostat slot's mu, on first Mirostat admission
         self.prefix_cache = model.enable_prefix_cache() if prefix_cache else None
         self.reused_tokens: dict[int, int] = {}
         self.reused_total = 0
@@ -360,6 +366,12 @@ class ContinuousBatcher:
             vocab = self.model.vocab_size
             self.token_state = torch.zeros((self.batch_size, vocab), dtype=torch.int32, device=request.prefill_tokens.device)
         token_state_row(request.prefill_tokens, [request.next_token], self.token_state.shape[1], out=self.token_state[slot])
+        if request.sampling is not None and request.sampling.mirostat:
+            # the slot goes on from the request's mu after its first token (drawn at 2 tau); a released slot keeps
+            # whatever it held, which no other request reads
+            if self.mirostat_mu is None:
+                self.mirostat_mu = torch.zeros(self.batch_size, dtype=torch.float32, device=request.prefill_tokens.device)
+            self.mirostat_mu[slot : slot + 1].copy_(request.mirostat_mu)
 
     def _admit_constraint(self, request: Request, slot: int) -> None:
         """Copy the request's constraint row into the slot's row (a device copy of its state), or clear the row.  The
@@ -473,7 +485,8 @@ class ContinuousBatcher:
                     positions = [0 if s is None else o + 1 for s, o in zip(self.slots, offsets)]
                     sampled = sample_tokens(logits, params, positions, self.token_state if any_penalized(params) else None,
                                             self.constraint_rows if any_constrained(params) else None,
-                                            self.control_rows if any_controlled(params) else None, batch.reshape(-1))
+                                            self.control_rows if any_controlled(params) else None, batch.reshape(-1),
+                                            **({} if self.mirostat_mu is None else {"mirostat_mu": self.mirostat_mu}))
                 if self.logprobs_n is not None:
                     live = torch.tensor([s is not None for s in self.slots], device=sampled.device)
                     targets = torch.where(live, sampled.reshape(-1).to(torch.int32), -1)

@@ -15,6 +15,8 @@ see checkpoint.py; there is no hub download here).
         (logits controls: a per-token bias, banned sequences; also --allowed-token-ids and --min-tokens)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --sampler-temp 0.8 --dry-multiplier 0.8 --xtc-probability 0.5
         (DRY penalises tokens that extend a verbatim repeat; XTC drops the most likely choices with a seeded probability)
+    python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --prompt-ids 5,17,3 --sampler-temp 0.8 --typical-p 0.9 --top-n-sigma 1.5
+        (locally typical sampling and top-n-sigma; --mirostat 2 --mirostat-tau 5 --mirostat-eta 0.1 for Mirostat 2.0)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3
         (speculative decoding: same ids as greedy; acceptance stats on stderr)
     python -m tiny_llm_b200.cli generate --synthetic tiny-d128 --draft-synthetic tiny-d128 --proposal-length 4 --prompt-ids 5,17,3 --sampler-temp 0.7 --sampler-top-p 0.9 --seed 3
@@ -173,11 +175,30 @@ def _print_logprobs(entries, tokenizer, file=None) -> None:
 
 
 def _penalties(args) -> dict:
-    """The ``SamplingParams`` penalty fields the flags turn on (an empty dict when every one is off)."""
+    """The ``SamplingParams`` penalty and truncation fields the flags turn on (an empty dict when every one is off)."""
     given = dict(repetition_penalty=args.repetition_penalty, presence_penalty=args.presence_penalty,
                  frequency_penalty=args.frequency_penalty, min_p=args.min_p)
     off = dict(repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_p=0.0)
-    return {k: v for k, v in given.items() if v != off[k]}
+    return {**{k: v for k, v in given.items() if v != off[k]}, **_truncation(args)}
+
+
+def _truncation(args) -> dict:
+    """The ``SamplingParams`` truncation fields of ``--typical-p``, ``--top-n-sigma`` and ``--mirostat*`` (an empty
+    dict when every sampler is off; tau and eta only with ``--mirostat 2``)."""
+    out = {}
+    if args.typical_p != 1.0:
+        out["typical_p"] = args.typical_p
+    if args.top_n_sigma != 0.0:
+        out["top_n_sigma"] = args.top_n_sigma
+    if args.mirostat:
+        out.update(mirostat=args.mirostat, mirostat_tau=args.mirostat_tau, mirostat_eta=args.mirostat_eta)
+    return out
+
+
+def _truncation_flags(args) -> list:
+    """The truncation flags given, by name."""
+    return [f for f, on in (("--typical-p", args.typical_p != 1.0), ("--top-n-sigma", args.top_n_sigma != 0.0),
+                            ("--mirostat", args.mirostat != 0)) if on]
 
 
 def parse_controls(logit_bias=None, allowed_token_ids=None, bad_words=None, min_tokens=0) -> dict:
@@ -371,6 +392,8 @@ def cmd_generate(args) -> int:
         raise SystemExit("speculative decoding and prompt lookup are greedy and unconstrained: drop --grammar")
     if speculative and dry_xtc:
         raise SystemExit("speculative decoding and prompt lookup take no --dry-multiplier or --xtc-probability")
+    if speculative and _truncation_flags(args):
+        raise SystemExit(f"speculative decoding and prompt lookup take no {_truncation_flags(args)[0]}: drop it or the proposer")
     if speculative and controls:
         raise SystemExit("speculative decoding takes no --logit-bias, --allowed-token-ids, --bad-words or --min-tokens")
     if controls and args.grammar is not None:
@@ -495,7 +518,8 @@ def _beam_search(args, model, tokenizer, ids, penalties, device) -> int:
     finished or not), then its text (its ids for ``--prompt-ids`` runs)."""
     from .generate import beam_search_ids
 
-    refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("penalties or --min-p", bool(penalties)),
+    refused = [("a non-zero --sampler-temp", args.sampler_temp != 0), ("--typical-p", args.typical_p != 1.0),
+               ("--top-n-sigma", args.top_n_sigma != 0.0), ("--mirostat", args.mirostat != 0), ("penalties or --min-p", bool(penalties)),
                ("--regex", args.regex is not None), ("--json", args.json),
                ("--json-schema", args.json_schema is not None), ("--grammar", args.grammar is not None),
                ("--logprobs", args.logprobs is not None),
@@ -764,6 +788,14 @@ def main(argv=None) -> int:
                                        help="XTC: tokens at least this likely are the top choices (in (0, 1])")
         sub.choices[name].add_argument("--xtc-probability", type=float, default=0.0,
                                        help="XTC: the chance per draw of excluding all top choices but the least likely (0: off)")
+        sub.choices[name].add_argument("--typical-p", type=float, default=1.0,
+                                       help="locally typical sampling: keep the tokens closest to the entropy up to this mass (1: off)")
+        sub.choices[name].add_argument("--top-n-sigma", type=float, default=0.0,
+                                       help="keep tokens within this many standard deviations of the top logit (0: off)")
+        sub.choices[name].add_argument("--mirostat", type=int, default=0, choices=(0, 2),
+                                       help="Mirostat 2.0: keep the surprise of each draw near --mirostat-tau (0: off)")
+        sub.choices[name].add_argument("--mirostat-tau", type=float, default=5.0, help="Mirostat: the target surprise in bits (> 0)")
+        sub.choices[name].add_argument("--mirostat-eta", type=float, default=0.1, help="Mirostat: the learning rate of mu (> 0)")
         sub.choices[name].add_argument("--regex", default=None, metavar="PATTERN",
                                        help="constrain the generated text to fullmatch PATTERN (re.ASCII semantics over UTF-8 bytes)")
         sub.choices[name].add_argument("--json", action="store_true",

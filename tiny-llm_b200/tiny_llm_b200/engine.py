@@ -51,6 +51,8 @@ FUSED_ATTENTION_MAX_SLOT_TOKENS = 16384
 # ``controlled == DRY`` adds one tl_dry_penalty launch after tl_logit_controls
 XTC = "xtc"
 DRY = "dry"
+# ``penalized == TRUNC`` draws with the truncation samplers (DESIGN.md section 25) and XTC
+TRUNC = "trunc"
 
 # Grouped decode attention (tl_shared_prefix_attention, DESIGN.md section 16) replaces the step's attention for a group
 # of COUNT slots sharing SHARED_TOKENS prompt tokens only where tools/parallel_sample_bench.py measured it faster.
@@ -439,6 +441,16 @@ class DecodeEngine(_GraphEngine):
         self._pen_host = None
         self._pen_dev = None
         self._pen_key = None
+        # decode_on_device(sampling=<typical, top-n-sigma or Mirostat>): every penalised graph kind has a twin
+        # (penalized == TRUNC) that also reads the truncation block (typical_p | top_n_sigma | mirostat_tau |
+        # mirostat_eta, f32, B each, pinned beside the penalty block) and reads and writes mirostat_mu [B], each slot's
+        # Mirostat mu; all on first use.  _miro_key holds the SamplingParams each slot's mu belongs to.
+        self._graph_pen_trunc = None
+        self._trunc_host = None
+        self._trunc_dev = None
+        self._trunc_key = None
+        self.mirostat_mu = None
+        self._miro_key = None
         # decode_on_device(sampling=<constrained>): one graph per (penalised, logprobs N or None), the step with
         # tl_sample_constrained as its token choice, over a [B, 5] int64 slab of tl_constraint_row descriptors whose
         # states the launches advance; all on first use
@@ -534,9 +546,13 @@ class DecodeEngine(_GraphEngine):
             if controlled == DRY:
                 ext.dry_penalty(logits, tab.dry.table[:R], self.context_lens[:R], self.tokens[:R], tab.dry.history[:R], tab.dry.scratch[:R])
         xtc = {}
-        if penalized == XTC:
+        if penalized == XTC or penalized == TRUNC:
             p = self._pen_dev.view(torch.float32).view(6, self.B)
             xtc = dict(xtc_threshold=p[4, :R], xtc_probability=p[5, :R])
+        if penalized == TRUNC:
+            t = self._trunc_dev.view(torch.float32).view(4, self.B)
+            xtc.update(typical_p=t[0, :R], top_n_sigma=t[1, :R], mirostat_tau=t[2, :R], mirostat_eta=t[3, :R],
+                       mirostat_mu=self.mirostat_mu[:R])
         if spec_draft is not None:
             ext.speculative_sample(logits, spec_draft, self.tokens[1:R], *self._spec_params, self.context_lens[:R], out=self.next_tokens[:R])
             return
@@ -739,6 +755,7 @@ class DecodeEngine(_GraphEngine):
         self._graph_sample = None  # captured again on first use, over the current slabs
         self._graph_pen = None
         self._graph_pen_xtc = None
+        self._graph_pen_trunc = None
         self._graph_lp = {}
         self._graph_con = {}
         self._graph_json = {}
@@ -888,9 +905,10 @@ class DecodeEngine(_GraphEngine):
         return out
 
     def _ensure_penalized_graph(self, penalized=True) -> None:
-        """Capture the penalised sampled self-advancing step (``penalized == XTC``: with XTC; same conditions as
-        ``_ensure_sample_graph``; the warm-up runs at context 0, so it counts nothing)."""
-        if (self._graph_pen_xtc if penalized == XTC else self._graph_pen) is not None:
+        """Capture the penalised sampled self-advancing step (``penalized == XTC``: with XTC, ``penalized == TRUNC``: with
+        the truncation samplers; same conditions as ``_ensure_sample_graph``; the warm-up runs at context 0, so it counts
+        nothing and leaves mu alone)."""
+        if {XTC: self._graph_pen_xtc, TRUNC: self._graph_pen_trunc}.get(penalized, self._graph_pen) is not None:
             return
         forward = self._forward_fused if self.fused else self._forward_unfused
 
@@ -904,6 +922,8 @@ class DecodeEngine(_GraphEngine):
             graph = self._graph_of(penalized_step, pool=self._graph.pool(), warmups=1)
             if penalized == XTC:
                 self._graph_pen_xtc = graph
+            elif penalized == TRUNC:
+                self._graph_pen_trunc = graph
             else:
                 self._graph_pen = graph
                 self.kernels_per_penalized_step = self._launches
@@ -1196,6 +1216,38 @@ class DecodeEngine(_GraphEngine):
             self._pen_host = torch.zeros(24 * self.B, dtype=torch.uint8, pin_memory=True)
             self._pen_dev = self._pen_host.to(self.device, copy=True)
 
+    def _alloc_truncation(self) -> None:
+        """The truncation block and mirostat_mu, on first use (before the TRUNC graphs are captured over them)."""
+        if self._trunc_dev is None:
+            self._trunc_host = torch.zeros(16 * self.B, dtype=torch.uint8, pin_memory=True)
+            self._trunc_dev = self._trunc_host.to(self.device, copy=True)
+            self.mirostat_mu = torch.zeros(self.B, dtype=torch.float32, device=self.device)
+            self._miro_key = [None] * self.B
+
+    def _set_truncation(self, per: list, mirostat_mu) -> None:
+        """Upload the truncation parameters if they changed, and set each slot's mu: from ``mirostat_mu[b]`` when it is
+        given, 2 tau when the slot is newly under Mirostat, else the slot goes on from the device's value."""
+        from .sampler import mirostat_start, truncation_tensors
+
+        B = self.B
+        key = tuple(per)
+        if key != self._trunc_key:
+            self._host_write_begin()
+            host = self._trunc_host.numpy()
+            for j, t in enumerate(truncation_tensors(per, "cpu")):
+                host[4 * B * j : 4 * B * (j + 1)] = t.numpy().view(np.uint8)
+            self._upload_meta(self._trunc_dev, self._trunc_host)
+            self.h2d_bytes += 16 * B
+            self._trunc_key = key
+        given = [None] * B if mirostat_mu is None else list(mirostat_mu)
+        for b, p in enumerate(per):
+            miro = p is not None and p.mirostat == 2
+            if miro and given[b] is not None:
+                self.mirostat_mu[b].fill_(float(given[b]))
+            elif miro and self._miro_key[b] != p:
+                self.mirostat_mu[b].fill_(mirostat_start(p))
+            self._miro_key[b] = p if miro else None
+
     def _set_penalties(self, per: list, history) -> None:
         """Rebuild the token-count rows ``history`` gives (per slot ``(prompt_ids, generated_ids)`` or None: keep the
         row) and upload the penalty parameters if they changed."""
@@ -1429,7 +1481,7 @@ class DecodeEngine(_GraphEngine):
         return self.logits.view(B, 1, self.V), self.next_tokens
 
     def decode_on_device(self, tokens, offsets, caches, steps: int, sampling=None, logprobs=None, history=None, adapter_ids=None,
-                         keep_logits: bool = False, groups=None, eos_token_ids=()):
+                         keep_logits: bool = False, groups=None, eos_token_ids=(), mirostat_mu=None):
         """``steps`` greedy decode steps with no host round trip: pages for all
         steps are allocated ahead, then the self-advancing graph is replayed
         back to back.  Returns the sampled tokens ``[steps, B]`` (device).
@@ -1468,7 +1520,12 @@ class DecodeEngine(_GraphEngine):
         draw on the controlled rows; logprobs still read the raw rows.  ``history`` writes a controlled slot's row and
         history tail (its last id must be the token the slot is fed); without it the slot continues from the row the
         engine holds.  ``eos_token_ids`` are the ids ``min_tokens`` holds back.  Controls are refused together with a
-        constraint and with ``keep_logits``."""
+        constraint and with ``keep_logits``.
+        With a slot that runs typical sampling, top-n-sigma or Mirostat (DESIGN.md section 25) every penalised graph
+        kind above is replayed as its truncation twin.  Each slot's Mirostat mu lives in ``mirostat_mu [B]`` (device,
+        f32), which the launches update; ``history`` cannot rebuild it, so ``mirostat_mu`` (one float or None per slot)
+        sets it: a slot with a value starts from it, a slot newly under Mirostat without one starts at 2 tau, and every
+        other slot goes on from the engine's value."""
         if steps > self.log_capacity:
             raise ValueError("steps exceed the engine's token log capacity")
         if keep_logits:
@@ -1479,6 +1536,13 @@ class DecodeEngine(_GraphEngine):
                 raise ValueError("keep_logits takes plain sampling: no grammar constraint")
             if per is not None and any(p is not None and p.xtc for p in per):
                 raise ValueError("keep_logits takes plain sampling: no XTC (xtc_probability)")
+            for p in per or ():
+                if p is not None and p.typical_p < 1:
+                    raise ValueError("keep_logits takes plain sampling: no typical sampling (typical_p)")
+                if p is not None and p.top_n_sigma > 0:
+                    raise ValueError("keep_logits takes plain sampling: no top-n-sigma (top_n_sigma)")
+                if p is not None and p.mirostat:
+                    raise ValueError("keep_logits takes plain sampling: no Mirostat (mirostat)")
             if per is not None and any(p is not None and p.dry for p in per):
                 raise ValueError("keep_logits takes plain sampling: no DRY (dry_multiplier)")
             if per is None or logprobs is not None or any_penalized(per) or any_constrained(per):
@@ -1501,6 +1565,8 @@ class DecodeEngine(_GraphEngine):
             penalized, constrained, controlled = any_penalized(per), any_constrained(per), any_controlled(per)
             if any(p is not None and p.xtc for p in per):
                 penalized = XTC
+            if any(p is not None and p.truncation for p in per):
+                penalized = TRUNC
             if any(p is not None and p.dry for p in per):
                 controlled = DRY
             if controlled and any(p is not None and p.grammar for p in per):
@@ -1523,8 +1589,12 @@ class DecodeEngine(_GraphEngine):
             if not plain or not any(d[2] for d in descriptors):
                 descriptors = None
         self._adapters_of_call(adapter_ids)
+        if mirostat_mu is not None and len(list(mirostat_mu)) != B:
+            raise ValueError(f"mirostat_mu must hold one float or None per slot ({B})")
         if penalized:
             self._alloc_penalties()
+        if penalized == TRUNC:
+            self._alloc_truncation()
         json = constrained and any(isinstance(p.constraint, JsonConstraint) for p in per if p is not None)
         schema = constrained and any(isinstance(p.constraint, JsonSchemaConstraint) for p in per if p is not None)
         grammar = constrained and any(p.grammar for p in per if p is not None)
@@ -1592,6 +1662,8 @@ class DecodeEngine(_GraphEngine):
             self._set_sampling(sampling)
         if penalized:
             self._set_penalties(self._per_slot_sampling(sampling), history)
+        if penalized == TRUNC:
+            self._set_truncation(self._per_slot_sampling(sampling), mirostat_mu)
         if grammar or schema:
             pass  # the grammar and schema tables' rows are set above, before their graph is captured, which sizes the masks launches
         elif json:
@@ -1617,7 +1689,7 @@ class DecodeEngine(_GraphEngine):
         elif top_n is not None:
             graph = self._graph_lp[(sampling is not None, penalized)]
         elif penalized:
-            graph = self._graph_pen_xtc if penalized == XTC else self._graph_pen
+            graph = {XTC: self._graph_pen_xtc, TRUNC: self._graph_pen_trunc}.get(penalized, self._graph_pen)
         elif keep_logits:
             graph = self._graph_keep
         else:
@@ -1756,6 +1828,12 @@ class VerifyEngine(DecodeEngine):
                 raise ValueError("the sampled verify pass takes no grammar constraint")
             if sampling.xtc:
                 raise ValueError("the sampled verify pass takes no XTC: xtc_probability must be 0")
+            if sampling.typical_p < 1:
+                raise ValueError("the sampled verify pass takes no typical sampling: typical_p must be 1")
+            if sampling.top_n_sigma > 0:
+                raise ValueError("the sampled verify pass takes no top-n-sigma: top_n_sigma must be 0")
+            if sampling.mirostat:
+                raise ValueError("the sampled verify pass takes no Mirostat: mirostat must be 0")
             if sampling.dry:
                 raise ValueError("the sampled verify pass takes no DRY: dry_multiplier must be 0")
             if sampling.penalized or sampling.constraint is not None:

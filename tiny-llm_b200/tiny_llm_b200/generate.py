@@ -17,7 +17,7 @@ from .kv_cache import BatchingKvCache
 from .logprobs import _check_n, _host_rows, entries_from_host, token_logprobs
 from .logit_controls import ControlRows
 from .lora import adapter_ids_of
-from .sampler import sample_tokens, token_state_row
+from .sampler import mirostat_start, sample_tokens, token_state_row
 
 
 def _release_kv_cache(kv_cache) -> None:
@@ -59,7 +59,7 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
     kv_cache = model.create_kv_cache()
     produced: list[int] = []
     entries: list = []
-    state = constraints = controls = None
+    state = constraints = controls = mu = None
     try:
         ids = [int(t) for t in prompt_ids]
         prompt = torch.as_tensor(ids, dtype=torch.int32, device=device)
@@ -78,7 +78,10 @@ def greedy_generate_ids(model, prompt_ids, max_new_tokens: int, eos_token_id: in
                 if sampling.controls and controls is None:
                     controls = ControlRows(1, logits.shape[-1], logits.device, history_capacity=len(ids) + max_new_tokens)
                     controls.set_row(0, sampling, ids, (), () if eos_token_id is None else (eos_token_id,))
-                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state, constraints, controls, tokens[-1:])
+                if sampling.mirostat and mu is None:  # Mirostat's mu, from 2 tau at the first token on
+                    mu = torch.full((1,), mirostat_start(sampling), dtype=torch.float32, device=logits.device)
+                token = sample_tokens(logits[:, -1, :], [sampling], [offset + tokens.numel()], state, constraints, controls, tokens[-1:],
+                                      **({} if mu is None else {"mirostat_mu": mu}))
             elif sampler is None:
                 token = greedy_tokens(logits[:, -1, :])
             else:
@@ -397,6 +400,7 @@ def _spec_sampling(sampling, constraint):
         raise ValueError("speculative decoding is unconstrained: sampling must carry no constraint")
     if sampling.xtc:
         raise ValueError("speculative decoding and prompt lookup take no XTC: xtc_probability must be 0")
+    _refuse_truncation(sampling, "speculative decoding and prompt lookup take")
     if sampling.dry:
         raise ValueError("speculative decoding and prompt lookup take no DRY: dry_multiplier must be 0")
     if sampling.penalized:
@@ -404,6 +408,17 @@ def _spec_sampling(sampling, constraint):
     if sampling.controls:
         raise ValueError("speculative decoding takes no logit_bias, allowed_token_ids, bad_words_ids or min_tokens")
     return None if sampling.temperature == 0 else sampling
+
+
+def _refuse_truncation(sampling, what: str) -> None:
+    """The ValueError for a truncation sampler (DESIGN.md section 25) where ``what`` (a phrase ending in a verb) has
+    none: the message names the field."""
+    if sampling.typical_p < 1:
+        raise ValueError(f"{what} no typical sampling: typical_p must be 1")
+    if sampling.top_n_sigma > 0:
+        raise ValueError(f"{what} no top-n-sigma: top_n_sigma must be 0")
+    if sampling.mirostat:
+        raise ValueError(f"{what} no Mirostat: mirostat must be 0")
 
 
 def speculative_generate_ids(draft_model, model, prompt_ids, max_new_tokens: int, proposal_length: int = 4, eos_token_ids=(),
@@ -871,7 +886,9 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
     done = [False] * (P * n)
     penalized = any(p.penalized for p in params)
     constrained = any(p.constraint is not None for p in params)
-    state = constraints = None
+    mirostat = any(p.mirostat for p in params)
+    state = constraints = mu = None
+    mu_first = None  # the samples' mu after their first tokens, handed to the first decode_on_device round
 
     def take(b, token, entry) -> None:
         if done[b]:
@@ -898,19 +915,26 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
                 st = torch.stack([token_state_row(torch.as_tensor(prompt), [], rows.shape[-1], device=rows.device)] * n)
             if constrained:
                 con = ConstraintRows.build(params[i * n : i * n + n], rows.shape[-1], rows.device)
-            tok = sample_tokens(rows, params[i * n : i * n + n], [len(prompt)] * n, st, con)
+            m = None
+            if mirostat:
+                m = torch.tensor([mirostat_start(p) if p.mirostat else 0.0 for p in params[i * n : i * n + n]], dtype=torch.float32,
+                                 device=rows.device)
+            tok = sample_tokens(rows, params[i * n : i * n + n], [len(prompt)] * n, st, con, **({} if m is None else {"mirostat_mu": m}))
             ent = token_logprobs(rows, tok, logprobs) if logprobs is not None else [None] * n
-            firsts.append((tok.tolist(), ent, st, con))
+            firsts.append((tok.tolist(), ent, st, con, m))
             if n > 1:
                 slots[i * n + 1 : i * n + n] = fork([(cache, n - 1)])[0]
         tokens = [0] * (P * n)
-        for i, (tok, ent, st, con) in enumerate(firsts):
+        for i, (tok, ent, st, con, _) in enumerate(firsts):
             for j in range(n):
                 tokens[i * n + j] = tok[j]
                 take(i * n + j, tok[j], ent[j])
         if not graph:
             state = torch.cat([f[2] for f in firsts]) if penalized else None
             constraints = ConstraintRows.concat([f[3] for f in firsts]) if constrained else None
+            mu = torch.cat([f[4] for f in firsts]) if mirostat else None
+        elif mirostat:
+            mu_first = [float(v) if p.mirostat else None for v, p in zip(torch.cat([f[4] for f in firsts]).tolist(), params)]
         offsets = [len(prompts[b // n]) for b in range(P * n)]
         batch = [BatchingKvCache(P * n) for _ in range(len(slots[0]))]
         for layer, slot in enumerate(batch):
@@ -923,7 +947,9 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
                 history = None
                 if penalized or constrained:
                     history = [(prompts[b // n], out[b // n][b % n].ids) for b in range(P * n)]
-                got = engine.decode_on_device(tokens, offsets, batch, steps, sampling=params, logprobs=logprobs, history=history, groups=groups)
+                got = engine.decode_on_device(tokens, offsets, batch, steps, sampling=params, logprobs=logprobs, history=history, groups=groups,
+                                              **({} if mu_first is None else {"mirostat_mu": mu_first}))
+                mu_first = None  # later rounds go on from the device's mu
                 ids, lp = (got, None) if logprobs is None else got
                 host = ids.tolist()  # the round's device->host read
                 lp_host = None if lp is None else [_host_rows(ids[s], *[t[s] for t in lp]) for s in range(steps)]
@@ -937,7 +963,7 @@ def parallel_sample_ids(model, prompts, num_samples: int, sampling, max_new_toke
                 for _ in range(steps):
                     y = torch.as_tensor(tokens, dtype=torch.int32, device=device).view(P * n, 1)
                     rows = model(y, list(offsets), batch, logits_to_keep=1)[:, -1, :]
-                    tok = sample_tokens(rows, params, [o + 1 for o in offsets], state, constraints)
+                    tok = sample_tokens(rows, params, [o + 1 for o in offsets], state, constraints, **({} if mu is None else {"mirostat_mu": mu}))
                     ent = token_logprobs(rows, tok, logprobs) if logprobs is not None else [None] * (P * n)
                     tokens = tok.tolist()
                     for b in range(P * n):

@@ -73,7 +73,15 @@ class SamplingParams:
     the last ``dry_penalty_last_n`` tokens (0: all of them); a repeat never runs through a
     ``dry_sequence_breakers`` id (at most 64, stored as a sorted tuple).  XTC (the penalised form, DESIGN.md section
     24): with probability ``xtc_probability`` per draw, every kept token whose probability is at least
-    ``xtc_threshold`` but the least likely of them is excluded, when there are two or more."""
+    ``xtc_threshold`` but the least likely of them is excluded, when there are two or more.
+
+    Truncation samplers (the penalised form, DESIGN.md section 25), each off at its default: ``top_n_sigma`` n > 0 keeps
+    only tokens whose logit is at least ``max - n * sigma`` (sigma the standard deviation of the row's finite logits);
+    ``typical_p`` p < 1 (locally typical sampling) keeps, of the tokens left, those closest to the row's entropy in
+    surprise until their probability reaches p; ``mirostat=2`` (Mirostat 2.0) keeps the tokens whose surprise
+    ``-log2 p`` is at most the request's mu, which starts at ``2 * mirostat_tau`` and after every draw moves by
+    ``-mirostat_eta * (surprise - mirostat_tau)``.  Mirostat replaces top-k, top-p, min-p, typical, top-n-sigma and
+    XTC, and is refused beside any of them."""
 
     temperature: float
     top_k: int | None = None
@@ -95,6 +103,11 @@ class SamplingParams:
     dry_sequence_breakers: object = ()
     xtc_threshold: float = 0.1
     xtc_probability: float = 0.0
+    typical_p: float = 1.0
+    top_n_sigma: float = 0.0
+    mirostat: int = 0
+    mirostat_tau: float = 5.0
+    mirostat_eta: float = 0.1
 
     def __post_init__(self):
         t = self.temperature
@@ -131,6 +144,31 @@ class SamplingParams:
             raise ValueError(f"xtc_threshold must be a number in (0, 1], got {th!r}")
         object.__setattr__(self, "xtc_probability", float(q))
         object.__setattr__(self, "xtc_threshold", float(th))
+        tp = self.typical_p
+        if not real(tp) or not 0 < tp <= 1:
+            raise ValueError(f"typical_p must be a number in (0, 1], got {tp!r}")
+        ns = self.top_n_sigma
+        if not real(ns) or not ns >= 0:
+            raise ValueError(f"top_n_sigma must be a finite number >= 0, got {ns!r}")
+        mo = self.mirostat
+        if isinstance(mo, bool) or not isinstance(mo, numbers.Integral) or mo not in (0, 1, 2):
+            raise ValueError(f"mirostat must be 0 (off) or 2, got {mo!r}")
+        if mo == 1:
+            raise ValueError("Mirostat 1.0 is not supported; use mirostat=2")
+        for name in ("mirostat_tau", "mirostat_eta"):
+            v = getattr(self, name)
+            if not real(v) or not v > 0:
+                raise ValueError(f"{name} must be a finite number > 0, got {v!r}")
+            object.__setattr__(self, name, float(v))
+        object.__setattr__(self, "typical_p", float(tp))
+        object.__setattr__(self, "top_n_sigma", float(ns))
+        object.__setattr__(self, "mirostat", int(mo))
+        if self.mirostat:
+            for name, on in (("top_k", (self.top_k or 0) > 0), ("top_p", self.top_p is not None and 0 < self.top_p < 1),
+                             ("min_p", self.min_p > 0), ("typical_p", self.typical_p < 1), ("top_n_sigma", self.top_n_sigma > 0),
+                             ("xtc_probability", self.xtc)):
+                if on:
+                    raise ValueError(f"mirostat=2 replaces the other truncation samplers: {name} must be off beside it")
         from .dry import normalized_dry
 
         for name, value in normalized_dry(self).items():
@@ -171,6 +209,11 @@ class SamplingParams:
         return self.xtc_probability > 0
 
     @property
+    def truncation(self) -> bool:
+        """Whether the draw runs a truncation sampler: typical (``typical_p < 1``), top-n-sigma or Mirostat."""
+        return self.typical_p < 1 or self.top_n_sigma > 0 or self.mirostat == 2
+
+    @property
     def grammar(self) -> bool:
         """Whether the request carries a ``GrammarConstraint``."""
         from .grammar import GrammarConstraint
@@ -179,9 +222,9 @@ class SamplingParams:
 
     @property
     def penalized(self) -> bool:
-        """Whether the request needs ``tl_sample_penalized``: a penalty, min-p or XTC is on."""
+        """Whether the request needs ``tl_sample_penalized``: a penalty, min-p, XTC or a truncation sampler is on."""
         return (self.repetition_penalty != 1 or self.presence_penalty != 0 or self.frequency_penalty != 0 or self.min_p > 0
-                or self.xtc)
+                or self.xtc or self.truncation)
 
 
 GREEDY = SamplingParams(0.0)
@@ -226,6 +269,14 @@ def any_xtc(params) -> bool:
     return any(p is not None and p.xtc for p in params)
 
 
+def any_truncation(params) -> bool:
+    return any(p is not None and p.truncation for p in params)
+
+
+def any_mirostat(params) -> bool:
+    return any(p is not None and p.mirostat == 2 for p in params)
+
+
 def any_constrained(params) -> bool:
     return any(p is not None and p.constraint is not None for p in params)
 
@@ -244,6 +295,22 @@ def xtc_tensors(params, device) -> tuple[torch.Tensor, ...]:
     params = [GREEDY if p is None else p for p in params]
     return tuple(torch.tensor([float(getattr(p, name)) for p in params], dtype=torch.float32, device=device)
                  for name in ("xtc_threshold", "xtc_probability"))
+
+
+def truncation_tensors(params, device) -> tuple[torch.Tensor, ...]:
+    """The per-row truncation arrays (typical_p, top_n_sigma, mirostat_tau, mirostat_eta) ``ext.sample_penalized`` and
+    ``ext.sample_constrained`` take beside ``penalty_tensors``' (None: greedy, all off).  ``mirostat_tau`` is 0 on the
+    rows without Mirostat, which turns it off there."""
+    params = [GREEDY if p is None else p for p in params]
+    return (torch.tensor([p.typical_p for p in params], dtype=torch.float32, device=device),
+            torch.tensor([p.top_n_sigma for p in params], dtype=torch.float32, device=device),
+            torch.tensor([p.mirostat_tau if p.mirostat == 2 else 0.0 for p in params], dtype=torch.float32, device=device),
+            torch.tensor([p.mirostat_eta if p.mirostat == 2 else 0.0 for p in params], dtype=torch.float32, device=device))
+
+
+def mirostat_start(params) -> float:
+    """The mu a Mirostat request starts from: ``2 * mirostat_tau``, in fp32."""
+    return float(torch.tensor(2.0 * params.mirostat_tau, dtype=torch.float32))
 
 
 STATE_PROMPT = 1 << 30  # token state: bit 30 marks a prompt token, bits 0-29 count the draws
@@ -271,7 +338,7 @@ def token_state_row(prompt_ids, generated_ids, vocab: int, out: torch.Tensor | N
 
 
 def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor | None = None,
-                  constraints: torch.Tensor | None = None, controls=None, tokens=None) -> torch.Tensor:
+                  constraints: torch.Tensor | None = None, controls=None, tokens=None, mirostat_mu: torch.Tensor | None = None) -> torch.Tensor:
     """One seeded token per row of ``logits [rows, vocab]`` with the ``tl_sample`` kernel; ``params`` one
     ``SamplingParams`` (or None: greedy) per row, ``positions`` the index of each drawn token -> int32 ``[rows]``.
     When a row is penalised the launch is ``tl_sample_penalized`` over ``state`` (int32 ``[rows, vocab]``, required
@@ -284,7 +351,9 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
     (uncontrolled rows are copied exactly) over ``controls`` (a ``ControlRows`` of at least ``rows`` rows, required
     then), appending ``tokens`` (the step's input token per row) to its history tails, and the draw runs on those rows.
     When a row has DRY on, ``tl_dry_penalty`` then penalises those rows in place over ``controls.dry`` and appends
-    ``tokens`` to its histories.  XTC rows pass the ``xtc_tensors`` to the penalised or constrained draw.
+    ``tokens`` to its histories.  XTC rows pass the ``xtc_tensors`` to the penalised or constrained draw, and rows with
+    a truncation sampler the ``truncation_tensors``; a Mirostat row needs ``mirostat_mu`` (float32 ``[rows]`` on the
+    device, each Mirostat row's mu, updated in place for rows with position > 0).
     Rows of other requests may carry a constraint in the same launch: the constrained draw then runs on their exact
     fp32 copies, which draws the tokens it draws on the raw rows (a request never carries both)."""
     from extensions_b200 import tiny_llm_ext_b200 as ext
@@ -304,6 +373,15 @@ def sample_tokens(logits: torch.Tensor, params, positions, state: torch.Tensor |
     xtc = {}
     if any_xtc(params):
         xtc = dict(zip(("xtc_threshold", "xtc_probability"), xtc_tensors(params, logits.device)))
+    if any_truncation(params):
+        names = ("typical_p", "top_n_sigma", "mirostat_tau", "mirostat_eta")
+        xtc.update(zip(names, truncation_tensors(params, logits.device)))
+        if any_mirostat(params):
+            if mirostat_mu is None:
+                raise ValueError("a Mirostat SamplingParams needs the request's mu (mirostat_mu)")
+            xtc["mirostat_mu"] = mirostat_mu[: len(params)]
+        else:
+            del xtc["mirostat_tau"], xtc["mirostat_eta"]
     if any_constrained(params):
         if constraints is None:
             raise ValueError("a constrained SamplingParams needs the request's constraint descriptor")
